@@ -3,14 +3,15 @@
 
 One "step" = one complete fit of the resident rows through the C-ABI (b2_fit): four kernel launches --
     tc_shift_kernel     per-column shift from a 2048-row sample
-    gram_tc_kernel      tcgen05 Gram over every row of this rank's shard (the roofline kernel)
+    gram_tc_kernel      wgmma Gram over every row of this rank's shard (the roofline kernel)
     tc_finalize_kernel  reduce the per-CTA partials, fold into S, store S into every peer's exchange slot over NVLink (2-4 GPUs)
     solve kernel        waits for the peers' slots and sums them (2-4 GPUs), LDL^T, coefficients written to pinned host memory
-At more than 4 GPUs the exchange is one ncclAllReduce of S between the finalize and the solve kernel instead: measured faster
-there (profiles/r02_exchange_n8_diag.txt); `exchange.exchange_used` says which ran, B2_FORCE_P2P=1 / B2_NO_P2P=1 override.
+At more than 4 GPUs the exchange is one ncclAllReduce of S between the finalize and the solve kernel instead;
+`exchange.exchange_used` says which ran, B2_FORCE_P2P=1 / B2_NO_P2P=1 override.
 
 Arms
     python bench.py [--gpus N --steps K --warmup W]          this repo (one process per GPU under torchrun)
+                    [--dump-outputs DIR]                     also write the last timed fit's coef_ / intercept_ as .npy
     python bench.py --impl reference [...]                   the reference's own CPU path: scikit-learn
                                                              LinearRegression.fit (stage_1_train_model.py:105-106)
                                                              on a bounded sample, all host threads, rank 0 only
@@ -18,8 +19,7 @@ Arms
 Every N runs the SAME per-GPU shard (12.5 M x 128: BASELINE configs[2] over 8 GPUs), carries `parity` (the headline
 fit against the exact fp64 kernel over the same full-size rows and the same exchange, S bit-identical across ranks) and
 `exchange` (which exchange actually ran).  N = 1 adds `north_star` (100 M x 128 on one GPU), `config1_10Mx128`,
-`companion_score`, `cpu_baseline`; N > 1 adds `strong_100M` and `score_shard`.  Keys follow the driver's contract; see
-DESIGN.md "Measurement".
+`companion_score`, `cpu_baseline`; N > 1 adds `strong_100M` and `score_shard`.  See DESIGN.md "Measurement".
 """
 from __future__ import annotations
 
@@ -50,31 +50,22 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3, 700 W card); roofline.copy_gbs_this_gpu is this GPU's own copy rate"
 
 
 def measured_tensor_peak():
-    """dense bf16 TFLOP/s (burst) of this pool's B200s, driver-written; fallback = the profiling recipe's figure"""
+    """dense bf16 TFLOP/s: MEASURED_PEAKS.json when present, else the H100 SXM data sheet's figure (700 W card)"""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as fh:
-            return float(json.load(fh).get("bf16_tflops", 1688.7))
-    return 1688.7
-
-
-def ncu_traffic_per_launch(workload_key: str):
-    """dram bytes per launch of the Gram kernel from the committed ncu capture, if one matches."""
-    path = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(path):
-        with open(path) as fh:
-            return json.load(fh).get(workload_key)
-    return None
+            return float(json.load(fh).get("bf16_tflops", 989.0))
+    return 989.0
 
 
 class ClockSampler:
     """SM clock / throttle reasons DURING the timed region, polled in-process through NVML every ~2 ms
     (the timed region of a 20-step run is ~20 ms -- too short for an `nvidia-smi -lms` subprocess to start).
-    Falls back to the B200_PROFILING.md nvidia-smi recipe when pynvml is unavailable."""
+    Falls back to one nvidia-smi query when pynvml is unavailable."""
     _REASONS = (("hw_slowdown", 0x8), ("sw_power_cap", 0x4), ("sw_thermal_slowdown", 0x20),
                 ("hw_thermal_slowdown", 0x40), ("hw_power_brake_slowdown", 0x80))
 
@@ -225,7 +216,7 @@ def workload_config(n_gpus: int, x_kind: str, rows: int = 0) -> dict:
                          f"`config1_10Mx128` object of the N = 1 line"),
             "rows_per_gpu": rows, "features": D, "x_storage": x_kind,
             "parallelism": f"row-shard x{n_gpus}, one exchange of the (D+2)^2 fp64 statistic per fit",
-            "l2": f"inputs larger than L2 ({rows * (D * (4 if x_kind == 'f32' else 2) + 4) / 1e9:.2f} GB per pass vs 126 MB)"}
+            "l2": f"inputs larger than L2 ({rows * (D * (4 if x_kind == 'f32' else 2) + 4) / 1e9:.2f} GB per pass vs 50 MB)"}
 
 
 def max_over_ranks(dist, value: float) -> float:
@@ -309,6 +300,8 @@ def main() -> None:
     ap.add_argument("--no-variants", action="store_true", help="alias of --no-extras")
     ap.add_argument("--precision", default="split", choices=["split", "bf16"],
                     help="tensor-core operand precision: bf16 hi+lo split (default) or a single bf16 operand")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed fit returned (coef.npy, intercept.npy; float64) into DIR, rank 0")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     extras = not (args.no_extras or args.no_variants)
@@ -348,9 +341,8 @@ def main() -> None:
             sys.stdout.flush()
             os.dup2(saved_stdout, 1)
             os.close(saved_stdout)
-        # which exchange: measured on 8 GPUs, alternating runs on one box (profiles/r02_exchange_n8_diag.txt): NCCL 1.18-1.20 ms
-        # per fit, the peer-memory exchange 1.39-1.51 ms (its system-scope fences do not scale with the number of peers);
-        # at 2 and 4 GPUs the two are within 1-2 %.  So: peer-memory exchange up to 4 ranks, NCCL beyond;
+        # which exchange: the peer-memory exchange's system-scope fences do not scale with the number of peers, so it is
+        # used up to 4 ranks and one NCCL all-reduce beyond (not re-measured on H100 boxes);
         # B2_FORCE_P2P=1 / B2_NO_P2P=1 override.
         want_p2p = os.environ.get("B2_NO_P2P") != "1" and world <= 8 and (world <= 4 or os.environ.get("B2_FORCE_P2P") == "1")
         if want_p2p:
@@ -417,6 +409,11 @@ def main() -> None:
     t_host = time.perf_counter() - t_host0
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        # the inputs are device Philox rows of a fixed seed: two builds given the same arguments fit the same rows
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "coef.npy"), np.asarray(coef, dtype=np.float64))
+        np.save(os.path.join(args.dump_outputs, "intercept.npy"), np.asarray([b0], dtype=np.float64))
     kernel_ms, kernel_launches = ctx.last_kernel_ms()
     launches = ctx.launch_count() - launches0
     fused_fits = ctx.stats()["fused_fits"] - fused0
@@ -434,9 +431,8 @@ def main() -> None:
                 "algorithmic_bytes_per_row": bytes_per_row, "rows_per_launch": rows,
                 "kernel_ms_avg": gram_ms, "kernel_share_of_step": gram_ms / (ms / args.steps),
                 "step_tail_us": 1e3 * (ms / args.steps - gram_ms),
-                "whole_fit_frac_of_hbm_peak": rows * bytes_per_row / (ms / args.steps * 1e-3) / 1e9 / peak,
-                "traffic": ncu_traffic_per_launch(f"{kind}_{rows}x{D}")}
-    try:       # this box's own copy bandwidth next to the pool's figure: the fraction above varies 0.8-0.97 box to box
+                "whole_fit_frac_of_hbm_peak": rows * bytes_per_row / (ms / args.steps * 1e-3) / 1e9 / peak}
+    try:       # this GPU's own copy bandwidth next to the data-sheet figure
         box = ctx.copy_bandwidth_gbs()
         roofline["copy_gbs_this_gpu"] = box
         roofline["frac_of_this_gpu_copy"] = achieved / box
@@ -502,7 +498,7 @@ def main() -> None:
                    "coef_linf_vs_exact": parity["coef_linf"]}
         if world == 1:
             rec["what"] = ("BASELINE.json north_star: >= 70 % of the HBM roofline on the Gram kernel at N = 100 M, "
-                           "D = 128 on 1 B200, coefficient error < 1e-4")
+                           "D = 128 on 1 H100, coefficient error < 1e-4")
             north_star = rec
         else:
             rec["what"] = (f"SURVEY 8(d) config 3: the SAME 100 M x 128 rows strong-scaled over {world} GPUs "
@@ -574,7 +570,7 @@ def main() -> None:
     config1 = None
     if world == 1 and extras:
         config1 = {"what": "BASELINE.json configs[1]: 10 M x 128 rows resident on one GPU; complete fits (b2_fit); bf16-stored "
-                           "rows run gram_b16_kernel; coef_linf_vs_exact: against the exact fp64 kernel over the same stored rows",
+                           "rows run gram_tc_kernel<bf16>; coef_linf_vs_exact: against the exact fp64 kernel over the same stored rows",
                    "rows": ROWS_CONFIG1}
         exact_c1 = {}
         for vk, vprec in (("f32", "split"), ("f32", "bf16"), ("bf16", "split"), ("bf16", "bf16")):

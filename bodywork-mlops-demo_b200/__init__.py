@@ -1,4 +1,4 @@
-"""B200-native retrain hot path of AlexIoannides/bodywork-mlops-demo (stage_1's least-squares fit).
+"""H100-native (sm_90a) retrain hot path of AlexIoannides/bodywork-mlops-demo (stage_1's least-squares fit).
 
 Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- the directory name
 ``bodywork-mlops-demo_b200`` is not a valid Python identifier).

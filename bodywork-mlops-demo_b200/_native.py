@@ -1,7 +1,7 @@
 """ctypes binding of libb2gram.so (include/b2gram.h) and a thin object wrapper.
 
 There is deliberately no CPU implementation behind these calls: if the shared library is missing
-or no B200 is visible, every compute entry point raises ``RuntimeError`` (the reference's error
+or no H100 is visible, every compute entry point raises ``RuntimeError`` (the reference's error
 style, stage_1_train_model.py:74,125,142).
 """
 from __future__ import annotations
@@ -321,7 +321,7 @@ class Context:
 
     def copy_bandwidth_gbs(self, nbytes: int = 2 << 30, reps: int = 10) -> float:
         """This GPU's device-to-device copy bandwidth (read + write bytes per second, GB/s, best of ``reps``) -- the quantity
-        MEASURED_PEAKS.json holds for the pool; boxes differ."""
+        bench.py reports next to the data-sheet figure."""
         a, b = DeviceArray(self, (nbytes,), "u8"), DeviceArray(self, (nbytes,), "u8")
         try:
             _check(load().b2_dev_memset(self._h, a.ptr, 1, nbytes), "b2_dev_memset")

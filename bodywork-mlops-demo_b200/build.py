@@ -1,4 +1,4 @@
-"""Build libb2gram.so (sm_100a) in-tree with nvcc.  No torch, no JIT cache: the .so ships with the tree."""
+"""Build libb2gram.so (sm_90a, H100) in-tree with nvcc.  No torch, no JIT cache: the .so ships with the tree."""
 from __future__ import annotations
 
 import glob
@@ -12,7 +12,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb2gram.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "-Xptxas", "-v",

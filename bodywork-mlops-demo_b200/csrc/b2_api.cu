@@ -1,5 +1,5 @@
 // b2_api.cu -- the C-ABI of libb2gram.so (declared in include/b2gram.h): context, caller-buffer
-// helpers, dispatch between the tcgen05 and CUDA-core Gram kernels, host-streamed accumulation
+// helpers, dispatch between the tensor-core and CUDA-core Gram kernels, host-streamed accumulation
 // (pinned ring -> HBM staging, copy/compute overlap), NCCL all-reduce of the statistic, timing.
 #include <dlfcn.h>
 #include <math.h>
@@ -111,7 +111,7 @@ int gram_block(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t 
   const bool nw_ok = gram_narrow_supported(X, x_dtype, y, n, d, ldx, mask);
   int mode = ctx->kernel_mode;
   if (mode == B2_KERNEL_TCGEN05 && !tc_ok) {
-    set_error("tcgen05 path needs d%%4==0 (fp32) / d%%8==0 (bf16), 16-byte aligned X/y/mask/row pitch, n>=32");
+    set_error("tensor-core path needs d%%4==0 (fp32) / d%%8==0 (bf16), 16-byte aligned X/y/mask/row pitch, n>=32");
     return B2_E_UNSUPPORTED;
   }
   if (mode == B2_KERNEL_NARROW && !nw_ok) {
@@ -174,7 +174,7 @@ static int copy_threads() {
 }
 
 void parallel_copy_rows(char* dst, const char* src, int64_t rows, size_t row_bytes, size_t src_pitch) {
-  // copy threads: half the hardware threads, at most 16 (measured on the 64-thread GPU box, tools/perf_pageable.py);
+  // copy threads: half the hardware threads, at most 16;
   // B2_COPY_THREADS overrides
   int nt = copy_threads();
   if ((size_t)rows * row_bytes < ((size_t)8 << 20)) nt = 1;
@@ -316,8 +316,8 @@ int b2_ctx_create(int device, b2_ctx** out) {
   B2_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; libb2gram is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; libb2gram is built for sm_90a (H100) only", device, prop.major, prop.minor);
     return B2_E_UNSUPPORTED;
   }
   b2_ctx* ctx = new (std::nothrow) b2_ctx();

@@ -18,7 +18,7 @@ constexpr size_t kXchgSlotDoubles = (size_t)kMaxS * kMaxS;                 // on
 constexpr size_t kXchgDataDoubles = 2 * kMaxRanks * kXchgSlotDoubles;       // two epochs (parity) x ranks
 constexpr size_t kXchgBytes = kXchgDataDoubles * sizeof(double) + 256;      // + flags[8] (u32) + ticket
 
-// ---- tcgen05 Gram kernel geometry (gram_tc.cu) ------------------------------------------
+// ---- tensor-core Gram kernel geometry (gram_tc.cu) --------------------------------------
 constexpr int kTcRows = 64;              // rows of X per pipeline stage (4 MMA K-steps of 16)
 constexpr int kTcM = 128;                // MMA M: feature index (zero padded)
 constexpr int kTcN = 144;                // MMA N: 128 feature columns (hi) + 16 extra columns [1, y_hi, y_lo, 0...]
@@ -59,7 +59,7 @@ struct b2_ctx {
   int d = 0;                           // feature count of the current statistic (0 = not reset)
   double* S = nullptr;                 // device, kMaxS*kMaxS (only (d+2)^2 used, row stride d+2)
 
-  // tcgen05 path scratch
+  // tensor-core path scratch
   double* tc_part = nullptr;           // [sm_count][kTcAccElems]   per-CTA fp64 partial Gram (col-major)
   double* tc_side = nullptr;           // [sm_count][kTcSideDoubles]
   double* tc_red = nullptr;            // [kTcAccElems + 16 + 129 + pad]: reduced partials, y sums, barrier slot, shift
@@ -67,7 +67,7 @@ struct b2_ctx {
   bool tc_attr_set = false;
   bool solve_attr_set = false;
   double* solve_host = nullptr;        // pinned mirror of solve_out (D2H without a staging copy)
-  // tensor-map cache of the most recent tcgen05 launch (a refit of resident rows re-uses the same maps)
+  // tensor-map cache of the most recent tensor-core launch (a refit of resident rows re-uses the same maps)
   struct TmCache {
     const void* X = nullptr; const float* y = nullptr; const uint8_t* mask = nullptr;
     int64_t n = 0, ldx = 0; int d = 0, x_dtype = -1, y_map_2d = 0;

@@ -42,15 +42,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, uint32_
     else if (now - t0 > 4000000000ull) __trap();
   }
 }
-// One lane of a converged warp.  ptxas treats a region guarded by elect.sync as single-threaded: the tcgen05.mma / TMA
-// instructions inside compile to back-to-back uniform-datapath instructions with their operands in uniform registers.
-// Guarded by `lane == 0` instead, every one of them is wrapped in an ELECT / BRA.U.ANY waterfall loop behind a chain of
-// R2UR moves.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }

@@ -5,8 +5,8 @@
 //     double slot[2 parities][kMaxRanks][kMaxS * kMaxS]      slot[e & 1][r] = rank r's partial S of exchange e
 //     u32    flag[kMaxRanks]                                 flag[r] = last exchange whose slot r is complete here
 //     u32    ticket (word 32), status (word 48)
-// A producer stores its partial into slot[e & 1][rank] of EVERY buffer (st.global on peer pointers: NVLink 5 /
-// NVSwitch), fences at system scope and then writes e into flag[rank] of every buffer; a consumer waits until all
+// A producer stores its partial into slot[e & 1][rank] of EVERY buffer (st.global on peer pointers over
+// NVLink / NVSwitch), fences at system scope and then writes e into flag[rank] of every buffer; a consumer waits until all
 // flags of its OWN buffer carry e and sums the slots in rank order (bit-identical on every rank).  Slots are double
 // buffered by parity: a rank can be at most one exchange ahead of a peer (its next wait needs that peer's next flag).
 #pragma once

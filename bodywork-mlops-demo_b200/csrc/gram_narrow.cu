@@ -3,7 +3,7 @@
 // Replaces the pass over the training rows inside LinearRegression.fit (stage_1_train_model.py:105-106) for the
 // reference's own shape (one feature, `X.reshape(-1, 1)`, stage_1_train_model.py:95) and its narrow generalisations.
 //
-// Why not the tcgen05 kernel: a D x D Gram with D <= 16 is 1..17 products per loaded float -- HBM-bound on CUDA
+// Why not the tensor-core kernel: a D x D Gram with D <= 16 is 1..17 products per loaded float -- HBM-bound on CUDA
 // cores with room to spare -- while zero-padding D to the MMA's M = 128 caps the tensor path at its tile rate
 // (0.08 of the HBM roofline at D = 8).  So: stream, do not reshape.
 //
@@ -88,8 +88,8 @@ __global__ void narrow_shift_kernel(const T* __restrict__ X, const float* __rest
   }
 }
 
-// ---- packed fp32 pairs: FFMA2 / FADD2 do two lanes of arithmetic per issue slot and are the only way to the full fp32
-// rate on sm_100 (a 3-register FFMA issues every other cycle); a pack2(v, v) operand compiles to the scalar-broadcast form
+// ---- fp32 pairs: the accumulators below are written as pairs of lanes; sm_90 has no packed fp32 arithmetic, so a pair
+// operation is two scalar FFMA / FADD (full rate on Hopper) with the same round-to-nearest result per lane
 __device__ __forceinline__ uint64_t pack2(float a, float b) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
@@ -99,14 +99,14 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& a, float& b) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 
 // ---- the kernel ----------------------------------------------------------------------------------------------

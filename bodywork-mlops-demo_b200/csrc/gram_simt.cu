@@ -1,6 +1,6 @@
 // gram_simt.cu -- CUDA-core Gram accumulator: S += [X 1 y]^T [X 1 y] with fp64 accumulation.
 //
-// Role: (1) the path for shapes the tcgen05 kernel does not take (D % 4 != 0, unaligned
+// Role: (1) the path for shapes the tensor-core kernel does not take (D % 4 != 0, unaligned
 // leading dimension, tiny tranches such as the reference's 1 440-row x 1-feature day,
 // stage_3_synthetic_data_generation.py:19); (2) the on-device cross-check of the tensor-core
 // kernel.  Products of two fp32 (or bf16) values are exact in fp64, so the only rounding is

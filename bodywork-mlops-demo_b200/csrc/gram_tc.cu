@@ -1,4 +1,4 @@
-// gram_tc.cu -- the hot kernel: row-block streaming Gram accumulator on tcgen05 (sm_100a).
+// gram_tc.cu -- the hot kernel: row-block streaming Gram accumulator on the Hopper tensor core (wgmma, sm_90a).
 //
 // Replaces the pass over the training rows inside LinearRegression.fit
 // (stage_1_train_model.py:105-106 -> sklearn/linear_model/_base.py: centre + LAPACK gelsd).
@@ -6,21 +6,19 @@
 // Data flow per CTA (persistent, one CTA per SM, contiguous range of 64-row tiles):
 //
 //   HBM --TMA (cp.async.bulk.tensor, evict-first)--> smem raw tile [64 rows][D] (+ y, + row mask)
-//     --16 transform warps: v = x - c (per-column shift), bf16 split v = hi + lo
+//     --6 transform warps: v = x - c (per-column shift), bf16 split v = hi + lo
 //     -- 1 "E" warp: extra columns E = [1, y'_hi, y'_lo] (y' = y - c_y), CUDA-core sums of y', y'^2, rows
 //     --> operands, K-major canonical layout (8 x 16 B core matrices, no swizzle; one 16-byte chunk =
-//         8 consecutive rows of X for one feature):
-//            smem  rows j = 0..127 hi | 128..143 E                      (B = [hi | E], and A = hi)
-//            D = 128:  A = lo goes to TENSOR MEMORY (tcgen05.st, lane = feature, 4 packed columns per 8 rows);
-//            D < 128:  lo is a third smem block (rows 144..271), A = lo read through a descriptor
-//     --tcgen05.mma.cta_group::1.kind::f16 (bf16 x bf16 -> fp32 in TMEM), M=128, N=144, K=16, two per K-step:
-//            D1[i][j] += sum_r hi[r][i] * [hi | E][r][j]      TMEM columns 0..143 / 144..287 (double buffered)
-//            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]      TMEM columns 288..431 (never drained mid-kernel)
+//         8 consecutive rows of X for one feature), per 8-row K group:
+//            rows j = 0..127 hi | 128..143 E | 144..271 lo          (B = [hi | E], A = hi or A = lo)
+//     --wgmma.mma_async m64n144k16 (bf16 x bf16 -> fp32 in registers); warpgroup c (c = 0, 1) owns features
+//       64c..64c+63 of both accumulators, two wgmma per K step of 16 rows:
+//            D1[i][j] += sum_r hi[r][i] * [hi | E][r][j]      drained every `drain_rows` rows
+//            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]      small zero-mean terms: drained once at the end
 //        so D1[:, :128] = hi^T hi, D2[:, :128] = lo^T hi, column 128 = sum v, columns 129/130 = sum v*y'.
-//        (TMEM columns 432..495: the two stages of the A = lo operand.)
-//     --every `drain_rows` rows: epilogue warps tcgen05.ld the D1 buffer just finished and fold it into this
-//        CTA's fp64 partial in global memory while the MMAs continue into the other D1 buffer; D2 holds
-//        only the small zero-mean lo terms, so its fp32 sums are drained once at the end.
+//     --every `drain_rows` rows the two consumer warpgroups fold D1 into this CTA's fp64 partial in global
+//        memory (L2-resident) and restart it from zero; the producer warps keep filling stages meanwhile.
+//       The 144 accumulator registers per consumer thread come from the producers (setmaxnreg).
 //
 // Why the shift and the split: the tensor core accumulates fp32 with truncation, so raw (uncentred)
 // second moments cannot reach the 1e-4 coefficient tolerance; after the shift the Gram is ~diagonal and
@@ -44,18 +42,24 @@ namespace {
 // ------------------------------------------------------------------------------------------
 constexpr int kRawStages = 4;
 constexpr int kOpStages = 2;
-constexpr int kXformWarps = 16;
-constexpr int kThreads = 32 * (8 + kXformWarps);  // warps: 0 TMA, 1 MMA(+TMEM alloc), 2-3 E, 4-7 epilogue, 8.. transform
-constexpr int kProducers = kXformWarps + 2;        // warps that fill an operand stage (transform + 2 E warps)
+constexpr int kConsumerWGs = 2;                    // warpgroups 0-1: wgmma + drain, 64 features each
+constexpr int kXformWarps = 6;
+constexpr int kThreads = 128 * (kConsumerWGs + 2); // warps: 0-7 consumers, 8 TMA, 9 E, 10-15 transform
+constexpr int kTmaWarp = 4 * kConsumerWGs, kEWarp = kTmaWarp + 1, kFirstXformWarp = kTmaWarp + 2;
+static_assert(kFirstXformWarp + kXformWarps == kThreads / 32, "warp roles");
+constexpr int kProducers = kXformWarps + 1;        // arrivals that fill an operand stage (transform warps + E warp)
+constexpr int kConsumerWarps = 4 * kConsumerWGs;   // arrivals that free an operand stage
+constexpr uint32_t kConsumerRegs = 200, kProducerRegs = 56;   // setmaxnreg split of the 128 x 512 register file
+static_assert(kConsumerRegs * 128 * kConsumerWGs + kProducerRegs * (kThreads - 128 * kConsumerWGs) <= 65536,
+              "register budget");
+constexpr int kAccRegs = kTcN / 2;                 // fp32 accumulator registers per thread (64 x 144 per warpgroup)
 constexpr int kKGroups = kTcRows / 8;              // 8-row K groups per stage
 constexpr uint32_t kRawStageBytes = kTcRows * kMaxD * 4;      // 32768 (fp32, D = 128)
 constexpr uint32_t kOpSBO = 128;                              // bytes between 8-row j groups (core matrices along M/N)
-constexpr uint32_t kOpLBO_SS = (16 + 2 + 16) * kOpSBO;        // 4352: hi | E | lo groups per K group (operands all in smem)
-constexpr uint32_t kOpLBO_TS = (16 + 2) * kOpSBO;             // 2304: hi | E only; A = lo is staged in TMEM (D = 128 path)
+constexpr uint32_t kOpLBO = (16 + 2 + 16) * kOpSBO;           // 4352: hi | E | lo groups per K group
 constexpr uint32_t kOpEOff = 16 * kOpSBO;                     // E block inside a K group
-constexpr uint32_t kOpLoOff = 18 * kOpSBO;                    // lo block inside a K group (SS layout only)
-constexpr uint32_t kOpStageBytes = kKGroups * kOpLBO_SS;      // 34816 (sized for the SS layout)
-constexpr uint32_t kTmemALoCol = 432;                         // TS: A = lo operand, 2 stages x 32 columns (432..495)
+constexpr uint32_t kOpLoOff = 18 * kOpSBO;                    // lo block inside a K group
+constexpr uint32_t kOpStageBytes = kKGroups * kOpLBO;         // 34816
 constexpr uint32_t kOffRaw = 0;
 constexpr uint32_t kOffOp = kOffRaw + kRawStages * kRawStageBytes;     // 131072
 constexpr uint32_t kOffY = kOffOp + kOpStages * kOpStageBytes;         // 200704
@@ -66,24 +70,14 @@ constexpr uint32_t kMStageBytes = 384;                                  // 64 * 
 static_assert(kMStageBytes >= kTcRows * kMaxPack && kMStageBytes % 128 == 0 && kYStageBytes % 128 == 0, "stage alignment");
 constexpr uint32_t kOffMask = kOffY + kRawStages * kYStageBytes;
 constexpr uint32_t kOffBar = kOffMask + kRawStages * kMStageBytes;
-constexpr int kNumBars = 2 * kRawStages + 2 * kOpStages + 4;
-constexpr uint32_t kOffTmemPtr = kOffBar + kNumBars * 8;
-constexpr uint32_t kOffShift = kOffTmemPtr + 16;
+constexpr int kNumBars = 2 * kRawStages + 2 * kOpStages;
+constexpr uint32_t kOffShift = kOffBar + kNumBars * 8;
 constexpr uint32_t kSmemBytes = kOffShift + (kMaxD + 4) * 4 + 1024;    // + alignment slack (~204 KB)
 static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
-constexpr uint32_t kTmemD1Stride = 144;   // D1 (A = hi) is double buffered: columns 0..143 and 144..287
-constexpr uint32_t kTmemD2Col = 288;      // D2 (A = lo): columns 288..431, accumulates for the whole kernel
-
-// instruction descriptor: D=f32, A=B=bf16, both K-major, N=144, M=128 (cute::UMMA::InstrDescriptor layout)
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kTcN >> 3) << 17) |
-                            ((uint32_t)(kTcM >> 4) << 24);
 
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;  // L2 cache hint: streaming data, read once
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar) {
@@ -104,47 +98,86 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr, uint32_t lbo) {
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) |
-         ((uint64_t)(kOpSBO >> 4) << 32) | (1ull << 46);
+// K-major, no-swizzle ("interleave") wgmma shared-memory matrix descriptor: start address, LBO = bytes between the two
+// core matrices along K (one K group to the next), SBO = bytes between 8-row core matrices along M / N
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr) {
+  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(kOpLBO >> 4) << 16) | ((uint64_t)(kOpSBO >> 4) << 32);
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// D[64 x 144] (+)= A[64 x 16] * B[16 x 144]: bf16 operands from shared memory (both K-major), fp32 accumulators in
+// registers (wgmma fragment layout); scale_d = 0 overwrites D.  Issued by all 128 threads of a warpgroup.
+__device__ __forceinline__ void wgmma_m64n144k16(float (&d)[72], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %74, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n144k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
+      " %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      " %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, "
+      " %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, "
+      " %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, "
+      "%72, %73, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// A operand from tensor memory (128 lanes x 8 columns of packed bf16 pairs per K = 16)
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128]: A K-major, B MN-major (the raw 128B-swizzled TMA tile)
+__device__ __forceinline__ void wgmma_m64n128k16_bmn(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t (&v)[4]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]: both K-major (B = the E columns)
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// MN-major, 128B-swizzled descriptor of the raw bf16 tile of the D = 128 bf16 path: two TMA boxes of [64 rows][64
+// features] (128-byte rows, 8-row swizzle atoms of 1024 bytes); LBO = bytes from features 0..63 to 64..127 (one box),
+// SBO = bytes from one 8-row K group to the next
+constexpr uint32_t kRawBoxBytes = kTcRows * 64 * 2;   // 8192
+__device__ __forceinline__ uint64_t make_raw_desc(uint32_t addr) {
+  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(kRawBoxBytes >> 4) << 16) | ((uint64_t)(1024u >> 4) << 32) |
+         (1ull << 62);
+}
 
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint32_t (&v)[4]) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
@@ -240,7 +273,7 @@ __device__ __forceinline__ void tc_reduce_range(const double* part, const double
       quarter[q * epb + e] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
     } else if (idx < e1 && idx < kRedElems) {
       // the three CUDA-core sums (sum y', sum y'^2, rows): same quarter scheme, loads 8 deep (a serial walk over the
-      // CTAs costs one L2 round trip each: 148 x ~140 ns was most of this phase)
+      // CTAs costs one L2 round trip each, ~140 ns per CTA)
       const int k = idx - kTcAccElems;
       double acc[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       int c = c0;
@@ -335,7 +368,6 @@ __device__ __forceinline__ double tc_fold_value(const double* red, const CT* c, 
   return val;
 }
 
-
 // ------------------------------------------------------------------------------------------
 // the Gram kernel
 // ------------------------------------------------------------------------------------------
@@ -344,7 +376,14 @@ __device__ __forceinline__ double tc_fold_value(const double* red, const CT* c, 
 // SPLIT = true : operands hi + lo (16 mantissa bits, the default);
 // SPLIT = false: single bf16 operand hi = rn(x - c) ("bf16-accum" mode of BASELINE.json configs[1]): half the MMAs,
 //                no lo arithmetic; the operand rounding error (2^-9 relative, zero mean) averages out as 1/sqrt(n).
-template <typename T, int DFIX, bool SPLIT>
+// RAWB (bf16 rows, D = 128, no packing): the raw TMA tile itself (128B-swizzled) is the B operand, so the transform
+//   writes only the A operands.  D1[i][j] = sum_r hi[r][i] x[r][j] (raw, unshifted x) and E1[i][e] = sum_r hi[r][i] E[r][e];
+//   the drain subtracts c_j * sum_r hi[r][i] (the ones column of E1), which leaves sum hi_i v_j with the B side exact.
+//   lo has its own accumulators (D2, E2, small zero-mean sums, drained once at the end), stored halved in the feature
+//   columns so that the fold's D2(a,b) + D2(b,a) adds sum lo_a v_b once, symmetrised -- the partial means what the other
+//   variants' partials mean.  The raw stage is
+//   held until the MMAs have read it; masked-out rows are zeroed in it (0 * NaN would poison the sums).
+template <typename T, int DFIX, bool SPLIT, bool RAWB = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                const __grid_constant__ CUtensorMap tmM, int y_map_2d, int has_mask, int keep,
@@ -358,8 +397,6 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   (void)dbg_arg;
 #endif
   const int d = DFIX ? DFIX : d_arg;
-  constexpr bool kTS = (DFIX == 128);                         // A = lo from TMEM (needs warp%4 == feature quad)
-  constexpr uint32_t kLBO = kTS ? kOpLBO_TS : kOpLBO_SS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (sbase - smem_u32(smem_raw));
@@ -370,9 +407,6 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const uint32_t bar_raw_empty = bar_raw_full + 8 * kRawStages;        // [kRawStages]
   const uint32_t bar_op_full = bar_raw_empty + 8 * kRawStages;         // [kOpStages]
   const uint32_t bar_op_empty = bar_op_full + 8 * kOpStages;           // [kOpStages]
-  const uint32_t bar_acc_full = bar_op_empty + 8 * kOpStages;          // [2]
-  const uint32_t bar_acc_empty = bar_acc_full + 16;                    // [2]
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmemPtr);
   float* shift_s = reinterpret_cast<float*>(smem + kOffShift);
 
   // contiguous tile range of this CTA
@@ -380,33 +414,23 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int64_t tile_begin = (int64_t)blockIdx.x * total_tiles / gridDim.x;
   const int64_t tile_end = (int64_t)(blockIdx.x + 1) * total_tiles / gridDim.x;
   const int my_tiles = (int)(tile_end - tile_begin);
-  const int n_chunks = (my_tiles + chunk_tiles - 1) / chunk_tiles;
 
   // ---- one-time setup --------------------------------------------------------------------
   if (threadIdx.x == 0) {
     for (int s = 0; s < kRawStages; ++s) {
       mbar_init(bar_raw_full + 8 * s, 1);
-      mbar_init(bar_raw_empty + 8 * s, kProducers);
+      mbar_init(bar_raw_empty + 8 * s, kProducers + (RAWB ? kConsumerWarps : 0));
     }
     for (int s = 0; s < kOpStages; ++s) {
       mbar_init(bar_op_full + 8 * s, kProducers);
-      mbar_init(bar_op_empty + 8 * s, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_acc_full + 8 * b, 1);
-      mbar_init(bar_acc_empty + 8 * b, 4);
+      mbar_init(bar_op_empty + 8 * s, kConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == kTmaWarp && lane == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmY);
     if (has_mask) tma_prefetch_desc(&tmM);
-  }
-  if (warp == 1) {  // TMEM: 512 columns (D1 x2 at 0 / 144, D2 at 288, TS operand A = lo at 432)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(sbase + kOffTmemPtr)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // zero the operand stages once: feature rows >= d, the unused E rows and the lo/hi padding read as 0
   for (uint32_t o = threadIdx.x * 16; o < kOpStages * kOpStageBytes; o += kThreads * 16)
@@ -417,275 +441,332 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
     shift_s[j] = (j == kMaxD) ? shift_value(shift, kMaxD, n_shift)
                               : (j < pack * d_orig ? shift_value(shift, j % d_orig, n_shift) : 0.f);
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   // ---- warp roles --------------------------------------------------------------------------
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      const uint32_t tx = (uint32_t)(kTcRows * d * sizeof(T)) + kTcRows * pack * 4 + (has_mask ? kTcRows * pack : 0);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        mbar_wait(bar_raw_empty + 8 * s, ph ^ 1, wait_ns);
-        const uint32_t full = bar_raw_full + 8 * s;
-        mbar_expect_tx(full, tx);
-        const int64_t row0 = (tile_begin + it) * kTcRows;
-        tma_load_2d(sbase + kOffRaw + s * kRawStageBytes, &tmX, 0, (int)row0, full);
-        const int sub0 = (int)row0 * pack;                               // first original row of the tile
-        if (y_map_2d) tma_load_2d(sbase + kOffY + s * kYStageBytes, &tmY, 0, sub0 >> 2, full);
-        else tma_load_1d(sbase + kOffY + s * kYStageBytes, &tmY, sub0, full);
-        if (has_mask == 2) tma_load_2d(sbase + kOffMask + s * kMStageBytes, &tmM, 0, sub0 >> 4, full);
-        else if (has_mask) tma_load_1d(sbase + kOffMask + s * kMStageBytes, &tmM, sub0, full);
-        if (++s == kRawStages) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one elected thread: straight-line UTCHMMA, see elect_one) =====
-    if (elect_one()) {
-      int os = 0;
-      uint32_t oph = 0;
-      int in_chunk = 0, chunk = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        const int b = chunk & 1;
-        if (in_chunk == 0) {  // this D1 buffer must have been drained (two chunks ago)
-          mbar_wait(bar_acc_empty + 8 * b, ((chunk >> 1) & 1) ^ 1);
-          tc_fence_after();
-        }
-        mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
-        tc_fence_after();
-        const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-        const uint32_t tmem_d1 = tmem_base + (uint32_t)b * kTmemD1Stride;
+  if (warp < kConsumerWarps) {
+    // ===== consumers: wgmma into register accumulators, fp64 drain to the CTA's partial in global =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int wg = warp >> 2;
+    if constexpr (RAWB) {
+    // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
+    // column 8 j + 2 (lane % 4) + e, in accX (columns = the 128 raw features) and in accE (columns = E); accX2 / accE2: lo
+    float accX[64], accE[8], accX2[64], accE2[8];
+    double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int col0 = 2 * (lane & 3);
+    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;
+    int os = 0, held = -1, in_chunk = 0;                   // held: the tile whose stages wait for their MMAs
+    uint32_t oph = 0;
+    bool first_chunk = true;
+    for (int it = 0; it < my_tiles; ++it) {
+      mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
+      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
+      const uint32_t raw_addr = sbase + kOffRaw + (uint32_t)(it % kRawStages) * kRawStageBytes;
+      wgmma_fence();
 #pragma unroll
-        for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
-          const uint64_t b_desc = make_smem_desc(op_addr + k2 * 2 * kLBO, kLBO);            // [hi | E], also A = hi
-          if (!(dbg & 2u)) umma_bf16(tmem_d1, b_desc, b_desc, (in_chunk > 0 || k2 > 0) ? 1u : 0u);
-          if (SPLIT && !(dbg & 3u)) {
-            if constexpr (kTS) {
-              umma_bf16_ts(tmem_base + kTmemD2Col, tmem_base + kTmemALoCol + (uint32_t)(os * 32 + k2 * 8), b_desc,
-                           (it > 0 || k2 > 0) ? 1u : 0u);
-            } else {
-              const uint64_t lo_desc = make_smem_desc(op_addr + k2 * 2 * kLBO + kOpLoOff, kLBO);   // A = lo
-              umma_bf16(tmem_base + kTmemD2Col, lo_desc, b_desc, (it > 0 || k2 > 0) ? 1u : 0u);
+      for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
+        const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
+        const uint64_t x_desc = make_raw_desc(raw_addr + k2 * 16 * 128);        // rows 16 k2 .. 16 k2 + 15
+        const uint64_t e_desc = make_smem_desc(k_addr + kOpEOff);
+        const uint64_t hi_desc = make_smem_desc(k_addr + a_off);
+        const uint32_t sc = (in_chunk > 0 || k2 > 0) ? 1u : 0u;
+        wgmma_m64n128k16_bmn(accX, hi_desc, x_desc, sc);
+        wgmma_m64n16k16(accE, hi_desc, e_desc, sc);
+        if constexpr (SPLIT) {
+          const uint64_t lo_desc = make_smem_desc(k_addr + kOpLoOff + a_off);
+          const uint32_t sc2 = (it > 0 || k2 > 0) ? 1u : 0u;
+          wgmma_m64n128k16_bmn(accX2, lo_desc, x_desc, sc2);
+          wgmma_m64n16k16(accE2, lo_desc, e_desc, sc2);
+        }
+      }
+      wgmma_commit();
+      const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
+      if (last) {
+        wgmma_wait<0>();
+        fence_regs(accX);
+        fence_regs(accE);
+      } else {
+        wgmma_wait<1>();
+      }
+      if (lane == 0) {
+        if (held >= 0) {
+          mbar_arrive(bar_op_empty + 8 * (held % kOpStages));
+          mbar_arrive(bar_raw_empty + 8 * (held % kRawStages));
+        }
+        if (last) {
+          mbar_arrive(bar_op_empty + 8 * os);
+          mbar_arrive(bar_raw_empty + 8 * (it % kRawStages));
+        }
+      }
+      held = last ? -1 : it;
+      if (last) {
+        // sum_r hi_i x_j - c_j sum_r hi_i = sum_r hi_i v_j; sum_r hi_i is E1's ones column, held by lane 4 * (lane / 4)
+        const double s1a = (double)__shfl_sync(0xffffffffu, accE[0], lane & ~3);
+        const double s1b = (double)__shfl_sync(0xffffffffu, accE[2], lane & ~3);
+#pragma unroll
+        for (int r = 0; r < 64; ++r) {
+          const int col = 8 * (r >> 2) + col0 + (r & 1);
+          const double val = (double)accX[r] - (double)shift_s[col] * (((r >> 1) & 1) ? s1b : s1a);
+          double* dst = my_part + (size_t)col * kTcM + 8 * ((r >> 1) & 1);
+          if (first_chunk) *dst = val;
+          else *dst += val;
+        }
+#pragma unroll
+        for (int r = 0; r < 8; ++r) {
+          double* dst = my_part + (size_t)(kMaxD + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1);
+          if (first_chunk) *dst = (double)accE[r];
+          else *dst += (double)accE[r];
+        }
+        first_chunk = false;
+        in_chunk = 0;
+      } else {
+        ++in_chunk;
+      }
+      if (++os == kOpStages) { os = 0; oph ^= 1; }
+    }
+    wgmma_wait<0>();
+    double* my_part2 = my_part + (size_t)kTcN * kTcM;      // partial columns [144, 288)
+    if constexpr (SPLIT) {
+      fence_regs(accX2);
+      fence_regs(accE2);
+      const double s1a = (double)__shfl_sync(0xffffffffu, accE2[0], lane & ~3);
+      const double s1b = (double)__shfl_sync(0xffffffffu, accE2[2], lane & ~3);
+#pragma unroll
+      for (int r = 0; r < 64; ++r) {
+        const int col = 8 * (r >> 2) + col0 + (r & 1);
+        my_part2[(size_t)col * kTcM + 8 * ((r >> 1) & 1)] =
+            0.5 * ((double)accX2[r] - (double)shift_s[col] * (((r >> 1) & 1) ? s1b : s1a));
+      }
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+        my_part2[(size_t)(kMaxD + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = (double)accE2[r];
+    } else {
+#pragma unroll
+      for (int r = 0; r < kAccRegs; ++r)
+        my_part2[(size_t)(8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = 0.0;
+    }
+    } else {
+    // no plain instruction may write the accumulators between wgmma (ptxas would serialise them): a chunk restarts D1,
+    // and the first tile starts D2, with scale-d = 0 on its first K step
+    float acc1[kAccRegs], acc2[kAccRegs];
+    // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
+    // column 8 j + 2 (lane % 4) + e; the partial is column-major [col][feature]
+    double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int col0 = 2 * (lane & 3);
+    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;      // this warpgroup's 64 features of A
+    int os = 0, held = -1, in_chunk = 0;
+    uint32_t oph = 0;
+    bool first_chunk = true;
+    for (int it = 0; it < my_tiles; ++it) {
+      mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
+      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
+        const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
+        const uint64_t b_desc = make_smem_desc(k_addr);                        // [hi | E]
+        if (!(dbg & 2u))                                                                        // A = hi
+          wgmma_m64n144k16(acc1, make_smem_desc(k_addr + a_off), b_desc, (in_chunk > 0 || k2 > 0) ? 1u : 0u);
+        if (SPLIT && !(dbg & 3u))                                                               // A = lo
+          wgmma_m64n144k16(acc2, make_smem_desc(k_addr + kOpLoOff + a_off), b_desc, (it > 0 || k2 > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
+      // the previous tile's MMAs are complete after wait_group 1 (this tile's too after wait_group 0): free their stages;
+      // the last tile of the range is always `last`, so the accumulators are settled when the loop ends
+      if (last) {
+        wgmma_wait<0>();
+        fence_regs(acc1);
+        if constexpr (SPLIT) fence_regs(acc2);
+      } else {
+        wgmma_wait<1>();
+      }
+      if (lane == 0) {
+        if (held >= 0) mbar_arrive(bar_op_empty + 8 * held);
+        if (last) mbar_arrive(bar_op_empty + 8 * os);
+      }
+      held = last ? -1 : os;
+      if (last) {
+        // D1 of this chunk: fold into partial columns [0, 144)
+#pragma unroll
+        for (int r = 0; r < kAccRegs; ++r) {
+          double* dst = my_part + (size_t)(8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1);
+          if (first_chunk) *dst = (double)acc1[r];
+          else *dst += (double)acc1[r];
+        }
+        first_chunk = false;
+        in_chunk = 0;
+      } else {
+        ++in_chunk;
+      }
+      if (++os == kOpStages) { os = 0; oph ^= 1; }
+    }
+    wgmma_wait<0>();     // a no-op at run time (see above), but ptxas cannot prove it and would wait inside the loop
+    if constexpr (SPLIT) fence_regs(acc2);
+    // D2 (A = lo) accumulated over the whole range (small zero-mean sums): partial columns [144, 288)
+#pragma unroll
+    for (int r = 0; r < kAccRegs; ++r)
+      my_part[(size_t)(kTcN + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = SPLIT ? (double)acc2[r] : 0.0;
+    }
+  } else {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == kTmaWarp) {
+      // ===== TMA producer =====
+      if (lane == 0) {
+        const uint32_t tx = (uint32_t)(kTcRows * d * sizeof(T)) + kTcRows * pack * 4 + (has_mask ? kTcRows * pack : 0);
+        int s = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < my_tiles; ++it) {
+          mbar_wait(bar_raw_empty + 8 * s, ph ^ 1, wait_ns);
+          const uint32_t full = bar_raw_full + 8 * s;
+          mbar_expect_tx(full, tx);
+          const int64_t row0 = (tile_begin + it) * kTcRows;
+          tma_load_2d(sbase + kOffRaw + s * kRawStageBytes, &tmX, 0, (int)row0, full);
+          if constexpr (RAWB) tma_load_2d(sbase + kOffRaw + s * kRawStageBytes + kRawBoxBytes, &tmX, 64, (int)row0, full);
+          const int sub0 = (int)row0 * pack;                               // first original row of the tile
+          if (y_map_2d) tma_load_2d(sbase + kOffY + s * kYStageBytes, &tmY, 0, sub0 >> 2, full);
+          else tma_load_1d(sbase + kOffY + s * kYStageBytes, &tmY, sub0, full);
+          if (has_mask == 2) tma_load_2d(sbase + kOffMask + s * kMStageBytes, &tmM, 0, sub0 >> 4, full);
+          else if (has_mask) tma_load_1d(sbase + kOffMask + s * kMStageBytes, &tmM, sub0, full);
+          if (++s == kRawStages) { s = 0; ph ^= 1; }
+        }
+      }
+    } else if (warp == kEWarp) {
+      // ===== E warp: extra operand columns [1, y'_hi, y'_lo] and the CUDA-core sums of y' =====
+      const float c_y = shift_s[kMaxD];
+      double sy = 0.0, syy = 0.0, cnt = 0.0;
+      int rs = 0, os = 0;
+      uint32_t rph = 0, oph = 0;
+      for (int it = 0; it < my_tiles; ++it) {
+        mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
+        mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
+        const int64_t row0 = (tile_begin + it) * kTcRows;
+        const uint32_t y_addr = sbase + kOffY + rs * kYStageBytes;
+        const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
+        const uint32_t e_addr = sbase + kOffOp + os * kOpStageBytes + kOpEOff;
+        const int64_t left = n_rows - row0;
+        const int rows_valid = left < kTcRows ? (int)left : kTcRows;
+        float a = 0.f, b = 0.f, c = 0.f;
+        for (int half = 0; half < kTcRows / 32; ++half) {   // one super-row per lane and half
+          const int rr = lane + 32 * half;                  // super-row inside the tile
+          const uint32_t dst = e_addr + (rr >> 3) * kOpLBO + (rr & 7) * 2;
+          for (int bl = 0; bl < pack; ++bl) {               // original row rr * pack + bl -> E columns 3*bl .. 3*bl+2
+            const int sub = rr * pack + bl;
+            bool use = rr < rows_valid;
+            if (use && has_mask) use = (ld_shared_u8(m_addr + sub) == (uint32_t)keep);
+            const float yv = use ? ld_shared_f32(y_addr + sub * 4) - c_y : 0.f;
+            uint32_t yh, yl;
+            split2(yv, 0.f, yh, yl);
+            st_shared_u16(dst + (3 * bl) * 16, use ? 0x3F80u : 0u);   // bf16(1.0): row-validity ("ones") column
+            st_shared_u16(dst + (3 * bl + 1) * 16, yh);
+            st_shared_u16(dst + (3 * bl + 2) * 16, yl);
+            if (RAWB && has_mask && !use) {         // the raw row is a B operand: clear it (both boxes)
+              const uint32_t row = sbase + kOffRaw + rs * kRawStageBytes + (uint32_t)rr * 128;
+              const uint32_t z[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+              for (int q = 0; q < 8; ++q) { st_shared_v4(row + 16 * q, z); st_shared_v4(row + kRawBoxBytes + 16 * q, z); }
+            }
+            a += yv;
+            b = fmaf(yv, yv, b);
+            c += use ? 1.f : 0.f;
+          }
+        }
+        sy += (double)a; syy += (double)b; cnt += (double)c;
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(bar_op_full + 8 * os);
+          mbar_arrive(bar_raw_empty + 8 * rs);
+        }
+        if (++rs == kRawStages) { rs = 0; rph ^= 1; }
+        if (++os == kOpStages) { os = 0; oph ^= 1; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        sy += __shfl_xor_sync(0xffffffffu, sy, o);
+        syy += __shfl_xor_sync(0xffffffffu, syy, o);
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+      }
+      if (lane == 0) {
+        double* ys = side + (size_t)blockIdx.x * kTcSideDoubles;
+        ys[0] = sy; ys[1] = syy; ys[2] = cnt;
+        ys[3] = 0.0; ys[4] = 0.0; ys[5] = 0.0;
+      }
+    } else {
+      // ===== transform: shift, bf16 hi/lo split, K-major operand store =====
+      // A task = (feature quad q of 32 features, 8-row group g) of a tile: nq * 8 tasks per tile over the transform warps.
+      const int t = warp - kFirstXformWarp;
+      const int nq = (d + 31) >> 5;
+      const int n_tasks = nq * kKGroups;
+      const uint32_t esz = sizeof(T);
+      const uint32_t pitch = (uint32_t)d * esz;       // raw tile row pitch in bytes
+      int rs = 0, os = 0;
+      uint32_t rph = 0, oph = 0;
+      for (int it = 0; it < my_tiles; ++it) {
+        mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
+        mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
+        const int64_t row0 = (tile_begin + it) * kTcRows;
+        const int64_t left = n_rows - row0;
+        const int rows_valid = left < kTcRows ? (int)left : kTcRows;
+        const bool full_tile = (!has_mask) && (rows_valid == kTcRows);
+        const uint32_t raw_addr = sbase + kOffRaw + rs * kRawStageBytes;
+        const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
+        const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
+        for (int tt = t; tt < n_tasks; tt += kXformWarps) {
+          const int q = tt % nq, g = tt / nq;
+          const int i = q * 32 + lane;
+          if (i < d) {
+            const int r0 = g * 8;
+            float v[8];
+            const uint32_t src = raw_addr + (uint32_t)r0 * pitch + (uint32_t)i * esz;
+            const float c_i = shift_s[i];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              // RAWB: feature i of row r0 + k sits in box i / 64, 16-byte chunk ((i % 64) / 8) ^ k of the 128-byte row
+              const uint32_t a = RAWB ? raw_addr + (uint32_t)(i >> 6) * kRawBoxBytes + (uint32_t)(r0 + k) * 128 +
+                                            ((((uint32_t)(i & 63) >> 3) ^ (uint32_t)k) << 4) + (uint32_t)(i & 7) * 2
+                                      : src + (uint32_t)k * pitch;
+              v[k] = ((dbg & 8u) ? __uint_as_float(src + k) : raw_ld_shared<T>(a)) - c_i;
+            }
+            if (!full_tile) {
+              const int blk = i / d_orig;                   // which original row of the super-row this feature belongs to
+#pragma unroll
+              for (int k = 0; k < 8; ++k) {
+                bool use = (r0 + k) < rows_valid;
+                if (use && has_mask) use = (ld_shared_u8(m_addr + (r0 + k) * pack + blk) == (uint32_t)keep);
+                if (!use) v[k] = 0.f;
+              }
+            }
+            uint32_t hp[4], lp[4];
+#pragma unroll
+            for (int p = 0; p < 4; ++p) {
+              if constexpr (SPLIT) {
+                split2(v[2 * p], v[2 * p + 1], hp[p], lp[p]);
+              } else {
+                const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * p], v[2 * p + 1]);
+                hp[p] = *reinterpret_cast<const uint32_t*>(&h);
+                lp[p] = 0u;
+              }
+            }
+            if (!(dbg & 4u)) {
+              const uint32_t dst = op_addr + (uint32_t)g * kOpLBO + (uint32_t)((i >> 3) * kOpSBO + (i & 7) * 16);
+              st_shared_v4(dst, hp);
+              if constexpr (SPLIT) st_shared_v4(dst + kOpLoOff, lp);
             }
           }
         }
-        umma_commit(bar_op_empty + 8 * os);  // frees the operand stage when these MMAs retire
-        const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
-        if (last) { umma_commit(bar_acc_full + 8 * b); in_chunk = 0; ++chunk; }
-        else ++in_chunk;
+        if (!(dbg & 32u)) fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core (async proxy)
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(bar_op_full + 8 * os);
+          mbar_arrive(bar_raw_empty + 8 * rs);
+        }
+        if (++rs == kRawStages) { rs = 0; rph ^= 1; }
         if (++os == kOpStages) { os = 0; oph ^= 1; }
       }
     }
-  } else if (warp == 2 || warp == 3) {
-    // ===== E warps: extra operand columns [1, y'_hi, y'_lo] and the CUDA-core sums of y' =====
-    const float c_y = shift_s[kMaxD];
-    double sy = 0.0, syy = 0.0, cnt = 0.0;
-    int rs = 0, os = 0;
-    uint32_t rph = 0, oph = 0;
-    for (int it = 0; it < my_tiles; ++it) {
-      mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
-      mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
-      tc_fence_after();
-      const int64_t row0 = (tile_begin + it) * kTcRows;
-      const uint32_t y_addr = sbase + kOffY + rs * kYStageBytes;
-      const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
-      const uint32_t e_addr = sbase + kOffOp + os * kOpStageBytes + kOpEOff;
-      const int64_t left = n_rows - row0;
-      const int rows_valid = left < kTcRows ? (int)left : kTcRows;
-      // warp 2 covers super-rows 0..31 of the tile, warp 3 covers 32..63: one super-row per lane
-      float a = 0.f, b = 0.f, c = 0.f;
-      {
-        const int rr = lane + 32 * (warp - 2);      // super-row inside the tile
-        const uint32_t dst = e_addr + (rr >> 3) * kLBO + (rr & 7) * 2;
-        for (int bl = 0; bl < pack; ++bl) {         // original row rr * pack + bl -> E columns 3*bl .. 3*bl+2
-          const int sub = rr * pack + bl;
-          bool use = rr < rows_valid;
-          if (use && has_mask) use = (ld_shared_u8(m_addr + sub) == (uint32_t)keep);
-          const float yv = use ? ld_shared_f32(y_addr + sub * 4) - c_y : 0.f;
-          uint32_t yh, yl;
-          split2(yv, 0.f, yh, yl);
-          st_shared_u16(dst + (3 * bl) * 16, use ? 0x3F80u : 0u);   // bf16(1.0): row-validity ("ones") column
-          st_shared_u16(dst + (3 * bl + 1) * 16, yh);
-          st_shared_u16(dst + (3 * bl + 2) * 16, yl);
-          a += yv;
-          b = fmaf(yv, yv, b);
-          c += use ? 1.f : 0.f;
-        }
-      }
-      sy += (double)a; syy += (double)b; cnt += (double)c;
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_op_full + 8 * os);
-        mbar_arrive(bar_raw_empty + 8 * rs);
-      }
-      if (++rs == kRawStages) { rs = 0; rph ^= 1; }
-      if (++os == kOpStages) { os = 0; oph ^= 1; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      sy += __shfl_xor_sync(0xffffffffu, sy, o);
-      syy += __shfl_xor_sync(0xffffffffu, syy, o);
-      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    }
-    if (lane == 0) {
-      double* ys = side + (size_t)blockIdx.x * kTcSideDoubles + 3 * (warp - 2);
-      ys[0] = sy; ys[1] = syy; ys[2] = cnt;
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===== epilogue: TMEM -> registers -> fp64 partial in global (column-major [col][feature]) =====
-    const int w = warp & 3;  // TMEM lane quadrant this warp may access
-    double* my_part = part + (size_t)blockIdx.x * kTcAccElems + w * 32 + lane;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(w * 32) << 16);
-    for (int chunk = 0; chunk < n_chunks; ++chunk) {
-      const int b = chunk & 1;
-      mbar_wait(bar_acc_full + 8 * b, (chunk >> 1) & 1);
-      tc_fence_after();
-      // D1 (A = hi) of this chunk: fold into partial columns [0, 144)
-#pragma unroll 1
-      for (int p = 0; p < kTcN / 16; ++p) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + (uint32_t)b * kTmemD1Stride + (uint32_t)(p * 16), r);
-        tmem_ld_wait();
-        double* dst = my_part + (size_t)(p * 16) * kTcM;
-        if (chunk == 0) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) dst[(size_t)j * kTcM] = (double)__uint_as_float(r[j]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) dst[(size_t)j * kTcM] += (double)__uint_as_float(r[j]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_empty + 8 * b);
-    }
-    // D2 (A = lo) accumulated over the whole range (small zero-mean sums): partial columns [144, 288)
-    tc_fence_after();
-#pragma unroll 1
-    for (int p = 0; p < kTcN / 16; ++p) {
-      uint32_t r[16];
-      if constexpr (SPLIT) {
-        tmem_ld16(lane_base + kTmemD2Col + (uint32_t)(p * 16), r);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) r[j] = 0u;     // no lo accumulator in single-operand mode
-      }
-      double* dst = my_part + (size_t)(kTcN + p * 16) * kTcM;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) dst[(size_t)j * kTcM] = (double)__uint_as_float(r[j]);
-    }
-  } else if (warp >= 8) {
-    // ===== transform: shift, bf16 hi/lo split, K-major operand store =====
-    // A task = (feature quad q, 8-row group g) of a tile; nq * 8 tasks per tile, at most 2 per warp.
-    const int t = warp - 8;
-    const int nq = (d + 31) >> 5;
-    const uint32_t esz = sizeof(T);
-    const uint32_t pitch = (uint32_t)d * esz;       // raw tile row pitch in bytes
-    bool tv[2];
-    float tc[2];
-    uint32_t tsrc[2], tdst[2];
-    int tr0[2], tblk[2];
-#pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      const int tt = t + kXformWarps * s;
-      const bool valid = tt < nq * kKGroups;
-      const int q = valid ? tt % nq : 0, g = valid ? tt / nq : 0;
-      const int i = q * 32 + lane;
-      tv[s] = valid && (i < d);
-      tc[s] = shift_s[tv[s] ? i : 0];
-      tr0[s] = g * 8;
-      tblk[s] = (tv[s] ? i : 0) / d_orig;           // which original row of the super-row this feature belongs to
-      tsrc[s] = (uint32_t)(g * 8) * pitch + (uint32_t)(tv[s] ? i : 0) * esz;
-      tdst[s] = (uint32_t)g * kLBO + (uint32_t)((i >> 3) * kOpSBO + (i & 7) * 16);
-    }
-    int rs = 0, os = 0;
-    uint32_t rph = 0, oph = 0;
-    for (int it = 0; it < my_tiles; ++it) {
-      mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
-      mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
-      tc_fence_after();
-      const int64_t row0 = (tile_begin + it) * kTcRows;
-      const int64_t left = n_rows - row0;
-      const int rows_valid = left < kTcRows ? (int)left : kTcRows;
-      const bool full_tile = (!has_mask) && (rows_valid == kTcRows);
-      const uint32_t raw_addr = sbase + kOffRaw + rs * kRawStageBytes;
-      const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
-      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-#pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        if (tv[s]) {
-          float v[8];
-          const uint32_t src = raw_addr + tsrc[s];
-          const float c_i = tc[s];
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            v[k] = ((dbg & 8u) ? __uint_as_float(src + k) : raw_ld_shared<T>(src + (uint32_t)k * pitch)) - c_i;
-          if (!full_tile) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              bool use = (tr0[s] + k) < rows_valid;
-              if (use && has_mask) use = (ld_shared_u8(m_addr + (tr0[s] + k) * pack + tblk[s]) == (uint32_t)keep);
-              if (!use) v[k] = 0.f;
-            }
-          }
-          uint32_t hp[4], lp[4];
-#pragma unroll
-          for (int p = 0; p < 4; ++p) {
-            if constexpr (SPLIT) {
-              split2(v[2 * p], v[2 * p + 1], hp[p], lp[p]);
-            } else {
-              const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * p], v[2 * p + 1]);
-              hp[p] = *reinterpret_cast<const uint32_t*>(&h);
-              lp[p] = 0u;
-            }
-          }
-          if (!(dbg & 4u)) {
-            st_shared_v4(op_addr + tdst[s], hp);
-            if constexpr (!SPLIT) {
-              // single-operand mode: no lo block / TMEM operand
-            } else if constexpr (kTS) {
-              // lane l of this warp owns TMEM lane 32*(warp%4)+l == feature i; K group g -> 4 packed columns
-              tmem_st4(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + kTmemALoCol +
-                           (uint32_t)(os * 32 + (tr0[s] >> 3) * 4), lp);
-            } else {
-              st_shared_v4(op_addr + tdst[s] + kOpLoOff, lp);
-            }
-          }
-        }
-      }
-      if constexpr (kTS && SPLIT) {
-        tmem_st_wait();
-        tc_fence_before();
-      }
-      if (!(dbg & 32u)) fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_op_full + 8 * os);
-        mbar_arrive(bar_raw_empty + 8 * rs);
-      }
-      if (++rs == kRawStages) { rs = 0; rph ^= 1; }
-      if (++os == kOpStages) { os = 0; oph ^= 1; }
-    }
-  }
-
-  // ---- teardown ---------------------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
-
-#include "gram_tc_b16.cuh"
-#include "gram_tc_b16_split.cuh"
 
 // ------------------------------------------------------------------------------------------
 // finalize: tc_reduce_kernel sums the per-CTA partials in CTA order (deterministic)
@@ -706,8 +787,8 @@ struct TcFinal {
 // shift in fp64 and fold into S, store S into the peers' exchange slots (b2_fit with an attached peer exchange), and
 // -- through a last-block ticket -- publish the exchange flags and re-arm the barrier.  Cooperative launch: every CTA
 // is resident, so the counter barrier is safe.  This work deliberately does NOT live in the Gram kernel's tail: with
-// it there (even out of line) the hot role loops lost 5 % (same box: 0.807 ms without, 0.849 ms with, 10 M x 128
-// rows) -- more than the launch it saves.
+// it there the hot role loops carry its registers and
+// code; a separate launch keeps them lean.
 constexpr int kFinalizeThreads = 1024;                           // 4 threads per element of the partials
 constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinalizeThreads / 4);   // 145: one pass
 
@@ -719,7 +800,7 @@ tc_finalize_kernel(const double* part, const double* side, int n_ctas, double* r
   __shared__ float c_part[kShiftBlocks * kShiftStride];          // the 64 partial sums of the shift sample (33 KB)
   // the same values shift_value() gives the Gram kernel -- same operands, same order of the 64 additions -- but with
   // all loads of the CTA in flight at once: the serial walk (8 batches of dependent-latency loads by 129 threads while
-  // 895 wait at the next barrier) was 40 % of this kernel (profiles/r02_tc_finalize_summary.txt)
+  // 895 wait at the next barrier) dominated this kernel
   for (int idx = threadIdx.x; idx < kShiftBlocks * kShiftStride; idx += blockDim.x) c_part[idx] = __ldg(shift + idx);
   __syncthreads();
   for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x) {
@@ -792,7 +873,7 @@ bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, in
 }
 
 // d: inner extent of the (super-)row tensor; d_box: inner extent of the smem tile (> d: the rest is zero fill)
-// swz64: the bf16 D = 128 kernel's raw layout -- [64 rows][64 features] boxes (128-byte rows) with SWIZZLE_128B
+// swz64: the raw tile of the bf16 D = 128 path -- [64 rows][64 features] boxes (128-byte rows) with SWIZZLE_128B
 static int encode_maps(PFN_encodeTiled encode, const void* X, int x_dtype, int es, const float* y, int64_t n, int d,
                        int d_box, int64_t ldx, int64_t n_y, int pack, const uint8_t* mask, bool swz64, CUtensorMap* tmX_out,
                        CUtensorMap* tmY_out, CUtensorMap* tmM_out, int* y_map_2d_out, int* m_map_2d_out) {
@@ -842,7 +923,7 @@ static int encode_maps(PFN_encodeTiled encode, const void* X, int x_dtype, int e
     }
   }
   if (mask != nullptr && (reinterpret_cast<uintptr_t>(mask) & 15) != 0) {
-    set_error("row_mask must be 16-byte aligned for the tcgen05 path");
+    set_error("row_mask must be 16-byte aligned for the tensor-core path");
     return B2_E_ARG;
   }
   int m_map_2d = 0;
@@ -911,10 +992,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   const int d_tensor = d_in * pack;                     // columns that exist; the tile is zero-filled beyond them
   const int64_t ldx = ldx_in * pack;
   const int64_t n_y = n_main;                           // y / mask elements covered by the tensor maps
-  // bf16-stored rows with D = 128 take their own kernels (gram_tc_b16.cuh: single operand, gram_tc_b16_split.cuh: hi + lo); B2_TC_B16_GENERIC=1 keeps them on the generic
-  // kernel (diagnostic switch for same-box A/B runs)
-  static const bool b16_generic = []() { const char* e = getenv("B2_TC_B16_GENERIC"); return e != nullptr && e[0] == '1'; }();
-  const bool b16 = x_dtype == B2_BF16 && d_in == 128 && pack == 1 && !b16_generic;
+  // bf16-stored rows with D = 128: the raw tile is the MMA's B operand (RAWB)
+  const bool rawb = x_dtype == B2_BF16 && d_in == 128 && pack == 1;
   CUtensorMap tmX, tmY, tmM;
   int y_map_2d = 0, m_map_2d = 0;
   b2_ctx::TmCache& tc = ctx->tm_cache;
@@ -924,7 +1003,7 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     memcpy(&tmX, tc.tmX, sizeof(tmX)); memcpy(&tmY, tc.tmY, sizeof(tmY)); memcpy(&tmM, tc.tmM, sizeof(tmM));
     y_map_2d = tc.y_map_2d & 1; m_map_2d = (tc.y_map_2d >> 1) & 1;
   } else {
-    if (int r = encode_maps(encode, X, x_dtype, es, y, n, d_tensor, d, ldx, n_y, pack, mask, b16, &tmX, &tmY, &tmM, &y_map_2d,
+    if (int r = encode_maps(encode, X, x_dtype, es, y, n, d_tensor, d, ldx, n_y, pack, mask, rawb, &tmX, &tmY, &tmM, &y_map_2d,
                             &m_map_2d))
       return r;
     tc.X = X; tc.y = y; tc.mask = mask; tc.n = n_in; tc.ldx = ldx_in; tc.d = d_in; tc.x_dtype = x_dtype;
@@ -935,7 +1014,9 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   const int64_t total_tiles = (n + kTcRows - 1) / kTcRows;
   const int sms = (ctx->sm_limit > 0 && ctx->sm_limit < ctx->sm_count) ? ctx->sm_limit : ctx->sm_count;
   const int grid = (int)(total_tiles < sms ? total_tiles : sms);
-  int chunk_tiles = ctx->drain_rows / kTcRows;
+  // the RAWB accumulators carry the unshifted x (sum hi_i x_j includes c_j sum hi_i): a quarter of the fp32 chain length
+  // keeps their truncation error at the level of the shifted operands' accumulators
+  int chunk_tiles = ctx->drain_rows / kTcRows / (rawb ? 4 : 1);
   if (chunk_tiles < 1) chunk_tiles = 1;
 
   if (!ctx->tc_attr_set) {
@@ -946,8 +1027,10 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     B2_SET_SMEM(__nv_bfloat16, 128, true); B2_SET_SMEM(__nv_bfloat16, 0, true);
     B2_SET_SMEM(__nv_bfloat16, 128, false); B2_SET_SMEM(__nv_bfloat16, 0, false);
 #undef B2_SET_SMEM
-    B2_CUDA(cudaFuncSetAttribute(b16::sp::gram_b16_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, b16::sp::kSmem));
-    B2_CUDA(cudaFuncSetAttribute(b16::gram_b16_single_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, b16::kSmem));
+    B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kSmemBytes));
+    B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kSmemBytes));
     ctx->tc_attr_set = true;
   }
 
@@ -982,22 +1065,16 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
 #endif
   const int pair = ctx->k_pairs % kKernelEventPairs;
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
-#define B2_LAUNCH_TC(T, DF, SP)                                                                          \
-  gram_tc_kernel<T, DF, SP><<<grid, kThreads, kSmemBytes, ctx->stream>>>(                                \
+#define B2_LAUNCH_TC(T, DF, SP, RB)                                                                      \
+  gram_tc_kernel<T, DF, SP, RB><<<grid, kThreads, kSmemBytes, ctx->stream>>>(                                \
       tmX, tmY, tmM, y_map_2d, mask != nullptr ? 1 + m_map_2d : 0, keep, n, d, pack, d_in, n_in, ctx->shift, \
       chunk_tiles,                                                                                        \
       ctx->tc_part, ctx->tc_side, wait_ns, dbg)
 #define B2_LAUNCH_TC_D(T, SP) \
-  do { if (d == 128) B2_LAUNCH_TC(T, 128, SP); else B2_LAUNCH_TC(T, 0, SP); } while (0)
+  do { if (d == 128) B2_LAUNCH_TC(T, 128, SP, false); else B2_LAUNCH_TC(T, 0, SP, false); } while (0)
   const bool split = ctx->precision == B2_PRECISION_SPLIT;
-  if (b16) {
-    const int hm = mask != nullptr ? 1 + m_map_2d : 0;
-    if (split)
-      b16::sp::gram_b16_split_kernel<<<grid, kThreads, b16::sp::kSmem, ctx->stream>>>(tmX, tmY, tmM, y_map_2d, hm, keep, n, n_in,
-                                                                                      ctx->shift, chunk_tiles, ctx->tc_part, ctx->tc_side);
-    else
-      b16::gram_b16_single_kernel<<<grid, kThreads, b16::kSmem, ctx->stream>>>(tmX, tmY, tmM, y_map_2d, hm, keep, n, n_in, ctx->shift,
-                                                                               chunk_tiles, ctx->tc_part, ctx->tc_side);
+  if (rawb) {
+    if (split) B2_LAUNCH_TC(__nv_bfloat16, 128, true, true); else B2_LAUNCH_TC(__nv_bfloat16, 128, false, true);
   } else if (x_dtype == B2_F32) {
     if (split) B2_LAUNCH_TC_D(float, true); else B2_LAUNCH_TC_D(float, false);
   } else {

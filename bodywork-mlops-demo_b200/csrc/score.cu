@@ -582,7 +582,7 @@ score_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* _
       const int64_t row0 = (int64_t)tile * G::kRows;
       // all rows of this lane first (loads, dot products, prediction store), then the statistics of all of them without
       // control flow in between: the fp64 / conversion chains of the RPT rows interleave (the kernel was issue- and
-      // dependency-bound at D = 1: profiles/r02_score_narrow_*_summary.txt)
+      // dependency-bound at D = 1)
       float yv[G::RPT];
       double pr[G::RPT];
       bool use[G::RPT];

@@ -68,8 +68,8 @@ __device__ void build_normal_equations(const double* S, int d, double alpha, int
   __syncthreads();
 }
 
-// 1/x for positive x without the library division (measured on the B200, tools/ubench_fp64.cu: a dependent `1.0 / x` is
-// ~59 cycles, an fp64 FMA 8; a reciprocal seeded through fp32 conversions is slower still, ~100): the fp64 MUFU seed
+// 1/x for positive x without the library division (a dependent `1.0 / x` is a long call sequence, several times the
+// latency of a few dependent fp64 FMAs): the fp64 MUFU seed
 // (rcp.approx.ftz.f64, ~2^-20 relative) and one cubic step y = y0 (1 + e + e^2), e = 1 - x y0 -- error e^3, below the
 // rounding of the last FMA.  MUFU + 3 dependent FMAs; the pivot recurrence of the factorisation is paced by this chain.
 __device__ __forceinline__ double rcp_pos(double x) {
@@ -99,7 +99,6 @@ struct SolveXchg {
 //   (3) trailing update A[i][j] -= sum_m M[i][m] U[j][m] (U = M D, the unscaled entries) as 8 x 8 tiles on the fp64
 //       tensor-core path (DMMA m8n8k4), 4 per tile, tiles of the lower triangle dealt round-robin to the 16 warps;
 //   (4) back substitution per block in registers: shuffle + FMA per unknown.
-// Measured per phase at D = 128 (clock64, B200): profiles/r02_solve_phases.txt.
 // A is (d+1) x (d+1) with row pitch d+1 (fp64, shared memory); row d = r^T.  U: (d+1) x 16 panel scratch.
 constexpr int kNB = 16;
 constexpr int kCholThreads = 512;
@@ -595,7 +594,7 @@ solve_eigvals_kernel(const double* S, int d, double cond, int fit_intercept, dou
     __syncthreads();
     const double tau = misc[1];
     if (tau != 0.0) {                     // block-uniform
-      // The fp64 pipe is what this phase runs on (measured: ~16 DFMA / clock / SM), so finished rows and columns are
+      // The fp64 pipe is what this phase runs on, so finished rows and columns are
       // skipped, not multiplied by zero: a warp whose 8 rows are all <= k does nothing, a 32-column group <= k is
       // jumped over (warp-uniform tests; the register-resident matrix needs compile-time column indices).
       const bool warp_live = ((tid >> 5) * 8 + 7) > k;

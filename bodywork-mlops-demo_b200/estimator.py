@@ -3,7 +3,7 @@
 ``B200LinearRegression`` keeps the constructor / ``fit`` / ``predict`` / attribute contract of
 ``sklearn.linear_model.LinearRegression`` as the reference uses it
 (stage_1_train_model.py:105-107: ``LinearRegression(fit_intercept=True)``, ``.fit(X_train, y_train)``,
-``.predict(X_test)``), with the arithmetic on the B200 through libb2gram.so.  ``alpha`` adds the
+``.predict(X_test)``), with the arithmetic on the H100 through libb2gram.so.  ``alpha`` adds the
 ridge term (alpha = 0 == the reference).
 
 ``to_sklearn()`` returns a genuine ``sklearn.linear_model.LinearRegression`` carrying our

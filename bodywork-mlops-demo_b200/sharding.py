@@ -10,7 +10,7 @@ from typing import List, Tuple
 
 import numpy as np
 
-TILE_ROWS = 64  # rows per TMA tile of the tcgen05 kernel: shard boundaries are tile aligned
+TILE_ROWS = 64  # rows per TMA tile of the tensor-core kernel: shard boundaries are tile aligned
 
 
 def shard_bounds(n_rows: int, world: int, rank: int, align: int = TILE_ROWS) -> Tuple[int, int]:

@@ -1,4 +1,4 @@
-"""B200 drop-in for the reference's ``mlops_simulation/stage_1_train_model.py``.
+"""GPU drop-in for the reference's ``mlops_simulation/stage_1_train_model.py``.
 
 Same stage contract (bodywork.yaml:8-26): run with no arguments, log to stdout, exit 0 / 1;
 same function names and return shapes as the reference module:

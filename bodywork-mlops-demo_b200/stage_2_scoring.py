@@ -32,7 +32,7 @@ def _coef_intercept(model):
 
 
 def score_batch(model, X, ctx: Optional[native.Context] = None) -> np.ndarray:
-    """``model.predict(X)`` for a fitted (sklearn or B200) linear model on the GPU; X is (B, D) or a DeviceArray."""
+    """``model.predict(X)`` for a fitted (sklearn or B200LinearRegression) linear model on the GPU; X is (B, D) or a DeviceArray."""
     ctx = ctx or default_context()
     coef, b0 = _coef_intercept(model)
     if isinstance(X, native.DeviceArray):

@@ -1,5 +1,5 @@
 /*
- * b2gram.h -- C-ABI of libb2gram.so: the B200 (sm_100a) retrain hot path of
+ * b2gram.h -- C-ABI of libb2gram.so: the H100 (sm_90a) retrain hot path of
  * AlexIoannides/bodywork-mlops-demo, i.e. the least-squares / ridge fit that
  * mlops_simulation/stage_1_train_model.py performs through scikit-learn.
  *
@@ -45,15 +45,15 @@ extern "C" {
 /* kernel selection for b2_gram_accumulate */
 #define B2_KERNEL_AUTO 0   /* d <= 16: NARROW; wider: TCGEN05; odd layouts / tiny blocks: SIMT */
 #define B2_KERNEL_SIMT 1   /* fp64-accumulating CUDA-core kernel (any D <= 128)       */
-#define B2_KERNEL_TCGEN05 2 /* TMA -> smem -> bf16 hi/lo split -> tcgen05.mma -> TMEM   */
+#define B2_KERNEL_TCGEN05 2 /* TMA -> smem -> bf16 hi/lo split -> wgmma -> registers */
 #define B2_KERNEL_NARROW 3  /* D <= 16: TMA bulk-copy pipeline -> fp32 FMA on CUDA cores */
-/* tcgen05 path requirements: 4 <= d <= 128, row bytes and row pitch multiples of 16, X / y / row_mask 16-byte
+/* tensor-core path requirements: 4 <= d <= 128, row bytes and row pitch multiples of 16, X / y / row_mask 16-byte
  * aligned, n_rows >= 64.  Contiguous rows with 17 <= d <= 64 are packed min(5, 128 / d) per 128-wide super-row.
  * narrow path requirements: d <= 16, contiguous rows (ldx == d), X / y / row_mask 16-byte aligned.
  * AUTO uses NARROW from 4096 rows and TCGEN05 from 2048 rows per call; smaller blocks (the reference's 1 440-row
  * daily tranche, stage_3_synthetic_data_generation.py:19) and every other layout take the exact fp64 SIMT kernel. */
 
-/* operand precision of the tcgen05 Gram kernel (b2_ctx_set_precision) */
+/* operand precision of the tensor-core Gram kernel (b2_ctx_set_precision) */
 #define B2_PRECISION_SPLIT 0 /* bf16 hi + lo operands (16 mantissa bits), default: coef error ~2e-6 at any n */
 #define B2_PRECISION_BF16 1  /* single bf16 operand ("bf16-accum", BASELINE.json configs[1]): error ~2.4e-2/sqrt(n) */
 
@@ -80,7 +80,7 @@ int b2_ctx_sync(b2_ctx* ctx);
 int b2_ctx_info(b2_ctx* ctx, char* name, int name_cap, int* sm_count, size_t* hbm_bytes);
 /* force a kernel family (B2_KERNEL_*); default AUTO */
 int b2_ctx_set_kernel(b2_ctx* ctx, int kernel);
-/* rows of fp32 tensor-core accumulation before a TMEM drain into fp64 (default 8192) */
+/* rows of fp32 tensor-core accumulation before the register accumulators are drained into fp64 (default 8192) */
 int b2_ctx_set_drain_rows(b2_ctx* ctx, int rows);
 /* the persistent Gram kernel uses at most n_sms SMs (0 = all): leaves room for other work on the device */
 int b2_ctx_set_sm_limit(b2_ctx* ctx, int n_sms);
@@ -218,7 +218,7 @@ int b2_comm_info(b2_ctx* ctx, int* n_ranks_out, int* rank_out, int* exchange_out
 
 /* ---- timing (CUDA events on the ctx stream) ---------------------------------------------------------
  * b2_timer_start/stop bracket any sequence of calls; *_ms is device time between the two events.
- * b2_last_kernel_ms: summed device time of the tcgen05 Gram kernel launches (one CUDA-event pair each, at most
+ * b2_last_kernel_ms: summed device time of the tensor-core Gram kernel launches (one CUDA-event pair each, at most
  * the 64 most recent) since the previous call to this function, and how many launches that sum covers. */
 int b2_timer_start(b2_ctx* ctx);
 int b2_timer_stop(b2_ctx* ctx, double* ms_out);

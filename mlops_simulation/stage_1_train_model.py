@@ -1,5 +1,5 @@
 """Entry point with the path bodywork.yaml names (``executable_module_path:
-mlops_simulation/stage_1_train_model.py``, bodywork.yaml:9): runs the B200 stage."""
+mlops_simulation/stage_1_train_model.py``, bodywork.yaml:9): runs the GPU stage."""
 import os
 import sys
 

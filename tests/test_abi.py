@@ -105,22 +105,20 @@ def test_plain_c_client_builds_against_the_header_and_refuses_to_run_on_the_cpu(
         assert "no CPU fallback" in proc.stdout
 
 
-def test_library_has_blackwell_native_sass():
-    """tcgen05 / TMA must be in the shipped binary (B200_PROFILING.md: UTC*MMA, UTMALDG, LDTM)."""
+def test_library_has_hopper_native_sass():
+    """wgmma / TMA must be in the shipped binary, compiled for sm_90a."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", b2.native.lib_path()], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    # tcgen05 MMA / TMA tensor loads / TMEM loads+stores (gram_tc), TMA bulk copies and packed fp32 FMAs
-    # (gram_narrow, score kernels), mbarrier try_wait pipelines
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "STTM", "UBLKCP", "FFMA2", "SYNCS.PHASECHK.TRANS64.TRYWAIT"):
-        assert mnemonic in sass, mnemonic
-    # the bf16-storage kernel (gram_tc_b16.cuh): transposing ldmatrix, 16-lane tensor-memory stores that take the ldmatrix
-    # fragments as they are, packed bf16 subtract, mixed-precision bf16 x bf16 + fp32 FMA
-    for mnemonic in ("LDSM.16.MT88.4", "STTM.16dp128bit.x2", "HFMA2.BF16_V2", "FHFMA.BF16"):
+    assert "sm_90a" in sass
+    # wgmma from shared-memory descriptors with register accumulators, the warpgroup register split and TMA tensor loads
+    # (gram_tc), TMA bulk copies (gram_narrow, score kernels), mbarrier try_wait pipelines
+    # and, for bf16-stored D = 128 rows, the raw swizzled TMA tile as an MN-major (transposed) B operand
+    for mnemonic in ("HGMMA.64x144x16.F32.BF16", "HGMMA.64x128x16.F32.BF16", ".tnspB", "WARPGROUP.ARRIVE", "USETMAXREG",
+                     "UTMALDG", "UBLKCP", "SYNCS.PHASECHK.TRANS64.TRYWAIT"):
         assert mnemonic in sass, mnemonic
 
 

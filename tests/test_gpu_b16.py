@@ -1,6 +1,5 @@
-"""The bf16-storage D = 128 Gram kernels (csrc/gram_tc_b16_split.cuh: hi + lo operands, swizzled TMA boxes -> ldmatrix.trans
--> both A operands in tensor memory, one symmetrised accumulator; csrc/gram_tc_b16.cuh: single operand, the raw TMA tile
-is the MMA's B operand) against the fp64 oracle of the SAME bf16-rounded rows.
+"""bf16-stored D = 128 rows through the tensor-core Gram kernel (csrc/gram_tc.cu, T = bf16: hi + lo operands, or a single
+operand) against the fp64 oracle of the SAME bf16-rounded rows.
 
 Tolerances: the statistic within 2e-6 relative, the row count exact, coefficients within 2e-5 (contract 1e-4) in the
 default hi+lo mode; the single-operand mode ('bf16-accum') within the 1e-4 contract at large n only (its operand
@@ -87,8 +86,8 @@ def test_b16_mask_equals_gather_and_row_pitch(ctx, n, keep, ldx):
 
 @pytest.mark.parametrize("precision", ["split", "bf16"])
 def test_b16_dropped_rows_may_hold_nan(ctx, precision):
-    """A masked-out row never reaches the statistic, whatever it holds: the single-operand kernel feeds the RAW tile to the
-    tensor core as the B operand, so it clears dropped rows in shared memory first (0 * NaN would poison the sums)."""
+    """A masked-out row never reaches the statistic, whatever it holds: dropped rows are zeroed before they become tensor
+    core operands (0 * NaN would poison the sums)."""
     n = 50_001
     bits, Xr, y = _rows(n, seed=17)
     mask = (np.random.RandomState(3).rand(n) < 0.7).astype(np.uint8)

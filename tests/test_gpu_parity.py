@@ -3,7 +3,7 @@ produced by the unmodified reference, and size-independent properties at BASELIN
 
 Tolerances (stated once):
   * CUDA-core Gram (fp64 accumulation of exact products): S within 1e-12 relative of the fp64 oracle.
-  * tcgen05 Gram (bf16 hi/lo operands, fp32 TMEM accumulation drained every 8192 rows, fp64 beyond):
+  * tensor-core Gram (bf16 hi/lo operands, fp32 register accumulation drained every 8192 rows, fp64 beyond):
     coefficient l_inf error < 1e-4 against the fit of the same rows (BASELINE.json north_star); measured
     values are ~1e-6, asserted at 2e-5 to catch regressions.  intercept_ within 3e-2 (ill-conditioned:
     leverage x_bar * sqrt(D), SURVEY.md H1).
@@ -179,7 +179,7 @@ def _random_case(i):
 
 @pytest.mark.parametrize("i", range(48))
 def test_randomized_shapes_through_the_auto_dispatch(ctx, i):
-    """Whatever kernel AUTO picks (exact fp64 / narrow / tcgen05 / packed), the statistic is the oracle's."""
+    """Whatever kernel AUTO picks (exact fp64 / narrow / tensor core / packed), the statistic is the oracle's."""
     n, d, kind, masked = _random_case(i)
     X, y = orc.generate_dataset(n, d, seed=i, dtype=np.float32)
     mask = (np.random.RandomState(i).rand(n) < 0.8).astype(np.uint8) if masked else None
@@ -375,9 +375,8 @@ def test_score_matches_oracle(ctx, n, d):
 @pytest.mark.parametrize("n,d", [(64, 128), (20_000, 128), (70_003, 64), (33_000, 96), (12_345, 100), (50_000, 72),
                                  (40_000, 32), (25_003, 20), (30_000, 48), (9_000, 24), (15_000, 40)])
 def test_streaming_score_path_matches_oracle(ctx, n, d, kind):
-    """Wide contiguous rows go through the TMA ring (full tiles) + the register-fed kernel (tail): same numbers."""
-    if kind == "bf16" and d % 8:
-        pytest.skip("bf16 rows need d % 8 == 0 for the 16-byte pitch")
+    """Wide contiguous rows go through the TMA ring (full tiles) + the register-fed kernel (tail): same numbers.  bf16 rows
+    whose pitch is not a multiple of 16 bytes (d = 100, 20) take the register-fed kernel for every row."""
     X, y = orc.generate_dataset(n, d, seed=n + 1, dtype=np.float32)
     if kind == "bf16":
         bits = b2.native.to_bf16_bits(X)
@@ -764,7 +763,7 @@ def test_strided_rows_ldx_greater_than_d(ctx, kernel):
 
 
 def test_unaligned_buffers_fall_back_to_the_simt_kernel(ctx):
-    """AUTO picks the CUDA-core kernel when X / y are not 16-byte aligned; forcing tcgen05 is refused."""
+    """AUTO picks the CUDA-core kernel when X / y are not 16-byte aligned; forcing the tensor-core kernel is refused."""
     n, d = 10_000, 8
     X, y = orc.generate_dataset(n + 1, d, seed=13, dtype=np.float32)
     Xd, yd = ctx.to_device(X), ctx.to_device(y)
@@ -775,7 +774,7 @@ def test_unaligned_buffers_fall_back_to_the_simt_kernel(ctx):
     ctx.set_kernel(b2.KERNEL_TCGEN05)
     ctx.gram_reset(d)
     assert _raw_accumulate(ctx, xp, yp, n, d, d) == -6      # B2_E_UNSUPPORTED
-    assert "tcgen05 path needs" in b2.native.last_error()
+    assert "tensor-core path needs" in b2.native.last_error()
     ctx.set_kernel(b2.KERNEL_AUTO)
 
 

@@ -38,7 +38,7 @@ if which in ("all", "narrow"):
         for a in (Xnd, ynd, mnd): a.free()
     ctx.set_kernel(b2.KERNEL_AUTO)
 if which in ("all", "packed"):
-    # packed super-rows on the tcgen05 path (pack = 5 with the 2-D mask view, pack = 3) and the streaming scorer
+    # packed super-rows on the tensor-core path (pack = 5 with the 2-D mask view, pack = 3) and the streaming scorer
     for d in (24, 40, 64):
         Xp, yp = orc.generate_dataset(6000 + d, d, seed=20 + d, dtype=np.float32)
         mp = (np.arange(len(yp)) % 3 != 0).astype(np.uint8)
@@ -67,7 +67,7 @@ if which in ("all", "fit"):
     print("metrics", ctx.metrics(y.astype(np.float64), y.astype(np.float64) * 1.01)[5])
     Xt, yt, kept = ctx.synth_tranche(5000, 7, seed=5); print("tranche", kept); Xt.free(); yt.free()
 if which in ("all", "b16"):
-    # bf16-stored rows, D = 128: gram_b16_kernel (ldmatrix.trans, tcgen05.st.16x128b, merged accumulator), both operand
+    # bf16-stored rows, D = 128: the raw swizzled tile as the wgmma B operand, one merged accumulator, both operand
     # modes, with a mask and a ragged last tile, short drain interval
     Xb = b2.native.to_bf16_bits(X)
     Xbd = ctx.to_device(Xb, "bf16")
