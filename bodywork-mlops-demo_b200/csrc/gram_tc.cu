@@ -6,8 +6,9 @@
 // Data flow per CTA (persistent, one CTA per SM, contiguous range of 64-row tiles):
 //
 //   HBM --TMA (cp.async.bulk.tensor, evict-first)--> smem raw tile [64 rows][D] (+ y, + row mask)
-//     --6 transform warps: v = x - c (per-column shift), bf16 split v = hi + lo
-//     -- 1 "E" warp: extra columns E = [1, y'_hi, y'_lo] (y' = y - c_y), CUDA-core sums of y', y'^2, rows
+//     --8 transform warps (two per SM sub-partition; one lane of one of them also issues the TMA loads):
+//        v = x - c (per-column shift), bf16 split v = hi + lo;
+//        one of them also writes the extra columns E = [1, y'_hi, y'_lo] (y' = y - c_y), CUDA-core sums of y', y'^2, rows
 //     --> operands, K-major canonical layout (8 x 16 B core matrices, no swizzle; one 16-byte chunk =
 //         8 consecutive rows of X for one feature), per 8-row K group:
 //            rows j = 0..127 hi | 128..143 E | 144..271 lo          (B = [hi | E], A = hi or A = lo)
@@ -40,18 +41,15 @@ namespace {
 // ------------------------------------------------------------------------------------------
 // geometry
 // ------------------------------------------------------------------------------------------
-constexpr int kRawStages = 4;
-constexpr int kOpStages = 2;
 constexpr int kConsumerWGs = 2;                    // warpgroups 0-1: wgmma + drain, 64 features each
-constexpr int kXformWarps = 6;
-constexpr int kThreads = 128 * (kConsumerWGs + 2); // warps: 0-7 consumers, 8 TMA, 9 E, 10-15 transform
-constexpr int kTmaWarp = 4 * kConsumerWGs, kEWarp = kTmaWarp + 1, kFirstXformWarp = kTmaWarp + 2;
+constexpr int kXformWarps = 8;                     // warpgroups 2-3: transform, two warps on each SM sub-partition
+constexpr int kThreads = 128 * (kConsumerWGs + 2); // warps: 0-7 consumers, 8-15 transform
+constexpr int kFirstXformWarp = 4 * kConsumerWGs;
+constexpr int kTmaWarp = kFirstXformWarp;          // its lane 0 also issues the TMA loads (sub-partition 0)
+constexpr int kEWarp = kFirstXformWarp + 1;        // also writes E and sums y' (sub-partition 1)
 static_assert(kFirstXformWarp + kXformWarps == kThreads / 32, "warp roles");
-constexpr int kProducers = kXformWarps + 1;        // arrivals that fill an operand stage (transform warps + E warp)
+constexpr int kProducers = kXformWarps;            // arrivals that fill an operand stage
 constexpr int kConsumerWarps = 4 * kConsumerWGs;   // arrivals that free an operand stage
-constexpr uint32_t kConsumerRegs = 200, kProducerRegs = 56;   // setmaxnreg split of the 128 x 512 register file
-static_assert(kConsumerRegs * 128 * kConsumerWGs + kProducerRegs * (kThreads - 128 * kConsumerWGs) <= 65536,
-              "register budget");
 constexpr int kAccRegs = kTcN / 2;                 // fp32 accumulator registers per thread (64 x 144 per warpgroup)
 constexpr int kKGroups = kTcRows / 8;              // 8-row K groups per stage
 constexpr uint32_t kRawStageBytes = kTcRows * kMaxD * 4;      // 32768 (fp32, D = 128)
@@ -60,20 +58,42 @@ constexpr uint32_t kOpLBO = (16 + 2 + 16) * kOpSBO;           // 4352: hi | E | 
 constexpr uint32_t kOpEOff = 16 * kOpSBO;                     // E block inside a K group
 constexpr uint32_t kOpLoOff = 18 * kOpSBO;                    // lo block inside a K group
 constexpr uint32_t kOpStageBytes = kKGroups * kOpLBO;         // 34816
-constexpr uint32_t kOffRaw = 0;
-constexpr uint32_t kOffOp = kOffRaw + kRawStages * kRawStageBytes;     // 131072
-constexpr uint32_t kOffY = kOffOp + kOpStages * kOpStageBytes;         // 200704
 constexpr int kMaxPack = 5;                                             // original rows per 128-wide super-row (3 E columns each)
 constexpr uint32_t kYStageBytes = kTcRows * kMaxPack * 4;               // 1280
 constexpr uint32_t kMStageBytes = 384;                                  // 64 * kMaxPack = 320 mask bytes, padded: TMA
                                                                         // destinations are 128-byte aligned
 static_assert(kMStageBytes >= kTcRows * kMaxPack && kMStageBytes % 128 == 0 && kYStageBytes % 128 == 0, "stage alignment");
-constexpr uint32_t kOffMask = kOffY + kRawStages * kYStageBytes;
-constexpr uint32_t kOffBar = kOffMask + kRawStages * kMStageBytes;
-constexpr int kNumBars = 2 * kRawStages + 2 * kOpStages;
-constexpr uint32_t kOffShift = kOffBar + kNumBars * 8;
-constexpr uint32_t kSmemBytes = kOffShift + (kMaxD + 4) * 4 + 1024;    // + alignment slack (~204 KB)
-static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
+
+// Pipeline depth and shared-memory layout of a variant.  The consumers hold operand stage `it` until the MMAs of it + 1
+// are issued, so with 3 operand stages the transform of it + 2 overlaps the MMAs of it + 1 instead of waiting for
+// those of `it` (3 raw + 3 operand stages: ~205 KB; 4 + 3 does not fit in 227 KB).  RAWB also holds its raw stage
+// until its MMAs have read it, so it keeps 4 raw stages (two tiles of prefetch) and 2 operand stages.
+template <bool RAWB>
+struct TcGeo {
+  static constexpr int kRawStages = RAWB ? 4 : 3;
+  static constexpr int kOpStages = RAWB ? 2 : 3;
+  // tiles the TMA issue (lane 0 of kTmaWarp) runs ahead of its own transform: before converting tile `it` it waits for
+  // the raw stage of tile it + kAhead - kRawStages.  The transform warps release tile it - 1 without waiting for this
+  // warp; RAWB's consumers release tile k only after the MMAs of k + 1 are issued, which needs this warp's transform of
+  // k + 1, so RAWB may wait for tile it - 2 at most.
+  static constexpr int kAhead = RAWB ? kRawStages - 2 : kRawStages - 1;
+  static constexpr uint32_t kOffRaw = 0;
+  static constexpr uint32_t kOffOp = kOffRaw + kRawStages * kRawStageBytes;
+  static constexpr uint32_t kOffY = kOffOp + kOpStages * kOpStageBytes;
+  static constexpr uint32_t kOffMask = kOffY + kRawStages * kYStageBytes;
+  static constexpr uint32_t kOffBar = kOffMask + kRawStages * kMStageBytes;
+  static constexpr int kNumBars = 2 * kRawStages + 2 * kOpStages;
+  static constexpr uint32_t kOffShift = kOffBar + kNumBars * 8;
+  static constexpr uint32_t kOffESum = kOffShift + (kMaxD + 4) * 4;    // kEWarp's per-lane fp64 sums [3][32]
+  static constexpr uint32_t kSmemBytes = kOffESum + 3 * 32 * 8 + 1024;  // + alignment slack (~205 KB)
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
+  // setmaxnreg split of the 64 K-register file (128 x 512 threads): 144 fp32 accumulators per consumer thread.  A
+  // transform lane holds 16 values of two features and, at runtime d, eight row addresses: 64 registers.  RAWB's
+  // consumers also hold the raw-tile descriptors and need 200, which leaves its transform (fixed pitch) 56.
+  static constexpr uint32_t kConsumerRegs = RAWB ? 200 : 192, kProducerRegs = RAWB ? 56 : 64;
+  static_assert(kConsumerRegs * 128 * kConsumerWGs + kProducerRegs * (kThreads - 128 * kConsumerWGs) <= 65536,
+                "register budget");
+};
 
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -182,6 +202,19 @@ __device__ __forceinline__ uint64_t make_raw_desc(uint32_t addr) {
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint32_t (&v)[4]) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
                : "memory");
+}
+__device__ __forceinline__ uint32_t lane_id() {   // volatile: re-read where used instead of kept in a register
+  uint32_t l;
+  asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+  return l;
+}
+__device__ __forceinline__ void st_shared_f64(uint32_t addr, double v) {
+  asm volatile("st.shared.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
+}
+__device__ __forceinline__ double ld_shared_f64(uint32_t addr) {
+  double v;
+  asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr) : "memory");
+  return v;
 }
 __device__ __forceinline__ void st_shared_u16(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)v) : "memory");
@@ -396,6 +429,9 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   constexpr uint32_t dbg = 0u;       // product build: the ablation branches compile away
   (void)dbg_arg;
 #endif
+  using G = TcGeo<RAWB>;
+  constexpr int kRawStages = G::kRawStages, kOpStages = G::kOpStages;
+  constexpr uint32_t kOffRaw = G::kOffRaw, kOffOp = G::kOffOp, kOffY = G::kOffY, kOffMask = G::kOffMask;
   const int d = DFIX ? DFIX : d_arg;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -403,11 +439,11 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  const uint32_t bar_raw_full = sbase + kOffBar;                       // [kRawStages]
+  const uint32_t bar_raw_full = sbase + G::kOffBar;                    // [kRawStages]
   const uint32_t bar_raw_empty = bar_raw_full + 8 * kRawStages;        // [kRawStages]
   const uint32_t bar_op_full = bar_raw_empty + 8 * kRawStages;         // [kOpStages]
   const uint32_t bar_op_empty = bar_op_full + 8 * kOpStages;           // [kOpStages]
-  float* shift_s = reinterpret_cast<float*>(smem + kOffShift);
+  float* shift_s = reinterpret_cast<float*>(smem + G::kOffShift);
 
   // contiguous tile range of this CTA
   const int64_t total_tiles = (n_rows + kTcRows - 1) / kTcRows;
@@ -446,7 +482,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   // ---- warp roles --------------------------------------------------------------------------
   if (warp < kConsumerWarps) {
     // ===== consumers: wgmma into register accumulators, fp64 drain to the CTA's partial in global =====
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G::kConsumerRegs));
     const int wg = warp >> 2;
     if constexpr (RAWB) {
     // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
@@ -609,43 +645,62 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       my_part[(size_t)(kTcN + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = SPLIT ? (double)acc2[r] : 0.0;
     }
   } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
-    if (warp == kTmaWarp) {
-      // ===== TMA producer =====
-      if (lane == 0) {
-        const uint32_t tx = (uint32_t)(kTcRows * d * sizeof(T)) + kTcRows * pack * 4 + (has_mask ? kTcRows * pack : 0);
-        int s = 0;
-        uint32_t ph = 0;
-        for (int it = 0; it < my_tiles; ++it) {
-          mbar_wait(bar_raw_empty + 8 * s, ph ^ 1, wait_ns);
-          const uint32_t full = bar_raw_full + 8 * s;
-          mbar_expect_tx(full, tx);
-          const int64_t row0 = (tile_begin + it) * kTcRows;
-          tma_load_2d(sbase + kOffRaw + s * kRawStageBytes, &tmX, 0, (int)row0, full);
-          if constexpr (RAWB) tma_load_2d(sbase + kOffRaw + s * kRawStageBytes + kRawBoxBytes, &tmX, 64, (int)row0, full);
-          const int sub0 = (int)row0 * pack;                               // first original row of the tile
-          if (y_map_2d) tma_load_2d(sbase + kOffY + s * kYStageBytes, &tmY, 0, sub0 >> 2, full);
-          else tma_load_1d(sbase + kOffY + s * kYStageBytes, &tmY, sub0, full);
-          if (has_mask == 2) tma_load_2d(sbase + kOffMask + s * kMStageBytes, &tmM, 0, sub0 >> 4, full);
-          else if (has_mask) tma_load_1d(sbase + kOffMask + s * kMStageBytes, &tmM, sub0, full);
-          if (++s == kRawStages) { s = 0; ph ^= 1; }
-        }
-      }
-    } else if (warp == kEWarp) {
-      // ===== E warp: extra operand columns [1, y'_hi, y'_lo] and the CUDA-core sums of y' =====
-      const float c_y = shift_s[kMaxD];
-      double sy = 0.0, syy = 0.0, cnt = 0.0;
-      int rs = 0, os = 0;
-      uint32_t rph = 0, oph = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
-        mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
-        const int64_t row0 = (tile_begin + it) * kTcRows;
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(G::kProducerRegs));
+    // ===== producers: eight transform warps, two on each SM sub-partition =====
+    // Lane 0 of kTmaWarp also issues the TMA loads, G::kAhead tiles ahead of its own transform.  kEWarp also writes the
+    // E columns [1, y'_hi, y'_lo] of the whole tile and sums y', y'^2, rows on CUDA cores: one warp, so that each
+    // lane's fp32 sum over a tile covers the same rows in the same order for every split of the work.
+    const uint32_t tx = (uint32_t)(kTcRows * d * sizeof(T)) + kTcRows * pack * 4 + (has_mask ? kTcRows * pack : 0);
+    auto issue = [&](int j) {                   // TMA loads of tile j
+      const int s = j % kRawStages;
+      mbar_wait(bar_raw_empty + 8 * s, ((uint32_t)(j / kRawStages) & 1u) ^ 1u, wait_ns);
+      const uint32_t full = bar_raw_full + 8 * s;
+      mbar_expect_tx(full, tx);
+      const int64_t row0 = (tile_begin + j) * kTcRows;
+      tma_load_2d(sbase + kOffRaw + s * kRawStageBytes, &tmX, 0, (int)row0, full);
+      if constexpr (RAWB) tma_load_2d(sbase + kOffRaw + s * kRawStageBytes + kRawBoxBytes, &tmX, 64, (int)row0, full);
+      const int sub0 = (int)row0 * pack;                               // first original row of the tile
+      if (y_map_2d) tma_load_2d(sbase + kOffY + s * kYStageBytes, &tmY, 0, sub0 >> 2, full);
+      else tma_load_1d(sbase + kOffY + s * kYStageBytes, &tmY, sub0, full);
+      if (has_mask == 2) tma_load_2d(sbase + kOffMask + s * kMStageBytes, &tmM, 0, sub0 >> 4, full);
+      else if (has_mask) tma_load_1d(sbase + kOffMask + s * kMStageBytes, &tmM, sub0, full);
+    };
+    const bool issuer = warp == kTmaWarp && lane == 0;
+    if (issuer)
+      for (int j = 0; j < G::kAhead && j < my_tiles; ++j) issue(j);
+
+    // Transform: shift, bf16 hi/lo split, K-major operand store.  A lane owns the adjacent features i, i + 1 of a
+    // 64-feature block (one 8- or 4-byte load per row); a task is (block, 8-row K group g): nb * 8 tasks per tile.
+    // nb (1 or 2) divides kXformWarps, so a warp always converts the same block and loads its shifts once per tile.
+    const int t = warp - kFirstXformWarp;
+    const int nb = (d + 63) >> 6;
+    const int i = 64 * (t % nb) + 2 * lane;
+    // Store order: the lanes of a quarter warp write 8 different 16-byte columns of the 128-byte core-matrix rows only
+    // if half of them store feature i + 1 first (features i and i + 1 share a bank group otherwise).
+    const uint32_t swp = ((uint32_t)lane >> 2) & 1u;
+    const uint32_t st_off = (uint32_t)((i >> 3) * kOpSBO + (i & 7) * 16);
+    // kEWarp's per-lane sums of y', y'^2, rows live in shared memory, and their address is recomputed where it is used:
+    // registers are what the transform is short of
+    auto esum = [&]() { return sbase + G::kOffESum + 8 * lane_id(); };
+    if (warp == kEWarp) { st_shared_f64(esum(), 0.0); st_shared_f64(esum() + 256, 0.0); st_shared_f64(esum() + 512, 0.0); }
+    int rs = 0, os = 0;
+    uint32_t rph = 0, oph = 0;
+    for (int it = 0; it < my_tiles; ++it) {
+      if (issuer && it + G::kAhead < my_tiles) issue(it + G::kAhead);
+      __syncwarp();      // reconverge kTmaWarp: its lanes must not run the transform below in two divergent passes
+      mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
+      mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
+      const int64_t row0 = (tile_begin + it) * kTcRows;
+      const int64_t left = n_rows - row0;
+      const int rows_valid = left < kTcRows ? (int)left : kTcRows;
+      const bool full_tile = (!has_mask) && (rows_valid == kTcRows);
+      const uint32_t raw_addr = sbase + kOffRaw + rs * kRawStageBytes;
+      const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
+      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
+      if (warp == kEWarp && !(dbg & 192u)) {
         const uint32_t y_addr = sbase + kOffY + rs * kYStageBytes;
-        const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
-        const uint32_t e_addr = sbase + kOffOp + os * kOpStageBytes + kOpEOff;
-        const int64_t left = n_rows - row0;
-        const int rows_valid = left < kTcRows ? (int)left : kTcRows;
+        const uint32_t e_addr = op_addr + kOpEOff;
+        const float c_y = shift_s[kMaxD];
         float a = 0.f, b = 0.f, c = 0.f;
         for (int half = 0; half < kTcRows / 32; ++half) {   // one super-row per lane and half
           const int rr = lane + 32 * half;                  // super-row inside the tile
@@ -661,7 +716,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
             st_shared_u16(dst + (3 * bl + 1) * 16, yh);
             st_shared_u16(dst + (3 * bl + 2) * 16, yl);
             if (RAWB && has_mask && !use) {         // the raw row is a B operand: clear it (both boxes)
-              const uint32_t row = sbase + kOffRaw + rs * kRawStageBytes + (uint32_t)rr * 128;
+              const uint32_t row = raw_addr + (uint32_t)rr * 128;
               const uint32_t z[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
               for (int q = 0; q < 8; ++q) { st_shared_v4(row + 16 * q, z); st_shared_v4(row + kRawBoxBytes + 16 * q, z); }
@@ -671,16 +726,81 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
             c += use ? 1.f : 0.f;
           }
         }
-        sy += (double)a; syy += (double)b; cnt += (double)c;
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(bar_op_full + 8 * os);
-          mbar_arrive(bar_raw_empty + 8 * rs);
-        }
-        if (++rs == kRawStages) { rs = 0; rph ^= 1; }
-        if (++os == kOpStages) { os = 0; oph ^= 1; }
+        const uint32_t es = esum();
+        st_shared_f64(es, ld_shared_f64(es) + (double)a);
+        st_shared_f64(es + 256, ld_shared_f64(es + 256) + (double)b);
+        st_shared_f64(es + 512, ld_shared_f64(es + 512) + (double)c);
       }
+      if (i < d && !(dbg & 128u)) {
+        float c_i[2];                               // (a volatile load: kept out of the registers live across tiles)
+        ld_vals_vec<float, 2>(sbase + G::kOffShift + 4 * (uint32_t)i, c_i);
+        for (int g = t / nb; g < kKGroups; g += kXformWarps / nb) {
+          const int r0 = g * 8;
+          float v0[8], v1[8];                       // features i, i + 1 of rows r0 .. r0 + 7
+          const uint32_t src = raw_addr + (uint32_t)r0 * ((uint32_t)d * sizeof(T)) + (uint32_t)i * sizeof(T);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            // RAWB: feature i of row r0 + k sits in box i / 64, 16-byte chunk ((i % 64) / 8) ^ k of the 128-byte row
+            const uint32_t a = RAWB ? raw_addr + (uint32_t)(i >> 6) * kRawBoxBytes + (uint32_t)(r0 + k) * 128 +
+                                          ((((uint32_t)(i & 63) >> 3) ^ (uint32_t)k) << 4) + (uint32_t)(i & 7) * 2
+                                    : src + (uint32_t)k * ((uint32_t)d * sizeof(T));
+            float x[2];
+            if (dbg & 8u) { x[0] = __uint_as_float(src + k); x[1] = __uint_as_float(src - k); }
+            else ld_vals_vec<T, 2>(a, x);
+            v0[k] = x[0] - c_i[0];
+            v1[k] = x[1] - c_i[1];
+          }
+          if (!full_tile) {
+            const int blk = i / d_orig;             // which original row of the super-row features i, i + 1 belong to
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              bool use = (r0 + k) < rows_valid;
+              if (use && has_mask) use = (ld_shared_u8(m_addr + (r0 + k) * pack + blk) == (uint32_t)keep);
+              if (!use) { v0[k] = 0.f; v1[k] = 0.f; }
+            }
+          }
+          uint32_t h0[4], l0[4], h1[4], l1[4];
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            if constexpr (SPLIT) {
+              split2(v0[2 * p], v0[2 * p + 1], h0[p], l0[p]);
+              split2(v1[2 * p], v1[2 * p + 1], h1[p], l1[p]);
+            } else {
+              const __nv_bfloat162 e0 = __floats2bfloat162_rn(v0[2 * p], v0[2 * p + 1]);
+              const __nv_bfloat162 e1 = __floats2bfloat162_rn(v1[2 * p], v1[2 * p + 1]);
+              h0[p] = *reinterpret_cast<const uint32_t*>(&e0);
+              h1[p] = *reinterpret_cast<const uint32_t*>(&e1);
+              l0[p] = l1[p] = 0u;
+            }
+          }
+          if (!(dbg & 4u)) {
+            const uint32_t dst = op_addr + (uint32_t)g * kOpLBO + st_off;
+            uint32_t f[4], s[4];                    // first / second store: feature i + swp, then i + 1 - swp
+#pragma unroll
+            for (int p = 0; p < 4; ++p) { f[p] = swp ? h1[p] : h0[p]; s[p] = swp ? h0[p] : h1[p]; }
+            st_shared_v4(dst + 16 * swp, f);
+            st_shared_v4(dst + 16 - 16 * swp, s);
+            if constexpr (SPLIT) {
+#pragma unroll
+              for (int p = 0; p < 4; ++p) { f[p] = swp ? l1[p] : l0[p]; s[p] = swp ? l0[p] : l1[p]; }
+              st_shared_v4(dst + kOpLoOff + 16 * swp, f);
+              st_shared_v4(dst + kOpLoOff + 16 - 16 * swp, s);
+            }
+          }
+        }
+      }
+      if (!(dbg & 32u)) fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core (async proxy)
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(bar_op_full + 8 * os);
+        mbar_arrive(bar_raw_empty + 8 * rs);
+      }
+      if (++rs == kRawStages) { rs = 0; rph ^= 1; }
+      if (++os == kOpStages) { os = 0; oph ^= 1; }
+    }
+    if (warp == kEWarp) {
+      const uint32_t es = esum();
+      double sy = ld_shared_f64(es), syy = ld_shared_f64(es + 256), cnt = ld_shared_f64(es + 512);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         sy += __shfl_xor_sync(0xffffffffu, sy, o);
@@ -691,78 +811,6 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         double* ys = side + (size_t)blockIdx.x * kTcSideDoubles;
         ys[0] = sy; ys[1] = syy; ys[2] = cnt;
         ys[3] = 0.0; ys[4] = 0.0; ys[5] = 0.0;
-      }
-    } else {
-      // ===== transform: shift, bf16 hi/lo split, K-major operand store =====
-      // A task = (feature quad q of 32 features, 8-row group g) of a tile: nq * 8 tasks per tile over the transform warps.
-      const int t = warp - kFirstXformWarp;
-      const int nq = (d + 31) >> 5;
-      const int n_tasks = nq * kKGroups;
-      const uint32_t esz = sizeof(T);
-      const uint32_t pitch = (uint32_t)d * esz;       // raw tile row pitch in bytes
-      int rs = 0, os = 0;
-      uint32_t rph = 0, oph = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        mbar_wait(bar_raw_full + 8 * rs, rph, wait_ns);
-        mbar_wait(bar_op_empty + 8 * os, oph ^ 1, wait_ns);
-        const int64_t row0 = (tile_begin + it) * kTcRows;
-        const int64_t left = n_rows - row0;
-        const int rows_valid = left < kTcRows ? (int)left : kTcRows;
-        const bool full_tile = (!has_mask) && (rows_valid == kTcRows);
-        const uint32_t raw_addr = sbase + kOffRaw + rs * kRawStageBytes;
-        const uint32_t m_addr = sbase + kOffMask + rs * kMStageBytes;
-        const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-        for (int tt = t; tt < n_tasks; tt += kXformWarps) {
-          const int q = tt % nq, g = tt / nq;
-          const int i = q * 32 + lane;
-          if (i < d) {
-            const int r0 = g * 8;
-            float v[8];
-            const uint32_t src = raw_addr + (uint32_t)r0 * pitch + (uint32_t)i * esz;
-            const float c_i = shift_s[i];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              // RAWB: feature i of row r0 + k sits in box i / 64, 16-byte chunk ((i % 64) / 8) ^ k of the 128-byte row
-              const uint32_t a = RAWB ? raw_addr + (uint32_t)(i >> 6) * kRawBoxBytes + (uint32_t)(r0 + k) * 128 +
-                                            ((((uint32_t)(i & 63) >> 3) ^ (uint32_t)k) << 4) + (uint32_t)(i & 7) * 2
-                                      : src + (uint32_t)k * pitch;
-              v[k] = ((dbg & 8u) ? __uint_as_float(src + k) : raw_ld_shared<T>(a)) - c_i;
-            }
-            if (!full_tile) {
-              const int blk = i / d_orig;                   // which original row of the super-row this feature belongs to
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                bool use = (r0 + k) < rows_valid;
-                if (use && has_mask) use = (ld_shared_u8(m_addr + (r0 + k) * pack + blk) == (uint32_t)keep);
-                if (!use) v[k] = 0.f;
-              }
-            }
-            uint32_t hp[4], lp[4];
-#pragma unroll
-            for (int p = 0; p < 4; ++p) {
-              if constexpr (SPLIT) {
-                split2(v[2 * p], v[2 * p + 1], hp[p], lp[p]);
-              } else {
-                const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * p], v[2 * p + 1]);
-                hp[p] = *reinterpret_cast<const uint32_t*>(&h);
-                lp[p] = 0u;
-              }
-            }
-            if (!(dbg & 4u)) {
-              const uint32_t dst = op_addr + (uint32_t)g * kOpLBO + (uint32_t)((i >> 3) * kOpSBO + (i & 7) * 16);
-              st_shared_v4(dst, hp);
-              if constexpr (SPLIT) st_shared_v4(dst + kOpLoOff, lp);
-            }
-          }
-        }
-        if (!(dbg & 32u)) fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(bar_op_full + 8 * os);
-          mbar_arrive(bar_raw_empty + 8 * rs);
-        }
-        if (++rs == kRawStages) { rs = 0; rph ^= 1; }
-        if (++os == kOpStages) { os = 0; oph ^= 1; }
       }
     }
   }
@@ -1021,16 +1069,16 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
 
   if (!ctx->tc_attr_set) {
 #define B2_SET_SMEM(T, DF, SP) \
-  B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<T, DF, SP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes))
+  B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<T, DF, SP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<false>::kSmemBytes))
     B2_SET_SMEM(float, 128, true); B2_SET_SMEM(float, 0, true);
     B2_SET_SMEM(float, 128, false); B2_SET_SMEM(float, 0, false);
     B2_SET_SMEM(__nv_bfloat16, 128, true); B2_SET_SMEM(__nv_bfloat16, 0, true);
     B2_SET_SMEM(__nv_bfloat16, 128, false); B2_SET_SMEM(__nv_bfloat16, 0, false);
 #undef B2_SET_SMEM
     B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kSmemBytes));
+                                 TcGeo<true>::kSmemBytes));
     B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kSmemBytes));
+                                 TcGeo<true>::kSmemBytes));
     ctx->tc_attr_set = true;
   }
 
@@ -1056,7 +1104,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   constexpr uint32_t wait_ns = 20000u;     // try_wait suspend hint (ns); measured insensitive 0..20000 (r01)
 #endif
 #ifdef B2_DEV_KNOBS
-  static const uint32_t dbg = []() {       // ablations: bit0 skip MMA2, bit1 skip all MMAs, bit2 skip STS, bit3 skip LDS, bit5 skip proxy fence
+  static const uint32_t dbg = []() {       // ablations: bit0 skip MMA2, bit1 skip all MMAs, bit2 skip STS, bit3 skip LDS, bit5 skip proxy fence,
+                                           // bit6 skip the E columns and the y' sums, bit7 skip the whole transform
     const char* e = getenv("B2_TC_DEBUG");
     return e ? (uint32_t)atoi(e) : 0u;
   }();
@@ -1066,7 +1115,7 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   const int pair = ctx->k_pairs % kKernelEventPairs;
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
 #define B2_LAUNCH_TC(T, DF, SP, RB)                                                                      \
-  gram_tc_kernel<T, DF, SP, RB><<<grid, kThreads, kSmemBytes, ctx->stream>>>(                                \
+  gram_tc_kernel<T, DF, SP, RB><<<grid, kThreads, TcGeo<RB>::kSmemBytes, ctx->stream>>>(                     \
       tmX, tmY, tmM, y_map_2d, mask != nullptr ? 1 + m_map_2d : 0, keep, n, d, pack, d_in, n_in, ctx->shift, \
       chunk_tiles,                                                                                        \
       ctx->tc_part, ctx->tc_side, wait_ns, dbg)
