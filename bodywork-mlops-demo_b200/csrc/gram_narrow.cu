@@ -66,7 +66,8 @@ __device__ __forceinline__ float shfl_bfly_ordered(float v, int off) {
   return r;
 }
 
-// ---- per-column shift: mean of a strided row sample (any c is algebraically exact, see narrow_fold_kernel) --------
+// ---- per-column shift: mean of the finite values of a strided row sample (any c is algebraically exact, see
+// narrow_fold_kernel) ---------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void narrow_shift_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n, int d,
                                     float* __restrict__ cvec) {
@@ -76,14 +77,21 @@ __global__ void narrow_shift_kernel(const T* __restrict__ X, const float* __rest
   const int64_t samples = n < kNwShiftSamples ? n : kNwShiftSamples;
   const int64_t stride = n / samples;
   float acc = 0.f;
+  int cnt = 0;
   for (int64_t s = lane; s < samples; s += 32) {
     const int64_t row = s * stride;
-    acc += (w < d) ? raw_ld_global<T>(X + row * d + w) : __ldg(y + row);
+    const float v = (w < d) ? raw_ld_global<T>(X + row * d + w) : __ldg(y + row);
+    const bool finite = fabsf(v) <= 3.0e38f;    // the sample ignores the row mask: a dropped row may hold NaN / Inf
+    acc += finite ? v : 0.f;
+    cnt += finite ? 1 : 0;
   }
 #pragma unroll
-  for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+  for (int off = 16; off > 0; off >>= 1) {
+    acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+  }
   if (lane == 0) {
-    cvec[w < d ? w : kNwCY] = acc / (float)samples;
+    cvec[w < d ? w : kNwCY] = cnt > 0 ? acc / (float)cnt : 0.f;
     if (w == d && d < kNwMaxDP) cvec[d] = 0.f;
   }
 }

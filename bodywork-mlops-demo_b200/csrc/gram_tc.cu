@@ -229,21 +229,31 @@ __device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_
 }
 
 // ------------------------------------------------------------------------------------------
-// per-column shift c: mean of a strided row sample (any value near the column mean will do;
+// per-column shift c: mean of the finite values of a strided row sample (any value near the column mean will do;
 // the algebra in tc_fold_kernel is exact for every c)
 // ------------------------------------------------------------------------------------------
-constexpr int kShiftBlocks = 64;                 // partial sums of the row sample, one per block
+constexpr int kShiftBlocks = 64;                 // partial means of the row sample, one per block
 constexpr int kShiftStride = kMaxD + 1;          // floats per partial: features, then y (slot kMaxD)
 
 __host__ __device__ __forceinline__ int64_t shift_samples(int64_t n) { return n < 2048 ? n : 2048; }
 
-// c_j from the 64 partial sums; bf16-representable so that (bf16 input - c) is exact in fp32.
-// Called with identical arguments by the Gram kernel and by tc_fold_kernel -> identical c.
-__device__ __forceinline__ float shift_value(const float* __restrict__ sp, int j, int64_t n) {
+// c_j from the 64 partial means (NaN: a block without a finite sample), kept in fp32: the operands carry |x - c| / sigma,
+// so a c rounded to bf16 (spacing 64 at a column mean of 1e4) would cost fp32 rows digits wherever a column's mean is
+// large against its spread.  For bf16 rows (`round_bf16`) the feature shifts are rounded to bf16: x and c then share
+// one grid, x - c is exact, and hi + lo holds it.  The Gram kernel and tc_finalize_kernel call this on the same 64
+// values -> identical c.
+__host__ __device__ __forceinline__ float shift_round(float c, bool round_bf16) {
+  return round_bf16 ? __bfloat162float(__float2bfloat16_rn(c)) : c;
+}
+__device__ __forceinline__ float shift_value(const float* sp, int j, bool round_bf16) {
   float acc = 0.f;
+  int cnt = 0;
 #pragma unroll 8
-  for (int b = 0; b < kShiftBlocks; ++b) acc += sp[b * kShiftStride + j];
-  return __bfloat162float(__float2bfloat16_rn(acc / (float)shift_samples(n)));
+  for (int b = 0; b < kShiftBlocks; ++b) {
+    const float p = sp[b * kShiftStride + j];
+    if (p == p) { acc += p; ++cnt; }
+  }
+  return shift_round(cnt > 0 ? acc / (float)cnt : 0.f, round_bf16);
 }
 
 // 64 blocks x (4 row groups x 160 columns): a thread sums 8 sample rows (one batch of loads in flight -- the rows are
@@ -256,6 +266,7 @@ __global__ void __launch_bounds__(kShiftCols * kShiftGroups)
 tc_shift_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n, int d,
                 int64_t ldx, float* __restrict__ sp) {
   __shared__ float sub[kShiftGroups][kShiftCols];
+  __shared__ int subn[kShiftGroups][kShiftCols];
   const int j = threadIdx.x % kShiftCols, g = threadIdx.x / kShiftCols;
   const int64_t samples = shift_samples(n);
   const int64_t stride = n / samples;
@@ -263,17 +274,25 @@ tc_shift_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n,
   const int64_t s0 = blockIdx.x * per;
   const int64_t s1 = (s0 + per < samples) ? s0 + per : samples;
   float acc = 0.f;
+  int cnt = 0;
   if (j <= d) {
 #pragma unroll 8
     for (int64_t s = s0 + g; s < s1; s += kShiftGroups) {
       const int64_t row = s * stride;
       const float v = (j < d) ? raw_ld_global<T>(X + row * ldx + j) : __ldg(y + row);
-      acc += (fabsf(v) <= 3.0e38f) ? v : 0.f;     // the sample ignores the row mask: a dropped row may hold NaN / Inf
+      const bool finite = fabsf(v) <= 3.0e38f;    // the sample ignores the row mask: a dropped row may hold NaN / Inf
+      acc += finite ? v : 0.f;
+      cnt += finite ? 1 : 0;
     }
   }
   sub[g][j] = acc;
+  subn[g][j] = cnt;
   __syncthreads();
-  if (g == 0 && j <= d) sp[blockIdx.x * kShiftStride + (j == d ? kMaxD : j)] = ((sub[0][j] + sub[1][j]) + sub[2][j]) + sub[3][j];
+  if (g == 0 && j <= d) {
+    const int c = subn[0][j] + subn[1][j] + subn[2][j] + subn[3][j];
+    sp[blockIdx.x * kShiftStride + (j == d ? kMaxD : j)] =
+        c > 0 ? (((sub[0][j] + sub[1][j]) + sub[2][j]) + sub[3][j]) / (float)c : __int_as_float(0x7fc00000);
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -354,7 +373,8 @@ __device__ __forceinline__ void grid_barrier(unsigned int* ctr) {
 template <typename CT>
 __device__ __forceinline__ double tc_fold_value(const double* red, const CT* c, int d, int pack, int idx) {
   const int dp = d + 2;
-  const int a = idx / dp, b = idx % dp;
+  // (a, b) and (b, a) evaluate the same expression in the same order: S is exactly symmetric
+  const int a = min(idx / dp, idx % dp), b = max(idx / dp, idx % dp);
   // D1[i][j] = red[j*128 + i], D2[i][j] = red[(144 + j)*128 + i]
   auto D1 = [&](int i, int j) { return __ldcg(red + (size_t)j * kTcM + i); };
   auto D2 = [&](int i, int j) { return __ldcg(red + (size_t)(kTcN + j) * kTcM + i); };
@@ -420,7 +440,7 @@ template <typename T, int DFIX, bool SPLIT, bool RAWB = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                const __grid_constant__ CUtensorMap tmM, int y_map_2d, int has_mask, int keep,
-               int64_t n_rows, int d_arg, int pack, int d_orig, int64_t n_shift, const float* __restrict__ shift,
+               int64_t n_rows, int d_arg, int pack, int d_orig, const float* __restrict__ shift,
                int chunk_tiles,
                double* __restrict__ part, double* __restrict__ side, uint32_t wait_ns, uint32_t dbg_arg) {
 #ifdef B2_DEV_KNOBS
@@ -474,8 +494,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   // packed rows (pack > 1): super-row feature i < pack * d_orig is original feature i % d_orig -> the shift repeats;
   // the columns from pack * d_orig to 127 are TMA out-of-bounds zero fill and keep shift 0 (they contribute nothing)
   for (int j = threadIdx.x; j <= kMaxD; j += kThreads)
-    shift_s[j] = (j == kMaxD) ? shift_value(shift, kMaxD, n_shift)
-                              : (j < pack * d_orig ? shift_value(shift, j % d_orig, n_shift) : 0.f);
+    shift_s[j] = (j == kMaxD) ? shift_value(shift, kMaxD, false)
+                              : (j < pack * d_orig ? shift_value(shift, j % d_orig, sizeof(T) == 2) : 0.f);
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -842,21 +862,17 @@ constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinaliz
 
 __global__ void __launch_bounds__(kFinalizeThreads, 1)
 tc_finalize_kernel(const double* part, const double* side, int n_ctas, double* red, const float* __restrict__ shift,
-                   int64_t n_rows, int d, int pack, double* S, unsigned int* sync, const TcFinal fin) {
+                   int d, int pack, int x_bf16, double* S, unsigned int* sync, const TcFinal fin) {
   __shared__ double quarter[kFinalizeThreads];
   __shared__ double c_s[kMaxD + 1];                              // the shift as fp64 (c_s[kMaxD]: c_y)
-  __shared__ float c_part[kShiftBlocks * kShiftStride];          // the 64 partial sums of the shift sample (33 KB)
-  // the same values shift_value() gives the Gram kernel -- same operands, same order of the 64 additions -- but with
+  __shared__ float c_part[kShiftBlocks * kShiftStride];          // the 64 partial means of the shift sample (33 KB)
+  // the same values shift_value() gives the Gram kernel -- the same function on the same 64 partials -- but with
   // all loads of the CTA in flight at once: the serial walk (8 batches of dependent-latency loads by 129 threads while
   // 895 wait at the next barrier) dominated this kernel
   for (int idx = threadIdx.x; idx < kShiftBlocks * kShiftStride; idx += blockDim.x) c_part[idx] = __ldg(shift + idx);
   __syncthreads();
-  for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x) {
-    float acc = 0.f;
-#pragma unroll 8
-    for (int b = 0; b < kShiftBlocks; ++b) acc += c_part[b * kShiftStride + j];
-    c_s[j] = (j < d || j == kMaxD) ? (double)__bfloat162float(__float2bfloat16_rn(acc / (float)shift_samples(n_rows))) : 0.0;
-  }
+  for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x)
+    c_s[j] = (j < d || j == kMaxD) ? (double)shift_value(c_part, j, x_bf16 != 0 && j < d) : 0.0;
   {
     constexpr int epb = kFinalizeThreads / 4;                    // elements per pass of a CTA
     const int per = (((kRedElems + (int)gridDim.x - 1) / (int)gridDim.x) + epb - 1) / epb * epb;
@@ -1116,7 +1132,7 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
 #define B2_LAUNCH_TC(T, DF, SP, RB)                                                                      \
   gram_tc_kernel<T, DF, SP, RB><<<grid, kThreads, TcGeo<RB>::kSmemBytes, ctx->stream>>>(                     \
-      tmX, tmY, tmM, y_map_2d, mask != nullptr ? 1 + m_map_2d : 0, keep, n, d, pack, d_in, n_in, ctx->shift, \
+      tmX, tmY, tmM, y_map_2d, mask != nullptr ? 1 + m_map_2d : 0, keep, n, d, pack, d_in, ctx->shift,       \
       chunk_tiles,                                                                                        \
       ctx->tc_part, ctx->tc_side, wait_ns, dbg)
 #define B2_LAUNCH_TC_D(T, SP) \
@@ -1155,7 +1171,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     cfg.attrs = attr; cfg.numAttrs = 1;
     const double* part_arg = ctx->tc_part; const double* side_arg = ctx->tc_side;
     const float* shift_arg = ctx->shift;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, side_arg, grid, ctx->tc_red, shift_arg, n_in, d_in, pack,
+    const int x_bf16 = x_dtype == B2_BF16 ? 1 : 0;
+    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, side_arg, grid, ctx->tc_red, shift_arg, d_in, pack, x_bf16,
                                ctx->S, ctx->tc_sync, fin));
   }
   ctx->launches += 3;

@@ -33,6 +33,9 @@ oracle function       reference it follows
                       reference's single ``X`` column to ``X0..X{D-1}``)
 ``generate_dataset``  ``generate_dataset`` stage_3_synthetic_data_generation.py:28-43, seeded and
                       generalised to D columns
+``column_table``      (no reference counterpart: seeded columns of the shapes real tables have --
+                      offset, scaled, integer / 0-1, constant, correlated -- for the kernels' precision)
+``stat_error``        (no reference counterpart: a scale-free distance between two statistics)
 ====================  =====================================================================
 
 Pinning.  The reference has no tests and no golden vectors for this path (SURVEY.md section 8c);
@@ -243,3 +246,118 @@ def generate_dataset(n: int, d: int = 1, seed: int = 0, alpha: float = 1.0, beta
         keep = y >= 0
         X, y = X[keep], y[keep]
     return np.ascontiguousarray(X.astype(dtype)), np.ascontiguousarray(y.astype(dtype))
+
+
+# --------------------------------------------------------------------------------------
+# structured columns: the shapes of real tabular features, for the kernels' precision
+# --------------------------------------------------------------------------------------
+COLUMN_FAMILIES = ("offset", "scaled", "integer", "constant", "correlated")
+
+_OFFSET_COLUMNS = ((2021.0, 1.0), (1.0e4, 1.0), (-3.0e3, 10.0), (1.0e5, 10.0))   # (mean, sigma): a year, price levels
+_SCALED_SIGMAS = (0.1, 0.3, 1.0, 3.0, 10.0)                                       # times the table's scale
+_SCALED_MEANS = (0.0, 3.0, -3.0)                                                   # in units of the column's sigma
+CONSTANT_VALUE = 2021.5                                                            # not representable in bf16
+
+
+def bf16_spacing(x) -> np.ndarray:
+    """Distance between adjacent bf16 values (8 significand bits) at |x|."""
+    a = np.maximum(np.abs(np.asarray(x, dtype=np.float64)), np.finfo(np.float32).tiny)
+    return np.exp2(np.floor(np.log2(a)) - 7.0)
+
+
+def column_table(n: int, d: int, family: str, seed: int = 0, rho: float = 0.9, scale: float = 1.0,
+                 bf16: bool = False) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Seeded float64 (X, y, sigma): n rows of d columns of one family, and each column's design spread.
+
+    offset      means 2021, 1e4, -3e3, 1e5 with sigma 1 or 10 (cycled over the columns)
+    scaled      sigma ``scale`` * (0.1 .. 10) with means 0, +3 sigma, -3 sigma; tables at scale 1e-3 and 1e3 cover
+                sigma 1e-4 .. 1e4 (one table spans two decades only: sigma ratios of 1e6 within a table would make the
+                centred Gram singular at the 1e-6 cutoff of sklearn's gelsd)
+    integer     small integers 0..9, sparse 0/1 (p = 0.05), integers -3..3
+    constant    column 0 holds CONSTANT_VALUE, the others are the offset family
+    correlated  blocks of 8 columns with pairwise correlation ``rho``, mean 0, sigma 1
+
+    Column j moves y by beta_j = b_j / sigma_j with |b_j| in [0.5, 2], so every column matters whatever its scale;
+    y = 3 + X beta + N(0, 1).  ``bf16=True``: each offset column's sigma is raised to twice the bf16 spacing at its mean,
+    so that rows stored as bf16 still vary (the caller rounds them).
+    """
+    if family not in COLUMN_FAMILIES:
+        raise ValueError(f"unknown column family {family!r}")
+    rng = np.random.RandomState(seed)
+    j = np.arange(d)
+    if family == "scaled":
+        sigma = scale * np.array([_SCALED_SIGMAS[k % len(_SCALED_SIGMAS)] for k in j])
+        mu = np.array([_SCALED_MEANS[k % len(_SCALED_MEANS)] for k in j]) * sigma
+        X = mu + sigma * rng.standard_normal((n, d))
+    elif family == "integer":
+        kind = j % 3
+        X = np.empty((n, d))
+        X[:, kind == 0] = rng.randint(0, 10, size=(n, int((kind == 0).sum())))
+        X[:, kind == 1] = (rng.rand(n, int((kind == 1).sum())) < 0.05)
+        X[:, kind == 2] = rng.randint(-3, 4, size=(n, int((kind == 2).sum())))
+        sigma = np.where(kind == 0, math.sqrt(99.0 / 12.0), np.where(kind == 1, math.sqrt(0.05 * 0.95), 2.0))
+    elif family == "correlated":
+        X = np.empty((n, d))
+        for b0 in range(0, d, 8):
+            w = min(8, d - b0)
+            common = rng.standard_normal((n, 1))
+            X[:, b0:b0 + w] = math.sqrt(rho) * common + math.sqrt(1.0 - rho) * rng.standard_normal((n, w))
+        sigma = np.ones(d)
+    else:                                           # offset, constant
+        mu = np.array([_OFFSET_COLUMNS[k % len(_OFFSET_COLUMNS)][0] for k in j])
+        sigma = np.array([_OFFSET_COLUMNS[k % len(_OFFSET_COLUMNS)][1] for k in j])
+        if bf16:
+            sigma = np.maximum(sigma, 2.0 * bf16_spacing(mu))
+        X = mu + sigma * rng.standard_normal((n, d))
+        if family == "constant":
+            X[:, 0] = CONSTANT_VALUE
+            sigma[0] = 0.0
+    b = rng.uniform(0.5, 2.0, size=d) * rng.choice([-1.0, 1.0], size=d)
+    beta = np.where(sigma > 0, b / np.where(sigma > 0, sigma, 1.0), 0.0)
+    y = 3.0 + X @ beta + rng.standard_normal(n)
+    return np.ascontiguousarray(X), y, sigma
+
+
+def centred_moments(S: np.ndarray) -> Tuple[float, np.ndarray, np.ndarray]:
+    """(n, means, C) of the statistic S: C = the centred second moments of [X y] (features 0..d-1, then y)."""
+    S = np.asarray(S, dtype=np.float64)
+    d = S.shape[0] - 2
+    idx = list(range(d)) + [d + 1]
+    n = float(S[d, d])
+    m = S[idx, d] / n
+    return n, m, S[np.ix_(idx, idx)] - n * np.outer(m, m)
+
+
+def stat_error(S: np.ndarray, So: np.ndarray, floor: float = 1e-10) -> Tuple[float, float]:
+    """Scale-free distance of a statistic S from the oracle's So, both [X 1 y]^T [X 1 y].
+
+    Returns (max_ab |C_ab - Co_ab| / sqrt(Co_aa Co_bb),  max_j |xbar_j - xbaro_j| / sigma_j) over the features and y,
+    with C the centred second moments (``centred_moments``) and sigma_j^2 = Co_jj / n.  Both are invariant to a column's
+    offset and scale, so an error in a column's centred variance counts the same whether the column has mean 0 or
+    1e5, and whether the largest entry of S is 1e3 or 1e13.  A column whose centred variance is zero (a constant) is
+    measured against ``floor`` times its raw second moment: the level at which fp64 centring of S cancels anyway.
+    """
+    _, m, C = centred_moments(S)
+    no, mo, Co = centred_moments(So)
+    d = np.asarray(So).shape[0] - 2
+    raw = np.abs(np.diag(np.asarray(So, dtype=np.float64)))[list(range(d)) + [d + 1]]
+    var = np.maximum(np.diag(Co), floor * raw)
+    stat = float(np.max(np.abs(C - Co) / np.sqrt(np.outer(var, var))))
+    mean = float(np.max(np.abs(m - mo) / np.sqrt(var / no)))
+    return stat, mean
+
+
+def centred_condition(S: np.ndarray) -> float:
+    """Condition number (largest / smallest eigenvalue) of the centred feature Gram of S."""
+    C = centred_moments(S)[2][:-1, :-1]
+    lam = np.linalg.eigvalsh(0.5 * (C + C.T))
+    return float(lam[-1] / lam[0]) if lam[0] > 0 else float("inf")
+
+
+def coef_error(coef: np.ndarray, coef_o: np.ndarray, So: np.ndarray) -> float:
+    """max_j |coef_j - coefo_j| * sigma_j (sigma_j: the oracle's spread of feature j): the largest change of a
+    prediction, in units of y, when feature j moves by one standard deviation.  For sigma = 1 columns it is the plain
+    coefficient error."""
+    no, _, Co = centred_moments(So)
+    sd = np.sqrt(np.maximum(np.diag(Co)[:-1], 0.0) / no)
+    return float(np.max(np.abs(np.asarray(coef) - np.asarray(coef_o)) * sd))

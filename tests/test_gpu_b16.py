@@ -1,7 +1,8 @@
 """bf16-stored D = 128 rows through the tensor-core Gram kernel (csrc/gram_tc.cu, T = bf16: hi + lo operands, or a single
 operand) against the fp64 oracle of the SAME bf16-rounded rows.
 
-Tolerances: the statistic within 2e-6 relative, the row count exact, coefficients within 2e-5 (contract 1e-4) in the
+Tolerances: the statistic within 2e-5 in the scale-free error of oracle.stat_error (centred moments and means; the
+largest value measured on an H100 is 9.6e-7), the row count exact, coefficients within 2e-5 (contract 1e-4) in the
 default hi+lo mode; the single-operand mode ('bf16-accum') within the 1e-4 contract at large n only (its operand
 rounding error falls as 1/sqrt(n)), so small cases check its statistic at the operand precision (2^-8).
 """
@@ -14,10 +15,17 @@ from oracle import ols_oracle as orc
 pytestmark = pytest.mark.gpu
 
 COEF_TOL = 2e-5
+SF_TOL = 2e-5        # scale-free statistic error of the tensor-core kernel (oracle.stat_error)
+SF_TOL_SINGLE = 2e-4  # the same, single bf16 operand (measured 3.6e-5)
 
 
 def _rel(a, b):
     return float(np.max(np.abs(a - b)) / max(float(np.max(np.abs(b))), 1e-300))
+
+
+def _sf(S, So):
+    """Scale-free error of the statistic S against So: the larger of oracle.stat_error's centred-moment and mean errors."""
+    return max(orc.stat_error(S, So))
 
 
 def _rows(n, seed):
@@ -61,7 +69,7 @@ def test_b16_gram_matches_oracle(ctx, n):
     So = orc.gram_stats(Xr, y)
     assert S[128, 128] == n
     assert _rel(S[:128, 128], So[:128, 128]) < 1e-6
-    assert _rel(S, So) < 2e-6
+    assert _sf(S, So) < SF_TOL
     assert np.array_equal(S, S.T)
     if n > 1000:
         ctx.gram_import(S)
@@ -77,7 +85,7 @@ def test_b16_mask_equals_gather_and_row_pitch(ctx, n, keep, ldx):
     sel = mask == keep
     So = orc.gram_stats(Xr[sel], y[sel])
     assert S[128, 128] == int(sel.sum())
-    assert _rel(S, So) < 2e-6
+    assert _sf(S, So) < SF_TOL
     assert np.array_equal(S, S.T)
     ctx.gram_import(S)
     coef, _ = ctx.solve()
@@ -102,7 +110,7 @@ def test_b16_dropped_rows_may_hold_nan(ctx, precision):
     sel = mask == 1
     So = orc.gram_stats(Xr[sel], y[sel])
     assert S[128, 128] == int(sel.sum())
-    assert _rel(S, So) < (2e-6 if precision == "split" else 2e-4)
+    assert _sf(S, So) < (SF_TOL if precision == "split" else SF_TOL_SINGLE)
 
 
 def test_b16_is_deterministic_and_additive(ctx):
@@ -119,7 +127,7 @@ def test_b16_is_deterministic_and_additive(ctx):
     parts = ctx.gram_export()
     ctx.set_kernel(b2.KERNEL_AUTO)
     assert parts[128, 128] == 150_000
-    assert _rel(parts, a) < 2e-6
+    assert _sf(parts, a) < SF_TOL
 
 
 def test_b16_single_operand_mode(ctx):
@@ -151,4 +159,4 @@ def test_b16_generic_kernel_agrees(ctx, monkeypatch):
     exact = ctx.gram_export()
     Xd.free(); yd.free()
     ctx.set_kernel(b2.KERNEL_AUTO)
-    assert _rel(S, exact) < 2e-6
+    assert _sf(S, exact) < SF_TOL
