@@ -79,54 +79,71 @@ int use_device(b2_ctx* ctx) {
   return B2_OK;
 }
 
-int check_shape(b2_ctx* ctx, int x_dtype, int64_t n, int d, int64_t ldx, int mem_kind) {
+int check_shape(int x_dtype, int64_t n, int d, int64_t ldx, int mem_kind) {
   if (x_dtype != B2_F32 && x_dtype != B2_BF16) { set_error("x_dtype must be B2_F32 or B2_BF16"); return B2_E_ARG; }
   if (d < 1 || d > kMaxD) { set_error("d=%d out of range [1,%d]", d, kMaxD); return B2_E_ARG; }
   if (n < 0) { set_error("n_rows < 0"); return B2_E_ARG; }
   if (ldx < d) { set_error("ldx=%lld < d=%d", (long long)ldx, d); return B2_E_ARG; }
   if (mem_kind != B2_MEM_DEVICE && mem_kind != B2_MEM_HOST) { set_error("bad mem_kind %d", mem_kind); return B2_E_ARG; }
-  (void)ctx;
   return B2_OK;
 }
 
 constexpr int64_t kMaxRowsPerLaunch = (int64_t)1 << 30;   // TMA coordinates / tile counters are int32
 
-// One device-resident block through the selected Gram kernel.
-int gram_block(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
-               const uint8_t* mask, int keep) {
-  if (n == 0) return B2_OK;
-  if (n > kMaxRowsPerLaunch) {   // more rows than one launch indexes: same kernel family, several launches
-    const int es = x_dtype == B2_F32 ? 4 : 2;
-    for (int64_t r0 = 0; r0 < n; r0 += kMaxRowsPerLaunch) {
-      const int64_t rows = n - r0 < kMaxRowsPerLaunch ? n - r0 : kMaxRowsPerLaunch;
-      if (int r = gram_block(ctx, static_cast<const char*>(X) + (size_t)r0 * ldx * es, x_dtype, y + r0, rows, d, ldx,
-                             mask != nullptr ? mask + r0 : nullptr, keep))
-        return r;
+// Device-resident rows into S: the one place that picks a Gram kernel.  Blocks of more than kMaxRowsPerLaunch rows
+// take several launches.  Per launch, the rows the main kernel's tiling leaves over (packing remainder, partial
+// narrow tile; all rows on the SIMT kernel) run first on the exact fp64 kernel, then the main kernel takes the first
+// main_rows rows; its shift sample covers all of them.  The first kernel to write S after b2_gram_reset overwrites it.
+// scatter_epoch != nullptr (b2_fit): with an attached peer exchange, a final tensor-core launch stores S into the
+// peers' exchange slots, and *scatter_epoch is that exchange's number (0: none).  *tc_last: the final launch was
+// tensor-core.
+int gram_dispatch(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
+                  const uint8_t* mask, int keep, bool* tc_last = nullptr, unsigned int* scatter_epoch = nullptr) {
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  for (int64_t r0 = 0; r0 < n; r0 += kMaxRowsPerLaunch) {
+    const int64_t rows = n - r0 < kMaxRowsPerLaunch ? n - r0 : kMaxRowsPerLaunch;
+    const char* Xb = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
+    const float* yb = y + r0;
+    const uint8_t* mb = mask != nullptr ? mask + r0 : nullptr;
+    const bool tc_ok = gram_tc_supported(Xb, x_dtype, yb, rows, d, ldx, mb);
+    const bool nw_ok = gram_narrow_supported(Xb, x_dtype, yb, rows, d, ldx, mb);
+    int mode = ctx->kernel_mode;
+    if (mode == B2_KERNEL_TCGEN05 && !tc_ok) {
+      set_error("tensor-core path needs d%%4==0 (fp32) / d%%8==0 (bf16), 16-byte aligned X/y/mask/row pitch, n>=32");
+      return B2_E_UNSUPPORTED;
     }
-    return B2_OK;
+    if (mode == B2_KERNEL_NARROW && !nw_ok) {
+      set_error("narrow path needs d<=16, contiguous rows (ldx==d) and 16-byte aligned X/y/mask");
+      return B2_E_UNSUPPORTED;
+    }
+    if (mode == B2_KERNEL_AUTO) {
+      // narrow rows stream through the CUDA-core pipeline (HBM-bound); wide rows go to the tensor core;
+      // tiny tranches (the reference's 1 440-row day) and odd layouts stay on the exact fp64 kernel
+      if (nw_ok && rows >= 4096) mode = B2_KERNEL_NARROW;
+      else mode = (tc_ok && rows >= 2048) ? B2_KERNEL_TCGEN05 : B2_KERNEL_SIMT;
+    }
+    const int64_t main_rows = mode == B2_KERNEL_NARROW ? gram_narrow_main_rows(rows, d)
+                            : mode == B2_KERNEL_TCGEN05 ? gram_tc_main_rows(rows, d, ldx, nullptr) : 0;
+    if (main_rows < rows) {
+      if (int r = launch_gram_simt(ctx, Xb + (size_t)main_rows * ldx * es, x_dtype, yb + main_rows, rows - main_rows, d,
+                                   ldx, mb != nullptr ? mb + main_rows : nullptr, keep, ctx->s_zero_pending))
+        return r;
+      ctx->s_zero_pending = false;
+    }
+    const bool last = r0 + rows == n;
+    if (main_rows > 0 && mode == B2_KERNEL_NARROW) {
+      if (int r = launch_gram_narrow(ctx, Xb, x_dtype, yb, rows, d, mb, keep, ctx->s_zero_pending)) return r;
+      ctx->s_zero_pending = false;
+    } else if (main_rows > 0) {
+      const unsigned int epoch =
+          last && scatter_epoch != nullptr && ctx->n_ranks > 1 && ctx->p2p_ready ? ++ctx->xchg_epoch : 0u;
+      if (int r = launch_gram_tc(ctx, Xb, x_dtype, yb, rows, d, ldx, mb, keep, ctx->s_zero_pending, epoch)) return r;
+      ctx->s_zero_pending = false;
+      if (scatter_epoch != nullptr) *scatter_epoch = epoch;
+    }
+    if (last && tc_last != nullptr) *tc_last = mode == B2_KERNEL_TCGEN05;
   }
-  if (int r = ensure_s_cleared(ctx)) return r;
-  const bool tc_ok = gram_tc_supported(X, x_dtype, y, n, d, ldx) &&
-                     (mask == nullptr || (reinterpret_cast<uintptr_t>(mask) & 15) == 0);
-  const bool nw_ok = gram_narrow_supported(X, x_dtype, y, n, d, ldx, mask);
-  int mode = ctx->kernel_mode;
-  if (mode == B2_KERNEL_TCGEN05 && !tc_ok) {
-    set_error("tensor-core path needs d%%4==0 (fp32) / d%%8==0 (bf16), 16-byte aligned X/y/mask/row pitch, n>=32");
-    return B2_E_UNSUPPORTED;
-  }
-  if (mode == B2_KERNEL_NARROW && !nw_ok) {
-    set_error("narrow path needs d<=16, contiguous rows (ldx==d) and 16-byte aligned X/y/mask");
-    return B2_E_UNSUPPORTED;
-  }
-  if (mode == B2_KERNEL_AUTO) {
-    // narrow rows stream through the CUDA-core pipeline (HBM-bound); wide rows go to the tensor core;
-    // tiny tranches (the reference's 1 440-row day) and odd layouts stay on the exact fp64 kernel
-    if (nw_ok && n >= 4096) mode = B2_KERNEL_NARROW;
-    else mode = (tc_ok && n >= 2048) ? B2_KERNEL_TCGEN05 : B2_KERNEL_SIMT;
-  }
-  if (mode == B2_KERNEL_NARROW) return launch_gram_narrow(ctx, X, x_dtype, y, n, d, ldx, mask, keep);
-  if (mode == B2_KERNEL_TCGEN05) return launch_gram_tc(ctx, X, x_dtype, y, n, d, ldx, mask, keep);
-  return launch_gram_simt(ctx, X, x_dtype, y, n, d, ldx, mask, keep);
+  return B2_OK;
 }
 
 int ensure_staging(b2_ctx* ctx) {
@@ -236,8 +253,50 @@ int stage_rows_h2d(b2_ctx* ctx, int buf, const void* X, int es, const float* y, 
   return B2_OK;
 }
 
-}  // namespace
+// Host rows through the two-deep HBM staging ring, in blocks of blk_rows: stage(buf, r0, rows) enqueues the copies of
+// one block into staging buffer buf on copy_stream, consume(buf, r0, rows) the work that reads it on stream; copies
+// overlap the work on the other buffer.  The caller may reuse its host buffers on return -- also when a block failed.
+template <typename Stage, typename Consume>
+int stream_host_blocks(b2_ctx* ctx, int64_t n_rows, int64_t blk_rows, Stage stage, Consume consume) {
+  auto block = [&](int buf, int64_t r0, int64_t rows) -> int {
+    // work of this call -- or of an EARLIER call that returned without a stream sync -- may still read this buffer
+    if (ctx->ev_consumed_valid[buf]) B2_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_consumed[buf], 0));
+    if (int r = stage(buf, r0, rows)) return r;
+    B2_CUDA(cudaEventRecord(ctx->ev_copied[buf], ctx->copy_stream));
+    B2_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copied[buf], 0));
+    if (int r = consume(buf, r0, rows)) return r;
+    B2_CUDA(cudaEventRecord(ctx->ev_consumed[buf], ctx->stream));
+    ctx->ev_consumed_valid[buf] = true;
+    return B2_OK;
+  };
+  int rc = B2_OK;
+  int64_t blk = 0;
+  for (int64_t r0 = 0; r0 < n_rows && rc == B2_OK; r0 += blk_rows, ++blk)
+    rc = block((int)(blk & 1), r0, n_rows - r0 < blk_rows ? n_rows - r0 : blk_rows);
+  const cudaError_t drained = cudaStreamSynchronize(ctx->copy_stream);
+  if (rc != B2_OK) return rc;
+  B2_CUDA(drained);
+  return B2_OK;
+}
 
+// host rows of b2_gram_accumulate / b2_fit, one staged block at a time through the Gram dispatch
+int gram_host_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                   const uint8_t* mask, int keep) {
+  if (int r = ensure_staging(ctx)) return r;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = host_pointer_is_pinned(X);
+  return stream_host_blocks(
+      ctx, n_rows, ctx->stage_rows,
+      [&](int buf, int64_t r0, int64_t rows) {
+        return stage_rows_h2d(ctx, buf, X, es, y, mask, r0, rows, d, ldx, x_pinned);
+      },
+      [&](int buf, int64_t, int64_t rows) {
+        return gram_dispatch(ctx, ctx->stage_x[buf], x_dtype, ctx->stage_y[buf], rows, d, d,
+                             mask != nullptr ? ctx->stage_m[buf] : nullptr, keep);
+      });
+}
+
+// honours a lazy b2_gram_reset where S is read before any kernel wrote it (exchange, export, solves after zero rows)
 int ensure_s_cleared(b2_ctx* ctx) {
   if (ctx->s_zero_pending) {
     B2_CUDA(cudaMemsetAsync(ctx->S, 0, sizeof(double) * kMaxS * kMaxS, ctx->stream));
@@ -245,6 +304,8 @@ int ensure_s_cleared(b2_ctx* ctx) {
   }
   return B2_OK;
 }
+
+}  // namespace
 
 }  // namespace b2
 
@@ -527,48 +588,19 @@ int b2_gram_reset(b2_ctx* ctx, int d) {
   if (int r = use_device(ctx)) return r;
   if (d < 1 || d > kMaxD) { set_error("d=%d out of range [1,%d]", d, kMaxD); return B2_E_ARG; }
   ctx->d = d;
-  ctx->s_zero_pending = true;   // cleared (or overwritten) by the first kernel that adds to S: one launch less per fit
+  ctx->s_zero_pending = true;   // the first kernel that writes S overwrites it: no memset launch
   return B2_OK;
 }
 
 int b2_gram_accumulate(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                        int mem_kind, const uint8_t* row_mask, int mask_keep) {
   if (int r = use_device(ctx)) return r;
-  if (int r = check_shape(ctx, x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
   if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
   if (d != ctx->d) { set_error("d=%d differs from the statistic's d=%d", d, ctx->d); return B2_E_ARG; }
   if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
-  ctx->k_launches = 0;
-  if (mem_kind == B2_MEM_DEVICE) return gram_block(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep);
-
-  // host rows: stream blocks through a 2-deep HBM staging ring, copies overlapping the kernels
-  if (int r = ensure_staging(ctx)) return r;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = host_pointer_is_pinned(X);
-  int64_t blk = 0;
-  int rc = B2_OK;
-  auto step = [&](int64_t r0, int buf, int64_t rows) -> int {
-    // a kernel of this call -- or of an EARLIER call that returned without a stream sync -- may still read this block
-    if (ctx->ev_consumed_valid[buf]) B2_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_consumed[buf], 0));
-    if (int r = stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned)) return r;
-    B2_CUDA(cudaEventRecord(ctx->ev_copied[buf], ctx->copy_stream));
-    B2_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copied[buf], 0));
-    if (int r = gram_block(ctx, ctx->stage_x[buf], x_dtype, ctx->stage_y[buf], rows, d, d,
-                           row_mask ? ctx->stage_m[buf] : nullptr, mask_keep))
-      return r;
-    B2_CUDA(cudaEventRecord(ctx->ev_consumed[buf], ctx->stream));
-    ctx->ev_consumed_valid[buf] = true;
-    return B2_OK;
-  };
-  for (int64_t r0 = 0; r0 < n_rows && rc == B2_OK; r0 += ctx->stage_rows, ++blk) {
-    const int64_t rows = (n_rows - r0 < ctx->stage_rows) ? n_rows - r0 : ctx->stage_rows;
-    rc = step(r0, (int)(blk & 1), rows);
-  }
-  // the caller may reuse its host buffers on return -- also when a block failed
-  const cudaError_t drained = cudaStreamSynchronize(ctx->copy_stream);
-  if (rc != B2_OK) return rc;
-  B2_CUDA(drained);
-  return B2_OK;
+  if (mem_kind == B2_MEM_DEVICE) return gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep);
+  return gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep);
 }
 
 // The peer-memory exchange reports a peer that did not deliver within the timeout through a status word in the
@@ -713,54 +745,30 @@ int b2_solve_eigvals(b2_ctx* ctx, double cond, int fit_intercept, double* singul
 }
 
 // ---- the whole fit in one call ----------------------------------------------------------------------------
-// reset + accumulate + all-reduce + solve.  Device-resident rows that take the tensor-core kernel run as four launches
-// with no memset, no separate scatter / gather kernels and no D2H copy node: shift sample, Gram kernel, finalize kernel
-// (reduces and folds the per-CTA partials, overwrites S, stores it straight into the peers' exchange slots) and the
-// solve kernel (waits for the peers' slots, sums them, factors, writes the coefficients into pinned host memory).
-// Everything else is the plain sequence of the four calls.
+// reset + accumulate + all-reduce + solve.  With an attached peer exchange and device rows whose final Gram launch is
+// tensor-core, the exchange rides on the kernels: the finalize kernel stores S straight into the peers' exchange slots,
+// and the solve kernel waits for them and sums them before it factors.  Otherwise the stand-alone exchange of
+// b2_gram_allreduce runs before the solve.  The solve kernel writes the coefficients into pinned host memory.
 int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
            const uint8_t* row_mask, int mask_keep, double alpha, int fit_intercept, double* coef, double* intercept) {
   if (int r = use_device(ctx)) return r;
-  if (int r = check_shape(ctx, x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
   if (!(alpha >= 0.0)) { set_error("alpha must be >= 0"); return B2_E_ARG; }
   if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
-  static const bool no_fused = getenv("B2_NO_FUSED") != nullptr;      // diagnostic switch: the four-call sequence
-  bool fused = !no_fused && mem_kind == B2_MEM_DEVICE && n_rows <= kMaxRowsPerLaunch &&
-               gram_tc_supported(X, x_dtype, y, n_rows, d, ldx) &&
-               (row_mask == nullptr || (reinterpret_cast<uintptr_t>(row_mask) & 15) == 0);
-  if (fused) {
-    const bool nw_ok = gram_narrow_supported(X, x_dtype, y, n_rows, d, ldx, row_mask);
-    if (ctx->kernel_mode == B2_KERNEL_AUTO) fused = !(nw_ok && n_rows >= 4096) && n_rows >= 2048;
-    else fused = ctx->kernel_mode == B2_KERNEL_TCGEN05;
-  }
-  if (!fused) {
-    if (int r = b2_gram_reset(ctx, d)) return r;
-    if (int r = b2_gram_accumulate(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
-    if (int r = b2_gram_allreduce(ctx)) return r;
-    return b2_solve(ctx, alpha, fit_intercept, coef, intercept);
-  }
-  ctx->d = d;
-  ctx->k_launches = 0;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const int64_t n_main = gram_tc_main_rows(n_rows, d, ldx, nullptr);
-  TcFuse fuse;
-  fuse.assign = 1; fuse.scatter = 0; fuse.epoch = 0;
-  if (n_main < n_rows) {   // the few rows the packed layout leaves over go in first; the fused fold then adds to S
-    ctx->s_zero_pending = true;
-    if (int r = ensure_s_cleared(ctx)) return r;
-    if (int r = launch_gram_simt(ctx, static_cast<const char*>(X) + (size_t)n_main * ldx * es, x_dtype, y + n_main,
-                                 n_rows - n_main, d, ldx, row_mask != nullptr ? row_mask + n_main : nullptr, mask_keep))
+  if (int r = b2_gram_reset(ctx, d)) return r;
+  unsigned int gather_epoch = 0;
+  if (mem_kind == B2_MEM_DEVICE) {
+    bool tc_last = false;
+    if (int r = gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep, &tc_last, &gather_epoch))
       return r;
-    fuse.assign = 0;
+    if (tc_last) ctx->fused_fits += 1;
+  } else if (int r = gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) {
+    return r;
   }
-  const bool p2p = ctx->n_ranks > 1 && ctx->p2p_ready;
-  if (p2p) { fuse.scatter = 1; fuse.epoch = ++ctx->xchg_epoch; }
-  if (int r = launch_gram_tc(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep, &fuse)) return r;
-  ctx->fused_fits += 1;
-  if (!p2p && ctx->comm != nullptr) {
+  if (gather_epoch == 0) {
     if (int r = b2_gram_allreduce(ctx)) return r;
   }
-  if (int r = launch_solve_cholesky(ctx, alpha, fit_intercept, p2p ? fuse.epoch : 0u)) return r;
+  if (int r = launch_solve_cholesky(ctx, alpha, fit_intercept, gather_epoch)) return r;
   return finish_cholesky(ctx, coef, intercept);
 }
 
@@ -769,7 +777,7 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
              const double* coef, double intercept, const float* y, const uint8_t* row_mask, int mask_keep,
              float* yhat, double* stats_out) {
   if (int r = use_device(ctx)) return r;
-  if (int r = check_shape(ctx, x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
   if (coef == nullptr || (n_rows > 0 && X == nullptr)) { set_error("coef / X is null"); return B2_E_ARG; }
   // coefficients go up through one of two pinned slots (no stream sync per call: the slot is only waited for when it
   // is reused, two calls later)
@@ -807,28 +815,22 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
         yhat_dev[b] = ctx->yhat_stage[b];
       }
     }
-    int64_t blk = 0;
-    int rc = B2_OK;
-    for (int64_t r0 = 0; r0 < n_rows && rc == B2_OK; r0 += ctx->stage_rows, ++blk) {
-      const int buf = (int)(blk & 1);
-      const int64_t rows = (n_rows - r0 < ctx->stage_rows) ? n_rows - r0 : ctx->stage_rows;
-      if (ctx->ev_consumed_valid[buf]) cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_consumed[buf], 0);
-      rc = stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-      if (rc != B2_OK) break;
-      cudaEventRecord(ctx->ev_copied[buf], ctx->copy_stream);
-      cudaStreamWaitEvent(ctx->stream, ctx->ev_copied[buf], 0);
-      rc = launch_score(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, y ? ctx->stage_y[buf] : nullptr,
-                        row_mask ? ctx->stage_m[buf] : nullptr, mask_keep, yhat ? yhat_dev[buf] : nullptr, blk == 0);
-      if (rc != B2_OK) break;
-      if (yhat != nullptr)
-        cudaMemcpyAsync(yhat + r0, yhat_dev[buf], (size_t)rows * 4, cudaMemcpyDeviceToHost, ctx->stream);
-      cudaEventRecord(ctx->ev_consumed[buf], ctx->stream);
-      ctx->ev_consumed_valid[buf] = true;
-    }
-    cudaStreamSynchronize(ctx->copy_stream);
-    cudaStreamSynchronize(ctx->stream);
+    const int rc = stream_host_blocks(
+        ctx, n_rows, ctx->stage_rows,
+        [&](int buf, int64_t r0, int64_t rows) {
+          return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
+        },
+        [&](int buf, int64_t r0, int64_t rows) -> int {
+          if (int r = launch_score(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, y ? ctx->stage_y[buf] : nullptr,
+                                   row_mask ? ctx->stage_m[buf] : nullptr, mask_keep, yhat_dev[buf], r0 == 0))
+            return r;
+          if (yhat != nullptr)
+            B2_CUDA(cudaMemcpyAsync(yhat + r0, yhat_dev[buf], (size_t)rows * 4, cudaMemcpyDeviceToHost, ctx->stream));
+          return B2_OK;
+        });
+    const cudaError_t done = cudaStreamSynchronize(ctx->stream);   // the predictions' copies into the caller's yhat
     if (rc != B2_OK) return rc;
-    B2_CUDA(cudaGetLastError());
+    B2_CUDA(done);
   }
   if (stats_out != nullptr && y != nullptr) {
     B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * 10, cudaMemcpyDeviceToHost, ctx->stream));
@@ -870,7 +872,7 @@ int b2_score_allreduce(b2_ctx* ctx, double* stats) {
 int b2_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n_rows, int d, int64_t ldx, int x_dtype,
              double alpha, double beta, double sigma, void* X_dev, float* y_dev) {
   if (int r = use_device(ctx)) return r;
-  if (int r = check_shape(ctx, x_dtype, n_rows, d, ldx, B2_MEM_DEVICE)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, B2_MEM_DEVICE)) return r;
   if (n_rows > 0 && (X_dev == nullptr || y_dev == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
   return launch_synth(ctx, seed, row_offset, n_rows, d, ldx, x_dtype, alpha, beta, sigma, X_dev, y_dev);
 }
@@ -917,30 +919,30 @@ int b2_metrics(b2_ctx* ctx, const void* y_actual, const void* y_predicted, int d
     // is too small for fp64, so both vectors share the X block: [rows] actual then [rows] predicted)
     if (int r = ensure_staging(ctx)) return r;
     const int64_t blk_rows = (int64_t)(ctx->stage_bytes_x / (2 * es));
-    int64_t blk = 0;
-    for (int64_t r0 = 0; r0 < n_rows; r0 += blk_rows, ++blk) {
-      const int buf = (int)(blk & 1);
-      const int64_t rows = n_rows - r0 < blk_rows ? n_rows - r0 : blk_rows;
-      if (ctx->ev_consumed_valid[buf]) B2_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_consumed[buf], 0));
-      char* dst = static_cast<char*>(ctx->stage_x[buf]);
-      B2_CUDA(cudaMemcpyAsync(dst, static_cast<const char*>(y_actual) + (size_t)r0 * es, (size_t)rows * es,
-                              cudaMemcpyHostToDevice, ctx->copy_stream));
-      B2_CUDA(cudaMemcpyAsync(dst + (size_t)blk_rows * es, static_cast<const char*>(y_predicted) + (size_t)r0 * es,
-                              (size_t)rows * es, cudaMemcpyHostToDevice, ctx->copy_stream));
-      B2_CUDA(cudaEventRecord(ctx->ev_copied[buf], ctx->copy_stream));
-      B2_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_copied[buf], 0));
-      if (int r = launch_metrics(ctx, dst, dst + (size_t)blk_rows * es, dtype, rows, blk == 0)) return r;
-      B2_CUDA(cudaEventRecord(ctx->ev_consumed[buf], ctx->stream));
-      ctx->ev_consumed_valid[buf] = true;
-    }
-    B2_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+    if (int r = stream_host_blocks(
+            ctx, n_rows, blk_rows,
+            [&](int buf, int64_t r0, int64_t rows) -> int {
+              char* dst = static_cast<char*>(ctx->stage_x[buf]);
+              const size_t off = (size_t)r0 * es, bytes = (size_t)rows * es;
+              B2_CUDA(cudaMemcpyAsync(dst, static_cast<const char*>(y_actual) + off, bytes, cudaMemcpyHostToDevice,
+                                      ctx->copy_stream));
+              B2_CUDA(cudaMemcpyAsync(dst + (size_t)blk_rows * es, static_cast<const char*>(y_predicted) + off, bytes,
+                                      cudaMemcpyHostToDevice, ctx->copy_stream));
+              return B2_OK;
+            },
+            [&](int buf, int64_t r0, int64_t rows) {
+              const char* src = static_cast<const char*>(ctx->stage_x[buf]);
+              return launch_metrics(ctx, src, src + (size_t)blk_rows * es, dtype, rows, r0 == 0);
+            }))
+      return r;
   }
   B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * 10, cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
 }
 
-// counters of the context: [0] fits that took the fused path of b2_fit, [1] exchanges started, [2] kernels launched
+// counters of the context: [0] b2_fit calls whose device rows ended on the tensor-core kernel, [1] exchanges started,
+// [2] kernels launched
 int b2_ctx_stats(b2_ctx* ctx, int64_t* out3) {
   if (ctx == nullptr || out3 == nullptr) { set_error("null argument"); return B2_E_ARG; }
   out3[0] = ctx->fused_fits;

@@ -49,7 +49,6 @@ struct b2_ctx {
   cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
   cudaEvent_t ev_k[b2::kKernelEventPairs][2];
   int k_pairs = 0;                     // pairs recorded since the last b2_last_kernel_ms
-  int k_launches = 0;                  // kernels launched by the most recent accumulate
   int64_t launches = 0;                // kernels launched since ctx creation
 
   int kernel_mode = B2_KERNEL_AUTO;
@@ -86,7 +85,6 @@ struct b2_ctx {
   long long* synth_count = nullptr;    // device counter of b2_synth_tranche (rows kept by the y >= 0 filter)
   // solve scratch
   double* solve_out = nullptr;         // [kMaxD + 2 + kMaxD]: coef, intercept, info, singular
-  double* solve_work = nullptr;        // [2 * kMaxD * kMaxD] eigenvectors etc.
   // host staging ring (B2_MEM_HOST)
   void* stage_x[2] = {nullptr, nullptr};
   float* stage_y[2] = {nullptr, nullptr};
@@ -99,7 +97,7 @@ struct b2_ctx {
   float* yhat_stage[2] = {nullptr, nullptr};    // prediction staging blocks of the host-streamed b2_score
   void* bounce[2] = {nullptr, nullptr};         // pinned bounce blocks for pageable host rows (filled by host threads)
   cudaEvent_t ev_bounce[2] = {nullptr, nullptr};
-  bool s_zero_pending = false;         // b2_gram_reset is lazy: S is cleared (or overwritten) by the first kernel that adds to it
+  bool s_zero_pending = false;         // b2_gram_reset is lazy: the first kernel to write S overwrites it
   // NCCL
   void* comm = nullptr;
   int n_ranks = 1, rank = 0;
@@ -112,9 +110,9 @@ struct b2_ctx {
   unsigned long long xchg_timeout_ns = 10000000000ull;   // bound of the wait for a peer's flag (b2_comm_set_timeout_ms)
   bool xchg_pending = false;           // an exchange was launched since the status word was last read
   unsigned int* xchg_status_host = nullptr;  // pinned mirror of the exchange status word
-  // fused fit (b2_fit): in-kernel grid barrier / ticket words of the Gram kernel's reduce + fold tail
+  // grid barrier / ticket words of the tensor-core finalize kernel (reduce + fold + peer scatter)
   unsigned int* tc_sync = nullptr;     // [0], [1] barrier arrivals, [2] ticket
-  int fused_fits = 0;                  // fits that took the fused path (b2_ctx_stats)
+  int fused_fits = 0;                  // b2_fit calls whose device rows ended on the tensor-core kernel (b2_ctx_stats)
   int sm_limit = 0;                    // > 0: persistent kernels use at most this many SMs (b2_ctx_set_sm_limit)
   bool sm_limit_auto = false;          // the limit was set by b2_comm_p2p_attach_local (contexts sharing a device)
 };
@@ -122,23 +120,22 @@ struct b2_ctx {
 namespace b2 {
 
 // ---- kernel launchers (each enqueues on ctx->stream and bumps ctx->launches) -----------------
+// The three Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites
+// it instead of adding to it (the first writer after b2_gram_reset).  The tensor-core and narrow launchers cover the
+// first gram_*_main_rows(n) rows; their per-column shift is sampled from all n rows.
 int launch_gram_simt(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
-                     int64_t ldx, const uint8_t* mask, int keep);
-bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx);
+                     int64_t ldx, const uint8_t* mask, int keep, bool assign);
+bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
+                       const uint8_t* mask);
 int64_t gram_tc_main_rows(int64_t n, int d, int64_t ldx, int* pack_out);
-// fuse != nullptr: the Gram kernel computes its own shift, reduces the per-CTA partials and folds them into S in the
-// same launch (grid barriers), and -- with an attached peer exchange -- stores S into every peer's slot (b2_fit)
-struct TcFuse {
-  int assign;                 // S = value instead of S += value (fresh statistic, no memset needed)
-  int scatter;                // 1: store the folded S into the exchange slots of all ranks and publish the flags
-  unsigned int epoch;         // exchange number when scatter == 1
-};
+// scatter_epoch != 0: the finalize also stores S into every peer's exchange slot as exchange `scatter_epoch`
 int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
-                   int64_t ldx, const uint8_t* mask, int keep, const TcFuse* fuse = nullptr);
+                   int64_t ldx, const uint8_t* mask, int keep, bool assign, unsigned int scatter_epoch);
 bool gram_narrow_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
                            const uint8_t* mask);
+int64_t gram_narrow_main_rows(int64_t n, int d);
 int launch_gram_narrow(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
-                       int64_t ldx, const uint8_t* mask, int keep);
+                       const uint8_t* mask, int keep, bool assign);
 // gather_epoch != 0: the solve kernel first waits for the peer exchange `gather_epoch` and sums the slots into S
 int launch_solve_cholesky(b2_ctx* ctx, double alpha, int fit_intercept, unsigned int gather_epoch = 0);
 int launch_solve_eigvals(b2_ctx* ctx, double cond, int fit_intercept);
@@ -151,6 +148,5 @@ int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int 
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);
 int launch_synth_tranche(b2_ctx* ctx, uint64_t seed, int64_t n, double alpha, double beta, double sigma, float* X, float* y,
                          int64_t* n_kept_dev);
-int ensure_s_cleared(b2_ctx* ctx);   // honours a lazy b2_gram_reset before a kernel that does S += ...
 
 }  // namespace b2

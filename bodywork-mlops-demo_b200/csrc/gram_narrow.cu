@@ -398,11 +398,11 @@ gram_narrow_kernel(const T* __restrict__ X, const float* __restrict__ y, const u
   }
 }
 
-// ---- finalize: sum the CTA partials in order, undo the shift in fp64, S += ------------------------------------
+// ---- finalize: sum the CTA partials in order, undo the shift in fp64, S += (S = when assign) ---------------------
 // m(i, j), i <= j over internal indices (features 0..DP-1, DP = ones, DP + 1 = y'), row stride DP + 2.
 __global__ void __launch_bounds__(384)
 narrow_fold_kernel(const double* __restrict__ part, int n_ctas, int DP, int d, const float* __restrict__ cvec,
-                   double* __restrict__ S) {
+                   int assign, double* __restrict__ S) {
   __shared__ double m[kNwMM];
   const int MS = DP + 2;
   for (int k = threadIdx.x; k < MS * MS; k += blockDim.x) {
@@ -435,7 +435,7 @@ narrow_fold_kernel(const double* __restrict__ part, int n_ctas, int DP, int d, c
     } else {
       val = sy + n * cy;
     }
-    S[idx] += val;
+    S[idx] = assign ? val : S[idx] + val;
   }
 }
 
@@ -467,15 +467,19 @@ int launch_narrow_dp(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mas
   return B2_OK;
 }
 
+int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
+
+int narrow_tile_rows(int DP) {
+  return DP == 1 ? NwGeom<1>::kRows : DP == 2 ? NwGeom<2>::kRows : DP == 4 ? NwGeom<4>::kRows
+       : DP == 8 ? NwGeom<8>::kRows : NwGeom<16>::kRows;
+}
+
+// the full tiles of the first gram_narrow_main_rows(n, d) rows; the shift sample covers all n rows
 template <typename T>
 int launch_narrow_t(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask, int keep, int64_t n, int d,
-                    int64_t* rows_done) {
-  const int DP = d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16;
-  const int rows = DP == 1 ? NwGeom<1>::kRows : DP == 2 ? NwGeom<2>::kRows : DP == 4 ? NwGeom<4>::kRows
-                 : DP == 8 ? NwGeom<8>::kRows : NwGeom<16>::kRows;
-  const int n_tiles = (int)(n / rows);            // n <= INT32_MAX rows (gram_narrow_supported)
-  *rows_done = (int64_t)n_tiles * rows;
-  if (n_tiles == 0) return B2_OK;
+                    bool assign) {
+  const int DP = narrow_dp(d);
+  const int n_tiles = (int)(n / narrow_tile_rows(DP));   // n <= INT32_MAX rows (gram_narrow_supported)
   narrow_shift_kernel<T><<<1, 32 * (kNwMaxDP + 1), 0, ctx->stream>>>(X, y, n, d, ctx->shift);
   B2_CUDA(cudaGetLastError());
   const int pair = ctx->k_pairs % kKernelEventPairs;
@@ -491,16 +495,15 @@ int launch_narrow_t(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask
   if (rc != B2_OK) return rc;
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][1], ctx->stream));
   ctx->k_pairs += 1;
-  narrow_fold_kernel<<<1, 384, 0, ctx->stream>>>(ctx->simt_part, grid, DP, d, ctx->shift, ctx->S);
+  narrow_fold_kernel<<<1, 384, 0, ctx->stream>>>(ctx->simt_part, grid, DP, d, ctx->shift, assign ? 1 : 0, ctx->S);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 3;
-  ctx->k_launches += 3;
   return B2_OK;
 }
 
 }  // namespace
 
-// rows contiguous (ldx == d), X / y / mask 16-byte aligned; full tiles here, the < kRows leftover rows on the fp64 kernel
+// rows contiguous (ldx == d), X / y / mask 16-byte aligned
 bool gram_narrow_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
                            const uint8_t* mask) {
   (void)x_dtype;
@@ -510,22 +513,15 @@ bool gram_narrow_supported(const void* X, int x_dtype, const float* y, int64_t n
   return true;
 }
 
-int launch_gram_narrow(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
-                       const uint8_t* mask, int keep) {
+// Full kRows tiles only: the < kRows rows left over take the fp64 kernel
+int64_t gram_narrow_main_rows(int64_t n, int d) { return n - n % narrow_tile_rows(narrow_dp(d)); }
+
+int launch_gram_narrow(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
+                       const uint8_t* mask, int keep, bool assign) {
   static_assert(2 * kNwMM <= kMaxS * kMaxS, "two CTAs per SM of partials fit the CUDA-core scratch (simt_part)");
-  int64_t done = 0;
-  int rc;
   if (x_dtype == B2_F32)
-    rc = launch_narrow_t<float>(ctx, static_cast<const float*>(X), y, mask, keep, n, d, &done);
-  else
-    rc = launch_narrow_t<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), y, mask, keep, n, d, &done);
-  if (rc != B2_OK) return rc;
-  if (done < n) {
-    const int es = x_dtype == B2_F32 ? 4 : 2;
-    const char* Xt = static_cast<const char*>(X) + (size_t)done * ldx * es;
-    return launch_gram_simt(ctx, Xt, x_dtype, y + done, n - done, d, ldx, mask != nullptr ? mask + done : nullptr, keep);
-  }
-  return B2_OK;
+    return launch_narrow_t<float>(ctx, static_cast<const float*>(X), y, mask, keep, n, d, assign);
+  return launch_narrow_t<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), y, mask, keep, n, d, assign);
 }
 
 }  // namespace b2

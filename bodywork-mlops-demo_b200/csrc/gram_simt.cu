@@ -93,19 +93,20 @@ gram_simt_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n
   }
 }
 
-// S[a][b] += sum over CTAs (fixed order -> deterministic)
-__global__ void gram_simt_reduce(const double* __restrict__ part, int n_ctas, int dp, double* __restrict__ S) {
+// S[a][b] (+)= sum over CTAs (fixed order -> deterministic); assign: S = sum (a fresh statistic)
+__global__ void gram_simt_reduce(const double* __restrict__ part, int n_ctas, int dp, int assign,
+                                 double* __restrict__ S) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= dp * dp) return;
   double s = 0.0;
   for (int c = 0; c < n_ctas; ++c) s += part[(size_t)c * kMaxS * kMaxS + idx];
-  S[idx] += s;
+  S[idx] = assign ? s : S[idx] + s;
 }
 
 }  // namespace
 
 int launch_gram_simt(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
-                     int64_t ldx, const uint8_t* mask, int keep) {
+                     int64_t ldx, const uint8_t* mask, int keep, bool assign) {
   if (n <= 0) return B2_OK;
   const int dp = d + 2;
   const int nb = (dp + 7) / 8;
@@ -122,10 +123,9 @@ int launch_gram_simt(b2_ctx* ctx, const void* X, int x_dtype, const float* y, in
         static_cast<const __nv_bfloat16*>(X), y, n, d, ldx, mask, keep, ctx->simt_part);
   }
   B2_CUDA(cudaGetLastError());
-  gram_simt_reduce<<<(dp * dp + 255) / 256, 256, 0, ctx->stream>>>(ctx->simt_part, grid, dp, ctx->S);
+  gram_simt_reduce<<<(dp * dp + 255) / 256, 256, 0, ctx->stream>>>(ctx->simt_part, grid, dp, assign ? 1 : 0, ctx->S);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 2;
-  ctx->k_launches += 2;
   return B2_OK;
 }
 

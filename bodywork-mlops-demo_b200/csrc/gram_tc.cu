@@ -845,7 +845,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
 
 // What tc_finalize_kernel does after the reduce + fold (passed by value).
 struct TcFinal {
-  int assign;                 // S = value instead of S += value (fresh statistic: no memset launch)
+  int assign;                 // S = value instead of S += value (first writer of a fresh statistic)
   int n_ranks, rank;          // n_ranks > 1: store S into the exchange slot of every rank and publish the flags
   unsigned int epoch;
   PeerPtrs peers;
@@ -925,12 +925,14 @@ PFN_encodeTiled get_encode() {
 
 }  // namespace
 
-bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx) {
+bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,
+                       const uint8_t* mask) {
   const int es = x_dtype == B2_F32 ? 4 : 2;
   if (d < 4 || d > kMaxD) return false;
   if ((d * es) % 16 != 0) return false;
   if ((ldx * es) % 16 != 0) return false;
   if ((reinterpret_cast<uintptr_t>(X) & 15) != 0 || (reinterpret_cast<uintptr_t>(y) & 15) != 0) return false;
+  if (mask != nullptr && (reinterpret_cast<uintptr_t>(mask) & 15) != 0) return false;
   if (n < kTcRows) return false;
   if (n > (int64_t)0x7fffffff) return false;  // TMA coordinates are int32
   return true;
@@ -986,10 +988,6 @@ static int encode_maps(PFN_encodeTiled encode, const void* X, int x_dtype, int e
       }
     }
   }
-  if (mask != nullptr && (reinterpret_cast<uintptr_t>(mask) & 15) != 0) {
-    set_error("row_mask must be 16-byte aligned for the tensor-core path");
-    return B2_E_ARG;
-  }
   int m_map_2d = 0;
   if (mask != nullptr) {
     cuuint64_t dims[1] = {(cuuint64_t)n_y};
@@ -1037,7 +1035,7 @@ int64_t gram_tc_main_rows(int64_t n_in, int d_in, int64_t ldx_in, int* pack_out)
 }
 
 int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_in, int d_in, int64_t ldx_in,
-                   const uint8_t* mask, int keep, const TcFuse* fuse) {
+                   const uint8_t* mask, int keep, bool assign, unsigned int scatter_epoch) {
   PFN_encodeTiled encode = get_encode();
   if (encode == nullptr) {
     set_error("cuTensorMapEncodeTiled is not available from the driver");
@@ -1047,8 +1045,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   // Row packing: `pack` contiguous rows of 17..64 features are viewed as one super-row of pack * d_in <= 128 columns
   // ([n / pack][pack * d_in], zero-filled by TMA to the 128-wide tile) and run on the D = 128 fast path; the diagonal
   // d_in x d_in blocks of the 128 x 128 Gram sum to the true statistic (tc_fold_kernel).  The tensor maps cover a
-  // multiple of lcm(pack, 16) rows (the y / mask views are 16-byte rows); the < 80 leftover rows go through the
-  // CUDA-core kernel.
+  // multiple of lcm(pack, 16) rows (the y / mask views are 16-byte rows); the caller runs the < 80 leftover rows on
+  // the CUDA-core kernel.
   int pack = 1;
   const int64_t n_main = gram_tc_main_rows(n_in, d_in, ldx_in, &pack);   // original rows handled here
   const int64_t n = n_main / pack;                      // super-rows
@@ -1098,11 +1096,6 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     ctx->tc_attr_set = true;
   }
 
-  // S: a fresh statistic is overwritten by the finalize kernel (no memset launch); otherwise it must be cleared first
-  const bool assign = fuse != nullptr && fuse->assign != 0;
-  if (!assign) {
-    if (int r = ensure_s_cleared(ctx)) return r;
-  }
   if (x_dtype == B2_F32)
     tc_shift_kernel<float><<<kShiftBlocks, kShiftCols * kShiftGroups, 0, ctx->stream>>>(static_cast<const float*>(X), y, n_in, d_in,
                                                                   ldx_in, ctx->shift);
@@ -1156,8 +1149,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   memset(&fin, 0, sizeof(fin));
   fin.assign = assign ? 1 : 0;
   fin.n_ranks = 1;
-  if (fuse != nullptr && fuse->scatter) {
-    fin.n_ranks = ctx->n_ranks; fin.rank = ctx->rank; fin.epoch = fuse->epoch;
+  if (scatter_epoch != 0) {
+    fin.n_ranks = ctx->n_ranks; fin.rank = ctx->rank; fin.epoch = scatter_epoch;
     for (int r = 0; r < kMaxRanks; ++r) fin.peers.p[r] = ctx->xchg_peer[r];
   }
   {
@@ -1176,14 +1169,6 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
                                ctx->S, ctx->tc_sync, fin));
   }
   ctx->launches += 3;
-  ctx->k_launches += 3;
-  ctx->s_zero_pending = false;
-  const bool fused = fuse != nullptr;
-  if (n_main < n_in && !fused) {   // the n % pack leftover rows (the fused caller accumulates them first)
-    const char* Xt = static_cast<const char*>(X) + (size_t)n_main * ldx_in * es;
-    return launch_gram_simt(ctx, Xt, x_dtype, y + n_main, n_in - n_main, d_in, ldx_in,
-                            mask != nullptr ? mask + n_main : nullptr, keep);
-  }
   return B2_OK;
 }
 

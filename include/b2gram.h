@@ -135,10 +135,10 @@ int b2_split_mask(int64_t n_rows, int64_t n_test, uint32_t seed, uint8_t* mask_o
 
 /* ---- the whole fit in one call: LinearRegression(fit_intercept).fit(X, y) / Ridge(alpha) ----------------------
  * reference: stage_1_train_model.py:105-106.  Equivalent to b2_gram_reset + b2_gram_accumulate + b2_gram_allreduce +
- * b2_solve with the same arguments.  Device-resident rows that take the tensor-core kernel skip the memset, the separate
- * scatter / gather launches and the D2H copy: the finalize kernel behind the Gram kernel folds the partials and stores
- * S into the peers' exchange slots (when a peer exchange is attached), the solve kernel sums the peers' slots, factors
- * and writes coef / intercept to the host. */
+ * b2_solve with the same arguments, and runs the same Gram kernels; the solve kernel writes coef / intercept straight
+ * to pinned host memory.  With a peer exchange attached and device-resident rows whose last Gram launch is the
+ * tensor-core kernel, the exchange takes no launches of its own: the finalize kernel behind the Gram kernel stores S
+ * into the peers' exchange slots and the solve kernel sums them. */
 int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
            int mem_kind, const uint8_t* row_mask, int mask_keep, double alpha, int fit_intercept,
            double* coef, double* intercept);
@@ -225,7 +225,8 @@ int b2_timer_stop(b2_ctx* ctx, double* ms_out);
 int b2_last_kernel_ms(b2_ctx* ctx, double* gram_ms_out, int* launches_out);
 /* total number of kernels this ctx has launched since creation (bench.py's gpu_launches) */
 int b2_launch_count(b2_ctx* ctx, int64_t* n_out);
-/* out3[0] fits that took the fused path of b2_fit, [1] peer exchanges started, [2] kernels launched */
+/* out3[0] b2_fit calls whose device rows ended on the tensor-core kernel, [1] peer exchanges started, [2] kernels
+ * launched */
 int b2_ctx_stats(b2_ctx* ctx, int64_t* out3);
 
 #ifdef __cplusplus

@@ -80,20 +80,42 @@ def test_fused_fit_matches_oracle_and_takes_four_launches(ctx, n, d, kind, maske
 
 
 def test_fused_fit_is_bit_deterministic_and_agrees_with_the_four_call_sequence(ctx):
-    n, d = 150_000, 128
-    X, y = orc.generate_dataset(n, d, seed=5, dtype=np.float32)
-    Xd, yd = ctx.to_device(X), ctx.to_device(y)
-    ctx.set_kernel(b2.KERNEL_TCGEN05)
-    try:
-        c1, b1 = ctx.fit(Xd, yd); S1 = ctx.gram_export()
-        c2, b2_ = ctx.fit(Xd, yd); S2 = ctx.gram_export()
-        ctx.gram_reset(d); ctx.gram_accumulate(Xd, yd); c3, b3 = ctx.solve(); S3 = ctx.gram_export()
-    finally:
-        ctx.set_kernel(b2.KERNEL_AUTO)
-    assert np.array_equal(S1, S2) and np.array_equal(c1, c2) and b1 == b2_
-    # the same kernels in the same order: the one-call fit and the four-call sequence agree bit for bit
-    assert np.array_equal(S1, S3) and np.array_equal(c1, c3) and b1 == b3
-    Xd.free(); yd.free()
+    cases = [
+        (150_000, 128, "f32", b2.KERNEL_TCGEN05, False),    # no leftover rows
+        (50_001, 32, "f32", b2.KERNEL_TCGEN05, False),      # 4 rows per super-row: 1 leftover row on the fp64 kernel
+        (70_007, 24, "f32", b2.KERNEL_TCGEN05, False),      # 5 rows per super-row: 7 leftover rows
+        (70_007, 24, "f32", b2.KERNEL_TCGEN05, True),       # the same with a row mask
+        (30_011, 48, "bf16", b2.KERNEL_TCGEN05, False),     # bf16, 2 rows per super-row: 11 leftover rows
+        (120_003, 8, "f32", b2.KERNEL_AUTO, False),         # narrow rows: 163 rows past the last full tile
+        (20_000, 128, "f32", b2.KERNEL_SIMT, False)]
+    for case in cases:
+        n, d, kind, kernel, masked = case
+        X, y = orc.generate_dataset(n, d, seed=5, dtype=np.float32)
+        Xd = ctx.to_device(b2.native.to_bf16_bits(X), "bf16") if kind == "bf16" else ctx.to_device(X)
+        yd = ctx.to_device(y)
+        md = ctx.to_device((np.random.RandomState(d).rand(n) < 0.8).astype(np.uint8)) if masked else None
+        tensor_core = kernel == b2.KERNEL_TCGEN05
+        ctx.set_kernel(kernel)
+        try:
+            before = ctx.stats()["fused_fits"]
+            c1, b1 = ctx.fit(Xd, yd, md, 1); S1 = ctx.gram_export()
+            l0 = ctx.launch_count()
+            c2, b2_ = ctx.fit(Xd, yd, md, 1); S2 = ctx.gram_export()
+            l1 = ctx.launch_count()
+            ctx.gram_reset(d); ctx.gram_accumulate(Xd, yd, md, 1); c3, b3 = ctx.solve(); S3 = ctx.gram_export()
+            l2 = ctx.launch_count()
+            fused_fits = ctx.stats()["fused_fits"] - before
+        finally:
+            ctx.set_kernel(b2.KERNEL_AUTO)
+            for a in (Xd, yd, md):
+                if a is not None:
+                    a.free()
+        assert np.array_equal(S1, S2) and np.array_equal(c1, c2) and b1 == b2_, case
+        # the same kernels in the same order: the one-call fit and the four-call sequence agree bit for bit
+        assert np.array_equal(S1, S3) and np.array_equal(c1, c3) and b1 == b3, case
+        assert fused_fits == (2 if tensor_core else 0), case
+        if tensor_core:
+            assert l1 - l0 == l2 - l1, case
 
 
 @pytest.mark.parametrize("i", range(32))
