@@ -93,7 +93,8 @@ constexpr int64_t kMaxRowsPerLaunch = (int64_t)1 << 30;   // TMA coordinates / t
 // Device-resident rows into S: the one place that picks a Gram kernel.  Blocks of more than kMaxRowsPerLaunch rows
 // take several launches.  Per launch, the rows the main kernel's tiling leaves over (packing remainder, partial
 // narrow tile; all rows on the SIMT kernel) run first on the exact fp64 kernel, then the main kernel takes the first
-// main_rows rows; its shift sample covers all of them.  The first kernel to write S after b2_gram_reset overwrites it.
+// main_rows rows.  Before both, the shift sample of the tensor-core and narrow kernels covers all rows of the launch.
+// The first kernel to write S after b2_gram_reset overwrites it.
 // scatter_epoch != nullptr (b2_fit): with an attached peer exchange, a final tensor-core launch stores S into the
 // peers' exchange slots, and *scatter_epoch is that exchange's number (0: none).  *tc_last: the final launch was
 // tensor-core.
@@ -124,6 +125,8 @@ int gram_dispatch(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64
     }
     const int64_t main_rows = mode == B2_KERNEL_NARROW ? gram_narrow_main_rows(rows, d)
                             : mode == B2_KERNEL_TCGEN05 ? gram_tc_main_rows(rows, d, ldx, nullptr) : 0;
+    if (main_rows > 0)
+      if (int r = launch_gram_shift(ctx, Xb, x_dtype, yb, rows, d, ldx)) return r;
     if (main_rows < rows) {
       if (int r = launch_gram_simt(ctx, Xb + (size_t)main_rows * ldx * es, x_dtype, yb + main_rows, rows - main_rows, d,
                                    ldx, mb != nullptr ? mb + main_rows : nullptr, keep, ctx->s_zero_pending))
@@ -345,8 +348,8 @@ static int ctx_allocate(b2_ctx* ctx) {
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->S), sizeof(double) * kMaxS * kMaxS));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_part), sizeof(double) * (size_t)ctx->sm_count * kTcAccElems));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_side), sizeof(double) * (size_t)ctx->sm_count * kTcSideDoubles));
-  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_red), sizeof(double) * (kTcAccElems + 16 + kMaxD + 8)));
-  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->shift), sizeof(float) * 64 * (kMaxD + 1)));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_red), sizeof(double) * (kTcAccElems + 16)));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->shift), gram_shift_bytes()));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->simt_part), sizeof(double) * (size_t)ctx->simt_ctas * kMaxS * kMaxS));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->score_part), sizeof(double) * ((size_t)ctx->score_ctas + 2) * 10));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->coef_dev), sizeof(double) * (kMaxD + 1)));
@@ -358,10 +361,10 @@ static int ctx_allocate(b2_ctx* ctx) {
   ctx->xchg_status_host[0] = 0u;
   B2_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&ctx->coef_host), 2 * sizeof(double) * (kMaxD + 1), cudaHostAllocDefault));
   for (int b = 0; b < 2; ++b) B2_CUDA(cudaEventCreateWithFlags(&ctx->ev_coef[b], cudaEventDisableTiming));
-  B2_CUDA(cudaMemset(ctx->shift, 0, sizeof(float) * 64 * (kMaxD + 1)));
+  B2_CUDA(cudaMemset(ctx->shift, 0, gram_shift_bytes()));
   B2_CUDA(cudaMemset(ctx->S, 0, sizeof(double) * kMaxS * kMaxS));
   B2_CUDA(cudaMemset(ctx->tc_side, 0, sizeof(double) * (size_t)ctx->sm_count * kTcSideDoubles));
-  B2_CUDA(cudaMemset(ctx->tc_red, 0, sizeof(double) * (kTcAccElems + 16 + kMaxD + 8)));
+  B2_CUDA(cudaMemset(ctx->tc_red, 0, sizeof(double) * (kTcAccElems + 16)));
   return B2_OK;
 }
 

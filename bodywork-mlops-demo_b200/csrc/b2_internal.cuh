@@ -61,8 +61,8 @@ struct b2_ctx {
   // tensor-core path scratch
   double* tc_part = nullptr;           // [sm_count][kTcAccElems]   per-CTA fp64 partial Gram (col-major)
   double* tc_side = nullptr;           // [sm_count][kTcSideDoubles]
-  double* tc_red = nullptr;            // [kTcAccElems + 16 + 129 + pad]: reduced partials, y sums, barrier slot, shift
-  float* shift = nullptr;              // [64][kMaxD + 1] partial sums of the row sample -> per-column shift c
+  double* tc_red = nullptr;            // [kTcAccElems + 16]: reduced partials, y sums, b2_comm_barrier's slot at + 8
+  float* shift = nullptr;              // gram_shift_bytes(): per-column shift c[kMaxD + 1] (c_y at kMaxD), sample scratch
   bool tc_attr_set = false;
   bool solve_attr_set = false;
   double* solve_host = nullptr;        // pinned mirror of solve_out (D2H without a staging copy)
@@ -120,9 +120,11 @@ struct b2_ctx {
 namespace b2 {
 
 // ---- kernel launchers (each enqueues on ctx->stream and bumps ctx->launches) -----------------
-// The three Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites
+// The Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites
 // it instead of adding to it (the first writer after b2_gram_reset).  The tensor-core and narrow launchers cover the
-// first gram_*_main_rows(n) rows; their per-column shift is sampled from all n rows.
+// first gram_*_main_rows(n) rows and read the per-column shift c that launch_gram_shift sampled from all n rows.
+size_t gram_shift_bytes();
+int launch_gram_shift(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx);
 int launch_gram_simt(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
                      int64_t ldx, const uint8_t* mask, int keep, bool assign);
 bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, int d, int64_t ldx,

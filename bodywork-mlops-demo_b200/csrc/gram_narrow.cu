@@ -24,6 +24,7 @@
 
 #include "b2_internal.cuh"
 #include "b2_ptx.cuh"
+#include "b2_shift.cuh"
 
 namespace b2 {
 namespace {
@@ -33,8 +34,6 @@ constexpr int kNwMaxDP = 16;
 constexpr int kNwM = kNwMaxDP + 2;            // side of the per-CTA partial (features | ones | y)
 constexpr int kNwMM = kNwM * kNwM;            // doubles per CTA partial (row stride DP + 2 inside)
 constexpr int kNwFlushRows = 2048;            // rows per lane between fp32 -> fp64 folds
-constexpr int kNwShiftSamples = 2048;
-constexpr int kNwCY = kNwMaxDP;               // slot of c_y in the shift vector
 
 template <int DP>
 struct NwGeom {
@@ -64,36 +63,6 @@ __device__ __forceinline__ float shfl_bfly_ordered(float v, int off) {
   float r;
   asm volatile("shfl.sync.bfly.b32 %0, %1, %2, 0x1f, 0xffffffff;" : "=f"(r) : "f"(v), "r"(off));
   return r;
-}
-
-// ---- per-column shift: mean of the finite values of a strided row sample (any c is algebraically exact, see
-// narrow_fold_kernel) ---------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void narrow_shift_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n, int d,
-                                    float* __restrict__ cvec) {
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;   // warp w: feature w (w < d), warp d: y
-  if (w > kNwMaxDP) return;
-  if (w > d) { if (lane == 0 && w < kNwMaxDP) cvec[w] = 0.f; return; }
-  const int64_t samples = n < kNwShiftSamples ? n : kNwShiftSamples;
-  const int64_t stride = n / samples;
-  float acc = 0.f;
-  int cnt = 0;
-  for (int64_t s = lane; s < samples; s += 32) {
-    const int64_t row = s * stride;
-    const float v = (w < d) ? raw_ld_global<T>(X + row * d + w) : __ldg(y + row);
-    const bool finite = fabsf(v) <= 3.0e38f;    // the sample ignores the row mask: a dropped row may hold NaN / Inf
-    acc += finite ? v : 0.f;
-    cnt += finite ? 1 : 0;
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    acc += __shfl_xor_sync(0xffffffffu, acc, off);
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-  }
-  if (lane == 0) {
-    cvec[w < d ? w : kNwCY] = cnt > 0 ? acc / (float)cnt : 0.f;
-    if (w == d && d < kNwMaxDP) cvec[d] = 0.f;
-  }
 }
 
 // ---- fp32 pairs: the accumulators below are written as pairs of lanes; sm_90 has no packed fp32 arithmetic, so a pair
@@ -183,14 +152,14 @@ gram_narrow_kernel(const T* __restrict__ X, const float* __restrict__ y, const u
   // minus the shift: registers when a lane owns the whole row; for the two-lane split they would not fit beside the
   // accumulators, so the row loop re-reads them from shared memory (broadcast loads)
   const uint32_t cs = sbase + G::kOffShift;
-  if (ctid < 20) reinterpret_cast<float*>(smem_raw + G::kOffShift)[ctid] = ctid <= kNwCY ? -cvec[ctid] : 0.f;
+  if (ctid < 20) reinterpret_cast<float*>(smem_raw + G::kOffShift)[ctid] = ctid < kNwMaxDP ? -cvec[ctid] : 0.f;
   asm volatile("bar.sync 1, %0;" ::"n"(G::kConsumers) : "memory");
   uint64_t ncP[NQ];
   if constexpr (TPR == 1) {
 #pragma unroll
     for (int q = 0; q < NQ; ++q) ncP[q] = pack2(-cvec[2 * q], NP >= 2 ? -cvec[2 * q + 1] : 0.f);
   }
-  const float cy = cvec[kNwCY];
+  const float cy = cvec[kMaxD];
   const float cvec_c0 = cvec[0];
 
   uint64_t tri2[NT2], py2[NQ], p12[NQ], ab2[(NA / 2) * NB], ys2 = 0ull;
@@ -416,25 +385,12 @@ narrow_fold_kernel(const double* __restrict__ part, int n_ctas, int DP, int d, c
   const int dp = d + 2;
   auto M = [&](int i, int j) { return i <= j ? m[i * MS + j] : m[j * MS + i]; };
   const int ONE = DP, Y = DP + 1;
-  const double n = M(ONE, ONE), sy = M(ONE, Y), syy = M(Y, Y), cy = (double)cvec[kNwCY];
+  auto s1 = [&](int i) { return M(i, ONE); };
+  auto sxy = [&](int i) { return M(i, Y); };
+  const double n = M(ONE, ONE), sy = M(ONE, Y), syy = M(Y, Y);
   for (int idx = threadIdx.x; idx < dp * dp; idx += blockDim.x) {
     const int r = idx / dp, q = idx % dp;
-    const int a = r < q ? r : q, b = r < q ? q : r;   // (a, b) and (b, a) evaluate the same expression: S stays bit-symmetric
-    double val;
-    if (b < d) {
-      const double ca = (double)cvec[a], cb = (double)cvec[b];
-      val = M(a, b) + ca * M(b, ONE) + cb * M(a, ONE) + n * ca * cb;
-    } else if (a < d) {
-      const double ci = (double)cvec[a];
-      if (b == d) val = M(a, ONE) + n * ci;
-      else val = M(a, Y) + cy * M(a, ONE) + ci * sy + n * ci * cy;
-    } else if (a == d && b == d) {
-      val = n;
-    } else if (a == d + 1) {
-      val = syy + 2.0 * cy * sy + n * cy * cy;
-    } else {
-      val = sy + n * cy;
-    }
+    const double val = unshift_entry(r < q ? r : q, r < q ? q : r, d, cvec, M, s1, sxy, n, sy, syy);
     S[idx] = assign ? val : S[idx] + val;
   }
 }
@@ -474,14 +430,12 @@ int narrow_tile_rows(int DP) {
        : DP == 8 ? NwGeom<8>::kRows : NwGeom<16>::kRows;
 }
 
-// the full tiles of the first gram_narrow_main_rows(n, d) rows; the shift sample covers all n rows
+// the full tiles of the first gram_narrow_main_rows(n, d) rows
 template <typename T>
 int launch_narrow_t(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask, int keep, int64_t n, int d,
                     bool assign) {
   const int DP = narrow_dp(d);
   const int n_tiles = (int)(n / narrow_tile_rows(DP));   // n <= INT32_MAX rows (gram_narrow_supported)
-  narrow_shift_kernel<T><<<1, 32 * (kNwMaxDP + 1), 0, ctx->stream>>>(X, y, n, d, ctx->shift);
-  B2_CUDA(cudaGetLastError());
   const int pair = ctx->k_pairs % kKernelEventPairs;
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
   int grid = 0, rc = B2_OK;
@@ -497,7 +451,7 @@ int launch_narrow_t(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask
   ctx->k_pairs += 1;
   narrow_fold_kernel<<<1, 384, 0, ctx->stream>>>(ctx->simt_part, grid, DP, d, ctx->shift, assign ? 1 : 0, ctx->S);
   B2_CUDA(cudaGetLastError());
-  ctx->launches += 3;
+  ctx->launches += 2;
   return B2_OK;
 }
 

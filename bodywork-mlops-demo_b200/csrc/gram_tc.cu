@@ -26,13 +26,14 @@
 // the centring in the solve subtracts almost nothing.  hi+lo carries 16 mantissa bits, i.e. products are
 // accurate to ~2^-17 relative (lo*lo is dropped).
 //
-// tc_reduce_kernel sums the per-CTA partials in a fixed order (deterministic); tc_fold_kernel undoes the shift
-// in fp64 and adds the result to the context's raw statistic S = [X 1 y]^T [X 1 y].
+// The shift c comes from gram_shift.cu.  tc_finalize_kernel sums the per-CTA partials in a fixed order
+// (deterministic), undoes the shift in fp64 and adds the result to the context's raw statistic S = [X 1 y]^T [X 1 y].
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
 #include "b2_internal.cuh"
 #include "b2_ptx.cuh"
+#include "b2_shift.cuh"
 #include "b2_xchg.cuh"
 
 namespace b2 {
@@ -229,75 +230,7 @@ __device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_
 }
 
 // ------------------------------------------------------------------------------------------
-// per-column shift c: mean of the finite values of a strided row sample (any value near the column mean will do;
-// the algebra in tc_fold_kernel is exact for every c)
-// ------------------------------------------------------------------------------------------
-constexpr int kShiftBlocks = 64;                 // partial means of the row sample, one per block
-constexpr int kShiftStride = kMaxD + 1;          // floats per partial: features, then y (slot kMaxD)
-
-__host__ __device__ __forceinline__ int64_t shift_samples(int64_t n) { return n < 2048 ? n : 2048; }
-
-// c_j from the 64 partial means (NaN: a block without a finite sample), kept in fp32: the operands carry |x - c| / sigma,
-// so a c rounded to bf16 (spacing 64 at a column mean of 1e4) would cost fp32 rows digits wherever a column's mean is
-// large against its spread.  For bf16 rows (`round_bf16`) the feature shifts are rounded to bf16: x and c then share
-// one grid, x - c is exact, and hi + lo holds it.  The Gram kernel and tc_finalize_kernel call this on the same 64
-// values -> identical c.
-__host__ __device__ __forceinline__ float shift_round(float c, bool round_bf16) {
-  return round_bf16 ? __bfloat162float(__float2bfloat16_rn(c)) : c;
-}
-__device__ __forceinline__ float shift_value(const float* sp, int j, bool round_bf16) {
-  float acc = 0.f;
-  int cnt = 0;
-#pragma unroll 8
-  for (int b = 0; b < kShiftBlocks; ++b) {
-    const float p = sp[b * kShiftStride + j];
-    if (p == p) { acc += p; ++cnt; }
-  }
-  return shift_round(cnt > 0 ? acc / (float)cnt : 0.f, round_bf16);
-}
-
-// 64 blocks x (4 row groups x 160 columns): a thread sums 8 sample rows (one batch of loads in flight -- the rows are
-// megabytes apart, every load is a DRAM round trip), the 4 groups are combined in a fixed order.
-constexpr int kShiftCols = 160;                  // >= kMaxD + 1, a multiple of 32
-constexpr int kShiftGroups = 4;
-
-template <typename T>
-__global__ void __launch_bounds__(kShiftCols * kShiftGroups)
-tc_shift_kernel(const T* __restrict__ X, const float* __restrict__ y, int64_t n, int d,
-                int64_t ldx, float* __restrict__ sp) {
-  __shared__ float sub[kShiftGroups][kShiftCols];
-  __shared__ int subn[kShiftGroups][kShiftCols];
-  const int j = threadIdx.x % kShiftCols, g = threadIdx.x / kShiftCols;
-  const int64_t samples = shift_samples(n);
-  const int64_t stride = n / samples;
-  const int64_t per = (samples + kShiftBlocks - 1) / kShiftBlocks;
-  const int64_t s0 = blockIdx.x * per;
-  const int64_t s1 = (s0 + per < samples) ? s0 + per : samples;
-  float acc = 0.f;
-  int cnt = 0;
-  if (j <= d) {
-#pragma unroll 8
-    for (int64_t s = s0 + g; s < s1; s += kShiftGroups) {
-      const int64_t row = s * stride;
-      const float v = (j < d) ? raw_ld_global<T>(X + row * ldx + j) : __ldg(y + row);
-      const bool finite = fabsf(v) <= 3.0e38f;    // the sample ignores the row mask: a dropped row may hold NaN / Inf
-      acc += finite ? v : 0.f;
-      cnt += finite ? 1 : 0;
-    }
-  }
-  sub[g][j] = acc;
-  subn[g][j] = cnt;
-  __syncthreads();
-  if (g == 0 && j <= d) {
-    const int c = subn[0][j] + subn[1][j] + subn[2][j] + subn[3][j];
-    sp[blockIdx.x * kShiftStride + (j == d ? kMaxD : j)] =
-        c > 0 ? (((sub[0][j] + sub[1][j]) + sub[2][j]) + sub[3][j]) / (float)c : __int_as_float(0x7fc00000);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// finalize, shared by the stand-alone kernels (tc_reduce_kernel / tc_fold_kernel: the b2_gram_accumulate path) and
-// by the fused tail of the Gram kernel (b2_fit): the same summation order in both, so the two paths agree bit for bit.
+// finalize: the per-CTA partials reduced into
 //   red[col * 128 + i], col in [0, 288):  col < 144: D1 (A = hi), col >= 144: D2 (A = lo), columns of [hi | E]
 //   red[kTcAccElems + 0..2]            : sum y', sum y'^2, rows used
 // ------------------------------------------------------------------------------------------
@@ -368,12 +301,9 @@ __device__ __forceinline__ void grid_barrier(unsigned int* ctr) {
 // `pack` original rows share one 128-wide super-row (d * pack == 128 when pack > 1): original feature a of
 // sub-row blk is super-feature blk*d + a, and its E columns are 128 + 3*blk (+0 ones, +1 y'_hi, +2 y'_lo).
 // The true statistic is the sum over blk of the diagonal (blk, blk) blocks.
-// Returns the contribution of this launch to S[idx]; c[j] = the shift of feature j, c[kMaxD] = the shift of y
-// (fp64 copy in `red` for the stand-alone kernel, the CTA's fp32 smem copy in the fused tail -- the same values).
-template <typename CT>
-__device__ __forceinline__ double tc_fold_value(const double* red, const CT* c, int d, int pack, int idx) {
+// Returns the contribution of this launch to S[idx]; c[j] = the shift of feature j, c[kMaxD] = the shift of y.
+__device__ __forceinline__ double tc_fold_value(const double* red, const double* c, int d, int pack, int idx) {
   const int dp = d + 2;
-  // (a, b) and (b, a) evaluate the same expression in the same order: S is exactly symmetric
   const int a = min(idx / dp, idx % dp), b = max(idx / dp, idx % dp);
   // D1[i][j] = red[j*128 + i], D2[i][j] = red[(144 + j)*128 + i]
   auto D1 = [&](int i, int j) { return __ldcg(red + (size_t)j * kTcM + i); };
@@ -391,34 +321,16 @@ __device__ __forceinline__ double tc_fold_value(const double* red, const CT* c, 
     }
     return t;
   };
-  const double sy = __ldcg(red + kTcAccElems + 0);
-  const double syy = __ldcg(red + kTcAccElems + 1);
-  const double n = __ldcg(red + kTcAccElems + 2);
-  const double cy = (double)c[kMaxD];
-  double val;
-  if (a < d && b < d) {
-    const double ca = (double)c[a], cb = (double)c[b];
-    // G'(a,b) = sum (x_a-c_a)(x_b-c_b) ~= hi.hi + lo.hi + hi.lo   (lo.lo dropped, ~2^-18 relative)
+  auto G = [&](int i, int j) {                    // sum v_i v_j ~= hi.hi + lo.hi + hi.lo   (lo.lo dropped, ~2^-18 relative)
     double g = 0.0;
     for (int blk = 0; blk < pack; ++blk) {
-      const int ia = blk * d + a, ib = blk * d + b;
+      const int ia = blk * d + i, ib = blk * d + j;
       g += 0.5 * (D1(ia, ib) + D1(ib, ia)) + D2(ia, ib) + D2(ib, ia);
     }
-    val = g + ca * s1(b) + cb * s1(a) + n * ca * cb;
-  } else if (a < d || b < d) {
-    const int i = a < d ? a : b;
-    const int o = a < d ? b : a;  // d (ones) or d+1 (y)
-    const double ci = (double)c[i];
-    if (o == d) val = s1(i) + n * ci;
-    else val = sxy(i) + cy * s1(i) + ci * sy + n * ci * cy;
-  } else if (a == d && b == d) {
-    val = n;
-  } else if (a == d + 1 && b == d + 1) {
-    val = syy + 2.0 * cy * sy + n * cy * cy;
-  } else {
-    val = sy + n * cy;
-  }
-  return val;
+    return g;
+  };
+  return unshift_entry(a, b, d, c, G, s1, sxy, __ldcg(red + kTcAccElems + 2), __ldcg(red + kTcAccElems + 0),
+                       __ldcg(red + kTcAccElems + 1));
 }
 
 // ------------------------------------------------------------------------------------------
@@ -494,8 +406,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   // packed rows (pack > 1): super-row feature i < pack * d_orig is original feature i % d_orig -> the shift repeats;
   // the columns from pack * d_orig to 127 are TMA out-of-bounds zero fill and keep shift 0 (they contribute nothing)
   for (int j = threadIdx.x; j <= kMaxD; j += kThreads)
-    shift_s[j] = (j == kMaxD) ? shift_value(shift, kMaxD, false)
-                              : (j < pack * d_orig ? shift_value(shift, j % d_orig, sizeof(T) == 2) : 0.f);
+    shift_s[j] = j == kMaxD ? shift[kMaxD] : (j < pack * d_orig ? shift[j % d_orig] : 0.f);
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -836,13 +747,6 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// finalize: tc_reduce_kernel sums the per-CTA partials in CTA order (deterministic)
-//   red[col * 128 + i], col in [0, 288):  col < 144: D1 (A = hi), col >= 144: D2 (A = lo), columns of [hi | E]
-//   red[kTcAccElems + 0..2]            : sum y', sum y'^2, rows used
-// tc_fold_kernel undoes the shift in fp64 and adds the result into the raw statistic S ((d+2)^2, stride d+2).
-// ------------------------------------------------------------------------------------------
-
 // What tc_finalize_kernel does after the reduce + fold (passed by value).
 struct TcFinal {
   int assign;                 // S = value instead of S += value (first writer of a fresh statistic)
@@ -862,17 +766,10 @@ constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinaliz
 
 __global__ void __launch_bounds__(kFinalizeThreads, 1)
 tc_finalize_kernel(const double* part, const double* side, int n_ctas, double* red, const float* __restrict__ shift,
-                   int d, int pack, int x_bf16, double* S, unsigned int* sync, const TcFinal fin) {
+                   int d, int pack, double* S, unsigned int* sync, const TcFinal fin) {
   __shared__ double quarter[kFinalizeThreads];
   __shared__ double c_s[kMaxD + 1];                              // the shift as fp64 (c_s[kMaxD]: c_y)
-  __shared__ float c_part[kShiftBlocks * kShiftStride];          // the 64 partial means of the shift sample (33 KB)
-  // the same values shift_value() gives the Gram kernel -- the same function on the same 64 partials -- but with
-  // all loads of the CTA in flight at once: the serial walk (8 batches of dependent-latency loads by 129 threads while
-  // 895 wait at the next barrier) dominated this kernel
-  for (int idx = threadIdx.x; idx < kShiftBlocks * kShiftStride; idx += blockDim.x) c_part[idx] = __ldg(shift + idx);
-  __syncthreads();
-  for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x)
-    c_s[j] = (j < d || j == kMaxD) ? (double)shift_value(c_part, j, x_bf16 != 0 && j < d) : 0.0;
+  for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x) c_s[j] = (double)shift[j];
   {
     constexpr int epb = kFinalizeThreads / 4;                    // elements per pass of a CTA
     const int per = (((kRedElems + (int)gridDim.x - 1) / (int)gridDim.x) + epb - 1) / epb * epb;
@@ -1044,7 +941,7 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   const int es = x_dtype == B2_F32 ? 4 : 2;
   // Row packing: `pack` contiguous rows of 17..64 features are viewed as one super-row of pack * d_in <= 128 columns
   // ([n / pack][pack * d_in], zero-filled by TMA to the 128-wide tile) and run on the D = 128 fast path; the diagonal
-  // d_in x d_in blocks of the 128 x 128 Gram sum to the true statistic (tc_fold_kernel).  The tensor maps cover a
+  // d_in x d_in blocks of the 128 x 128 Gram sum to the true statistic (tc_fold_value).  The tensor maps cover a
   // multiple of lcm(pack, 16) rows (the y / mask views are 16-byte rows); the caller runs the < 80 leftover rows on
   // the CUDA-core kernel.
   int pack = 1;
@@ -1095,14 +992,6 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
                                  TcGeo<true>::kSmemBytes));
     ctx->tc_attr_set = true;
   }
-
-  if (x_dtype == B2_F32)
-    tc_shift_kernel<float><<<kShiftBlocks, kShiftCols * kShiftGroups, 0, ctx->stream>>>(static_cast<const float*>(X), y, n_in, d_in,
-                                                                  ldx_in, ctx->shift);
-  else
-    tc_shift_kernel<__nv_bfloat16><<<kShiftBlocks, kShiftCols * kShiftGroups, 0, ctx->stream>>>(static_cast<const __nv_bfloat16*>(X), y,
-                                                                          n_in, d_in, ldx_in, ctx->shift);
-  B2_CUDA(cudaGetLastError());
 
 #ifdef B2_DEV_KNOBS
   static const uint32_t wait_ns = []() {   // development knob: suspend-time hint of the pipeline waits
@@ -1164,11 +1053,10 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     cfg.attrs = attr; cfg.numAttrs = 1;
     const double* part_arg = ctx->tc_part; const double* side_arg = ctx->tc_side;
     const float* shift_arg = ctx->shift;
-    const int x_bf16 = x_dtype == B2_BF16 ? 1 : 0;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, side_arg, grid, ctx->tc_red, shift_arg, d_in, pack, x_bf16,
+    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, side_arg, grid, ctx->tc_red, shift_arg, d_in, pack,
                                ctx->S, ctx->tc_sync, fin));
   }
-  ctx->launches += 3;
+  ctx->launches += 2;
   return B2_OK;
 }
 
