@@ -58,6 +58,9 @@ _SIGNATURES = {
     "b2_upload_columns": (C.c_int, [_vp, _vp, _vp, C.c_int, _c_i64, C.c_int, _vp]),
     "b2_fit": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_double, C.c_int, _vp,
                          C.POINTER(C.c_double)]),
+    "b2_fit_refined": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_double,
+                                 C.c_int, C.c_int, C.c_double, _vp, C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                 C.POINTER(C.c_double)]),
     "b2_solve": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_double)]),
     "b2_solve_eigvals": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_int), C.POINTER(_c_i64)]),
     "b2_solve_spectral": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_double), _vp, C.POINTER(C.c_int)]),
@@ -387,6 +390,27 @@ class Context:
             raise np.linalg.LinAlgError(last_error())
         _check(rc, "b2_fit")
         return coef, float(b0.value)
+
+    def fit_refined(self, X, y, row_mask=None, mask_keep: int = 1, alpha: float = 0.0, fit_intercept: bool = True,
+                    max_passes: int = 2, tol: float = 1e-10) -> Tuple[np.ndarray, float, int, float]:
+        """``fit``, then up to ``max_passes`` residual passes over the same rows (b2_fit_refined): each pass reads the
+        rows once for the fp64 gradient and corrects the solution through the factor of the Gram.  Returns (coef,
+        intercept, passes kept, last step); the step is max_j |dcoef_j| sigma_j / sigma_y.  Raises
+        ``np.linalg.LinAlgError`` on a rank-deficient Gram."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        coef = np.empty(d, dtype=np.float64)
+        b0, step, passes = C.c_double(0.0), C.c_double(0.0), C.c_int(0)
+        rc = load().b2_fit_refined(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(alpha),
+                                   int(bool(fit_intercept)), int(max_passes), float(tol), coef.ctypes.data, C.byref(b0),
+                                   C.byref(passes), C.byref(step))
+        self.d = int(d)
+        self.serial += 1
+        if rc == E_SINGULAR:
+            raise np.linalg.LinAlgError(last_error())
+        _check(rc, "b2_fit_refined")
+        return coef, float(b0.value), int(passes.value), float(step.value)
 
     # -- solve -----------------------------------------------------------------------------------------
     def solve(self, alpha: float = 0.0, fit_intercept: bool = True) -> Tuple[np.ndarray, float]:

@@ -353,6 +353,8 @@ static int ctx_allocate(b2_ctx* ctx) {
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->simt_part), sizeof(double) * (size_t)ctx->simt_ctas * kMaxS * kMaxS));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->score_part), sizeof(double) * ((size_t)ctx->score_ctas + 2) * 10));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->coef_dev), sizeof(double) * (kMaxD + 1)));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->grad_part), sizeof(double) * (size_t)ctx->score_ctas * kGradOut));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->refine), sizeof(double) * kRfDoubles));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->solve_out), sizeof(double) * (2 * kMaxD + 8)));
   B2_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&ctx->solve_host), sizeof(double) * (2 * kMaxD + 8), cudaHostAllocDefault));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_sync), 64));
@@ -407,7 +409,8 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   if (ctx->xchg != nullptr) cudaFree(ctx->xchg);
   void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_side, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
-                  ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count};
+                  ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
+                  ctx->grad_part, ctx->refine};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -773,6 +776,86 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
   }
   if (int r = launch_solve_cholesky(ctx, alpha, fit_intercept, gather_epoch)) return r;
   return finish_cholesky(ctx, coef, intercept);
+}
+
+// ---- the refined fit: b2_fit, then residual passes over the same rows (DESIGN.md section 2) ------------------------
+// Per pass: the gradient kernels (+ their ordered reduce) over the rows -- host rows re-stream through the staging ring --
+// then the Cholesky kernel in refinement mode, which refactors A + alpha I from S, solves for the correction and moves
+// the state; one host synchronisation reads the step and the guard.
+int b2_fit_refined(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                   int mem_kind, const uint8_t* row_mask, int mask_keep, double alpha, int fit_intercept, int max_passes,
+                   double tol, double* coef, double* intercept, int* passes_out, double* step_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (max_passes < 0 || max_passes > 16) { set_error("max_passes=%d out of range [0,16]", max_passes); return B2_E_ARG; }
+  if (!(tol >= 0.0)) { set_error("tol must be >= 0"); return B2_E_ARG; }
+  if (coef == nullptr || intercept == nullptr) { set_error("coef / intercept is null"); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) {
+    set_error("b2_fit_refined runs on one rank only (the residual gradient is not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (passes_out != nullptr) *passes_out = 0;
+  if (step_out != nullptr) *step_out = 0.0;
+  if (int r = b2_fit(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, alpha, fit_intercept, coef,
+                     intercept))
+    return r;
+  if (max_passes == 0) return B2_OK;
+  // the state: beta from the fit; m and b0' from S as the solve forms them
+  const int dp = d + 2;
+  std::vector<double> S((size_t)dp * dp), st(kRfDoubles, 0.0);
+  B2_CUDA(cudaMemcpyAsync(S.data(), ctx->S, sizeof(double) * dp * dp, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const double n = S[(size_t)d * dp + d];
+  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
+  for (int j = 0; j < d; ++j) {
+    st[kRfBeta + j] = coef[j];
+    st[kRfPrevBeta + j] = coef[j];
+    st[kRfMean + j] = fit_intercept ? S[(size_t)j * dp + d] * inv_n : 0.0;
+  }
+  st[kRfB0] = st[kRfPrevB0] = fit_intercept ? S[(size_t)d * dp + d + 1] * inv_n : 0.0;
+  st[kRfStep] = INFINITY;
+  B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = mem_kind == B2_MEM_HOST && host_pointer_is_pinned(X);
+  if (mem_kind == B2_MEM_HOST)
+    if (int r = ensure_staging(ctx)) return r;
+  const double* h = ctx->solve_host;
+  int kept = 0;
+  for (int pass = 0; pass < max_passes; ++pass) {
+    if (mem_kind == B2_MEM_DEVICE) {
+      if (int r = launch_grad(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, true)) return r;
+    } else if (int r = stream_host_blocks(
+                   ctx, n_rows, ctx->stage_rows,
+                   [&](int buf, int64_t r0, int64_t rows) {
+                     return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
+                   },
+                   [&](int buf, int64_t r0, int64_t rows) {
+                     return launch_grad(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
+                                        row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, r0 == 0);
+                   })) {
+      return r;
+    }
+    if (n_rows == 0 && mem_kind == B2_MEM_HOST)
+      if (int r = launch_grad(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, true)) return r;
+    if (int r = launch_solve_refine(ctx, alpha, fit_intercept)) return r;
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h[kMaxD + 1] != 0.0) {
+      set_error("pivot %d of the LDL^T factorisation is not positive in a refinement pass", (int)h[kMaxD + 1]);
+      return B2_E_SINGULAR;
+    }
+    if (step_out != nullptr) *step_out = h[kOutRefineStep];
+    if (h[kOutRefineGuard] != 0.0) {         // the state went back to before the last kept correction
+      kept = kept > 0 ? kept - 1 : 0;
+      break;
+    }
+    ++kept;
+    if (h[kOutRefineStep] <= tol) break;
+  }
+  memcpy(coef, h, sizeof(double) * d);
+  *intercept = h[kMaxD];
+  if (passes_out != nullptr) *passes_out = kept;
+  return B2_OK;
 }
 
 // ---- scoring ---------------------------------------------------------------------------------------

@@ -26,6 +26,21 @@ constexpr int kTcAccCols = 2 * kTcN;     // two accumulators: A = hi and A = lo 
 constexpr int kTcAccElems = kTcM * kTcAccCols;  // fp32 accumulators drained per chunk (36 864)
 constexpr int kTcSideDoubles = 8;        // per-CTA CUDA-core sums: sum y', sum y'^2, rows used
 
+// ---- refined fit (b2_fit_refined): the model y = b0' + (x - m).beta and its residual passes -----------------------
+constexpr int kGradOut = kMaxD + 1;      // one gradient: g_j = sum (x_j - m_j) e at j < kMaxD, g_1 = sum e at kMaxD
+// doubles of ctx->refine
+constexpr int kRfBeta = 0;               // beta
+constexpr int kRfB0 = kMaxD;             // b0'
+constexpr int kRfMean = kMaxD + 1;       // m: S's column means (0 without an intercept)
+constexpr int kRfPrevBeta = 2 * kMaxD + 1;   // beta and b0' before the last kept correction (where the guard returns)
+constexpr int kRfPrevB0 = 3 * kMaxD + 1;
+constexpr int kRfStep = 3 * kMaxD + 2;   // step of the last kept correction (+inf before the first)
+constexpr int kRfGrad = 3 * kMaxD + 3;   // the reduced gradient of the current pass [kGradOut]
+constexpr int kRfDoubles = kRfGrad + kGradOut;
+// solve_out / solve_host slots of the refinement solve (beside coef [0, d), intercept kMaxD, info kMaxD + 1)
+constexpr int kOutRefineStep = 2 * kMaxD + 3;
+constexpr int kOutRefineGuard = 2 * kMaxD + 4;
+
 void set_error(const char* fmt, ...);
 
 #define B2_CUDA(call)                                                                      \
@@ -79,6 +94,9 @@ struct b2_ctx {
   double* score_part = nullptr;        // [score_ctas][6]
   int score_ctas = 0;
   double* coef_dev = nullptr;          // [kMaxD + 1]
+  // refined fit scratch
+  double* grad_part = nullptr;         // [score_ctas][kGradOut] per-CTA gradient partials
+  double* refine = nullptr;            // [kRfDoubles] beta, b0', m, the state before the last correction, step, gradient
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -145,6 +163,13 @@ int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int6
 int launch_solve_spectral(b2_ctx* ctx, double cond, int fit_intercept);
 int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx,
                  const float* y, const uint8_t* mask, int keep, float* yhat, bool first_block);
+// residual gradient of the refined fit over the model in ctx->refine; `first_block` overwrites the gradient, otherwise
+// the rows' sums are added to it
+int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                const uint8_t* mask, int keep, bool first_block);
+// the correction solve of one refinement pass: (A + alpha I) dbeta = g - alpha beta from the factor of S, then the
+// update of ctx->refine; the result goes to ctx->solve_host
+int launch_solve_refine(b2_ctx* ctx, double alpha, int fit_intercept);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

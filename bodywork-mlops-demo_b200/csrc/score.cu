@@ -755,6 +755,357 @@ metrics_kernel(const V* __restrict__ ya, const V* __restrict__ yp, int64_t n, do
   }
 }
 
+// ---- residual gradient of the refined fit (b2_fit_refined; DESIGN.md section 2) -----------------------------------------
+// The model is yhat = b0' + (x - m).beta (st: ctx->refine).  Per kept row e = y - b0' - (x - m).beta, and the pass sums
+// g_j = sum (x_j - m_j) e and g_1 = sum e, everything in fp64 from the exactly converted x: e is a small difference of
+// large terms.  The three layouts of scoring carry it: register-fed (any layout, the tails), the TMA ring (wide contiguous
+// rows), one lane per row (d <= 16).  A lane keeps the fp64 sums of the features it loads.  A dropped row gets x = 0 and
+// e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA combines its sums in a fixed order into
+// part[blockIdx.x][kGradOut] (features, then g_1 at kMaxD); grad_reduce_kernel adds the CTAs in order.
+template <typename T>
+__device__ __forceinline__ float ld_x_f32(const T* __restrict__ p);
+template <>
+__device__ __forceinline__ float ld_x_f32<float>(const float* __restrict__ p) { return __ldg(p); }
+template <>
+__device__ __forceinline__ float ld_x_f32<__nv_bfloat16>(const __nv_bfloat16* __restrict__ p) { return __bfloat162float(*p); }
+
+// register-fed: one warp per row, four rows in flight; lane features lane * 4 + k (vec) or lane + 32 k
+template <typename T>
+__global__ void __launch_bounds__(kScoreThreads)
+grad_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double* __restrict__ st,
+            const float* __restrict__ y, const uint8_t* __restrict__ mask, int keep, int vec, double* __restrict__ part) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double cf[4], mv[4], acc[4], acc1 = 0.0;
+  int fj[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    fj[k] = vec ? lane * 4 + k : lane + 32 * k;
+    cf[k] = fj[k] < d ? st[kRfBeta + fj[k]] : 0.0;
+    mv[k] = fj[k] < d ? st[kRfMean + fj[k]] : 0.0;
+    acc[k] = 0.0;
+  }
+  const double b0 = st[kRfB0];
+  const int64_t warps_total = (int64_t)gridDim.x * kScoreWarps;
+  const int64_t gw = (int64_t)blockIdx.x * kScoreWarps + warp;
+  constexpr int kU = 4;
+  for (int64_t base = gw * kU; base < n; base += warps_total * kU) {
+    float x[kU][4];
+    bool use[kU];
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const int64_t row = base + u;
+      use[u] = row < n;
+      if (use[u] && mask != nullptr) use[u] = (__ldg(mask + row) == (uint8_t)keep);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) x[u][k] = 0.f;
+      const T* xr = X + row * ldx;
+      if (use[u]) {
+        if (vec) {
+          if (lane * 4 < d) {
+            if constexpr (sizeof(T) == 4) {
+              const float4 v = __ldg(reinterpret_cast<const float4*>(xr) + lane);
+              x[u][0] = v.x; x[u][1] = v.y; x[u][2] = v.z; x[u][3] = v.w;
+            } else {
+              const uint2 v = __ldg(reinterpret_cast<const uint2*>(xr) + lane);
+              x[u][0] = __uint_as_float(v.x << 16); x[u][1] = __uint_as_float(v.x & 0xffff0000u);
+              x[u][2] = __uint_as_float(v.y << 16); x[u][3] = __uint_as_float(v.y & 0xffff0000u);
+            }
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (fj[k] < d) x[u][k] = ld_x_f32<T>(xr + fj[k]);
+        }
+      }
+    }
+    double dot[kU];
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      double a = 0.0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) a = fma((double)x[u][k] - mv[k], cf[k], a);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) a += shfl_xor_d(a, o);   // every lane ends with the same sum (a + b == b + a)
+      dot[u] = a;
+    }
+#pragma unroll
+    for (int u = 0; u < kU; ++u) {
+      const float yv = use[u] ? __ldg(y + base + u) : 0.f;
+      const double e = use[u] ? ((double)yv - b0) - dot[u] : 0.0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc[k] = fma((double)x[u][k] - mv[k], e, acc[k]);
+      acc1 += e;
+    }
+  }
+  __shared__ double red[kScoreWarps][kGradOut];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (fj[k] < d) red[warp][fj[k]] = acc[k];
+  if (lane == 0) red[warp][kMaxD] = acc1;
+  __syncthreads();
+  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
+    double v = 0.0;
+    if (t < d || t == kMaxD)
+      for (int w = 0; w < kScoreWarps; ++w) v += red[w][t];
+    part[(size_t)blockIdx.x * kGradOut + t] = v;
+  }
+}
+
+// TMA ring: the producer and the lane layout of score_tma_kernel; the labels are always streamed.  beta and the sums stay in
+// registers, m is read from shared memory (two 16-byte loads per chunk): all three in registers spill at 128 per thread.
+template <typename T, int LPR>
+__global__ void __launch_bounds__(kTmThreads, 1)
+grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const double* __restrict__ st,
+                const float* __restrict__ y, const uint8_t* __restrict__ mask, int keep, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const uint32_t sbase = smem_u32(smem_raw);
+  const uint32_t bar_full = sbase + kTmOffBar, bar_empty = bar_full + 8 * kTmStages;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int RPI = 32 / LPR, kSweepRows = kTmWarps * RPI;
+  const int tile_rows = sweeps * kSweepRows;
+  const uint32_t pitch = (uint32_t)d * sizeof(T);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kTmStages; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, kTmWarps);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  __shared__ double red[kTmWarps][kGradOut];
+  __shared__ __align__(16) double m_s[kMaxD];
+  for (int f = threadIdx.x; f < kMaxD; f += blockDim.x) m_s[f] = f < d ? st[kRfMean + f] : 0.0;
+  __syncthreads();
+  if (warp == kTmWarps) {
+    if (lane == 0) {
+      const uint32_t xb = (uint32_t)tile_rows * pitch, yb = (uint32_t)tile_rows * 4u;
+      int it = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+        const int s = it % kTmStages;
+        if (it >= kTmStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kTmStages - 1) & 1));
+        const uint32_t full = bar_full + 8 * s;
+        mbar_expect_tx(full, xb + yb);
+        const int64_t row0 = (int64_t)tile * tile_rows;
+        bulk_load_1d(sbase + s * kTmXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * pitch, xb, full);
+        bulk_load_1d(sbase + kTmOffY + s * kTmYStage, y + row0, yb, full);
+      }
+    }
+  } else {
+    const int g = lane / LPR, j = lane % LPR;
+    double cf[4][4], acc[4][4];
+    bool col_ok[4];
+    uint32_t coff[4];
+    int f0[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int c = ((k + g) & 3) * LPR + j;
+      f0[k] = 4 * c;
+      col_ok[k] = f0[k] < d;
+      coff[k] = (uint32_t)c * 4u * (uint32_t)sizeof(T);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int f = f0[k] + e;
+        cf[k][e] = f < d ? st[kRfBeta + f] : 0.0;
+        acc[k][e] = 0.0;
+      }
+    }
+    const double b0 = st[kRfB0];
+    double acc1 = 0.0;
+    int s = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      const int64_t row0 = (int64_t)tile * tile_rows;
+      unsigned use_bits = 0xfu;
+      if (mask != nullptr) {
+        use_bits = 0u;
+#pragma unroll
+        for (int sw = 0; sw < kTmMaxSweeps; ++sw)
+          if (sw < sweeps)
+            use_bits |= (__ldg(mask + row0 + sw * kSweepRows + warp * RPI + g) == (uint8_t)keep ? 1u : 0u) << sw;
+      }
+      mbar_wait(bar_full + 8 * s, phase);
+      const uint32_t xs = sbase + s * kTmXStage, ys = sbase + kTmOffY + s * kTmYStage;
+      for (int sw = 0; sw < sweeps; ++sw) {
+        const int r = sw * kSweepRows + warp * RPI + g;
+        const bool use = (use_bits >> sw) & 1u;
+        const uint32_t row_addr = xs + (uint32_t)r * pitch;
+        float x[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) lds_row4<T>(row_addr + coff[k], use && col_ok[k], x[k]);
+        double v[4][4];                                                // x - m, exact inputs, one fp64 rounding
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const double2 m01 = *reinterpret_cast<const double2*>(&m_s[f0[k] & (kMaxD - 1)]);
+          const double2 m23 = *reinterpret_cast<const double2*>(&m_s[(f0[k] & (kMaxD - 1)) + 2]);
+          v[k][0] = (double)x[k][0] - m01.x; v[k][1] = (double)x[k][1] - m01.y;
+          v[k][2] = (double)x[k][2] - m23.x; v[k][3] = (double)x[k][3] - m23.y;
+        }
+        double a0 = 0.0, a1 = 0.0;                                     // two chains for latency
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          a0 = fma(v[0][e], cf[0][e], a0);
+          a1 = fma(v[2][e], cf[2][e], a1);
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          a0 = fma(v[1][e], cf[1][e], a0);
+          a1 = fma(v[3][e], cf[3][e], a1);
+        }
+        double a = a0 + a1;
+#pragma unroll
+        for (int o = LPR / 2; o >= 1; o >>= 1) a += shfl_xor_d(a, o);
+        const float yv = use ? ld_shared_f32(ys + 4u * (uint32_t)r) : 0.f;
+        const double e = use ? ((double)yv - b0) - a : 0.0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) acc[k][q] = fma(v[k][q], e, acc[k][q]);
+        if (j == 0) acc1 += e;
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+      if (++s == kTmStages) { s = 0; phase ^= 1u; }
+    }
+    // the row groups of a warp hold the same features (rotated): they add into red[warp] one group after the other
+#pragma unroll 1
+    for (int gg = 0; gg < RPI; ++gg) {
+      if (g == gg) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int f = f0[k] + q;
+            if (f < d) red[warp][f] = gg == 0 ? acc[k][q] : red[warp][f] + acc[k][q];
+          }
+        if (j == 0) red[warp][kMaxD] = gg == 0 ? acc1 : red[warp][kMaxD] + acc1;
+      }
+      __syncwarp();
+    }
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
+    double v = 0.0;
+    if (t < d || t == kMaxD)
+      for (int w = 0; w < kTmWarps; ++w) v += red[w][t];
+    part[(size_t)blockIdx.x * kGradOut + t] = v;
+  }
+}
+
+// narrow rows (d <= 16): one lane per row behind the bulk-copy ring of score_narrow_kernel
+template <typename T, int DP, bool EXACT>
+__global__ void __launch_bounds__(kSnThreads, DP >= 16 ? 1 : 2)   // 16 features: 3 x 16 doubles per lane need > 128 registers
+grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __restrict__ st, const float* __restrict__ y,
+                   const uint8_t* __restrict__ mask, int keep, double* __restrict__ part) {
+  using G = SnGeom<DP>;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const uint32_t sbase = smem_u32(smem_raw);
+  const uint32_t bar_full = sbase + G::kOffBar, bar_empty = bar_full + 8 * kSnStages;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool has_mask = mask != nullptr;
+  const uint32_t row_bytes = (uint32_t)d * sizeof(T);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kSnStages; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, kSnWarps);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  __shared__ double red[kSnWarps][kGradOut];
+  if (warp == kSnWarps) {
+    if (lane == 0) {
+      const uint32_t xb = (uint32_t)G::kRows * row_bytes;
+      const uint32_t tx = xb + G::kYStage + (has_mask ? G::kMStage : 0u);
+      int it = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+        const int s = it % kSnStages;
+        if (it >= kSnStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kSnStages - 1) & 1));
+        const uint32_t full = bar_full + 8 * s;
+        mbar_expect_tx(full, tx);
+        const int64_t row0 = (int64_t)tile * G::kRows;
+        bulk_load_1d(sbase + s * G::kXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * row_bytes, xb, full);
+        bulk_load_1d(sbase + G::kOffY + s * G::kYStage, y + row0, G::kYStage, full);
+        if (has_mask) bulk_load_1d(sbase + G::kOffM + s * G::kMStage, mask + row0, G::kMStage, full);
+      }
+    }
+  } else {
+    double cf[DP], mv[DP], acc[DP];
+#pragma unroll
+    for (int k = 0; k < DP; ++k) {
+      cf[k] = k < d ? st[kRfBeta + k] : 0.0;
+      mv[k] = k < d ? st[kRfMean + k] : 0.0;
+      acc[k] = 0.0;
+    }
+    const double b0 = st[kRfB0];
+    double acc1 = 0.0;
+    int s = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      mbar_wait(bar_full + 8 * s, phase);
+      const uint32_t xs = sbase + s * G::kXStage, ys = sbase + G::kOffY + s * G::kYStage, ms = sbase + G::kOffM + s * G::kMStage;
+#pragma unroll
+      for (int rr = 0; rr < G::RPT; ++rr) {
+        const int r = rr * kSnConsumers + threadIdx.x;
+        const bool use = !has_mask || ld_shared_u8(ms + (uint32_t)r) == (uint32_t)keep;
+        float x[DP];
+        if constexpr (EXACT) ld_vals_vec<T, DP>(xs + (uint32_t)r * row_bytes, x);
+        else ld_vals_any<T, DP>(xs + (uint32_t)r * row_bytes, 0, d, x);
+#pragma unroll
+        for (int k = 0; k < DP; ++k) x[k] = use ? x[k] : 0.f;
+        double a0 = 0.0, a1 = 0.0;
+#pragma unroll
+        for (int k = 0; k < DP; k += 2) {
+          a0 = fma((double)x[k] - mv[k], cf[k], a0);
+          if (k + 1 < DP) a1 = fma((double)x[k + 1] - mv[k + 1], cf[k + 1], a1);
+        }
+        const float yv = use ? ld_shared_f32(ys + 4u * (uint32_t)r) : 0.f;
+        const double e = use ? ((double)yv - b0) - (a0 + a1) : 0.0;
+#pragma unroll
+        for (int k = 0; k < DP; ++k) acc[k] = fma((double)x[k] - mv[k], e, acc[k]);
+        acc1 += e;
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+      if (++s == kSnStages) { s = 0; phase ^= 1u; }
+    }
+#pragma unroll
+    for (int k = 0; k <= DP; ++k) {
+      double v = k < DP ? acc[k] : acc1;
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) v += shfl_xor_d(v, o);
+      if (lane == 0) {
+        if (k < DP && k < d) red[warp][k] = v;
+        if (k == DP) red[warp][kMaxD] = v;
+      }
+    }
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
+    double v = 0.0;
+    if (t < d || t == kMaxD)
+      for (int w = 0; w < kSnWarps; ++w) v += red[w][t];
+    part[(size_t)blockIdx.x * kGradOut + t] = v;
+  }
+}
+
+// acc[kGradOut] (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites
+__global__ void grad_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
+  const int t = threadIdx.x;
+  if (t >= kGradOut) return;
+  double v = first ? 0.0 : acc[t];
+  int c = 0;
+  for (; c + 8 <= n_ctas; c += 8) {          // eight loads in flight, the adds in CTA order
+    double p[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) p[u] = part[(size_t)(c + u) * kGradOut + t];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v += p[u];
+  }
+  for (; c < n_ctas; ++c) v += part[(size_t)c * kGradOut + t];
+  acc[t] = v;
+}
+
 }  // namespace
 
 int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int64_t n, bool first) {
@@ -830,6 +1181,111 @@ int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int6
     return launch_score_direct(ctx, Xt, x_dtype, n - done, d, ldx, y != nullptr ? y + done : nullptr,
                                mask != nullptr ? mask + done : nullptr, keep, yhat != nullptr ? yhat + done : nullptr,
                                first_block);
+  }
+  return B2_OK;
+}
+
+// The residual gradient over the rows [0, n): the layout choice of launch_score (the labels are always present).  Every
+// gradient launch is followed by grad_reduce_kernel, which adds its CTA partials in order into ctx->refine + kRfGrad.
+static int grad_reduce(b2_ctx* ctx, int grid, bool first) {
+  B2_CUDA(cudaGetLastError());
+  grad_reduce_kernel<<<1, 160, 0, ctx->stream>>>(ctx->grad_part, grid, first ? 1 : 0, ctx->refine + kRfGrad);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  return B2_OK;
+}
+
+template <typename T, int DP>
+static int launch_grad_narrow_dp(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
+                                 bool first, int64_t* done) {
+  using G = SnGeom<DP>;
+  const int64_t n_tiles = n / G::kRows;
+  *done = 0;
+  if (n_tiles == 0 || n_tiles > 0x7fffffff) return B2_OK;
+  const int cap = ctx->sm_count * 2;
+  const int grid = (int)(n_tiles < cap ? n_tiles : cap);
+#define B2_LAUNCH_GN(EX)                                                                                                 \
+  do {                                                                                                                   \
+    B2_CUDA(cudaFuncSetAttribute(grad_narrow_kernel<T, DP, EX>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem)); \
+    grad_narrow_kernel<T, DP, EX><<<grid, kSnThreads, G::kSmem, ctx->stream>>>(X, (int)n_tiles, d, ctx->refine, y, mask, \
+                                                                               keep, ctx->grad_part);                    \
+  } while (0)
+  if (d == DP) B2_LAUNCH_GN(true); else B2_LAUNCH_GN(false);
+#undef B2_LAUNCH_GN
+  if (int r = grad_reduce(ctx, grid, first)) return r;
+  *done = n_tiles * G::kRows;
+  return B2_OK;
+}
+
+template <typename T>
+static int launch_grad_narrow(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
+                              bool first, int64_t* done) {
+  if (d <= 1) return launch_grad_narrow_dp<T, 1>(ctx, X, n, d, y, mask, keep, first, done);
+  if (d <= 2) return launch_grad_narrow_dp<T, 2>(ctx, X, n, d, y, mask, keep, first, done);
+  if (d <= 4) return launch_grad_narrow_dp<T, 4>(ctx, X, n, d, y, mask, keep, first, done);
+  if (d <= 8) return launch_grad_narrow_dp<T, 8>(ctx, X, n, d, y, mask, keep, first, done);
+  return launch_grad_narrow_dp<T, 16>(ctx, X, n, d, y, mask, keep, first, done);
+}
+
+int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                const uint8_t* mask, int keep, bool first_block) {
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool wide = ldx == d && d > 16 && d % 4 == 0 && (d * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(y) & 15) == 0;
+  const bool narrow = ldx == d && d <= 16 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
+                      (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
+                      (mask == nullptr || (reinterpret_cast<uintptr_t>(mask) & 15) == 0);
+  int64_t done = 0;
+  if (narrow) {
+    int rc;
+    if (x_dtype == B2_F32)
+      rc = launch_grad_narrow<float>(ctx, static_cast<const float*>(X), n, d, y, mask, keep, first_block, &done);
+    else
+      rc = launch_grad_narrow<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), n, d, y, mask, keep, first_block,
+                                             &done);
+    if (rc != B2_OK) return rc;
+    if (done > 0) first_block = false;
+  } else if (wide) {
+    const int lpr = d <= 32 ? 2 : (d <= 64 ? 4 : 8);
+    const int sweep_rows = kTmWarps * (32 / lpr);
+    int sweeps = (int)(kTmXStage / (uint32_t)(sweep_rows * d * es));
+    if (sweeps > kTmTileRowsMax / sweep_rows) sweeps = kTmTileRowsMax / sweep_rows;
+    const int tile_rows = sweeps * sweep_rows;
+    const int64_t n_tiles = n / tile_rows;
+    if (n_tiles > 0 && n_tiles <= 0x7fffffff) {
+      const int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
+#define B2_LAUNCH_GT(T, LPR)                                                                                          \
+  do {                                                                                                                \
+    B2_CUDA(cudaFuncSetAttribute(grad_tma_kernel<T, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmSmem));     \
+    grad_tma_kernel<T, LPR><<<grid, kTmThreads, kTmSmem, ctx->stream>>>(static_cast<const T*>(X), (int)n_tiles, sweeps, \
+                                                                        d, ctx->refine, y, mask, keep, ctx->grad_part); \
+  } while (0)
+#define B2_LAUNCH_GT_T(T) \
+  do { if (lpr == 2) B2_LAUNCH_GT(T, 2); else if (lpr == 4) B2_LAUNCH_GT(T, 4); else B2_LAUNCH_GT(T, 8); } while (0)
+      if (x_dtype == B2_F32) B2_LAUNCH_GT_T(float); else B2_LAUNCH_GT_T(__nv_bfloat16);
+#undef B2_LAUNCH_GT_T
+#undef B2_LAUNCH_GT
+      if (int r = grad_reduce(ctx, grid, first_block)) return r;
+      done = n_tiles * tile_rows;
+      first_block = false;
+    }
+  }
+  if (done < n || n == 0) {
+    const char* Xt = static_cast<const char*>(X) + (size_t)done * ldx * es;
+    const int64_t rows = n - done;
+    const int vec = (d % 4 == 0) && ((ldx * es) % (4 * es) == 0) && ((reinterpret_cast<uintptr_t>(Xt) % (4 * es)) == 0);
+    int64_t want = (rows + kScoreWarps * 4 - 1) / (kScoreWarps * 4);
+    if (want < 1) want = 1;
+    const int grid = (int)(want < ctx->score_ctas ? want : ctx->score_ctas);
+    const uint8_t* mt = mask != nullptr ? mask + done : nullptr;
+    if (x_dtype == B2_F32)
+      grad_kernel<float><<<grid, kScoreThreads, 0, ctx->stream>>>(reinterpret_cast<const float*>(Xt), rows, d, ldx,
+                                                                  ctx->refine, y + done, mt, keep, vec, ctx->grad_part);
+    else
+      grad_kernel<__nv_bfloat16><<<grid, kScoreThreads, 0, ctx->stream>>>(reinterpret_cast<const __nv_bfloat16*>(Xt), rows,
+                                                                          d, ldx, ctx->refine, y + done, mt, keep, vec,
+                                                                          ctx->grad_part);
+    return grad_reduce(ctx, grid, first_block);
   }
   return B2_OK;
 }

@@ -104,8 +104,15 @@ constexpr int kNB = 16;
 constexpr int kCholThreads = 512;
 constexpr int kUPitch = kNB + 1;
 
+// Refinement mode (REFINE, b2_fit_refined): the right-hand side is g - alpha beta from rf (ctx->refine) instead of r from S,
+// so the same factor of A + alpha I gives the correction dbeta; refine_update then moves the state.
+__device__ void refine_update(const double* S, int d, int fit_intercept, bool singular, const double* dbeta, double* misc,
+                              double* __restrict__ rf, double* __restrict__ out);
+
+template <bool REFINE>
 __global__ void __launch_bounds__(kCholThreads, 1)
-solve_cholesky_kernel(double* S, int d, double alpha, int fit_intercept, double* __restrict__ out, const SolveXchg xc) {
+solve_cholesky_kernel(double* S, int d, double alpha, int fit_intercept, double* __restrict__ out, const SolveXchg xc,
+                      double* __restrict__ rf) {
   extern __shared__ double sm[];
   const int pitch = d + 1;
   double* A = sm;                        // rows 0..d-1 = A, row d = r^T
@@ -148,6 +155,10 @@ solve_cholesky_kernel(double* S, int d, double alpha, int fit_intercept, double*
     __syncthreads();
   }
   build_normal_equations(S, d, alpha, fit_intercept, A, r, mean, &misc[0]);
+  if constexpr (REFINE) {
+    if (tid < d) r[tid] = rf[kRfGrad + tid] - alpha * rf[kRfBeta + tid];
+    __syncthreads();
+  }
   tm[0] = clock64() - tc0;
   if (warp == 0) {
     double mx = 0.0;
@@ -345,6 +356,10 @@ solve_cholesky_kernel(double* S, int d, double alpha, int fit_intercept, double*
     }
   }
   tm[4] = clock64() - tc0;
+  if constexpr (REFINE) {
+    refine_update(S, d, fit_intercept, singular, r, misc, rf, out);
+    return;
+  }
   if (tid == 0)
     for (int k = 0; k < 5; ++k) out[kOutSingular + k] = (double)tm[k];
   for (int i = tid; i < d; i += blockDim.x) out[i] = singular ? 0.0 : r[i];
@@ -356,6 +371,73 @@ solve_cholesky_kernel(double* S, int d, double alpha, int fit_intercept, double*
     if (lane == 0) {
       out[kOutIntercept] = singular ? 0.0 : misc[0] - part;
       out[kOutInfo] = misc[2];
+    }
+  }
+}
+
+// step = max_j |dbeta_j| sigma_j / sigma_y, sigma from S's centred diagonal.  A step above the last kept one means the last
+// kept correction left a larger error than it found (the next correction estimates what the previous one left), so the
+// state returns to before it and the pass reports the guard (out[kOutRefineGuard] = 1); so does a non-finite correction
+// or a failed factorisation.  Otherwise beta += dbeta, b0' += g_1 / n.  out: coef = beta, intercept = b0' - m.beta.
+__device__ void refine_update(const double* S, int d, int fit_intercept, bool singular, const double* dbeta, double* misc,
+                              double* __restrict__ rf, double* __restrict__ out) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int dp = d + 2;
+  const double n = __ldcg(S + d * dp + d);
+  if (warp == 0) {
+    double mx = 0.0;
+    bool finite = true;
+    for (int i = lane; i < d; i += 32) {
+      const double sx = __ldcg(S + i * dp + d);
+      const double c = __ldcg(S + i * dp + i) - sx * (sx / n);
+      mx = fmax(mx, fabs(dbeta[i]) * sqrt(fmax(c, 0.0)));
+      finite = finite && isfinite(dbeta[i]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    finite = __all_sync(0xffffffffu, finite) && isfinite(rf[kRfGrad + kMaxD]);
+    if (lane == 0) {
+      const double sy = __ldcg(S + d * dp + d + 1);
+      const double cy = __ldcg(S + (d + 1) * dp + d + 1) - sy * (sy / n);
+      const double sig = sqrt(fmax(cy, 0.0));
+      const double step = sig > 0.0 ? mx / sig : mx;
+      misc[3] = step;
+      misc[4] = (singular || !finite || !(step <= rf[kRfStep])) ? 1.0 : 0.0;
+    }
+  }
+  __syncthreads();
+  const bool guard = misc[4] != 0.0;
+  for (int i = tid; i < d; i += blockDim.x) {
+    const double b = rf[kRfBeta + i];
+    if (guard) {
+      rf[kRfBeta + i] = rf[kRfPrevBeta + i];
+    } else {
+      rf[kRfPrevBeta + i] = b;
+      rf[kRfBeta + i] = b + dbeta[i];
+    }
+  }
+  if (tid == 0) {
+    const double b0 = rf[kRfB0];
+    if (guard) {
+      rf[kRfB0] = rf[kRfPrevB0];
+    } else {
+      rf[kRfPrevB0] = b0;
+      rf[kRfB0] = fit_intercept ? b0 + rf[kRfGrad + kMaxD] / n : b0;
+      rf[kRfStep] = misc[3];
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < d; i += blockDim.x) out[i] = rf[kRfBeta + i];
+  if (warp == 0) {
+    double part = 0.0;
+    for (int i = lane; i < d; i += 32) part += rf[kRfMean + i] * rf[kRfBeta + i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if (lane == 0) {
+      out[kOutIntercept] = rf[kRfB0] - part;
+      out[kOutInfo] = misc[2];
+      out[kOutRefineStep] = misc[3];
+      out[kOutRefineGuard] = misc[4];
     }
   }
 }
@@ -757,7 +839,8 @@ size_t solve_smem_bytes(int d) {
 int ensure_solve_attrs(b2_ctx* ctx) {
   if (!ctx->solve_attr_set) {
     const int bytes = (int)solve_smem_bytes(kMaxD);
-    B2_CUDA(cudaFuncSetAttribute(solve_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B2_CUDA(cudaFuncSetAttribute(solve_cholesky_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B2_CUDA(cudaFuncSetAttribute(solve_cholesky_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B2_CUDA(cudaFuncSetAttribute(solve_spectral_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B2_CUDA(cudaFuncSetAttribute(solve_eigvals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     ctx->solve_attr_set = true;
@@ -776,8 +859,24 @@ int launch_solve_cholesky(b2_ctx* ctx, double alpha, int fit_intercept, unsigned
   xc.n_ranks = ctx->n_ranks;
   xc.epoch = gather_epoch;
   xc.timeout_ns = ctx->xchg_timeout_ns;
-  solve_cholesky_kernel<<<1, kCholThreads, solve_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, alpha, fit_intercept,
-                                                                                    ctx->solve_host, xc);
+  solve_cholesky_kernel<false><<<1, kCholThreads, solve_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, alpha,
+                                                                                           fit_intercept, ctx->solve_host,
+                                                                                           xc, nullptr);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_solve_refine(b2_ctx* ctx, double alpha, int fit_intercept) {
+  if (int r = ensure_solve_attrs(ctx)) return r;
+  SolveXchg xc;
+  xc.own = nullptr;
+  xc.n_ranks = 1;
+  xc.epoch = 0;
+  xc.timeout_ns = 0;
+  solve_cholesky_kernel<true><<<1, kCholThreads, solve_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, alpha,
+                                                                                          fit_intercept, ctx->solve_host,
+                                                                                          xc, ctx->refine);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return B2_OK;

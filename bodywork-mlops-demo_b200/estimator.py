@@ -12,6 +12,7 @@ joblib importable, calls ``.predict`` and ``str(model)`` -- a custom class could
 """
 from __future__ import annotations
 
+import warnings
 from typing import Optional
 
 import numpy as np
@@ -28,6 +29,7 @@ def default_context() -> native.Context:
     return _shared_ctx
 
 
+_REFINE_TOL = 1e-10             # the refined fit's step tolerance (max_j |dcoef_j| sigma_j / sigma_y)
 _F64_UPLOAD_LIMIT = 64 << 30     # float64 host rows larger than this (as fp32, bytes) are converted and streamed block-wise
 
 
@@ -49,10 +51,13 @@ class B200LinearRegression:
     other's rows."""
 
     def __init__(self, *, fit_intercept: bool = True, alpha: float = 0.0, tol: float = 1e-6,
-                 ctx: Optional[native.Context] = None):
+                 ctx: Optional[native.Context] = None, refine: int = 0):
         self.fit_intercept = fit_intercept
         self.alpha = float(alpha)
         self.tol = tol
+        # refine > 0: fit() adds up to `refine` residual passes over the same rows (b2_fit_refined), which take the
+        # tensor-core fit to the fp64 least-squares solution on correlated features; 0 keeps the plain fit
+        self.refine = int(refine)
         self._ctx = ctx
         self._S: Optional[np.ndarray] = None     # this estimator's statistic (set by partial_fit / deferred attributes)
         self._serial = -1                        # ctx.serial right after this estimator's last fit
@@ -123,7 +128,18 @@ class B200LinearRegression:
         self._drop_spectrum()
         singular = False
         try:
-            coef, b0 = ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
+            if self.refine > 0:
+                self.n_refine_passes_, self.refine_step_ = 0, 0.0      # the min-norm fallback below stays unrefined
+                coef, b0, passes, step = ctx.fit_refined(X, y, row_mask, mask_keep, alpha=self.alpha,
+                                                         fit_intercept=self.fit_intercept, max_passes=self.refine,
+                                                         tol=_REFINE_TOL)
+                self.n_refine_passes_, self.refine_step_ = passes, step
+                if step > _REFINE_TOL:
+                    warnings.warn(f"refined fit stopped at step {step:.3e} after {passes} kept correction(s) "
+                                  f"(tolerance {_REFINE_TOL:.0e}): more passes may help, or the features are too "
+                                  "ill-conditioned for the Gram path's precision", RuntimeWarning, stacklevel=2)
+            else:
+                coef, b0 = ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
             self._set_solution(coef, b0, d)
         except np.linalg.LinAlgError:
             singular = True         # rank deficient and alpha == 0: the minimum-norm solution gelsd would return
@@ -135,8 +151,14 @@ class B200LinearRegression:
             self._spectrum(d, need_coef=singular)
         return self
 
+    def _no_refine(self, what: str) -> None:
+        if self.refine > 0:
+            raise ValueError(f"{what} solves from a statistic and has no rows to re-read: refine must be 0 "
+                             f"(got refine={self.refine})")
+
     def partial_fit(self, X, y, with_spectrum: bool = False) -> "B200LinearRegression":
         """Fold one more tranche into THIS estimator's running statistic and re-solve (incremental daily refit)."""
+        self._no_refine("partial_fit")
         ctx = self.ctx
         Xh = X if isinstance(X, native.DeviceArray) else _as_f32_matrix(X)
         d = Xh.shape[1]
@@ -165,6 +187,7 @@ class B200LinearRegression:
     def solve_resident(self, d: int, S: Optional[np.ndarray] = None) -> "B200LinearRegression":
         """Solve from the statistic currently resident in the context (after gram_import / gram_accumulate calls made
         by the caller, e.g. IncrementalTrainer); ``S``: the caller's host copy of it, kept for deferred attributes."""
+        self._no_refine("solve_resident")
         ctx = self.ctx
         self._drop_spectrum()
         self._S = S
@@ -216,4 +239,5 @@ class B200LinearRegression:
         return reg
 
     def __repr__(self) -> str:
-        return "B200LinearRegression()" if self.alpha == 0.0 else f"B200LinearRegression(alpha={self.alpha})"
+        args = ([f"alpha={self.alpha}"] if self.alpha != 0.0 else []) + ([f"refine={self.refine}"] if self.refine else [])
+        return f"B200LinearRegression({', '.join(args)})"

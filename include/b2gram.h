@@ -143,7 +143,18 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
            int mem_kind, const uint8_t* row_mask, int mask_keep, double alpha, int fit_intercept,
            double* coef, double* intercept);
 
-/* ---- solve: replaces scipy.linalg.lstsq + _set_intercept ----------------------------------------
+/* b2_fit, then up to max_passes (0..16) residual passes over the same rows (see DESIGN section 2).  Each pass streams
+ * the rows once for the fp64 gradient g = [X-m 1]^T (y - yhat) of the current solution and corrects it through the
+ * factor of the approximate Gram, which takes a tensor-core fit to the fp64 least-squares solution of the stored rows.
+ * tol >= 0: stop when the scale-free step max_j |dcoef_j| sigma_j / sigma_y <= tol.  A step larger than the one before
+ * stops the passes and returns the state before the last kept correction.  passes_out: corrections kept; step_out: the
+ * last step (0 when max_passes == 0).  max_passes == 0 is bit-identical to b2_fit.  S afterwards is b2_fit's S.
+ * B2_E_UNSUPPORTED with more than one rank; B2_E_SINGULAR as b2_fit. */
+int b2_fit_refined(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                   int mem_kind, const uint8_t* row_mask, int mask_keep, double alpha, int fit_intercept,
+                   int max_passes, double tol, double* coef, double* intercept, int* passes_out, double* step_out);
+
+/* ---- solve:replaces scipy.linalg.lstsq + _set_intercept ----------------------------------------
  * reference: sklearn/linear_model/_base.py (lstsq on centred data; intercept_ = y_mean - x_mean.coef_)
  * Single-SM fp64 LDL^T (square-root-free Cholesky) of (Xc^T Xc + alpha I).  coef: d doubles, intercept: 1 double
  * (host).  fit_intercept = 0 solves the uncentred problem.  Returns B2_E_SINGULAR on a non-positive pivot and
