@@ -351,7 +351,7 @@ static int ctx_allocate(b2_ctx* ctx) {
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_red), sizeof(double) * (kTcAccElems + 16)));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->shift), gram_shift_bytes()));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->simt_part), sizeof(double) * (size_t)ctx->simt_ctas * kMaxS * kMaxS));
-  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->score_part), sizeof(double) * ((size_t)ctx->score_ctas + 2) * 10));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->score_part), sizeof(double) * ((size_t)ctx->score_ctas + 2) * kNStats));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->coef_dev), sizeof(double) * (kMaxD + 1)));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->grad_part), sizeof(double) * (size_t)ctx->score_ctas * kGradOut));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->refine), sizeof(double) * kRfDoubles));
@@ -878,9 +878,9 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
     B2_CUDA(cudaMemcpyAsync(ctx->coef_dev, cbuf, sizeof(double) * (kMaxD + 1), cudaMemcpyHostToDevice, ctx->stream));
     B2_CUDA(cudaEventRecord(ctx->ev_coef[slot], ctx->stream));
   }
-  double* acc = ctx->score_part + (size_t)ctx->score_ctas * 10;
+  double* acc = score_totals(ctx);
   if (n_rows == 0) {
-    B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 10, ctx->stream));
+    B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * kNStats, ctx->stream));
   } else if (mem_kind == B2_MEM_DEVICE) {
     if (int r = launch_score(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, yhat, true)) return r;
   } else {
@@ -919,7 +919,7 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
     B2_CUDA(done);
   }
   if (stats_out != nullptr && y != nullptr) {
-    B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * 10, cudaMemcpyDeviceToHost, ctx->stream));
+    B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * kNStats, cudaMemcpyDeviceToHost, ctx->stream));
     B2_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   return B2_OK;
@@ -934,17 +934,17 @@ int b2_score_allreduce(b2_ctx* ctx, double* stats) {
   }
   NcclApi* api = nccl();
   if (api == nullptr) { set_error("libnccl.so.2 could not be loaded"); return B2_E_COMM; }
-  double* acc = ctx->score_part + (size_t)ctx->score_ctas * 10;   // 10 sums
-  double* mx = acc + 10;                                          // 2 maxima
+  double* acc = score_totals(ctx);   // kNStats sums
+  double* mx = acc + kNStats;         // 2 maxima
   B2_CUDA(cudaStreamSynchronize(ctx->stream));   // the previous b2_score may still be reading its totals
-  double host[10], hmax[2];
+  double host[kNStats], hmax[2];
   memcpy(host, stats, sizeof(host));
   hmax[0] = host[4]; hmax[1] = host[9];
   host[4] = 0.0; host[9] = 0.0;
   B2_CUDA(cudaMemcpyAsync(acc, host, sizeof(host), cudaMemcpyHostToDevice, ctx->stream));
   B2_CUDA(cudaMemcpyAsync(mx, hmax, sizeof(hmax), cudaMemcpyHostToDevice, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));   // host / hmax live on this stack frame
-  B2_NCCL(api, api->AllReduce(acc, acc, 10, kNcclFloat64, kNcclSum, ctx->comm, ctx->stream));
+  B2_NCCL(api, api->AllReduce(acc, acc, kNStats, kNcclFloat64, kNcclSum, ctx->comm, ctx->stream));
   B2_NCCL(api, api->AllReduce(mx, mx, 2, kNcclFloat64, kNcclMax, ctx->comm, ctx->stream));
   B2_CUDA(cudaMemcpyAsync(host, acc, sizeof(host), cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaMemcpyAsync(hmax, mx, sizeof(hmax), cudaMemcpyDeviceToHost, ctx->stream));
@@ -994,10 +994,10 @@ int b2_metrics(b2_ctx* ctx, const void* y_actual, const void* y_predicted, int d
     return B2_E_ARG;
   }
   if (mem_kind != B2_MEM_DEVICE && mem_kind != B2_MEM_HOST) { set_error("bad mem_kind %d", mem_kind); return B2_E_ARG; }
-  double* acc = ctx->score_part + (size_t)ctx->score_ctas * 10;
+  double* acc = score_totals(ctx);
   const size_t es = dtype == B2_F32 ? 4 : 8;
   if (n_rows == 0) {
-    B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 10, ctx->stream));
+    B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * kNStats, ctx->stream));
   } else if (mem_kind == B2_MEM_DEVICE) {
     if (int r = launch_metrics(ctx, y_actual, y_predicted, dtype, n_rows, true)) return r;
   } else {
@@ -1022,7 +1022,7 @@ int b2_metrics(b2_ctx* ctx, const void* y_actual, const void* y_predicted, int d
             }))
       return r;
   }
-  B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * 10, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * kNStats, cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
 }

@@ -1,10 +1,13 @@
 // b2_internal.cuh -- shared declarations of libb2gram.so (not part of the public C-ABI).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "../../include/b2gram.h"
 
@@ -26,7 +29,9 @@ constexpr int kTcAccCols = 2 * kTcN;     // two accumulators: A = hi and A = lo 
 constexpr int kTcAccElems = kTcM * kTcAccCols;  // fp32 accumulators drained per chunk (36 864)
 constexpr int kTcSideDoubles = 8;        // per-CTA CUDA-core sums: sum y', sum y'^2, rows used
 
-// ---- refined fit (b2_fit_refined): the model y = b0' + (x - m).beta and its residual passes -----------------------
+// ---- scoring (b2_score, b2_metrics) and the refined fit (b2_fit_refined) ---------------------------------------------
+constexpr int kNStats = 10;              // include/b2gram.h: b2_score stats_out layout (maxima at 4 and 9, sums elsewhere)
+// the refined fit's model y = b0' + (x - m).beta and its residual passes
 constexpr int kGradOut = kMaxD + 1;      // one gradient: g_j = sum (x_j - m_j) e at j < kMaxD, g_1 = sum e at kMaxD
 // doubles of ctx->refine
 constexpr int kRfBeta = 0;               // beta
@@ -40,6 +45,9 @@ constexpr int kRfDoubles = kRfGrad + kGradOut;
 // solve_out / solve_host slots of the refinement solve (beside coef [0, d), intercept kMaxD, info kMaxD + 1)
 constexpr int kOutRefineStep = 2 * kMaxD + 3;
 constexpr int kOutRefineGuard = 2 * kMaxD + 4;
+
+// template width of the one-lane-per-row kernels (gram_narrow.cu, score.cu) for d <= 16 features: the next power of two
+inline int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
 
 void set_error(const char* fmt, ...);
 
@@ -91,7 +99,7 @@ struct b2_ctx {
   double* simt_part = nullptr;         // [simt_ctas][kMaxS*kMaxS]
   int simt_ctas = 0;
   // scoring scratch
-  double* score_part = nullptr;        // [score_ctas][6]
+  double* score_part = nullptr;        // [score_ctas + 2][kNStats]: per-CTA partials, running totals (b2::score_totals)
   int score_ctas = 0;
   double* coef_dev = nullptr;          // [kMaxD + 1]
   // refined fit scratch
@@ -136,6 +144,34 @@ struct b2_ctx {
 };
 
 namespace b2 {
+
+// the kNStats running totals of the current b2_score / b2_metrics call (behind the per-CTA partials; b2_score_allreduce
+// keeps its two maxima in the kNStats doubles after them)
+inline double* score_totals(const b2_ctx* ctx) { return ctx->score_part + (size_t)ctx->score_ctas * kNStats; }
+
+// ---- launch helpers of the ring kernels (score.cu, gram_narrow.cu) ----------------------------------------------------
+// One launch with `smem` bytes of dynamic shared memory; the attribute is set before every launch.
+template <typename... P, typename... A>
+int launch_smem(void (*kernel)(P...), int grid, int threads, uint32_t smem, cudaStream_t stream, A... args) {
+  B2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  kernel<<<grid, threads, smem, stream>>>(args...);
+  B2_CUDA(cudaGetLastError());
+  return B2_OK;
+}
+// f(std::integral_constant<int, V>{}) for the first V of Vs equal to v, the last V when none is
+template <int V, int... Vs, typename F>
+int with_int(int v, F&& f) {
+  if constexpr (sizeof...(Vs) == 0) return f(std::integral_constant<int, V>{});
+  else return v == V ? f(std::integral_constant<int, V>{}) : with_int<Vs...>(v, f);
+}
+// f(X as const float* or const __nv_bfloat16*)
+template <typename F>
+int with_rows(int x_dtype, const void* X, F&& f) {
+  if (x_dtype == B2_F32) return f(static_cast<const float*>(X));
+  return f(static_cast<const __nv_bfloat16*>(X));
+}
+template <typename P>
+using row_t = std::remove_const_t<std::remove_pointer_t<P>>;
 
 // ---- kernel launchers (each enqueues on ctx->stream and bumps ctx->launches) -----------------
 // The Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites

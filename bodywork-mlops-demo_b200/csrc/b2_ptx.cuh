@@ -1,4 +1,6 @@
-// b2_ptx.cuh -- PTX wrappers shared by the TMA / mbarrier pipelines (gram_tc.cu, gram_narrow.cu).
+// b2_ptx.cuh -- PTX wrappers shared by the TMA / mbarrier pipelines (gram_tc.cu, gram_narrow.cu, score.cu), and the
+// bulk-copy ring (ring_init, ring_produce) of the streaming kernels gram_narrow_kernel, score_tma_kernel,
+// score_narrow_kernel, grad_tma_kernel and grad_narrow_kernel.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -156,6 +158,43 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar), "l"(0x12F0000000000000ull)
       : "memory");
+}
+
+// ---- the bulk-copy ring: STAGES slots in shared memory, each with a full barrier (the producer's arrive plus the copied
+// bytes) at bar_full + 8 s and an empty barrier (one arrive per consumer warp) at bar_empty + 8 s ------------------------
+template <int STAGES>
+__device__ __forceinline__ void ring_init(uint32_t bar_full, uint32_t bar_empty, uint32_t consumer_warps) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, consumer_warps);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+}
+
+// The loop of the one producer lane: tiles blockIdx.x, + gridDim.x, ... < n_tiles of tile_rows rows each.  Tile `it`
+// goes to slot s = it % STAGES once the consumers have released it: tile_rows * row_bytes bytes of X at xs + s * x_stride,
+// with has_y tile_rows floats of y at ys + s * y_stride, with has_mask tile_rows mask bytes at ms + s * m_stride.
+template <int STAGES>
+__device__ __forceinline__ void ring_produce(uint32_t bar_full, uint32_t bar_empty, int n_tiles, int tile_rows,
+                                             const void* X, uint32_t row_bytes, uint32_t xs, uint32_t x_stride,
+                                             bool has_y, const float* y, uint32_t ys, uint32_t y_stride,
+                                             bool has_mask, const uint8_t* mask, uint32_t ms, uint32_t m_stride) {
+  const uint32_t xb = (uint32_t)tile_rows * row_bytes, yb = (uint32_t)tile_rows * 4u, mb = (uint32_t)tile_rows;
+  const uint32_t tx = xb + (has_y ? yb : 0u) + (has_mask ? mb : 0u);
+  int it = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    const int s = it % STAGES;
+    if (it >= STAGES) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / STAGES - 1) & 1));
+    const uint32_t full = bar_full + 8 * s;
+    mbar_expect_tx(full, tx);
+    const int64_t row0 = (int64_t)tile * tile_rows;
+    bulk_load_1d(xs + s * x_stride, reinterpret_cast<const char*>(X) + (size_t)row0 * row_bytes, xb, full);
+    if (has_y) bulk_load_1d(ys + s * y_stride, y + row0, yb, full);
+    if (has_mask) bulk_load_1d(ms + s * m_stride, mask + row0, mb, full);
+  }
 }
 
 }  // namespace b2

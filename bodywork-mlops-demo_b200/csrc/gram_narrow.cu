@@ -112,33 +112,14 @@ gram_narrow_kernel(const T* __restrict__ X, const float* __restrict__ y, const u
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool has_mask = mask != nullptr;
   const uint32_t row_bytes = (uint32_t)d * sizeof(T);
-  const uint32_t x_bytes = (uint32_t)G::kRows * row_bytes;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kNwStages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, G::kConsumerWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init<kNwStages>(bar_full, bar_empty, G::kConsumerWarps);
 
   if (warp == G::kConsumerWarps) {
     // ---- producer: one elected lane feeds the ring ----
-    if (lane == 0) {
-      const uint32_t tx = x_bytes + G::kYStage + (has_mask ? G::kMStage : 0u);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int s = it % kNwStages;
-        if (it >= kNwStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kNwStages - 1) & 1));
-        const uint32_t full = bar_full + 8 * s;
-        mbar_expect_tx(full, tx);
-        const int64_t row0 = (int64_t)tile * G::kRows;
-        bulk_load_1d(sbase + s * G::kXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * row_bytes, x_bytes, full);
-        bulk_load_1d(sbase + G::kOffY + s * G::kYStage, y + row0, G::kYStage, full);
-        if (has_mask) bulk_load_1d(sbase + G::kOffM + s * G::kMStage, mask + row0, G::kMStage, full);
-      }
-    }
+    if (lane == 0)
+      ring_produce<kNwStages>(bar_full, bar_empty, n_tiles, G::kRows, X, row_bytes, sbase, G::kXStage, true, y,
+                              sbase + G::kOffY, G::kYStage, has_mask, mask, sbase + G::kOffM, G::kMStage);
     return;
   }
 
@@ -395,64 +376,8 @@ narrow_fold_kernel(const double* __restrict__ part, int n_ctas, int DP, int d, c
   }
 }
 
-template <typename T, int DP>
-int launch_narrow_dp(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask, int keep, int n_tiles, int d,
-                     int* grid_out) {
-  using G = NwGeom<DP>;
-  const int mode = d == DP ? 2 : ((d * (int)sizeof(T)) % 16 == 0 ? 1 : 0);
-  const int cap = ctx->sm_count * G::kMinBlocks;
-  const int grid = n_tiles < cap ? n_tiles : cap;
-  *grid_out = grid;
-#define B2_LAUNCH_NW(MODE)                                                                                          \
-  do {                                                                                                              \
-    B2_CUDA(cudaFuncSetAttribute(gram_narrow_kernel<T, DP, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
-                                 G::kSmem));                                                                        \
-    gram_narrow_kernel<T, DP, MODE><<<grid, G::kThreads, G::kSmem, ctx->stream>>>(X, y, mask, keep, n_tiles, d,     \
-                                                                                  ctx->shift, ctx->simt_part);      \
-  } while (0)
-  if (mode == 2) {
-    B2_LAUNCH_NW(2);
-  } else if (mode == 1) {
-    if constexpr (DP == 16 && sizeof(T) == 4) B2_LAUNCH_NW(1);   // fp32 d = 12 is the only such shape
-    else B2_LAUNCH_NW(0);
-  } else {
-    B2_LAUNCH_NW(0);
-  }
-#undef B2_LAUNCH_NW
-  B2_CUDA(cudaGetLastError());
-  return B2_OK;
-}
-
-int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
-
 int narrow_tile_rows(int DP) {
-  return DP == 1 ? NwGeom<1>::kRows : DP == 2 ? NwGeom<2>::kRows : DP == 4 ? NwGeom<4>::kRows
-       : DP == 8 ? NwGeom<8>::kRows : NwGeom<16>::kRows;
-}
-
-// the full tiles of the first gram_narrow_main_rows(n, d) rows
-template <typename T>
-int launch_narrow_t(b2_ctx* ctx, const T* X, const float* y, const uint8_t* mask, int keep, int64_t n, int d,
-                    bool assign) {
-  const int DP = narrow_dp(d);
-  const int n_tiles = (int)(n / narrow_tile_rows(DP));   // n <= INT32_MAX rows (gram_narrow_supported)
-  const int pair = ctx->k_pairs % kKernelEventPairs;
-  B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
-  int grid = 0, rc = B2_OK;
-  switch (DP) {
-    case 1: rc = launch_narrow_dp<T, 1>(ctx, X, y, mask, keep, n_tiles, d, &grid); break;
-    case 2: rc = launch_narrow_dp<T, 2>(ctx, X, y, mask, keep, n_tiles, d, &grid); break;
-    case 4: rc = launch_narrow_dp<T, 4>(ctx, X, y, mask, keep, n_tiles, d, &grid); break;
-    case 8: rc = launch_narrow_dp<T, 8>(ctx, X, y, mask, keep, n_tiles, d, &grid); break;
-    default: rc = launch_narrow_dp<T, 16>(ctx, X, y, mask, keep, n_tiles, d, &grid); break;
-  }
-  if (rc != B2_OK) return rc;
-  B2_CUDA(cudaEventRecord(ctx->ev_k[pair][1], ctx->stream));
-  ctx->k_pairs += 1;
-  narrow_fold_kernel<<<1, 384, 0, ctx->stream>>>(ctx->simt_part, grid, DP, d, ctx->shift, assign ? 1 : 0, ctx->S);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
+  return with_int<1, 2, 4, 8, 16>(DP, [](auto V) { return NwGeom<decltype(V)::value>::kRows; });
 }
 
 }  // namespace
@@ -470,12 +395,39 @@ bool gram_narrow_supported(const void* X, int x_dtype, const float* y, int64_t n
 // Full kRows tiles only: the < kRows rows left over take the fp64 kernel
 int64_t gram_narrow_main_rows(int64_t n, int d) { return n - n % narrow_tile_rows(narrow_dp(d)); }
 
+// the full tiles of the first gram_narrow_main_rows(n, d) rows
 int launch_gram_narrow(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n, int d,
                        const uint8_t* mask, int keep, bool assign) {
   static_assert(2 * kNwMM <= kMaxS * kMaxS, "two CTAs per SM of partials fit the CUDA-core scratch (simt_part)");
-  if (x_dtype == B2_F32)
-    return launch_narrow_t<float>(ctx, static_cast<const float*>(X), y, mask, keep, n, d, assign);
-  return launch_narrow_t<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), y, mask, keep, n, d, assign);
+  const int DP = narrow_dp(d);
+  const int n_tiles = (int)(n / narrow_tile_rows(DP));   // n <= INT32_MAX rows (gram_narrow_supported)
+  const int pair = ctx->k_pairs % kKernelEventPairs;
+  B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
+  int grid = 0;
+  const int rc = with_rows(x_dtype, X, [&](auto* Xr) {
+    using T = row_t<decltype(Xr)>;
+    return with_int<1, 2, 4, 8, 16>(DP, [&](auto V) {
+      constexpr int kDP = decltype(V)::value;
+      using G = NwGeom<kDP>;
+      // MODE 2: d == DP; MODE 1: a row pitch of whole 16-byte vectors, which only fp32 d = 12 has; MODE 0: the rest
+      auto kernel = gram_narrow_kernel<T, kDP, 0>;
+      if (d == kDP) kernel = gram_narrow_kernel<T, kDP, 2>;
+      else if constexpr (kDP == 16 && sizeof(T) == 4) {
+        if ((d * 4) % 16 == 0) kernel = gram_narrow_kernel<T, kDP, 1>;
+      }
+      const int cap = ctx->sm_count * G::kMinBlocks;
+      grid = n_tiles < cap ? n_tiles : cap;
+      return launch_smem(kernel, grid, G::kThreads, G::kSmem, ctx->stream, Xr, y, mask, keep, n_tiles, d,
+                         ctx->shift, ctx->simt_part);
+    });
+  });
+  if (rc != B2_OK) return rc;
+  B2_CUDA(cudaEventRecord(ctx->ev_k[pair][1], ctx->stream));
+  ctx->k_pairs += 1;
+  narrow_fold_kernel<<<1, 384, 0, ctx->stream>>>(ctx->simt_part, grid, DP, d, ctx->shift, assign ? 1 : 0, ctx->S);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  return B2_OK;
 }
 
 }  // namespace b2

@@ -20,7 +20,6 @@ constexpr int kScoreThreads = 256;
 constexpr int kScoreWarps = kScoreThreads / 32;
 constexpr double kEpsF64 = 2.220446049250313e-16;
 
-constexpr int kNStats = 10;   // include/b2gram.h: b2_score stats_out layout
 // The per-row statistics are the fp64-pipe cost of scoring (they bind the narrow-row and bf16 kernels), so they are kept
 // to 13 fp64 instructions: one residual, one reciprocal refined by a single Newton step from the fp32 seed (the seed is
 // good to 2^-23, one step gives 2^-46 = 1.4e-14 relative -- the parity bar is 1e-12), fused multiply-adds for the four
@@ -92,8 +91,54 @@ struct RowStats {
     sp += p; spp = fma(p, p, spp); syp = fma(y, p, syp);
     mxape = fmax(mxape, e / ay);
   }
+  // in the stats_out order of include/b2gram.h
+  __device__ __forceinline__ void values(double (&v)[kNStats]) const {
+    v[0] = ape; v[1] = sse; v[2] = sy; v[3] = syy; v[4] = mx; v[5] = cnt(); v[6] = sp; v[7] = spp; v[8] = syp; v[9] = mxape;
+  }
 };
 __device__ __forceinline__ bool stat_is_max(int k) { return k == 4 || k == 9; }
+__device__ __forceinline__ double shfl_xor_d(double v, int m) { return __shfl_xor_sync(0xffffffffu, v, m); }
+
+// ---- the CTA reductions: statistics combined across lanes 16, 8, ..., LAST of a warp, then one warp's values in
+// red[warp] (lane 0 stores), then the NW warps in order into part[blockIdx.x]; the gradient sums likewise ---------------
+template <int LAST>
+__device__ __forceinline__ void stats_butterfly(double (&v)[kNStats]) {
+#pragma unroll
+  for (int k = 0; k < kNStats; ++k) {
+#pragma unroll
+    for (int o = 16; o >= LAST; o >>= 1) {
+      const double other = shfl_xor_d(v[k], o);
+      v[k] = stat_is_max(k) ? fmax(v[k], other) : v[k] + other;
+    }
+  }
+}
+__device__ __forceinline__ void stats_store(double (*red)[kNStats], int warp, int lane, const double (&v)[kNStats]) {
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < kNStats; ++k) red[warp][k] = v[k];
+  }
+}
+template <int NW>
+__device__ __forceinline__ void stats_fold(const double (*red)[kNStats], double* __restrict__ part) {
+  __syncthreads();
+  if (threadIdx.x < kNStats) {
+    const int k = threadIdx.x;
+    double acc = 0.0;
+    for (int w = 0; w < NW; ++w) acc = stat_is_max(k) ? fmax(acc, red[w][k]) : acc + red[w][k];
+    part[(size_t)blockIdx.x * kNStats + k] = acc;
+  }
+}
+// red[w] holds warp w's gradient sums at the features < d and at kMaxD (g_1); every other entry of the partial is zero
+template <int NW>
+__device__ __forceinline__ void grad_fold(const double (*red)[kGradOut], int d, double* __restrict__ part) {
+  __syncthreads();
+  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
+    double v = 0.0;
+    if (t < d || t == kMaxD)
+      for (int w = 0; w < NW; ++w) v += red[w][t];
+    part[(size_t)blockIdx.x * kGradOut + t] = v;
+  }
+}
 
 template <typename T>
 __device__ __forceinline__ double lane_dot(const T* __restrict__ row, int d, int lane, const double* cf, bool vec);
@@ -187,17 +232,10 @@ score_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const doubl
     }
   }
   __shared__ double red[kScoreWarps][kNStats];
-  if (lane == 0) {
-    red[warp][0] = st.ape; red[warp][1] = st.sse; red[warp][2] = st.sy;  red[warp][3] = st.syy; red[warp][4] = st.mx;
-    red[warp][5] = st.cnt(); red[warp][6] = st.sp;  red[warp][7] = st.spp; red[warp][8] = st.syp; red[warp][9] = st.mxape;
-  }
-  __syncthreads();
-  if (threadIdx.x < kNStats) {
-    const int k = threadIdx.x;
-    double v = 0.0;
-    for (int w = 0; w < kScoreWarps; ++w) v = stat_is_max(k) ? fmax(v, red[w][k]) : v + red[w][k];
-    part[(size_t)blockIdx.x * kNStats + k] = v;
-  }
+  double v[kNStats];
+  st.values(v);
+  stats_store(red, warp, lane, v);
+  stats_fold<kScoreWarps>(red, part);
 }
 
 // ---- fast path (d % 4 == 0, 16-byte aligned rows): 4 rows per warp iteration, 32 warps per SM ---------------
@@ -232,8 +270,6 @@ __device__ __forceinline__ void load_row4<__nv_bfloat16>(const __nv_bfloat16* __
   x[0] = __uint_as_float(u0 << 16); x[1] = __uint_as_float(u0 & 0xffff0000u);
   x[2] = __uint_as_float(u1 << 16); x[3] = __uint_as_float(u1 & 0xffff0000u);
 }
-
-__device__ __forceinline__ double shfl_xor_d(double v, int m) { return __shfl_xor_sync(0xffffffffu, v, m); }
 
 constexpr int kRowsPerIter = 4;
 
@@ -304,27 +340,12 @@ score_kernel_rows8(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
     }
   }
   // block reduce: first across the 4 row-owning lanes of each warp (lanes 0, 8, 16, 24), then across warps
-  double v[kNStats] = {st.ape, st.sse, st.sy, st.syy, st.mx, st.cnt(), st.sp, st.spp, st.syp, st.mxape};
-#pragma unroll
-  for (int k = 0; k < kNStats; ++k) {
-#pragma unroll
-    for (int o = 16; o >= 8; o >>= 1) {
-      const double other = shfl_xor_d(v[k], o);
-      v[k] = stat_is_max(k) ? fmax(v[k], other) : v[k] + other;
-    }
-  }
+  double v[kNStats];
+  st.values(v);
+  stats_butterfly<8>(v);
   __shared__ double red[kScoreWarps][kNStats];
-  if (lane == 0) {
-#pragma unroll
-    for (int k = 0; k < kNStats; ++k) red[warp][k] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x < kNStats) {
-    const int k = threadIdx.x;
-    double acc = 0.0;
-    for (int w = 0; w < kScoreWarps; ++w) acc = stat_is_max(k) ? fmax(acc, red[w][k]) : acc + red[w][k];
-    part[(size_t)blockIdx.x * kNStats + k] = acc;
-  }
+  stats_store(red, warp, lane, v);
+  stats_fold<kScoreWarps>(red, part);
 }
 
 // ---- streaming path (wide contiguous rows): TMA bulk copies -> smem ring -> the same 4-rows-per-warp arithmetic -------
@@ -383,31 +404,13 @@ score_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const 
   const int tile_rows = sweeps * kSweepRows;
   const uint32_t pitch = (uint32_t)d * sizeof(T);
   const bool has_mask = mask != nullptr, has_y = y != nullptr;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kTmStages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, kTmWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init<kTmStages>(bar_full, bar_empty, kTmWarps);
 
   __shared__ double red[kTmWarps][kNStats];
   if (warp == kTmWarps) {
-    if (lane == 0) {
-      const uint32_t xb = (uint32_t)tile_rows * pitch, yb = (uint32_t)tile_rows * 4u;
-      const uint32_t tx = xb + (has_y ? yb : 0u);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int s = it % kTmStages;
-        if (it >= kTmStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kTmStages - 1) & 1));
-        const uint32_t full = bar_full + 8 * s;
-        mbar_expect_tx(full, tx);
-        const int64_t row0 = (int64_t)tile * tile_rows;
-        bulk_load_1d(sbase + s * kTmXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * pitch, xb, full);
-        if (has_y) bulk_load_1d(sbase + kTmOffY + s * kTmYStage, y + row0, yb, full);
-      }
-    }
+    if (lane == 0)
+      ring_produce<kTmStages>(bar_full, bar_empty, n_tiles, tile_rows, X, pitch, sbase, kTmXStage, has_y, y,
+                              sbase + kTmOffY, kTmYStage, false, nullptr, 0u, 0u);
   } else {
     // LPR lanes per row, RPI rows per warp iteration: lane (g, j) = (lane / LPR, lane % LPR) reads the 4-feature chunks
     // kk * LPR + j of row g, kk = (k + g) mod 4 for k = 0..3 -- the rotation by g keeps the rows of one shared-memory
@@ -482,27 +485,12 @@ score_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const 
       if (++s == kTmStages) { s = 0; phase ^= 1u; }
     }
     if (have) st.add((double)y_keep, p_keep);
-    double v[kNStats] = {st.ape, st.sse, st.sy, st.syy, st.mx, st.cnt(), st.sp, st.spp, st.syp, st.mxape};
-#pragma unroll
-    for (int k = 0; k < kNStats; ++k) {
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) {
-        const double other = shfl_xor_d(v[k], o);
-        v[k] = stat_is_max(k) ? fmax(v[k], other) : v[k] + other;
-      }
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int k = 0; k < kNStats; ++k) red[warp][k] = v[k];
-    }
+    double v[kNStats];
+    st.values(v);
+    stats_butterfly<1>(v);
+    stats_store(red, warp, lane, v);
   }
-  __syncthreads();
-  if (threadIdx.x < kNStats) {
-    const int k = threadIdx.x;
-    double acc = 0.0;
-    for (int w = 0; w < kTmWarps; ++w) acc = stat_is_max(k) ? fmax(acc, red[w][k]) : acc + red[w][k];
-    part[(size_t)blockIdx.x * kNStats + k] = acc;
-  }
+  stats_fold<kTmWarps>(red, part);
 }
 
 // ---- narrow rows (D <= 16): one lane per row behind the same bulk-copy ring ---------------------------------------
@@ -543,31 +531,12 @@ score_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* _
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool has_mask = mask != nullptr, has_y = PLAIN || y != nullptr;
   const uint32_t row_bytes = (uint32_t)d * sizeof(T);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kSnStages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, kSnWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init<kSnStages>(bar_full, bar_empty, kSnWarps);
   __shared__ double red[kSnWarps][kNStats];
   if (warp == kSnWarps) {
-    if (lane == 0) {
-      const uint32_t xb = (uint32_t)G::kRows * row_bytes;
-      const uint32_t tx = xb + (has_y ? G::kYStage : 0u) + (has_mask ? G::kMStage : 0u);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int s = it % kSnStages;
-        if (it >= kSnStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kSnStages - 1) & 1));
-        const uint32_t full = bar_full + 8 * s;
-        mbar_expect_tx(full, tx);
-        const int64_t row0 = (int64_t)tile * G::kRows;
-        bulk_load_1d(sbase + s * G::kXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * row_bytes, xb, full);
-        if (has_y) bulk_load_1d(sbase + G::kOffY + s * G::kYStage, y + row0, G::kYStage, full);
-        if (has_mask) bulk_load_1d(sbase + G::kOffM + s * G::kMStage, mask + row0, G::kMStage, full);
-      }
-    }
+    if (lane == 0)
+      ring_produce<kSnStages>(bar_full, bar_empty, n_tiles, G::kRows, X, row_bytes, sbase, G::kXStage, has_y, y,
+                              sbase + G::kOffY, G::kYStage, has_mask, mask, sbase + G::kOffM, G::kMStage);
   } else {
     double cf[DP];
 #pragma unroll
@@ -620,30 +589,16 @@ score_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* _
       if (lane == 0) mbar_arrive(bar_empty + 8 * s);
       if (++s == kSnStages) { s = 0; phase ^= 1u; }
     }
-    double v[kNStats] = {st.ape, st.sse, st.sy, st.syy, st.mx, st.cnt(), st.sp, st.spp, st.syp, st.mxape};
-#pragma unroll
-    for (int k = 0; k < kNStats; ++k) {
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) {
-        const double other = shfl_xor_d(v[k], o);
-        v[k] = stat_is_max(k) ? fmax(v[k], other) : v[k] + other;
-      }
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int k = 0; k < kNStats; ++k) red[warp][k] = v[k];
-    }
+    double v[kNStats];
+    st.values(v);
+    stats_butterfly<1>(v);
+    stats_store(red, warp, lane, v);
   }
-  __syncthreads();
-  if (threadIdx.x < kNStats) {
-    const int k = threadIdx.x;
-    double acc = 0.0;
-    for (int w = 0; w < kSnWarps; ++w) acc = stat_is_max(k) ? fmax(acc, red[w][k]) : acc + red[w][k];
-    part[(size_t)blockIdx.x * kNStats + k] = acc;
-  }
+  stats_fold<kSnWarps>(red, part);
 }
 
-// acc[0..5] (at part + n_ctas*6 ... see launch) = combine over CTAs in order; `first` overwrites.
+// acc[kNStats] (the running totals, score_totals) = the partials of n_ctas CTAs combined in CTA order; `first`
+// overwrites, otherwise they are combined with acc.
 __global__ void score_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
   const int k = threadIdx.x;
   if (k >= kNStats) return;
@@ -651,76 +606,6 @@ __global__ void score_reduce_kernel(const double* __restrict__ part, int n_ctas,
   for (int c = 0; c < n_ctas; ++c)
     v = stat_is_max(k) ? fmax(v, part[(size_t)c * kNStats + k]) : v + part[(size_t)c * kNStats + k];
   acc[k] = v;
-}
-
-// register-fed kernels (any layout); `first` overwrites the running totals, otherwise they accumulate
-static int launch_score_direct(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
-                               const uint8_t* mask, int keep, float* yhat, bool first) {
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const int vec = (d % 4 == 0) && ((ldx * es) % (4 * es) == 0) && ((reinterpret_cast<uintptr_t>(X) % (4 * es)) == 0);
-  int64_t want = (n + kScoreWarps * 4 - 1) / (kScoreWarps * 4);
-  if (want < 1) want = 1;
-  const int grid = (int)(want < ctx->score_ctas ? want : ctx->score_ctas);
-  double* acc = ctx->score_part + (size_t)ctx->score_ctas * kNStats;
-  const bool rows16 = vec && ((ldx * es) % 16 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0 || x_dtype != B2_F32);
-  if (rows16 && x_dtype == B2_F32)
-    score_kernel_rows8<float><<<grid, kScoreThreads, 0, ctx->stream>>>(static_cast<const float*>(X), n, d, ldx,
-                                                                       ctx->coef_dev, y, mask, keep, yhat,
-                                                                       ctx->score_part);
-  else if (rows16)
-    score_kernel_rows8<__nv_bfloat16><<<grid, kScoreThreads, 0, ctx->stream>>>(
-        static_cast<const __nv_bfloat16*>(X), n, d, ldx, ctx->coef_dev, y, mask, keep, yhat, ctx->score_part);
-  else if (x_dtype == B2_F32)
-    score_kernel<float><<<grid, kScoreThreads, 0, ctx->stream>>>(static_cast<const float*>(X), n, d, ldx,
-                                                                 ctx->coef_dev, y, mask, keep, yhat, vec,
-                                                                 ctx->score_part);
-  else
-    score_kernel<__nv_bfloat16><<<grid, kScoreThreads, 0, ctx->stream>>>(static_cast<const __nv_bfloat16*>(X), n, d,
-                                                                         ldx, ctx->coef_dev, y, mask, keep, yhat,
-                                                                         vec, ctx->score_part);
-  B2_CUDA(cudaGetLastError());
-  score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first ? 1 : 0, acc);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
-}
-
-template <typename T, int DP>
-static int launch_score_narrow_dp(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
-                                  float* yhat, bool first, int64_t* done) {
-  using G = SnGeom<DP>;
-  const int64_t n_tiles = n / G::kRows;
-  *done = 0;
-  if (n_tiles == 0 || n_tiles > 0x7fffffff) return B2_OK;
-  const int cap = ctx->sm_count * 2;
-  const int grid = (int)(n_tiles < cap ? n_tiles : cap);
-#define B2_LAUNCH_SN(EX, PL)                                                                                              \
-  do {                                                                                                                    \
-    B2_CUDA(cudaFuncSetAttribute(score_narrow_kernel<T, DP, EX, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem)); \
-    score_narrow_kernel<T, DP, EX, PL><<<grid, kSnThreads, G::kSmem, ctx->stream>>>(X, (int)n_tiles, d, ctx->coef_dev, y, mask, \
-                                                                                    keep, yhat, ctx->score_part);         \
-  } while (0)
-  const bool plain = mask == nullptr && yhat == nullptr && y != nullptr;
-  if (d == DP) { if (plain) B2_LAUNCH_SN(true, true); else B2_LAUNCH_SN(true, false); }
-  else B2_LAUNCH_SN(false, false);
-#undef B2_LAUNCH_SN
-  B2_CUDA(cudaGetLastError());
-  score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first ? 1 : 0,
-                                                 ctx->score_part + (size_t)ctx->score_ctas * kNStats);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  *done = n_tiles * G::kRows;
-  return B2_OK;
-}
-
-template <typename T>
-static int launch_score_narrow(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
-                               float* yhat, bool first, int64_t* done) {
-  if (d <= 1) return launch_score_narrow_dp<T, 1>(ctx, X, n, d, y, mask, keep, yhat, first, done);
-  if (d <= 2) return launch_score_narrow_dp<T, 2>(ctx, X, n, d, y, mask, keep, yhat, first, done);
-  if (d <= 4) return launch_score_narrow_dp<T, 4>(ctx, X, n, d, y, mask, keep, yhat, first, done);
-  if (d <= 8) return launch_score_narrow_dp<T, 8>(ctx, X, n, d, y, mask, keep, yhat, first, done);
-  return launch_score_narrow_dp<T, 16>(ctx, X, n, d, y, mask, keep, yhat, first, done);
 }
 
 // ---- model_metrics on two vectors (stage_1_train_model.py:79-90): no X, no dot product -- the statistics alone, on
@@ -731,28 +616,13 @@ metrics_kernel(const V* __restrict__ ya, const V* __restrict__ yp, int64_t n, do
   RowStats st;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) st.add_exact((double)ya[i], (double)yp[i]);
-  double v[kNStats] = {st.ape, st.sse, st.sy, st.syy, st.mx, st.cnt(), st.sp, st.spp, st.syp, st.mxape};
+  double v[kNStats];
+  st.values(v);
   __shared__ double red[kScoreWarps][kNStats];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kNStats; ++k) {
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-      const double other = __shfl_xor_sync(0xffffffffu, v[k], o);
-      v[k] = stat_is_max(k) ? fmax(v[k], other) : v[k] + other;
-    }
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int k = 0; k < kNStats; ++k) red[warp][k] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x < kNStats) {
-    const int k = threadIdx.x;
-    double acc = 0.0;
-    for (int w = 0; w < kScoreWarps; ++w) acc = stat_is_max(k) ? fmax(acc, red[w][k]) : acc + red[w][k];
-    part[(size_t)blockIdx.x * kNStats + k] = acc;
-  }
+  stats_butterfly<1>(v);
+  stats_store(red, warp, lane, v);
+  stats_fold<kScoreWarps>(red, part);
 }
 
 // ---- residual gradient of the refined fit (b2_fit_refined; DESIGN.md section 2) -----------------------------------------
@@ -842,13 +712,7 @@ grad_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double
   for (int k = 0; k < 4; ++k)
     if (fj[k] < d) red[warp][fj[k]] = acc[k];
   if (lane == 0) red[warp][kMaxD] = acc1;
-  __syncthreads();
-  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
-    double v = 0.0;
-    if (t < d || t == kMaxD)
-      for (int w = 0; w < kScoreWarps; ++w) v += red[w][t];
-    part[(size_t)blockIdx.x * kGradOut + t] = v;
-  }
+  grad_fold<kScoreWarps>(red, d, part);
 }
 
 // TMA ring: the producer and the lane layout of score_tma_kernel; the labels are always streamed.  beta and the sums stay in
@@ -864,33 +728,16 @@ grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const d
   constexpr int RPI = 32 / LPR, kSweepRows = kTmWarps * RPI;
   const int tile_rows = sweeps * kSweepRows;
   const uint32_t pitch = (uint32_t)d * sizeof(T);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kTmStages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, kTmWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init<kTmStages>(bar_full, bar_empty, kTmWarps);
 
   __shared__ double red[kTmWarps][kGradOut];
   __shared__ __align__(16) double m_s[kMaxD];
   for (int f = threadIdx.x; f < kMaxD; f += blockDim.x) m_s[f] = f < d ? st[kRfMean + f] : 0.0;
   __syncthreads();
   if (warp == kTmWarps) {
-    if (lane == 0) {
-      const uint32_t xb = (uint32_t)tile_rows * pitch, yb = (uint32_t)tile_rows * 4u;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int s = it % kTmStages;
-        if (it >= kTmStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kTmStages - 1) & 1));
-        const uint32_t full = bar_full + 8 * s;
-        mbar_expect_tx(full, xb + yb);
-        const int64_t row0 = (int64_t)tile * tile_rows;
-        bulk_load_1d(sbase + s * kTmXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * pitch, xb, full);
-        bulk_load_1d(sbase + kTmOffY + s * kTmYStage, y + row0, yb, full);
-      }
-    }
+    if (lane == 0)
+      ring_produce<kTmStages>(bar_full, bar_empty, n_tiles, tile_rows, X, pitch, sbase, kTmXStage, true, y,
+                              sbase + kTmOffY, kTmYStage, false, nullptr, 0u, 0u);
   } else {
     const int g = lane / LPR, j = lane % LPR;
     double cf[4][4], acc[4][4];
@@ -983,13 +830,7 @@ grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const d
       __syncwarp();
     }
   }
-  __syncthreads();
-  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
-    double v = 0.0;
-    if (t < d || t == kMaxD)
-      for (int w = 0; w < kTmWarps; ++w) v += red[w][t];
-    part[(size_t)blockIdx.x * kGradOut + t] = v;
-  }
+  grad_fold<kTmWarps>(red, d, part);
 }
 
 // narrow rows (d <= 16): one lane per row behind the bulk-copy ring of score_narrow_kernel
@@ -1004,31 +845,12 @@ grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool has_mask = mask != nullptr;
   const uint32_t row_bytes = (uint32_t)d * sizeof(T);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kSnStages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, kSnWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+  ring_init<kSnStages>(bar_full, bar_empty, kSnWarps);
   __shared__ double red[kSnWarps][kGradOut];
   if (warp == kSnWarps) {
-    if (lane == 0) {
-      const uint32_t xb = (uint32_t)G::kRows * row_bytes;
-      const uint32_t tx = xb + G::kYStage + (has_mask ? G::kMStage : 0u);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int s = it % kSnStages;
-        if (it >= kSnStages) mbar_wait(bar_empty + 8 * s, (uint32_t)((it / kSnStages - 1) & 1));
-        const uint32_t full = bar_full + 8 * s;
-        mbar_expect_tx(full, tx);
-        const int64_t row0 = (int64_t)tile * G::kRows;
-        bulk_load_1d(sbase + s * G::kXStage, reinterpret_cast<const char*>(X) + (size_t)row0 * row_bytes, xb, full);
-        bulk_load_1d(sbase + G::kOffY + s * G::kYStage, y + row0, G::kYStage, full);
-        if (has_mask) bulk_load_1d(sbase + G::kOffM + s * G::kMStage, mask + row0, G::kMStage, full);
-      }
-    }
+    if (lane == 0)
+      ring_produce<kSnStages>(bar_full, bar_empty, n_tiles, G::kRows, X, row_bytes, sbase, G::kXStage, true, y,
+                              sbase + G::kOffY, G::kYStage, has_mask, mask, sbase + G::kOffM, G::kMStage);
   } else {
     double cf[DP], mv[DP], acc[DP];
 #pragma unroll
@@ -1080,13 +902,7 @@ grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __
       }
     }
   }
-  __syncthreads();
-  for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
-    double v = 0.0;
-    if (t < d || t == kMaxD)
-      for (int w = 0; w < kSnWarps; ++w) v += red[w][t];
-    part[(size_t)blockIdx.x * kGradOut + t] = v;
-  }
+  grad_fold<kSnWarps>(red, d, part);
 }
 
 // acc[kGradOut] (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites
@@ -1106,6 +922,78 @@ __global__ void grad_reduce_kernel(const double* __restrict__ part, int n_ctas, 
   acc[t] = v;
 }
 
+// ---- host ---------------------------------------------------------------------------------------------------------
+// Every kernel writes per-CTA partials, and an ordered reduce combines them into the running totals: 2 launches per
+// segment of rows.  `first` overwrites the totals, otherwise the segment's rows are added to them.
+int score_reduce(b2_ctx* ctx, int grid, bool first) {
+  B2_CUDA(cudaGetLastError());
+  score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first ? 1 : 0, score_totals(ctx));
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  return B2_OK;
+}
+// the gradient's totals are ctx->refine + kRfGrad
+int grad_reduce(b2_ctx* ctx, int grid, bool first) {
+  B2_CUDA(cudaGetLastError());
+  grad_reduce_kernel<<<1, 160, 0, ctx->stream>>>(ctx->grad_part, grid, first ? 1 : 0, ctx->refine + kRfGrad);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  return B2_OK;
+}
+
+// Which kernels read the rows [0, n) of one call.  Contiguous 16-byte aligned rows stream through a bulk-copy ring in
+// whole tiles: one lane per row for d <= 16 (narrow, the mask aligned too), LPR lanes per row when a row is a multiple of
+// 16 bytes (wide).  The rows after the last whole tile, and all rows of any other layout, go to the register-fed kernels
+// (direct).  Scoring and the residual gradient share this plan, so a pass of the refined fit reads its rows the way
+// b2_score does, in as many launches.
+struct RowPlan {
+  enum Kind { kDirect, kNarrow, kWide } kind = kDirect;
+  int dp = 0;                   // narrow: the template width narrow_dp(d)
+  int lpr = 0, sweeps = 0;      // wide: lanes per row, consumer sweeps per tile
+  int n_tiles = 0, grid = 0;    // whole ring tiles and the ring's grid (n_tiles == 0: no ring launch)
+  int64_t done = 0;             // rows [0, done) go through the ring
+  bool direct = false;          // the register-fed kernels take the rows [done, n) (one launch when n == 0)
+  int64_t rest = 0;
+  int vec = 0, direct_grid = 0; // their 4-feature vector loads and grid
+};
+
+RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                  const uint8_t* mask) {
+  RowPlan p;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool ring_rows = ldx == d && aligned16(X) && (y == nullptr || aligned16(y));
+  int tile_rows = 0, cap = 0;
+  if (ring_rows && d <= 16 && (mask == nullptr || aligned16(mask))) {
+    p.kind = RowPlan::kNarrow;
+    p.dp = narrow_dp(d);
+    tile_rows = with_int<1, 2, 4, 8, 16>(p.dp, [](auto DP) { return SnGeom<decltype(DP)::value>::kRows; });
+    cap = ctx->sm_count * 2;
+  } else if (ring_rows && d > 16 && d % 4 == 0 && (d * es) % 16 == 0) {
+    p.kind = RowPlan::kWide;
+    p.lpr = d <= 32 ? 2 : (d <= 64 ? 4 : 8);                     // lanes per row: 4 chunks of 4 features per lane
+    const int sweep_rows = kTmWarps * (32 / p.lpr);
+    p.sweeps = (int)(kTmXStage / (uint32_t)(sweep_rows * d * es));
+    if (p.sweeps > kTmTileRowsMax / sweep_rows) p.sweeps = kTmTileRowsMax / sweep_rows;
+    tile_rows = p.sweeps * sweep_rows;
+    cap = ctx->sm_count;
+  }
+  const int64_t n_tiles = tile_rows > 0 ? n / tile_rows : 0;
+  if (n_tiles > 0 && n_tiles <= 0x7fffffff) {
+    p.n_tiles = (int)n_tiles;
+    p.grid = p.n_tiles < cap ? p.n_tiles : cap;
+    p.done = n_tiles * tile_rows;
+  }
+  p.direct = p.done < n || n == 0;
+  p.rest = n - p.done;
+  const uintptr_t x_rest = reinterpret_cast<uintptr_t>(X) + (size_t)p.done * ldx * es;
+  p.vec = (d % 4 == 0) && ((ldx * es) % (4 * es) == 0) && (x_rest % (4 * es) == 0);
+  int64_t want = (p.rest + kScoreWarps * 4 - 1) / (kScoreWarps * 4);
+  if (want < 1) want = 1;
+  p.direct_grid = (int)(want < ctx->score_ctas ? want : ctx->score_ctas);
+  return p;
+}
+
 }  // namespace
 
 int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int64_t n, bool first) {
@@ -1118,176 +1006,87 @@ int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int6
   else
     metrics_kernel<double><<<grid, kScoreThreads, 0, ctx->stream>>>(static_cast<const double*>(y),
                                                                     static_cast<const double*>(yhat), n, ctx->score_part);
-  B2_CUDA(cudaGetLastError());
-  score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first ? 1 : 0,
-                                                 ctx->score_part + (size_t)ctx->score_ctas * kNStats);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
+  return score_reduce(ctx, grid, first);
 }
 
-// ctx->score_part layout: [score_ctas][10] partials, then 10 doubles of running totals.
 int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                  const uint8_t* mask, int keep, float* yhat, bool first_block) {
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  // wide contiguous rows stream through the TMA ring; everything else (and the < one-tile tail) is register-fed
-  const bool wide = ldx == d && d > 16 && d % 4 == 0 && (d * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
-                    (y == nullptr || (reinterpret_cast<uintptr_t>(y) & 15) == 0);
-  const bool narrow = ldx == d && d <= 16 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
-                      (y == nullptr || (reinterpret_cast<uintptr_t>(y) & 15) == 0) &&
-                      (mask == nullptr || (reinterpret_cast<uintptr_t>(mask) & 15) == 0);
-  int64_t done = 0;
-  if (narrow) {
-    int rc;
-    if (x_dtype == B2_F32)
-      rc = launch_score_narrow<float>(ctx, static_cast<const float*>(X), n, d, y, mask, keep, yhat, first_block, &done);
-    else
-      rc = launch_score_narrow<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), n, d, y, mask, keep, yhat,
-                                              first_block, &done);
+  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
+  if (p.n_tiles > 0) {
+    const int rc = with_rows(x_dtype, X, [&](auto* Xr) {
+      using T = row_t<decltype(Xr)>;
+      if (p.kind == RowPlan::kWide)
+        return with_int<2, 4, 8>(p.lpr, [&](auto LPR) {
+          return launch_smem(score_tma_kernel<T, decltype(LPR)::value>, p.grid, kTmThreads, kTmSmem, ctx->stream, Xr,
+                             p.n_tiles, p.sweeps, d, ctx->coef_dev, y, mask, keep, yhat, ctx->score_part);
+        });
+      return with_int<1, 2, 4, 8, 16>(p.dp, [&](auto DP) {
+        constexpr int kDP = decltype(DP)::value;
+        const bool plain = mask == nullptr && yhat == nullptr && y != nullptr;
+        auto kernel = d != kDP ? score_narrow_kernel<T, kDP, false, false>
+                    : plain    ? score_narrow_kernel<T, kDP, true, true> : score_narrow_kernel<T, kDP, true, false>;
+        return launch_smem(kernel, p.grid, kSnThreads, SnGeom<kDP>::kSmem, ctx->stream, Xr, p.n_tiles, d, ctx->coef_dev,
+                           y, mask, keep, yhat, ctx->score_part);
+      });
+    });
     if (rc != B2_OK) return rc;
-    if (done > 0) first_block = false;
-  } else if (wide) {
-    const int lpr = d <= 32 ? 2 : (d <= 64 ? 4 : 8);             // lanes per row: 4 chunks of 4 features per lane
-    const int sweep_rows = kTmWarps * (32 / lpr);
-    int sweeps = (int)(kTmXStage / (uint32_t)(sweep_rows * d * es));
-    if (sweeps > kTmTileRowsMax / sweep_rows) sweeps = kTmTileRowsMax / sweep_rows;
-    const int tile_rows = sweeps * sweep_rows;
-    const int64_t n_tiles = n / tile_rows;
-    if (n_tiles > 0 && n_tiles <= 0x7fffffff) {
-      const int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
-      double* acc = ctx->score_part + (size_t)ctx->score_ctas * kNStats;
-#define B2_LAUNCH_TM(T, LPR)                                                                                          \
-  do {                                                                                                                \
-    B2_CUDA(cudaFuncSetAttribute(score_tma_kernel<T, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmSmem));    \
-    score_tma_kernel<T, LPR><<<grid, kTmThreads, kTmSmem, ctx->stream>>>(static_cast<const T*>(X), (int)n_tiles, sweeps, \
-                                                                         d, ctx->coef_dev, y, mask, keep, yhat,       \
-                                                                         ctx->score_part);                            \
-  } while (0)
-#define B2_LAUNCH_TM_T(T) \
-  do { if (lpr == 2) B2_LAUNCH_TM(T, 2); else if (lpr == 4) B2_LAUNCH_TM(T, 4); else B2_LAUNCH_TM(T, 8); } while (0)
-      if (x_dtype == B2_F32) B2_LAUNCH_TM_T(float); else B2_LAUNCH_TM_T(__nv_bfloat16);
-#undef B2_LAUNCH_TM_T
-#undef B2_LAUNCH_TM
-      B2_CUDA(cudaGetLastError());
-      score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first_block ? 1 : 0, acc);
-      B2_CUDA(cudaGetLastError());
-      ctx->launches += 2;
-      done = n_tiles * tile_rows;
-      first_block = false;
-    }
+    if (int r = score_reduce(ctx, p.grid, first_block)) return r;
+    first_block = false;
   }
-  if (done < n || n == 0) {
-    const char* Xt = static_cast<const char*>(X) + (size_t)done * ldx * es;
-    return launch_score_direct(ctx, Xt, x_dtype, n - done, d, ldx, y != nullptr ? y + done : nullptr,
-                               mask != nullptr ? mask + done : nullptr, keep, yhat != nullptr ? yhat + done : nullptr,
-                               first_block);
-  }
-  return B2_OK;
+  if (!p.direct) return B2_OK;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const char* Xt = static_cast<const char*>(X) + (size_t)p.done * ldx * es;
+  const float* yt = y != nullptr ? y + p.done : nullptr;
+  const uint8_t* mt = mask != nullptr ? mask + p.done : nullptr;
+  float* yhat_t = yhat != nullptr ? yhat + p.done : nullptr;
+  const bool rows16 = p.vec && ((ldx * es) % 16 == 0) && ((reinterpret_cast<uintptr_t>(Xt) & 15) == 0 || x_dtype != B2_F32);
+  with_rows(x_dtype, Xt, [&](auto* Xr) {
+    using T = row_t<decltype(Xr)>;
+    if (rows16)
+      score_kernel_rows8<T><<<p.direct_grid, kScoreThreads, 0, ctx->stream>>>(Xr, p.rest, d, ldx, ctx->coef_dev, yt, mt,
+                                                                               keep, yhat_t, ctx->score_part);
+    else
+      score_kernel<T><<<p.direct_grid, kScoreThreads, 0, ctx->stream>>>(Xr, p.rest, d, ldx, ctx->coef_dev, yt, mt, keep,
+                                                                         yhat_t, p.vec, ctx->score_part);
+    return B2_OK;
+  });
+  return score_reduce(ctx, p.direct_grid, first_block);
 }
 
-// The residual gradient over the rows [0, n): the layout choice of launch_score (the labels are always present).  Every
-// gradient launch is followed by grad_reduce_kernel, which adds its CTA partials in order into ctx->refine + kRfGrad.
-static int grad_reduce(b2_ctx* ctx, int grid, bool first) {
-  B2_CUDA(cudaGetLastError());
-  grad_reduce_kernel<<<1, 160, 0, ctx->stream>>>(ctx->grad_part, grid, first ? 1 : 0, ctx->refine + kRfGrad);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
-}
-
-template <typename T, int DP>
-static int launch_grad_narrow_dp(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
-                                 bool first, int64_t* done) {
-  using G = SnGeom<DP>;
-  const int64_t n_tiles = n / G::kRows;
-  *done = 0;
-  if (n_tiles == 0 || n_tiles > 0x7fffffff) return B2_OK;
-  const int cap = ctx->sm_count * 2;
-  const int grid = (int)(n_tiles < cap ? n_tiles : cap);
-#define B2_LAUNCH_GN(EX)                                                                                                 \
-  do {                                                                                                                   \
-    B2_CUDA(cudaFuncSetAttribute(grad_narrow_kernel<T, DP, EX>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem)); \
-    grad_narrow_kernel<T, DP, EX><<<grid, kSnThreads, G::kSmem, ctx->stream>>>(X, (int)n_tiles, d, ctx->refine, y, mask, \
-                                                                               keep, ctx->grad_part);                    \
-  } while (0)
-  if (d == DP) B2_LAUNCH_GN(true); else B2_LAUNCH_GN(false);
-#undef B2_LAUNCH_GN
-  if (int r = grad_reduce(ctx, grid, first)) return r;
-  *done = n_tiles * G::kRows;
-  return B2_OK;
-}
-
-template <typename T>
-static int launch_grad_narrow(b2_ctx* ctx, const T* X, int64_t n, int d, const float* y, const uint8_t* mask, int keep,
-                              bool first, int64_t* done) {
-  if (d <= 1) return launch_grad_narrow_dp<T, 1>(ctx, X, n, d, y, mask, keep, first, done);
-  if (d <= 2) return launch_grad_narrow_dp<T, 2>(ctx, X, n, d, y, mask, keep, first, done);
-  if (d <= 4) return launch_grad_narrow_dp<T, 4>(ctx, X, n, d, y, mask, keep, first, done);
-  if (d <= 8) return launch_grad_narrow_dp<T, 8>(ctx, X, n, d, y, mask, keep, first, done);
-  return launch_grad_narrow_dp<T, 16>(ctx, X, n, d, y, mask, keep, first, done);
-}
-
+// The residual gradient over the rows [0, n): the kernels of launch_score's plan (the labels are always present).
 int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                 const uint8_t* mask, int keep, bool first_block) {
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool wide = ldx == d && d > 16 && d % 4 == 0 && (d * es) % 16 == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
-                    (reinterpret_cast<uintptr_t>(y) & 15) == 0;
-  const bool narrow = ldx == d && d <= 16 && (reinterpret_cast<uintptr_t>(X) & 15) == 0 &&
-                      (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
-                      (mask == nullptr || (reinterpret_cast<uintptr_t>(mask) & 15) == 0);
-  int64_t done = 0;
-  if (narrow) {
-    int rc;
-    if (x_dtype == B2_F32)
-      rc = launch_grad_narrow<float>(ctx, static_cast<const float*>(X), n, d, y, mask, keep, first_block, &done);
-    else
-      rc = launch_grad_narrow<__nv_bfloat16>(ctx, static_cast<const __nv_bfloat16*>(X), n, d, y, mask, keep, first_block,
-                                             &done);
+  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
+  if (p.n_tiles > 0) {
+    const int rc = with_rows(x_dtype, X, [&](auto* Xr) {
+      using T = row_t<decltype(Xr)>;
+      if (p.kind == RowPlan::kWide)
+        return with_int<2, 4, 8>(p.lpr, [&](auto LPR) {
+          return launch_smem(grad_tma_kernel<T, decltype(LPR)::value>, p.grid, kTmThreads, kTmSmem, ctx->stream, Xr,
+                             p.n_tiles, p.sweeps, d, ctx->refine, y, mask, keep, ctx->grad_part);
+        });
+      return with_int<1, 2, 4, 8, 16>(p.dp, [&](auto DP) {
+        constexpr int kDP = decltype(DP)::value;
+        auto kernel = d == kDP ? grad_narrow_kernel<T, kDP, true> : grad_narrow_kernel<T, kDP, false>;
+        return launch_smem(kernel, p.grid, kSnThreads, SnGeom<kDP>::kSmem, ctx->stream, Xr, p.n_tiles, d, ctx->refine, y,
+                           mask, keep, ctx->grad_part);
+      });
+    });
     if (rc != B2_OK) return rc;
-    if (done > 0) first_block = false;
-  } else if (wide) {
-    const int lpr = d <= 32 ? 2 : (d <= 64 ? 4 : 8);
-    const int sweep_rows = kTmWarps * (32 / lpr);
-    int sweeps = (int)(kTmXStage / (uint32_t)(sweep_rows * d * es));
-    if (sweeps > kTmTileRowsMax / sweep_rows) sweeps = kTmTileRowsMax / sweep_rows;
-    const int tile_rows = sweeps * sweep_rows;
-    const int64_t n_tiles = n / tile_rows;
-    if (n_tiles > 0 && n_tiles <= 0x7fffffff) {
-      const int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
-#define B2_LAUNCH_GT(T, LPR)                                                                                          \
-  do {                                                                                                                \
-    B2_CUDA(cudaFuncSetAttribute(grad_tma_kernel<T, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmSmem));     \
-    grad_tma_kernel<T, LPR><<<grid, kTmThreads, kTmSmem, ctx->stream>>>(static_cast<const T*>(X), (int)n_tiles, sweeps, \
-                                                                        d, ctx->refine, y, mask, keep, ctx->grad_part); \
-  } while (0)
-#define B2_LAUNCH_GT_T(T) \
-  do { if (lpr == 2) B2_LAUNCH_GT(T, 2); else if (lpr == 4) B2_LAUNCH_GT(T, 4); else B2_LAUNCH_GT(T, 8); } while (0)
-      if (x_dtype == B2_F32) B2_LAUNCH_GT_T(float); else B2_LAUNCH_GT_T(__nv_bfloat16);
-#undef B2_LAUNCH_GT_T
-#undef B2_LAUNCH_GT
-      if (int r = grad_reduce(ctx, grid, first_block)) return r;
-      done = n_tiles * tile_rows;
-      first_block = false;
-    }
+    if (int r = grad_reduce(ctx, p.grid, first_block)) return r;
+    first_block = false;
   }
-  if (done < n || n == 0) {
-    const char* Xt = static_cast<const char*>(X) + (size_t)done * ldx * es;
-    const int64_t rows = n - done;
-    const int vec = (d % 4 == 0) && ((ldx * es) % (4 * es) == 0) && ((reinterpret_cast<uintptr_t>(Xt) % (4 * es)) == 0);
-    int64_t want = (rows + kScoreWarps * 4 - 1) / (kScoreWarps * 4);
-    if (want < 1) want = 1;
-    const int grid = (int)(want < ctx->score_ctas ? want : ctx->score_ctas);
-    const uint8_t* mt = mask != nullptr ? mask + done : nullptr;
-    if (x_dtype == B2_F32)
-      grad_kernel<float><<<grid, kScoreThreads, 0, ctx->stream>>>(reinterpret_cast<const float*>(Xt), rows, d, ldx,
-                                                                  ctx->refine, y + done, mt, keep, vec, ctx->grad_part);
-    else
-      grad_kernel<__nv_bfloat16><<<grid, kScoreThreads, 0, ctx->stream>>>(reinterpret_cast<const __nv_bfloat16*>(Xt), rows,
-                                                                          d, ldx, ctx->refine, y + done, mt, keep, vec,
-                                                                          ctx->grad_part);
-    return grad_reduce(ctx, grid, first_block);
-  }
-  return B2_OK;
+  if (!p.direct) return B2_OK;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const char* Xt = static_cast<const char*>(X) + (size_t)p.done * ldx * es;
+  const uint8_t* mt = mask != nullptr ? mask + p.done : nullptr;
+  with_rows(x_dtype, Xt, [&](auto* Xr) {
+    using T = row_t<decltype(Xr)>;
+    grad_kernel<T><<<p.direct_grid, kScoreThreads, 0, ctx->stream>>>(Xr, p.rest, d, ldx, ctx->refine, y + p.done, mt, keep,
+                                                                      p.vec, ctx->grad_part);
+    return B2_OK;
+  });
+  return grad_reduce(ctx, p.direct_grid, first_block);
 }
 
 }  // namespace b2

@@ -27,7 +27,6 @@ TC, NARROW, SIMT = b2.KERNEL_TCGEN05, b2.KERNEL_NARROW, b2.KERNEL_SIMT
 E_ARG, E_SINGULAR, E_UNSUPPORTED = -1, -4, -6
 REFINED_TOL = 1e-10             # refined fit on correlated columns
 SIMT_TOL = 1e-6                 # the exact kernel's coefficient tolerance (test_gpu_columns.TOL[SIMT])
-PASSES_PER_LAUNCH_SET = 3       # DESIGN.md section 3: gradient kernel + ordered reduce + refinement solve
 
 
 def _sk(Xr, y, mask=None, keep=1, **kw):
@@ -227,23 +226,46 @@ def test_single_operand_mode_refines_to_the_contract_and_beyond(ctx):
     assert e < 1e-6, (e0, e, passes, step)
 
 
+# One pass streams the rows through the kernels of b2_score's row plan: each segment of rows is one kernel plus its ordered
+# reduce.  (d, kind, n, ldx, segments); a tail is the rows after the ring's whole tiles, left to the register-fed kernel.
+LAUNCH_LAYOUTS = {
+    "narrow-d1-tail": (1, "f32", 100_001, 1, 2),
+    "narrow-d12-tail": (12, "f32", 100_001, 12, 2),
+    "wide-d128": (128, "f32", 600_000, 128, 1),        # a whole number of 60-row TMA tiles: no register-fed tail
+    "wide-d48-tail": (48, "f32", 100_001, 48, 2),
+    "wide-d24-tail": (24, "f32", 100_001, 24, 2),
+    "bf16-d100": (100, "bf16", 100_001, 100, 1),       # 200-byte rows: register-fed only
+    "strided-d24": (24, "f32", 50_000, 29, 1),
+}
+
+
 def test_repeatable_and_launches_per_pass(ctx):
-    n, d = 600_000, 128                                   # a whole number of 60-row TMA tiles: no register-fed tail
-    _, up, y = _table(n, d, "correlated", "f32", seed=91)
-    Xd, yd = ctx.to_device(up), ctx.to_device(y)
-    try:
-        r1 = ctx.fit_refined(Xd, yd, max_passes=2, tol=0.0)
-        r2 = ctx.fit_refined(Xd, yd, max_passes=2, tol=0.0)
-        assert np.array_equal(r1[0], r2[0]) and r1[1:] == r2[1:]
-        l0 = ctx.launch_count()
-        ctx.fit_refined(Xd, yd, max_passes=0)
-        l1 = ctx.launch_count()
-        _, _, passes, _ = ctx.fit_refined(Xd, yd, max_passes=2, tol=0.0)
-        l2 = ctx.launch_count()
-    finally:
-        Xd.free(); yd.free()
-    assert passes == 2
-    assert (l2 - l1) - (l1 - l0) == 2 * PASSES_PER_LAUNCH_SET
+    for layout, (d, kind, n, ldx, segments) in LAUNCH_LAYOUTS.items():
+        _, up, y = _table(n, d, "correlated", kind, seed=91)
+        rows = np.zeros((n, ldx), dtype=up.dtype)
+        rows[:, :d] = up
+        xdt = b2.F32 if kind == "f32" else b2.BF16
+        Xd, yd = ctx.to_device(rows, kind), ctx.to_device(y)
+        try:
+            r1 = _raw_refined(ctx, Xd.ptr, xdt, yd.ptr, n, d, ldx, max_passes=2, tol=0.0)
+            r2 = _raw_refined(ctx, Xd.ptr, xdt, yd.ptr, n, d, ldx, max_passes=2, tol=0.0)
+            assert r1[0] == 0, (layout, b2.native.last_error())
+            assert np.array_equal(r1[1], r2[1]) and r1[2:] == r2[2:], layout
+            l0 = ctx.launch_count()
+            _raw_refined(ctx, Xd.ptr, xdt, yd.ptr, n, d, ldx, max_passes=0)
+            l1 = ctx.launch_count()
+            rc, coef, b0, passes, _ = _raw_refined(ctx, Xd.ptr, xdt, yd.ptr, n, d, ldx, max_passes=2, tol=0.0)
+            l2 = ctx.launch_count()
+            stats = np.zeros(10, dtype=np.float64)
+            rc_s = b2.native.load().b2_score(ctx._h, Xd.ptr, xdt, n, d, ldx, b2.native.MEM_DEVICE, coef.ctypes.data, b0,
+                                             yd.ptr, None, 1, None, stats.ctypes.data)
+            l3 = ctx.launch_count()
+        finally:
+            Xd.free(); yd.free()
+        assert rc == 0 and rc_s == 0 and passes == 2, (layout, rc, rc_s, passes)
+        # a pass: the refinement solve + b2_score's launches on the same rows
+        assert (l2 - l1) - (l1 - l0) == 2 * (1 + (l3 - l2)), (layout, l0, l1, l2, l3)
+        assert l3 - l2 == 2 * segments, (layout, l3 - l2)
 
 
 def test_errors(ctx):
