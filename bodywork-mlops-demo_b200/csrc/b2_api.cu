@@ -346,8 +346,8 @@ static int ctx_allocate(b2_ctx* ctx) {
   ctx->simt_ctas = ctx->sm_count;
   ctx->score_ctas = ctx->sm_count * 8;
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->S), sizeof(double) * kMaxS * kMaxS));
-  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_part), sizeof(double) * (size_t)ctx->sm_count * kTcAccElems));
-  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_side), sizeof(double) * (size_t)ctx->sm_count * kTcSideDoubles));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_part),
+                     sizeof(double) * (size_t)ctx->sm_count * (kTcAccElems + kTcSums)));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_red), sizeof(double) * (kTcAccElems + 16)));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->shift), gram_shift_bytes()));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->simt_part), sizeof(double) * (size_t)ctx->simt_ctas * kMaxS * kMaxS));
@@ -365,7 +365,6 @@ static int ctx_allocate(b2_ctx* ctx) {
   for (int b = 0; b < 2; ++b) B2_CUDA(cudaEventCreateWithFlags(&ctx->ev_coef[b], cudaEventDisableTiming));
   B2_CUDA(cudaMemset(ctx->shift, 0, gram_shift_bytes()));
   B2_CUDA(cudaMemset(ctx->S, 0, sizeof(double) * kMaxS * kMaxS));
-  B2_CUDA(cudaMemset(ctx->tc_side, 0, sizeof(double) * (size_t)ctx->sm_count * kTcSideDoubles));
   B2_CUDA(cudaMemset(ctx->tc_red, 0, sizeof(double) * (kTcAccElems + 16)));
   return B2_OK;
 }
@@ -407,7 +406,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   if (ctx->comm != nullptr) b2_comm_destroy(ctx);
   b2_comm_p2p_detach(ctx);
   if (ctx->xchg != nullptr) cudaFree(ctx->xchg);
-  void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_side, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
+  void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine};

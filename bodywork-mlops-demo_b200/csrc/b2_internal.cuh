@@ -27,7 +27,9 @@ constexpr int kTcM = 128;                // MMA M: feature index (zero padded)
 constexpr int kTcN = 144;                // MMA N: 128 feature columns (hi) + 16 extra columns [1, y_hi, y_lo, 0...]
 constexpr int kTcAccCols = 2 * kTcN;     // two accumulators: A = hi and A = lo against the same B = [hi | E]
 constexpr int kTcAccElems = kTcM * kTcAccCols;  // fp32 accumulators drained per chunk (36 864)
-constexpr int kTcSideDoubles = 8;        // per-CTA CUDA-core sums: sum y', sum y'^2, rows used
+constexpr int kTcSums = 3;               // per-CTA CUDA-core sums: sum y', sum y'^2, rows used
+// ctx->tc_part of a Gram launch on n_ctas CTAs: [n_ctas][kTcAccElems] fp64 accumulators, then [n_ctas][kTcSums] sums.
+// The finalize locates the sums through its n_ctas, which must equal the Gram grid.  Allocated for n_ctas = sm_count.
 
 // ---- scoring (b2_score, b2_metrics) and the refined fit (b2_fit_refined) ---------------------------------------------
 constexpr int kNStats = 10;              // include/b2gram.h: b2_score stats_out layout (maxima at 4 and 9, sums elsewhere)
@@ -82,17 +84,16 @@ struct b2_ctx {
   double* S = nullptr;                 // device, kMaxS*kMaxS (only (d+2)^2 used, row stride d+2)
 
   // tensor-core path scratch
-  double* tc_part = nullptr;           // [sm_count][kTcAccElems]   per-CTA fp64 partial Gram (col-major)
-  double* tc_side = nullptr;           // [sm_count][kTcSideDoubles]
+  double* tc_part = nullptr;           // sm_count * (kTcAccElems + kTcSums): per-CTA fp64 partial Gram (col-major), y sums
   double* tc_red = nullptr;            // [kTcAccElems + 16]: reduced partials, y sums, b2_comm_barrier's slot at + 8
   float* shift = nullptr;              // gram_shift_bytes(): per-column shift c[kMaxD + 1] (c_y at kMaxD), sample scratch
-  bool tc_attr_set = false;
   bool solve_attr_set = false;
   double* solve_host = nullptr;        // pinned mirror of solve_out (D2H without a staging copy)
   // tensor-map cache of the most recent tensor-core launch (a refit of resident rows re-uses the same maps)
   struct TmCache {
     const void* X = nullptr; const float* y = nullptr; const uint8_t* mask = nullptr;
-    int64_t n = 0, ldx = 0; int d = 0, x_dtype = -1, y_map_2d = 0;
+    int64_t n = 0, ldx = 0; int d = 0, x_dtype = -1;
+    int y_map_2d = 0, m_map_2d = 0;    // y / the mask read through a [n / k][k] view (gram_tc.cu: encode_vec)
     alignas(64) unsigned char tmX[128], tmY[128], tmM[128];
   } tm_cache;
   // SIMT path scratch
@@ -149,7 +150,7 @@ namespace b2 {
 // keeps its two maxima in the kNStats doubles after them)
 inline double* score_totals(const b2_ctx* ctx) { return ctx->score_part + (size_t)ctx->score_ctas * kNStats; }
 
-// ---- launch helpers of the ring kernels (score.cu, gram_narrow.cu) ----------------------------------------------------
+// ---- launch helpers (score.cu, gram_narrow.cu; gram_tc.cu selects its instantiation with with_rows / with_int) -------
 // One launch with `smem` bytes of dynamic shared memory; the attribute is set before every launch.
 template <typename... P, typename... A>
 int launch_smem(void (*kernel)(P...), int grid, int threads, uint32_t smem, cudaStream_t stream, A... args) {

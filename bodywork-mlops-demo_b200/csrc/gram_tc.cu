@@ -159,8 +159,9 @@ __device__ __forceinline__ void wgmma_m64n144k16(float (&d)[72], uint64_t adesc,
         "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// D[64 x 128] (+)= A[64 x 16] * B[16 x 128]: A K-major, B MN-major (the raw 128B-swizzled TMA tile)
-__device__ __forceinline__ void wgmma_m64n128k16_bmn(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128]: A K-major, B MN-major (the raw 128B-swizzled TMA tile); d[0..63] are
+// registers 0..63 of an m64n144 fragment (its columns 0..127)
+__device__ __forceinline__ void wgmma_m64n128k16_bmn(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %66, 0;\n\t"
@@ -180,8 +181,9 @@ __device__ __forceinline__ void wgmma_m64n128k16_bmn(float (&d)[64], uint64_t ad
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]: both K-major (B = the E columns)
-__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]: both K-major (B = the E columns); d[0..7] are registers 64..71 of an
+// m64n144 fragment (its columns 128..143)
+__device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %10, 0;\n\t"
@@ -232,47 +234,40 @@ __device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_
 // ------------------------------------------------------------------------------------------
 // finalize: the per-CTA partials reduced into
 //   red[col * 128 + i], col in [0, 288):  col < 144: D1 (A = hi), col >= 144: D2 (A = lo), columns of [hi | E]
-//   red[kTcAccElems + 0..2]            : sum y', sum y'^2, rows used
+//   red[kTcAccElems + 0..2]            : sum y', sum y'^2, rows used (the E warp's CUDA-core sums)
+// Element idx of CTA c of an n_ctas grid sits at part[c * kTcAccElems + idx] (the accumulators) or, from kTcAccElems on,
+// at part[n_ctas * kTcAccElems + c * kTcSums + idx - kTcAccElems] (the sums, behind all accumulators, so that every
+// CTA's accumulators keep the kTcAccElems stride).
 // ------------------------------------------------------------------------------------------
-constexpr int kRedElems = kTcAccElems + 3;
+constexpr int kRedElems = kTcAccElems + kTcSums;
 
 // Sum over the CTAs of elements [e0, e1) of the per-CTA partials.  4 threads per element: thread (e, q) sums the q-th
-// quarter of the CTAs with 8 loads in flight (the loads are the latency), the quarters are combined in the fixed order
-// 0..3 -> deterministic.  `quarter`: shared scratch of 4 * (blockDim.x / 4) doubles.  Call with the whole block.
-__device__ __forceinline__ void tc_reduce_range(const double* part, const double* side, int n_ctas, double* red,
-                                                int e0, int e1, double* quarter) {
+// quarter of the CTAs with 8 loads in flight (the loads are the latency: a serial walk over the CTAs costs one L2
+// round trip each, ~140 ns per CTA), the quarters are combined in the fixed order 0..3 -> deterministic.  `quarter`:
+// shared scratch of 4 * (blockDim.x / 4) doubles.  Call with the whole block.
+__device__ __forceinline__ void tc_reduce_range(const double* part, int n_ctas, double* red, int e0, int e1,
+                                                double* quarter) {
   const int epb = blockDim.x >> 2;                 // elements per pass
   const int e = threadIdx.x % epb, q = threadIdx.x / epb;
   const int per = (n_ctas + 3) / 4;
   const int c0 = q * per, c1 = (c0 + per < n_ctas) ? c0 + per : n_ctas;
   for (int base = e0; base < e1; base += epb) {
     const int idx = base + e;
-    if (idx < e1 && idx < kTcAccElems) {
+    if (idx < e1) {
+      const bool sum = idx >= kTcAccElems;
+      const double* src = sum ? part + (size_t)n_ctas * kTcAccElems + (idx - kTcAccElems) : part + idx;
+      const size_t stride = sum ? kTcSums : kTcAccElems;                        // from one CTA to the next
       double acc[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       int c = c0;
       for (; c + 8 <= c1; c += 8) {
 #pragma unroll
-        for (int u = 0; u < 8; ++u) acc[u] += __ldcg(part + (size_t)(c + u) * kTcAccElems + idx);
+        for (int u = 0; u < 8; ++u) acc[u] += __ldcg(src + (size_t)(c + u) * stride);
       }
-      for (; c < c1; ++c) acc[0] += __ldcg(part + (size_t)c * kTcAccElems + idx);
-      quarter[q * epb + e] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
-    } else if (idx < e1 && idx < kRedElems) {
-      // the three CUDA-core sums (sum y', sum y'^2, rows): same quarter scheme, loads 8 deep (a serial walk over the
-      // CTAs costs one L2 round trip each, ~140 ns per CTA)
-      const int k = idx - kTcAccElems;
-      double acc[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-      int c = c0;
-      for (; c + 8 <= c1; c += 8) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u)
-          acc[u] += __ldcg(side + (size_t)(c + u) * kTcSideDoubles + k) + __ldcg(side + (size_t)(c + u) * kTcSideDoubles + 3 + k);
-      }
-      for (; c < c1; ++c) acc[0] += __ldcg(side + (size_t)c * kTcSideDoubles + k) + __ldcg(side + (size_t)c * kTcSideDoubles + 3 + k);
+      for (; c < c1; ++c) acc[0] += __ldcg(src + (size_t)c * stride);
       quarter[q * epb + e] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
     }
     __syncthreads();
-    if (q == 0 && idx < e1 && idx < kRedElems)
-      red[idx] = ((quarter[e] + quarter[epb + e]) + quarter[2 * epb + e]) + quarter[3 * epb + e];
+    if (q == 0 && idx < e1) red[idx] = ((quarter[e] + quarter[epb + e]) + quarter[2 * epb + e]) + quarter[3 * epb + e];
     __syncthreads();
   }
 }
@@ -353,8 +348,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                const __grid_constant__ CUtensorMap tmM, int y_map_2d, int has_mask, int keep,
                int64_t n_rows, int d_arg, int pack, int d_orig, const float* __restrict__ shift,
-               int chunk_tiles,
-               double* __restrict__ part, double* __restrict__ side, uint32_t wait_ns, uint32_t dbg_arg) {
+               int chunk_tiles, double* __restrict__ part, uint32_t wait_ns, uint32_t dbg_arg) {
 #ifdef B2_DEV_KNOBS
   const uint32_t dbg = dbg_arg;      // ablation switches (tools/build_dev.sh): results are WRONG when non-zero
 #else
@@ -415,127 +409,70 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
     // ===== consumers: wgmma into register accumulators, fp64 drain to the CTA's partial in global =====
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G::kConsumerRegs));
     const int wg = warp >> 2;
-    if constexpr (RAWB) {
+    // no plain instruction may write the accumulators between wgmma (ptxas would serialise them): a chunk restarts D1,
+    // and the first tile starts D2, with scale-d = 0 on its first K step
+    float acc1[kAccRegs], acc2[kAccRegs];
     // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
-    // column 8 j + 2 (lane % 4) + e, in accX (columns = the 128 raw features) and in accE (columns = E); accX2 / accE2: lo
-    float accX[64], accE[8], accX2[64], accE2[8];
+    // column 8 j + 2 (lane % 4) + e (RAWB fills registers 0..63 from the raw tile and 64..71 from E with separate MMAs);
+    // the partial is column-major [col][feature].  store(dst, add, val) writes (or adds) val(r, col, h) for every r.
     double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
-    const int col0 = 2 * (lane & 3);
-    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;
+    auto store = [&](double* dst, bool add, auto val) {
+#pragma unroll
+      for (int r = 0; r < kAccRegs; ++r) {
+        const int col = 8 * (r >> 2) + 2 * (lane & 3) + (r & 1), h = (r >> 1) & 1;
+        const double v = val(r, col, h);
+        double* p = dst + (size_t)col * kTcM + 8 * h;
+        if (add) *p += v;
+        else *p = v;
+      }
+    };
+    // RAWB's feature columns carry the raw x: sum_r a_i x_j - c_j sum_r a_i = sum_r a_i v_j, where sum_r a_i is E's ones
+    // column (registers 64 / 66, held by lane 4 * (lane / 4)); D2 stores them halved (x_scale = 0.5, see above)
+    auto drain = [&](const float (&acc)[kAccRegs], double* dst, bool add, double x_scale) {
+      if constexpr (RAWB) {
+        const double s1[2] = {(double)__shfl_sync(0xffffffffu, acc[64], lane & ~3),
+                              (double)__shfl_sync(0xffffffffu, acc[66], lane & ~3)};
+        store(dst, add, [&](int r, int col, int h) {
+          return r < 64 ? x_scale * ((double)acc[r] - (double)shift_s[col] * s1[h]) : (double)acc[r];
+        });
+      } else {
+        store(dst, add, [&](int r, int, int) { return (double)acc[r]; });
+      }
+    };
+    // the stages of a tile: RAWB's consumers also hold its raw stage, the B operand of its MMAs
+    auto release = [&](int tile) {
+      mbar_arrive(bar_op_empty + 8 * (tile % kOpStages));
+      if constexpr (RAWB) mbar_arrive(bar_raw_empty + 8 * (tile % kRawStages));
+    };
+    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;      // this warpgroup's 64 features of A
     int os = 0, held = -1, in_chunk = 0;                   // held: the tile whose stages wait for their MMAs
     uint32_t oph = 0;
     bool first_chunk = true;
     for (int it = 0; it < my_tiles; ++it) {
       mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
       const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-      const uint32_t raw_addr = sbase + kOffRaw + (uint32_t)(it % kRawStages) * kRawStageBytes;
       wgmma_fence();
 #pragma unroll
       for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
         const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
-        const uint64_t x_desc = make_raw_desc(raw_addr + k2 * 16 * 128);        // rows 16 k2 .. 16 k2 + 15
-        const uint64_t e_desc = make_smem_desc(k_addr + kOpEOff);
-        const uint64_t hi_desc = make_smem_desc(k_addr + a_off);
-        const uint32_t sc = (in_chunk > 0 || k2 > 0) ? 1u : 0u;
-        wgmma_m64n128k16_bmn(accX, hi_desc, x_desc, sc);
-        wgmma_m64n16k16(accE, hi_desc, e_desc, sc);
-        if constexpr (SPLIT) {
-          const uint64_t lo_desc = make_smem_desc(k_addr + kOpLoOff + a_off);
-          const uint32_t sc2 = (it > 0 || k2 > 0) ? 1u : 0u;
-          wgmma_m64n128k16_bmn(accX2, lo_desc, x_desc, sc2);
-          wgmma_m64n16k16(accE2, lo_desc, e_desc, sc2);
+        const uint64_t hi_desc = make_smem_desc(k_addr + a_off), lo_desc = make_smem_desc(k_addr + kOpLoOff + a_off);
+        const uint32_t sc1 = (in_chunk > 0 || k2 > 0) ? 1u : 0u, sc2 = (it > 0 || k2 > 0) ? 1u : 0u;
+        if constexpr (RAWB) {
+          // rows 16 k2 .. 16 k2 + 15 of the raw tile, and E
+          const uint64_t x_desc =
+              make_raw_desc(sbase + kOffRaw + (uint32_t)(it % kRawStages) * kRawStageBytes + k2 * 16 * 128);
+          const uint64_t e_desc = make_smem_desc(k_addr + kOpEOff);
+          wgmma_m64n128k16_bmn(acc1, hi_desc, x_desc, sc1);
+          wgmma_m64n16k16(acc1 + 64, hi_desc, e_desc, sc1);
+          if constexpr (SPLIT) {
+            wgmma_m64n128k16_bmn(acc2, lo_desc, x_desc, sc2);
+            wgmma_m64n16k16(acc2 + 64, lo_desc, e_desc, sc2);
+          }
+        } else {
+          const uint64_t b_desc = make_smem_desc(k_addr);                               // [hi | E]
+          if (!(dbg & 2u)) wgmma_m64n144k16(acc1, hi_desc, b_desc, sc1);                // A = hi
+          if (SPLIT && !(dbg & 3u)) wgmma_m64n144k16(acc2, lo_desc, b_desc, sc2);       // A = lo
         }
-      }
-      wgmma_commit();
-      const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
-      if (last) {
-        wgmma_wait<0>();
-        fence_regs(accX);
-        fence_regs(accE);
-      } else {
-        wgmma_wait<1>();
-      }
-      if (lane == 0) {
-        if (held >= 0) {
-          mbar_arrive(bar_op_empty + 8 * (held % kOpStages));
-          mbar_arrive(bar_raw_empty + 8 * (held % kRawStages));
-        }
-        if (last) {
-          mbar_arrive(bar_op_empty + 8 * os);
-          mbar_arrive(bar_raw_empty + 8 * (it % kRawStages));
-        }
-      }
-      held = last ? -1 : it;
-      if (last) {
-        // sum_r hi_i x_j - c_j sum_r hi_i = sum_r hi_i v_j; sum_r hi_i is E1's ones column, held by lane 4 * (lane / 4)
-        const double s1a = (double)__shfl_sync(0xffffffffu, accE[0], lane & ~3);
-        const double s1b = (double)__shfl_sync(0xffffffffu, accE[2], lane & ~3);
-#pragma unroll
-        for (int r = 0; r < 64; ++r) {
-          const int col = 8 * (r >> 2) + col0 + (r & 1);
-          const double val = (double)accX[r] - (double)shift_s[col] * (((r >> 1) & 1) ? s1b : s1a);
-          double* dst = my_part + (size_t)col * kTcM + 8 * ((r >> 1) & 1);
-          if (first_chunk) *dst = val;
-          else *dst += val;
-        }
-#pragma unroll
-        for (int r = 0; r < 8; ++r) {
-          double* dst = my_part + (size_t)(kMaxD + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1);
-          if (first_chunk) *dst = (double)accE[r];
-          else *dst += (double)accE[r];
-        }
-        first_chunk = false;
-        in_chunk = 0;
-      } else {
-        ++in_chunk;
-      }
-      if (++os == kOpStages) { os = 0; oph ^= 1; }
-    }
-    wgmma_wait<0>();
-    double* my_part2 = my_part + (size_t)kTcN * kTcM;      // partial columns [144, 288)
-    if constexpr (SPLIT) {
-      fence_regs(accX2);
-      fence_regs(accE2);
-      const double s1a = (double)__shfl_sync(0xffffffffu, accE2[0], lane & ~3);
-      const double s1b = (double)__shfl_sync(0xffffffffu, accE2[2], lane & ~3);
-#pragma unroll
-      for (int r = 0; r < 64; ++r) {
-        const int col = 8 * (r >> 2) + col0 + (r & 1);
-        my_part2[(size_t)col * kTcM + 8 * ((r >> 1) & 1)] =
-            0.5 * ((double)accX2[r] - (double)shift_s[col] * (((r >> 1) & 1) ? s1b : s1a));
-      }
-#pragma unroll
-      for (int r = 0; r < 8; ++r)
-        my_part2[(size_t)(kMaxD + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = (double)accE2[r];
-    } else {
-#pragma unroll
-      for (int r = 0; r < kAccRegs; ++r)
-        my_part2[(size_t)(8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = 0.0;
-    }
-    } else {
-    // no plain instruction may write the accumulators between wgmma (ptxas would serialise them): a chunk restarts D1,
-    // and the first tile starts D2, with scale-d = 0 on its first K step
-    float acc1[kAccRegs], acc2[kAccRegs];
-    // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
-    // column 8 j + 2 (lane % 4) + e; the partial is column-major [col][feature]
-    double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
-    const int col0 = 2 * (lane & 3);
-    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;      // this warpgroup's 64 features of A
-    int os = 0, held = -1, in_chunk = 0;
-    uint32_t oph = 0;
-    bool first_chunk = true;
-    for (int it = 0; it < my_tiles; ++it) {
-      mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
-      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
-        const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
-        const uint64_t b_desc = make_smem_desc(k_addr);                        // [hi | E]
-        if (!(dbg & 2u))                                                                        // A = hi
-          wgmma_m64n144k16(acc1, make_smem_desc(k_addr + a_off), b_desc, (in_chunk > 0 || k2 > 0) ? 1u : 0u);
-        if (SPLIT && !(dbg & 3u))                                                               // A = lo
-          wgmma_m64n144k16(acc2, make_smem_desc(k_addr + kOpLoOff + a_off), b_desc, (it > 0 || k2 > 0) ? 1u : 0u);
       }
       wgmma_commit();
       const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
@@ -549,18 +486,12 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         wgmma_wait<1>();
       }
       if (lane == 0) {
-        if (held >= 0) mbar_arrive(bar_op_empty + 8 * held);
-        if (last) mbar_arrive(bar_op_empty + 8 * os);
+        if (held >= 0) release(held);
+        if (last) release(it);
       }
-      held = last ? -1 : os;
+      held = last ? -1 : it;
       if (last) {
-        // D1 of this chunk: fold into partial columns [0, 144)
-#pragma unroll
-        for (int r = 0; r < kAccRegs; ++r) {
-          double* dst = my_part + (size_t)(8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1);
-          if (first_chunk) *dst = (double)acc1[r];
-          else *dst += (double)acc1[r];
-        }
+        drain(acc1, my_part, !first_chunk, 1.0);           // D1 of this chunk: partial columns [0, 144)
         first_chunk = false;
         in_chunk = 0;
       } else {
@@ -569,11 +500,13 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       if (++os == kOpStages) { os = 0; oph ^= 1; }
     }
     wgmma_wait<0>();     // a no-op at run time (see above), but ptxas cannot prove it and would wait inside the loop
-    if constexpr (SPLIT) fence_regs(acc2);
     // D2 (A = lo) accumulated over the whole range (small zero-mean sums): partial columns [144, 288)
-#pragma unroll
-    for (int r = 0; r < kAccRegs; ++r)
-      my_part[(size_t)(kTcN + 8 * (r >> 2) + col0 + (r & 1)) * kTcM + 8 * ((r >> 1) & 1)] = SPLIT ? (double)acc2[r] : 0.0;
+    double* my_part2 = my_part + (size_t)kTcN * kTcM;
+    if constexpr (SPLIT) {
+      fence_regs(acc2);
+      drain(acc2, my_part2, false, 0.5);
+    } else {
+      store(my_part2, false, [](int, int, int) { return 0.0; });
     }
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(G::kProducerRegs));
@@ -739,9 +672,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
       }
       if (lane == 0) {
-        double* ys = side + (size_t)blockIdx.x * kTcSideDoubles;
+        double* ys = part + (size_t)gridDim.x * kTcAccElems + kTcSums * blockIdx.x;   // behind all accumulators
         ys[0] = sy; ys[1] = syy; ys[2] = cnt;
-        ys[3] = 0.0; ys[4] = 0.0; ys[5] = 0.0;
       }
     }
   }
@@ -765,8 +697,8 @@ constexpr int kFinalizeThreads = 1024;                           // 4 threads pe
 constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinalizeThreads / 4);   // 145: one pass
 
 __global__ void __launch_bounds__(kFinalizeThreads, 1)
-tc_finalize_kernel(const double* part, const double* side, int n_ctas, double* red, const float* __restrict__ shift,
-                   int d, int pack, double* S, unsigned int* sync, const TcFinal fin) {
+tc_finalize_kernel(const double* part, int n_ctas, double* red, const float* __restrict__ shift, int d, int pack,
+                   double* S, unsigned int* sync, const TcFinal fin) {
   __shared__ double quarter[kFinalizeThreads];
   __shared__ double c_s[kMaxD + 1];                              // the shift as fp64 (c_s[kMaxD]: c_y)
   for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x) c_s[j] = (double)shift[j];
@@ -775,7 +707,7 @@ tc_finalize_kernel(const double* part, const double* side, int n_ctas, double* r
     const int per = (((kRedElems + (int)gridDim.x - 1) / (int)gridDim.x) + epb - 1) / epb * epb;
     const int e0 = (int)blockIdx.x * per;
     const int e1 = e0 + per < kRedElems ? e0 + per : kRedElems;
-    if (e0 < kRedElems) tc_reduce_range(part, side, n_ctas, red, e0, e1, quarter);
+    if (e0 < kRedElems) tc_reduce_range(part, n_ctas, red, e0, e1, quarter);
   }
   grid_barrier(sync + 0);
   {
@@ -835,14 +767,42 @@ bool gram_tc_supported(const void* X, int x_dtype, const float* y, int64_t n, in
   return true;
 }
 
+// A vector of n elements of es bytes (y, the row mask) read `box` elements per tile: a 1-D map, else a [n / k][k] view
+// with 16-byte rows (k = 16 / es) that lands the same bytes in shared memory.  Box extents stop at 256 (pack = 5 tiles
+// read 320), and a driver may refuse rank-1 maps.  The view is taken only when k divides n: otherwise its last row
+// would reach past the vector.
+static int encode_vec(PFN_encodeTiled encode, CUtensorMap* tm, CUtensorMapDataType type, int es, const void* v,
+                      int64_t n, cuuint32_t box, int* view_2d, const char* what) {
+  const cuuint32_t estr[2] = {1, 1};
+  const cuuint64_t dims[1] = {(cuuint64_t)n}, strides[1] = {0};
+  CUresult r = CUDA_ERROR_INVALID_VALUE;
+  if (box <= 256)
+    r = encode(tm, type, 1, const_cast<void*>(v), dims, strides, &box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  *view_2d = r != CUDA_SUCCESS;
+  const int k = 16 / es;
+  if (r != CUDA_SUCCESS && n % k == 0) {
+    const cuuint64_t dims2[2] = {(cuuint64_t)k, (cuuint64_t)(n / k)}, strides2[1] = {16};
+    const cuuint32_t box2[2] = {(cuuint32_t)k, box / k};
+    r = encode(tm, type, 2, const_cast<void*>(v), dims2, strides2, box2, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(%s) failed with %d (n=%lld box=%u)", what, (int)r, (long long)n, (unsigned)box);
+    return B2_E_CUDA;
+  }
+  return B2_OK;
+}
+
 // d: inner extent of the (super-)row tensor; d_box: inner extent of the smem tile (> d: the rest is zero fill)
 // swz64: the raw tile of the bf16 D = 128 path -- [64 rows][64 features] boxes (128-byte rows) with SWIZZLE_128B
 static int encode_maps(PFN_encodeTiled encode, const void* X, int x_dtype, int es, const float* y, int64_t n, int d,
                        int d_box, int64_t ldx, int64_t n_y, int pack, const uint8_t* mask, bool swz64, CUtensorMap* tmX_out,
                        CUtensorMap* tmY_out, CUtensorMap* tmM_out, int* y_map_2d_out, int* m_map_2d_out) {
   const cuuint32_t y_box = (cuuint32_t)(kTcRows * pack);   // original rows per tile
-  CUtensorMap& tmX = *tmX_out; CUtensorMap& tmY = *tmY_out; CUtensorMap& tmM = *tmM_out;
-  memset(&tmM, 0, sizeof(tmM));
+  CUtensorMap& tmX = *tmX_out;
+  memset(tmM_out, 0, sizeof(*tmM_out));
+  *m_map_2d_out = 0;
   {
     cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)n};
     cuuint64_t strides[1] = {(cuuint64_t)ldx * es};
@@ -858,64 +818,9 @@ static int encode_maps(PFN_encodeTiled encode, const void* X, int x_dtype, int e
       return B2_E_CUDA;
     }
   }
-  int y_map_2d = 0;
-  {
-    cuuint64_t dims[1] = {(cuuint64_t)n_y};
-    cuuint64_t strides[1] = {0};
-    cuuint32_t box[1] = {y_box};
-    cuuint32_t estr[1] = {1};
-    CUresult r = CUDA_ERROR_INVALID_VALUE;
-    if (y_box <= 256)
-      r = encode(&tmY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, const_cast<float*>(y), dims, strides, box, estr,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      // rank-1 maps refused: view y as [ceil(n/4)][4] (16-byte rows) -- the same bytes land in smem
-      cuuint64_t dims2[2] = {4, (cuuint64_t)((n_y + 3) / 4)};
-      cuuint64_t strides2[1] = {16};
-      cuuint32_t box2[2] = {4, y_box / 4};
-      cuuint32_t estr2[2] = {1, 1};
-      r = encode(&tmY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(y), dims2, strides2, box2, estr2,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      y_map_2d = 1;
-      if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(y) failed with %d", (int)r);
-        return B2_E_CUDA;
-      }
-    }
-  }
-  int m_map_2d = 0;
-  if (mask != nullptr) {
-    cuuint64_t dims[1] = {(cuuint64_t)n_y};
-    cuuint64_t strides[1] = {0};
-    cuuint32_t box[1] = {y_box};
-    cuuint32_t estr[1] = {1};
-    CUresult r = CUDA_ERROR_INVALID_VALUE;
-    if (y_box <= 256)
-      r = encode(&tmM, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, const_cast<uint8_t*>(mask), dims, strides, box, estr,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS && n_y % 16 == 0) {
-      // box extents stop at 256: view the mask as [n/16][16] (16-byte rows) -- the same bytes land in smem
-      cuuint64_t dims2[2] = {16, (cuuint64_t)(n_y / 16)};
-      cuuint64_t strides2[1] = {16};
-      cuuint32_t box2[2] = {16, y_box / 16};
-      cuuint32_t estr2[2] = {1, 1};
-      r = encode(&tmM, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(mask), dims2, strides2, box2, estr2,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      m_map_2d = 1;
-    }
-    if (r != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(mask) failed with %d", (int)r);
-      return B2_E_CUDA;
-    }
-  }
-
-  *m_map_2d_out = m_map_2d;
-  *y_map_2d_out = y_map_2d;
-  return B2_OK;
+  if (int r = encode_vec(encode, tmY_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, n_y, y_box, y_map_2d_out, "y")) return r;
+  if (mask == nullptr) return B2_OK;
+  return encode_vec(encode, tmM_out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, mask, n_y, y_box, m_map_2d_out, "mask");
 }
 
 // Row packing rule: how many of the n rows the tensor-core launch covers (the rest, < 80 rows, take the CUDA-core kernel)
@@ -954,19 +859,18 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   // bf16-stored rows with D = 128: the raw tile is the MMA's B operand (RAWB)
   const bool rawb = x_dtype == B2_BF16 && d_in == 128 && pack == 1;
   CUtensorMap tmX, tmY, tmM;
-  int y_map_2d = 0, m_map_2d = 0;
   b2_ctx::TmCache& tc = ctx->tm_cache;
   const bool cached = tc.X == X && tc.y == y && tc.mask == mask && tc.n == n_in && tc.ldx == ldx_in && tc.d == d_in &&
                       tc.x_dtype == x_dtype;
   if (cached) {
     memcpy(&tmX, tc.tmX, sizeof(tmX)); memcpy(&tmY, tc.tmY, sizeof(tmY)); memcpy(&tmM, tc.tmM, sizeof(tmM));
-    y_map_2d = tc.y_map_2d & 1; m_map_2d = (tc.y_map_2d >> 1) & 1;
   } else {
+    int y_map_2d = 0, m_map_2d = 0;
     if (int r = encode_maps(encode, X, x_dtype, es, y, n, d_tensor, d, ldx, n_y, pack, mask, rawb, &tmX, &tmY, &tmM, &y_map_2d,
                             &m_map_2d))
       return r;
     tc.X = X; tc.y = y; tc.mask = mask; tc.n = n_in; tc.ldx = ldx_in; tc.d = d_in; tc.x_dtype = x_dtype;
-    tc.y_map_2d = y_map_2d | (m_map_2d << 1);
+    tc.y_map_2d = y_map_2d; tc.m_map_2d = m_map_2d;
     memcpy(tc.tmX, &tmX, sizeof(tmX)); memcpy(tc.tmY, &tmY, sizeof(tmY)); memcpy(tc.tmM, &tmM, sizeof(tmM));
   }
 
@@ -977,21 +881,6 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   // keeps their truncation error at the level of the shifted operands' accumulators
   int chunk_tiles = ctx->drain_rows / kTcRows / (rawb ? 4 : 1);
   if (chunk_tiles < 1) chunk_tiles = 1;
-
-  if (!ctx->tc_attr_set) {
-#define B2_SET_SMEM(T, DF, SP) \
-  B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<T, DF, SP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<false>::kSmemBytes))
-    B2_SET_SMEM(float, 128, true); B2_SET_SMEM(float, 0, true);
-    B2_SET_SMEM(float, 128, false); B2_SET_SMEM(float, 0, false);
-    B2_SET_SMEM(__nv_bfloat16, 128, true); B2_SET_SMEM(__nv_bfloat16, 0, true);
-    B2_SET_SMEM(__nv_bfloat16, 128, false); B2_SET_SMEM(__nv_bfloat16, 0, false);
-#undef B2_SET_SMEM
-    B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 TcGeo<true>::kSmemBytes));
-    B2_CUDA(cudaFuncSetAttribute(gram_tc_kernel<__nv_bfloat16, 128, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 TcGeo<true>::kSmemBytes));
-    ctx->tc_attr_set = true;
-  }
 
 #ifdef B2_DEV_KNOBS
   static const uint32_t wait_ns = []() {   // development knob: suspend-time hint of the pipeline waits
@@ -1010,25 +899,28 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
 #else
   constexpr uint32_t dbg = 0u;
 #endif
+  decltype(&gram_tc_kernel<float, 0, false>) kernel = nullptr;
+  uint32_t smem = TcGeo<false>::kSmemBytes;
+  with_rows(x_dtype, X, [&](auto* Xr) {
+    using T = row_t<decltype(Xr)>;
+    return with_int<0, 1>(ctx->precision == B2_PRECISION_SPLIT, [&](auto SP) {
+      constexpr bool kSplit = decltype(SP)::value;
+      kernel = d == 128 ? gram_tc_kernel<T, 128, kSplit> : gram_tc_kernel<T, 0, kSplit>;
+      if constexpr (std::is_same_v<T, __nv_bfloat16>) {
+        if (rawb) {
+          kernel = gram_tc_kernel<T, 128, kSplit, true>;
+          smem = TcGeo<true>::kSmemBytes;
+        }
+      }
+      return B2_OK;
+    });
+  });
+  // set before the start event: the call's host latency is not part of the kernel time the events report
+  B2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int pair = ctx->k_pairs % kKernelEventPairs;
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][0], ctx->stream));
-#define B2_LAUNCH_TC(T, DF, SP, RB)                                                                      \
-  gram_tc_kernel<T, DF, SP, RB><<<grid, kThreads, TcGeo<RB>::kSmemBytes, ctx->stream>>>(                     \
-      tmX, tmY, tmM, y_map_2d, mask != nullptr ? 1 + m_map_2d : 0, keep, n, d, pack, d_in, ctx->shift,       \
-      chunk_tiles,                                                                                        \
-      ctx->tc_part, ctx->tc_side, wait_ns, dbg)
-#define B2_LAUNCH_TC_D(T, SP) \
-  do { if (d == 128) B2_LAUNCH_TC(T, 128, SP, false); else B2_LAUNCH_TC(T, 0, SP, false); } while (0)
-  const bool split = ctx->precision == B2_PRECISION_SPLIT;
-  if (rawb) {
-    if (split) B2_LAUNCH_TC(__nv_bfloat16, 128, true, true); else B2_LAUNCH_TC(__nv_bfloat16, 128, false, true);
-  } else if (x_dtype == B2_F32) {
-    if (split) B2_LAUNCH_TC_D(float, true); else B2_LAUNCH_TC_D(float, false);
-  } else {
-    if (split) B2_LAUNCH_TC_D(__nv_bfloat16, true); else B2_LAUNCH_TC_D(__nv_bfloat16, false);
-  }
-#undef B2_LAUNCH_TC_D
-#undef B2_LAUNCH_TC
+  kernel<<<grid, kThreads, smem, ctx->stream>>>(tmX, tmY, tmM, tc.y_map_2d, mask != nullptr ? 1 + tc.m_map_2d : 0, keep,
+                                                n, d, pack, d_in, ctx->shift, chunk_tiles, ctx->tc_part, wait_ns, dbg);
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaEventRecord(ctx->ev_k[pair][1], ctx->stream));
   ctx->k_pairs += 1;
@@ -1051,10 +943,10 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     attr[0].id = cudaLaunchAttributeCooperative;
     attr[0].val.cooperative = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    const double* part_arg = ctx->tc_part; const double* side_arg = ctx->tc_side;
+    const double* part_arg = ctx->tc_part;
     const float* shift_arg = ctx->shift;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, side_arg, grid, ctx->tc_red, shift_arg, d_in, pack,
-                               ctx->S, ctx->tc_sync, fin));
+    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, grid, ctx->tc_red, shift_arg, d_in, pack, ctx->S,
+                               ctx->tc_sync, fin));
   }
   ctx->launches += 2;
   return B2_OK;
