@@ -18,7 +18,8 @@
 //            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]      small zero-mean terms: drained once at the end
 //        so D1[:, :128] = hi^T hi, D2[:, :128] = lo^T hi, column 128 = sum v, columns 129/130 = sum v*y'.
 //     --every `drain_rows` rows the two consumer warpgroups fold D1 into this CTA's fp64 partial in global
-//        memory (L2-resident) and restart it from zero; the producer warps keep filling stages meanwhile.
+//        memory (L2-resident; fire-and-forget red.add.f64) and restart it from zero; the producer warps keep filling
+//        stages meanwhile.
 //       The 144 accumulator registers per consumer thread come from the producers (setmaxnreg).
 //
 // Why the shift and the split: the tensor core accumulates fp32 with truncation, so raw (uncentred)
@@ -219,6 +220,9 @@ __device__ __forceinline__ double ld_shared_f64(uint32_t addr) {
   asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr) : "memory");
   return v;
 }
+__device__ __forceinline__ void red_add_f64(double* p, double v) {
+  asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+}
 __device__ __forceinline__ void st_shared_u16(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)v) : "memory");
 }
@@ -415,6 +419,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
     // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
     // column 8 j + 2 (lane % 4) + e (RAWB fills registers 0..63 from the raw tile and 64..71 from E with separate MMAs);
     // the partial is column-major [col][feature].  store(dst, add, val) writes (or adds) val(r, col, h) for every r.
+    // The add is a fire-and-forget reduction in L2 (red.add.f64, one IEEE fp64 add like `*p += v`): a load-add-store
+    // would stall the consumers for an L2 round trip per few registers, and since every CTA drains after the same
+    // number of tiles, all SMs would stop reading HBM at the same time.  Each element has one writer, whose
+    // store and reductions to it take effect in program order (same-address coherence): the sums are those of `*p += v`.
     double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
     auto store = [&](double* dst, bool add, auto val) {
 #pragma unroll
@@ -422,7 +430,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         const int col = 8 * (r >> 2) + 2 * (lane & 3) + (r & 1), h = (r >> 1) & 1;
         const double v = val(r, col, h);
         double* p = dst + (size_t)col * kTcM + 8 * h;
-        if (add) *p += v;
+        if (add) red_add_f64(p, v);
         else *p = v;
       }
     };
