@@ -24,9 +24,25 @@ constexpr size_t kXchgBytes = kXchgDataDoubles * sizeof(double) + 256;      // +
 // ---- tensor-core Gram kernel geometry (gram_tc.cu) --------------------------------------
 constexpr int kTcRows = 64;              // rows of X per pipeline stage (4 MMA K-steps of 16)
 constexpr int kTcM = 128;                // MMA M: feature index (zero padded)
-constexpr int kTcN = 144;                // MMA N: 128 feature columns (hi) + 16 extra columns [1, y_hi, y_lo, 0...]
-constexpr int kTcAccCols = 2 * kTcN;     // two accumulators: A = hi and A = lo against the same B = [hi | E]
-constexpr int kTcAccElems = kTcM * kTcAccCols;  // fp32 accumulators drained per chunk (36 864)
+constexpr int kTcEMax = 16;              // extra columns E = [1, y'_hi, y'_lo] per packed row: 3 * pack <= 16
+// Width of the E block the MMAs cover: 8 columns hold up to pack = 2, 16 up to pack = 5 (kMaxPack).
+inline int tc_e_width(int pack) { return pack >= 3 ? 16 : 8; }
+// The per-CTA partial of the tensor-core Gram kernel holds, in fp64, exactly the accumulator entries the fold reads.
+// Accumulator 0 is D1 = hi^T [hi | E] (RAWB: v^T-exact [x | E], lo added in), accumulator 1 is D2 = lo^T [hi | E]; row i
+// is a feature (A side), column j < 128 a feature and j = 128 + e an E column (B side).  With `ew` E columns:
+//   [0, kTcTri)                       D1, i <= j < 128: the upper triangle, packed column by column
+//   [kTcTri, kTcTri + ew * 128)       D1, E columns
+//   then (128 + ew) * 128             D2, every column (written only by hi + lo operands without RAWB)
+// The entries a launch writes are the prefix [0, tc_part_elems(ew, d2)).
+constexpr int kTcTri = kTcM * (kTcM + 1) / 2;   // 8256
+__host__ __device__ constexpr int tc_part_index(int acc, int i, int j, int ew) {
+  return acc == 0 ? (j < kTcM ? j * (j + 1) / 2 + i : kTcTri + (j - kTcM) * kTcM + i)
+                  : kTcTri + ew * kTcM + j * kTcM + i;
+}
+__host__ __device__ constexpr int tc_part_elems(int ew, bool d2) {
+  return kTcTri + ew * kTcM + (d2 ? (kTcM + ew) * kTcM : 0);
+}
+constexpr int kTcAccElems = tc_part_elems(kTcEMax, true);   // stride of one CTA's partial (28 736)
 constexpr int kTcSums = 3;               // per-CTA CUDA-core sums: sum y', sum y'^2, rows used
 // ctx->tc_part of a Gram launch on n_ctas CTAs: [n_ctas][kTcAccElems] fp64 accumulators, then [n_ctas][kTcSums] sums.
 // The finalize locates the sums through its n_ctas, which must equal the Gram grid.  Allocated for n_ctas = sm_count.

@@ -12,15 +12,18 @@
 //     --> operands, K-major canonical layout (8 x 16 B core matrices, no swizzle; one 16-byte chunk =
 //         8 consecutive rows of X for one feature), per 8-row K group:
 //            rows j = 0..127 hi | 128..143 E | 144..271 lo          (B = [hi | E], A = hi or A = lo)
-//     --wgmma.mma_async m64n144k16 (bf16 x bf16 -> fp32 in registers); warpgroup c (c = 0, 1) owns features
-//       64c..64c+63 of both accumulators, two wgmma per K step of 16 rows:
-//            D1[i][j] += sum_r hi[r][i] * [hi | E][r][j]      drained every `drain_rows` rows
-//            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]      small zero-mean terms: drained once at the end
-//        so D1[:, :128] = hi^T hi, D2[:, :128] = lo^T hi, column 128 = sum v, columns 129/130 = sum v*y'.
-//     --every `drain_rows` rows the two consumer warpgroups fold D1 into this CTA's fp64 partial in global
-//        memory (L2-resident; fire-and-forget red.add.f64) and restart it from zero; the producer warps keep filling
-//        stages meanwhile.
-//       The 144 accumulator registers per consumer thread come from the producers (setmaxnreg).
+//     --wgmma.mma_async (bf16 x bf16 -> fp32 in registers); warpgroup c (c = 0, 1) owns features 64c..64c+63 (A side),
+//       two wgmma per K step of 16 rows, EW = 8 E columns (16 for rows packed 3 or more to a super-row):
+//            D1[i][j] += sum_r hi[r][i] * [hi | E][r][j], j >= 64c   m64n(128 - 64c + EW): hi^T hi is symmetric, so
+//                                                                     warpgroup 1 skips the block warpgroup 0 has
+//                                                                     transposed; drained every `drain_rows` rows
+//            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]             m64n(128 + EW): small zero-mean terms, drained
+//                                                                     once at the end
+//        so D1[:, :128] = hi^T hi (i <= j), D2[:, :128] = lo^T hi, column 128 = sum v, columns 129/130 = sum v*y'.
+//     --every `drain_rows` rows the two consumer warpgroups fold the entries of D1 the fold reads (i <= j, and E) into
+//        this CTA's fp64 partial in global memory (L2-resident; fire-and-forget red.add.f64; layout: tc_part_index)
+//        and restart it from zero; the producer warps keep filling stages meanwhile.
+//       The accumulator registers (136 or 144 per thread of warpgroup 0) come from the producers (setmaxnreg).
 //
 // Why the shift and the split: the tensor core accumulates fp32 with truncation, so raw (uncentred)
 // second moments cannot reach the 1e-4 coefficient tolerance; after the shift the Gram is ~diagonal and
@@ -28,7 +31,8 @@
 // accurate to ~2^-17 relative (lo*lo is dropped).
 //
 // The shift c comes from gram_shift.cu.  tc_finalize_kernel sums the per-CTA partials in a fixed order
-// (deterministic), undoes the shift in fp64 and adds the result to the context's raw statistic S = [X 1 y]^T [X 1 y].
+// (deterministic), reading only the entries this launch wrote, undoes the shift in fp64 and adds the result to the
+// context's raw statistic S = [X 1 y]^T [X 1 y].
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
@@ -52,7 +56,6 @@ constexpr int kEWarp = kFirstXformWarp + 1;        // also writes E and sums y' 
 static_assert(kFirstXformWarp + kXformWarps == kThreads / 32, "warp roles");
 constexpr int kProducers = kXformWarps;            // arrivals that fill an operand stage
 constexpr int kConsumerWarps = 4 * kConsumerWGs;   // arrivals that free an operand stage
-constexpr int kAccRegs = kTcN / 2;                 // fp32 accumulator registers per thread (64 x 144 per warpgroup)
 constexpr int kKGroups = kTcRows / 8;              // 8-row K groups per stage
 constexpr uint32_t kRawStageBytes = kTcRows * kMaxD * 4;      // 32768 (fp32, D = 128)
 constexpr uint32_t kOpSBO = 128;                              // bytes between 8-row j groups (core matrices along M/N)
@@ -89,7 +92,7 @@ struct TcGeo {
   static constexpr uint32_t kOffESum = kOffShift + (kMaxD + 4) * 4;    // kEWarp's per-lane fp64 sums [3][32]
   static constexpr uint32_t kSmemBytes = kOffESum + 3 * 32 * 8 + 1024;  // + alignment slack (~205 KB)
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
-  // setmaxnreg split of the 64 K-register file (128 x 512 threads): 144 fp32 accumulators per consumer thread.  A
+  // setmaxnreg split of the 64 K-register file (128 x 512 threads): up to 144 fp32 accumulators per consumer thread.  A
   // transform lane holds 16 values of two features and, at runtime d, eight row addresses: 64 registers.  RAWB's
   // consumers also hold the raw-tile descriptors and need 200, which leaves its transform (fixed pitch) 56.
   static constexpr uint32_t kConsumerRegs = RAWB ? 200 : 192, kProducerRegs = RAWB ? 56 : 64;
@@ -135,65 +138,101 @@ __device__ __forceinline__ void fence_regs(float (&r)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-// D[64 x 144] (+)= A[64 x 16] * B[16 x 144]: bf16 operands from shared memory (both K-major), fp32 accumulators in
-// registers (wgmma fragment layout); scale_d = 0 overwrites D.  Issued by all 128 threads of a warpgroup.
-__device__ __forceinline__ void wgmma_m64n144k16(float (&d)[72], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]: bf16 operands from shared memory, A K-major; B K-major (TB = 0) or MN-major
+// (TB = 1: the raw 128B-swizzled TMA tile).  fp32 accumulators d[0 .. N/2) in registers (wgmma fragment layout);
+// scale_d = 0 overwrites D.  Issued by all 128 threads of a warpgroup.
+template <int N, int TB>
+__device__ __forceinline__ void wgmma(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d);
+#define B2_ACC4(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3])
+#define B2_ACC8(o) B2_ACC4(o), B2_ACC4(o + 4)
+template <>
+__device__ __forceinline__ void wgmma<8, 0>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %74, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n144k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
-      " %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-      " %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, "
-      " %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, "
-      " %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, "
-      "%72, %73, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3}, "
+      "%4, %5, p, 1, 1, 0, 0;\n\t}"
+      : B2_ACC4(0)
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// D[64 x 128] (+)= A[64 x 16] * B[16 x 128]: A K-major, B MN-major (the raw 128B-swizzled TMA tile); d[0..63] are
-// registers 0..63 of an m64n144 fragment (its columns 0..127)
-__device__ __forceinline__ void wgmma_m64n128k16_bmn(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+template <>
+__device__ __forceinline__ void wgmma<72, 0>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %38, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n72k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35}, "
+      "%36, %37, p, 1, 1, 0, 0;\n\t}"
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24), B2_ACC4(32)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma<80, 0>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39}, "
+      "%40, %41, p, 1, 1, 0, 0;\n\t}"
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24), B2_ACC8(32)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma<136, 0>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %70, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n136k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67}, "
+      "%68, %69, p, 1, 1, 0, 0;\n\t}"
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24), B2_ACC8(32), B2_ACC8(40), B2_ACC8(48), B2_ACC8(56), B2_ACC4(64)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma<144, 0>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n144k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71}, "
+      "%72, %73, p, 1, 1, 0, 0;\n\t}"
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24), B2_ACC8(32), B2_ACC8(40), B2_ACC8(48), B2_ACC8(56), B2_ACC8(64)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma<64, 1>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 1;\n\t}"
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma<128, 1>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
       "%64, %65, p, 1, 1, 0, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : B2_ACC8(0), B2_ACC8(8), B2_ACC8(16), B2_ACC8(24), B2_ACC8(32), B2_ACC8(40), B2_ACC8(48), B2_ACC8(56)
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]: both K-major (B = the E columns); d[0..7] are registers 64..71 of an
-// m64n144 fragment (its columns 128..143)
-__device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
-      "%8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(adesc), "l"(bdesc), "r"(scale_d));
-}
+#undef B2_ACC8
+#undef B2_ACC4
 // MN-major, 128B-swizzled descriptor of the raw bf16 tile of the D = 128 bf16 path: two TMA boxes of [64 rows][64
 // features] (128-byte rows, 8-row swizzle atoms of 1024 bytes); LBO = bytes from features 0..63 to 64..127 (one box),
 // SBO = bytes from one 8-row K group to the next
@@ -220,8 +259,15 @@ __device__ __forceinline__ double ld_shared_f64(uint32_t addr) {
   asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr) : "memory");
   return v;
 }
-__device__ __forceinline__ void red_add_f64(double* p, double v) {
-  asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+// *p += v (add, a fire-and-forget reduction in L2) or *p = v, where `on`: a predicated instruction, not a branch -- a
+// divergent path around the registers wgmma owns makes ptxas serialise the wgmma
+__device__ __forceinline__ void put_f64(double* p, double v, bool add, bool on) {
+  if (add)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p red.global.add.f64 [%0], %1;\n\t}"
+                 ::"l"(p), "d"(v), "r"((uint32_t)on) : "memory");
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.f64 [%0], %1;\n\t}"
+                 ::"l"(p), "d"(v), "r"((uint32_t)on) : "memory");
 }
 __device__ __forceinline__ void st_shared_u16(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)v) : "memory");
@@ -237,19 +283,20 @@ __device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_
 
 // ------------------------------------------------------------------------------------------
 // finalize: the per-CTA partials reduced into
-//   red[col * 128 + i], col in [0, 288):  col < 144: D1 (A = hi), col >= 144: D2 (A = lo), columns of [hi | E]
+//   red[0 .. n_acc)                    : the accumulator entries a launch writes (tc_part_index, b2_internal.cuh)
 //   red[kTcAccElems + 0..2]            : sum y', sum y'^2, rows used (the E warp's CUDA-core sums)
-// Element idx of CTA c of an n_ctas grid sits at part[c * kTcAccElems + idx] (the accumulators) or, from kTcAccElems on,
-// at part[n_ctas * kTcAccElems + c * kTcSums + idx - kTcAccElems] (the sums, behind all accumulators, so that every
-// CTA's accumulators keep the kTcAccElems stride).
+// Entry idx < n_acc of CTA c of an n_ctas grid sits at part[c * kTcAccElems + idx]; sum s at
+// part[n_ctas * kTcAccElems + c * kTcSums + s] (behind all accumulators, so that every CTA's accumulators keep the
+// kTcAccElems stride).  Entries from n_acc to kTcAccElems were not written by this launch and are never read.
 // ------------------------------------------------------------------------------------------
-constexpr int kRedElems = kTcAccElems + kTcSums;
+constexpr int kRedElems = kTcAccElems + kTcSums;   // the most elements a reduce covers
 
-// Sum over the CTAs of elements [e0, e1) of the per-CTA partials.  4 threads per element: thread (e, q) sums the q-th
-// quarter of the CTAs with 8 loads in flight (the loads are the latency: a serial walk over the CTAs costs one L2
-// round trip each, ~140 ns per CTA), the quarters are combined in the fixed order 0..3 -> deterministic.  `quarter`:
-// shared scratch of 4 * (blockDim.x / 4) doubles.  Call with the whole block.
-__device__ __forceinline__ void tc_reduce_range(const double* part, int n_ctas, double* red, int e0, int e1,
+// Sum over the CTAs of elements [e0, e1) of the n_acc + kTcSums written elements: element idx < n_acc is accumulator
+// entry idx, element n_acc + s is sum s.  4 threads per element: thread (e, q) sums the q-th quarter of the CTAs with
+// 8 loads in flight (the loads are the latency: a serial walk over the CTAs costs one L2 round trip each, ~140 ns per
+// CTA), the quarters are combined in the fixed order 0..3 -> deterministic.  `quarter`: shared scratch of
+// 4 * (blockDim.x / 4) doubles.  Call with the whole block.
+__device__ __forceinline__ void tc_reduce_range(const double* part, int n_ctas, int n_acc, double* red, int e0, int e1,
                                                 double* quarter) {
   const int epb = blockDim.x >> 2;                 // elements per pass
   const int e = threadIdx.x % epb, q = threadIdx.x / epb;
@@ -257,9 +304,9 @@ __device__ __forceinline__ void tc_reduce_range(const double* part, int n_ctas, 
   const int c0 = q * per, c1 = (c0 + per < n_ctas) ? c0 + per : n_ctas;
   for (int base = e0; base < e1; base += epb) {
     const int idx = base + e;
+    const bool sum = idx >= n_acc;
     if (idx < e1) {
-      const bool sum = idx >= kTcAccElems;
-      const double* src = sum ? part + (size_t)n_ctas * kTcAccElems + (idx - kTcAccElems) : part + idx;
+      const double* src = sum ? part + (size_t)n_ctas * kTcAccElems + (idx - n_acc) : part + idx;
       const size_t stride = sum ? kTcSums : kTcAccElems;                        // from one CTA to the next
       double acc[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       int c = c0;
@@ -271,7 +318,9 @@ __device__ __forceinline__ void tc_reduce_range(const double* part, int n_ctas, 
       quarter[q * epb + e] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
     }
     __syncthreads();
-    if (q == 0 && idx < e1) red[idx] = ((quarter[e] + quarter[epb + e]) + quarter[2 * epb + e]) + quarter[3 * epb + e];
+    if (q == 0 && idx < e1)
+      red[sum ? kTcAccElems + (idx - n_acc) : idx] =
+          ((quarter[e] + quarter[epb + e]) + quarter[2 * epb + e]) + quarter[3 * epb + e];
     __syncthreads();
   }
 }
@@ -301,22 +350,26 @@ __device__ __forceinline__ void grid_barrier(unsigned int* ctr) {
 // sub-row blk is super-feature blk*d + a, and its E columns are 128 + 3*blk (+0 ones, +1 y'_hi, +2 y'_lo).
 // The true statistic is the sum over blk of the diagonal (blk, blk) blocks.
 // Returns the contribution of this launch to S[idx]; c[j] = the shift of feature j, c[kMaxD] = the shift of y.
-__device__ __forceinline__ double tc_fold_value(const double* red, const double* c, int d, int pack, int idx) {
+// ew: the E columns of the launch; d2: it wrote D2 (hi + lo operands without RAWB), whose lo^T hi terms enter in both
+// orientations.  Otherwise D1 already holds sum v_a v_b for a <= b (one operand, or RAWB with lo added in).
+__device__ __forceinline__ double tc_fold_value(const double* red, const double* c, int d, int pack, int ew, bool d2,
+                                                int idx) {
   const int dp = d + 2;
   const int a = min(idx / dp, idx % dp), b = max(idx / dp, idx % dp);
-  // D1[i][j] = red[j*128 + i], D2[i][j] = red[(144 + j)*128 + i]
-  auto D1 = [&](int i, int j) { return __ldcg(red + (size_t)j * kTcM + i); };
-  auto D2 = [&](int i, int j) { return __ldcg(red + (size_t)(kTcN + j) * kTcM + i); };
+  auto P = [&](int acc, int i, int j) { return __ldcg(red + tc_part_index(acc, i, j, ew)); };
   auto s1 = [&](int i) {                                                     // sum (x_i - c_i)
     double t = 0.0;
-    for (int blk = 0; blk < pack; ++blk) t += D1(blk * d + i, 128 + 3 * blk) + D2(blk * d + i, 128 + 3 * blk);
+    for (int blk = 0; blk < pack; ++blk) {
+      const int r = blk * d + i, e = kTcM + 3 * blk;
+      t += d2 ? P(0, r, e) + P(1, r, e) : P(0, r, e);
+    }
     return t;
   };
   auto sxy = [&](int i) {                                                    // sum (x_i - c_i) y'
     double t = 0.0;
     for (int blk = 0; blk < pack; ++blk) {
-      const int r = blk * d + i, e = 128 + 3 * blk;
-      t += D1(r, e + 1) + D1(r, e + 2) + D2(r, e + 1) + D2(r, e + 2);
+      const int r = blk * d + i, e = kTcM + 3 * blk;
+      t += d2 ? P(0, r, e + 1) + P(0, r, e + 2) + P(1, r, e + 1) + P(1, r, e + 2) : P(0, r, e + 1) + P(0, r, e + 2);
     }
     return t;
   };
@@ -324,7 +377,8 @@ __device__ __forceinline__ double tc_fold_value(const double* red, const double*
     double g = 0.0;
     for (int blk = 0; blk < pack; ++blk) {
       const int ia = blk * d + i, ib = blk * d + j;
-      g += 0.5 * (D1(ia, ib) + D1(ib, ia)) + D2(ia, ib) + D2(ib, ia);
+      const double g1 = P(0, min(ia, ib), max(ia, ib));
+      g += d2 ? g1 + P(1, ia, ib) + P(1, ib, ia) : g1;
     }
     return g;
   };
@@ -343,11 +397,11 @@ __device__ __forceinline__ double tc_fold_value(const double* red, const double*
 // RAWB (bf16 rows, D = 128, no packing): the raw TMA tile itself (128B-swizzled) is the B operand, so the transform
 //   writes only the A operands.  D1[i][j] = sum_r hi[r][i] x[r][j] (raw, unshifted x) and E1[i][e] = sum_r hi[r][i] E[r][e];
 //   the drain subtracts c_j * sum_r hi[r][i] (the ones column of E1), which leaves sum hi_i v_j with the B side exact.
-//   lo has its own accumulators (D2, E2, small zero-mean sums, drained once at the end), stored halved in the feature
-//   columns so that the fold's D2(a,b) + D2(b,a) adds sum lo_a v_b once, symmetrised -- the partial means what the other
-//   variants' partials mean.  The raw stage is
-//   held until the MMAs have read it; masked-out rows are zeroed in it (0 * NaN would poison the sums).
-template <typename T, int DFIX, bool SPLIT, bool RAWB = false>
+//   lo has its own accumulators (small zero-mean sums); since the B side is the exact v, sum v_a v_b = sum hi_a v_b +
+//   sum lo_a v_b for a <= b, so the end of the range adds them, unhalved, into the same D1 entries and writes no D2.
+//   The raw stage is held until the MMAs have read it; masked-out rows are zeroed in it (0 * NaN would poison the sums).
+// EW: the E columns the MMAs cover (tc_e_width: 8 up to pack = 2, 16 beyond; runtime-d kernels are unpacked).
+template <typename T, int DFIX, bool SPLIT, bool RAWB = false, int EW = 8>
 __global__ void __launch_bounds__(kThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                const __grid_constant__ CUtensorMap tmM, int y_map_2d, int has_mask, int keep,
@@ -412,110 +466,128 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   if (warp < kConsumerWarps) {
     // ===== consumers: wgmma into register accumulators, fp64 drain to the CTA's partial in global =====
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G::kConsumerRegs));
-    const int wg = warp >> 2;
-    // no plain instruction may write the accumulators between wgmma (ptxas would serialise them): a chunk restarts D1,
-    // and the first tile starts D2, with scale-d = 0 on its first K step
-    float acc1[kAccRegs], acc2[kAccRegs];
-    // fragment of this thread: register 4j + 2h + e holds row (feature) 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
-    // column 8 j + 2 (lane % 4) + e (RAWB fills registers 0..63 from the raw tile and 64..71 from E with separate MMAs);
-    // the partial is column-major [col][feature].  store(dst, add, val) writes (or adds) val(r, col, h) for every r.
-    // The add is a fire-and-forget reduction in L2 (red.add.f64, one IEEE fp64 add like `*p += v`): a load-add-store
-    // would stall the consumers for an L2 round trip per few registers, and since every CTA drains after the same
-    // number of tiles, all SMs would stop reading HBM at the same time.  Each element has one writer, whose
-    // store and reductions to it take effect in program order (same-address coherence): the sums are those of `*p += v`.
-    double* my_part = part + (size_t)blockIdx.x * kTcAccElems + 64 * wg + 16 * (warp & 3) + (lane >> 2);
-    auto store = [&](double* dst, bool add, auto val) {
+    // Warpgroup WG owns features 64 WG .. 64 WG + 63 (the A side).  hi^T hi is symmetric, so its D1 covers only the
+    // B columns from 64 WG on: [hi rows 64 WG .. 127 | E], kF1 feature columns; in the operand stage those rows and E
+    // are contiguous at stride kOpSBO, so the B descriptor starts at the same address as the warpgroup's A.  D2 (A = lo)
+    // needs both orientations and covers [hi | E] in full, except with RAWB, whose lo sums enter D1 (see above).
+    // One copy of the loop per warpgroup: every wgmma in it has a fixed shape.
+    auto consume = [&](auto wg_c) {
+      constexpr int WG = decltype(wg_c)::value;
+      constexpr int kF1 = kTcM - 64 * WG;                        // D1 feature columns: 64 WG .. 127
+      constexpr int kF2 = RAWB ? kF1 : kTcM;                     // D2 feature columns: 64 WG .. 127 or 0 .. 127
+      constexpr int kC1 = 64 * WG;                               // D1's partial column of accumulator column 0
+      constexpr int kR1 = (kF1 + EW) / 2, kR2 = (kF2 + EW) / 2;  // fp32 accumulator registers per thread
+      // no plain instruction may write the accumulators between wgmma (ptxas would serialise them): a chunk restarts D1,
+      // and the first tile starts D2, with scale-d = 0 on its first K step
+      float acc1[kR1], acc2[kR2];
+      // fragment of this thread: register 4j + 2h + e holds row (feature) 64 WG + 16 (warp % 4) + lane / 4 + 8 h,
+      // accumulator column 8 j + 2 (lane % 4) + e, partial column col0 + that (an E column from 128 on).
+      // store(dst_acc, col0, add, val) writes (or adds) val(r, col, h) for every register r whose element the fold reads
+      // from accumulator dst_acc: D1's upper triangle i <= j and E columns, every D2 column.
+      // The add is a fire-and-forget reduction in L2 (red.add.f64, one IEEE fp64 add like `*p += v`): a load-add-store
+      // would stall the consumers for an L2 round trip per few registers, and since every CTA drains after the same
+      // number of tiles, all SMs would stop reading HBM at the same time.  Each element has one writer, whose
+      // store and reductions to it take effect in program order (same-address coherence): the sums are those of `*p += v`.
+      double* my_part = part + (size_t)blockIdx.x * kTcAccElems;
+      auto store = [&](auto n_regs, int dst_acc, int col0, bool add, auto val) {
+        // the lane is re-read here: partial indices computed from a kept one are hoisted out of the tile loop and hold a
+        // register each
+        const int ln = (int)lane_id(), row0 = 64 * WG + 16 * (warp & 3) + (ln >> 2);
 #pragma unroll
-      for (int r = 0; r < kAccRegs; ++r) {
-        const int col = 8 * (r >> 2) + 2 * (lane & 3) + (r & 1), h = (r >> 1) & 1;
-        const double v = val(r, col, h);
-        double* p = dst + (size_t)col * kTcM + 8 * h;
-        if (add) red_add_f64(p, v);
-        else *p = v;
-      }
-    };
-    // RAWB's feature columns carry the raw x: sum_r a_i x_j - c_j sum_r a_i = sum_r a_i v_j, where sum_r a_i is E's ones
-    // column (registers 64 / 66, held by lane 4 * (lane / 4)); D2 stores them halved (x_scale = 0.5, see above)
-    auto drain = [&](const float (&acc)[kAccRegs], double* dst, bool add, double x_scale) {
-      if constexpr (RAWB) {
-        const double s1[2] = {(double)__shfl_sync(0xffffffffu, acc[64], lane & ~3),
-                              (double)__shfl_sync(0xffffffffu, acc[66], lane & ~3)};
-        store(dst, add, [&](int r, int col, int h) {
-          return r < 64 ? x_scale * ((double)acc[r] - (double)shift_s[col] * s1[h]) : (double)acc[r];
-        });
-      } else {
-        store(dst, add, [&](int r, int, int) { return (double)acc[r]; });
-      }
-    };
-    // the stages of a tile: RAWB's consumers also hold its raw stage, the B operand of its MMAs
-    auto release = [&](int tile) {
-      mbar_arrive(bar_op_empty + 8 * (tile % kOpStages));
-      if constexpr (RAWB) mbar_arrive(bar_raw_empty + 8 * (tile % kRawStages));
-    };
-    const uint32_t a_off = (uint32_t)wg * 8 * kOpSBO;      // this warpgroup's 64 features of A
-    int os = 0, held = -1, in_chunk = 0;                   // held: the tile whose stages wait for their MMAs
-    uint32_t oph = 0;
-    bool first_chunk = true;
-    for (int it = 0; it < my_tiles; ++it) {
-      mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
-      const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
-        const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
-        const uint64_t hi_desc = make_smem_desc(k_addr + a_off), lo_desc = make_smem_desc(k_addr + kOpLoOff + a_off);
-        const uint32_t sc1 = (in_chunk > 0 || k2 > 0) ? 1u : 0u, sc2 = (it > 0 || k2 > 0) ? 1u : 0u;
-        if constexpr (RAWB) {
-          // rows 16 k2 .. 16 k2 + 15 of the raw tile, and E
-          const uint64_t x_desc =
-              make_raw_desc(sbase + kOffRaw + (uint32_t)(it % kRawStages) * kRawStageBytes + k2 * 16 * 128);
-          const uint64_t e_desc = make_smem_desc(k_addr + kOpEOff);
-          wgmma_m64n128k16_bmn(acc1, hi_desc, x_desc, sc1);
-          wgmma_m64n16k16(acc1 + 64, hi_desc, e_desc, sc1);
-          if constexpr (SPLIT) {
-            wgmma_m64n128k16_bmn(acc2, lo_desc, x_desc, sc2);
-            wgmma_m64n16k16(acc2 + 64, lo_desc, e_desc, sc2);
-          }
-        } else {
-          const uint64_t b_desc = make_smem_desc(k_addr);                               // [hi | E]
-          if (!(dbg & 2u)) wgmma_m64n144k16(acc1, hi_desc, b_desc, sc1);                // A = hi
-          if (SPLIT && !(dbg & 3u)) wgmma_m64n144k16(acc2, lo_desc, b_desc, sc2);       // A = lo
+        for (int r = 0; r < decltype(n_regs)::value; ++r) {
+          const int col = col0 + 8 * (r >> 2) + 2 * (ln & 3) + (r & 1), h = (r >> 1) & 1, i = row0 + 8 * h;
+          const bool lower = dst_acc == 0 && col < kTcM && i > col;   // D1's lower triangle: (col, i) holds it
+          put_f64(my_part + tc_part_index(dst_acc, i, col, EW), val(r, col, h), add, !lower);
         }
+      };
+      // RAWB's feature columns carry the raw x: sum_r a_i x_j - c_j sum_r a_i = sum_r a_i v_j, where sum_r a_i is E's ones
+      // column (registers kF / 2 and kF / 2 + 2, held by lane 4 * (lane / 4))
+      auto drain = [&](const auto& acc, int dst_acc, int col0, bool add) {
+        constexpr int kR = sizeof(acc) / sizeof(float);
+        if constexpr (RAWB) {
+          constexpr int kF = 2 * kR - EW;
+          const double s1[2] = {(double)__shfl_sync(0xffffffffu, acc[kF / 2], lane & ~3),
+                                (double)__shfl_sync(0xffffffffu, acc[kF / 2 + 2], lane & ~3)};
+          store(std::integral_constant<int, kR>{}, dst_acc, col0, add, [&](int r, int col, int h) {
+            return col < kTcM ? (double)acc[r] - (double)shift_s[col] * s1[h] : (double)acc[r];
+          });
+        } else {
+          store(std::integral_constant<int, kR>{}, dst_acc, col0, add, [&](int r, int, int) { return (double)acc[r]; });
+        }
+      };
+      // the stages of a tile: RAWB's consumers also hold its raw stage, the B operand of its MMAs
+      auto release = [&](int tile) {
+        mbar_arrive(bar_op_empty + 8 * (tile % kOpStages));
+        if constexpr (RAWB) mbar_arrive(bar_raw_empty + 8 * (tile % kRawStages));
+      };
+      constexpr uint32_t a_off = (uint32_t)WG * 8 * kOpSBO;      // this warpgroup's 64 features of A
+      int os = 0, held = -1, in_chunk = 0;                       // held: the tile whose stages wait for their MMAs
+      uint32_t oph = 0;
+      bool first_chunk = true;
+      for (int it = 0; it < my_tiles; ++it) {
+        mbar_wait(bar_op_full + 8 * os, oph, wait_ns);
+        const uint32_t op_addr = sbase + kOffOp + os * kOpStageBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k2 = 0; k2 < kTcRows / 16; ++k2) {
+          const uint32_t k_addr = op_addr + k2 * 2 * kOpLBO;
+          const uint64_t hi_desc = make_smem_desc(k_addr + a_off), lo_desc = make_smem_desc(k_addr + kOpLoOff + a_off);
+          const uint32_t sc1 = (in_chunk > 0 || k2 > 0) ? 1u : 0u, sc2 = (it > 0 || k2 > 0) ? 1u : 0u;
+          if constexpr (RAWB) {
+            // rows 16 k2 .. 16 k2 + 15 of the raw tile from box WG (features 64 WG on), and E
+            const uint64_t x_desc = make_raw_desc(sbase + kOffRaw + (uint32_t)(it % kRawStages) * kRawStageBytes +
+                                                  (uint32_t)WG * kRawBoxBytes + k2 * 16 * 128);
+            const uint64_t e_desc = make_smem_desc(k_addr + kOpEOff);
+            if (!(dbg & 2u)) {
+              wgmma<kF1, 1>(acc1, hi_desc, x_desc, sc1);
+              wgmma<EW, 0>(acc1 + kF1 / 2, hi_desc, e_desc, sc1);
+            }
+            if (SPLIT && !(dbg & 3u)) {
+              wgmma<kF2, 1>(acc2, lo_desc, x_desc, sc2);
+              wgmma<EW, 0>(acc2 + kF2 / 2, lo_desc, e_desc, sc2);
+            }
+          } else {
+            if (!(dbg & 2u)) wgmma<kF1 + EW, 0>(acc1, hi_desc, make_smem_desc(k_addr + a_off), sc1);   // [hi_WG.. | E]
+            if (SPLIT && !(dbg & 3u)) wgmma<kF2 + EW, 0>(acc2, lo_desc, make_smem_desc(k_addr), sc2);   // [hi | E]
+          }
+        }
+        wgmma_commit();
+        const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
+        // the previous tile's MMAs are complete after wait_group 1 (this tile's too after wait_group 0): free their
+        // stages; the last tile of the range is always `last`, so the accumulators are settled when the loop ends
+        if (last) {
+          wgmma_wait<0>();
+          fence_regs(acc1);
+          if constexpr (SPLIT) fence_regs(acc2);
+        } else {
+          wgmma_wait<1>();
+        }
+        if (lane == 0) {
+          if (held >= 0) release(held);
+          if (last) release(it);
+        }
+        held = last ? -1 : it;
+        if (last) {
+          drain(acc1, 0, kC1, !first_chunk);                     // D1 of this chunk
+          first_chunk = false;
+          in_chunk = 0;
+        } else {
+          ++in_chunk;
+        }
+        if (++os == kOpStages) { os = 0; oph ^= 1; }
       }
-      wgmma_commit();
-      const bool last = (in_chunk == chunk_tiles - 1) || (it == my_tiles - 1);
-      // the previous tile's MMAs are complete after wait_group 1 (this tile's too after wait_group 0): free their stages;
-      // the last tile of the range is always `last`, so the accumulators are settled when the loop ends
-      if (last) {
-        wgmma_wait<0>();
-        fence_regs(acc1);
-        if constexpr (SPLIT) fence_regs(acc2);
-      } else {
-        wgmma_wait<1>();
+      wgmma_wait<0>();   // a no-op at run time (see above), but ptxas cannot prove it and would wait inside the loop
+      // A = lo accumulated over the whole range (small zero-mean sums): D2, or with RAWB added into D1 after its last
+      // drain (same thread, same element: program order)
+      if constexpr (SPLIT) {
+        fence_regs(acc2);
+        drain(acc2, RAWB ? 0 : 1, RAWB ? kC1 : 0, RAWB);
       }
-      if (lane == 0) {
-        if (held >= 0) release(held);
-        if (last) release(it);
-      }
-      held = last ? -1 : it;
-      if (last) {
-        drain(acc1, my_part, !first_chunk, 1.0);           // D1 of this chunk: partial columns [0, 144)
-        first_chunk = false;
-        in_chunk = 0;
-      } else {
-        ++in_chunk;
-      }
-      if (++os == kOpStages) { os = 0; oph ^= 1; }
-    }
-    wgmma_wait<0>();     // a no-op at run time (see above), but ptxas cannot prove it and would wait inside the loop
-    // D2 (A = lo) accumulated over the whole range (small zero-mean sums): partial columns [144, 288)
-    double* my_part2 = my_part + (size_t)kTcN * kTcM;
-    if constexpr (SPLIT) {
-      fence_regs(acc2);
-      drain(acc2, my_part2, false, 0.5);
-    } else {
-      store(my_part2, false, [](int, int, int) { return 0.0; });
-    }
+    };
+    // branch on a shuffled warp index: ptxas serialises the wgmma of both copies when the branch depends on the thread
+    // index directly (it cannot tell that the condition is uniform over each warpgroup)
+    if (__shfl_sync(0xffffffffu, warp, 0) >= 4) consume(std::integral_constant<int, 1>{});
+    else consume(std::integral_constant<int, 0>{});
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(G::kProducerRegs));
     // ===== producers: eight transform warps, two on each SM sub-partition =====
@@ -702,20 +774,22 @@ struct TcFinal {
 // it there the hot role loops carry its registers and
 // code; a separate launch keeps them lean.
 constexpr int kFinalizeThreads = 1024;                           // 4 threads per element of the partials
-constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinalizeThreads / 4);   // 145: one pass
+constexpr int kFinalizeCtas = (kRedElems + kFinalizeThreads / 4 - 1) / (kFinalizeThreads / 4);   // 113: one pass
 
 __global__ void __launch_bounds__(kFinalizeThreads, 1)
 tc_finalize_kernel(const double* part, int n_ctas, double* red, const float* __restrict__ shift, int d, int pack,
-                   double* S, unsigned int* sync, const TcFinal fin) {
+                   int ew, int d2, double* S, unsigned int* sync, const TcFinal fin) {
   __shared__ double quarter[kFinalizeThreads];
   __shared__ double c_s[kMaxD + 1];                              // the shift as fp64 (c_s[kMaxD]: c_y)
   for (int j = threadIdx.x; j <= kMaxD; j += blockDim.x) c_s[j] = (double)shift[j];
   {
     constexpr int epb = kFinalizeThreads / 4;                    // elements per pass of a CTA
-    const int per = (((kRedElems + (int)gridDim.x - 1) / (int)gridDim.x) + epb - 1) / epb * epb;
+    const int n_acc = tc_part_elems(ew, d2 != 0);                // the entries the Gram launch wrote
+    const int n_red = n_acc + kTcSums;
+    const int per = (((n_red + (int)gridDim.x - 1) / (int)gridDim.x) + epb - 1) / epb * epb;
     const int e0 = (int)blockIdx.x * per;
-    const int e1 = e0 + per < kRedElems ? e0 + per : kRedElems;
-    if (e0 < kRedElems) tc_reduce_range(part, n_ctas, red, e0, e1, quarter);
+    const int e1 = e0 + per < n_red ? e0 + per : n_red;
+    if (e0 < n_red) tc_reduce_range(part, n_ctas, n_acc, red, e0, e1, quarter);
   }
   grid_barrier(sync + 0);
   {
@@ -723,7 +797,7 @@ tc_finalize_kernel(const double* part, int n_ctas, double* red, const float* __r
     const int total = dp * dp;
     const size_t slot = xchg_slot_offset(fin.epoch, fin.rank);
     for (int idx = (int)(blockIdx.x * blockDim.x + threadIdx.x); idx < total; idx += (int)(gridDim.x * blockDim.x)) {
-      const double val = tc_fold_value(red, c_s, d, pack, idx);
+      const double val = tc_fold_value(red, c_s, d, pack, ew, d2 != 0, idx);
       const double sv = fin.assign ? val : S[idx] + val;
       S[idx] = sv;
       if (fin.n_ranks > 1) xchg_store_all(fin.peers, fin.n_ranks, slot, idx, sv);
@@ -907,13 +981,20 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
 #else
   constexpr uint32_t dbg = 0u;
 #endif
+  // the E columns the MMAs cover, and whether the launch writes D2 (hi + lo operands without RAWB): the finalize reads
+  // exactly the partial entries these two select
+  const bool split = ctx->precision == B2_PRECISION_SPLIT;
+  const int ew = tc_e_width(pack);
+  const bool d2 = split && !rawb;
   decltype(&gram_tc_kernel<float, 0, false>) kernel = nullptr;
   uint32_t smem = TcGeo<false>::kSmemBytes;
   with_rows(x_dtype, X, [&](auto* Xr) {
     using T = row_t<decltype(Xr)>;
-    return with_int<0, 1>(ctx->precision == B2_PRECISION_SPLIT, [&](auto SP) {
+    return with_int<0, 1>(split, [&](auto SP) {
       constexpr bool kSplit = decltype(SP)::value;
-      kernel = d == 128 ? gram_tc_kernel<T, 128, kSplit> : gram_tc_kernel<T, 0, kSplit>;
+      if (d != 128) kernel = gram_tc_kernel<T, 0, kSplit>;                   // runtime d: never packed (ew = 8)
+      else if (ew == 16) kernel = gram_tc_kernel<T, 128, kSplit, false, 16>;
+      else kernel = gram_tc_kernel<T, 128, kSplit>;
       if constexpr (std::is_same_v<T, __nv_bfloat16>) {
         if (rawb) {
           kernel = gram_tc_kernel<T, 128, kSplit, true>;
@@ -953,8 +1034,8 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     cfg.attrs = attr; cfg.numAttrs = 1;
     const double* part_arg = ctx->tc_part;
     const float* shift_arg = ctx->shift;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, grid, ctx->tc_red, shift_arg, d_in, pack, ctx->S,
-                               ctx->tc_sync, fin));
+    B2_CUDA(cudaLaunchKernelEx(&cfg, tc_finalize_kernel, part_arg, grid, ctx->tc_red, shift_arg, d_in, pack, ew,
+                               d2 ? 1 : 0, ctx->S, ctx->tc_sync, fin));
   }
   ctx->launches += 2;
   return B2_OK;
