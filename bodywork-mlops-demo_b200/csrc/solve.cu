@@ -7,7 +7,7 @@
 //
 //   solve_cholesky_kernel : A = Xc^T Xc + alpha I = L L^T in shared memory, two triangular solves.
 //   solve_spectral_kernel : one-sided Jacobi on A (A V = W, columns of W orthogonal => w_k = lambda_k v_k):
-//                           singular_ = sqrt(lambda) (descending), rank_ = #{sqrt(lambda) > cond * max},
+//                           singular_ = sqrt(max(lambda, 0)) (descending), rank_ = #{singular > cond * max},
 //                           coef = minimum-norm solution = what gelsd returns for rank-deficient X.
 //
 // One CTA: the matrices are <= 128 x 128 fp64 (132 KB with padding) -- latency bound, not a
@@ -508,11 +508,30 @@ solve_spectral_kernel(const double* __restrict__ S, int d, double cond, int fit_
     if (!rotated) break;
     __syncthreads();
   }
-  // eigenvalues = column norms
-  for (int k = threadIdx.x; k < d; k += blockDim.x) {
-    double s2 = 0.0;
-    for (int row = 0; row < d; ++row) s2 += W[k * pitch + row] * W[k * pitch + row];
-    lam[k] = sqrt(s2);
+  // |eigenvalues| = column norms.  The sign is lost in W^T W = V A^2 V^T; it comes back from lambda_k^3 = w_k^T A w_k,
+  // with A formed again from S exactly as build_normal_equations formed it (one warp per column, lane = row of A w_k).
+  // A centred Gram that rounding has made slightly indefinite then reports its negative eigenvalues as 0, as the
+  // eigenvalue kernel and sklearn's gelsd (singular values of the centred rows) do: they are not counted in rank_ and
+  // give no term of the minimum-norm solution.
+  {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5, dp = d + 2;
+    const double n = __ldcg(S + d * dp + d);
+    for (int k = warp; k < d; k += nwarps) {
+      const double* w = W + k * pitch;
+      double s2 = 0.0, cube = 0.0;
+      for (int i = lane; i < d; i += 32) {
+        double aw = 0.0;
+        for (int j = 0; j < d; ++j) aw = fma(__ldcg(S + i * dp + j) - n * mean[i] * mean[j], w[j], aw);
+        s2 = fma(w[i], w[i], s2);
+        cube = fma(w[i], aw, cube);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+        cube += __shfl_xor_sync(0xffffffffu, cube, o);
+      }
+      if (lane == 0) lam[k] = cube > 0.0 ? sqrt(s2) : 0.0;
+    }
   }
   __syncthreads();
   if (threadIdx.x == 0) {

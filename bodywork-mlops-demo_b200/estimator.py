@@ -75,19 +75,37 @@ class B200LinearRegression:
         self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
         self.n_features_in_ = int(d)
 
-    def _spectrum(self, d: int, need_coef: bool):
-        """singular_ / rank_ of the statistic resident in the context (eigenvalues only, b2_solve_eigvals); when the
-        centred Gram is numerically rank deficient (or the factorisation failed) also the minimum-norm coefficients
-        gelsd would return (b2_solve_spectral, device Jacobi)."""
-        ctx = self.ctx
-        sing, rank, rows = ctx.solve_eigvals(cond=self.tol, fit_intercept=self.fit_intercept)
+    def _spectrum(self, d: int) -> int:
+        """singular_ / rank_ of the statistic resident in the context (eigenvalues only, b2_solve_eigvals); returns the
+        number of rows in the statistic."""
+        sing, rank, rows = self.ctx.solve_eigvals(cond=self.tol, fit_intercept=self.fit_intercept)
+        if rows == 0:
+            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
+                             "B200LinearRegression.")
         self.singular_ = sing[: min(rows, d)]
         self.rank_ = int(rank)
-        if (need_coef or (rank < min(rows, d) and self.alpha == 0.0)) and d > 0:
-            coef, b0, sing_j, rank_j = ctx.solve_spectral(cond=self.tol, fit_intercept=self.fit_intercept)
-            self.singular_ = sing_j[: min(rows, d)]
-            self.rank_ = int(rank_j)
-            self._set_solution(coef, b0, d)
+        return rows
+
+    def _solve_statistic(self, d: int, solve, with_spectrum: bool) -> None:
+        """The model of the statistic that ``solve()`` leaves resident in the context; ``solve`` returns the LDL^T
+        solution (coef, intercept) or raises ``LinAlgError`` when a pivot is not positive.
+
+        One rank rule, whichever call produced the statistic: with alpha = 0 the eigenvalue kernel's rank_ decides, and
+        the minimum-norm solution gelsd would return (b2_solve_spectral) replaces the LDL^T solution when
+        rank_ < min(rows, D) -- the factorisation accepts pivots down to 1e-12 of the largest diagonal entry, while
+        sklearn's cond = 1e-6 on the singular values drops eigenvalues below 1e-12 of the largest, so a statistic can
+        pass the first test and still be rank deficient.  With alpha > 0 the ridge solution stands and the spectrum
+        is computed only if ``with_spectrum``; a statistic the factorisation refuses always gets the minimum-norm
+        solution."""
+        try:
+            coef, b0 = solve()
+        except np.linalg.LinAlgError:
+            coef, b0 = None, 0.0
+        if coef is None or self.alpha == 0.0 or with_spectrum:
+            rows = self._spectrum(d)
+            if coef is None or (self.alpha == 0.0 and self.rank_ < min(rows, d)):
+                coef, b0, _, _ = self.ctx.solve_spectral(cond=self.tol, fit_intercept=self.fit_intercept)
+        self._set_solution(coef, b0, d)
 
     def _drop_spectrum(self) -> None:
         for name in ("singular_", "rank_"):
@@ -97,7 +115,10 @@ class B200LinearRegression:
     def fit(self, X, y, row_mask=None, mask_keep: int = 1, with_spectrum: bool = True) -> "B200LinearRegression":
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16).
         ``row_mask`` (uint8 per row) restricts the fit to rows equal to ``mask_keep``.
-        ``with_spectrum=False`` defers ``singular_`` / ``rank_`` (computed on first use, e.g. by ``to_sklearn``)."""
+        ``with_spectrum=False`` defers ``singular_`` / ``rank_`` (computed on first use, e.g. by ``to_sklearn``) when
+        alpha > 0; with alpha = 0 the spectrum decides between the LDL^T and the minimum-norm solution, so it is always
+        computed.  Wherever the spectrum is computed, a fit that keeps no rows (e.g. through ``row_mask``) raises
+        ``ValueError``, as sklearn does for 0 samples."""
         ctx = self.ctx
         owned = []                  # device buffers this call created (float64 host rows: converted on the way up)
         if isinstance(X, native.DeviceArray):
@@ -126,29 +147,26 @@ class B200LinearRegression:
             d = X.shape[1]
         self._S = None
         self._drop_spectrum()
-        singular = False
+
+        def solve():
+            if self.refine == 0:
+                return ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
+            self.n_refine_passes_, self.refine_step_ = 0, 0.0      # the min-norm fallback stays unrefined
+            coef, b0, passes, step = ctx.fit_refined(X, y, row_mask, mask_keep, alpha=self.alpha,
+                                                     fit_intercept=self.fit_intercept, max_passes=self.refine,
+                                                     tol=_REFINE_TOL)
+            self.n_refine_passes_, self.refine_step_ = passes, step
+            if step > _REFINE_TOL:
+                warnings.warn(f"refined fit stopped at step {step:.3e} after {passes} kept correction(s) "
+                              f"(tolerance {_REFINE_TOL:.0e}): more passes may help, or the features are too "
+                              "ill-conditioned for the Gram path's precision", RuntimeWarning, stacklevel=4)
+            return coef, b0
         try:
-            if self.refine > 0:
-                self.n_refine_passes_, self.refine_step_ = 0, 0.0      # the min-norm fallback below stays unrefined
-                coef, b0, passes, step = ctx.fit_refined(X, y, row_mask, mask_keep, alpha=self.alpha,
-                                                         fit_intercept=self.fit_intercept, max_passes=self.refine,
-                                                         tol=_REFINE_TOL)
-                self.n_refine_passes_, self.refine_step_ = passes, step
-                if step > _REFINE_TOL:
-                    warnings.warn(f"refined fit stopped at step {step:.3e} after {passes} kept correction(s) "
-                                  f"(tolerance {_REFINE_TOL:.0e}): more passes may help, or the features are too "
-                                  "ill-conditioned for the Gram path's precision", RuntimeWarning, stacklevel=2)
-            else:
-                coef, b0 = ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
-            self._set_solution(coef, b0, d)
-        except np.linalg.LinAlgError:
-            singular = True         # rank deficient and alpha == 0: the minimum-norm solution gelsd would return
+            self._solve_statistic(d, solve, with_spectrum)
         finally:
             for a in owned:
                 a.free()
         self._serial = ctx.serial
-        if with_spectrum or singular:
-            self._spectrum(d, need_coef=singular)
         return self
 
     def _no_refine(self, what: str) -> None:
@@ -172,16 +190,9 @@ class B200LinearRegression:
             ctx.gram_reset(d)          # first tranche of this estimator
         ctx.gram_accumulate(Xh, y)
         self._drop_spectrum()
-        singular = False
-        try:
-            coef, b0 = ctx.solve(alpha=self.alpha, fit_intercept=self.fit_intercept)
-            self._set_solution(coef, b0, d)
-        except np.linalg.LinAlgError:
-            singular = True
+        self._solve_statistic(d, lambda: ctx.solve(alpha=self.alpha, fit_intercept=self.fit_intercept), with_spectrum)
         self._S = ctx.gram_export()
         self._serial = ctx.serial
-        if with_spectrum or singular:
-            self._spectrum(d, need_coef=singular)
         return self
 
     def solve_resident(self, d: int, S: Optional[np.ndarray] = None) -> "B200LinearRegression":
@@ -191,11 +202,7 @@ class B200LinearRegression:
         ctx = self.ctx
         self._drop_spectrum()
         self._S = S
-        try:
-            coef, b0 = ctx.solve(alpha=self.alpha, fit_intercept=self.fit_intercept)
-            self._set_solution(coef, b0, d)
-        except np.linalg.LinAlgError:
-            self._spectrum(d, need_coef=True)
+        self._solve_statistic(d, lambda: ctx.solve(alpha=self.alpha, fit_intercept=self.fit_intercept), False)
         self._serial = ctx.serial
         return self
 
@@ -208,7 +215,7 @@ class B200LinearRegression:
         elif self._serial != ctx.serial:
             raise RuntimeError("singular_ / rank_ were deferred (with_spectrum=False) and the statistic of this fit is no "
                                "longer resident in the context: refit, or fit with with_spectrum=True")
-        self._spectrum(self.n_features_in_, need_coef=False)
+        self._spectrum(self.n_features_in_)
         self._serial = ctx.serial
 
     # -- predict -------------------------------------------------------------------------------------

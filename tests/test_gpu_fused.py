@@ -491,16 +491,22 @@ def test_pageable_host_rows_take_the_bounce_ring_and_equal_pinned_rows(ctx):
         a.free()
 
 
-def test_estimators_sharing_a_context_do_not_share_a_statistic(ctx):
+def test_estimators_sharing_a_context_do_not_share_a_statistic_or_a_deferred_spectrum(ctx):
+    from sklearn.linear_model import LinearRegression
     Xa, ya = orc.generate_dataset(6000, 8, seed=1, dtype=np.float32)
     Xb, yb = orc.generate_dataset(5000, 8, seed=2, dtype=np.float32)
     yb = (yb + 7.0).astype(np.float32)
-    e1 = b2.B200LinearRegression(ctx=ctx).fit(Xa, ya, with_spectrum=False)
+    e0 = b2.B200LinearRegression(ctx=ctx).fit(Xa, ya, with_spectrum=False)    # alpha = 0: the rank rule needs the spectrum
+    e1 = b2.B200LinearRegression(ctx=ctx, alpha=1e-6).fit(Xa, ya, with_spectrum=False)   # ridge: the spectrum is deferred
     e2 = b2.B200LinearRegression(ctx=ctx).partial_fit(Xb, yb)     # must NOT fold B into A's rows
     ref_b = _oracle_fit(Xb, yb)
     assert np.max(np.abs(e2.coef_ - ref_b["coef"])) < COEF_TOL and abs(e2.intercept_ - ref_b["intercept"]) < 1e-2
     with pytest.raises(RuntimeError, match="no longer resident"):
         e1.to_sklearn()                                           # A's deferred spectrum would come from B's rows
+    reg0 = e0.to_sklearn()                                        # A's own spectrum, computed when e0 was fitted
+    sk_a = LinearRegression().fit(Xa.astype(np.float64), ya.astype(np.float64))
+    assert reg0.rank_ == sk_a.rank_ == 8
+    np.testing.assert_allclose(reg0.singular_, sk_a.singular_, rtol=1e-4)
     e2.partial_fit(Xa, ya)                                        # e2 = B then A, from its own statistic
     e3 = b2.B200LinearRegression(ctx=ctx).fit(Xa, ya)             # someone else uses the context in between
     e2.partial_fit(Xb, yb)
