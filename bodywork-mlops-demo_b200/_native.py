@@ -23,6 +23,7 @@ E_COMM = -5
 EXCHANGE_NONE, EXCHANGE_NCCL, EXCHANGE_PEER = 0, 1, 2
 ABI_VERSION = 2
 MAX_D = 128
+MAX_ALPHAS = 64
 
 _c_i64 = C.c_int64
 _vp = C.c_void_p
@@ -64,6 +65,9 @@ _SIGNATURES = {
     "b2_solve": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_double)]),
     "b2_solve_eigvals": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_int), C.POINTER(_c_i64)]),
     "b2_solve_spectral": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_double), _vp, C.POINTER(C.c_int)]),
+    "b2_solve_eigh": (C.c_int, [_vp, C.c_int, _vp, _vp]),
+    "b2_ridge_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
+                               C.c_int, _vp, _vp, C.POINTER(C.c_int), _vp, C.POINTER(C.c_double)]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -438,6 +442,39 @@ class Context:
         _check(load().b2_solve_eigvals(self._h, float(cond), int(bool(fit_intercept)), sing.ctypes.data,
                                        C.byref(rank), C.byref(rows)), "b2_solve_eigvals")
         return sing, int(rank.value), int(rows.value)
+
+    def solve_eigh(self, fit_intercept: bool = True) -> Tuple[np.ndarray, np.ndarray]:
+        """(lambda, Q): eigenvalues (ascending, negative rounding values as 0) and orthonormal eigenvectors (column k for
+        eigenvalue k) of the centred Gram (uncentred without an intercept) of the resident statistic."""
+        lam = np.empty(self.d, dtype=np.float64)
+        Q = np.empty((self.d, self.d), dtype=np.float64)
+        _check(load().b2_solve_eigh(self._h, int(bool(fit_intercept)), lam.ctypes.data, Q.ctypes.data), "b2_solve_eigh")
+        return lam, Q
+
+    def ridge_loo(self, X, y, alphas, row_mask=None, mask_keep: int = 1, fit_intercept: bool = True,
+                  store_cv: bool = False):
+        """RidgeCV(alphas).fit's leave-one-out search in one call (b2_ridge_loo): returns (mse per alpha, index of the
+        first smallest, coef, intercept at that alpha, cv) where cv is None or the (n, n_alphas) e^2 per row and alpha
+        (NaN on rows not kept) -- a float64 ndarray for host rows, an f64 DeviceArray for device rows.  Up to MAX_ALPHAS
+        alphas per call."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        al = np.ascontiguousarray(np.asarray(alphas, dtype=np.float64).ravel())
+        mse = np.empty(max(al.size, 1), dtype=np.float64)
+        coef = np.empty(d, dtype=np.float64)
+        b0, best = C.c_double(0.0), C.c_int(0)
+        cv, cv_ptr = None, None
+        if store_cv:
+            cv = self.empty((n, al.size), "f64") if mk == MEM_DEVICE else np.empty((n, al.size), dtype=np.float64)
+            cv_ptr = cv.ptr if mk == MEM_DEVICE else cv.ctypes.data
+        rc = load().b2_ridge_loo(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), al.ctypes.data, int(al.size),
+                                 int(bool(fit_intercept)), mse.ctypes.data, cv_ptr, C.byref(best), coef.ctypes.data,
+                                 C.byref(b0))
+        self.d = int(d)
+        self.serial += 1
+        _check(rc, "b2_ridge_loo")
+        return mse[: al.size], int(best.value), coef, float(b0.value), cv
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

@@ -355,6 +355,8 @@ static int ctx_allocate(b2_ctx* ctx) {
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->coef_dev), sizeof(double) * (kMaxD + 1)));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->grad_part), sizeof(double) * (size_t)ctx->score_ctas * kGradOut));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->refine), sizeof(double) * kRfDoubles));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->loo), sizeof(double) * kLooDoubles));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->loo_part), sizeof(double) * (size_t)ctx->sm_count * kMaxAlphas));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->solve_out), sizeof(double) * (2 * kMaxD + 8)));
   B2_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&ctx->solve_host), sizeof(double) * (2 * kMaxD + 8), cudaHostAllocDefault));
   B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->tc_sync), 64));
@@ -409,7 +411,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
-                  ctx->grad_part, ctx->refine};
+                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1]};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -855,6 +857,123 @@ int b2_fit_refined(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   *intercept = h[kMaxD];
   if (passes_out != nullptr) *passes_out = kept;
   return B2_OK;
+}
+
+// the Jacobi kernel's convergence flag (ctx->loo + kLooMisc + 3) as a return code
+static int eigh_converged(double flag) {
+  if (flag != 0.0) return B2_OK;
+  set_error("the Jacobi eigendecomposition did not converge within its sweep limit");
+  return B2_E_SINGULAR;
+}
+
+// ---- eigendecomposition and RidgeCV's leave-one-out error (DESIGN.md section 6) ---------------------------------
+int b2_solve_eigh(b2_ctx* ctx, int fit_intercept, double* eigvals, double* eigvecs) {
+  if (int r = use_device(ctx)) return r;
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  if (int r = launch_solve_eigh(ctx, fit_intercept)) return r;
+  const int d = ctx->d;
+  double converged = 0.0;
+  B2_CUDA(cudaMemcpyAsync(&converged, ctx->loo + kLooMisc + 3, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (eigvals != nullptr)
+    B2_CUDA(cudaMemcpyAsync(eigvals, ctx->loo + kLooLam, sizeof(double) * d, cudaMemcpyDeviceToHost, ctx->stream));
+  if (eigvecs != nullptr)
+    B2_CUDA(cudaMemcpy2DAsync(eigvecs, sizeof(double) * d, ctx->loo + kLooQ, sizeof(double) * kMaxD, sizeof(double) * d, d,
+                              cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return eigh_converged(converged);
+}
+
+// The Gram of b2_fit, the eigendecomposition of its centred Gram, one leave-one-out pass over the same rows (host rows
+// re-stream through the staging ring, their e^2 through a device block per row block), then the LDL^T solve of b2_fit
+// at the chosen alpha from the same S.
+int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                 int mem_kind, const uint8_t* row_mask, int mask_keep, const double* alphas, int n_alphas,
+                 int fit_intercept, double* mse_out, double* cv_out, int* best_out, double* coef, double* intercept) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (alphas == nullptr || n_alphas < 1 || n_alphas > kMaxAlphas) {
+    set_error("n_alphas=%d out of range [1,%d] (or alphas is null)", n_alphas, kMaxAlphas);
+    return B2_E_ARG;
+  }
+  for (int a = 0; a < n_alphas; ++a)
+    if (!(isfinite(alphas[a]) && alphas[a] > 0.0)) {
+      set_error("alphas[%d] == %g, must be > 0.0 and finite", a, alphas[a]);
+      return B2_E_ARG;
+    }
+  if (mse_out == nullptr || best_out == nullptr || coef == nullptr || intercept == nullptr) {
+    set_error("mse_out / best_out / coef / intercept is null");
+    return B2_E_ARG;
+  }
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) {
+    set_error("b2_ridge_loo runs on one rank only (the leave-one-out pass is not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (int r = b2_gram_reset(ctx, d)) return r;
+  if (mem_kind == B2_MEM_DEVICE) {
+    if (int r = gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) return r;
+  } else if (int r = gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) {
+    return r;
+  }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  if (int r = launch_solve_eigh(ctx, fit_intercept)) return r;
+  B2_CUDA(cudaMemcpyAsync(ctx->loo + kLooAlpha, alphas, sizeof(double) * n_alphas, cudaMemcpyHostToDevice, ctx->stream));
+  double misc[4];
+  B2_CUDA(cudaMemcpyAsync(misc, ctx->loo + kLooMisc, sizeof(misc), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const double n_kept = misc[1];
+  if (!(n_kept > 0.0)) { set_error("no row kept: the leave-one-out error needs at least one row"); return B2_E_ARG; }
+  if (int r = eigh_converged(misc[3])) return r;
+  if (mem_kind == B2_MEM_DEVICE) {
+    if (int r = launch_loo(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, n_alphas, cv_out, true)) return r;
+  } else {
+    const int es = x_dtype == B2_F32 ? 4 : 2;
+    const bool x_pinned = host_pointer_is_pinned(X);
+    if (cv_out != nullptr && ctx->cv_stage_alphas < n_alphas) {     // sized to the widest call so far
+      B2_CUDA(cudaStreamSynchronize(ctx->stream));                 // an earlier call's copies may still read them
+      for (int b = 0; b < 2; ++b) {
+        if (ctx->cv_stage[b] != nullptr) cudaFree(ctx->cv_stage[b]);
+        ctx->cv_stage[b] = nullptr;
+      }
+      ctx->cv_stage_alphas = 0;
+      for (int b = 0; b < 2; ++b)
+        if (cudaMalloc(reinterpret_cast<void**>(&ctx->cv_stage[b]), sizeof(double) * ctx->stage_rows * n_alphas) !=
+            cudaSuccess) {
+          cudaGetLastError();
+          set_error("out of device memory for the leave-one-out staging blocks");
+          return B2_E_CUDA;
+        }
+      ctx->cv_stage_alphas = n_alphas;
+    }
+    const int rc = stream_host_blocks(
+        ctx, n_rows, ctx->stage_rows,
+        [&](int buf, int64_t r0, int64_t rows) {
+          return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
+        },
+        [&](int buf, int64_t r0, int64_t rows) -> int {
+          double* cv_dev = cv_out != nullptr ? ctx->cv_stage[buf] : nullptr;
+          if (int r = launch_loo(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
+                                 row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, n_alphas, cv_dev, r0 == 0))
+            return r;
+          if (cv_out != nullptr)
+            B2_CUDA(cudaMemcpyAsync(cv_out + r0 * n_alphas, cv_dev, sizeof(double) * rows * n_alphas,
+                                    cudaMemcpyDeviceToHost, ctx->stream));
+          return B2_OK;
+        });
+    if (rc != B2_OK) return rc;
+  }
+  double sums[kMaxAlphas];
+  B2_CUDA(cudaMemcpyAsync(sums, ctx->loo + kLooSum, sizeof(double) * n_alphas, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  int best = 0;
+  for (int a = 0; a < n_alphas; ++a) {
+    mse_out[a] = sums[a] / n_kept;
+    if (mse_out[a] < mse_out[best]) best = a;        // the first of equal minima, as sklearn's argmax of the score
+  }
+  *best_out = best;
+  if (int r = launch_solve_cholesky(ctx, alphas[best], fit_intercept)) return r;
+  return finish_cholesky(ctx, coef, intercept);
 }
 
 // ---- scoring ---------------------------------------------------------------------------------------

@@ -64,6 +64,20 @@ constexpr int kRfDoubles = kRfGrad + kGradOut;
 constexpr int kOutRefineStep = 2 * kMaxD + 3;
 constexpr int kOutRefineGuard = 2 * kMaxD + 4;
 
+// ---- the leave-one-out pass of b2_ridge_loo (ridge_loo.cu) and its eigendecomposition (solve_eigh_kernel) ----------
+constexpr int kMaxAlphas = B2_MAX_ALPHAS;
+// doubles of ctx->loo
+constexpr int kLooQ = 0;                          // Q[i][k], row pitch kMaxD: column k is the eigenvector of eigenvalue k
+constexpr int kLooLam = kMaxD * kMaxD;            // eigenvalues, ascending, >= 0
+constexpr int kLooMean = kLooLam + kMaxD;         // m: S's column means (0 without an intercept)
+constexpr int kLooC = kLooMean + kMaxD;           // c = Q^T r
+constexpr int kLooMisc = kLooC + kMaxD;           // [0] ybar, [1] n, [2] h0, [3] 1: the Jacobi sweeps converged
+constexpr int kLooAlpha = kLooMisc + 8;           // the alphas of the call [kMaxAlphas]
+constexpr int kLooCw = kLooAlpha + kMaxAlphas;    // [kMaxD][kMaxAlphas] c_j / (lambda_j + alpha_a)
+constexpr int kLooW = kLooCw + kMaxD * kMaxAlphas;   // [kMaxD][kMaxAlphas] 1 / (lambda_j + alpha_a)
+constexpr int kLooSum = kLooW + kMaxD * kMaxAlphas;  // the reduced sums of e^2 per alpha [kMaxAlphas]
+constexpr int kLooDoubles = kLooSum + kMaxAlphas;
+
 // template width of the one-lane-per-row kernels (gram_narrow.cu, score.cu) for d <= 16 features: the next power of two
 inline int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
 
@@ -122,6 +136,11 @@ struct b2_ctx {
   // refined fit scratch
   double* grad_part = nullptr;         // [score_ctas][kGradOut] per-CTA gradient partials
   double* refine = nullptr;            // [kRfDoubles] beta, b0', m, the state before the last correction, step, gradient
+  // ridge leave-one-out scratch
+  double* loo = nullptr;               // [kLooDoubles] Q, lambda, m, c, ybar / n / h0, alphas, the B operands, the sums
+  double* loo_part = nullptr;          // [sm_count][kMaxAlphas] per-CTA sums of e^2
+  double* cv_stage[2] = {nullptr, nullptr};   // e^2 staging blocks of host rows [stage_rows][cv_stage_alphas]
+  int cv_stage_alphas = 0;             // alphas per row the staging blocks hold (grown to a call's n_alphas)
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -190,6 +209,25 @@ int with_rows(int x_dtype, const void* X, F&& f) {
 template <typename P>
 using row_t = std::remove_const_t<std::remove_pointer_t<P>>;
 
+// Which kernels read the rows [0, n) of one call.  Contiguous 16-byte aligned rows stream through a bulk-copy ring in
+// whole tiles: one lane per row for d <= 16 (narrow, the mask aligned too), LPR lanes per row when a row is a multiple of
+// 16 bytes (wide).  The rows after the last whole tile, and all rows of any other layout, go to the register-fed kernels
+// (direct).  Scoring and the residual gradient share this plan, so a pass of the refined fit (and the leave-one-out pass
+// of b2_ridge_loo) reads its rows the way b2_score does, in as many launches.
+struct RowPlan {
+  enum Kind { kDirect, kNarrow, kWide } kind = kDirect;
+  int dp = 0;                   // narrow: the template width narrow_dp(d)
+  int lpr = 0, sweeps = 0;      // wide: lanes per row, consumer sweeps per tile
+  int n_tiles = 0, grid = 0;    // whole ring tiles and the ring's grid (n_tiles == 0: no ring launch)
+  int64_t done = 0;             // rows [0, done) go through the ring
+  bool direct = false;          // the register-fed kernels take the rows [done, n) (one launch when n == 0)
+  int64_t rest = 0;
+  int vec = 0, direct_grid = 0; // their 4-feature vector loads and grid
+};
+
+RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                  const uint8_t* mask);
+
 // ---- kernel launchers (each enqueues on ctx->stream and bumps ctx->launches) -----------------
 // The Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites
 // it instead of adding to it (the first writer after b2_gram_reset).  The tensor-core and narrow launchers cover the
@@ -223,6 +261,13 @@ int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64
 // the correction solve of one refinement pass: (A + alpha I) dbeta = g - alpha beta from the factor of S, then the
 // update of ctx->refine; the result goes to ctx->solve_host
 int launch_solve_refine(b2_ctx* ctx, double alpha, int fit_intercept);
+// eigenvalues, orthonormal eigenvectors, m, ybar, n, h0 and c = Q^T r of the centred Gram of S into ctx->loo
+int launch_solve_eigh(b2_ctx* ctx, int fit_intercept);
+// the leave-one-out pass over the rows [0, n) for the n_alphas alphas at ctx->loo + kLooAlpha: the B operands (once per
+// call, `first_block`), the pass (e^2 per row and alpha into cv when not null, NaN for rows not kept) and the ordered
+// reduce of the per-CTA sums into ctx->loo + kLooSum (`first_block` overwrites, otherwise adds)
+int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+               const uint8_t* mask, int keep, int n_alphas, double* cv, bool first_block);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

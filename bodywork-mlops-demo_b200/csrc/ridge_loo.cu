@@ -1,0 +1,306 @@
+// ridge_loo.cu -- the leave-one-out pass of RidgeCV(alphas).fit(X, y) with cv=None (b2_ridge_loo; DESIGN.md section 6).
+//
+// With A = Q diag(lambda) Q^T the centred Gram of the kept rows, c = Q^T r and w_ja = 1 / (lambda_j + alpha_a), a kept
+// row's leave-one-out error at alpha_a is e = ((y - ybar) - yhat) / (1 - h) with z = Q^T (x - m), yhat = sum_j z_j c_j
+// w_ja and h = h0 + sum_j z_j^2 w_ja: what scikit-learn's _RidgeGCV computes from an SVD of the whole design matrix.  Per
+// row that is 2 D^2 + 4 A D flops against D * 4 bytes of row: the pass is fp64-compute bound, so both products run on the
+// fp64 tensor core (mma.sync m8n8k4 f64):
+//   (1) a tile of 32 rows -> shared memory as v = x - m in fp64 from the stored value (one rounding), 0 for rows not kept;
+//   (2) Z = V Q (Q resident in shared memory for the whole launch), written back over V;
+//   (3) [yhat | h - h0] = [Z (c o w) | (Z o Z) w], the B operands read from a D x 64 table built once per call; the
+//       per-row, per-alpha epilogue forms e in fp64 (y - yhat cancels) and adds e^2 to the lane's sums.
+// The rows take scoring's plan (plan_rows): where it streams contiguous rows through the bulk-copy ring, a producer warp
+// runs ring_produce with 32-row tiles of X and y and the consumers convert each slot in (1); the rows after the last whole
+// tile, and every other layout, are read by the same consumers straight from global memory.
+// A row not kept has v = 0 and e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA writes its sums per
+// alpha in a fixed order; loo_reduce_kernel adds the CTAs in order, so two calls return identical sums.
+#include "b2_internal.cuh"
+#include "b2_ptx.cuh"
+
+namespace b2 {
+namespace {
+
+constexpr int kLooRows = 32;                       // rows per tile
+constexpr int kLooMT = kLooRows / 8;               // m-tiles of the DMMA per tile
+constexpr int kLooWarps = 8;                       // consumer warps
+constexpr int kLooConsumers = 32 * kLooWarps;
+constexpr int kLooThreads = kLooConsumers + 32;    // + the producer warp of the ring
+constexpr int kLooStages = 3;
+constexpr uint32_t kLooXStage = kLooRows * kMaxD * 4;                       // 16 KB: 32 fp32 rows of 128 features
+constexpr uint32_t kLooYStage = kLooRows * 4;
+constexpr uint32_t kLooOffY = kLooStages * kLooXStage;
+constexpr uint32_t kLooOffBar = kLooOffY + kLooStages * kLooYStage;
+constexpr uint32_t kLooRingBytes = kLooOffBar + 2 * kLooStages * 8 + 16;    // the doubles start here (16-byte aligned)
+
+__host__ __device__ inline int loo_dp(int d) { return (d + 7) & ~7; }
+__host__ __device__ inline int loo_qpitch(int dp) { return dp + 8; }
+__host__ __device__ inline int loo_vpitch(int dp) { return dp + 4; }
+size_t loo_smem_bytes(int dp, bool ring) {
+  return (ring ? kLooRingBytes : 0) +
+         sizeof(double) * ((size_t)dp * loo_qpitch(dp) + (size_t)kLooRows * loo_vpitch(dp) + 2 * kLooRows + kMaxD +
+                           (size_t)kLooWarps * kMaxAlphas);
+}
+
+__device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
+  asm volatile("bar.sync 1, %0;" ::"r"(kLooConsumers) : "memory");
+}
+
+__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {
+  // fragments (PTX mma.m8n8k4.f64): A row = lane / 4, col = lane % 4; B row(k) = lane % 4, col(n) = lane / 4;
+  // C row = lane / 4, cols = 2 (lane % 4) + {0, 1}
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+
+template <typename T>
+__device__ __forceinline__ float ld_row_val(const T* __restrict__ p);
+template <>
+__device__ __forceinline__ float ld_row_val<float>(const float* __restrict__ p) { return __ldg(p); }
+template <>
+__device__ __forceinline__ float ld_row_val<__nv_bfloat16>(const __nv_bfloat16* __restrict__ p) {
+  return __bfloat162float(*p);
+}
+
+// the B operands of (3): Cw[j][a] = c_j / (lambda_j + alpha_a), W[j][a] = 1 / (lambda_j + alpha_a); 0 outside d x n_alphas
+__global__ void loo_prep_kernel(double* __restrict__ loo, int d, int n_alphas) {
+  for (int t = threadIdx.x; t < kMaxD * kMaxAlphas; t += blockDim.x) {
+    const int j = t / kMaxAlphas, a = t - j * kMaxAlphas;
+    double cw = 0.0, w = 0.0;
+    if (j < d && a < n_alphas) {
+      w = 1.0 / (loo[kLooLam + j] + loo[kLooAlpha + a]);
+      cw = loo[kLooC + j] * w;
+    }
+    loo[kLooCw + t] = cw;
+    loo[kLooW + t] = w;
+  }
+}
+
+// RING: rows [0, n), n a multiple of kLooRows, contiguous (ldx == d) and 16-byte aligned with y, through the bulk-copy
+// ring; otherwise rows [0, n) of any layout (stride ldx, fp32 or bf16, any alignment) from global memory.  Tiles
+// blockIdx.x, + gridDim.x, ...
+// Work of (3): the n_alphas are ceil(n_alphas / 8) n-tiles; each gets G = 8 / n-tiles warps, each warp a group of
+// ceil(kLooMT / G) m-tiles, so every warp holds at most one (n-tile, group) for the whole launch and its sums stay in
+// registers.
+template <typename T, bool RING>
+__global__ void __launch_bounds__(kLooThreads, 1)
+loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
+           const uint8_t* __restrict__ mask, int keep, const double* __restrict__ loo, int n_alphas,
+           double* __restrict__ cv, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const uint32_t sbase = smem_u32(smem_raw);
+  const uint32_t bar_full = sbase + kLooOffBar, bar_empty = bar_full + 8 * kLooStages;
+  const int dp = loo_dp(d), qp = loo_qpitch(dp), vp = loo_vpitch(dp);
+  double* Qs = reinterpret_cast<double*>(smem_raw + (RING ? kLooRingBytes : 0));   // Q[i][k], zero padded to dp x dp
+  double* Vs = Qs + dp * qp;               // the tile: v = x - m, then Z = V Q
+  double* yc = Vs + kLooRows * vp;         // y - ybar (0 for rows not kept)
+  double* usef = yc + kLooRows;            // 1: kept
+  double* mean = usef + kLooRows;          // [kMaxD]
+  double* sums = mean + kMaxD;             // [group][kMaxAlphas]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t4 = lane & 3;
+  for (int t = tid; t < dp * dp; t += blockDim.x) {
+    const int i = t / dp, k = t - i * dp;
+    Qs[i * qp + k] = (i < d && k < d) ? loo[kLooQ + i * kMaxD + k] : 0.0;
+  }
+  for (int t = tid; t < kMaxD; t += blockDim.x) mean[t] = t < d ? loo[kLooMean + t] : 0.0;
+  for (int t = tid; t < kLooWarps * kMaxAlphas; t += blockDim.x) sums[t] = 0.0;
+  const double ybar = loo[kLooMisc], h0 = loo[kLooMisc + 2];
+  const int na = (n_alphas + 7) >> 3;
+  const int G = kLooWarps / na, mpg = (kLooMT + G - 1) / G;
+  const bool has_item = warp < na * G;     // warp-uniform
+  const int nt_a = has_item ? warp / G : 0, grp = has_item ? warp % G : 0, mt0 = grp * mpg;
+  const int a0 = 8 * nt_a + 2 * t4;        // the two alphas of this lane's accumulators
+  const int ab = 8 * nt_a + g;             // the alpha of this lane's B fragment
+  const int64_t n_tiles = (n + kLooRows - 1) / kLooRows;
+  if constexpr (RING) ring_init<kLooStages>(bar_full, bar_empty, kLooWarps);   // includes a block barrier
+  else __syncthreads();
+  if (RING && warp == kLooWarps) {
+    if (lane == 0)
+      ring_produce<kLooStages>(bar_full, bar_empty, (int)n_tiles, kLooRows, X, (uint32_t)(d * sizeof(T)), sbase,
+                               kLooXStage, true, y, sbase + kLooOffY, kLooYStage, false, nullptr, 0u, 0u);
+  } else {
+    double acc_e[2] = {0.0, 0.0};
+    int s = 0;
+    uint32_t phase = 0;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      const int64_t row0 = tile * kLooRows;
+      // (1) the tile
+      if constexpr (RING) {
+        bool use[kLooRows / kLooWarps];
+#pragma unroll
+        for (int u = 0; u < kLooRows / kLooWarps; ++u)   // the mask comes from global memory, before the wait
+          use[u] = mask == nullptr || __ldg(mask + row0 + warp + kLooWarps * u) == (uint8_t)keep;
+        mbar_wait(bar_full + 8 * s, phase);
+        const uint32_t xs = sbase + s * kLooXStage, ys = sbase + kLooOffY + s * kLooYStage;
+#pragma unroll
+        for (int u = 0; u < kLooRows / kLooWarps; ++u) {
+          const int r = warp + kLooWarps * u;
+          const uint32_t xr = xs + (uint32_t)(r * d) * (uint32_t)sizeof(T);
+          for (int j = lane; j < dp; j += 32) {
+            const bool live = use[u] && j < d;
+            const float x = live ? raw_ld_shared<T>(xr + (uint32_t)j * (uint32_t)sizeof(T)) : 0.f;
+            Vs[r * vp + j] = live ? (double)x - mean[j] : 0.0;
+          }
+          if (lane == 0) {
+            yc[r] = use[u] ? (double)ld_shared_f32(ys + 4u * (uint32_t)r) - ybar : 0.0;
+            usef[r] = use[u] ? 1.0 : 0.0;
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * s);      // the slot is converted: the producer may refill it
+        if (++s == kLooStages) { s = 0; phase ^= 1u; }
+      } else {
+        for (int r = warp; r < kLooRows; r += kLooWarps) {
+          const int64_t row = row0 + r;
+          bool use = row < n;
+          if (use && mask != nullptr) use = __ldg(mask + row) == (uint8_t)keep;
+          const T* xr = X + row * ldx;
+          for (int j = lane; j < dp; j += 32) {
+            const bool live = use && j < d;
+            const float x = live ? ld_row_val<T>(xr + j) : 0.f;
+            Vs[r * vp + j] = live ? (double)x - mean[j] : 0.0;
+          }
+          if (lane == 0) {
+            yc[r] = use ? (double)__ldg(y + row) - ybar : 0.0;
+            usef[r] = use ? 1.0 : 0.0;
+          }
+        }
+      }
+      consumer_sync();
+      // (2) Z = V Q: warp w takes the n-tiles w and w + 8 of the dp / 8, all m-tiles
+      double z[2][kLooMT][2];
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+#pragma unroll
+        for (int mt = 0; mt < kLooMT; ++mt) { z[u][mt][0] = 0.0; z[u][mt][1] = 0.0; }
+        const int nt = warp + kLooWarps * u;
+        if (nt < dp / 8) {
+          for (int ks = 0; ks < dp / 4; ++ks) {
+            const double b = Qs[(4 * ks + t4) * qp + 8 * nt + g];
+            double a[kLooMT];
+#pragma unroll
+            for (int mt = 0; mt < kLooMT; ++mt) a[mt] = Vs[(8 * mt + g) * vp + 4 * ks + t4];
+#pragma unroll
+            for (int mt = 0; mt < kLooMT; ++mt) dmma(z[u][mt][0], z[u][mt][1], a[mt], b);
+          }
+        }
+      }
+      consumer_sync();
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int nt = warp + kLooWarps * u;
+        if (nt < dp / 8) {
+#pragma unroll
+          for (int mt = 0; mt < kLooMT; ++mt) {
+            Vs[(8 * mt + g) * vp + 8 * nt + 2 * t4] = z[u][mt][0];
+            Vs[(8 * mt + g) * vp + 8 * nt + 2 * t4 + 1] = z[u][mt][1];
+          }
+        }
+      }
+      consumer_sync();
+      // (3) yhat and h of every kept row and alpha, then e^2
+      if (has_item) {
+        double yh[kLooMT][2], hh[kLooMT][2];
+#pragma unroll
+        for (int mm = 0; mm < kLooMT; ++mm) { yh[mm][0] = yh[mm][1] = hh[mm][0] = hh[mm][1] = 0.0; }
+        for (int ks = 0; ks < dp / 4; ++ks) {
+          const int j = 4 * ks + t4;
+          const double bc = __ldg(loo + kLooCw + j * kMaxAlphas + ab);
+          const double bw = __ldg(loo + kLooW + j * kMaxAlphas + ab);
+#pragma unroll
+          for (int mm = 0; mm < kLooMT; ++mm) {
+            if (mm < mpg && mt0 + mm < kLooMT) {              // warp-uniform
+              const double zz = Vs[(8 * (mt0 + mm) + g) * vp + j];
+              dmma(yh[mm][0], yh[mm][1], zz, bc);
+              dmma(hh[mm][0], hh[mm][1], zz * zz, bw);
+            }
+          }
+        }
+#pragma unroll
+        for (int mm = 0; mm < kLooMT; ++mm) {
+          if (mm < mpg && mt0 + mm < kLooMT) {
+            const int r = 8 * (mt0 + mm) + g;
+            const int64_t row = row0 + r;
+            const bool use = usef[r] != 0.0;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const double err = use ? (yc[r] - yh[mm][e]) / (1.0 - (h0 + hh[mm][e])) : 0.0;
+              const double e2 = err * err;
+              acc_e[e] += e2;
+              const int a = a0 + e;
+              if (cv != nullptr && row < n && a < n_alphas)
+                cv[row * n_alphas + a] = use ? e2 : __longlong_as_double(0x7ff8000000000000ll);
+            }
+          }
+        }
+      }
+      consumer_sync();
+    }
+    // the CTA's sums: the 8 row lanes of an alpha pair combined, then the groups of an alpha in group order
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      double v = acc_e[e];
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (has_item && g == 0) sums[grp * kMaxAlphas + a0 + e] = v;
+    }
+  }
+  __syncthreads();
+  for (int a = tid; a < kMaxAlphas; a += blockDim.x) {
+    double v = 0.0;
+    for (int q = 0; q < kLooWarps; ++q) v += sums[q * kMaxAlphas + a];
+    part[(size_t)blockIdx.x * kMaxAlphas + a] = v;
+  }
+}
+
+// acc[kMaxAlphas] (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites
+__global__ void loo_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
+  const int a = threadIdx.x;
+  if (a >= kMaxAlphas) return;
+  double v = first ? 0.0 : acc[a];
+  for (int c = 0; c < n_ctas; ++c) v += part[(size_t)c * kMaxAlphas + a];
+  acc[a] = v;
+}
+
+}  // namespace
+
+// The rows [0, n) in the launches of scoring's plan: whole 32-row tiles of what plan_rows streams through the ring go to the
+// ring flavour, the rest (or every row of another layout) to the direct one; each launch is followed by its ordered reduce.
+int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+               const uint8_t* mask, int keep, int n_alphas, double* cv, bool first_block) {
+  if (first_block) {
+    loo_prep_kernel<<<1, 256, 0, ctx->stream>>>(ctx->loo, d, n_alphas);
+    B2_CUDA(cudaGetLastError());
+    ctx->launches += 1;
+  }
+  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
+  const int64_t ring_rows = p.kind != RowPlan::kDirect ? (n / kLooRows) * kLooRows : 0;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  bool first = first_block;
+  for (int part = 0; part < 2; ++part) {
+    const bool ring = part == 0;
+    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
+    if (ring ? rows == 0 : (rows == 0 && !first)) continue;            // an empty call still writes the sums once
+    const int64_t n_tiles = (rows + kLooRows - 1) / kLooRows;
+    int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
+    if (grid < 1) grid = 1;
+    const char* Xt = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
+    const float* yt = y != nullptr ? y + r0 : nullptr;
+    const uint8_t* mt = mask != nullptr ? mask + r0 : nullptr;
+    double* cvt = cv != nullptr ? cv + r0 * n_alphas : nullptr;
+    const uint32_t smem = (uint32_t)loo_smem_bytes(loo_dp(d), ring);
+    const int rc = with_rows(x_dtype, Xt, [&](auto* Xr) {
+      using T = row_t<decltype(Xr)>;
+      auto kernel = ring ? loo_kernel<T, true> : loo_kernel<T, false>;
+      return launch_smem(kernel, grid, ring ? kLooThreads : kLooConsumers, smem, ctx->stream, Xr, rows, d, ldx, yt, mt,
+                         keep, static_cast<const double*>(ctx->loo), n_alphas, cvt, ctx->loo_part);
+    });
+    if (rc != B2_OK) return rc;
+    loo_reduce_kernel<<<1, kMaxAlphas, 0, ctx->stream>>>(ctx->loo_part, grid, first ? 1 : 0, ctx->loo + kLooSum);
+    B2_CUDA(cudaGetLastError());
+    ctx->launches += 2;
+    first = false;
+  }
+  return B2_OK;
+}
+
+}  // namespace b2

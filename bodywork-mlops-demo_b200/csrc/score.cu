@@ -941,21 +941,7 @@ int grad_reduce(b2_ctx* ctx, int grid, bool first) {
   return B2_OK;
 }
 
-// Which kernels read the rows [0, n) of one call.  Contiguous 16-byte aligned rows stream through a bulk-copy ring in
-// whole tiles: one lane per row for d <= 16 (narrow, the mask aligned too), LPR lanes per row when a row is a multiple of
-// 16 bytes (wide).  The rows after the last whole tile, and all rows of any other layout, go to the register-fed kernels
-// (direct).  Scoring and the residual gradient share this plan, so a pass of the refined fit reads its rows the way
-// b2_score does, in as many launches.
-struct RowPlan {
-  enum Kind { kDirect, kNarrow, kWide } kind = kDirect;
-  int dp = 0;                   // narrow: the template width narrow_dp(d)
-  int lpr = 0, sweeps = 0;      // wide: lanes per row, consumer sweeps per tile
-  int n_tiles = 0, grid = 0;    // whole ring tiles and the ring's grid (n_tiles == 0: no ring launch)
-  int64_t done = 0;             // rows [0, done) go through the ring
-  bool direct = false;          // the register-fed kernels take the rows [done, n) (one launch when n == 0)
-  int64_t rest = 0;
-  int vec = 0, direct_grid = 0; // their 4-feature vector loads and grid
-};
+}  // namespace
 
 RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                   const uint8_t* mask) {
@@ -993,8 +979,6 @@ RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int 
   p.direct_grid = (int)(want < ctx->score_ctas ? want : ctx->score_ctas);
   return p;
 }
-
-}  // namespace
 
 int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int64_t n, bool first) {
   int64_t want = (n + kScoreThreads * 8 - 1) / (kScoreThreads * 8);

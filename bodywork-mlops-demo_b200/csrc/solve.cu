@@ -848,6 +848,159 @@ solve_eigvals_kernel(const double* S, int d, double cond, int fit_intercept, dou
   }
 }
 
+// ---- eigenvalues and orthonormal eigenvectors: b2_solve_eigh and the leave-one-out pass of b2_ridge_loo -------------
+// The one-sided Jacobi above keeps only W = A V; normalising a column of W whose eigenvalue is near zero gives noise.
+// Here two-sided cyclic Jacobi rotates A itself (packed upper triangle, 66 KB at D = 128) and accumulates V = the product
+// of the rotations (131 KB), so V is orthonormal to working precision whatever the spectrum.  One round of the
+// round-robin tournament (rr_pair) rotates m / 2 disjoint pairs at once: (1) each pair's (c, s) from its 2 x 2 diagonal
+// block, (2) every 2 x 2 block of pairs (P1, P2) becomes J1^T B J2 in one step -- the blocks are disjoint, so no thread
+// reads what another writes -- and the columns p, q of V rotate.  A pair rotates when |a_pq| > eps/2 sqrt(|a_pp a_qq|) and
+// above 1e-20 of the largest diagonal entry; the sweeps stop after one without a rotation.  Cyclic Jacobi converges
+// quadratically once the off-diagonal part is small; if kEighMaxSweeps sweeps still rotate, the kernel reports it (the
+// host turns that into an error) instead of returning an unconverged Q.
+// Output (ctx->loo): eigenvalues ascending, negative rounding values as 0; Q[i][k] (row pitch kMaxD), column k for
+// eigenvalue k; the means m, ybar, n, h0 = 1 / n (0 without an intercept), c = Q^T r and whether the sweeps converged.
+constexpr int kEighThreads = 512;
+constexpr int kEighMaxSweeps = 30;
+
+__host__ __device__ inline int eigh_m(int d) { return d + (d & 1); }
+__device__ __forceinline__ int packed_ix(int i, int j) { return i <= j ? j * (j + 1) / 2 + i : i * (i + 1) / 2 + j; }
+
+size_t eigh_smem_bytes(int d) {
+  const size_t m = (size_t)eigh_m(d);
+  const size_t full = (size_t)d * (d + 1) > m * m ? (size_t)d * (d + 1) : m * m;   // A (build) then V, same region
+  return sizeof(double) * (m * (m + 1) / 2 + full + 3 * (size_t)kMaxD + 16 + 2 * (kMaxD / 2)) + sizeof(int) * kMaxD;
+}
+
+__global__ void __launch_bounds__(kEighThreads, 1)
+solve_eigh_kernel(const double* __restrict__ S, int d, int fit_intercept, double* __restrict__ loo) {
+  extern __shared__ double sm[];
+  const int m = eigh_m(d), M = m / 2, pitch = d + 1;
+  double* AP = sm;                                   // packed upper triangle of the m x m matrix (row/column d: phantom)
+  double* V = AP + m * (m + 1) / 2;                  // V^T: V[k * m + i] = V_ik; first holds A (pitch d + 1) from the build
+  const size_t full = (size_t)d * (d + 1) > (size_t)m * m ? (size_t)d * (d + 1) : (size_t)m * m;
+  double* r = V + full;
+  double* mean = r + kMaxD;
+  double* lam = mean + kMaxD;
+  double* misc = lam + kMaxD;                        // [0] ybar, [1] largest |diagonal|
+  double* cs = misc + 16;                            // [kMaxD / 2] c, [kMaxD / 2] s of the current round
+  int* pq = reinterpret_cast<int*>(cs + kMaxD);      // [kMaxD / 2] p | q << 16
+  __shared__ int rotated, converged;
+  const int tid = threadIdx.x;
+  if (tid == 0) converged = d <= 1 ? 1 : 0;
+  build_normal_equations(S, d, 0.0, fit_intercept, V, r, mean, &misc[0]);
+  for (int t = tid; t < m * (m + 1) / 2; t += blockDim.x) AP[t] = 0.0;
+  __syncthreads();
+  for (int t = tid; t < d * d; t += blockDim.x) {
+    const int i = t / d, j = t - i * d;
+    if (i <= j) AP[packed_ix(i, j)] = V[i * pitch + j];
+  }
+  if (tid == 0) {
+    double mx = 0.0;
+    for (int i = 0; i < d; ++i) mx = fmax(mx, fabs(V[i * pitch + i]));
+    misc[1] = mx;
+  }
+  __syncthreads();
+  for (int t = tid; t < m * m; t += blockDim.x) V[t] = (t / m == t % m) ? 1.0 : 0.0;
+  __syncthreads();
+  const double floor_abs = 1e-20 * misc[1];
+  constexpr double kHalfEps = 1.1102230246251565e-16;
+  for (int sweep = 0; sweep < kEighMaxSweeps && d > 1; ++sweep) {
+    if (tid == 0) rotated = 0;
+    __syncthreads();
+    for (int round = 0; round < m - 1; ++round) {
+      // (1) the rotation of each pair
+      if (tid < M) {
+        int p, q;
+        rr_pair(m, round, tid, &p, &q);
+        const double app = AP[packed_ix(p, p)], aqq = AP[packed_ix(q, q)], apq = AP[packed_ix(p, q)];
+        double c = 1.0, s = 0.0;
+        if (fabs(apq) > floor_abs && fabs(apq) > kHalfEps * sqrt(fabs(app) * fabs(aqq))) {
+          const double tau = (aqq - app) / (2.0 * apq);
+          const double t = fabs(tau) > 1e150 ? 0.5 / tau
+                                             : (tau >= 0.0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1.0 + tau * tau));
+          c = 1.0 / sqrt(1.0 + t * t);
+          s = t * c;
+          rotated = 1;
+        }
+        cs[tid] = c;
+        cs[kMaxD / 2 + tid] = s;
+        pq[tid] = p | (q << 16);
+      }
+      __syncthreads();
+      // (2) A <- J^T A J block by block, V <- V J
+      for (int t = tid; t < M * M; t += blockDim.x) {
+        const int P1 = t / M, P2 = t - P1 * M;
+        if (P2 < P1) continue;
+        const int p1 = pq[P1] & 0xffff, q1 = pq[P1] >> 16, p2 = pq[P2] & 0xffff, q2 = pq[P2] >> 16;
+        const double c1 = cs[P1], s1 = cs[kMaxD / 2 + P1];
+        if (P1 == P2) {
+          if (s1 != 0.0) {
+            const double app = AP[packed_ix(p1, p1)], aqq = AP[packed_ix(q1, q1)], apq = AP[packed_ix(p1, q1)];
+            const double tt = s1 / c1;
+            AP[packed_ix(p1, p1)] = app - tt * apq;
+            AP[packed_ix(q1, q1)] = aqq + tt * apq;
+            AP[packed_ix(p1, q1)] = 0.0;
+          }
+          continue;
+        }
+        const double c2 = cs[P2], s2 = cs[kMaxD / 2 + P2];
+        if (s1 == 0.0 && s2 == 0.0) continue;
+        const int i11 = packed_ix(p1, p2), i12 = packed_ix(p1, q2), i21 = packed_ix(q1, p2), i22 = packed_ix(q1, q2);
+        const double x11 = AP[i11], x12 = AP[i12], x21 = AP[i21], x22 = AP[i22];
+        const double u11 = c1 * x11 - s1 * x21, u12 = c1 * x12 - s1 * x22;     // rows: J1^T B
+        const double u21 = s1 * x11 + c1 * x21, u22 = s1 * x12 + c1 * x22;
+        AP[i11] = c2 * u11 - s2 * u12;                                          // columns: (J1^T B) J2
+        AP[i12] = s2 * u11 + c2 * u12;
+        AP[i21] = c2 * u21 - s2 * u22;
+        AP[i22] = s2 * u21 + c2 * u22;
+      }
+      for (int t = tid; t < M * d; t += blockDim.x) {
+        const int P = t / d, i = t - P * d;
+        const double s = cs[kMaxD / 2 + P];
+        if (s == 0.0) continue;
+        const double c = cs[P];
+        const int p = pq[P] & 0xffff, q = pq[P] >> 16;
+        const double vp = V[p * m + i], vq = V[q * m + i];
+        V[p * m + i] = c * vp - s * vq;
+        V[q * m + i] = s * vp + c * vq;
+      }
+      __syncthreads();
+    }
+    if (!rotated) {
+      if (tid == 0) converged = 1;
+      break;
+    }
+    __syncthreads();
+  }
+  __syncthreads();
+  // ascending order by rank (ties by index), negative rounding eigenvalues as 0; c = Q^T r
+  for (int k = tid; k < d; k += blockDim.x) lam[k] = AP[packed_ix(k, k)];
+  __syncthreads();
+  const int dp = d + 2;
+  const double n = __ldcg(S + d * dp + d);
+  for (int k = tid; k < d; k += blockDim.x) {
+    const double lk = lam[k];
+    int rank = 0;
+    for (int j = 0; j < d; ++j) rank += (lam[j] < lk || (lam[j] == lk && j < k)) ? 1 : 0;
+    double ck = 0.0;
+    for (int i = 0; i < d; ++i) {
+      const double v = V[k * m + i];
+      loo[kLooQ + i * kMaxD + rank] = v;
+      ck = fma(v, r[i], ck);
+    }
+    loo[kLooLam + rank] = fmax(lk, 0.0);
+    loo[kLooC + rank] = ck;
+  }
+  for (int i = tid; i < d; i += blockDim.x) loo[kLooMean + i] = mean[i];
+  if (tid == 0) {
+    loo[kLooMisc + 0] = misc[0];
+    loo[kLooMisc + 1] = n;
+    loo[kLooMisc + 2] = fit_intercept && n > 0.0 ? 1.0 / n : 0.0;
+    loo[kLooMisc + 3] = converged ? 1.0 : 0.0;
+  }
+}
+
 size_t solve_smem_bytes(int d) {
   // Cholesky: A, mean, invd, misc, U panel; eigenvalue kernel: A, r, mean, misc, (v, w) x 2, pv, dd, ee2, lam
   const size_t chol = (size_t)(d + 1) * (d + 1) + 3 * d + 16 + (size_t)(d + 1) * kUPitch;
@@ -862,6 +1015,8 @@ int ensure_solve_attrs(b2_ctx* ctx) {
     B2_CUDA(cudaFuncSetAttribute(solve_cholesky_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B2_CUDA(cudaFuncSetAttribute(solve_spectral_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B2_CUDA(cudaFuncSetAttribute(solve_eigvals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B2_CUDA(cudaFuncSetAttribute(solve_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)eigh_smem_bytes(kMaxD)));
     ctx->solve_attr_set = true;
   }
   return B2_OK;
@@ -904,6 +1059,14 @@ int launch_solve_refine(b2_ctx* ctx, double alpha, int fit_intercept) {
 int launch_solve_spectral(b2_ctx* ctx, double cond, int fit_intercept) {
   if (int r = ensure_solve_attrs(ctx)) return r;
   solve_spectral_kernel<<<1, 512, solve_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, cond, fit_intercept, ctx->solve_out);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_solve_eigh(b2_ctx* ctx, int fit_intercept) {
+  if (int r = ensure_solve_attrs(ctx)) return r;
+  solve_eigh_kernel<<<1, kEighThreads, eigh_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, fit_intercept, ctx->loo);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return B2_OK;

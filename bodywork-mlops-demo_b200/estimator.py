@@ -44,6 +44,36 @@ def _as_f32_matrix(X) -> np.ndarray:
     return np.ascontiguousarray(X, dtype=np.float32)
 
 
+def _stage_rows(ctx: native.Context, X, y, row_mask):
+    """(X, y, row_mask, owned) in a form the context's fit entry points take: a ``DeviceArray`` as it is, float64 host
+    rows (65 536 or more) converted on the way up by ``upload_columns`` and left resident (``owned``: the device buffers
+    this call created, for the caller to free), any other host rows as contiguous float32."""
+    owned = []
+    if isinstance(X, native.DeviceArray):
+        return X, y, row_mask, owned
+    Xh = np.asarray(X)
+    if Xh.ndim == 2 and Xh.dtype == np.float64 and 0 < Xh.shape[1] <= native.MAX_D and Xh.shape[0] >= 65_536 \
+            and Xh.size * 4 <= _F64_UPLOAD_LIMIT:
+        # what scikit-learn users hand over: float64 rows.  numpy's astype(float32) is one thread; b2_upload_columns
+        # converts with the host threads of the bounce ring beside the H2D copies and leaves the rows resident
+        if np.asarray(y).size != Xh.shape[0]:
+            raise ValueError(f"Found input variables with inconsistent numbers of samples: "
+                             f"[{Xh.shape[0]}, {np.asarray(y).size}]")
+        X = ctx.upload_columns([Xh[:, j] for j in range(Xh.shape[1])])
+        y = ctx.to_device(np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32))
+        owned = [X, y]
+        if row_mask is not None and not isinstance(row_mask, native.DeviceArray):
+            row_mask = ctx.to_device(np.ascontiguousarray(row_mask, dtype=np.uint8))
+            owned.append(row_mask)
+        return X, y, row_mask, owned
+    X = _as_f32_matrix(X)
+    y = np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32)
+    if y.shape[0] != X.shape[0]:
+        raise ValueError(f"Found input variables with inconsistent numbers of samples: "
+                         f"[{X.shape[0]}, {y.shape[0]}]")
+    return X, y, row_mask, owned
+
+
 class B200LinearRegression:
     """The statistic S = [X 1 y]^T [X 1 y] of a fit lives in the (shared) context while the fit runs; whatever an
     estimator needs of it later -- the next ``partial_fit``, a deferred ``singular_`` / ``rank_`` -- is kept per
@@ -120,31 +150,8 @@ class B200LinearRegression:
         computed.  Wherever the spectrum is computed, a fit that keeps no rows (e.g. through ``row_mask``) raises
         ``ValueError``, as sklearn does for 0 samples."""
         ctx = self.ctx
-        owned = []                  # device buffers this call created (float64 host rows: converted on the way up)
-        if isinstance(X, native.DeviceArray):
-            d = X.shape[1]
-        else:
-            Xh = np.asarray(X)
-            if Xh.ndim == 2 and Xh.dtype == np.float64 and 0 < Xh.shape[1] <= native.MAX_D and Xh.shape[0] >= 65_536 \
-                    and Xh.size * 4 <= _F64_UPLOAD_LIMIT:
-                # what scikit-learn users hand over: float64 rows.  numpy's astype(float32) is one thread; b2_upload_columns
-                # converts with the host threads of the bounce ring beside the H2D copies and leaves the rows resident
-                if np.asarray(y).size != Xh.shape[0]:
-                    raise ValueError(f"Found input variables with inconsistent numbers of samples: "
-                                     f"[{Xh.shape[0]}, {np.asarray(y).size}]")
-                X = ctx.upload_columns([Xh[:, j] for j in range(Xh.shape[1])])
-                y = ctx.to_device(np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32))
-                owned = [X, y]
-                if row_mask is not None and not isinstance(row_mask, native.DeviceArray):
-                    row_mask = ctx.to_device(np.ascontiguousarray(row_mask, dtype=np.uint8))
-                    owned.append(row_mask)
-            else:
-                X = _as_f32_matrix(X)
-                y = np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32)
-                if y.shape[0] != X.shape[0]:
-                    raise ValueError(f"Found input variables with inconsistent numbers of samples: "
-                                     f"[{X.shape[0]}, {y.shape[0]}]")
-            d = X.shape[1]
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        d = X.shape[1]
         self._S = None
         self._drop_spectrum()
 
@@ -248,3 +255,121 @@ class B200LinearRegression:
     def __repr__(self) -> str:
         args = ([f"alpha={self.alpha}"] if self.alpha != 0.0 else []) + ([f"refine={self.refine}"] if self.refine else [])
         return f"B200LinearRegression({', '.join(args)})"
+
+
+def _check_alphas(alphas) -> np.ndarray:
+    """sklearn RidgeCV's validation of the grid (same wording)."""
+    al = np.asarray(alphas, dtype=np.float64).ravel()
+    if al.size == 0:
+        raise ValueError("alphas must be a non-empty array-like of floats > 0.0")
+    for i, a in enumerate(al):
+        if not np.isfinite(a):
+            raise ValueError(f"alphas[{i}] == {a}, must be a finite float > 0.0.")
+        if a <= 0.0:
+            raise ValueError(f"alphas[{i}] == {a}, must be > 0.0.")
+    return al
+
+
+def merge_alpha_chunks(chunks):
+    """The first-minimum rule of sklearn's RidgeCV over a grid searched in chunks of at most MAX_ALPHAS alphas:
+    ``chunks`` is a list of (offset, mse of the chunk); returns the global index of the first smallest mse."""
+    best, best_mse = 0, None
+    for off, mse in chunks:
+        for k, v in enumerate(np.asarray(mse, dtype=np.float64)):
+            if best_mse is None or v < best_mse:
+                best, best_mse = off + k, v
+    return best
+
+
+class B200RidgeCV:
+    """``sklearn.linear_model.RidgeCV(alphas, fit_intercept=..., store_cv_results=...)`` with its default ``cv=None``:
+    the alpha with the smallest exact leave-one-out squared error, found on the H100 by ``b2_ridge_loo`` (Gram,
+    eigendecomposition and one fp64 pass over the rows per chunk of up to MAX_ALPHAS alphas).  Ties go to the lowest
+    index, as in sklearn.  ``to_sklearn()`` returns a genuine RidgeCV carrying the fitted attributes."""
+
+    def __init__(self, alphas=(0.1, 1.0, 10.0), *, fit_intercept: bool = True, store_cv_results: bool = False,
+                 ctx: Optional[native.Context] = None):
+        self.alphas = alphas
+        self.fit_intercept = fit_intercept
+        self.store_cv_results = store_cv_results
+        self._ctx = ctx
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1) -> "B200RidgeCV":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets alpha_, best_score_, coef_, intercept_,
+        n_features_in_ and, with store_cv_results, cv_results_ of shape (rows kept, n_alphas)."""
+        al = _check_alphas(self.alphas)
+        ctx = self.ctx
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        d = X.shape[1]
+        try:
+            chunks, cvs, sols = [], [], []
+            for off in range(0, al.size, native.MAX_ALPHAS):
+                part = al[off: off + native.MAX_ALPHAS]
+                try:
+                    mse, best, coef, b0, cv = ctx.ridge_loo(X, y, part, row_mask, mask_keep,
+                                                            fit_intercept=self.fit_intercept,
+                                                            store_cv=self.store_cv_results)
+                except RuntimeError as exc:
+                    if "no row kept" in str(exc):
+                        raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is "
+                                         "required by B200RidgeCV.") from None
+                    raise
+                chunks.append((off, mse))
+                sols.append((off + best, coef, b0))
+                if cv is not None:
+                    cvs.append(cv.to_host() if isinstance(cv, native.DeviceArray) else cv)
+                    if isinstance(cv, native.DeviceArray):
+                        cv.free()
+        finally:
+            for a in owned:
+                a.free()
+        best = merge_alpha_chunks(chunks)
+        mse_all = np.concatenate([m for _, m in chunks])
+        coef, b0 = next((c, b) for i, c, b in sols if i == best)
+        if not (np.all(np.isfinite(coef)) and np.isfinite(b0) and np.isfinite(mse_all[best])):
+            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        self.alpha_ = float(al[best])
+        self.best_score_ = float(-mse_all[best])
+        self.coef_ = coef
+        self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
+        self.n_features_in_ = int(d)
+        if self.store_cv_results:
+            cv = np.concatenate(cvs, axis=1)
+            keep = ~np.isnan(cv[:, 0]) if cv.shape[0] else np.zeros(0, bool)
+            self.cv_results_ = cv[keep]
+        return self
+
+    def predict(self, X):
+        ctx = self.ctx
+        if isinstance(X, native.DeviceArray):
+            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
+            return yhat
+        Xh = _as_f32_matrix(X)
+        if Xh.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {Xh.shape[1]} features, but B200RidgeCV is expecting "
+                             f"{self.n_features_in_} features as input.")
+        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
+        return yhat.astype(np.float64)
+
+    def to_sklearn(self):
+        """A real sklearn RidgeCV with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
+        intercept_)."""
+        from sklearn.linear_model import RidgeCV
+        reg = RidgeCV(alphas=np.asarray(self.alphas, dtype=np.float64), fit_intercept=self.fit_intercept,
+                      store_cv_results=self.store_cv_results)
+        reg.alpha_ = float(self.alpha_)
+        reg.best_score_ = float(self.best_score_)
+        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
+        reg.intercept_ = np.float64(self.intercept_)
+        reg.n_features_in_ = int(self.n_features_in_)
+        if self.store_cv_results:
+            reg.cv_results_ = np.asarray(self.cv_results_, dtype=np.float64).copy()
+        return reg
+
+    def __repr__(self) -> str:
+        return f"B200RidgeCV(alphas={self.alphas!r})"

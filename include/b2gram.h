@@ -172,6 +172,31 @@ int b2_solve_spectral(b2_ctx* ctx, double cond, int fit_intercept, double* coef,
 int b2_solve_eigvals(b2_ctx* ctx, double cond, int fit_intercept, double* singular, int* rank,
                      int64_t* n_rows_out /* rows in S; may be NULL */);
 
+/* eigenvalues (ascending, d doubles) and eigenvectors (d x d row-major, column k belongs to eigenvalue k) of the
+ * centred Gram (uncentred when fit_intercept == 0) of the resident S; either pointer may be NULL.  Two-sided cyclic
+ * Jacobi on one SM: the eigenvectors are orthonormal to working precision for every eigenvalue, zero and clustered ones
+ * included.  Negative rounding eigenvalues are returned as 0.  B2_E_SINGULAR if the sweeps have not converged within
+ * their limit (30), which finite statistics at D <= 128 do not reach. */
+int b2_solve_eigh(b2_ctx* ctx, int fit_intercept, double* eigvals, double* eigvecs);
+
+/* ---- ridge with the alpha chosen by leave-one-out error: replaces sklearn.linear_model.RidgeCV(alphas).fit ------
+ * RidgeCV(alphas, fit_intercept).fit(X, y), cv=None: b2_fit's Gram of the kept rows, the eigendecomposition of its
+ * centred Gram, then one fp64 pass over the same rows for the leave-one-out error of every alpha (DESIGN section 6).
+ *   alphas    n_alphas (1..B2_MAX_ALPHAS) finite values > 0 (host)
+ *   mse_out   n_alphas doubles (host): mean squared leave-one-out error per alpha (sklearn: best_score_ = -mse_out[best])
+ *   cv_out    NULL, or n_rows x n_alphas doubles (row-major) where X lives (mem_kind): e^2 per row and alpha, NaN for
+ *             rows not kept (sklearn: cv_results_ with store_cv_results=True, after dropping those rows)
+ *   best_out  first index of the smallest mse (sklearn's tie rule); coef / intercept: the LDL^T solve at
+ *             alphas[best] from the same S, bit-identical to b2_fit(alpha = alphas[best]) on the same rows and settings
+ * Host rows with cv_out hold two device staging blocks of 262 144 x n_alphas doubles (134 MB at 64 alphas) in the
+ * context, grown to the widest call and freed with it.
+ * S afterwards is b2_fit's S.  B2_E_ARG: bad alphas / null outputs / no row kept; B2_E_UNSUPPORTED with > 1 rank;
+ * B2_E_SINGULAR as b2_solve_eigh. */
+#define B2_MAX_ALPHAS 64
+int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                 int mem_kind, const uint8_t* row_mask, int mask_keep, const double* alphas, int n_alphas,
+                 int fit_intercept, double* mse_out, double* cv_out, int* best_out, double* coef, double* intercept);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
