@@ -18,6 +18,7 @@ F32, BF16, F64 = 0, 1, 2
 MEM_DEVICE, MEM_HOST = 0, 1
 KERNEL_AUTO, KERNEL_SIMT, KERNEL_TCGEN05, KERNEL_NARROW = 0, 1, 2, 3
 PRECISION_SPLIT, PRECISION_BF16 = 0, 1
+E_ARG = -1
 E_SINGULAR = -4
 E_COMM = -5
 EXCHANGE_NONE, EXCHANGE_NCCL, EXCHANGE_PEER = 0, 1, 2
@@ -66,6 +67,8 @@ _SIGNATURES = {
     "b2_solve_eigvals": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_int), C.POINTER(_c_i64)]),
     "b2_solve_spectral": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.POINTER(C.c_double), _vp, C.POINTER(C.c_int)]),
     "b2_solve_eigh": (C.c_int, [_vp, C.c_int, _vp, _vp]),
+    "b2_solve_enet_path": (C.c_int, [_vp, C.c_int, C.c_double, _vp, C.c_int, C.c_double, C.c_int, C.c_double, C.c_int,
+                                     _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(C.c_double)]),
     "b2_ridge_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
                                C.c_int, _vp, _vp, C.POINTER(C.c_int), _vp, C.POINTER(C.c_double)]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
@@ -450,6 +453,41 @@ class Context:
         Q = np.empty((self.d, self.d), dtype=np.float64)
         _check(load().b2_solve_eigh(self._h, int(bool(fit_intercept)), lam.ctypes.data, Q.ctypes.data), "b2_solve_eigh")
         return lam, Q
+
+    def solve_enet_path(self, l1_ratio: float = 1.0, alphas=None, n_alphas: int = 100, eps: float = 1e-3,
+                        max_iter: int = 1000, tol: float = 1e-4, positive: bool = False, coef_init=None,
+                        fit_intercept: bool = True) -> dict:
+        """The elastic-net path of the resident statistic in one launch (b2_solve_enet_path): coordinate descent on the
+        centred Gram, as sklearn's enet_path(precompute=Gram).  ``alphas``: None for sklearn's grid of ``n_alphas``
+        values, else the alphas in the order they are solved.  Returns a dict of numpy arrays: alphas, coefs
+        (n_alphas, d), intercepts, gaps (dual gap / n), n_iter, and the scalar tol (tol ||yc||^2 / n).  Raises
+        ``ValueError`` for bad arguments and for a statistic without rows."""
+        d = self.d
+        al = None
+        if alphas is not None:
+            al = np.ascontiguousarray(np.asarray(alphas, dtype=np.float64).ravel())
+            n_alphas = al.size
+        ci = None
+        if coef_init is not None:
+            ci = np.ascontiguousarray(np.asarray(coef_init, dtype=np.float64).ravel())
+            if ci.size != d:
+                raise ValueError(f"coef_init has {ci.size} entries, the statistic has {d} features")
+        n_alphas = int(n_alphas)
+        k = max(n_alphas, 1)
+        out = {"alphas": np.empty(k), "coefs": np.empty((k, d)), "intercepts": np.empty(k), "gaps": np.empty(k),
+               "n_iter": np.empty(k, dtype=np.int32)}
+        tol_out = C.c_double(0.0)
+        rc = load().b2_solve_enet_path(self._h, int(bool(fit_intercept)), float(l1_ratio),
+                                       al.ctypes.data if al is not None else None, n_alphas, float(eps), int(max_iter),
+                                       float(tol), int(bool(positive)), ci.ctypes.data if ci is not None else None,
+                                       out["alphas"].ctypes.data, out["coefs"].ctypes.data,
+                                       out["intercepts"].ctypes.data, out["gaps"].ctypes.data,
+                                       out["n_iter"].ctypes.data, C.byref(tol_out))
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_solve_enet_path")
+        out["tol"] = float(tol_out.value)
+        return out
 
     def ridge_loo(self, X, y, alphas, row_mask=None, mask_keep: int = 1, fit_intercept: bool = True,
                   store_cv: bool = False):

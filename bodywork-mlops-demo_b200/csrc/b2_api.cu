@@ -411,7 +411,8 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
-                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1]};
+                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1],
+                  ctx->enet};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -882,6 +883,89 @@ int b2_solve_eigh(b2_ctx* ctx, int fit_intercept, double* eigvals, double* eigve
                               cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return eigh_converged(converged);
+}
+
+// ---- ElasticNet / Lasso: the coordinate-descent path of the resident S (DESIGN.md section 7) -------------------------
+// Host checks, the inputs into ctx->enet, one launch, the outputs back.  ctx->enet holds
+// [alphas A | coef_init kMaxD | coefs A x d | intercepts A | gaps A | iters A | tol_out 1] and grows to the largest call.
+int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const double* alphas, int n_alphas, double eps,
+                       int max_iter, double tol, int positive, const double* coef_init, double* alphas_out,
+                       double* coefs_out, double* intercepts_out, double* gaps_out, int* n_iter_out, double* tol_out) {
+  if (int r = use_device(ctx)) return r;
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (!(l1_ratio >= 0.0 && l1_ratio <= 1.0)) { set_error("l1_ratio=%g must be in [0, 1]", l1_ratio); return B2_E_ARG; }
+  if (n_alphas < 1) { set_error("n_alphas=%d must be >= 1", n_alphas); return B2_E_ARG; }
+  if (alphas == nullptr && l1_ratio == 0.0) {
+    set_error("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a grid by providing "
+              "your estimator with the appropriate `alphas=` argument.");
+    return B2_E_ARG;
+  }
+  if (alphas == nullptr && !(eps > 0.0 && isfinite(eps))) { set_error("eps=%g must be > 0 and finite", eps); return B2_E_ARG; }
+  if (alphas != nullptr)
+    for (int a = 0; a < n_alphas; ++a)
+      if (!(isfinite(alphas[a]) && alphas[a] >= 0.0)) {
+        set_error("alphas[%d] == %g, must be >= 0.0 and finite", a, alphas[a]);
+        return B2_E_ARG;
+      }
+  if (max_iter < 1) { set_error("max_iter=%d must be >= 1", max_iter); return B2_E_ARG; }
+  if (!(tol >= 0.0)) { set_error("tol must be >= 0"); return B2_E_ARG; }
+  if (alphas_out == nullptr || coefs_out == nullptr || intercepts_out == nullptr || gaps_out == nullptr ||
+      n_iter_out == nullptr) {
+    set_error("alphas_out / coefs_out / intercepts_out / gaps_out / n_iter_out is null");
+    return B2_E_ARG;
+  }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  const int d = ctx->d;
+  double n = 0.0;
+  B2_CUDA(cudaMemcpyAsync(&n, ctx->S + (size_t)d * (d + 2) + d, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (!(n > 0.0)) { set_error("no row kept: the statistic holds no rows"); return B2_E_ARG; }
+  const size_t A = (size_t)n_alphas;
+  const size_t need = A + kMaxD + A * d + 3 * A + 1;
+  if (ctx->enet_doubles < need) {
+    if (ctx->enet != nullptr) cudaFree(ctx->enet);
+    ctx->enet = nullptr;
+    ctx->enet_doubles = 0;
+    if (cudaMalloc(reinterpret_cast<void**>(&ctx->enet), sizeof(double) * need) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("out of device memory for the elastic-net path (%d alphas)", n_alphas);
+      return B2_E_CUDA;
+    }
+    ctx->enet_doubles = need;
+  }
+  EnetArgs args;
+  args.l1_ratio = l1_ratio;
+  args.eps = eps;
+  args.tol = tol;
+  args.n_alphas = n_alphas;
+  args.grid = alphas == nullptr ? 1 : 0;
+  args.max_iter = max_iter;
+  args.positive = positive ? 1 : 0;
+  args.fit_intercept = fit_intercept ? 1 : 0;
+  args.alphas = ctx->enet;
+  args.coef_init = coef_init != nullptr ? ctx->enet + A : nullptr;
+  args.coefs = ctx->enet + A + kMaxD;
+  args.intercepts = args.coefs + A * d;
+  args.gaps = args.intercepts + A;
+  args.iters = args.gaps + A;
+  args.tol_out = args.iters + A;
+  if (alphas != nullptr)
+    B2_CUDA(cudaMemcpyAsync(args.alphas, alphas, sizeof(double) * A, cudaMemcpyHostToDevice, ctx->stream));
+  if (coef_init != nullptr)
+    B2_CUDA(cudaMemcpyAsync(ctx->enet + A, coef_init, sizeof(double) * d, cudaMemcpyHostToDevice, ctx->stream));
+  if (int r = launch_solve_enet(ctx, args)) return r;
+  std::vector<double> iters(A);
+  double tol_abs = 0.0;
+  B2_CUDA(cudaMemcpyAsync(alphas_out, args.alphas, sizeof(double) * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(coefs_out, args.coefs, sizeof(double) * A * d, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(intercepts_out, args.intercepts, sizeof(double) * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(gaps_out, args.gaps, sizeof(double) * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(iters.data(), args.iters, sizeof(double) * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(&tol_abs, args.tol_out, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (size_t a = 0; a < A; ++a) n_iter_out[a] = (int)iters[a];
+  if (tol_out != nullptr) *tol_out = tol_abs;
+  return B2_OK;
 }
 
 // The Gram of b2_fit, the eigendecomposition of its centred Gram, one leave-one-out pass over the same rows (host rows

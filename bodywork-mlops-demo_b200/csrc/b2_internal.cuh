@@ -78,6 +78,18 @@ constexpr int kLooW = kLooCw + kMaxD * kMaxAlphas;   // [kMaxD][kMaxAlphas] 1 / 
 constexpr int kLooSum = kLooW + kMaxD * kMaxAlphas;  // the reduced sums of e^2 per alpha [kMaxAlphas]
 constexpr int kLooDoubles = kLooSum + kMaxAlphas;
 
+// ---- the elastic-net path of b2_solve_enet_path (solve.cu: solve_enet_kernel) -----------------------------------------
+// Every pointer is into ctx->enet.  alphas: the call's alphas (grid != 0: the kernel writes sklearn's grid there);
+// coef_init: nullptr or d starting coefficients; outputs per alpha: coefs [n_alphas][d], intercepts, gaps (dual gap / n)
+// and iters (as doubles); tol_out: tol * y_norm2 / n.
+struct EnetArgs {
+  double l1_ratio, eps, tol;
+  int n_alphas, grid, max_iter, positive, fit_intercept;
+  double* alphas;
+  const double* coef_init;
+  double *coefs, *intercepts, *gaps, *iters, *tol_out;
+};
+
 // template width of the one-lane-per-row kernels (gram_narrow.cu, score.cu) for d <= 16 features: the next power of two
 inline int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
 
@@ -141,6 +153,9 @@ struct b2_ctx {
   double* loo_part = nullptr;          // [sm_count][kMaxAlphas] per-CTA sums of e^2
   double* cv_stage[2] = {nullptr, nullptr};   // e^2 staging blocks of host rows [stage_rows][cv_stage_alphas]
   int cv_stage_alphas = 0;             // alphas per row the staging blocks hold (grown to a call's n_alphas)
+  // elastic-net path: inputs and outputs of b2_solve_enet_path (b2::EnetArgs), grown to the largest call
+  double* enet = nullptr;
+  size_t enet_doubles = 0;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -268,6 +283,8 @@ int launch_solve_eigh(b2_ctx* ctx, int fit_intercept);
 // reduce of the per-CTA sums into ctx->loo + kLooSum (`first_block` overwrites, otherwise adds)
 int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                const uint8_t* mask, int keep, int n_alphas, double* cv, bool first_block);
+// the elastic-net path of the resident S (one launch; `args` points into ctx->enet)
+int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

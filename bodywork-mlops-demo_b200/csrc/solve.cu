@@ -1001,6 +1001,267 @@ solve_eigh_kernel(const double* __restrict__ S, int d, int fit_intercept, double
   }
 }
 
+// ---- elastic net: a whole regularisation path by cyclic coordinate descent on the centred Gram (b2_solve_enet_path) --
+// Restates scikit-learn's enet_coordinate_descent_gram (sklearn/linear_model/_cd_fast.pyx) with enet_path's scaling
+// (l1_reg = alpha l1_ratio n, l2_reg = alpha (1 - l1_ratio) n) and, without user alphas, its _alpha_grid.  Q, q come
+// from build_normal_equations at alpha = 0; y_norm2 = S_yy - n ybar^2.  DESIGN.md section 7.
+//   Constant columns: a column whose centred diagonal is not above kEnetConstCol times its raw one (standard deviation
+//   <= 1e-6 of its root mean square, 16 fp32 ulps) has a centred Gram row and column of rounding noise; it is treated as
+//   exactly constant -- Q row and column and q_j zeroed, coefficient 0, never updated -- which is what sklearn does for
+//   Q_jj == 0 on exactly centred rows.
+//   One warp runs everything after the build (the sweeps are one dependent chain): lane l holds (Qw, w, q, Q_jj and
+//   1 / (Q_jj + l2_reg)) of features l + 32 u, so there is no division in the chain.  The step of coordinate j, formed by
+//   its owner lane, goes to every lane by one shuffle and each lane applies its entries of Q's row j (shared memory).  The
+//   active set is a 128-bit mask walked with __ffs inside a static loop over u, so the register arrays stay statically
+//   indexed.  Reductions are xor butterflies: every lane gets the same value, and repeated calls are bit-identical.
+constexpr int kEnetThreads = 256;
+constexpr double kEnetConstCol = 1e-12;
+constexpr double kF64Resolution = 1e-15;     // np.finfo(np.float64).resolution
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double warp_max(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// gap_enet_gram: formulation A (l1 > 0), B (l1 == 0 < l2) or the squared OLS gradient (both 0); xta = X^T R - l2 w (X^T R
+// without an L1 term) per owned feature, *dual_norm as sklearn's dual_norm_XtA.  Features >= d hold zeros throughout.
+__device__ __forceinline__ double enet_gap(const double (&w)[4], const double (&qw)[4], const double (&q)[4], int d,
+                                           int lane, double l1, double l2, double y_norm2, bool positive,
+                                           double (&xta)[4], double* dual_norm) {
+  double ww = 0.0, qdw = 0.0, wqw = 0.0, wl1 = 0.0, dn = l1 == 0.0 ? 0.0 : -INFINITY;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const bool live = lane + 32 * u < d;
+    ww = fma(w[u], w[u], ww);
+    qdw = fma(w[u], q[u], qdw);
+    wqw = fma(w[u], qw[u], wqw);
+    wl1 += fabs(w[u]);
+    if (l1 == 0.0) {
+      xta[u] = q[u] - qw[u];
+      dn = fma(xta[u], xta[u], dn);
+    } else {
+      xta[u] = q[u] - qw[u] - l2 * w[u];
+      if (live) dn = fmax(dn, positive ? xta[u] : fabs(xta[u]));
+    }
+  }
+  qdw = warp_sum(qdw);
+  wqw = warp_sum(wqw);
+  ww = l2 > 0.0 ? warp_sum(ww) : 0.0;
+  const double r_norm2 = y_norm2 + wqw - 2.0 * qdw;
+  const double ry = y_norm2 - qdw;
+  if (l1 == 0.0) {
+    dn = warp_sum(dn);
+    *dual_norm = dn;
+    if (l2 == 0.0) return dn;
+    return r_norm2 + 0.5 * l2 * ww - ry + 1.0 / (2.0 * l2) * dn;
+  }
+  dn = warp_max(dn);
+  wl1 = warp_sum(wl1);
+  *dual_norm = dn;
+  const double primal = 0.5 * (r_norm2 + l2 * ww) + l1 * wl1;
+  const double scale = dn > l1 ? l1 / dn : 1.0;
+  const double dual = -0.5 * (scale * scale) * (r_norm2 + l2 * ww) + scale * ry;
+  return primal - dual;
+}
+
+__global__ void __launch_bounds__(kEnetThreads, 1)
+solve_enet_kernel(const double* __restrict__ S, int d, EnetArgs a) {
+  extern __shared__ double sm[];
+  const int pitch = d + 1, dp = d + 2;
+  double* Q = sm;                          // d x d, pitch d + 1; row d = q
+  double* r = Q + d * pitch;
+  double* mean = Q + (d + 1) * pitch;
+  double* wsh = mean + d;                  // [kMaxD] w at the start of an alpha (for Q w)
+  double* misc = wsh + kMaxD;              // [0] ybar
+  build_normal_equations(S, d, 0.0, a.fit_intercept, Q, r, mean, &misc[0]);
+  if (threadIdx.x >= 32) return;           // one warp from here on: __syncwarp only
+  const int lane = threadIdx.x;
+  const double n = __ldcg(S + d * dp + d);
+  const double ybar = misc[0];
+  const double y_norm2 = __ldcg(S + (d + 1) * dp + d + 1) - n * ybar * ybar;
+  const bool positive = a.positive != 0;
+
+  // constant columns: zero their row, column and q entry (the build has finished: its last barrier preceded this)
+  unsigned int live[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int f = lane + 32 * u;
+    const bool ok = f < d && Q[f * pitch + f] > kEnetConstCol * __ldcg(S + f * dp + f);
+    const bool dead = f < d && !ok;
+    live[u] = __ballot_sync(0xffffffffu, ok);
+    unsigned int m = __ballot_sync(0xffffffffu, dead);
+    while (m) {
+      const int j = __ffs(m) - 1 + 32 * u;
+      m &= m - 1;
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const int g = lane + 32 * v;
+        if (g < d) { Q[j * pitch + g] = 0.0; Q[g * pitch + j] = 0.0; }
+      }
+      if (lane == 0) r[j] = 0.0;
+    }
+  }
+  __syncwarp();
+  double w[4], qw[4], q[4], qjj[4], rinv[4], xta[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int f = lane + 32 * u;
+    const bool ok = (live[u] >> lane) & 1u;
+    q[u] = f < d ? r[f] : 0.0;
+    qjj[u] = f < d ? Q[f * pitch + f] : 0.0;
+    w[u] = (ok && a.coef_init != nullptr) ? a.coef_init[f] : 0.0;
+  }
+
+  // sklearn's _alpha_grid: geomspace(alpha_max, alpha_max eps, n_alphas), or a constant grid at the fp64 resolution
+  if (a.grid) {
+    double mx = 0.0;
+#pragma unroll
+    for (int u = 0; u < 4; ++u) mx = fmax(mx, positive ? q[u] : fabs(q[u]));
+    mx = warp_max(mx);
+    const double amax = mx / (n * a.l1_ratio);
+    const double amin = amax * a.eps;
+    const double ls = log10(amax), step = a.n_alphas > 1 ? (log10(amin) - ls) / (double)(a.n_alphas - 1) : 0.0;
+    for (int i = lane; i < a.n_alphas; i += 32) {
+      double v = exp10(__dadd_rn(__dmul_rn((double)i, step), ls));
+      if (i == 0) v = amax;
+      if (i == a.n_alphas - 1 && i > 0) v = amin;
+      a.alphas[i] = amax <= kF64Resolution ? kF64Resolution : v;
+    }
+    __syncwarp();
+  }
+
+  const double tol_abs = a.tol * y_norm2;
+  if (lane == 0) *a.tol_out = tol_abs / n;
+  for (int ia = 0; ia < a.n_alphas; ++ia) {
+    const double alpha = a.alphas[ia];
+    const double l1 = alpha * a.l1_ratio * n, l2 = alpha * (1.0 - a.l1_ratio) * n;
+    // Qw = Q w from scratch (as sklearn's np.dot at every alpha), Q read by columns: lane-consecutive addresses
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (lane + 32 * u < d) wsh[lane + 32 * u] = w[u];
+      rinv[u] = qjj[u] > 0.0 ? 1.0 / (qjj[u] + l2) : 0.0;
+      qw[u] = 0.0;
+    }
+    __syncwarp();
+    for (int k = 0; k < d; ++k) {
+      const double wk = wsh[k];
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+        if (lane + 32 * u < d) qw[u] = fma(Q[k * pitch + lane + 32 * u], wk, qw[u]);
+    }
+    double dn;
+    double gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
+    int iters = 0;
+    if (!(gap >= 0.0 && gap <= tol_abs)) {
+      const bool screening = l1 > 0.0;
+      unsigned int act[4];
+      // gap-safe screening (sklearn: Fercoq et al. eq. 11) over the candidates `cand`: kept features form the active
+      // set, the others leave it for good, their w (if any) taken out of Qw in feature order
+      auto screen = [&](const unsigned int (&cand)[4]) {
+        const double radius = sqrt(2.0 * fabs(gap)) / l1;
+        const double theta_scale = fmax(l1, dn);
+        unsigned int drop[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const bool c = (cand[u] >> lane) & 1u;
+          const bool keep = c && qjj[u] != 0.0 && (1.0 - fabs(xta[u] / theta_scale)) / sqrt(qjj[u] + l2) <= radius;
+          act[u] = __ballot_sync(0xffffffffu, keep);
+          drop[u] = __ballot_sync(0xffffffffu, c && !keep && w[u] != 0.0);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          unsigned int m = drop[u];
+          while (m) {
+            const int l = __ffs(m) - 1;
+            m &= m - 1;
+            const double wj = __shfl_sync(0xffffffffu, w[u], l);
+            if (lane == l) w[u] = 0.0;
+            const double* row = Q + (l + 32 * u) * pitch;
+#pragma unroll
+            for (int v = 0; v < 4; ++v)
+              if (lane + 32 * v < d) qw[v] = fma(-wj, row[lane + 32 * v], qw[v]);
+          }
+        }
+      };
+      if (screening) {
+        unsigned int all[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) all[u] = __ballot_sync(0xffffffffu, lane + 32 * u < d);
+        screen(all);
+      } else {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) act[u] = live[u];
+      }
+      iters = a.max_iter;
+      for (int it = 0; it < a.max_iter; ++it) {
+        double dw_max = 0.0, w_max = 0.0;
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          unsigned int m = act[u];
+          while (m) {
+            const int l = __ffs(m) - 1;
+            m &= m - 1;
+            const double* row = Q + (l + 32 * u) * pitch;
+            double rv[4];                                  // row j: its loads do not wait for the step
+#pragma unroll
+            for (int v = 0; v < 4; ++v) rv[v] = lane + 32 * v < d ? row[lane + 32 * v] : 0.0;
+            // Branch-free: every lane evaluates the update of its own feature lane + 32 u and the shuffle takes lane
+            // l's.  The chain per coordinate is t -> soft threshold -> step -> shuffle -> the owner's Qw FMA.  A zero
+            // step adds an exact zero to Qw (sklearn skips it; the value is the same).
+            const double wj = w[u];
+            const double t = fma(wj, qjj[u], q[u]) - qw[u];
+            const double mag = fmax(fabs(t) - l1, 0.0) * rinv[u];
+            const double nw = (positive && t < 0.0) ? 0.0 : (t > 0.0 ? mag : (t < 0.0 ? -mag : 0.0));
+            const double delta = __shfl_sync(0xffffffffu, nw - wj, l);
+            const bool own = lane == l;
+            w[u] = own ? nw : wj;
+            dw_max = own ? fmax(dw_max, fabs(delta)) : dw_max;
+            w_max = own ? fmax(w_max, fabs(nw)) : w_max;
+#pragma unroll
+            for (int v = 0; v < 4; ++v) qw[v] = fma(delta, rv[v], qw[v]);
+          }
+        }
+        dw_max = warp_max(dw_max);
+        w_max = warp_max(w_max);
+        if (w_max == 0.0 || dw_max / w_max <= a.tol || it == a.max_iter - 1) {
+          gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
+          if (gap <= tol_abs) {
+            iters = it + 1;
+            break;
+          }
+          if (screening) {
+            const unsigned int cand[4] = {act[0], act[1], act[2], act[3]};
+            screen(cand);
+          }
+        }
+      }
+    }
+    double part = 0.0;
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int f = lane + 32 * u;
+      if (f < d) {
+        a.coefs[(size_t)ia * d + f] = w[u];
+        part = fma(mean[f], w[u], part);
+      }
+    }
+    part = warp_sum(part);
+    if (lane == 0) {
+      a.intercepts[ia] = ybar - part;
+      a.gaps[ia] = gap / n;
+      a.iters[ia] = (double)iters;
+    }
+  }
+}
+
+size_t enet_smem_bytes(int d) { return sizeof(double) * ((size_t)(d + 1) * (d + 1) + d + kMaxD + 8); }
+
 size_t solve_smem_bytes(int d) {
   // Cholesky: A, mean, invd, misc, U panel; eigenvalue kernel: A, r, mean, misc, (v, w) x 2, pv, dd, ee2, lam
   const size_t chol = (size_t)(d + 1) * (d + 1) + 3 * d + 16 + (size_t)(d + 1) * kUPitch;
@@ -1017,6 +1278,8 @@ int ensure_solve_attrs(b2_ctx* ctx) {
     B2_CUDA(cudaFuncSetAttribute(solve_eigvals_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B2_CUDA(cudaFuncSetAttribute(solve_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)eigh_smem_bytes(kMaxD)));
+    B2_CUDA(cudaFuncSetAttribute(solve_enet_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)enet_smem_bytes(kMaxD)));
     ctx->solve_attr_set = true;
   }
   return B2_OK;
@@ -1067,6 +1330,14 @@ int launch_solve_spectral(b2_ctx* ctx, double cond, int fit_intercept) {
 int launch_solve_eigh(b2_ctx* ctx, int fit_intercept) {
   if (int r = ensure_solve_attrs(ctx)) return r;
   solve_eigh_kernel<<<1, kEighThreads, eigh_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, fit_intercept, ctx->loo);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args) {
+  if (int r = ensure_solve_attrs(ctx)) return r;
+  solve_enet_kernel<<<1, kEnetThreads, enet_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, args);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return B2_OK;

@@ -373,3 +373,188 @@ class B200RidgeCV:
 
     def __repr__(self) -> str:
         return f"B200RidgeCV(alphas={self.alphas!r})"
+
+
+# ---- ElasticNet / Lasso: coordinate descent on the fp64 Gram (b2_solve_enet_path, DESIGN.md section 7) -----------------
+_MESSAGE_CONV = ("Objective did not converge. You might want to increase the number of iterations, check the scale of the "
+                 "features or consider increasing regularisation.")
+_MESSAGE_RIDGE = ("Linear regression models with a zero l1 penalization strength are more efficiently fitted using one of "
+                  "the solvers implemented in sklearn.linear_model.Ridge/RidgeCV instead.")
+
+
+def _gram_of_rows(ctx: native.Context, X, y, row_mask, mask_keep: int) -> int:
+    """S of the rows (b2_gram_reset + b2_gram_accumulate: the Gram dispatch every fit uses) left resident; returns D."""
+    X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+    d = X.shape[1]
+    try:
+        ctx.gram_reset(d)
+        ctx.gram_accumulate(X, y, row_mask, mask_keep)
+    finally:
+        for a in owned:
+            a.free()
+    return d
+
+
+def _solve_path(ctx: native.Context, d: int, who: str, **kw) -> dict:
+    try:
+        return ctx.solve_enet_path(**kw)
+    except ValueError as exc:
+        if "no row kept" in str(exc):
+            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
+                             f"{who}.") from None
+        raise
+
+
+def _warn_unconverged(ctx: native.Context, res: dict, l1_ratio: float, max_iter: int) -> None:
+    """sklearn's ConvergenceWarning for every alpha that ran out of sweeps above the gap tolerance (its wording, with the
+    gap and tolerance on cd_fast's scale: n times the dual_gaps scale)."""
+    late = [i for i in range(res["gaps"].size) if res["n_iter"][i] >= max_iter and res["gaps"][i] > res["tol"]]
+    if not late:
+        return
+    from sklearn.exceptions import ConvergenceWarning
+    n = float(ctx.gram_export()[-2, -2])
+    for i in late:
+        message = _MESSAGE_CONV + f" Duality gap: {res['gaps'][i] * n:.6e}, tolerance: {res['tol'] * n:.3e}"
+        if res["alphas"][i] * l1_ratio * n < np.finfo(np.float64).eps:
+            message += "\n" + _MESSAGE_RIDGE
+        warnings.warn(message, ConvergenceWarning, stacklevel=3)
+
+
+class B200ElasticNet:
+    """``sklearn.linear_model.ElasticNet`` (cyclic selection) fitted on the H100: the rows go through the Gram kernels
+    once, then ``b2_solve_enet_path`` runs sklearn's Gram coordinate descent (``precompute=True``) for the one alpha on
+    one SM.  Sets coef_, intercept_, dual_gap_, n_iter_ and n_features_in_; ``to_sklearn()`` returns a genuine
+    ElasticNet carrying them."""
+    _sk_name = "ElasticNet"
+
+    def __init__(self, alpha: float = 1.0, *, l1_ratio: float = 0.5, fit_intercept: bool = True, max_iter: int = 1000,
+                 tol: float = 1e-4, positive: bool = False, warm_start: bool = False, selection: str = "cyclic",
+                 ctx: Optional[native.Context] = None):
+        self.alpha = alpha
+        self.l1_ratio = l1_ratio
+        self.fit_intercept = fit_intercept
+        self.max_iter = max_iter
+        self.tol = tol
+        self.positive = positive
+        self.warm_start = warm_start
+        self.selection = selection
+        self._ctx = ctx
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1):
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``."""
+        if self.selection == "random":
+            raise ValueError("selection='random' is not supported: the GPU solver runs sklearn's cyclic order only")
+        if self.selection != "cyclic":
+            raise ValueError("selection should be either random or cyclic.")
+        if not (np.isfinite(self.alpha) and self.alpha >= 0):
+            raise ValueError(f"alpha must be a finite float >= 0, got {self.alpha!r}")
+        ctx = self.ctx
+        d = _gram_of_rows(ctx, X, y, row_mask, mask_keep)
+        coef_init = None
+        if self.warm_start and getattr(self, "coef_", None) is not None and np.asarray(self.coef_).size == d:
+            coef_init = self.coef_
+        res = _solve_path(ctx, d, f"B200{self._sk_name}", l1_ratio=self.l1_ratio, alphas=[float(self.alpha)],
+                          max_iter=self.max_iter, tol=self.tol, positive=self.positive, coef_init=coef_init,
+                          fit_intercept=self.fit_intercept)
+        coef, b0 = res["coefs"][0], float(res["intercepts"][0])
+        if not (np.all(np.isfinite(coef)) and np.isfinite(b0)):
+            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _warn_unconverged(ctx, res, self.l1_ratio, self.max_iter)
+        self.coef_ = coef.copy()
+        self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
+        self.dual_gap_ = np.float64(res["gaps"][0])
+        self.n_iter_ = int(res["n_iter"][0])
+        self.n_features_in_ = int(d)
+        return self
+
+    def predict(self, X):
+        ctx = self.ctx
+        if isinstance(X, native.DeviceArray):
+            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
+            return yhat
+        Xh = _as_f32_matrix(X)
+        if Xh.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
+        return yhat.astype(np.float64)
+
+    def _sk_params(self) -> dict:
+        return dict(alpha=self.alpha, l1_ratio=self.l1_ratio, fit_intercept=self.fit_intercept, precompute=True,
+                    max_iter=self.max_iter, tol=self.tol, positive=self.positive, warm_start=self.warm_start,
+                    selection=self.selection)
+
+    def to_sklearn(self):
+        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
+        intercept_).  ``precompute=True``: the Gram solver this fit restates."""
+        from sklearn import linear_model
+        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
+        reg.intercept_ = np.float64(self.intercept_)
+        reg.dual_gap_ = np.float64(self.dual_gap_)
+        reg.n_iter_ = int(self.n_iter_)
+        reg.n_features_in_ = int(self.n_features_in_)
+        return reg
+
+    def __repr__(self) -> str:
+        return f"B200{self._sk_name}(alpha={self.alpha}, l1_ratio={self.l1_ratio})"
+
+
+class B200Lasso(B200ElasticNet):
+    """``sklearn.linear_model.Lasso``: B200ElasticNet with l1_ratio = 1."""
+    _sk_name = "Lasso"
+
+    def __init__(self, alpha: float = 1.0, *, fit_intercept: bool = True, max_iter: int = 1000, tol: float = 1e-4,
+                 positive: bool = False, warm_start: bool = False, selection: str = "cyclic",
+                 ctx: Optional[native.Context] = None):
+        super().__init__(alpha, l1_ratio=1.0, fit_intercept=fit_intercept, max_iter=max_iter, tol=tol,
+                         positive=positive, warm_start=warm_start, selection=selection, ctx=ctx)
+
+    def _sk_params(self) -> dict:
+        p = super()._sk_params()
+        del p["l1_ratio"]
+        return p
+
+    def __repr__(self) -> str:
+        return f"B200Lasso(alpha={self.alpha})"
+
+
+def enet_path(X, y, *, l1_ratio=0.5, eps=1e-3, alphas=100, coef_init=None, return_n_iter=False, positive=False,
+              fit_intercept=False, max_iter=1000, tol=1e-4, row_mask=None, mask_keep=1, ctx=None):
+    """sklearn 1.9's ``enet_path`` on the H100: one Gram pass over the rows, then the whole path in one launch.
+    ``alphas``: an int (the size of sklearn's grid from alpha_max down to alpha_max * eps) or an array (sorted
+    descending, as sklearn does).  Returns (alphas, coefs of shape (D, n_alphas), dual_gaps), plus n_iters with
+    ``return_n_iter``.  ``fit_intercept=False`` (sklearn's path does not centre) solves on the raw rows; with
+    ``fit_intercept=True`` the path runs on the centred Gram and the intercepts of every alpha are appended to the
+    returned tuple."""
+    ctx = ctx if ctx is not None else default_context()
+    if isinstance(alphas, (int, np.integer)) and not isinstance(alphas, bool):
+        al, n_alphas = None, int(alphas)
+        if n_alphas < 1:
+            raise ValueError(f"alphas must be >= 1 when given as an integer, got {n_alphas}")
+    else:
+        al = np.sort(np.asarray(alphas, dtype=np.float64).ravel())[::-1]
+        n_alphas = al.size
+    d = _gram_of_rows(ctx, X, y, row_mask, mask_keep)
+    res = _solve_path(ctx, d, "enet_path", l1_ratio=l1_ratio, alphas=al, n_alphas=n_alphas, eps=eps,
+                      max_iter=max_iter, tol=tol, positive=positive, coef_init=coef_init, fit_intercept=fit_intercept)
+    _warn_unconverged(ctx, res, l1_ratio, max_iter)
+    out = (res["alphas"], res["coefs"].T.copy(), res["gaps"])
+    if return_n_iter:
+        out += ([int(k) for k in res["n_iter"]],)
+    if fit_intercept:
+        out += (res["intercepts"],)
+    return out
+
+
+def lasso_path(X, y, *, eps=1e-3, alphas=100, coef_init=None, return_n_iter=False, positive=False,
+               fit_intercept=False, max_iter=1000, tol=1e-4, row_mask=None, mask_keep=1, ctx=None):
+    """sklearn 1.9's ``lasso_path``: ``enet_path`` with l1_ratio = 1."""
+    return enet_path(X, y, l1_ratio=1.0, eps=eps, alphas=alphas, coef_init=coef_init, return_n_iter=return_n_iter,
+                     positive=positive, fit_intercept=fit_intercept, max_iter=max_iter, tol=tol, row_mask=row_mask,
+                     mask_keep=mask_keep, ctx=ctx)

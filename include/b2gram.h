@@ -179,6 +179,27 @@ int b2_solve_eigvals(b2_ctx* ctx, double cond, int fit_intercept, double* singul
  * their limit (30), which finite statistics at D <= 128 do not reach. */
 int b2_solve_eigh(b2_ctx* ctx, int fit_intercept, double* eigvals, double* eigvecs);
 
+/* ---- elastic net / lasso path: replaces sklearn.linear_model.enet_path(precompute=Gram) / ElasticNet / Lasso -------
+ * reference: sklearn/linear_model/_coordinate_descent.py enet_path (alpha scaling, _alpha_grid) and _cd_fast.pyx
+ * enet_coordinate_descent_gram (cyclic coordinate descent, dual gap, gap-safe screening, stopping rule), run on the
+ * centred Gram Q = Xc^T Xc, q = Xc^T yc and ||yc||^2 of the resident S (uncentred without fit_intercept); one
+ * single-SM launch for the whole path (DESIGN section 7).  Minimises, per alpha,
+ *   1 / (2 n) ||yc - Xc w||^2 + alpha l1_ratio ||w||_1 + alpha (1 - l1_ratio) / 2 ||w||^2   (w >= 0 with positive)
+ *   alphas      NULL: sklearn's grid geomspace(alpha_max, alpha_max eps, n_alphas), alpha_max = max |q| / (n l1_ratio)
+ *               (max(0, max q) with positive); else n_alphas finite values >= 0, solved in the order given (host)
+ *   coef_init   NULL (zeros) or d doubles: the start of the first alpha; each later alpha starts from the previous one
+ *   outputs     (host) alphas_out n_alphas, coefs_out n_alphas x d (row-major), intercepts_out ybar - m.w,
+ *               gaps_out the dual gap / n (sklearn's dual_gaps), n_iter_out sweeps (0: the start already met the gap),
+ *               tol_out NULL or tol ||yc||^2 / n, the gap each alpha had to reach
+ * A column whose centred diagonal is <= 1e-12 of its raw one is constant: coefficient 0, never updated.  Not reaching
+ * the gap within max_iter sweeps is no error: n_iter_out == max_iter and gaps_out > tol_out.  The outputs are staged in
+ * a device block of the context, grown to the largest call and freed with it.  B2_E_ARG: l1_ratio outside [0, 1], a
+ * grid with l1_ratio == 0 or eps <= 0, an alpha < 0 or not finite, n_alphas < 1, max_iter < 1, tol < 0, a null output,
+ * or a statistic without rows. */
+int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const double* alphas, int n_alphas, double eps,
+                       int max_iter, double tol, int positive, const double* coef_init, double* alphas_out,
+                       double* coefs_out, double* intercepts_out, double* gaps_out, int* n_iter_out, double* tol_out);
+
 /* ---- ridge with the alpha chosen by leave-one-out error: replaces sklearn.linear_model.RidgeCV(alphas).fit ------
  * RidgeCV(alphas, fit_intercept).fit(X, y), cv=None: b2_fit's Gram of the kept rows, the eigendecomposition of its
  * centred Gram, then one fp64 pass over the same rows for the leave-one-out error of every alpha (DESIGN section 6).
