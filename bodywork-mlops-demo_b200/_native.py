@@ -69,6 +69,9 @@ _SIGNATURES = {
     "b2_solve_eigh": (C.c_int, [_vp, C.c_int, _vp, _vp]),
     "b2_solve_enet_path": (C.c_int, [_vp, C.c_int, C.c_double, _vp, C.c_int, C.c_double, C.c_int, C.c_double, C.c_int,
                                      _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(C.c_double)]),
+    "b2_gram_folds": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp]),
+    "b2_solve_enet_cv": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_double, C.c_int,
+                                   C.c_double, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "b2_ridge_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
                                C.c_int, _vp, _vp, C.POINTER(C.c_int), _vp, C.POINTER(C.c_double)]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
@@ -487,6 +490,59 @@ class Context:
             raise ValueError(last_error())
         _check(rc, "b2_solve_enet_path")
         out["tol"] = float(tol_out.value)
+        return out
+
+    def gram_folds(self, X, y, fold_of_row, n_folds: int) -> np.ndarray:
+        """The statistic of every fold in one call (b2_gram_folds): row r belongs to fold ``fold_of_row[r]`` (uint8, where
+        X lives; ids >= n_folds drop the row).  Leaves S = the sum of the folds resident and the fold statistics in the
+        context for ``solve_enet_cv``; returns them, (n_folds, d + 2, d + 2)."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        fp = _vec_ptr(fold_of_row, "u8", mk, n, "fold_of_row")
+        out = np.empty((int(n_folds), d + 2, d + 2), dtype=np.float64)
+        self.serial += 1
+        rc = load().b2_gram_folds(self._h, ptr, xdt, yp, n, d, d, mk, fp, int(n_folds), out.ctypes.data)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_gram_folds")
+        self.d = d
+        return out
+
+    def solve_enet_cv(self, n_folds: int, l1_ratios=(1.0,), alphas=None, n_alphas: int = 100, eps: float = 1e-3,
+                      max_iter: int = 1000, tol: float = 1e-4, positive: bool = False, fit_intercept: bool = True,
+                      fold_S=None, want_coefs: bool = False) -> dict:
+        """Every (l1_ratio, fold) path of a cross-validation and its held-out error in one launch (b2_solve_enet_cv), on
+        the fold statistics of the last ``gram_folds`` or on ``fold_S`` ((n_folds, d + 2, d + 2), uploaded; S becomes
+        their sum).  ``alphas``: None for sklearn's grid of the summed statistic per l1_ratio, else the alphas in the
+        order they are solved, shared by every l1_ratio.  Returns a dict of numpy arrays: alphas (n_l1, n_alphas),
+        mse (n_l1, n_alphas, n_folds), n_iter and gaps (n_l1, n_folds, n_alphas) and, with ``want_coefs``, coefs
+        (n_l1, n_folds, n_alphas, d).  Raises ``ValueError`` for bad arguments."""
+        l1 = np.ascontiguousarray(np.atleast_1d(np.asarray(l1_ratios, dtype=np.float64)).ravel())
+        al = None
+        if alphas is not None:
+            al = np.ascontiguousarray(np.asarray(alphas, dtype=np.float64).ravel())
+            n_alphas = al.size
+        fs = None
+        if fold_S is not None:
+            fs = np.ascontiguousarray(np.asarray(fold_S, dtype=np.float64))
+            if fs.ndim != 3 or fs.shape[0] != int(n_folds) or fs.shape[1] != fs.shape[2] or fs.shape[1] < 3:
+                raise ValueError(f"fold_S must have shape ({int(n_folds)}, d + 2, d + 2), got {fs.shape}")
+            if self.d != fs.shape[1] - 2:
+                self.gram_reset(fs.shape[1] - 2)
+            self.serial += 1
+        d, L, K, A = self.d, l1.size, int(n_folds), max(int(n_alphas), 1)
+        out = {"alphas": np.empty((L, A)), "mse": np.empty((L, A, K)), "n_iter": np.empty((L, K, A), dtype=np.int32),
+               "gaps": np.empty((L, K, A))}
+        if want_coefs:
+            out["coefs"] = np.empty((L, K, A, d))
+        rc = load().b2_solve_enet_cv(self._h, fs.ctypes.data if fs is not None else None, K, int(bool(fit_intercept)),
+                                     l1.ctypes.data if L else None, L, al.ctypes.data if al is not None else None,
+                                     int(n_alphas), float(eps), int(max_iter), float(tol), int(bool(positive)),
+                                     out["alphas"].ctypes.data, out["mse"].ctypes.data, out["n_iter"].ctypes.data,
+                                     out["gaps"].ctypes.data, out["coefs"].ctypes.data if want_coefs else None)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_solve_enet_cv")
         return out
 
     def ridge_loo(self, X, y, alphas, row_mask=None, mask_keep: int = 1, fit_intercept: bool = True,

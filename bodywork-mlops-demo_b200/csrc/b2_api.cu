@@ -412,7 +412,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1],
-                  ctx->enet};
+                  ctx->enet, ctx->folds, ctx->fold_range};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -886,20 +886,19 @@ int b2_solve_eigh(b2_ctx* ctx, int fit_intercept, double* eigvals, double* eigve
 }
 
 // ---- ElasticNet / Lasso: the coordinate-descent path of the resident S (DESIGN.md section 7) -------------------------
-// Host checks, the inputs into ctx->enet, one launch, the outputs back.  ctx->enet holds
-// [alphas A | coef_init kMaxD | coefs A x d | intercepts A | gaps A | iters A | tol_out 1] and grows to the largest call.
-int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const double* alphas, int n_alphas, double eps,
-                       int max_iter, double tol, int positive, const double* coef_init, double* alphas_out,
-                       double* coefs_out, double* intercepts_out, double* gaps_out, int* n_iter_out, double* tol_out) {
-  if (int r = use_device(ctx)) return r;
-  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
-  if (!(l1_ratio >= 0.0 && l1_ratio <= 1.0)) { set_error("l1_ratio=%g must be in [0, 1]", l1_ratio); return B2_E_ARG; }
-  if (n_alphas < 1) { set_error("n_alphas=%d must be >= 1", n_alphas); return B2_E_ARG; }
-  if (alphas == nullptr && l1_ratio == 0.0) {
-    set_error("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a grid by providing "
-              "your estimator with the appropriate `alphas=` argument.");
-    return B2_E_ARG;
+// The argument checks of b2_solve_enet_path and b2_solve_enet_cv (n_l1 l1_ratios, host arrays).
+static int check_enet_args(const double* l1_ratios, int n_l1, const double* alphas, int n_alphas, double eps,
+                           int max_iter, double tol) {
+  for (int l = 0; l < n_l1; ++l) {
+    const double l1_ratio = l1_ratios[l];
+    if (!(l1_ratio >= 0.0 && l1_ratio <= 1.0)) { set_error("l1_ratio=%g must be in [0, 1]", l1_ratio); return B2_E_ARG; }
+    if (alphas == nullptr && l1_ratio == 0.0) {
+      set_error("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a grid by providing "
+                "your estimator with the appropriate `alphas=` argument.");
+      return B2_E_ARG;
+    }
   }
+  if (n_alphas < 1) { set_error("n_alphas=%d must be >= 1", n_alphas); return B2_E_ARG; }
   if (alphas == nullptr && !(eps > 0.0 && isfinite(eps))) { set_error("eps=%g must be > 0 and finite", eps); return B2_E_ARG; }
   if (alphas != nullptr)
     for (int a = 0; a < n_alphas; ++a)
@@ -909,6 +908,32 @@ int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const do
       }
   if (max_iter < 1) { set_error("max_iter=%d must be >= 1", max_iter); return B2_E_ARG; }
   if (!(tol >= 0.0)) { set_error("tol must be >= 0"); return B2_E_ARG; }
+  return B2_OK;
+}
+
+// ctx->enet grown to `need` doubles (its contents are not kept)
+static int ensure_enet_block(b2_ctx* ctx, size_t need) {
+  if (ctx->enet_doubles >= need) return B2_OK;
+  if (ctx->enet != nullptr) cudaFree(ctx->enet);
+  ctx->enet = nullptr;
+  ctx->enet_doubles = 0;
+  if (cudaMalloc(reinterpret_cast<void**>(&ctx->enet), sizeof(double) * need) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("out of device memory for the elastic-net paths (%zu doubles)", need);
+    return B2_E_CUDA;
+  }
+  ctx->enet_doubles = need;
+  return B2_OK;
+}
+
+// Host checks, the inputs into ctx->enet, one launch, the outputs back.  ctx->enet holds
+// [alphas A | coef_init kMaxD | coefs A x d | intercepts A | gaps A | iters A | tol_out 1] and grows to the largest call.
+int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const double* alphas, int n_alphas, double eps,
+                       int max_iter, double tol, int positive, const double* coef_init, double* alphas_out,
+                       double* coefs_out, double* intercepts_out, double* gaps_out, int* n_iter_out, double* tol_out) {
+  if (int r = use_device(ctx)) return r;
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (int r = check_enet_args(&l1_ratio, 1, alphas, n_alphas, eps, max_iter, tol)) return r;
   if (alphas_out == nullptr || coefs_out == nullptr || intercepts_out == nullptr || gaps_out == nullptr ||
       n_iter_out == nullptr) {
     set_error("alphas_out / coefs_out / intercepts_out / gaps_out / n_iter_out is null");
@@ -921,18 +946,7 @@ int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const do
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   if (!(n > 0.0)) { set_error("no row kept: the statistic holds no rows"); return B2_E_ARG; }
   const size_t A = (size_t)n_alphas;
-  const size_t need = A + kMaxD + A * d + 3 * A + 1;
-  if (ctx->enet_doubles < need) {
-    if (ctx->enet != nullptr) cudaFree(ctx->enet);
-    ctx->enet = nullptr;
-    ctx->enet_doubles = 0;
-    if (cudaMalloc(reinterpret_cast<void**>(&ctx->enet), sizeof(double) * need) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("out of device memory for the elastic-net path (%d alphas)", n_alphas);
-      return B2_E_CUDA;
-    }
-    ctx->enet_doubles = need;
-  }
+  if (int r = ensure_enet_block(ctx, A + kMaxD + A * d + 3 * A + 1)) return r;
   EnetArgs args;
   args.l1_ratio = l1_ratio;
   args.eps = eps;
@@ -965,6 +979,164 @@ int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const do
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   for (size_t a = 0; a < A; ++a) n_iter_out[a] = (int)iters[a];
   if (tol_out != nullptr) *tol_out = tol_abs;
+  return B2_OK;
+}
+
+// ---- LassoCV / ElasticNetCV: fold statistics and the paths of every (l1_ratio, fold) (DESIGN.md section 8) ------------
+// ctx->folds grown to n_folds statistics of (d+2)^2 doubles
+static int ensure_folds_block(b2_ctx* ctx, int n_folds, int d) {
+  const size_t need = (size_t)n_folds * (d + 2) * (d + 2);
+  if (ctx->fold_range == nullptr)
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->fold_range), sizeof(unsigned long long) * 2 * kMaxFolds));
+  ctx->n_folds = 0;
+  if (ctx->folds_doubles >= need) return B2_OK;
+  if (ctx->folds != nullptr) cudaFree(ctx->folds);
+  ctx->folds = nullptr;
+  ctx->folds_doubles = 0;
+  if (cudaMalloc(reinterpret_cast<void**>(&ctx->folds), sizeof(double) * need) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("out of device memory for %d fold statistics at d=%d", n_folds, d);
+    return B2_E_CUDA;
+  }
+  ctx->folds_doubles = need;
+  return B2_OK;
+}
+
+int b2_gram_folds(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                  int mem_kind, const uint8_t* fold_of_row, int n_folds, double* fold_S_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_folds < 2 || n_folds > kMaxFolds) { set_error("n_folds=%d must be in [2, %d]", n_folds, kMaxFolds); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) { set_error("cross-validation folds are computed on one rank only"); return B2_E_UNSUPPORTED; }
+  if (n_rows > 0 && (X == nullptr || y == nullptr || fold_of_row == nullptr)) {
+    set_error("X / y / fold_of_row is null");
+    return B2_E_ARG;
+  }
+  if (int r = ensure_folds_block(ctx, n_folds, d)) return r;
+  // first and last row of every fold
+  std::vector<int64_t> first(n_folds, n_rows), last(n_folds, -1);
+  if (mem_kind == B2_MEM_DEVICE) {
+    std::vector<unsigned long long> rg(2 * n_folds);
+    if (int r = launch_fold_ranges(ctx, fold_of_row, n_rows, n_folds, ctx->fold_range)) return r;
+    B2_CUDA(cudaMemcpyAsync(rg.data(), ctx->fold_range, sizeof(unsigned long long) * 2 * n_folds, cudaMemcpyDeviceToHost,
+                            ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < n_folds; ++k)
+      if (rg[2 * k + 1] != 0ull) { first[k] = n_rows - (int64_t)rg[2 * k]; last[k] = (int64_t)rg[2 * k + 1] - 1; }
+  } else {
+    for (int64_t r = 0; r < n_rows; ++r) {
+      const int f = fold_of_row[r];
+      if (f < n_folds) {
+        if (first[f] > r) first[f] = r;
+        last[f] = r;
+      }
+    }
+  }
+  for (int k = 0; k < n_folds; ++k)
+    if (last[k] < 0) { set_error("fold %d has no rows", k); return B2_E_ARG; }
+  // fold k: the Gram dispatch over [first rounded down to 16, last + 1) keeping the rows whose id is k
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const size_t count = (size_t)(d + 2) * (d + 2);
+  ctx->d = d;
+  for (int k = 0; k < n_folds; ++k) {
+    const int64_t r0 = first[k] & ~(int64_t)15, rows = last[k] + 1 - r0;
+    const void* Xk = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
+    ctx->s_zero_pending = true;
+    const int rc = mem_kind == B2_MEM_DEVICE
+                       ? gram_dispatch(ctx, Xk, x_dtype, y + r0, rows, d, ldx, fold_of_row + r0, k)
+                       : gram_host_rows(ctx, Xk, x_dtype, y + r0, rows, d, ldx, fold_of_row + r0, k);
+    if (rc != B2_OK) return rc;
+    B2_CUDA(cudaMemcpyAsync(ctx->folds + k * count, ctx->S, sizeof(double) * count, cudaMemcpyDeviceToDevice,
+                            ctx->stream));
+  }
+  if (int r = launch_fold_sum(ctx, ctx->folds, n_folds, d, ctx->S)) return r;
+  ctx->s_zero_pending = false;
+  ctx->n_folds = n_folds;
+  ctx->folds_d = d;
+  if (fold_S_out != nullptr) {
+    B2_CUDA(cudaMemcpyAsync(fold_S_out, ctx->folds, sizeof(double) * n_folds * count, cudaMemcpyDeviceToHost,
+                            ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  return B2_OK;
+}
+
+// ctx->enet: [alphas n_l1 x A | l1_ratios n_l1 | coefs P x A x d | intercepts P x A | gaps P x A | iters P x A | tol P |
+// mse n_l1 x A x K], P = n_l1 K paths
+int b2_solve_enet_cv(b2_ctx* ctx, const double* fold_S, int n_folds, int fit_intercept, const double* l1_ratios, int n_l1,
+                     const double* alphas, int n_alphas, double eps, int max_iter, double tol, int positive,
+                     double* alphas_out, double* mse_out, int* n_iter_out, double* gaps_out, double* coefs_out) {
+  if (int r = use_device(ctx)) return r;
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (n_folds < 2 || n_folds > kMaxFolds) { set_error("n_folds=%d must be in [2, %d]", n_folds, kMaxFolds); return B2_E_ARG; }
+  if (n_l1 < 1 || l1_ratios == nullptr) { set_error("n_l1=%d must be >= 1 with l1_ratios given", n_l1); return B2_E_ARG; }
+  if (int r = check_enet_args(l1_ratios, n_l1, alphas, n_alphas, eps, max_iter, tol)) return r;
+  if (alphas_out == nullptr || mse_out == nullptr || n_iter_out == nullptr || gaps_out == nullptr) {
+    set_error("alphas_out / mse_out / n_iter_out / gaps_out is null");
+    return B2_E_ARG;
+  }
+  const int d = ctx->d;
+  const size_t count = (size_t)(d + 2) * (d + 2);
+  if (fold_S != nullptr) {
+    // designed statistics: the folds uploaded, S their sum in fold order (the additions of fold_sum_kernel)
+    for (int k = 0; k < n_folds; ++k)
+      if (!(fold_S[k * count + (size_t)d * (d + 2) + d] > 0.0)) { set_error("fold %d has no rows", k); return B2_E_ARG; }
+    if (int r = ensure_folds_block(ctx, n_folds, d)) return r;
+    std::vector<double> sum(count, 0.0);
+    for (int k = 0; k < n_folds; ++k)
+      for (size_t i = 0; i < count; ++i) sum[i] += fold_S[k * count + i];
+    B2_CUDA(cudaMemcpyAsync(ctx->folds, fold_S, sizeof(double) * n_folds * count, cudaMemcpyHostToDevice, ctx->stream));
+    B2_CUDA(cudaMemsetAsync(ctx->S, 0, sizeof(double) * kMaxS * kMaxS, ctx->stream));
+    B2_CUDA(cudaMemcpyAsync(ctx->S, sum.data(), sizeof(double) * count, cudaMemcpyHostToDevice, ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    ctx->s_zero_pending = false;
+    ctx->n_folds = n_folds;
+    ctx->folds_d = d;
+  } else if (ctx->n_folds != n_folds || ctx->folds_d != d) {
+    set_error("no statistics of %d folds at d=%d: call b2_gram_folds first", n_folds, d);
+    return B2_E_STATE;
+  }
+  const size_t A = (size_t)n_alphas, L = (size_t)n_l1, K = (size_t)n_folds, P = L * K;
+  if (int r = ensure_enet_block(ctx, L * A + L + P * A * d + 3 * P * A + P + L * A * K)) return r;
+  EnetArgs args;
+  args.l1_ratio = l1_ratios[0];
+  args.eps = eps;
+  args.tol = tol;
+  args.n_alphas = n_alphas;
+  args.grid = alphas == nullptr ? 1 : 0;
+  args.max_iter = max_iter;
+  args.positive = positive ? 1 : 0;
+  args.fit_intercept = fit_intercept ? 1 : 0;
+  args.alphas = ctx->enet;
+  args.coef_init = nullptr;
+  double* l1_dev = ctx->enet + L * A;
+  args.coefs = l1_dev + L;
+  args.intercepts = args.coefs + P * A * d;
+  args.gaps = args.intercepts + P * A;
+  args.iters = args.gaps + P * A;
+  args.tol_out = args.iters + P * A;
+  args.mse = args.tol_out + P;
+  args.folds = ctx->folds;
+  args.l1_ratios = l1_dev;
+  args.n_folds = n_folds;
+  args.n_l1 = n_l1;
+  if (alphas != nullptr)
+    B2_CUDA(cudaMemcpyAsync(args.alphas, alphas, sizeof(double) * A, cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(l1_dev, l1_ratios, sizeof(double) * L, cudaMemcpyHostToDevice, ctx->stream));
+  if (int r = launch_solve_enet(ctx, args)) return r;
+  std::vector<double> iters(P * A);
+  if (alphas == nullptr)
+    B2_CUDA(cudaMemcpyAsync(alphas_out, args.alphas, sizeof(double) * L * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(mse_out, args.mse, sizeof(double) * L * A * K, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(gaps_out, args.gaps, sizeof(double) * P * A, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(iters.data(), args.iters, sizeof(double) * P * A, cudaMemcpyDeviceToHost, ctx->stream));
+  if (coefs_out != nullptr)
+    B2_CUDA(cudaMemcpyAsync(coefs_out, args.coefs, sizeof(double) * P * A * d, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (alphas != nullptr)
+    for (size_t l = 0; l < L; ++l)
+      for (size_t a = 0; a < A; ++a) alphas_out[l * A + a] = alphas[a];
+  for (size_t i = 0; i < P * A; ++i) n_iter_out[i] = (int)iters[i];
   return B2_OK;
 }
 

@@ -78,17 +78,31 @@ constexpr int kLooW = kLooCw + kMaxD * kMaxAlphas;   // [kMaxD][kMaxAlphas] 1 / 
 constexpr int kLooSum = kLooW + kMaxD * kMaxAlphas;  // the reduced sums of e^2 per alpha [kMaxAlphas]
 constexpr int kLooDoubles = kLooSum + kMaxAlphas;
 
-// ---- the elastic-net path of b2_solve_enet_path (solve.cu: solve_enet_kernel) -----------------------------------------
-// Every pointer is into ctx->enet.  alphas: the call's alphas (grid != 0: the kernel writes sklearn's grid there);
-// coef_init: nullptr or d starting coefficients; outputs per alpha: coefs [n_alphas][d], intercepts, gaps (dual gap / n)
-// and iters (as doubles); tol_out: tol * y_norm2 / n.
+// ---- the elastic-net paths of b2_solve_enet_path / b2_solve_enet_cv (solve.cu: solve_enet_kernel) --------------------
+// Every pointer is into ctx->enet.  alphas: the call's alphas (grid != 0: the kernel writes sklearn's grid there, one row
+// of n_alphas per l1_ratio); coef_init: nullptr or d starting coefficients; outputs per path (CTA) and alpha: coefs
+// [n_alphas][d], intercepts, gaps (dual gap / n) and iters (as doubles); tol_out per path: tol * y_norm2 / n.
+// Cross-validation (folds != nullptr): one path per (l1_ratio l, fold k), CTA l n_folds + k, on the sum of the other
+// folds' statistics (folds: [n_folds][(d+2)^2]); mse [n_l1][n_alphas][n_folds] the held-out error from fold k's own.
 struct EnetArgs {
   double l1_ratio, eps, tol;
   int n_alphas, grid, max_iter, positive, fit_intercept;
   double* alphas;
   const double* coef_init;
   double *coefs, *intercepts, *gaps, *iters, *tol_out;
+  const double* folds = nullptr;
+  const double* l1_ratios = nullptr;   // [n_l1]; nullptr: l1_ratio
+  int n_folds = 1, n_l1 = 1;
+  double* mse = nullptr;
 };
+
+// ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
+constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
+// first and last row of every fold of fold ids in device memory: range[2 k] = n - first, range[2 k + 1] = last + 1
+// (both 0 for a fold without rows); range is zeroed by the launch
+int launch_fold_ranges(b2_ctx* ctx, const uint8_t* fold_of_row, int64_t n, int n_folds, unsigned long long* range);
+// S = the sum of the n_folds statistics of pitch (d+2)^2 in `folds`, added in fold order from 0
+int launch_fold_sum(b2_ctx* ctx, const double* folds, int n_folds, int d, double* S);
 
 // template width of the one-lane-per-row kernels (gram_narrow.cu, score.cu) for d <= 16 features: the next power of two
 inline int narrow_dp(int d) { return d <= 1 ? 1 : d <= 2 ? 2 : d <= 4 ? 4 : d <= 8 ? 8 : 16; }
@@ -156,6 +170,13 @@ struct b2_ctx {
   // elastic-net path: inputs and outputs of b2_solve_enet_path (b2::EnetArgs), grown to the largest call
   double* enet = nullptr;
   size_t enet_doubles = 0;
+  // cross-validation: the fold statistics of b2_gram_folds / b2_solve_enet_cv ([n_folds][(d+2)^2]), grown to the
+  // largest call, and the fold ranges of b2_gram_folds
+  double* folds = nullptr;
+  size_t folds_doubles = 0;
+  int n_folds = 0;                     // folds held in `folds` (0: none)
+  int folds_d = 0;                     // their d
+  unsigned long long* fold_range = nullptr;   // [2 kMaxFolds]
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;

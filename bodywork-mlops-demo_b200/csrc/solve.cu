@@ -24,21 +24,27 @@ constexpr int kOutRank = kMaxD + 2;
 constexpr int kOutSingular = kMaxD + 3;
 constexpr int kOutRows = kOutSingular + kMaxD;   // eigvals kernel only
 
-// Builds A (pitch d+1) and r in shared memory from the raw statistic; returns means.  S is read through L2 (__ldcg: the
-// fused solve has just written it from this CTA) with the loads of a whole batch issued before the first use -- the
-// phase is two L2 round trips, not one per element.
-__device__ void build_normal_equations(const double* S, int d, double alpha, int fit_intercept,
+// Element i of a statistic (pitch d + 2) read through L2 (__ldcg: the fused solve has just written S from this CTA).
+struct LdcgStat {
+  const double* S;
+  __device__ __forceinline__ double operator()(int i) const { return __ldcg(S + i); }
+};
+
+// Builds A (pitch d+1) and r in shared memory from the raw statistic `S` (S(i) = element i); returns means.  The loads
+// of a whole batch are issued before the first use -- the phase is two L2 round trips, not one per element.
+template <class Stat>
+__device__ void build_normal_equations_of(const Stat& S, int d, double alpha, int fit_intercept,
                                        double* A, double* r, double* mean, double* ybar_out) {
   const int dp = d + 2, pitch = d + 1;
-  const double n = __ldcg(S + d * dp + d);
+  const double n = S(d * dp + d);
   const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
   double sxy = 0.0;
   if ((int)threadIdx.x < d) {
-    const double sx = __ldcg(S + threadIdx.x * dp + d);
-    sxy = __ldcg(S + threadIdx.x * dp + d + 1);
+    const double sx = S(threadIdx.x * dp + d);
+    sxy = S(threadIdx.x * dp + d + 1);
     mean[threadIdx.x] = fit_intercept ? sx * inv_n : 0.0;
   }
-  const double ybar = fit_intercept ? __ldcg(S + d * dp + d + 1) * inv_n : 0.0;
+  const double ybar = fit_intercept ? S(d * dp + d + 1) * inv_n : 0.0;
   __syncthreads();
   if ((int)threadIdx.x < d) r[threadIdx.x] = sxy - n * mean[threadIdx.x] * ybar;
   // S is symmetric by construction (tc_fold / the SIMT reduce write both halves).  One warp per row, lane = column
@@ -50,8 +56,8 @@ __device__ void build_normal_equations(const double* S, int d, double alpha, int
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int j = lane + 32 * u;
-      v[u] = j < d ? __ldcg(S + i0 * dp + j) : 0.0;
-      v[4 + u] = (j < d && i1 < d) ? __ldcg(S + i1 * dp + j) : 0.0;
+      v[u] = j < d ? S(i0 * dp + j) : 0.0;
+      v[4 + u] = (j < d && i1 < d) ? S(i1 * dp + j) : 0.0;
     }
     const double m0 = mean[i0], m1 = i1 < d ? mean[i1] : 0.0;
 #pragma unroll
@@ -66,6 +72,11 @@ __device__ void build_normal_equations(const double* S, int d, double alpha, int
   }
   if (threadIdx.x == 0) *ybar_out = ybar;
   __syncthreads();
+}
+
+__device__ __forceinline__ void build_normal_equations(const double* S, int d, double alpha, int fit_intercept,
+                                                       double* A, double* r, double* mean, double* ybar_out) {
+  build_normal_equations_of(LdcgStat{S}, d, alpha, fit_intercept, A, r, mean, ybar_out);
 }
 
 // 1/x for positive x without the library division (a dependent `1.0 / x` is a long call sequence, several times the
@@ -1002,6 +1013,7 @@ solve_eigh_kernel(const double* __restrict__ S, int d, int fit_intercept, double
 }
 
 // ---- elastic net: a whole regularisation path by cyclic coordinate descent on the centred Gram (b2_solve_enet_path) --
+//      and every (l1_ratio, fold) path of a cross-validation in one launch (b2_solve_enet_cv)
 // Restates scikit-learn's enet_coordinate_descent_gram (sklearn/linear_model/_cd_fast.pyx) with enet_path's scaling
 // (l1_reg = alpha l1_ratio n, l2_reg = alpha (1 - l1_ratio) n) and, without user alphas, its _alpha_grid.  Q, q come
 // from build_normal_equations at alpha = 0; y_norm2 = S_yy - n ybar^2.  DESIGN.md section 7.
@@ -1070,29 +1082,30 @@ __device__ __forceinline__ double enet_gap(const double (&w)[4], const double (&
   return primal - dual;
 }
 
-__global__ void __launch_bounds__(kEnetThreads, 1)
-solve_enet_kernel(const double* __restrict__ S, int d, EnetArgs a) {
-  extern __shared__ double sm[];
-  const int pitch = d + 1, dp = d + 2;
-  double* Q = sm;                          // d x d, pitch d + 1; row d = q
-  double* r = Q + d * pitch;
-  double* mean = Q + (d + 1) * pitch;
-  double* wsh = mean + d;                  // [kMaxD] w at the start of an alpha (for Q w)
-  double* misc = wsh + kMaxD;              // [0] ybar
-  build_normal_equations(S, d, 0.0, a.fit_intercept, Q, r, mean, &misc[0]);
-  if (threadIdx.x >= 32) return;           // one warp from here on: __syncwarp only
-  const int lane = threadIdx.x;
-  const double n = __ldcg(S + d * dp + d);
-  const double ybar = misc[0];
-  const double y_norm2 = __ldcg(S + (d + 1) * dp + d + 1) - n * ybar * ybar;
-  const bool positive = a.positive != 0;
+// The statistic a CTA of solve_enet_kernel reads: S itself (folds == nullptr), or the sum of the fold statistics other
+// than fold `skip` (skip < 0: all of them), added in fold order from 0 -- the additions fold_sum_kernel makes for S.
+struct FoldStat {
+  const double* S;
+  const double* folds;
+  int n_folds, skip, stride;
+  __device__ __forceinline__ double operator()(int i) const {
+    if (folds == nullptr) return __ldcg(S + i);
+    double t = 0.0;
+    for (int j = 0; j < n_folds; ++j)
+      if (j != skip) t += __ldcg(folds + (size_t)j * stride + i);
+    return t;
+  }
+};
 
-  // constant columns: zero their row, column and q entry (the build has finished: its last barrier preceded this)
-  unsigned int live[4];
+// Warp 0 after a build of Q / r from S: constant columns get their Q row and column and their q entry zeroed (the
+// build's last barrier preceded this); lane l gets the live bits, q and Q_jj of features l + 32 u.
+__device__ __forceinline__ void enet_columns(const FoldStat& S, double* Q, double* r, int d, int lane,
+                                             unsigned int (&live)[4], double (&q)[4], double (&qjj)[4]) {
+  const int pitch = d + 1, dp = d + 2;
 #pragma unroll
   for (int u = 0; u < 4; ++u) {
     const int f = lane + 32 * u;
-    const bool ok = f < d && Q[f * pitch + f] > kEnetConstCol * __ldcg(S + f * dp + f);
+    const bool ok = f < d && Q[f * pitch + f] > kEnetConstCol * S(f * dp + f);
     const bool dead = f < d && !ok;
     live[u] = __ballot_sync(0xffffffffu, ok);
     unsigned int m = __ballot_sync(0xffffffffu, dead);
@@ -1108,154 +1121,251 @@ solve_enet_kernel(const double* __restrict__ S, int d, EnetArgs a) {
     }
   }
   __syncwarp();
-  double w[4], qw[4], q[4], qjj[4], rinv[4], xta[4];
 #pragma unroll
   for (int u = 0; u < 4; ++u) {
     const int f = lane + 32 * u;
-    const bool ok = (live[u] >> lane) & 1u;
     q[u] = f < d ? r[f] : 0.0;
     qjj[u] = f < d ? Q[f * pitch + f] : 0.0;
-    w[u] = (ok && a.coef_init != nullptr) ? a.coef_init[f] : 0.0;
   }
+}
 
-  // sklearn's _alpha_grid: geomspace(alpha_max, alpha_max eps, n_alphas), or a constant grid at the fp64 resolution
-  if (a.grid) {
-    double mx = 0.0;
+// sklearn's _alpha_grid: alpha_max = max |q| (max q with positive) / (n l1_ratio), then alpha i of
+// geomspace(alpha_max, alpha_max eps, n_alphas), or a constant grid at the fp64 resolution
+__device__ __forceinline__ double enet_alpha_max(const double (&q)[4], double n, double l1_ratio, bool positive) {
+  double mx = 0.0;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) mx = fmax(mx, positive ? q[u] : fabs(q[u]));
-    mx = warp_max(mx);
-    const double amax = mx / (n * a.l1_ratio);
-    const double amin = amax * a.eps;
-    const double ls = log10(amax), step = a.n_alphas > 1 ? (log10(amin) - ls) / (double)(a.n_alphas - 1) : 0.0;
-    for (int i = lane; i < a.n_alphas; i += 32) {
-      double v = exp10(__dadd_rn(__dmul_rn((double)i, step), ls));
-      if (i == 0) v = amax;
-      if (i == a.n_alphas - 1 && i > 0) v = amin;
-      a.alphas[i] = amax <= kF64Resolution ? kF64Resolution : v;
-    }
-    __syncwarp();
-  }
+  for (int u = 0; u < 4; ++u) mx = fmax(mx, positive ? q[u] : fabs(q[u]));
+  return warp_max(mx) / (n * l1_ratio);
+}
+__device__ __forceinline__ double enet_grid_alpha(int i, double amax, double eps, int n_alphas) {
+  const double amin = amax * eps;
+  const double ls = log10(amax), step = n_alphas > 1 ? (log10(amin) - ls) / (double)(n_alphas - 1) : 0.0;
+  double v = exp10(__dadd_rn(__dmul_rn((double)i, step), ls));
+  if (i == 0) v = amax;
+  if (i == n_alphas - 1 && i > 0) v = amin;
+  return amax <= kF64Resolution ? kF64Resolution : v;
+}
 
-  const double tol_abs = a.tol * y_norm2;
-  if (lane == 0) *a.tol_out = tol_abs / n;
-  for (int ia = 0; ia < a.n_alphas; ++ia) {
-    const double alpha = a.alphas[ia];
-    const double l1 = alpha * a.l1_ratio * n, l2 = alpha * (1.0 - a.l1_ratio) * n;
-    // Qw = Q w from scratch (as sklearn's np.dot at every alpha), Q read by columns: lane-consecutive addresses
+// One CTA per (l1_ratio l, fold k): blockIdx.x = l n_folds + k.  b2_solve_enet_path is the case n_folds = 1 without
+// folds (the path of S).  Cross-validation (a.folds): the grid comes from the summed statistic, built and screened as
+// the path's own; the path runs on T_k = the sum of the other folds; then all warps form the held-out error of every
+// alpha from S_k (DESIGN.md section 8).
+__global__ void __launch_bounds__(kEnetThreads, 1)
+solve_enet_kernel(const double* __restrict__ S, int d, EnetArgs a) {
+  extern __shared__ double sm[];
+  const int pitch = d + 1, dp = d + 2;
+  double* Q = sm;                          // d x d, pitch d + 1; row d = q
+  double* r = Q + d * pitch;
+  double* mean = Q + (d + 1) * pitch;
+  double* wsh = mean + d;                  // [kMaxD] w at the start of an alpha (for Q w)
+  double* misc = wsh + kMaxD;              // [0] ybar
+  const int l = blockIdx.x / a.n_folds, k = blockIdx.x - l * a.n_folds;
+  const double l1_ratio = a.l1_ratios != nullptr ? a.l1_ratios[l] : a.l1_ratio;
+  const bool positive = a.positive != 0;
+  const int lane = threadIdx.x & 31;
+  const size_t A = (size_t)a.n_alphas;
+  double* coefs = a.coefs + blockIdx.x * A * d;
+  double* intercepts = a.intercepts + blockIdx.x * A;
+  double amax = 0.0;
+  if (a.folds != nullptr) {
+    const FoldStat all{S, a.folds, a.n_folds, -1, dp * dp};
+    build_normal_equations_of(all, d, 0.0, a.fit_intercept, Q, r, mean, &misc[0]);
+    if (threadIdx.x < 32) {
+      unsigned int live[4];
+      double q[4], qjj[4];
+      enet_columns(all, Q, r, d, lane, live, q, qjj);
+      amax = enet_alpha_max(q, all(d * dp + d), l1_ratio, positive);
+    }
+    __syncthreads();
+  }
+  const FoldStat st{S, a.folds, a.n_folds, k, dp * dp};
+  build_normal_equations_of(st, d, 0.0, a.fit_intercept, Q, r, mean, &misc[0]);
+  if (threadIdx.x < 32) {                  // one warp from here to the end of the path: __syncwarp only
+    const double n = st(d * dp + d);
+    const double ybar = misc[0];
+    const double y_norm2 = st((d + 1) * dp + d + 1) - n * ybar * ybar;
+    unsigned int live[4];
+    double w[4], qw[4], q[4], qjj[4], rinv[4], xta[4];
+    enet_columns(st, Q, r, d, lane, live, q, qjj);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      if (lane + 32 * u < d) wsh[lane + 32 * u] = w[u];
-      rinv[u] = qjj[u] > 0.0 ? 1.0 / (qjj[u] + l2) : 0.0;
-      qw[u] = 0.0;
+      const bool ok = (live[u] >> lane) & 1u;
+      w[u] = (ok && a.coef_init != nullptr) ? a.coef_init[lane + 32 * u] : 0.0;
     }
-    __syncwarp();
-    for (int k = 0; k < d; ++k) {
-      const double wk = wsh[k];
+    if (a.folds == nullptr) amax = enet_alpha_max(q, n, l1_ratio, positive);
+    if (a.grid && k == 0)
+      for (int i = lane; i < a.n_alphas; i += 32) a.alphas[l * A + i] = enet_grid_alpha(i, amax, a.eps, a.n_alphas);
+
+    const double tol_abs = a.tol * y_norm2;
+    if (lane == 0) a.tol_out[blockIdx.x] = tol_abs / n;
+    for (int ia = 0; ia < a.n_alphas; ++ia) {
+      const double alpha = a.grid ? enet_grid_alpha(ia, amax, a.eps, a.n_alphas) : a.alphas[ia];
+      const double l1 = alpha * l1_ratio * n, l2 = alpha * (1.0 - l1_ratio) * n;
+      // Qw = Q w from scratch (as sklearn's np.dot at every alpha), Q read by columns: lane-consecutive addresses
 #pragma unroll
-      for (int u = 0; u < 4; ++u)
-        if (lane + 32 * u < d) qw[u] = fma(Q[k * pitch + lane + 32 * u], wk, qw[u]);
-    }
-    double dn;
-    double gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
-    int iters = 0;
-    if (!(gap >= 0.0 && gap <= tol_abs)) {
-      const bool screening = l1 > 0.0;
-      unsigned int act[4];
-      // gap-safe screening (sklearn: Fercoq et al. eq. 11) over the candidates `cand`: kept features form the active
-      // set, the others leave it for good, their w (if any) taken out of Qw in feature order
-      auto screen = [&](const unsigned int (&cand)[4]) {
-        const double radius = sqrt(2.0 * fabs(gap)) / l1;
-        const double theta_scale = fmax(l1, dn);
-        unsigned int drop[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const bool c = (cand[u] >> lane) & 1u;
-          const bool keep = c && qjj[u] != 0.0 && (1.0 - fabs(xta[u] / theta_scale)) / sqrt(qjj[u] + l2) <= radius;
-          act[u] = __ballot_sync(0xffffffffu, keep);
-          drop[u] = __ballot_sync(0xffffffffu, c && !keep && w[u] != 0.0);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          unsigned int m = drop[u];
-          while (m) {
-            const int l = __ffs(m) - 1;
-            m &= m - 1;
-            const double wj = __shfl_sync(0xffffffffu, w[u], l);
-            if (lane == l) w[u] = 0.0;
-            const double* row = Q + (l + 32 * u) * pitch;
-#pragma unroll
-            for (int v = 0; v < 4; ++v)
-              if (lane + 32 * v < d) qw[v] = fma(-wj, row[lane + 32 * v], qw[v]);
-          }
-        }
-      };
-      if (screening) {
-        unsigned int all[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) all[u] = __ballot_sync(0xffffffffu, lane + 32 * u < d);
-        screen(all);
-      } else {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) act[u] = live[u];
+      for (int u = 0; u < 4; ++u) {
+        if (lane + 32 * u < d) wsh[lane + 32 * u] = w[u];
+        rinv[u] = qjj[u] > 0.0 ? 1.0 / (qjj[u] + l2) : 0.0;
+        qw[u] = 0.0;
       }
-      iters = a.max_iter;
-      for (int it = 0; it < a.max_iter; ++it) {
-        double dw_max = 0.0, w_max = 0.0;
+      __syncwarp();
+      for (int j = 0; j < d; ++j) {
+        const double wj = wsh[j];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          unsigned int m = act[u];
-          while (m) {
-            const int l = __ffs(m) - 1;
-            m &= m - 1;
-            const double* row = Q + (l + 32 * u) * pitch;
-            double rv[4];                                  // row j: its loads do not wait for the step
+        for (int u = 0; u < 4; ++u)
+          if (lane + 32 * u < d) qw[u] = fma(Q[j * pitch + lane + 32 * u], wj, qw[u]);
+      }
+      double dn;
+      double gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
+      int iters = 0;
+      if (!(gap >= 0.0 && gap <= tol_abs)) {
+        const bool screening = l1 > 0.0;
+        unsigned int act[4];
+        // gap-safe screening (sklearn: Fercoq et al. eq. 11) over the candidates `cand`: kept features form the active
+        // set, the others leave it for good, their w (if any) taken out of Qw in feature order
+        auto screen = [&](const unsigned int (&cand)[4]) {
+          const double radius = sqrt(2.0 * fabs(gap)) / l1;
+          const double theta_scale = fmax(l1, dn);
+          unsigned int drop[4];
 #pragma unroll
-            for (int v = 0; v < 4; ++v) rv[v] = lane + 32 * v < d ? row[lane + 32 * v] : 0.0;
-            // Branch-free: every lane evaluates the update of its own feature lane + 32 u and the shuffle takes lane
-            // l's.  The chain per coordinate is t -> soft threshold -> step -> shuffle -> the owner's Qw FMA.  A zero
-            // step adds an exact zero to Qw (sklearn skips it; the value is the same).
-            const double wj = w[u];
-            const double t = fma(wj, qjj[u], q[u]) - qw[u];
-            const double mag = fmax(fabs(t) - l1, 0.0) * rinv[u];
-            const double nw = (positive && t < 0.0) ? 0.0 : (t > 0.0 ? mag : (t < 0.0 ? -mag : 0.0));
-            const double delta = __shfl_sync(0xffffffffu, nw - wj, l);
-            const bool own = lane == l;
-            w[u] = own ? nw : wj;
-            dw_max = own ? fmax(dw_max, fabs(delta)) : dw_max;
-            w_max = own ? fmax(w_max, fabs(nw)) : w_max;
-#pragma unroll
-            for (int v = 0; v < 4; ++v) qw[v] = fma(delta, rv[v], qw[v]);
+          for (int u = 0; u < 4; ++u) {
+            const bool c = (cand[u] >> lane) & 1u;
+            const bool keep = c && qjj[u] != 0.0 && (1.0 - fabs(xta[u] / theta_scale)) / sqrt(qjj[u] + l2) <= radius;
+            act[u] = __ballot_sync(0xffffffffu, keep);
+            drop[u] = __ballot_sync(0xffffffffu, c && !keep && w[u] != 0.0);
           }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            unsigned int m = drop[u];
+            while (m) {
+              const int j = __ffs(m) - 1;
+              m &= m - 1;
+              const double wj = __shfl_sync(0xffffffffu, w[u], j);
+              if (lane == j) w[u] = 0.0;
+              const double* row = Q + (j + 32 * u) * pitch;
+#pragma unroll
+              for (int v = 0; v < 4; ++v)
+                if (lane + 32 * v < d) qw[v] = fma(-wj, row[lane + 32 * v], qw[v]);
+            }
+          }
+        };
+        if (screening) {
+          unsigned int all[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) all[u] = __ballot_sync(0xffffffffu, lane + 32 * u < d);
+          screen(all);
+        } else {
+#pragma unroll
+          for (int u = 0; u < 4; ++u) act[u] = live[u];
         }
-        dw_max = warp_max(dw_max);
-        w_max = warp_max(w_max);
-        if (w_max == 0.0 || dw_max / w_max <= a.tol || it == a.max_iter - 1) {
-          gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
-          if (gap <= tol_abs) {
-            iters = it + 1;
-            break;
+        iters = a.max_iter;
+        for (int it = 0; it < a.max_iter; ++it) {
+          double dw_max = 0.0, w_max = 0.0;
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            unsigned int m = act[u];
+            while (m) {
+              const int j = __ffs(m) - 1;
+              m &= m - 1;
+              const double* row = Q + (j + 32 * u) * pitch;
+              double rv[4];                                  // row j: its loads do not wait for the step
+#pragma unroll
+              for (int v = 0; v < 4; ++v) rv[v] = lane + 32 * v < d ? row[lane + 32 * v] : 0.0;
+              // Branch-free: every lane evaluates the update of its own feature lane + 32 u and the shuffle takes lane
+              // j's.  The chain per coordinate is t -> soft threshold -> step -> shuffle -> the owner's Qw FMA.  A zero
+              // step adds an exact zero to Qw (sklearn skips it; the value is the same).
+              const double wj = w[u];
+              const double t = fma(wj, qjj[u], q[u]) - qw[u];
+              const double mag = fmax(fabs(t) - l1, 0.0) * rinv[u];
+              const double nw = (positive && t < 0.0) ? 0.0 : (t > 0.0 ? mag : (t < 0.0 ? -mag : 0.0));
+              const double delta = __shfl_sync(0xffffffffu, nw - wj, j);
+              const bool own = lane == j;
+              w[u] = own ? nw : wj;
+              dw_max = own ? fmax(dw_max, fabs(delta)) : dw_max;
+              w_max = own ? fmax(w_max, fabs(nw)) : w_max;
+#pragma unroll
+              for (int v = 0; v < 4; ++v) qw[v] = fma(delta, rv[v], qw[v]);
+            }
           }
-          if (screening) {
-            const unsigned int cand[4] = {act[0], act[1], act[2], act[3]};
-            screen(cand);
+          dw_max = warp_max(dw_max);
+          w_max = warp_max(w_max);
+          if (w_max == 0.0 || dw_max / w_max <= a.tol || it == a.max_iter - 1) {
+            gap = enet_gap(w, qw, q, d, lane, l1, l2, y_norm2, positive, xta, &dn);
+            if (gap <= tol_abs) {
+              iters = it + 1;
+              break;
+            }
+            if (screening) {
+              const unsigned int cand[4] = {act[0], act[1], act[2], act[3]};
+              screen(cand);
+            }
           }
         }
       }
-    }
-    double part = 0.0;
+      double part = 0.0;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int f = lane + 32 * u;
-      if (f < d) {
-        a.coefs[(size_t)ia * d + f] = w[u];
-        part = fma(mean[f], w[u], part);
+      for (int u = 0; u < 4; ++u) {
+        const int f = lane + 32 * u;
+        if (f < d) {
+          coefs[(size_t)ia * d + f] = w[u];
+          part = fma(mean[f], w[u], part);
+        }
+      }
+      part = warp_sum(part);
+      if (lane == 0) {
+        intercepts[ia] = ybar - part;
+        a.gaps[blockIdx.x * A + ia] = gap / n;
+        a.iters[blockIdx.x * A + ia] = (double)iters;
       }
     }
-    part = warp_sum(part);
+  }
+  if (a.folds == nullptr) return;
+  __syncthreads();                         // the path's coefficients and intercepts are in global memory; Q is free
+  // Held-out error of every alpha from the fold's own statistic S_k: C = the centred second moments of [x y] (y last,
+  // symmetric, pitch d + 1 in Q's place), mu and vbar its means.  mse = (vbar - b - mu.w)^2 + w~^T C w~ / n_k with
+  // w~ = [w; -1], the quadratic term clamped at 0.  Warp v takes alphas v, v + 8, ...; lane l rows l + 32 u of C w~.
+  const double* Sk = a.folds + (size_t)k * dp * dp;
+  const double nk = __ldcg(Sk + d * dp + d);
+  double* C = Q;
+  double* mu = wsh;                        // [d] means of x; misc[1] the mean of y
+  for (int i = threadIdx.x; i <= d; i += blockDim.x) {
+    const double m = __ldcg(Sk + (i < d ? i : d + 1) * dp + d) / nk;
+    if (i < d) mu[i] = m;
+    else misc[1] = m;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < pitch * pitch; t += blockDim.x) {
+    const int i = t / pitch, j = t - i * pitch;
+    const double mi = i < d ? mu[i] : misc[1], mj = j < d ? mu[j] : misc[1];
+    C[t] = __ldcg(Sk + (i < d ? i : d + 1) * dp + (j < d ? j : d + 1)) - nk * mi * mj;
+  }
+  __syncthreads();
+  const double vbar = misc[1];
+  for (int ia = threadIdx.x >> 5; ia < a.n_alphas; ia += kEnetThreads / 32) {
+    const double* w = coefs + (size_t)ia * d;
+    double cw[5] = {0.0, 0.0, 0.0, 0.0, 0.0};   // (C w~)_i, i = lane + 32 u <= d
+    for (int j = 0; j <= d; ++j) {
+      const double wj = j < d ? w[j] : -1.0;
+#pragma unroll
+      for (int u = 0; u < 5; ++u)
+        if (lane + 32 * u <= d) cw[u] = fma(C[j * pitch + lane + 32 * u], wj, cw[u]);
+    }
+    double quad = 0.0, mw = 0.0;
+#pragma unroll
+    for (int u = 0; u < 5; ++u) {
+      const int i = lane + 32 * u;
+      if (i < d) {
+        quad = fma(w[i], cw[u], quad);
+        mw = fma(mu[i], w[i], mw);
+      } else if (i == d) {
+        quad -= cw[u];
+      }
+    }
+    quad = warp_sum(quad);
+    mw = warp_sum(mw);
     if (lane == 0) {
-      a.intercepts[ia] = ybar - part;
-      a.gaps[ia] = gap / n;
-      a.iters[ia] = (double)iters;
+      const double res = vbar - intercepts[ia] - mw;
+      a.mse[((size_t)l * A + ia) * a.n_folds + k] = res * res + fmax(quad, 0.0) / nk;
     }
   }
 }
@@ -1337,7 +1447,8 @@ int launch_solve_eigh(b2_ctx* ctx, int fit_intercept) {
 
 int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args) {
   if (int r = ensure_solve_attrs(ctx)) return r;
-  solve_enet_kernel<<<1, kEnetThreads, enet_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, args);
+  const int ctas = args.folds != nullptr ? args.n_folds * args.n_l1 : 1;
+  solve_enet_kernel<<<ctas, kEnetThreads, enet_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, args);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return B2_OK;

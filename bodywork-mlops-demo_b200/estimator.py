@@ -405,14 +405,15 @@ def _solve_path(ctx: native.Context, d: int, who: str, **kw) -> dict:
         raise
 
 
-def _warn_unconverged(ctx: native.Context, res: dict, l1_ratio: float, max_iter: int) -> None:
+def _warn_unconverged(ctx: native.Context, res: dict, l1_ratio: float, max_iter: int, n: Optional[float] = None) -> None:
     """sklearn's ConvergenceWarning for every alpha that ran out of sweeps above the gap tolerance (its wording, with the
-    gap and tolerance on cd_fast's scale: n times the dual_gaps scale)."""
+    gap and tolerance on cd_fast's scale: n times the dual_gaps scale).  ``n``: the rows of the path's statistic, None for
+    the resident one."""
     late = [i for i in range(res["gaps"].size) if res["n_iter"][i] >= max_iter and res["gaps"][i] > res["tol"]]
     if not late:
         return
     from sklearn.exceptions import ConvergenceWarning
-    n = float(ctx.gram_export()[-2, -2])
+    n = float(ctx.gram_export()[-2, -2]) if n is None else float(n)
     for i in late:
         message = _MESSAGE_CONV + f" Duality gap: {res['gaps'][i] * n:.6e}, tolerance: {res['tol'] * n:.3e}"
         if res["alphas"][i] * l1_ratio * n < np.finfo(np.float64).eps:
@@ -558,3 +559,241 @@ def lasso_path(X, y, *, eps=1e-3, alphas=100, coef_init=None, return_n_iter=Fals
     return enet_path(X, y, l1_ratio=1.0, eps=eps, alphas=alphas, coef_init=coef_init, return_n_iter=return_n_iter,
                      positive=positive, fit_intercept=fit_intercept, max_iter=max_iter, tol=tol, row_mask=row_mask,
                      mask_keep=mask_keep, ctx=ctx)
+
+
+# ---- LassoCV / ElasticNetCV: every fold's statistic in one pass, every path in one launch (DESIGN.md section 8) ----------
+_MAX_FOLDS = 254
+_DROPPED = 255
+_CV_RESTRICTION = ("cv must be None, an int, or a splitter / iterable of (train, test) whose test sets partition the "
+                   "kept rows and whose train sets are the complements of their test sets (KFold, shuffled or not); "
+                   "ShuffleSplit, RepeatedKFold and other overlapping or partial splits are not supported")
+
+
+def fold_ids(n_rows: int, row_mask=None, mask_keep: int = 1, cv=None):
+    """(ids, n_folds): the fold of every row as uint8 (host), dropped rows 255 -- scikit-learn's folds of the kept rows
+    numbered 0, 1, ... in order.  ``cv``: None (5), an int k (KFold(k) without shuffling: contiguous folds, the first
+    n % k one row longer) or a splitter / iterable of (train, test) over the kept rows whose test sets partition them
+    and whose train sets are their complements.  A device ``row_mask`` is copied down (n bytes)."""
+    n_rows = int(n_rows)
+    if row_mask is None:
+        kept = None
+        m = n_rows
+    else:
+        mask = row_mask.to_host() if isinstance(row_mask, native.DeviceArray) else np.asarray(row_mask)
+        kept = np.flatnonzero(mask.ravel() == mask_keep)
+        m = kept.size
+    ids = np.full(n_rows, _DROPPED, dtype=np.uint8)
+    sel = slice(None) if kept is None else kept
+    if cv is None or (isinstance(cv, (int, np.integer)) and not isinstance(cv, bool)):
+        k = 5 if cv is None else int(cv)
+        if k < 2:
+            raise ValueError(f"k-fold cross-validation requires at least one train/test split by setting n_splits=2 "
+                             f"or more, got n_splits={k}.")
+        if k > _MAX_FOLDS:
+            raise ValueError(f"at most {_MAX_FOLDS} folds are supported, got {k}")
+        if m < k:
+            raise ValueError(f"Cannot have number of splits n_splits={k} greater than the number of samples: "
+                             f"n_samples={m}.")
+        sizes = np.full(k, m // k, dtype=np.int64)
+        sizes[: m % k] += 1
+        ids[sel] = np.repeat(np.arange(k, dtype=np.uint8), sizes)
+        return ids, k
+    splits = list(cv.split(np.zeros((m, 1)))) if hasattr(cv, "split") else list(cv)
+    k = len(splits)
+    if k > _MAX_FOLDS:
+        raise ValueError(f"at most {_MAX_FOLDS} folds are supported, got {k}")
+    if k < 2:
+        raise ValueError(_CV_RESTRICTION)
+    fold = np.full(m, -1, dtype=np.int64)
+    for j, (train, test) in enumerate(splits):
+        test = np.asarray(test, dtype=np.int64).ravel()
+        if test.size == 0 or np.any(test < 0) or np.any(test >= m) or np.any(fold[test] != -1):
+            raise ValueError(_CV_RESTRICTION)
+        fold[test] = j
+    if np.any(fold < 0):
+        raise ValueError(_CV_RESTRICTION)
+    for j, (train, test) in enumerate(splits):
+        train = np.asarray(train, dtype=np.int64).ravel()
+        if train.size != m - np.asarray(test).size or np.any(train < 0) or np.any(train >= m) \
+                or np.any(fold[train] == j) or np.unique(train).size != train.size:
+            raise ValueError(_CV_RESTRICTION)
+    ids[sel] = fold.astype(np.uint8)
+    return ids, k
+
+
+def _fold_tolerances(fold_S: np.ndarray, tol: float, fit_intercept: bool):
+    """(rows, tol y_norm2 / n) of each fold's training statistic T_k (the other folds, added in fold order)."""
+    K = fold_S.shape[0]
+    d = fold_S.shape[1] - 2
+    rows, tols = np.empty(K), np.empty(K)
+    for k in range(K):
+        T = np.zeros_like(fold_S[0])
+        for j in range(K):
+            if j != k:
+                T = T + fold_S[j]
+        n = T[d, d]
+        ybar = T[d, d + 1] / n if fit_intercept else 0.0
+        rows[k], tols[k] = n, tol * (T[d + 1, d + 1] - n * ybar * ybar) / n
+    return rows, tols
+
+
+class B200ElasticNetCV:
+    """``sklearn.linear_model.ElasticNetCV`` (Gram solver, cyclic selection) on the H100: one pass over the rows gives
+    the statistic of every fold (``b2_gram_folds``), one launch runs the path of every (l1_ratio, fold) on the sum of
+    the other folds and forms its held-out error from the fold's own statistic (``b2_solve_enet_cv``), and the refit at
+    the chosen (alpha, l1_ratio) runs on the summed statistic (``b2_solve_enet_path``).  Sets sklearn's attributes;
+    ``to_sklearn()`` returns a genuine ElasticNetCV carrying them."""
+    _sk_name = "ElasticNetCV"
+
+    def __init__(self, *, l1_ratio=0.5, eps: float = 1e-3, alphas=100, fit_intercept: bool = True, precompute="auto",
+                 max_iter: int = 1000, tol: float = 1e-4, cv=None, positive: bool = False, selection: str = "cyclic",
+                 ctx: Optional[native.Context] = None):
+        self.l1_ratio = l1_ratio
+        self.eps = eps
+        self.alphas = alphas
+        self.fit_intercept = fit_intercept
+        self.precompute = precompute         # accepted for sklearn's signature: the solver always uses the Gram
+        self.max_iter = max_iter
+        self.tol = tol
+        self.cv = cv
+        self.positive = positive
+        self.selection = selection
+        self._ctx = ctx
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def _l1_ratios(self) -> np.ndarray:
+        return np.atleast_1d(np.asarray(self.l1_ratio, dtype=np.float64)).ravel()
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1):
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit and the folds to rows equal to ``mask_keep``."""
+        if self.selection == "random":
+            raise ValueError("selection='random' is not supported: the GPU solver runs sklearn's cyclic order only")
+        if self.selection != "cyclic":
+            raise ValueError("selection should be either random or cyclic.")
+        l1 = self._l1_ratios()
+        grid = isinstance(self.alphas, (int, np.integer)) and not isinstance(self.alphas, bool)
+        if grid:
+            al, n_alphas = None, int(self.alphas)
+            if n_alphas < 1:
+                raise ValueError(f"alphas must be >= 1 when given as an integer, got {n_alphas}")
+            if np.any(l1 == 0.0):
+                raise ValueError("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a "
+                                 "grid by providing your estimator with the appropriate `alphas=` argument.")
+        else:
+            al = np.sort(np.asarray(self.alphas, dtype=np.float64).ravel())[::-1]
+            n_alphas = al.size
+        ctx = self.ctx
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        d = X.shape[1]
+        try:
+            ids, K = fold_ids(X.shape[0], row_mask, mask_keep, self.cv)
+            if isinstance(X, native.DeviceArray):
+                ids = ctx.to_device(ids)
+                owned.append(ids)
+            fold_S = ctx.gram_folds(X, y, ids, K)
+        finally:
+            for a in owned:
+                a.free()
+        res = ctx.solve_enet_cv(K, l1, alphas=al, n_alphas=n_alphas, eps=self.eps, max_iter=self.max_iter,
+                                tol=self.tol, positive=self.positive, fit_intercept=self.fit_intercept)
+        if not np.all(np.isfinite(res["mse"])):
+            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        rows, tols = _fold_tolerances(fold_S, self.tol, self.fit_intercept)
+        for li in range(l1.size):
+            for k in range(K):
+                _warn_unconverged(ctx, {"gaps": res["gaps"][li, k], "n_iter": res["n_iter"][li, k], "tol": tols[k],
+                                        "alphas": res["alphas"][li]}, float(l1[li]), self.max_iter, n=rows[k])
+        # sklearn: the mean over folds, the first minimum per l1_ratio, a later l1_ratio only when strictly better
+        mean_mse = np.mean(np.moveaxis(res["mse"], 2, 1), axis=1)
+        best_mse, best = np.inf, (0, 0)
+        for li in range(l1.size):
+            i = int(np.argmin(mean_mse[li]))
+            if mean_mse[li, i] < best_mse:
+                best_mse, best = mean_mse[li, i], (li, i)
+        best_l1, best_alpha = float(l1[best[0]]), float(res["alphas"][best[0], best[1]])
+        ref = _solve_path(ctx, d, f"B200{self._sk_name}", l1_ratio=best_l1, alphas=[best_alpha],
+                          max_iter=self.max_iter, tol=self.tol, positive=self.positive,
+                          fit_intercept=self.fit_intercept)
+        coef, b0 = ref["coefs"][0], float(ref["intercepts"][0])
+        if not (np.all(np.isfinite(coef)) and np.isfinite(b0)):
+            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _warn_unconverged(ctx, ref, best_l1, self.max_iter)
+        self.alpha_ = best_alpha
+        self.l1_ratio_ = best_l1
+        self.alphas_ = (res["alphas"][0] if l1.size == 1 else res["alphas"]) if grid else al.copy()
+        self.mse_path_ = np.squeeze(res["mse"])
+        self.coef_ = coef.copy()
+        self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
+        self.dual_gap_ = np.float64(ref["gaps"][0])
+        self.n_iter_ = int(ref["n_iter"][0])
+        self.n_features_in_ = int(d)
+        return self
+
+    def predict(self, X):
+        ctx = self.ctx
+        if isinstance(X, native.DeviceArray):
+            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
+            return yhat
+        Xh = _as_f32_matrix(X)
+        if Xh.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
+        return yhat.astype(np.float64)
+
+    def _sk_params(self) -> dict:
+        cv = self.cv
+        if cv is not None and not isinstance(cv, (int, np.integer)) and not hasattr(cv, "split") \
+                and not isinstance(cv, (list, tuple)):
+            cv = None                          # a one-shot iterator has been consumed by fit
+        return dict(l1_ratio=self.l1_ratio, eps=self.eps, alphas=self.alphas, fit_intercept=self.fit_intercept,
+                    precompute=True, max_iter=self.max_iter, tol=self.tol, cv=cv, positive=self.positive,
+                    selection=self.selection)
+
+    def to_sklearn(self):
+        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
+        intercept_).  ``precompute=True``: the Gram solver this fit restates."""
+        from sklearn import linear_model
+        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        reg.alpha_ = float(self.alpha_)
+        if hasattr(self, "l1_ratio_"):
+            reg.l1_ratio_ = float(self.l1_ratio_)
+        reg.alphas_ = np.asarray(self.alphas_, dtype=np.float64).copy()
+        reg.mse_path_ = np.asarray(self.mse_path_, dtype=np.float64).copy()
+        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
+        reg.intercept_ = np.float64(self.intercept_)
+        reg.dual_gap_ = np.float64(self.dual_gap_)
+        reg.n_iter_ = int(self.n_iter_)
+        reg.n_features_in_ = int(self.n_features_in_)
+        return reg
+
+    def __repr__(self) -> str:
+        return f"B200{self._sk_name}(l1_ratio={self.l1_ratio}, cv={self.cv!r})"
+
+
+class B200LassoCV(B200ElasticNetCV):
+    """``sklearn.linear_model.LassoCV``: B200ElasticNetCV with l1_ratio = 1 (no ``l1_ratio_``)."""
+    _sk_name = "LassoCV"
+
+    def __init__(self, *, eps: float = 1e-3, alphas=100, fit_intercept: bool = True, precompute="auto",
+                 max_iter: int = 1000, tol: float = 1e-4, cv=None, positive: bool = False, selection: str = "cyclic",
+                 ctx: Optional[native.Context] = None):
+        super().__init__(l1_ratio=1.0, eps=eps, alphas=alphas, fit_intercept=fit_intercept, precompute=precompute,
+                         max_iter=max_iter, tol=tol, cv=cv, positive=positive, selection=selection, ctx=ctx)
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1):
+        super().fit(X, y, row_mask, mask_keep)
+        del self.l1_ratio_
+        return self
+
+    def _sk_params(self) -> dict:
+        p = super()._sk_params()
+        del p["l1_ratio"]
+        return p
+
+    def __repr__(self) -> str:
+        return f"B200LassoCV(cv={self.cv!r})"

@@ -200,6 +200,35 @@ int b2_solve_enet_path(b2_ctx* ctx, int fit_intercept, double l1_ratio, const do
                        int max_iter, double tol, int positive, const double* coef_init, double* alphas_out,
                        double* coefs_out, double* intercepts_out, double* gaps_out, int* n_iter_out, double* tol_out);
 
+/* ---- cross-validated elastic net / lasso: replaces sklearn.linear_model.ElasticNetCV / LassoCV(precompute=True) --
+ * reference: sklearn/linear_model/_coordinate_descent.py LinearModelCV.fit and _path_residuals (DESIGN section 8).
+ * b2_gram_folds: the statistic S_k of every fold in one call.  Row r belongs to fold fold_of_row[r] (a value >= n_folds
+ * drops the row; the ids live where X lives: device or host).  Fold k is the Gram dispatch of b2_gram_accumulate over
+ * rows [first_k rounded down to a multiple of 16, last_k + 1) keeping the rows whose id is k: contiguous folds read each
+ * row once and stay on the tensor-core / narrow kernels, shuffled folds cost up to n_folds passes.  The statistics stay
+ * in a device block of the context (grown to the largest call); afterwards S = sum_k S_k, added in fold order, so
+ * b2_solve_enet_path can refit from it.  fold_S_out: NULL or host n_folds x (d+2)^2.
+ * B2_E_ARG: n_folds outside 2..254, a fold without rows, bad shapes; B2_E_UNSUPPORTED: more than one rank. */
+int b2_gram_folds(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                  int mem_kind, const uint8_t* fold_of_row, int n_folds, double* fold_S_out);
+
+/* b2_solve_enet_cv: every path of a cross-validation in one launch, one CTA per (l1_ratio l, fold k).  Path (l, k) is
+ * b2_solve_enet_path's arithmetic on T_k = sum of the other folds' statistics (added in fold order) over the grid of the
+ * summed statistic for l1_ratios[l] (alphas NULL; bit-identical to what b2_solve_enet_path writes for that S) or over
+ * `alphas` in the order given, shared by every l1_ratio.  The held-out error of each solution (w, b) comes from S_k:
+ *   mse = (vbar - b - mu.w)^2 + max(w~^T C w~, 0) / n_k,  w~ = [w; -1],
+ * mu / vbar the fold's means of x / y, C the centred second moments of [x y].
+ *   fold_S      NULL: the statistics of the last b2_gram_folds (same n_folds and d); else host n_folds x (d+2)^2 at the
+ *               context's d, uploaded, and S becomes their sum
+ *   outputs     (host) alphas_out [n_l1][n_alphas], mse_out [n_l1][n_alphas][n_folds] (sklearn's mse_path_),
+ *               n_iter_out and gaps_out [n_l1][n_folds][n_alphas] (gap / n of T_k), coefs_out NULL or
+ *               [n_l1][n_folds][n_alphas][d]
+ * B2_E_ARG as b2_solve_enet_path, n_folds outside 2..254, n_l1 < 1, or a fold without rows; B2_E_STATE: no fold
+ * statistics of this shape.  Repeated calls give identical results. */
+int b2_solve_enet_cv(b2_ctx* ctx, const double* fold_S, int n_folds, int fit_intercept, const double* l1_ratios, int n_l1,
+                     const double* alphas, int n_alphas, double eps, int max_iter, double tol, int positive,
+                     double* alphas_out, double* mse_out, int* n_iter_out, double* gaps_out, double* coefs_out);
+
 /* ---- ridge with the alpha chosen by leave-one-out error: replaces sklearn.linear_model.RidgeCV(alphas).fit ------
  * RidgeCV(alphas, fit_intercept).fit(X, y), cv=None: b2_fit's Gram of the kept rows, the eigendecomposition of its
  * centred Gram, then one fp64 pass over the same rows for the leave-one-out error of every alpha (DESIGN section 6).
