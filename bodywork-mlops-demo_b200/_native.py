@@ -74,6 +74,14 @@ _SIGNATURES = {
                                    C.c_double, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "b2_ridge_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
                                C.c_int, _vp, _vp, C.POINTER(C.c_int), _vp, C.POINTER(C.c_double)]),
+    "b2_residual_moments": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
+                                      C.c_double, C.c_int, _vp]),
+    "b2_solve_bayes_ridge": (C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_double, _vp, C.c_int, _vp,
+                                       C.POINTER(C.c_double), C.POINTER(C.c_double), _vp, C.POINTER(C.c_int), _vp, _vp]),
+    "b2_solve_ard": (C.c_int, [_vp, C.c_int, _vp, C.c_double, C.c_int, C.c_double, _vp, C.c_int, _vp,
+                               C.POINTER(C.c_double), C.POINTER(C.c_double), _vp, C.POINTER(C.c_int), _vp, _vp]),
+    "b2_score_std": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, _vp, C.c_double, _vp,
+                               C.c_double, _vp, _vp]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -569,6 +577,103 @@ class Context:
         self.serial += 1
         _check(rc, "b2_ridge_loo")
         return mse[: al.size], int(best.value), coef, float(b0.value), cv
+
+    # -- BayesianRidge / ARDRegression (DESIGN.md section 9) ---------------------------------------------------
+    def residual_moments(self, X, y, coef, intercept: float, row_mask=None, mask_keep: int = 1,
+                         fit_intercept: bool = True) -> np.ndarray:
+        """One fp64 pass over the kept rows at (coef, intercept) (b2_residual_moments): returns the d + 2 values
+        [sum (x - m) e, sum e, sum e^2], e = y - intercept - x.coef, m the column means of the resident statistic (0
+        without an intercept).  [coef, result] is the anchor of ``solve_bayes_ridge`` / ``solve_ard``."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
+        if w.size != d:
+            raise ValueError(f"coef has {w.size} entries, X has {d} columns")
+        out = np.empty(d + 2, dtype=np.float64)
+        _check(load().b2_residual_moments(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), w.ctypes.data,
+                                          float(intercept), int(bool(fit_intercept)), out.ctypes.data),
+               "b2_residual_moments")
+        return out
+
+    def _bayes_call(self, fn, what: str, args_before, ard: bool, max_iter: int, anchor, compute_score: bool,
+                    fit_intercept: bool, want_sigma: bool) -> dict:
+        d = self.d
+        n_lambda = d if ard else 1
+        an = None
+        if anchor is not None:
+            an = np.ascontiguousarray(anchor, dtype=np.float64).ravel()
+            if an.size != 2 * d + 2:
+                raise ValueError(f"anchor has {an.size} entries, {2 * d + 2} expected")
+        coef = np.empty(d, dtype=np.float64)
+        lam = np.empty(n_lambda, dtype=np.float64)
+        b0, alpha, n_iter = C.c_double(0.0), C.c_double(0.0), C.c_int(0)
+        scores = np.empty(max(int(max_iter), 0) + 1, dtype=np.float64) if compute_score else None
+        sigma = np.empty((d, d), dtype=np.float64) if want_sigma else None
+        rc = fn(self._h, int(bool(fit_intercept)), *args_before, an.ctypes.data if an is not None else None,
+                int(bool(compute_score)), coef.ctypes.data, C.byref(b0), C.byref(alpha), lam.ctypes.data,
+                C.byref(n_iter), scores.ctypes.data if scores is not None else None,
+                sigma.ctypes.data if sigma is not None else None)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        if rc == E_SINGULAR:
+            raise np.linalg.LinAlgError(last_error())
+        _check(rc, what)
+        k = int(n_iter.value)
+        return {"coef": coef, "intercept": float(b0.value), "alpha": float(alpha.value),
+                "lambda": lam if ard else float(lam[0]), "n_iter": k,
+                "scores": scores[: k if ard else k + 1] if scores is not None else None, "sigma": sigma}
+
+    def solve_bayes_ridge(self, alpha_1: float = 1e-6, alpha_2: float = 1e-6, lambda_1: float = 1e-6,
+                          lambda_2: float = 1e-6, alpha_init=None, lambda_init=None, max_iter: int = 300,
+                          tol: float = 1e-3, anchor=None, compute_score: bool = False, fit_intercept: bool = True,
+                          want_sigma: bool = True) -> dict:
+        """BayesianRidge's evidence maximisation on the resident statistic (b2_solve_bayes_ridge).  ``anchor``: None or
+        [w0 (d), g0 (d), s0, sse0] (w0 and ``residual_moments`` at w0).  Returns a dict: coef, intercept, alpha, lambda,
+        n_iter, scores (n_iter + 1 values with compute_score, else None) and sigma (d, d).  Raises ``ValueError`` for bad
+        arguments and a statistic without rows."""
+        nan = float("nan")
+        hyper = np.array([alpha_1, alpha_2, lambda_1, lambda_2, nan if alpha_init is None else alpha_init,
+                          nan if lambda_init is None else lambda_init], dtype=np.float64)
+        return self._bayes_call(load().b2_solve_bayes_ridge, "b2_solve_bayes_ridge",
+                                (hyper.ctypes.data, int(max_iter), float(tol)), False, max_iter, anchor, compute_score,
+                                fit_intercept, want_sigma)
+
+    def solve_ard(self, alpha_1: float = 1e-6, alpha_2: float = 1e-6, lambda_1: float = 1e-6, lambda_2: float = 1e-6,
+                  threshold_lambda: float = 1e4, max_iter: int = 300, tol: float = 1e-3, anchor=None,
+                  compute_score: bool = False, fit_intercept: bool = True, want_sigma: bool = True) -> dict:
+        """ARDRegression's iteration on the resident statistic (b2_solve_ard).  Returns ``solve_bayes_ridge``'s dict with
+        lambda per feature, n_iter scores and sigma (d, d): the kept x kept sigma_ at the kept rows and columns, zeros elsewhere.
+        Raises ``np.linalg.LinAlgError`` on a non-positive pivot."""
+        hyper = np.array([alpha_1, alpha_2, lambda_1, lambda_2], dtype=np.float64)
+        return self._bayes_call(load().b2_solve_ard, "b2_solve_ard",
+                                (hyper.ctypes.data, float(threshold_lambda), int(max_iter), float(tol)), True,
+                                max_iter, anchor, compute_score, fit_intercept, want_sigma)
+
+    def score_std(self, X, mean, sigma, noise_var: float, coef, intercept: float, want_yhat: bool = True):
+        """predict(X, return_std=True) of BayesianRidge / ARDRegression in one fp64 pass (b2_score_std): returns (yhat |
+        None, ystd), ystd = sqrt(max((x - mean)^T sigma (x - mean), 0) + noise_var) -- float64 ndarrays for host rows,
+        f64 DeviceArrays for device rows."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
+        m = np.ascontiguousarray(mean, dtype=np.float64).ravel() if mean is not None else None
+        sg = np.ascontiguousarray(sigma, dtype=np.float64)
+        if w.size != d or sg.shape != (d, d) or (m is not None and m.size != d):
+            raise ValueError(f"coef / mean need {d} entries and sigma shape ({d}, {d})")
+        if mk == MEM_DEVICE:
+            ystd = self.empty((n,), "f64")
+            yhat = self.empty((n,), "f64") if want_yhat else None
+            sp, hp = ystd.ptr, (yhat.ptr if yhat is not None else None)
+        else:
+            ystd = np.empty(n, dtype=np.float64)
+            yhat = np.empty(n, dtype=np.float64) if want_yhat else None
+            sp, hp = ystd.ctypes.data, (yhat.ctypes.data if yhat is not None else None)
+        rc = load().b2_score_std(self._h, ptr, xdt, n, d, d, mk, m.ctypes.data if m is not None else None,
+                                 sg.ctypes.data, float(noise_var), w.ctypes.data, float(intercept), hp, sp)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_score_std")
+        return yhat, ystd
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

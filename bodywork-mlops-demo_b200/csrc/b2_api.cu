@@ -780,6 +780,28 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
   return finish_cholesky(ctx, coef, intercept);
 }
 
+// One residual pass over the rows for the model in ctx->refine: the gradient kernels (+ their ordered reduce) write
+// g_j, g_1 and sum e^2 to ctx->refine + kRfGrad; host rows re-stream through the staging ring.
+static int grad_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const uint8_t* row_mask, int mask_keep) {
+  if (mem_kind == B2_MEM_DEVICE) return launch_grad(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, true);
+  if (int r = ensure_staging(ctx)) return r;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = host_pointer_is_pinned(X);
+  if (int r = stream_host_blocks(
+          ctx, n_rows, ctx->stage_rows,
+          [&](int buf, int64_t r0, int64_t rows) {
+            return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
+          },
+          [&](int buf, int64_t r0, int64_t rows) {
+            return launch_grad(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
+                               row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, r0 == 0);
+          }))
+    return r;
+  if (n_rows == 0) return launch_grad(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, true);
+  return B2_OK;
+}
+
 // ---- the refined fit: b2_fit, then residual passes over the same rows (DESIGN.md section 2) ------------------------
 // Per pass: the gradient kernels (+ their ordered reduce) over the rows -- host rows re-stream through the staging ring --
 // then the Cholesky kernel in refinement mode, which refactors A + alpha I from S, solves for the correction and moves
@@ -818,28 +840,10 @@ int b2_fit_refined(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
   st[kRfStep] = INFINITY;
   B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = mem_kind == B2_MEM_HOST && host_pointer_is_pinned(X);
-  if (mem_kind == B2_MEM_HOST)
-    if (int r = ensure_staging(ctx)) return r;
   const double* h = ctx->solve_host;
   int kept = 0;
   for (int pass = 0; pass < max_passes; ++pass) {
-    if (mem_kind == B2_MEM_DEVICE) {
-      if (int r = launch_grad(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, true)) return r;
-    } else if (int r = stream_host_blocks(
-                   ctx, n_rows, ctx->stage_rows,
-                   [&](int buf, int64_t r0, int64_t rows) {
-                     return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-                   },
-                   [&](int buf, int64_t r0, int64_t rows) {
-                     return launch_grad(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
-                                        row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, r0 == 0);
-                   })) {
-      return r;
-    }
-    if (n_rows == 0 && mem_kind == B2_MEM_HOST)
-      if (int r = launch_grad(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, true)) return r;
+    if (int r = grad_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
     if (int r = launch_solve_refine(ctx, alpha, fit_intercept)) return r;
     B2_CUDA(cudaStreamSynchronize(ctx->stream));
     if (h[kMaxD + 1] != 0.0) {
@@ -1140,6 +1144,27 @@ int b2_solve_enet_cv(b2_ctx* ctx, const double* fold_S, int n_folds, int fit_int
   return B2_OK;
 }
 
+// The device output blocks of host rows (b2_ridge_loo's e^2, b2_score_std's ystd and yhat): two blocks of stage_rows x
+// per_row doubles, grown to the widest call so far and freed with the context.
+static int ensure_cv_stage(b2_ctx* ctx, int per_row) {
+  if (ctx->cv_stage_alphas >= per_row) return B2_OK;
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));                 // an earlier call's copies may still read them
+  for (int b = 0; b < 2; ++b) {
+    if (ctx->cv_stage[b] != nullptr) cudaFree(ctx->cv_stage[b]);
+    ctx->cv_stage[b] = nullptr;
+  }
+  ctx->cv_stage_alphas = 0;
+  for (int b = 0; b < 2; ++b)
+    if (cudaMalloc(reinterpret_cast<void**>(&ctx->cv_stage[b]), sizeof(double) * ctx->stage_rows * per_row) !=
+        cudaSuccess) {
+      cudaGetLastError();
+      set_error("out of device memory for the staging blocks of the per-row outputs");
+      return B2_E_CUDA;
+    }
+  ctx->cv_stage_alphas = per_row;
+  return B2_OK;
+}
+
 // The Gram of b2_fit, the eigendecomposition of its centred Gram, one leave-one-out pass over the same rows (host rows
 // re-stream through the staging ring, their e^2 through a device block per row block), then the LDL^T solve of b2_fit
 // at the chosen alpha from the same S.
@@ -1186,22 +1211,8 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
   } else {
     const int es = x_dtype == B2_F32 ? 4 : 2;
     const bool x_pinned = host_pointer_is_pinned(X);
-    if (cv_out != nullptr && ctx->cv_stage_alphas < n_alphas) {     // sized to the widest call so far
-      B2_CUDA(cudaStreamSynchronize(ctx->stream));                 // an earlier call's copies may still read them
-      for (int b = 0; b < 2; ++b) {
-        if (ctx->cv_stage[b] != nullptr) cudaFree(ctx->cv_stage[b]);
-        ctx->cv_stage[b] = nullptr;
-      }
-      ctx->cv_stage_alphas = 0;
-      for (int b = 0; b < 2; ++b)
-        if (cudaMalloc(reinterpret_cast<void**>(&ctx->cv_stage[b]), sizeof(double) * ctx->stage_rows * n_alphas) !=
-            cudaSuccess) {
-          cudaGetLastError();
-          set_error("out of device memory for the leave-one-out staging blocks");
-          return B2_E_CUDA;
-        }
-      ctx->cv_stage_alphas = n_alphas;
-    }
+    if (cv_out != nullptr)
+      if (int r = ensure_cv_stage(ctx, n_alphas)) return r;
     const int rc = stream_host_blocks(
         ctx, n_rows, ctx->stage_rows,
         [&](int buf, int64_t r0, int64_t rows) {
@@ -1230,6 +1241,218 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
   *best_out = best;
   if (int r = launch_solve_cholesky(ctx, alphas[best], fit_intercept)) return r;
   return finish_cholesky(ctx, coef, intercept);
+}
+
+// ---- BayesianRidge / ARDRegression (DESIGN.md section 9) ------------------------------------------------------------
+// The anchor pass: the refined fit's gradient kernels at (coef, intercept), with m the column means of the resident S.
+int b2_residual_moments(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                        int mem_kind, const uint8_t* row_mask, int mask_keep, const double* coef, double intercept,
+                        int fit_intercept, double* out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (coef == nullptr || out == nullptr) { set_error("coef / out is null"); return B2_E_ARG; }
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) {
+    set_error("b2_residual_moments runs on one rank only (the residual moments are not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (ctx->d != d) { set_error("the resident statistic has %d features, the rows %d", ctx->d, d); return B2_E_STATE; }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  const int dp = d + 2;
+  std::vector<double> S((size_t)dp * dp), st(kRfDoubles, 0.0);
+  B2_CUDA(cudaMemcpyAsync(S.data(), ctx->S, sizeof(double) * dp * dp, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const double n = S[(size_t)d * dp + d];
+  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
+  double b0 = intercept;
+  for (int j = 0; j < d; ++j) {
+    st[kRfBeta + j] = coef[j];
+    st[kRfMean + j] = fit_intercept ? S[(size_t)j * dp + d] * inv_n : 0.0;
+    b0 += st[kRfMean + j] * coef[j];
+  }
+  st[kRfB0] = b0;                        // the model b0' + (x - m).w is intercept + x.w
+  B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
+  if (int r = grad_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
+  double g[kGradOut];
+  B2_CUDA(cudaMemcpyAsync(g, ctx->refine + kRfGrad, sizeof(g), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(out, g, sizeof(double) * d);
+  out[d] = g[kMaxD];
+  out[d + 1] = g[kMaxD + 1];
+  return B2_OK;
+}
+
+// The checks both solves share: hyper-parameters finite and >= 0, max_iter >= 1, tol >= 0, outputs present, and the rows
+// of the resident S (returned in n)
+static int check_bayes_args(b2_ctx* ctx, const double* hyper, int n_hyper, int max_iter, double tol, const double* coef,
+                            const double* intercept, const double* alpha_out, const void* lambda_out,
+                            const int* n_iter_out, double* n) {
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (hyper == nullptr) { set_error("hyper is null"); return B2_E_ARG; }
+  for (int k = 0; k < n_hyper; ++k) {
+    const bool init = k >= 4;             // alpha_init / lambda_init: NaN means the default
+    if (!(isnan(hyper[k]) && init) && !(isfinite(hyper[k]) && hyper[k] >= 0.0)) {
+      set_error("hyper[%d] == %g, must be >= 0 and finite%s", k, hyper[k], init ? " (or NaN for the default)" : "");
+      return B2_E_ARG;
+    }
+  }
+  if (max_iter < 1) { set_error("max_iter=%d must be >= 1", max_iter); return B2_E_ARG; }
+  if (!(tol >= 0.0)) { set_error("tol must be >= 0"); return B2_E_ARG; }
+  if (coef == nullptr || intercept == nullptr || alpha_out == nullptr || lambda_out == nullptr || n_iter_out == nullptr) {
+    set_error("coef / intercept / alpha_out / lambda_out / n_iter_out is null");
+    return B2_E_ARG;
+  }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  const int d = ctx->d;
+  B2_CUDA(cudaMemcpyAsync(n, ctx->S + (size_t)d * (d + 2) + d, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+// ctx->enet as [out kByDoubles | anchor 2 kMaxD + 2 | the ARD Gram kMaxD^2 | scores max_iter + 1]; the anchor uploaded
+static int bayes_block(b2_ctx* ctx, const double* anchor, int max_iter, int compute_score, int fit_intercept,
+                       BayesArgs* a) {
+  const size_t off_anchor = kByDoubles, off_A = off_anchor + 2 * kMaxD + 2, off_scores = off_A + (size_t)kMaxD * kMaxD;
+  if (int r = ensure_enet_block(ctx, off_scores + (size_t)max_iter + 1)) return r;
+  a->max_iter = max_iter;
+  a->compute_score = compute_score ? 1 : 0;
+  a->fit_intercept = fit_intercept ? 1 : 0;
+  a->out = ctx->enet;
+  a->A = ctx->enet + off_A;
+  a->scores = ctx->enet + off_scores;
+  a->anchor = nullptr;
+  if (anchor != nullptr) {
+    const int d = ctx->d;
+    std::vector<double> h(2 * kMaxD + 2, 0.0);
+    memcpy(h.data(), anchor, sizeof(double) * d);
+    memcpy(h.data() + kMaxD, anchor + d, sizeof(double) * d);
+    h[2 * kMaxD] = anchor[2 * d];
+    h[2 * kMaxD + 1] = anchor[2 * d + 1];
+    B2_CUDA(cudaMemcpyAsync(ctx->enet + off_anchor, h.data(), sizeof(double) * h.size(), cudaMemcpyHostToDevice,
+                            ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));   // h is on this frame's stack
+    a->anchor = ctx->enet + off_anchor;
+  }
+  return B2_OK;
+}
+
+// The outputs of either solve; n_lambda: 1 (BayesianRidge: one lambda_) or 0 (ARD: d of them).  Returns B2_E_SINGULAR on the kernel's info.
+static int fetch_bayes(b2_ctx* ctx, const BayesArgs& a, int n_lambda, double* coef, double* intercept, double* alpha_out,
+                       double* lambda_out, int* n_iter_out, double* scores_out, double* sigma_out) {
+  const int d = ctx->d;
+  double misc[8];
+  B2_CUDA(cudaMemcpyAsync(misc, a.out + kByMisc, sizeof(misc), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaMemcpyAsync(coef, a.out + kByCoef, sizeof(double) * d, cudaMemcpyDeviceToHost, ctx->stream));
+  if (n_lambda == 1) B2_CUDA(cudaMemcpyAsync(lambda_out, a.out + kByMisc + 2, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  else B2_CUDA(cudaMemcpyAsync(lambda_out, a.out + kByLambda, sizeof(double) * d, cudaMemcpyDeviceToHost, ctx->stream));
+  if (sigma_out != nullptr)
+    B2_CUDA(cudaMemcpyAsync(sigma_out, a.out + kBySigma, sizeof(double) * d * d, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (misc[4] != 0.0) {
+    set_error("pivot %d of the factorisation of diag(lambda) + alpha A is not positive", (int)misc[4]);
+    return B2_E_SINGULAR;
+  }
+  *intercept = misc[0];
+  *alpha_out = misc[1];
+  *n_iter_out = (int)misc[3];
+  if (scores_out != nullptr && a.compute_score) {     // BayesianRidge scores once more after the loop, ARD does not
+    const int n_scores = *n_iter_out + (n_lambda == 1 ? 1 : 0);
+    B2_CUDA(cudaMemcpyAsync(scores_out, a.scores, sizeof(double) * n_scores, cudaMemcpyDeviceToHost, ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  return B2_OK;
+}
+
+int b2_solve_bayes_ridge(b2_ctx* ctx, int fit_intercept, const double* hyper, int max_iter, double tol,
+                         const double* anchor, int compute_score, double* coef, double* intercept, double* alpha_out,
+                         double* lambda_out, int* n_iter_out, double* scores_out, double* sigma_out) {
+  if (int r = use_device(ctx)) return r;
+  double n = 0.0;
+  if (int r = check_bayes_args(ctx, hyper, 6, max_iter, tol, coef, intercept, alpha_out, lambda_out, n_iter_out, &n))
+    return r;
+  if (!(n > 0.0)) { set_error("no row kept: the statistic holds no rows"); return B2_E_ARG; }
+  BayesArgs a;
+  a.a1 = hyper[0]; a.a2 = hyper[1]; a.l1 = hyper[2]; a.l2 = hyper[3]; a.alpha_init = hyper[4]; a.lambda_init = hyper[5];
+  a.threshold_lambda = 0.0;
+  a.tol = tol;
+  if (int r = bayes_block(ctx, anchor, max_iter, compute_score, fit_intercept, &a)) return r;
+  if (int r = launch_solve_eigh(ctx, fit_intercept)) return r;
+  if (int r = launch_bayes_ridge(ctx, a)) return r;
+  double converged = 0.0;
+  B2_CUDA(cudaMemcpyAsync(&converged, ctx->loo + kLooMisc + 3, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (int r = fetch_bayes(ctx, a, 1, coef, intercept, alpha_out, lambda_out, n_iter_out, scores_out, sigma_out)) return r;
+  return eigh_converged(converged);
+}
+
+int b2_solve_ard(b2_ctx* ctx, int fit_intercept, const double* hyper, double threshold_lambda, int max_iter, double tol,
+                 const double* anchor, int compute_score, double* coef, double* intercept, double* alpha_out,
+                 double* lambda_out, int* n_iter_out, double* scores_out, double* sigma_out) {
+  if (int r = use_device(ctx)) return r;
+  double n = 0.0;
+  if (int r = check_bayes_args(ctx, hyper, 4, max_iter, tol, coef, intercept, alpha_out, lambda_out, n_iter_out, &n))
+    return r;
+  if (!(threshold_lambda >= 0.0)) { set_error("threshold_lambda=%g must be >= 0", threshold_lambda); return B2_E_ARG; }
+  if (!(n >= 2.0)) { set_error("the statistic holds %.0f rows, ARDRegression needs at least 2", n); return B2_E_ARG; }
+  BayesArgs a;
+  a.a1 = hyper[0]; a.a2 = hyper[1]; a.l1 = hyper[2]; a.l2 = hyper[3]; a.alpha_init = NAN; a.lambda_init = NAN;
+  a.threshold_lambda = threshold_lambda;
+  a.tol = tol;
+  if (int r = bayes_block(ctx, anchor, max_iter, compute_score, fit_intercept, &a)) return r;
+  if (int r = launch_ard(ctx, a)) return r;
+  return fetch_bayes(ctx, a, 0, coef, intercept, alpha_out, lambda_out, n_iter_out, scores_out, sigma_out);
+}
+
+// The operands into ctx->enet, then the pass; host rows re-stream through the staging ring, their outputs through two
+// device blocks of stage_rows x 2 doubles.
+int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+                 const double* mean, const double* sigma, double noise_var, const double* coef, double intercept,
+                 double* yhat, double* ystd) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (sigma == nullptr || coef == nullptr || ystd == nullptr) { set_error("sigma / coef / ystd is null"); return B2_E_ARG; }
+  if (n_rows > 0 && X == nullptr) { set_error("X is null"); return B2_E_ARG; }
+  if (!(noise_var >= 0.0) || !isfinite(noise_var)) { set_error("noise_var=%g must be >= 0 and finite", noise_var); return B2_E_ARG; }
+  if (n_rows == 0) return B2_OK;
+  if (int r = ensure_enet_block(ctx, kStdDoubles)) return r;
+  std::vector<double> op(kStdDoubles, 0.0);
+  memcpy(op.data() + kStdSigma, sigma, sizeof(double) * d * d);
+  double b_eff = intercept;
+  for (int j = 0; j < d; ++j) {
+    op[kStdMean + j] = mean != nullptr ? mean[j] : 0.0;
+    op[kStdCoef + j] = coef[j];
+    b_eff += op[kStdMean + j] * coef[j];
+  }
+  op[kStdMisc] = b_eff;
+  op[kStdMisc + 1] = noise_var;
+  B2_CUDA(cudaMemcpyAsync(ctx->enet, op.data(), sizeof(double) * kStdDoubles, cudaMemcpyHostToDevice, ctx->stream));
+  if (mem_kind == B2_MEM_DEVICE) {
+    if (int r = launch_score_std(ctx, X, x_dtype, n_rows, d, ldx, yhat, ystd)) return r;
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
+    return B2_OK;
+  }
+  if (int r = ensure_staging(ctx)) return r;
+  if (int r = ensure_cv_stage(ctx, 2)) return r;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = host_pointer_is_pinned(X);
+  const int64_t blk = ctx->stage_rows;
+  const int rc = stream_host_blocks(
+      ctx, n_rows, blk,
+      [&](int buf, int64_t r0, int64_t rows) {
+        return stage_rows_h2d(ctx, buf, X, es, nullptr, nullptr, r0, rows, d, ldx, x_pinned);
+      },
+      [&](int buf, int64_t r0, int64_t rows) -> int {
+        double* sd = ctx->cv_stage[buf];
+        double* yd = yhat != nullptr ? sd + blk : nullptr;
+        if (int r = launch_score_std(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, yd, sd)) return r;
+        B2_CUDA(cudaMemcpyAsync(ystd + r0, sd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+        if (yhat != nullptr)
+          B2_CUDA(cudaMemcpyAsync(yhat + r0, yd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+        return B2_OK;
+      });
+  const cudaError_t done = cudaStreamSynchronize(ctx->stream);
+  if (rc != B2_OK) return rc;
+  B2_CUDA(done);
+  return B2_OK;
 }
 
 // ---- scoring ---------------------------------------------------------------------------------------

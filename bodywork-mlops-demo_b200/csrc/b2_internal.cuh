@@ -50,7 +50,8 @@ constexpr int kTcSums = 3;               // per-CTA CUDA-core sums: sum y', sum 
 // ---- scoring (b2_score, b2_metrics) and the refined fit (b2_fit_refined) ---------------------------------------------
 constexpr int kNStats = 10;              // include/b2gram.h: b2_score stats_out layout (maxima at 4 and 9, sums elsewhere)
 // the refined fit's model y = b0' + (x - m).beta and its residual passes
-constexpr int kGradOut = kMaxD + 1;      // one gradient: g_j = sum (x_j - m_j) e at j < kMaxD, g_1 = sum e at kMaxD
+// one gradient: g_j = sum (x_j - m_j) e at j < kMaxD, g_1 = sum e at kMaxD, and sum e^2 at kMaxD + 1 (b2_residual_moments)
+constexpr int kGradOut = kMaxD + 2;
 // doubles of ctx->refine
 constexpr int kRfBeta = 0;               // beta
 constexpr int kRfB0 = kMaxD;             // b0'
@@ -94,6 +95,28 @@ struct EnetArgs {
   const double* l1_ratios = nullptr;   // [n_l1]; nullptr: l1_ratio
   int n_folds = 1, n_l1 = 1;
   double* mse = nullptr;
+};
+
+// ---- BayesianRidge / ARDRegression (solve.cu: bayes_ridge_kernel, ard_kernel; DESIGN.md section 9) -------------------
+// Every pointer is into ctx->enet.  anchor: nullptr or [w0 kMaxD | g0 kMaxD | s0 | sse0] (b2_residual_moments at w0);
+// out: kBy* below; scores: max_iter + 1 doubles (written with compute_score); A: ard_kernel's copy of the centred Gram.
+constexpr int kByCoef = 0;                       // [kMaxD] coef
+constexpr int kByMisc = kMaxD;                   // [0] intercept [1] alpha [2] lambda (BayesianRidge) [3] n_iter [4] info
+constexpr int kByLambda = kMaxD + 8;             // [kMaxD] ARD's lambda per feature
+constexpr int kBySigma = 2 * kMaxD + 8;          // [d][d] sigma (row-major, pitch d)
+constexpr int kByDoubles = kBySigma + kMaxD * kMaxD;
+// operands of b2_score_std at ctx->enet: sigma [d][d] (pitch d), m, w, then [0] b + m.w, [1] noise_var
+constexpr int kStdSigma = 0;
+constexpr int kStdMean = kMaxD * kMaxD;
+constexpr int kStdCoef = kStdMean + kMaxD;
+constexpr int kStdMisc = kStdCoef + kMaxD;
+constexpr int kStdDoubles = kStdMisc + 8;
+struct BayesArgs {
+  double a1, a2, l1, l2, alpha_init, lambda_init;   // a NaN init: scikit-learn's default
+  double threshold_lambda, tol;
+  int max_iter, compute_score, fit_intercept;
+  const double* anchor;
+  double *out, *scores, *A;
 };
 
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
@@ -306,6 +329,13 @@ int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
                const uint8_t* mask, int keep, int n_alphas, double* cv, bool first_block);
 // the elastic-net path of the resident S (one launch; `args` points into ctx->enet)
 int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args);
+// BayesianRidge's iteration in the eigenbasis of ctx->loo (launch_solve_eigh first); one launch
+int launch_bayes_ridge(b2_ctx* ctx, const BayesArgs& args);
+// ARDRegression's iteration on the resident S; one launch
+int launch_ard(b2_ctx* ctx, const BayesArgs& args);
+// ystd (and yhat when not null) of the rows [0, n): sqrt(max((x - m)^T sigma (x - m), 0) + noise_var) and x.w + b, from
+// the operands at ctx->enet (kStd* in score_std.cu, written by the caller)
+int launch_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* yhat, double* ystd);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

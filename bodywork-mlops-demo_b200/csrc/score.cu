@@ -128,13 +128,14 @@ __device__ __forceinline__ void stats_fold(const double (*red)[kNStats], double*
     part[(size_t)blockIdx.x * kNStats + k] = acc;
   }
 }
-// red[w] holds warp w's gradient sums at the features < d and at kMaxD (g_1); every other entry of the partial is zero
+// red[w] holds warp w's gradient sums at the features < d, at kMaxD (g_1) and at kMaxD + 1 (sum e^2); every other entry
+// of the partial is zero
 template <int NW>
 __device__ __forceinline__ void grad_fold(const double (*red)[kGradOut], int d, double* __restrict__ part) {
   __syncthreads();
   for (int t = threadIdx.x; t < kGradOut; t += blockDim.x) {
     double v = 0.0;
-    if (t < d || t == kMaxD)
+    if (t < d || t >= kMaxD)
       for (int w = 0; w < NW; ++w) v += red[w][t];
     part[(size_t)blockIdx.x * kGradOut + t] = v;
   }
@@ -627,11 +628,11 @@ metrics_kernel(const V* __restrict__ ya, const V* __restrict__ yp, int64_t n, do
 
 // ---- residual gradient of the refined fit (b2_fit_refined; DESIGN.md section 2) -----------------------------------------
 // The model is yhat = b0' + (x - m).beta (st: ctx->refine).  Per kept row e = y - b0' - (x - m).beta, and the pass sums
-// g_j = sum (x_j - m_j) e and g_1 = sum e, everything in fp64 from the exactly converted x: e is a small difference of
-// large terms.  The three layouts of scoring carry it: register-fed (any layout, the tails), the TMA ring (wide contiguous
+// g_j = sum (x_j - m_j) e, g_1 = sum e and sum e^2 (the last read only by b2_residual_moments), everything in fp64 from the
+// exactly converted x: e is a small difference of large terms.  The three layouts of scoring carry it: register-fed (any layout, the tails), the TMA ring (wide contiguous
 // rows), one lane per row (d <= 16).  A lane keeps the fp64 sums of the features it loads.  A dropped row gets x = 0 and
 // e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA combines its sums in a fixed order into
-// part[blockIdx.x][kGradOut] (features, then g_1 at kMaxD); grad_reduce_kernel adds the CTAs in order.
+// part[blockIdx.x][kGradOut] (features, then g_1 at kMaxD, sum e^2 at kMaxD + 1); grad_reduce_kernel adds the CTAs in order.
 template <typename T>
 __device__ __forceinline__ float ld_x_f32(const T* __restrict__ p);
 template <>
@@ -645,7 +646,7 @@ __global__ void __launch_bounds__(kScoreThreads)
 grad_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double* __restrict__ st,
             const float* __restrict__ y, const uint8_t* __restrict__ mask, int keep, int vec, double* __restrict__ part) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double cf[4], mv[4], acc[4], acc1 = 0.0;
+  double cf[4], mv[4], acc[4], acc1 = 0.0, acc2 = 0.0;
   int fj[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -705,13 +706,17 @@ grad_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double
 #pragma unroll
       for (int k = 0; k < 4; ++k) acc[k] = fma((double)x[u][k] - mv[k], e, acc[k]);
       acc1 += e;
+      acc2 = fma(e, e, acc2);
     }
   }
   __shared__ double red[kScoreWarps][kGradOut];
 #pragma unroll
   for (int k = 0; k < 4; ++k)
     if (fj[k] < d) red[warp][fj[k]] = acc[k];
-  if (lane == 0) red[warp][kMaxD] = acc1;
+  if (lane == 0) {
+    red[warp][kMaxD] = acc1;
+    red[warp][kMaxD + 1] = acc2;
+  }
   grad_fold<kScoreWarps>(red, d, part);
 }
 
@@ -732,7 +737,9 @@ grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const d
 
   __shared__ double red[kTmWarps][kGradOut];
   __shared__ __align__(16) double m_s[kMaxD];
+  __shared__ double e2_s[kTmWarps][32];   // sum e^2 of the row group whose first lane this is: a register would spill
   for (int f = threadIdx.x; f < kMaxD; f += blockDim.x) m_s[f] = f < d ? st[kRfMean + f] : 0.0;
+  for (int t = threadIdx.x; t < kTmWarps * 32; t += blockDim.x) e2_s[t / 32][t % 32] = 0.0;
   __syncthreads();
   if (warp == kTmWarps) {
     if (lane == 0)
@@ -808,7 +815,10 @@ grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const d
         for (int k = 0; k < 4; ++k)
 #pragma unroll
           for (int q = 0; q < 4; ++q) acc[k][q] = fma(v[k][q], e, acc[k][q]);
-        if (j == 0) acc1 += e;
+        if (j == 0) {
+          acc1 += e;
+          e2_s[warp][lane] = fma(e, e, e2_s[warp][lane]);
+        }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty + 8 * s);
@@ -825,7 +835,10 @@ grad_tma_kernel(const T* __restrict__ X, int n_tiles, int sweeps, int d, const d
             const int f = f0[k] + q;
             if (f < d) red[warp][f] = gg == 0 ? acc[k][q] : red[warp][f] + acc[k][q];
           }
-        if (j == 0) red[warp][kMaxD] = gg == 0 ? acc1 : red[warp][kMaxD] + acc1;
+        if (j == 0) {
+          red[warp][kMaxD] = gg == 0 ? acc1 : red[warp][kMaxD] + acc1;
+          red[warp][kMaxD + 1] = gg == 0 ? e2_s[warp][lane] : red[warp][kMaxD + 1] + e2_s[warp][lane];
+        }
       }
       __syncwarp();
     }
@@ -860,7 +873,7 @@ grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __
       acc[k] = 0.0;
     }
     const double b0 = st[kRfB0];
-    double acc1 = 0.0;
+    double acc1 = 0.0, acc2 = 0.0;
     int s = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -886,19 +899,20 @@ grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __
 #pragma unroll
         for (int k = 0; k < DP; ++k) acc[k] = fma((double)x[k] - mv[k], e, acc[k]);
         acc1 += e;
+        acc2 = fma(e, e, acc2);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty + 8 * s);
       if (++s == kSnStages) { s = 0; phase ^= 1u; }
     }
 #pragma unroll
-    for (int k = 0; k <= DP; ++k) {
-      double v = k < DP ? acc[k] : acc1;
+    for (int k = 0; k <= DP + 1; ++k) {
+      double v = k < DP ? acc[k] : (k == DP ? acc1 : acc2);
 #pragma unroll
       for (int o = 16; o >= 1; o >>= 1) v += shfl_xor_d(v, o);
       if (lane == 0) {
         if (k < DP && k < d) red[warp][k] = v;
-        if (k == DP) red[warp][kMaxD] = v;
+        if (k >= DP) red[warp][kMaxD + k - DP] = v;
       }
     }
   }

@@ -1372,6 +1372,341 @@ solve_enet_kernel(const double* __restrict__ S, int d, EnetArgs a) {
 
 size_t enet_smem_bytes(int d) { return sizeof(double) * ((size_t)(d + 1) * (d + 1) + d + kMaxD + 8); }
 
+// ---- BayesianRidge and ARDRegression: evidence maximisation on the centred Gram (b2_solve_bayes_ridge, b2_solve_ard) --
+// Both restate scikit-learn 1.9's fit loops (sklearn/linear_model/_bayes.py) on the fp64 statistic; DESIGN.md section 9.
+// The residual sum of squares both need comes from the anchor (b2_residual_moments at w0: g0 = sum (x - m) e, s0 = sum e,
+// sse0 = sum e^2), exactly: sse(w) = sse0 - s0^2 / n - 2 D.g0 + D^T A D with D = w - w0; without an anchor from S alone,
+// sse(w) = ||yc||^2 - 2 w.r + w^T A w.  Every reduction is a warp butterfly, then the warps in order, so repeated calls are
+// bit-identical.
+constexpr int kByThreads = 512;
+constexpr double kF64Eps = 2.220446049250313e-16;    // np.finfo(np.float64).eps
+constexpr double kLog2Pi = 1.8378770664093453;       // log(2 pi)
+
+// the sum of every thread's v, in a fixed order, returned to every thread; red: blockDim.x / 32 doubles
+__device__ __forceinline__ double block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
+// row . x over the first d entries with 4 threads per row (thread = 4 row + part); every thread of a warp must call it
+// (a row past the matrix passes d = 0).  The four partial sums are combined by a fixed butterfly.
+__device__ __forceinline__ double row_dot4(const double* __restrict__ rowp, const double* __restrict__ x, int d, int part) {
+  double v = 0.0;
+  for (int j = part; j < d; j += 4) v = fma(rowp[j], x[j], v);
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+// n, ybar (0 without an intercept), ||yc||^2 (||y||^2 without an intercept) and y.var() (always about the mean) from S
+struct YStats {
+  double n, ybar, yy, y_var;
+};
+__device__ __forceinline__ YStats y_stats(const double* __restrict__ S, int d, int fit_intercept) {
+  const int dp = d + 2;
+  const double n = S[d * dp + d], sy = S[d * dp + d + 1], syy = S[(d + 1) * dp + d + 1];
+  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
+  YStats t;
+  t.n = n;
+  t.ybar = fit_intercept ? sy * inv_n : 0.0;
+  t.yy = fit_intercept ? syy - n * t.ybar * t.ybar : syy;
+  t.y_var = fmax(syy * inv_n - (sy * inv_n) * (sy * inv_n), 0.0);
+  return t;
+}
+
+size_t bayes_smem_bytes(int d) { return sizeof(double) * ((size_t)d * (d + 1) + 8 * kMaxD + 32); }
+
+// BayesianRidge.fit in the eigenbasis A = Q diag(lam) Q^T of solve_eigh_kernel (ctx->loo): w~ = c / (lam + lambda_ /
+// alpha_), coef = Q w~ every iteration (the stopping test sum |coef_old - coef| < tol is in the original basis),
+// gamma = sum alpha_ lam / (lambda_ + alpha_ lam), then lambda_ and alpha_ in scikit-learn's order.  With an anchor
+// D~ = w~ - Q^T w0 and g~0 = Q^T g0 are formed once, so sse = sse0 - s0^2 / n + sum lam D~^2 - 2 D~.g~0; without one
+// sse = ||yc||^2 - sum c^2 (lam + 2 s) / (lam + s)^2, s = lambda_ / alpha_.  logdet runs over all d eigenvalues, which is
+// scikit-learn's n <= d branch as well (the eigenvalues past rank n are 0).  Finally sigma = Q diag(1 / (alpha_ lam +
+// lambda_)) Q^T, its upper triangle mirrored.
+__global__ void __launch_bounds__(kByThreads, 1)
+bayes_ridge_kernel(const double* __restrict__ S, int d, const double* __restrict__ loo, const BayesArgs a) {
+  extern __shared__ double sm[];
+  const int pitch = d + 1;
+  double* Qs = sm;                    // Q[i][k], pitch d + 1
+  double* lam = Qs + d * pitch;
+  double* c = lam + kMaxD;            // Q^T r
+  double* wt = c + kMaxD;             // w~
+  double* coef = wt + kMaxD;
+  double* coef_old = coef + kMaxD;
+  double* w0t = coef_old + kMaxD;     // Q^T w0
+  double* g0t = w0t + kMaxD;          // Q^T g0
+  double* inv = g0t + kMaxD;          // 1 / (alpha_ lam + lambda_)
+  double* red = inv + kMaxD;          // [32]
+  const int tid = threadIdx.x, row = tid >> 2, part = tid & 3;
+  for (int t = tid; t < d * d; t += blockDim.x) {
+    const int i = t / d, k = t - i * d;
+    Qs[i * pitch + k] = loo[kLooQ + i * kMaxD + k];
+  }
+  for (int k = tid; k < d; k += blockDim.x) {
+    lam[k] = loo[kLooLam + k];
+    c[k] = loo[kLooC + k];
+  }
+  const YStats ys = y_stats(S, d, a.fit_intercept);
+  const double n = ys.n;
+  const bool anchored = a.anchor != nullptr;
+  double sse_base = ys.yy;
+  __syncthreads();
+  if (anchored) {
+    for (int k = tid; k < d; k += blockDim.x) {
+      double w = 0.0, g = 0.0;
+      for (int i = 0; i < d; ++i) {
+        w = fma(Qs[i * pitch + k], a.anchor[i], w);
+        g = fma(Qs[i * pitch + k], a.anchor[kMaxD + i], g);
+      }
+      w0t[k] = w;
+      g0t[k] = g;
+    }
+    const double s0 = a.anchor[2 * kMaxD], sse0 = a.anchor[2 * kMaxD + 1];
+    sse_base = sse0 - (a.fit_intercept && n > 0.0 ? s0 * s0 / n : 0.0);
+    __syncthreads();
+  }
+  double alpha = isnan(a.alpha_init) ? 1.0 / (ys.y_var + kF64Eps) : a.alpha_init;
+  double lmb = isnan(a.lambda_init) ? 1.0 : a.lambda_init;
+  // coef and sse at (alpha, lmb)
+  auto update_coef = [&]() -> double {
+    const double s = lmb / alpha;
+    double term = 0.0;
+    if (tid < d) {
+      const double q = lam[tid] + s, w = c[tid] / q;
+      wt[tid] = w;
+      if (anchored) {
+        const double dt = w - w0t[tid];
+        term = fma(lam[tid] * dt, dt, -2.0 * dt * g0t[tid]);
+      } else {
+        term = -(c[tid] * c[tid]) * (lam[tid] + 2.0 * s) / (q * q);
+      }
+    }
+    const double sse = sse_base + block_sum(term, red);   // its barriers publish wt
+    const double v = row_dot4(Qs + (row < d ? row : 0) * pitch, wt, row < d ? d : 0, part);
+    if (row < d && part == 0) coef[row] = v;
+    __syncthreads();
+    return sse;
+  };
+  auto score = [&](double sse) -> double {   // _log_marginal_likelihood
+    double ld = 0.0, cs = 0.0;
+    if (tid < d) {
+      ld = log(lmb + alpha * lam[tid]);
+      cs = coef[tid] * coef[tid];
+    }
+    const double logdet = -block_sum(ld, red);
+    const double csq = block_sum(cs, red);
+    double s = a.l1 * log(lmb) - a.l2 * lmb;
+    s += a.a1 * log(alpha) - a.a2 * alpha;
+    s += 0.5 * (d * log(lmb) + n * log(alpha) - alpha * sse - lmb * csq + logdet - n * kLog2Pi);
+    return s;
+  };
+  int iter = 0;
+  for (; iter < a.max_iter; ++iter) {
+    const double sse = update_coef();
+    if (a.compute_score) {
+      const double s = score(sse);
+      if (tid == 0) a.scores[iter] = s;
+    }
+    double gl = 0.0, cs = 0.0;
+    if (tid < d) {
+      gl = alpha * lam[tid] / (lmb + alpha * lam[tid]);
+      cs = coef[tid] * coef[tid];
+    }
+    const double gamma = block_sum(gl, red);
+    const double csq = block_sum(cs, red);
+    lmb = (gamma + 2.0 * a.l1) / (csq + 2.0 * a.l2);
+    alpha = (n - gamma + 2.0 * a.a1) / (sse + 2.0 * a.a2);
+    if (iter != 0 && block_sum(tid < d ? fabs(coef_old[tid] - coef[tid]) : 0.0, red) < a.tol) break;
+    if (tid < d) coef_old[tid] = coef[tid];
+  }
+  const int n_iter = iter < a.max_iter ? iter + 1 : a.max_iter;
+  const double sse = update_coef();
+  if (a.compute_score) {
+    const double s = score(sse);
+    if (tid == 0) a.scores[n_iter] = s;
+  }
+  for (int k = tid; k < d; k += blockDim.x) inv[k] = 1.0 / (alpha * lam[k] + lmb);
+  const double mc = block_sum(tid < d ? loo[kLooMean + tid] * coef[tid] : 0.0, red);
+  for (int t = tid; t < d * d; t += blockDim.x) {
+    const int i = t / d, j = t - i * d;
+    if (i > j) continue;
+    double v = 0.0;
+    for (int k = 0; k < d; ++k) v = fma(Qs[i * pitch + k] * inv[k], Qs[j * pitch + k], v);
+    a.out[kBySigma + i * d + j] = v;
+    a.out[kBySigma + j * d + i] = v;
+  }
+  if (tid < d) a.out[kByCoef + tid] = coef[tid];
+  if (tid == 0) {
+    a.out[kByMisc + 0] = a.fit_intercept ? ys.ybar - mc : 0.0;
+    a.out[kByMisc + 1] = alpha;
+    a.out[kByMisc + 2] = lmb;
+    a.out[kByMisc + 3] = n_iter;
+    a.out[kByMisc + 4] = 0.0;
+  }
+}
+
+size_t ard_smem_bytes(int d) { return sizeof(double) * ((size_t)d * (d + 1) + 8 * kMaxD + 32 + 8); }
+
+// ARDRegression.fit.  Per iteration: M = diag(lambda) + alpha A on the kept set, with a unit row and column for every
+// pruned feature, so pruned features decouple and the kept block of M^-1 is scikit-learn's sigma_; M^-1 by the sweep
+// operator in place (M becomes -M^-1; the pivots are the LDL^T pivots, so log det M = sum log pivot); coef_K = alpha
+// sigma r_K; sse from the anchor (with A D); gamma = 1 - lambda sigma_jj, lambda_K, alpha; then the prune (keep = lambda <
+// threshold_lambda), the score (fast_logdet(sigma) = -log det M) and the stopping test, in scikit-learn's order: sse uses
+// the coefficients before the prune, the score and the test those after it.  A non-positive pivot stops the kernel with
+// info = its index + 1.  A (the centred Gram) lives in global memory beside the outputs: with M it would not fit in
+// shared memory at d = 128, and two matrix-vector reads of it per iteration come from L2.
+__global__ void __launch_bounds__(kByThreads, 1)
+ard_kernel(const double* __restrict__ S, int d, const BayesArgs a) {
+  extern __shared__ double sm[];
+  const int pitch = d + 1;
+  double* M = sm;
+  double* r = M + d * pitch;
+  double* mean = r + kMaxD;
+  double* lmb = mean + kMaxD;
+  double* coef = lmb + kMaxD;
+  double* coef_old = coef + kMaxD;
+  double* keep = coef_old + kMaxD;    // 1: kept
+  double* col = keep + kMaxD;         // the pivot column of a sweep step
+  double* dlt = col + kMaxD;          // coef - w0
+  double* red = dlt + kMaxD;          // [32]
+  double* misc = red + 32;            // [0] ybar, [1] info
+  double* A = a.A;
+  const int tid = threadIdx.x, row = tid >> 2, part = tid & 3;
+  if (tid == 0) misc[1] = 0.0;
+  build_normal_equations(S, d, 0.0, a.fit_intercept, M, r, mean, &misc[0]);
+  for (int t = tid; t < d * d; t += blockDim.x) {
+    const int i = t / d, j = t - i * d;
+    A[t] = M[i * pitch + j];
+  }
+  for (int j = tid; j < d; j += blockDim.x) {
+    lmb[j] = 1.0;
+    coef[j] = 0.0;
+    keep[j] = 1.0;
+  }
+  const YStats ys = y_stats(S, d, a.fit_intercept);
+  const double n = ys.n;
+  const bool anchored = a.anchor != nullptr;
+  const double sse_base = anchored ? a.anchor[2 * kMaxD + 1] -
+                                         (a.fit_intercept && n > 0.0 ? a.anchor[2 * kMaxD] * a.anchor[2 * kMaxD] / n : 0.0)
+                                   : ys.yy;
+  __syncthreads();
+  double alpha = 1.0 / (ys.y_var + kF64Eps);
+  // M -> -M^-1; returns log det M, NaN after a non-positive pivot.  Entry (i, j) becomes M_ij - (M_ik M_kj) / p, which
+  // keeps M exactly symmetric.
+  auto sweep = [&]() -> double {
+    double logdet = 0.0;
+    for (int k = 0; k < d; ++k) {
+      for (int i = tid; i < d; i += blockDim.x) col[i] = M[i * pitch + k];
+      __syncthreads();
+      const double p = col[k];
+      if (!(p > 0.0)) {                           // the same p in every thread: a uniform exit
+        if (tid == 0) misc[1] = k + 1;
+        return NAN;
+      }
+      const double rp = 1.0 / p;
+      logdet += log(p);
+      for (int t = tid; t < d * d; t += blockDim.x) {
+        const int i = t / d, j = t - i * d;
+        double v;
+        if (i == k) v = j == k ? -rp : col[j] * rp;
+        else if (j == k) v = col[i] * rp;
+        else v = M[i * pitch + j] - (col[i] * col[j]) * rp;
+        M[i * pitch + j] = v;
+      }
+      __syncthreads();
+    }
+    return logdet;
+  };
+  // M of the current (alpha, lambda, keep), sigma, coef_K = alpha sigma r_K
+  auto solve = [&]() -> double {
+    for (int t = tid; t < d * d; t += blockDim.x) {
+      const int i = t / d, j = t - i * d;
+      const bool kk = keep[i] != 0.0 && keep[j] != 0.0;
+      M[i * pitch + j] = kk ? fma(alpha, A[t], i == j ? lmb[i] : 0.0) : (i == j ? 1.0 : 0.0);
+    }
+    for (int j = tid; j < d; j += blockDim.x) dlt[j] = keep[j] != 0.0 ? r[j] : 0.0;
+    __syncthreads();
+    const double ld = sweep();
+    if (isnan(ld)) return ld;
+    const double v = row_dot4(M + (row < d ? row : 0) * pitch, dlt, row < d ? d : 0, part);
+    if (row < d && part == 0 && keep[row] != 0.0) coef[row] = -alpha * v;
+    __syncthreads();
+    return ld;
+  };
+  auto sse_of = [&]() -> double {
+    if (tid < d) dlt[tid] = coef[tid] - (anchored ? a.anchor[tid] : 0.0);
+    __syncthreads();
+    const double v = row_dot4(A + (row < d ? row : 0) * d, dlt, row < d ? d : 0, part);
+    double term = 0.0;
+    if (row < d && part == 0) term = dlt[row] * (v - 2.0 * (anchored ? a.anchor[kMaxD + row] : r[row]));
+    return sse_base + block_sum(term, red);
+  };
+  double nkeep = d;
+  bool singular = false;
+  int iter = 0;
+  for (; iter < a.max_iter; ++iter) {
+    const double ld = solve();
+    if (isnan(ld)) {
+      singular = true;
+      break;
+    }
+    const double sse = sse_of();
+    double g = 0.0;
+    if (tid < d && keep[tid] != 0.0) {
+      g = 1.0 + lmb[tid] * M[tid * pitch + tid];   // 1 - lambda_j sigma_jj
+      lmb[tid] = (g + 2.0 * a.l1) / (coef[tid] * coef[tid] + 2.0 * a.l2);
+    }
+    alpha = (n - block_sum(g, red) + 2.0 * a.a1) / (sse + 2.0 * a.a2);
+    double kept = 0.0;
+    if (tid < d) {
+      kept = lmb[tid] < a.threshold_lambda ? 1.0 : 0.0;
+      keep[tid] = kept;
+      if (kept == 0.0) coef[tid] = 0.0;
+    }
+    nkeep = block_sum(kept, red);
+    if (a.compute_score) {
+      double t1 = 0.0, t2 = 0.0, t3 = 0.0;
+      if (tid < d) {
+        t1 = a.l1 * log(lmb[tid]) - a.l2 * lmb[tid];
+        t2 = log(lmb[tid]);
+        t3 = lmb[tid] * coef[tid] * coef[tid];
+      }
+      double s = block_sum(t1, red);
+      const double slog = block_sum(t2, red), sq = block_sum(t3, red);
+      s += a.a1 * log(alpha) - a.a2 * alpha;
+      s += 0.5 * (-ld + n * log(alpha) + slog);
+      s -= 0.5 * (alpha * sse + sq);
+      if (tid == 0) a.scores[iter] = s;
+    }
+    if (iter > 0 && block_sum(tid < d ? fabs(coef_old[tid] - coef[tid]) : 0.0, red) < a.tol) break;
+    if (tid < d) coef_old[tid] = coef[tid];
+    if (nkeep == 0.0) break;
+  }
+  const int n_iter = iter < a.max_iter ? iter + 1 : a.max_iter;
+  if (!singular && nkeep > 0.0 && isnan(solve())) singular = true;
+  const double mc = block_sum(tid < d ? mean[tid] * coef[tid] : 0.0, red);
+  for (int t = tid; t < d * d; t += blockDim.x) {
+    const int i = t / d, j = t - i * d;
+    a.out[kBySigma + t] = !singular && nkeep > 0.0 && keep[i] != 0.0 && keep[j] != 0.0 ? -M[i * pitch + j] : 0.0;
+  }
+  if (tid < d) {
+    a.out[kByCoef + tid] = coef[tid];
+    a.out[kByLambda + tid] = lmb[tid];
+  }
+  if (tid == 0) {
+    a.out[kByMisc + 0] = a.fit_intercept ? misc[0] - mc : 0.0;
+    a.out[kByMisc + 1] = alpha;
+    a.out[kByMisc + 3] = n_iter;
+    a.out[kByMisc + 4] = misc[1];
+  }
+}
+
 size_t solve_smem_bytes(int d) {
   // Cholesky: A, mean, invd, misc, U panel; eigenvalue kernel: A, r, mean, misc, (v, w) x 2, pv, dd, ee2, lam
   const size_t chol = (size_t)(d + 1) * (d + 1) + 3 * d + 16 + (size_t)(d + 1) * kUPitch;
@@ -1390,6 +1725,9 @@ int ensure_solve_attrs(b2_ctx* ctx) {
                                  (int)eigh_smem_bytes(kMaxD)));
     B2_CUDA(cudaFuncSetAttribute(solve_enet_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)enet_smem_bytes(kMaxD)));
+    B2_CUDA(cudaFuncSetAttribute(bayes_ridge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)bayes_smem_bytes(kMaxD)));
+    B2_CUDA(cudaFuncSetAttribute(ard_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ard_smem_bytes(kMaxD)));
     ctx->solve_attr_set = true;
   }
   return B2_OK;
@@ -1449,6 +1787,22 @@ int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args) {
   if (int r = ensure_solve_attrs(ctx)) return r;
   const int ctas = args.folds != nullptr ? args.n_folds * args.n_l1 : 1;
   solve_enet_kernel<<<ctas, kEnetThreads, enet_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, args);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_bayes_ridge(b2_ctx* ctx, const BayesArgs& args) {
+  if (int r = ensure_solve_attrs(ctx)) return r;
+  bayes_ridge_kernel<<<1, kByThreads, bayes_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, ctx->loo, args);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_ard(b2_ctx* ctx, const BayesArgs& args) {
+  if (int r = ensure_solve_attrs(ctx)) return r;
+  ard_kernel<<<1, kByThreads, ard_smem_bytes(ctx->d), ctx->stream>>>(ctx->S, ctx->d, args);
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
   return B2_OK;

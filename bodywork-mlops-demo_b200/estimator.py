@@ -797,3 +797,178 @@ class B200LassoCV(B200ElasticNetCV):
 
     def __repr__(self) -> str:
         return f"B200LassoCV(cv={self.cv!r})"
+
+
+# ---- BayesianRidge / ARDRegression: evidence maximisation on the fp64 Gram (DESIGN.md section 9) -------------------------
+class _B200Bayes:
+    """What BayesianRidge and ARDRegression share: a fit is the Gram pass with the least-squares solution w0 (``ctx.fit``;
+    the minimum-norm solution when the factorisation refuses), one fp64 pass over the same rows for the anchor
+    (``residual_moments`` at w0, which makes the residual sum of squares of every iteration exact), then one solve on the
+    resident statistic.  ``predict(X, return_std=True)`` is one fp64 tensor-core pass (``score_std``)."""
+    _sk_name = ""
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def _solve(self, ctx: native.Context, anchor) -> dict:
+        raise NotImplementedError
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None):
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``."""
+        if sample_weight is not None:
+            raise ValueError(f"sample_weight is not supported by B200{self._sk_name}: every kept row has weight 1")
+        ctx = self.ctx
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        d = X.shape[1]
+        try:
+            try:
+                w0, b0 = ctx.fit(X, y, row_mask, mask_keep, 0.0, fit_intercept=self.fit_intercept)
+            except np.linalg.LinAlgError:
+                w0, b0, _, _ = ctx.solve_spectral(1e-12, fit_intercept=self.fit_intercept)
+            moments = ctx.residual_moments(X, y, w0, b0, row_mask, mask_keep, fit_intercept=self.fit_intercept)
+        finally:
+            for a in owned:
+                a.free()
+        S = ctx.gram_export()
+        n = S[d, d]
+        need = 2 if self._sk_name == "ARDRegression" else 1
+        if not n >= need:
+            raise ValueError(f"Found array with {int(n)} sample(s) (shape=({int(n)}, {d})) while a minimum of {need} is "
+                             f"required by B200{self._sk_name}.")
+        res = self._solve(ctx, np.concatenate([w0, moments]))
+        if not (np.all(np.isfinite(res["coef"])) and np.isfinite(res["intercept"]) and np.isfinite(res["alpha"])):
+            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        self.coef_ = res["coef"]
+        self.intercept_ = np.float64(res["intercept"] if self.fit_intercept else 0.0)
+        self.alpha_ = np.float64(res["alpha"])
+        self.n_iter_ = int(res["n_iter"])
+        self.X_offset_ = S[:d, d] / n if self.fit_intercept else np.zeros(d)
+        self.X_scale_ = np.ones(d)
+        self.n_features_in_ = int(d)
+        self.scores_ = np.asarray(res["scores"]) if self.compute_score else []
+        self._set_posterior(res)
+        return self
+
+    def _full_sigma(self) -> np.ndarray:
+        return self.sigma_
+
+    def predict(self, X, return_std: bool = False):
+        ctx = self.ctx
+        on_device = isinstance(X, native.DeviceArray)
+        Xh = X if on_device else _as_f32_matrix(X)
+        if Xh.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        if not return_std:
+            yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
+            return yhat if on_device else yhat.astype(np.float64)
+        return ctx.score_std(Xh, self.X_offset_, self._full_sigma(), 1.0 / float(self.alpha_), self.coef_,
+                             float(self.intercept_))
+
+    def _sk_params(self) -> dict:
+        raise NotImplementedError
+
+    def to_sklearn(self):
+        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable; its own
+        ``predict(X, return_std=True)`` works)."""
+        from sklearn import linear_model
+        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        for name in ("coef_", "intercept_", "alpha_", "lambda_", "sigma_", "scores_", "n_iter_", "X_offset_", "X_scale_",
+                     "n_features_in_"):
+            v = getattr(self, name)
+            setattr(reg, name, v.copy() if isinstance(v, np.ndarray) else v)
+        return reg
+
+
+class B200BayesianRidge(_B200Bayes):
+    """``sklearn.linear_model.BayesianRidge`` fitted on the H100: ``b2_solve_bayes_ridge`` runs scikit-learn 1.9's
+    iteration in the eigenbasis of the fp64 centred Gram.  Sets coef_, intercept_, alpha_, lambda_, sigma_, scores_ (with
+    compute_score), n_iter_, X_offset_, X_scale_ and n_features_in_.  copy_X and verbose have no effect."""
+    _sk_name = "BayesianRidge"
+
+    def __init__(self, *, max_iter: int = 300, tol: float = 1e-3, alpha_1: float = 1e-6, alpha_2: float = 1e-6,
+                 lambda_1: float = 1e-6, lambda_2: float = 1e-6, alpha_init=None, lambda_init=None,
+                 compute_score: bool = False, fit_intercept: bool = True, copy_X: bool = True, verbose: bool = False,
+                 ctx: Optional[native.Context] = None):
+        self.max_iter = max_iter
+        self.tol = tol
+        self.alpha_1 = alpha_1
+        self.alpha_2 = alpha_2
+        self.lambda_1 = lambda_1
+        self.lambda_2 = lambda_2
+        self.alpha_init = alpha_init
+        self.lambda_init = lambda_init
+        self.compute_score = compute_score
+        self.fit_intercept = fit_intercept
+        self.copy_X = copy_X
+        self.verbose = verbose
+        self._ctx = ctx
+
+    def _solve(self, ctx, anchor):
+        return ctx.solve_bayes_ridge(self.alpha_1, self.alpha_2, self.lambda_1, self.lambda_2, self.alpha_init,
+                                     self.lambda_init, max_iter=self.max_iter, tol=self.tol, anchor=anchor,
+                                     compute_score=self.compute_score, fit_intercept=self.fit_intercept)
+
+    def _set_posterior(self, res: dict) -> None:
+        self.lambda_ = np.float64(res["lambda"])
+        self.sigma_ = res["sigma"]
+
+    def _sk_params(self) -> dict:
+        return dict(max_iter=self.max_iter, tol=self.tol, alpha_1=self.alpha_1, alpha_2=self.alpha_2,
+                    lambda_1=self.lambda_1, lambda_2=self.lambda_2, alpha_init=self.alpha_init,
+                    lambda_init=self.lambda_init, compute_score=self.compute_score, fit_intercept=self.fit_intercept,
+                    copy_X=self.copy_X, verbose=self.verbose)
+
+    def __repr__(self) -> str:
+        return "B200BayesianRidge()"
+
+
+class B200ARDRegression(_B200Bayes):
+    """``sklearn.linear_model.ARDRegression`` fitted on the H100: ``b2_solve_ard`` runs scikit-learn 1.9's iteration,
+    pruning included, in one single-SM launch on the fp64 statistic.  Sets sklearn's attributes; sigma_ is kept x kept
+    ((0, 0) when every feature is pruned).  copy_X and verbose have no effect."""
+    _sk_name = "ARDRegression"
+
+    def __init__(self, *, max_iter: int = 300, tol: float = 1e-3, alpha_1: float = 1e-6, alpha_2: float = 1e-6,
+                 lambda_1: float = 1e-6, lambda_2: float = 1e-6, compute_score: bool = False,
+                 threshold_lambda: float = 1e4, fit_intercept: bool = True, copy_X: bool = True, verbose: bool = False,
+                 ctx: Optional[native.Context] = None):
+        self.max_iter = max_iter
+        self.tol = tol
+        self.alpha_1 = alpha_1
+        self.alpha_2 = alpha_2
+        self.lambda_1 = lambda_1
+        self.lambda_2 = lambda_2
+        self.compute_score = compute_score
+        self.threshold_lambda = threshold_lambda
+        self.fit_intercept = fit_intercept
+        self.copy_X = copy_X
+        self.verbose = verbose
+        self._ctx = ctx
+
+    def _solve(self, ctx, anchor):
+        return ctx.solve_ard(self.alpha_1, self.alpha_2, self.lambda_1, self.lambda_2,
+                             threshold_lambda=self.threshold_lambda, max_iter=self.max_iter, tol=self.tol,
+                             anchor=anchor, compute_score=self.compute_score, fit_intercept=self.fit_intercept)
+
+    def _set_posterior(self, res: dict) -> None:
+        self.lambda_ = np.asarray(res["lambda"], dtype=np.float64)
+        keep = self.lambda_ < self.threshold_lambda
+        self.sigma_ = res["sigma"][np.ix_(keep, keep)].copy()
+
+    def _full_sigma(self) -> np.ndarray:
+        keep = self.lambda_ < self.threshold_lambda
+        full = np.zeros((self.n_features_in_, self.n_features_in_))
+        full[np.ix_(keep, keep)] = self.sigma_
+        return full
+
+    def _sk_params(self) -> dict:
+        return dict(max_iter=self.max_iter, tol=self.tol, alpha_1=self.alpha_1, alpha_2=self.alpha_2,
+                    lambda_1=self.lambda_1, lambda_2=self.lambda_2, compute_score=self.compute_score,
+                    threshold_lambda=self.threshold_lambda, fit_intercept=self.fit_intercept, copy_X=self.copy_X,
+                    verbose=self.verbose)
+
+    def __repr__(self) -> str:
+        return "B200ARDRegression()"

@@ -247,6 +247,55 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
                  int mem_kind, const uint8_t* row_mask, int mask_keep, const double* alphas, int n_alphas,
                  int fit_intercept, double* mse_out, double* cv_out, int* best_out, double* coef, double* intercept);
 
+/* ---- BayesianRidge / ARDRegression: replaces sklearn.linear_model.BayesianRidge / ARDRegression .fit and
+ * .predict(X, return_std=True) (DESIGN section 9).
+ * b2_residual_moments: one fp64 pass over the kept rows at the model (coef, intercept), through the refined fit's
+ * gradient kernels: out (host, d + 2 doubles) = sum (x_j - m_j) e, then sum e, then sum e^2, e = y - intercept - x.coef,
+ * everything from the exactly converted stored values; m are the column means of the resident S (0 without
+ * fit_intercept), which must have d features.  At the least-squares solution w0 of S (b2_fit, or b2_solve_spectral when
+ * the factorisation refuses) with intercept ybar - m.w0 this is the anchor [w0 | out] of the solves below.
+ * B2_E_UNSUPPORTED with more than one rank; B2_E_STATE when the resident S has another d. */
+int b2_residual_moments(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                        int mem_kind, const uint8_t* row_mask, int mask_keep, const double* coef, double intercept,
+                        int fit_intercept, double* out);
+/* b2_solve_bayes_ridge: BayesianRidge(...).fit on the resident S, restating scikit-learn 1.9's BayesianRidge.fit
+ * (sklearn/linear_model/_bayes.py: _update_coef_, _log_marginal_likelihood, the MacKay updates of alpha_ / lambda_ and
+ * the stopping test sum |coef_old - coef| < tol) in the eigenbasis of the centred Gram A = Xc^T Xc (b2_solve_eigh's
+ * kernel, then one single-CTA kernel).
+ *   hyper       [alpha_1, alpha_2, lambda_1, lambda_2, alpha_init, lambda_init]; a NaN init takes scikit-learn's default
+ *               (1 / (y.var() + eps), 1)
+ *   anchor      NULL, or [w0 (d) | g0 (d) | s0 | sse0] from b2_residual_moments at w0.  The residual sum of squares is
+ *               sse(w) = sse0 - s0^2 / n - 2 (w - w0).g0 + (w - w0)^T A (w - w0) (the s0 term only with fit_intercept),
+ *               exact for any w; NULL takes sse from S alone, ||yc||^2 - 2 w.r + w^T A w, whose error grows with
+ *               ||yc||^2 / sse (statistics brought in by b2_gram_import)
+ *   outputs     (host) coef d, intercept, alpha_out, lambda_out 1, n_iter_out; scores_out NULL or max_iter + 1 doubles
+ *               (n_iter + 1 written, with compute_score: sklearn's scores_); sigma_out NULL or d x d (sklearn's sigma_)
+ * Not converging within max_iter is no error (n_iter == max_iter).  B2_E_ARG: a hyper-parameter < 0 or not finite,
+ * max_iter < 1, tol < 0, a null output, or a statistic without rows. */
+int b2_solve_bayes_ridge(b2_ctx* ctx, int fit_intercept, const double* hyper, int max_iter, double tol,
+                         const double* anchor, int compute_score, double* coef, double* intercept, double* alpha_out,
+                         double* lambda_out, int* n_iter_out, double* scores_out, double* sigma_out);
+/* b2_solve_ard: ARDRegression(...).fit on the resident S in one single-CTA launch, restating scikit-learn 1.9's
+ * ARDRegression.fit (_update_sigma, update_coeff, the updates of lambda_ / alpha_, the prune lambda_ < threshold_lambda,
+ * the score and the stopping test, in that order).  hyper = [alpha_1, alpha_2, lambda_1, lambda_2]; anchor as above;
+ * lambda_out d doubles; scores_out NULL or max_iter doubles (n_iter
+ * written); sigma_out NULL or d x d: sklearn's kept x kept sigma_ at the kept rows and columns, zeros
+ * elsewhere (all zeros when every feature is pruned).  sigma is the exact inverse of diag(lambda) + alpha A on the kept
+ * set; sklearn's pinvh drops eigenvalues below d eps lambda_max, so the two agree while that matrix has a condition
+ * number below 1 / (d eps).  B2_E_SINGULAR on a non-positive pivot; B2_E_ARG as b2_solve_bayes_ridge, threshold_lambda
+ * < 0, or fewer than 2 rows (sklearn's ensure_min_samples=2). */
+int b2_solve_ard(b2_ctx* ctx, int fit_intercept, const double* hyper, double threshold_lambda, int max_iter, double tol,
+                 const double* anchor, int compute_score, double* coef, double* intercept, double* alpha_out,
+                 double* lambda_out, int* n_iter_out, double* scores_out, double* sigma_out);
+/* b2_score_std: predict(X, return_std=True) of either model.  Per row, v = x - mean:
+ *   ystd = sqrt(max(v^T sigma v, 0) + noise_var),  yhat = x.coef + intercept
+ * mean (NULL: zeros; sklearn's X_offset_), sigma d x d, coef d: host; noise_var = 1 / alpha_.  yhat (may be NULL) and
+ * ystd are n_rows fp64 where X lives (mem_kind); host rows hold two device staging blocks of 262 144 x 2 doubles in the
+ * context.  One fp64 tensor-core pass over the rows.  B2_E_ARG: null sigma / coef / ystd, noise_var < 0 or not finite. */
+int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+                 const double* mean, const double* sigma, double noise_var, const double* coef, double intercept,
+                 double* yhat, double* ystd);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
