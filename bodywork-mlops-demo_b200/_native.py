@@ -25,6 +25,8 @@ EXCHANGE_NONE, EXCHANGE_NCCL, EXCHANGE_PEER = 0, 1, 2
 ABI_VERSION = 2
 MAX_D = 128
 MAX_ALPHAS = 64
+GLM_LOG, GLM_IDENTITY = 0, 1
+GLM_STEPS = 21
 
 _c_i64 = C.c_int64
 _vp = C.c_void_p
@@ -82,6 +84,11 @@ _SIGNATURES = {
                                C.POINTER(C.c_double), C.POINTER(C.c_double), _vp, C.POINTER(C.c_int), _vp, _vp]),
     "b2_score_std": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, _vp, C.c_double, _vp,
                                C.c_double, _vp, _vp]),
+    "b2_glm_pass": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_int,
+                              C.c_double, _vp, C.c_double, C.c_int, _vp, _vp]),
+    "b2_glm_line_search": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_int,
+                                     C.c_double, _vp, C.c_double, _vp, C.c_double, C.c_int, _vp]),
+    "b2_glm_predict": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, C.c_int, _vp, C.c_double, _vp]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -674,6 +681,67 @@ class Context:
             raise ValueError(last_error())
         _check(rc, "b2_score_std")
         return yhat, ystd
+
+    # -- PoissonRegressor / GammaRegressor / TweedieRegressor (DESIGN.md section 10) --------------------------------
+    def _glm_coef(self, coef, d: int) -> np.ndarray:
+        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
+        if w.size != d:
+            raise ValueError(f"coef has {w.size} entries, X has {d} columns")
+        return w
+
+    def glm_pass(self, X, y, coef, intercept: float, *, link: int = GLM_LOG, power: float = 1.0, row_mask=None,
+                 mask_keep: int = 1, fit_intercept: bool = True, hessian: bool = True) -> dict:
+        """One pass of the Newton solver's statistics at (coef, intercept) over the kept rows (b2_glm_pass).  Returns
+        a dict of unscaled sums: loss, const (constant_to_optimal_zero), sum_y, kept, y_out_of_range, h_nonpos,
+        y_nonfinite (floats), grad ((d + 1,): sum g x_j, then sum g) and hessian ((d + 1, d + 1) sum |h| [x 1][x 1]^T,
+        or None without ``hessian``).  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        w = self._glm_coef(coef, d)
+        sums = np.empty(d + 8, dtype=np.float64)
+        hess = np.empty((d + 1, d + 1), dtype=np.float64) if hessian else None
+        rc = load().b2_glm_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), int(link), float(power),
+                                w.ctypes.data, float(intercept), int(bool(fit_intercept)), sums.ctypes.data,
+                                hess.ctypes.data if hess is not None else None)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_glm_pass")
+        keys = ("loss", "const", "sum_y", "kept", "y_out_of_range", "h_nonpos", "y_nonfinite")
+        out = {k: float(sums[i]) for i, k in enumerate(keys)}
+        out["grad"] = sums[7:].copy()
+        out["hessian"] = hess
+        return out
+
+    def glm_line_search(self, X, y, coef, intercept: float, step, step_intercept: float, *, link: int = GLM_LOG,
+                        power: float = 1.0, n_steps: int = GLM_STEPS, row_mask=None, mask_keep: int = 1) -> np.ndarray:
+        """The backtracking ladder in one pass (b2_glm_line_search): the summed loss over the kept rows at
+        (coef, intercept) + 2^-k (step, step_intercept) for k < n_steps."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        w, s = self._glm_coef(coef, d), self._glm_coef(step, d)
+        out = np.empty(max(int(n_steps), 1), dtype=np.float64)
+        rc = load().b2_glm_line_search(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), int(link), float(power),
+                                       w.ctypes.data, float(intercept), s.ctypes.data, float(step_intercept),
+                                       int(n_steps), out.ctypes.data)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_glm_line_search")
+        return out
+
+    def glm_predict(self, X, coef, intercept: float, *, link: int = GLM_LOG):
+        """mu = exp(X coef + intercept) (GLM_LOG) or X coef + intercept per row in fp64 (b2_glm_predict): a float64
+        ndarray for host rows, an f64 DeviceArray for device rows."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        w = self._glm_coef(coef, d)
+        mu = self.empty((n,), "f64") if mk == MEM_DEVICE else np.empty(n, dtype=np.float64)
+        rc = load().b2_glm_predict(self._h, ptr, xdt, n, d, d, mk, int(link), w.ctypes.data, float(intercept),
+                                   mu.ptr if mk == MEM_DEVICE else mu.ctypes.data)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_glm_predict")
+        return mu
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

@@ -412,7 +412,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1],
-                  ctx->enet, ctx->folds, ctx->fold_range};
+                  ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1447,6 +1447,141 @@ int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d,
         B2_CUDA(cudaMemcpyAsync(ystd + r0, sd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
         if (yhat != nullptr)
           B2_CUDA(cudaMemcpyAsync(yhat + r0, yd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
+        return B2_OK;
+      });
+  const cudaError_t done = cudaStreamSynchronize(ctx->stream);
+  if (rc != B2_OK) return rc;
+  B2_CUDA(done);
+  return B2_OK;
+}
+
+// ---- PoissonRegressor / GammaRegressor / TweedieRegressor (DESIGN.md section 10) --------------------------------------
+// The sums and operands (ctx->glm) and the per-CTA partials (ctx->glm_part), allocated by the first call and freed with
+// the context.
+static int ensure_glm(b2_ctx* ctx) {
+  if (ctx->glm != nullptr) return B2_OK;
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->glm), sizeof(double) * kGlmDoubles));
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->glm_part), sizeof(double) * 2 * (size_t)ctx->sm_count * kGlmPart));
+  return B2_OK;
+}
+
+// The checks the three entry points share, then the operands (w, step, b, db) into ctx->glm
+static int glm_setup(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, const void* X,
+                     const float* y, bool need_y, int link, double power, const double* coef, double intercept,
+                     const double* step, double step_intercept) {
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (link != B2_GLM_LOG && link != B2_GLM_IDENTITY) { set_error("link=%d must be B2_GLM_LOG or B2_GLM_IDENTITY", link); return B2_E_ARG; }
+  if (!isfinite(power)) { set_error("power=%g must be finite", power); return B2_E_ARG; }
+  if (link == B2_GLM_IDENTITY && power != 0.0) {
+    set_error("the identity link is supported at power 0 only (got power=%g)", power);
+    return B2_E_ARG;
+  }
+  if (coef == nullptr) { set_error("coef is null"); return B2_E_ARG; }
+  if (n_rows > 0 && (X == nullptr || (need_y && y == nullptr))) { set_error("X / y is null"); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) {
+    set_error("the GLM passes run on one rank only (their sums are not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (int r = ensure_glm(ctx)) return r;
+  std::vector<double> op(2 * kMaxD + 8, 0.0);
+  memcpy(op.data() + kGlmOpW, coef, sizeof(double) * d);
+  if (step != nullptr) memcpy(op.data() + kGlmOpStep, step, sizeof(double) * d);
+  op[kGlmOpMisc] = intercept;
+  op[kGlmOpMisc + 1] = step_intercept;
+  B2_CUDA(cudaMemcpyAsync(ctx->glm + kGlmOp, op.data(), sizeof(double) * op.size(), cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
+  return B2_OK;
+}
+
+// One pass over the rows into ctx->glm: device rows in one call of launch_glm, host rows block by block through the
+// staging ring (the first block overwrites the sums, the others add to them).
+static int glm_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                    int mem_kind, const uint8_t* row_mask, int mask_keep, int mode, int link, double power, int n_steps) {
+  if (mem_kind == B2_MEM_DEVICE)
+    return launch_glm(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, mode, link, power, n_steps, true);
+  if (n_rows == 0)
+    return launch_glm(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, mode, link, power, n_steps, true);
+  if (int r = ensure_staging(ctx)) return r;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = host_pointer_is_pinned(X);
+  return stream_host_blocks(
+      ctx, n_rows, ctx->stage_rows,
+      [&](int buf, int64_t r0, int64_t rows) {
+        return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
+      },
+      [&](int buf, int64_t r0, int64_t rows) {
+        return launch_glm(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
+                          row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, mode, link, power, n_steps,
+                          r0 == 0);
+      });
+}
+
+int b2_glm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, int link, double power, const double* coef,
+                double intercept, int fit_intercept, double* sums_out, double* hess_out) {
+  if (int r = use_device(ctx)) return r;
+  if (sums_out == nullptr) { set_error("sums_out is null"); return B2_E_ARG; }
+  if (int r = glm_setup(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, link, power, coef,
+                        fit_intercept ? intercept : 0.0, nullptr, 0.0))
+    return r;
+  const int mode = hess_out != nullptr ? kGlmHessian : kGlmGradient;
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, mode, link, power, 0)) return r;
+  const int d1 = d + 1;
+  std::vector<double> h(hess_out != nullptr ? (size_t)kGlmPart : (size_t)kGlmHess);
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->glm, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, h.data(), sizeof(double) * 7);
+  memcpy(sums_out + 7, h.data() + kGlmGrad, sizeof(double) * d1);
+  if (hess_out != nullptr)
+    for (int i = 0; i < d1; ++i)
+      for (int j = i; j < d1; ++j)       // the upper triangle, mirrored
+        hess_out[(size_t)i * d1 + j] = hess_out[(size_t)j * d1 + i] = h[kGlmHess + (size_t)i * kGlmHp + j];
+  return B2_OK;
+}
+
+int b2_glm_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                       int mem_kind, const uint8_t* row_mask, int mask_keep, int link, double power, const double* coef,
+                       double intercept, const double* step, double step_intercept, int n_steps, double* loss_out) {
+  if (int r = use_device(ctx)) return r;
+  if (step == nullptr || loss_out == nullptr) { set_error("step / loss_out is null"); return B2_E_ARG; }
+  if (n_steps < 1 || n_steps > kGlmSteps) { set_error("n_steps=%d out of range [1,%d]", n_steps, kGlmSteps); return B2_E_ARG; }
+  if (int r = glm_setup(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, link, power, coef, intercept, step,
+                        step_intercept))
+    return r;
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, kGlmLadder, link, power,
+                       n_steps))
+    return r;
+  B2_CUDA(cudaMemcpyAsync(loss_out, ctx->glm, sizeof(double) * n_steps, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+int b2_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, int link,
+                   const double* coef, double intercept, double* mu_out) {
+  if (int r = use_device(ctx)) return r;
+  if (mu_out == nullptr) { set_error("mu_out is null"); return B2_E_ARG; }
+  if (int r = glm_setup(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, nullptr, false, link, 0.0, coef, intercept, nullptr,
+                        0.0))
+    return r;
+  if (mem_kind == B2_MEM_DEVICE) {
+    if (int r = launch_glm_predict(ctx, X, x_dtype, n_rows, d, ldx, link, mu_out)) return r;
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    return B2_OK;
+  }
+  if (n_rows == 0) return B2_OK;
+  if (int r = ensure_staging(ctx)) return r;
+  if (int r = ensure_cv_stage(ctx, 1)) return r;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  const bool x_pinned = host_pointer_is_pinned(X);
+  const int rc = stream_host_blocks(
+      ctx, n_rows, ctx->stage_rows,
+      [&](int buf, int64_t r0, int64_t rows) {
+        return stage_rows_h2d(ctx, buf, X, es, nullptr, nullptr, r0, rows, d, ldx, x_pinned);
+      },
+      [&](int buf, int64_t r0, int64_t rows) -> int {
+        if (int r = launch_glm_predict(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, link, ctx->cv_stage[buf])) return r;
+        B2_CUDA(cudaMemcpyAsync(mu_out + r0, ctx->cv_stage[buf], sizeof(double) * rows, cudaMemcpyDeviceToHost,
+                                ctx->stream));
         return B2_OK;
       });
   const cudaError_t done = cudaStreamSynchronize(ctx->stream);

@@ -119,6 +119,22 @@ struct BayesArgs {
   double *out, *scores, *A;
 };
 
+// ---- the generalised linear regressors (glm.cu; DESIGN.md section 10) -------------------------------------------------
+// ctx->glm: the reduced sums [kGlmPart] of the last pass, then the operands at kGlmOp: w [kMaxD], the Newton step [kMaxD],
+// [b, db].  The sums: [0] loss [1] const [2] sum y [3] rows kept [4] y out of range [5] h <= 0 [6] y not finite, the
+// gradient sum g x_j at kGlmGrad + j (sum g at kGlmGrad + d), the Hessian sum |h| z_i z_j (z = [x 1]) at kGlmHess +
+// i kGlmHp + j, i <= j; a line search leaves the loss at step k in [k].  ctx->glm_part holds one kGlmPart per CTA, for
+// up to two CTAs per SM.
+constexpr int kGlmSteps = 21;            // sklearn's backtracking steps t = 1, 1/2, ..., 2^-20
+constexpr int kGlmGrad = 8;
+constexpr int kGlmHess = 144;
+constexpr int kGlmHp = 144;              // pitch of the Hessian: D + 1 columns padded to 16
+constexpr int kGlmPart = kGlmHess + kGlmHp * kGlmHp;
+constexpr int kGlmOp = kGlmPart;
+constexpr int kGlmOpW = 0, kGlmOpStep = kMaxD, kGlmOpMisc = 2 * kMaxD;
+constexpr int kGlmDoubles = kGlmOp + 2 * kMaxD + 8;
+enum GlmMode { kGlmGradient = 0, kGlmHessian = 1, kGlmLadder = 2 };   // what a pass computes
+
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
 // first and last row of every fold of fold ids in device memory: range[2 k] = n - first, range[2 k + 1] = last + 1
@@ -200,6 +216,10 @@ struct b2_ctx {
   int n_folds = 0;                     // folds held in `folds` (0: none)
   int folds_d = 0;                     // their d
   unsigned long long* fold_range = nullptr;   // [2 kMaxFolds]
+  // generalised linear regressors: the sums and operands of b2_glm_* (b2::kGlm*), per-CTA partials [2 sm_count][kGlmPart];
+  // allocated by the first call
+  double* glm = nullptr;
+  double* glm_part = nullptr;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -336,6 +356,12 @@ int launch_ard(b2_ctx* ctx, const BayesArgs& args);
 // ystd (and yhat when not null) of the rows [0, n): sqrt(max((x - m)^T sigma (x - m), 0) + noise_var) and x.w + b, from
 // the operands at ctx->enet (kStd* in score_std.cu, written by the caller)
 int launch_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* yhat, double* ystd);
+// one pass of the GLM regressors over the rows [0, n) at the operands of ctx->glm (mode: GlmMode; kGlmLadder takes the
+// n_steps losses), then the ordered reduce of the per-CTA sums into ctx->glm (`first_block` overwrites, otherwise adds)
+int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+               const uint8_t* mask, int keep, int mode, int link, double power, int n_steps, bool first_block);
+// mu of the rows [0, n): exp(x.w + b) (B2_GLM_LOG) or x.w + b, fp64
+int launch_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, int link, double* mu);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

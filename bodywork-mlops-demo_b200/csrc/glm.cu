@@ -1,0 +1,428 @@
+// glm.cu -- the row passes of the generalised linear regressors (b2_glm_pass, b2_glm_line_search, b2_glm_predict;
+// DESIGN.md section 10).
+//
+// scikit-learn's Newton solver (solver="newton-cholesky") needs, at the coefficients w, b of each iteration and with
+// eta = x.w + b per kept row, the half-Tweedie loss, its gradient g and Hessian h (loss(y, eta) and its derivatives in
+// eta, the Cython formulas of sklearn/_loss/_loss.pyx.tp branch by branch), and from them
+//   sum loss, sum g [x 1] (HBM-bound) and sum |h| [x 1][x 1]^T (2 (D + 1)^2 flops per row: fp64-compute bound).
+// One pass per call over 32-row tiles:
+//   (1) the tile -> shared memory as z = [x 1] in fp64 from the stored value (exact), zero for rows not kept;
+//   (2) eta (and, for the line search, deta = x.step + db) per row: the lanes of a warp over the features, a butterfly;
+//   (3) loss, g, h (or the loss at eta + t deta for t = 1, 1/2, ..., one step per lane) per kept row, by selects;
+//   (4) the gradient: thread j adds g_r z_rj over the tile's rows in order;
+//   (5) the Hessian on the fp64 tensor core (mma.sync m8n8k4 f64): A = the |h|-scaled rows, B = the rows, K = the 32 rows of
+//       the tile.  The (D + 1)^2 output is cut in 16 x 16 blocks; only blocks on or above the diagonal are computed, each
+//       warp holding up to six of them in registers for the whole launch (4 DMMAs per 2 + 2 fragment loads), the 8 x 8
+//       tile below the diagonal of a diagonal block skipped: 153 of the 289 8 x 8 tiles at D = 128.
+// The rows take scoring's plan (plan_rows): contiguous 16-byte aligned rows stream through the bulk-copy ring in whole
+// tiles, the rest (and every other layout) is read by the same consumers from global memory.  Each CTA writes its sums
+// in a fixed order, glm_reduce_kernel adds the CTAs in order: two calls return identical sums.
+#include "b2_internal.cuh"
+#include "b2_dmma.cuh"
+#include "b2_ptx.cuh"
+
+namespace b2 {
+namespace {
+
+constexpr int kGlmRows = 32;                       // rows per tile
+constexpr int kGlmWarps = 8;                       // consumer warps
+constexpr int kGlmConsumers = 32 * kGlmWarps;
+constexpr int kGlmThreads = kGlmConsumers + 32;    // + the producer warp of the ring
+constexpr int kGlmStages = 3;
+constexpr int kGlmBlocks = (kMaxD + 1 + 15) / 16;  // 9 blocks of 16 columns of [x 1]
+constexpr int kGlmSB = (kGlmBlocks * (kGlmBlocks + 1) / 2 + kGlmWarps - 1) / kGlmWarps;   // 16 x 16 blocks per warp: 6
+constexpr uint32_t kGlmXStage = kGlmRows * kMaxD * 4;                       // 16 KB: 32 fp32 rows of 128 features
+constexpr uint32_t kGlmYStage = kGlmRows * 4;
+constexpr uint32_t kGlmOffY = kGlmStages * kGlmXStage;
+constexpr uint32_t kGlmOffBar = kGlmOffY + kGlmStages * kGlmYStage;
+constexpr uint32_t kGlmRingBytes = kGlmOffBar + 2 * kGlmStages * 8 + 16;    // the doubles start here (16-byte aligned)
+
+__host__ __device__ inline int glm_dp(int d) { return (d + 1 + 15) & ~15; }   // columns of [x 1], padded to 16
+__host__ __device__ inline int glm_zpitch(int dp) { return dp + 4; }          // 4 mod 16 doubles: no bank conflicts
+size_t glm_smem_bytes(int dp, bool ring, int mode) {
+  const size_t tile = (size_t)kGlmRows * glm_zpitch(dp);
+  return (ring ? kGlmRingBytes : 0) +
+         sizeof(double) * (tile * (mode == kGlmHessian ? 2 : 1) + 3 * kMaxD + 8 + 3 * kGlmRows + 2 * kGlmWarps * 32 + 48);
+}
+
+__device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
+  asm volatile("bar.sync 1, %0;" ::"r"(kGlmConsumers) : "memory");
+}
+
+// The pointwise half-Tweedie loss, gradient and Hessian in eta, sklearn's Cython branches: the log link at any power
+// (0, 1 and 2 have their own), the identity link at power 0.
+__device__ __forceinline__ double glm_loss(int link, double p, double y, double eta) {
+  if (link == B2_GLM_IDENTITY) return 0.5 * (eta - y) * (eta - y);
+  if (p == 0.0) {
+    const double e1 = exp(eta);
+    return 0.5 * (e1 - y) * (e1 - y);
+  }
+  if (p == 1.0) return exp(eta) - y * eta;
+  if (p == 2.0) return eta + y * exp(-eta);
+  return exp((2.0 - p) * eta) / (2.0 - p) - y * exp((1.0 - p) * eta) / (1.0 - p);
+}
+
+__device__ __forceinline__ void glm_point(int link, double p, double y, double eta, double& loss, double& g,
+                                          double& h) {
+  if (link == B2_GLM_IDENTITY) {
+    g = eta - y;
+    loss = 0.5 * g * g;
+    h = 1.0;
+  } else if (p == 0.0) {
+    const double e1 = exp(eta);
+    loss = 0.5 * (e1 - y) * (e1 - y);
+    g = e1 * (e1 - y);
+    h = e1 * (2 * e1 - y);
+  } else if (p == 1.0) {
+    const double e = exp(eta);
+    loss = e - y * eta;
+    g = e - y;
+    h = e;
+  } else if (p == 2.0) {
+    const double e = exp(-eta);
+    loss = eta + y * e;
+    g = 1.0 - y * e;
+    h = e * y;
+  } else {
+    const double e1 = exp((1.0 - p) * eta), e2 = exp((2.0 - p) * eta);
+    loss = e2 / (2.0 - p) - y * e1 / (1.0 - p);
+    g = e2 - y * e1;
+    h = (2.0 - p) * e2 - (1.0 - p) * y * e1;
+  }
+}
+
+// constant_to_optimal_zero(y): the term the loss drops (0 for squared error)
+__device__ __forceinline__ double glm_const(int link, double p, double y) {
+  if (link == B2_GLM_IDENTITY || p == 0.0) return 0.0;
+  if (p == 1.0) return (y == 0.0 ? 0.0 : y * log(y)) - y;          // xlogy(y, y) - y
+  if (p == 2.0) return -log(y) - 1.0;
+  return pow(fmax(y, 0.0), 2.0 - p) / (1.0 - p) / (2.0 - p);
+}
+
+// y inside the loss's interval: (-inf, inf) for p <= 0, [0, inf) for 0 < p < 2, (0, inf) for p >= 2
+__device__ __forceinline__ bool glm_y_in_range(double p, double y) {
+  const bool low = p <= 0.0 ? y > -INFINITY : (p < 2.0 ? y >= 0.0 : y > 0.0);
+  return low && y < INFINITY;
+}
+
+// MODE kGlmGradient / kGlmHessian: per-CTA [loss, const, sum y, kept, y out of range, h <= 0, y not finite, 0 | g.x (d), sum g,
+// zeros | (kGlmHessian) the Hessian blocks at kGlmHess, pitch kGlmHp]; kGlmLadder: the loss at step k in [k], k < n_steps.
+// op: w [kMaxD], step [kMaxD], [b, db] (kGlmOp* in b2_internal.cuh).
+template <typename T, bool RING, int MODE>
+__global__ void __launch_bounds__(kGlmThreads, 1)
+glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
+           const uint8_t* __restrict__ mask, int keep, const double* __restrict__ op, int link, double power,
+           int n_steps, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const uint32_t sbase = smem_u32(smem_raw);
+  const uint32_t bar_full = sbase + kGlmOffBar, bar_empty = bar_full + 8 * kGlmStages;
+  const int dp = glm_dp(d), zp = glm_zpitch(dp), nb = dp / 16, nsb = nb * (nb + 1) / 2;
+  double* Zs = reinterpret_cast<double*>(smem_raw + (RING ? kGlmRingBytes : 0));   // [row][zp]: z = [x 1 0...]
+  double* HZs = Zs + (MODE == kGlmHessian ? kGlmRows * zp : 0);                    // |h| z
+  double* wv = HZs + kGlmRows * zp;        // [kMaxD] w
+  double* sv = wv + kMaxD;                 // [kMaxD] the Newton step (kGlmLadder)
+  double* yv = sv + kMaxD;                 // y (0 for rows not kept)
+  double* gs = yv + kGlmRows;              // g (0 for rows not kept)
+  double* hs = gs + kGlmRows;              // |h| (0 for rows not kept)
+  double* red = hs + kGlmRows;             // [warp][32] the warps' sums
+  double* lsum = red + kGlmWarps * 32;     // [warp][u][8] the scalar sums of the rows warp + 8 u (kGlmGradient / Hessian)
+  double* gsum = lsum + kGlmWarps * 32;    // [kMaxD + 8] the gradient sums, entry j of thread j
+  int* sbi = reinterpret_cast<int*>(gsum + kMaxD + 8);   // the 16 x 16 blocks on and above the diagonal
+  int* sbj = sbi + 48;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
+  for (int t = tid; t < kGlmWarps * 32; t += blockDim.x) lsum[t] = 0.0;
+  for (int t = tid; t < kMaxD + 8; t += blockDim.x) gsum[t] = 0.0;
+  for (int t = tid; t < kMaxD; t += blockDim.x) {
+    wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
+    sv[t] = (MODE == kGlmLadder && t < d) ? op[kGlmOpStep + t] : 0.0;
+  }
+  if (tid == 0) {
+    int k = 0;
+    for (int i = 0; i < nb; ++i)
+      for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
+  }
+  const double b = op[kGlmOpMisc], db = op[kGlmOpMisc + 1];
+  const int64_t n_tiles = (n + kGlmRows - 1) / kGlmRows;
+  if constexpr (RING) ring_init<kGlmStages>(bar_full, bar_empty, kGlmWarps);   // includes a block barrier
+  else __syncthreads();
+  // kGlmLadder: lane k sums the loss at step k.  The other sums stay in shared memory (lsum, gsum), which leaves the
+  // registers to the Hessian's accumulators.
+  double s_loss = 0.0;
+  double acc[kGlmSB][4][2];
+#pragma unroll
+  for (int u = 0; u < kGlmSB; ++u)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
+  if (RING && warp == kGlmWarps) {
+    if (lane == 0)
+      ring_produce<kGlmStages>(bar_full, bar_empty, (int)n_tiles, kGlmRows, X, (uint32_t)(d * sizeof(T)), sbase,
+                               kGlmXStage, true, y, sbase + kGlmOffY, kGlmYStage, false, nullptr, 0u, 0u);
+  } else {
+    int s = 0;
+    uint32_t phase = 0;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      const int64_t row0 = tile * kGlmRows;
+      bool use[kGlmRows / kGlmWarps];
+      // (1) the tile
+      if constexpr (RING) {
+#pragma unroll
+        for (int u = 0; u < kGlmRows / kGlmWarps; ++u)   // the mask comes from global memory, before the wait
+          use[u] = mask == nullptr || __ldg(mask + row0 + warp + kGlmWarps * u) == (uint8_t)keep;
+        mbar_wait(bar_full + 8 * s, phase);
+        const uint32_t xs = sbase + s * kGlmXStage, ys = sbase + kGlmOffY + s * kGlmYStage;
+#pragma unroll
+        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
+          const int r = warp + kGlmWarps * u;
+          const uint32_t xr = xs + (uint32_t)(r * d) * (uint32_t)sizeof(T);
+          for (int j = lane; j < dp; j += 32) {
+            const bool live = use[u] && j < d;
+            const float x = live ? raw_ld_shared<T>(xr + (uint32_t)j * (uint32_t)sizeof(T)) : 0.f;
+            Zs[r * zp + j] = live ? (double)x : (use[u] && j == d ? 1.0 : 0.0);
+          }
+          if (lane == 0) yv[r] = use[u] ? (double)ld_shared_f32(ys + 4u * (uint32_t)r) : 0.0;
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * s);      // the slot is converted: the producer may refill it
+        if (++s == kGlmStages) { s = 0; phase ^= 1u; }
+      } else {
+#pragma unroll
+        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
+          const int r = warp + kGlmWarps * u;
+          const int64_t row = row0 + r;
+          use[u] = row < n && (mask == nullptr || __ldg(mask + row) == (uint8_t)keep);
+          const T* xr = X + row * ldx;
+          for (int j = lane; j < dp; j += 32) {
+            const bool live = use[u] && j < d;
+            const float x = live ? ld_row_val<T>(xr + j) : 0.f;
+            Zs[r * zp + j] = live ? (double)x : (use[u] && j == d ? 1.0 : 0.0);
+          }
+          if (lane == 0) yv[r] = use[u] ? (double)__ldg(y + row) : 0.0;
+        }
+      }
+      __syncwarp();
+      // (2) eta (and deta) of the warp's rows: every lane ends with the same value
+      double eta[kGlmRows / kGlmWarps], deta[kGlmRows / kGlmWarps];
+#pragma unroll
+      for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
+        const double* zr = Zs + (warp + kGlmWarps * u) * zp;
+        double a = 0.0, c = 0.0;
+        for (int j = lane; j < d; j += 32) {
+          a = fma(zr[j], wv[j], a);
+          if constexpr (MODE == kGlmLadder) c = fma(zr[j], sv[j], c);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          a += __shfl_xor_sync(0xffffffffu, a, o);
+          if constexpr (MODE == kGlmLadder) c += __shfl_xor_sync(0xffffffffu, c, o);
+        }
+        eta[u] = a + b;
+        deta[u] = c + db;
+      }
+      // (3) the pointwise terms
+      if constexpr (MODE == kGlmLadder) {
+        const double t = ldexp(1.0, -lane);           // t = 1, 1/2, ... 2^-20: lane k < n_steps takes step k
+#pragma unroll
+        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
+          const double l = glm_loss(link, power, yv[warp + kGlmWarps * u], eta[u] + t * deta[u]);
+          s_loss += (use[u] && lane < n_steps) ? l : 0.0;
+        }
+      } else {
+        if (lane < kGlmRows / kGlmWarps) {            // lane u takes row warp + 8 u
+          double e = eta[0];
+          bool kept = use[0];
+#pragma unroll
+          for (int u = 1; u < kGlmRows / kGlmWarps; ++u) {
+            e = lane == u ? eta[u] : e;
+            kept = lane == u ? use[u] : kept;
+          }
+          const int r = warp + kGlmWarps * lane;
+          const double yy = yv[r];
+          double l, gg, hh;
+          glm_point(link, power, yy, e, l, gg, hh);
+          const double cst = glm_const(link, power, yy);
+          double* ls = lsum + (warp * 4 + lane) * 8;
+          ls[0] += kept ? l : 0.0;
+          ls[1] += kept ? cst : 0.0;
+          ls[2] += kept ? yy : 0.0;
+          ls[3] += kept ? 1.0 : 0.0;
+          ls[4] += (kept && !glm_y_in_range(power, yy)) ? 1.0 : 0.0;
+          ls[5] += (kept && hh <= 0.0) ? 1.0 : 0.0;
+          ls[6] += (kept && !isfinite(yy)) ? 1.0 : 0.0;
+          gs[r] = kept ? gg : 0.0;
+          hs[r] = kept ? fabs(hh) : 0.0;
+        }
+        consumer_sync();
+        // (4) the gradient, then (kGlmHessian) the |h|-scaled rows
+        if (tid <= d) {
+          double a = gsum[tid];
+#pragma unroll 8
+          for (int r = 0; r < kGlmRows; ++r) a = fma(gs[r], Zs[r * zp + tid], a);
+          gsum[tid] = a;
+        }
+        if constexpr (MODE == kGlmHessian) {
+          for (int t = tid; t < kGlmRows * dp; t += kGlmConsumers) {
+            const int r = t / dp, j = t - r * dp;
+            HZs[r * zp + j] = hs[r] * Zs[r * zp + j];
+          }
+          consumer_sync();
+          // (5) H += (|h| z)^T z over the tile's rows, the warp's blocks
+#pragma unroll
+          for (int u = 0; u < kGlmSB; ++u) {
+            const int sb = warp + kGlmWarps * u;
+            if (sb < nsb) {                               // warp-uniform
+              const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
+              const bool diag = sbi[sb] == sbj[sb];
+#pragma unroll
+              for (int ks = 0; ks < kGlmRows / 4; ++ks) {
+                const int r = 4 * ks + t4;
+                const double a0 = HZs[r * zp + ci], a1 = HZs[r * zp + ci + 8];
+                const double b0 = Zs[r * zp + cj], b1 = Zs[r * zp + cj + 8];
+                dmma(acc[u][0][0], acc[u][0][1], a0, b0);
+                dmma(acc[u][1][0], acc[u][1][1], a0, b1);
+                if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
+                dmma(acc[u][3][0], acc[u][3][1], a1, b1);
+              }
+            }
+          }
+        }
+      }
+      consumer_sync();
+    }
+  }
+  // the CTA's sums in a fixed order: the lanes of a warp, then the warps in order
+  double* out = part + (size_t)blockIdx.x * kGlmPart;
+  if constexpr (MODE == kGlmLadder) {
+    if (warp < kGlmWarps) red[warp * 32 + lane] = s_loss;
+    __syncthreads();
+    if (tid < 32) {
+      double v = 0.0;
+      for (int w = 0; w < kGlmWarps; ++w) v += red[w * 32 + tid];
+      out[tid] = v;
+    }
+  } else {
+    __syncthreads();
+    if (tid < kGlmHess) {                          // the scalars, the gradient, zeros in the unused entries
+      double r = 0.0;
+      if (tid < 7)
+        for (int q = 0; q < kGlmWarps * 4; ++q) r += lsum[q * 8 + tid];
+      else if (tid >= kGlmGrad && tid <= kGlmGrad + d)
+        r = gsum[tid - kGlmGrad];
+      out[tid] = r;
+    }
+    if constexpr (MODE == kGlmHessian) {
+#pragma unroll
+      for (int u = 0; u < kGlmSB; ++u) {
+        const int sb = warp + kGlmWarps * u;
+        if (warp < kGlmWarps && sb < nsb) {
+          const bool diag = sbi[sb] == sbj[sb];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (q == 2 && diag) continue;
+            const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
+            out[kGlmHess + i * kGlmHp + j] = acc[u][q][0];
+            out[kGlmHess + i * kGlmHp + j + 1] = acc[u][q][1];
+          }
+        }
+      }
+    }
+  }
+}
+
+// acc (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites.  The entries [0, n_lin), then with d1 > 0
+// the Hessian entries i <= j < d1.
+__global__ void glm_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, int n_lin, int d1,
+                                  double* __restrict__ acc) {
+  const int total = n_lin + d1 * d1;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
+    int off = e;
+    if (e >= n_lin) {
+      const int q = e - n_lin, i = q / d1, j = q - i * d1;
+      if (i > j) continue;
+      off = kGlmHess + i * kGlmHp + j;
+    }
+    double v = first ? 0.0 : acc[off];
+    for (int c = 0; c < n_ctas; ++c) v += part[(size_t)c * kGlmPart + off];
+    acc[off] = v;
+  }
+}
+
+// mu = exp(eta) (log link) or eta (identity) per row, eta = x.w + b in fp64: one warp per row
+template <typename T>
+__global__ void __launch_bounds__(256)
+glm_predict_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double* __restrict__ op, int link,
+                   double* __restrict__ mu) {
+  __shared__ double wv[kMaxD];
+  for (int t = threadIdx.x; t < kMaxD; t += blockDim.x) wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
+  __syncthreads();
+  const double b = op[kGlmOpMisc];
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < n; row += warps) {
+    const T* xr = X + row * ldx;
+    double a = 0.0;
+    for (int j = lane; j < d; j += 32) a = fma((double)ld_row_val<T>(xr + j), wv[j], a);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) mu[row] = link == B2_GLM_LOG ? exp(a + b) : a + b;
+  }
+}
+
+}  // namespace
+
+// The rows [0, n) in the launches of scoring's plan: whole 32-row tiles of what plan_rows streams through the ring go to the
+// ring flavour, the rest (or every row of another layout) to the direct one; each launch is followed by its ordered reduce
+// into ctx->glm (`first_block` overwrites, otherwise adds).
+int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+               const uint8_t* mask, int keep, int mode, int link, double power, int n_steps, bool first_block) {
+  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
+  const int64_t ring_rows = p.kind != RowPlan::kDirect ? (n / kGlmRows) * kGlmRows : 0;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  bool first = first_block;
+  for (int part = 0; part < 2; ++part) {
+    const bool ring = part == 0;
+    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
+    if (ring ? rows == 0 : (rows == 0 && !first)) continue;            // an empty call still writes the sums once
+    // two CTAs per SM hide the latency of the per-tile steps where the shared memory allows it (all but the Hessian)
+    const int64_t n_tiles = (rows + kGlmRows - 1) / kGlmRows, cap = (int64_t)ctx->sm_count * (mode == kGlmHessian ? 1 : 2);
+    int grid = (int)(n_tiles < cap ? n_tiles : cap);
+    if (grid < 1) grid = 1;
+    const char* Xt = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
+    const float* yt = y != nullptr ? y + r0 : nullptr;
+    const uint8_t* mt = mask != nullptr ? mask + r0 : nullptr;
+    const uint32_t smem = (uint32_t)glm_smem_bytes(glm_dp(d), ring, mode);
+    const int rc = with_rows(x_dtype, Xt, [&](auto* Xr) {
+      using T = row_t<decltype(Xr)>;
+      return with_int<kGlmGradient, kGlmHessian, kGlmLadder>(mode, [&](auto M) {
+        constexpr int MODE = decltype(M)::value;
+        auto kernel = ring ? glm_kernel<T, true, MODE> : glm_kernel<T, false, MODE>;
+        return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, rows, d, ldx, yt,
+                           mt, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
+                           ctx->glm_part);
+      });
+    });
+    if (rc != B2_OK) return rc;
+    const int n_lin = mode == kGlmLadder ? 32 : kGlmHess, d1 = mode == kGlmHessian ? d + 1 : 0;
+    glm_reduce_kernel<<<(n_lin + d1 * d1 + 255) / 256, 256, 0, ctx->stream>>>(ctx->glm_part, grid, first ? 1 : 0, n_lin,
+                                                                               d1, ctx->glm);
+    B2_CUDA(cudaGetLastError());
+    ctx->launches += 2;
+    first = false;
+  }
+  return B2_OK;
+}
+
+int launch_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, int link, double* mu) {
+  if (n == 0) return B2_OK;
+  int64_t want = (n + 7) / 8;
+  const int64_t cap = (int64_t)ctx->sm_count * 8;
+  const int grid = (int)(want < cap ? want : cap);
+  with_rows(x_dtype, X, [&](auto* Xr) {
+    glm_predict_kernel<<<grid, 256, 0, ctx->stream>>>(Xr, n, d, ldx, ctx->glm + kGlmOp, link, mu);
+    return B2_OK;
+  });
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+}  // namespace b2

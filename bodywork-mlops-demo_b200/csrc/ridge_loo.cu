@@ -15,6 +15,7 @@
 // A row not kept has v = 0 and e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA writes its sums per
 // alpha in a fixed order; loo_reduce_kernel adds the CTAs in order, so two calls return identical sums.
 #include "b2_internal.cuh"
+#include "b2_dmma.cuh"
 #include "b2_ptx.cuh"
 
 namespace b2 {
@@ -43,22 +44,6 @@ size_t loo_smem_bytes(int dp, bool ring) {
 
 __device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
   asm volatile("bar.sync 1, %0;" ::"r"(kLooConsumers) : "memory");
-}
-
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {
-  // fragments (PTX mma.m8n8k4.f64): A row = lane / 4, col = lane % 4; B row(k) = lane % 4, col(n) = lane / 4;
-  // C row = lane / 4, cols = 2 (lane % 4) + {0, 1}
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
-template <typename T>
-__device__ __forceinline__ float ld_row_val(const T* __restrict__ p);
-template <>
-__device__ __forceinline__ float ld_row_val<float>(const float* __restrict__ p) { return __ldg(p); }
-template <>
-__device__ __forceinline__ float ld_row_val<__nv_bfloat16>(const __nv_bfloat16* __restrict__ p) {
-  return __bfloat162float(*p);
 }
 
 // the B operands of (3): Cw[j][a] = c_j / (lambda_j + alpha_a), W[j][a] = 1 / (lambda_j + alpha_a); 0 outside d x n_alphas

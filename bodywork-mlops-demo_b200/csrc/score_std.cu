@@ -11,6 +11,7 @@
 // bulk-copy ring (ring_produce), the rows after the last whole tile and every other layout are read by the same consumers
 // from global memory.  Every sum runs in a fixed order, so repeated calls give identical results.
 #include "b2_internal.cuh"
+#include "b2_dmma.cuh"
 #include "b2_ptx.cuh"
 
 namespace b2 {
@@ -38,22 +39,6 @@ size_t std_smem_bytes(int dp, bool ring) {
 
 __device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
   asm volatile("bar.sync 1, %0;" ::"r"(kStdConsumers) : "memory");
-}
-
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {
-  // fragments (PTX mma.m8n8k4.f64): A row = lane / 4, col = lane % 4; B row(k) = lane % 4, col(n) = lane / 4;
-  // C row = lane / 4, cols = 2 (lane % 4) + {0, 1}
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
-template <typename T>
-__device__ __forceinline__ float ld_row_val(const T* __restrict__ p);
-template <>
-__device__ __forceinline__ float ld_row_val<float>(const float* __restrict__ p) { return __ldg(p); }
-template <>
-__device__ __forceinline__ float ld_row_val<__nv_bfloat16>(const __nv_bfloat16* __restrict__ p) {
-  return __bfloat162float(*p);
 }
 
 // RING: rows [0, n), n a multiple of kStdRows, contiguous (ldx == d) and 16-byte aligned, through the bulk-copy ring;

@@ -972,3 +972,336 @@ class B200ARDRegression(_B200Bayes):
 
     def __repr__(self) -> str:
         return "B200ARDRegression()"
+
+
+# ---- PoissonRegressor / GammaRegressor / TweedieRegressor: Newton fits on GPU passes (DESIGN.md section 10) ------------
+_NAN_MESSAGE = "Input X or y contains NaN, infinity or a value too large for dtype('float32')."
+
+
+class _B200GLM:
+    """What the three generalised linear regressors share: scikit-learn 1.9's ``_GeneralizedLinearRegressor.fit`` with
+    ``solver="newton-cholesky"``, its ``NewtonSolver.solve`` restated on the host around GPU passes over the rows.  Each
+    Newton iteration is one pass for the loss, gradient and fp64 Hessian (``glm_pass``) and one pass for all 21 candidate
+    steps of the backtracking line search (``glm_line_search``); the (D + 1)^2 Newton solve, the Armijo rule and the
+    convergence tests run on the host as scikit-learn runs them.  A singular Hessian, a Hessian with many non-positive
+    pointwise values, a step that is not a descent direction or a failed line search hand over to L-BFGS-B on GPU
+    loss-and-gradient passes, with scikit-learn's warnings.
+
+    The fit is the float64 fit of the stored fp32 / bf16 values: it matches scikit-learn run on float64 copies of those
+    values (scikit-learn computes float32 input in float32)."""
+    _sk_name = ""
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def _link_power(self):
+        """(link, power, the name of scikit-learn's loss class)"""
+        raise NotImplementedError
+
+    def _sk_params(self) -> dict:
+        return dict(alpha=self.alpha, fit_intercept=self.fit_intercept, solver=self.solver, max_iter=self.max_iter,
+                    tol=self.tol, warm_start=self.warm_start, verbose=self.verbose)
+
+    def _check_params(self):
+        if self.solver != "newton-cholesky":
+            raise ValueError(f"solver={self.solver!r} is not supported: B200{self._sk_name} runs scikit-learn's "
+                             "'newton-cholesky' solver (L-BFGS-B runs only as its fallback)")
+        if not (np.isfinite(self.alpha) and self.alpha >= 0):
+            raise ValueError(f"The 'alpha' parameter of {self._sk_name} must be a float in the range [0.0, inf). "
+                             f"Got {self.alpha!r} instead.")
+        if isinstance(self.max_iter, bool) or not isinstance(self.max_iter, (int, np.integer)) or self.max_iter < 1:
+            raise ValueError(f"The 'max_iter' parameter of {self._sk_name} must be an int in the range [1, inf). "
+                             f"Got {self.max_iter!r} instead.")
+        if not (np.isfinite(self.tol) and self.tol > 0):
+            raise ValueError(f"The 'tol' parameter of {self._sk_name} must be a float in the range (0.0, inf). "
+                             f"Got {self.tol!r} instead.")
+        return self._link_power()
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None):
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, n_iter_ and
+        n_features_in_."""
+        if sample_weight is not None:
+            raise ValueError(f"sample_weight is not supported by B200{self._sk_name}: every kept row has weight 1")
+        link, power, loss_name = self._check_params()
+        ctx = self.ctx
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        d = X.shape[1]
+        try:
+            coef, n_iter = self._newton(ctx, X, y, row_mask, mask_keep, d, link, power, loss_name)
+        finally:
+            for a in owned:
+                a.free()
+        if self.fit_intercept:
+            self.coef_, self.intercept_ = coef[:-1].copy(), np.float64(coef[-1])
+        else:
+            self.coef_, self.intercept_ = coef.copy(), 0.0
+        self.n_iter_ = int(n_iter)
+        self.n_features_in_ = int(d)
+        return self
+
+    def _newton(self, ctx, X, y, row_mask, mask_keep, d, link, power, loss_name):
+        """NewtonSolver.solve (NewtonCholeskySolver) step by step; returns (coef with the intercept last, n_iter)."""
+        import scipy.linalg
+        import scipy.optimize
+        from sklearn.exceptions import ConvergenceWarning
+        from sklearn.utils.optimize import _check_optimize_result
+        fi, alpha, tol, max_iter = bool(self.fit_intercept), float(self.alpha), float(self.tol), int(self.max_iter)
+        n_dof = d + int(fi)
+
+        def run(c, hessian):
+            return ctx.glm_pass(X, y, c[:d], float(c[d]) if fi else 0.0, link=link, power=power, row_mask=row_mask,
+                                mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
+
+        def loss_of(c, loss_sum):                 # LinearModelLoss.loss: mean loss + alpha / 2 |w|^2
+            w = c[:d]
+            return float(loss_sum / n) + float(0.5 * alpha * (w @ w))
+
+        def grad_of(c, s):                        # LinearModelLoss.gradient
+            g = np.empty(n_dof)
+            g[:d] = s["grad"][:d] / n + alpha * c[:d]
+            if fi:
+                g[d] = s["grad"][d] / n
+            return g
+
+        warm = bool(self.warm_start) and getattr(self, "coef_", None) is not None
+        if warm:
+            coef = np.asarray(self.coef_, dtype=np.float64).ravel().copy()
+            if coef.size != d:
+                raise ValueError(f"X has {d} features, but the warm start coef_ has {coef.size}")
+            if fi:
+                coef = np.concatenate([coef, [float(self.intercept_)]])
+        else:
+            coef = np.zeros(n_dof)
+        first = run(coef, warm)
+        n = first["kept"]
+        if n == 0:
+            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
+                             f"B200{self._sk_name}.")
+        if first["y_nonfinite"] > 0 or not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
+            raise ValueError(_NAN_MESSAGE)
+        if first["y_out_of_range"] > 0:
+            raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
+        if warm:
+            cur = first
+        else:
+            if fi:
+                ybar = first["sum_y"] / n
+                coef[-1] = np.log(ybar) if link == native.GLM_LOG else ybar
+            cur = run(coef, True)
+        loss_value = loss_of(coef, cur["loss"])
+
+        beta, sigma = 0.5, 0.00048828125
+        eps = 16 * np.finfo(np.float64).eps
+        iteration, converged, fallback = 1, False, False
+        while iteration <= max_iter and not converged:
+            fallback = False
+            gradient = grad_of(coef, cur)
+            # inner_solve
+            if cur["h_nonpos"] / n > 0.25:
+                warnings.warn(f"The inner solver of NewtonCholeskySolver detected a pointwise hessian with many negative "
+                              f"values at iteration #{iteration}. It will now resort to lbfgs instead.",
+                              ConvergenceWarning, stacklevel=3)
+                fallback = True
+                break
+            hessian = cur["hessian"] / n
+            if not fi:
+                hessian = hessian[:d, :d].copy()
+            hessian[np.arange(d), np.arange(d)] += alpha
+            try:
+                with warnings.catch_warnings():
+                    warnings.simplefilter("error", scipy.linalg.LinAlgWarning)
+                    coef_newton = scipy.linalg.solve(hessian, -gradient, check_finite=False, assume_a="sym")
+                    gradient_times_newton = gradient @ coef_newton
+                    if gradient_times_newton > 0:
+                        fallback = True
+                        break
+            except (np.linalg.LinAlgError, scipy.linalg.LinAlgWarning) as e:
+                warnings.warn("The inner solver of NewtonCholeskySolver stumbled upon a singular or very ill-conditioned "
+                              f"Hessian matrix at iteration {iteration}. It will now resort to lbfgs instead.\n"
+                              "Further options are to use another solver or to avoid such situation in the first place. "
+                              "Possible remedies are removing collinear features of X or increasing the penalization "
+                              "strengths.\nThe original Linear Algebra message was:\n" + str(e),
+                              scipy.linalg.LinAlgWarning, stacklevel=3)
+                fallback = True
+                break
+            # line search: every candidate step from one pass
+            ladder = ctx.glm_line_search(X, y, coef[:d], float(coef[d]) if fi else 0.0, coef_newton[:d],
+                                         float(coef_newton[d]) if fi else 0.0, link=link, power=power,
+                                         n_steps=native.GLM_STEPS, row_mask=row_mask, mask_keep=mask_keep)
+            armijo_term = sigma * gradient_times_newton
+            coef_old, loss_value_old, gradient_old = coef, loss_value, gradient
+            sum_abs_grad_old = -1
+            t = 1
+            for i in range(native.GLM_STEPS):
+                coef = coef_old + t * coef_newton
+                loss_value = loss_of(coef, ladder[i])
+                loss_improvement = loss_value - loss_value_old
+                if loss_improvement <= t * armijo_term:
+                    break
+                if np.abs(loss_improvement) <= np.abs(loss_value_old * eps):
+                    if sum_abs_grad_old < 0:
+                        sum_abs_grad_old = scipy.linalg.norm(gradient_old, ord=1)
+                    if scipy.linalg.norm(grad_of(coef, run(coef, False)), ord=1) < sum_abs_grad_old:
+                        break
+                t *= beta
+            else:
+                warnings.warn(f"Line search of Newton solver NewtonCholeskySolver at iteration #{iteration} did not "
+                              "converge after 21 line search refinement iterations. It will now resort to lbfgs "
+                              "instead.", ConvergenceWarning, stacklevel=3)
+                fallback = True
+                break
+            # convergence: the gradient at the new coefficients comes with the next iteration's Hessian
+            cur = run(coef, iteration < max_iter)
+            if np.max(np.abs(grad_of(coef, cur))) <= tol:
+                if 0.5 * (coef_newton @ hessian @ coef_newton) <= tol:
+                    converged = True
+            iteration += 1
+
+        if not converged:
+            if fallback:
+                def fun(c):
+                    s = run(c, False)
+                    return loss_of(c, s["loss"]), grad_of(c, s)
+                maxiter = max_iter - iteration
+                opt_res = scipy.optimize.minimize(fun, coef, method="L-BFGS-B", jac=True,
+                                                  options={"maxiter": maxiter, "maxls": 50, "gtol": tol,
+                                                           "ftol": 64 * np.finfo(np.float64).eps})
+                iteration += _check_optimize_result("lbfgs", opt_res, max_iter=maxiter)
+                coef = opt_res.x
+            else:
+                warnings.warn(f"Newton solver did not converge after {iteration - 1} iterations.", ConvergenceWarning,
+                              stacklevel=3)
+        return coef, iteration - 1
+
+    def _staged(self, X):
+        on_device = isinstance(X, native.DeviceArray)
+        Xh = X if on_device else _as_f32_matrix(X)
+        if Xh.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        return Xh
+
+    def predict(self, X):
+        """mu = exp(X coef_ + intercept_) (log link) or X coef_ + intercept_ in fp64: float64 for host rows, an f64
+        ``DeviceArray`` for device rows."""
+        link = self._link_power()[0]
+        return self.ctx.glm_predict(self._staged(X), self.coef_, float(self.intercept_), link=link)
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """D^2, the fraction of deviance explained (scikit-learn's ``score``): one pass at the model and one at the
+        intercept-only model link(mean y), both over the kept rows."""
+        link, power, loss_name = self._link_power()
+        ctx = self.ctx
+        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
+        if X.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {X.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        d = X.shape[1]
+        try:
+            kw = dict(link=link, power=power, row_mask=row_mask, mask_keep=mask_keep, hessian=False)
+            model = ctx.glm_pass(X, y, self.coef_, float(self.intercept_), **kw)
+            n = model["kept"]
+            if n == 0:
+                raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required.")
+            if model["y_nonfinite"] > 0:
+                raise ValueError(_NAN_MESSAGE)
+            if model["y_out_of_range"] > 0:
+                raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
+            ybar = model["sum_y"] / n
+            y_mean = np.log(ybar) if link == native.GLM_LOG else ybar
+            null = ctx.glm_pass(X, y, np.zeros(d), float(y_mean), **kw)
+        finally:
+            for a in owned:
+                a.free()
+        constant = model["const"] / n
+        deviance, deviance_null = model["loss"] / n, null["loss"] / n
+        return float(1 - (deviance + constant) / (deviance_null + constant))
+
+    def to_sklearn(self):
+        """A real scikit-learn estimator with the attributes ``fit`` would have set (joblib-dumpable); ``_base_loss`` is
+        set as scikit-learn's fit sets it, because its ``predict`` and ``score`` read it."""
+        from sklearn import linear_model
+        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
+        reg.intercept_ = self.intercept_
+        reg.n_iter_ = int(self.n_iter_)
+        reg.n_features_in_ = int(self.n_features_in_)
+        reg._base_loss = reg._get_loss()
+        return reg
+
+    def __repr__(self) -> str:
+        return f"B200{self._sk_name}(alpha={self.alpha})"
+
+
+class B200PoissonRegressor(_B200GLM):
+    """``sklearn.linear_model.PoissonRegressor(solver="newton-cholesky")`` fitted on the H100: HalfPoissonLoss with the
+    log link.  verbose is accepted and has no effect."""
+    _sk_name = "PoissonRegressor"
+
+    def __init__(self, *, alpha: float = 1.0, fit_intercept: bool = True, solver: str = "newton-cholesky",
+                 max_iter: int = 100, tol: float = 1e-4, warm_start: bool = False, verbose: int = 0,
+                 ctx: Optional[native.Context] = None):
+        self.alpha = alpha
+        self.fit_intercept = fit_intercept
+        self.solver = solver
+        self.max_iter = max_iter
+        self.tol = tol
+        self.warm_start = warm_start
+        self.verbose = verbose
+        self._ctx = ctx
+
+    def _link_power(self):
+        return native.GLM_LOG, 1.0, "HalfPoissonLoss"
+
+
+class B200GammaRegressor(B200PoissonRegressor):
+    """``sklearn.linear_model.GammaRegressor(solver="newton-cholesky")`` fitted on the H100: HalfGammaLoss with the log
+    link.  verbose is accepted and has no effect."""
+    _sk_name = "GammaRegressor"
+
+    def _link_power(self):
+        return native.GLM_LOG, 2.0, "HalfGammaLoss"
+
+
+class B200TweedieRegressor(_B200GLM):
+    """``sklearn.linear_model.TweedieRegressor(power, link, solver="newton-cholesky")`` fitted on the H100:
+    HalfTweedieLoss (log link) at any power, HalfTweedieLossIdentity (identity link, the default for power <= 0) at power
+    0 only.  verbose is accepted and has no effect."""
+    _sk_name = "TweedieRegressor"
+
+    def __init__(self, *, power: float = 0.0, alpha: float = 1.0, fit_intercept: bool = True, link: str = "auto",
+                 solver: str = "newton-cholesky", max_iter: int = 100, tol: float = 1e-4, warm_start: bool = False,
+                 verbose: int = 0, ctx: Optional[native.Context] = None):
+        self.power = power
+        self.alpha = alpha
+        self.fit_intercept = fit_intercept
+        self.link = link
+        self.solver = solver
+        self.max_iter = max_iter
+        self.tol = tol
+        self.warm_start = warm_start
+        self.verbose = verbose
+        self._ctx = ctx
+
+    def _link_power(self):
+        power = float(self.power)
+        if not np.isfinite(power):
+            raise ValueError(f"The 'power' parameter of TweedieRegressor must be a finite float. Got {self.power!r}.")
+        if self.link not in ("auto", "identity", "log"):
+            raise ValueError(f"The 'link' parameter of TweedieRegressor must be a str among {{'auto', 'identity', "
+                             f"'log'}}. Got {self.link!r} instead.")
+        identity = self.link == "identity" or (self.link == "auto" and power <= 0)
+        if identity and power != 0.0:
+            raise ValueError(f"link='identity' (or link='auto' with power <= 0) is supported at power 0 only, got "
+                             f"power={self.power!r}")
+        if identity:
+            return native.GLM_IDENTITY, 0.0, "HalfTweedieLossIdentity"
+        return native.GLM_LOG, power, "HalfTweedieLoss"
+
+    def _sk_params(self) -> dict:
+        return dict(power=self.power, link=self.link, **super()._sk_params())
+
+    def __repr__(self) -> str:
+        return f"B200TweedieRegressor(power={self.power}, alpha={self.alpha}, link={self.link!r})"

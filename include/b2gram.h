@@ -296,6 +296,32 @@ int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d,
                  const double* mean, const double* sigma, double noise_var, const double* coef, double intercept,
                  double* yhat, double* ystd);
 
+/* ---- PoissonRegressor / GammaRegressor / TweedieRegressor (DESIGN.md section 10) --------------------------------
+ * The row passes of scikit-learn's Newton solver (solver="newton-cholesky") for the half-Tweedie losses, with constants
+ * dropped as sklearn drops them: per kept row eta = x.coef + intercept in fp64 from the stored value, then
+ * sklearn's pointwise loss(y, eta), gradient g and Hessian h in eta.  Sums over the kept rows are unscaled (no 1 / n, no
+ * penalty) and bit-identical between calls.  y: fp32 where X lives; row_mask / mask_keep as b2_score.
+ * fit_intercept = 0 takes the intercept as 0.  B2_E_ARG: bad shapes, link not one of the two below, power not finite,
+ * B2_GLM_IDENTITY with power != 0, null coef or outputs; B2_E_UNSUPPORTED with more than one rank. */
+#define B2_GLM_LOG 0       /* mu = exp(eta), HalfTweedieLoss(power); power 1 is HalfPoissonLoss, 2 HalfGammaLoss */
+#define B2_GLM_IDENTITY 1  /* mu = eta, HalfTweedieLossIdentity, power 0 only (squared error) */
+/* b2_glm_pass: one pass at (coef, intercept).  sums_out (host, d + 8 doubles): [0] sum loss [1] sum
+ * constant_to_optimal_zero(y) [2] sum y [3] rows kept [4] rows with y outside the loss's interval (NaN included) [5] rows
+ * with h <= 0 [6] rows with y not finite, [7, 7 + d) sum g x_j, [7 + d] sum g.  hess_out NULL (the pass skips the
+ * Hessian) or (d+1) x (d+1) host doubles: sum |h| z z^T with z = [x 1], on the fp64 tensor core. */
+int b2_glm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, int link, double power, const double* coef,
+                double intercept, int fit_intercept, double* sums_out, double* hess_out);
+/* b2_glm_line_search: the backtracking ladder of one Newton step in one pass: loss_out[k] = sum over kept rows of
+ * loss(y, eta + 2^-k (x.step + step_intercept)) for k < n_steps (1..21; sklearn tries t = 1, 1/2, ..., 2^-20). */
+int b2_glm_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                       int mem_kind, const uint8_t* row_mask, int mask_keep, int link, double power, const double* coef,
+                       double intercept, const double* step, double step_intercept, int n_steps, double* loss_out);
+/* b2_glm_predict: mu_out[i] = exp(eta_i) (B2_GLM_LOG) or eta_i, n_rows fp64 where X lives (mem_kind); host rows use two
+ * device staging blocks of 262 144 doubles in the context. */
+int b2_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, int link,
+                   const double* coef, double intercept, double* mu_out);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
