@@ -282,21 +282,85 @@ int stream_host_blocks(b2_ctx* ctx, int64_t n_rows, int64_t blk_rows, Stage stag
   return B2_OK;
 }
 
-// host rows of b2_gram_accumulate / b2_fit, one staged block at a time through the Gram dispatch
-int gram_host_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
-                   const uint8_t* mask, int keep) {
+// The row-output blocks grown to row_bytes per row (their contents are not kept)
+int ensure_row_out(b2_ctx* ctx, size_t row_bytes) {
+  if (ctx->row_out_bytes >= row_bytes) return B2_OK;
+  if (ctx->row_out[0] != nullptr) B2_CUDA(cudaStreamSynchronize(ctx->stream));   // an earlier call's copies may still read them
+  for (int b = 0; b < 2; ++b) {
+    if (ctx->row_out[b] != nullptr) cudaFree(ctx->row_out[b]);
+    ctx->row_out[b] = nullptr;
+  }
+  ctx->row_out_bytes = 0;
+  for (int b = 0; b < 2; ++b)
+    if (cudaMalloc(reinterpret_cast<void**>(&ctx->row_out[b]), (size_t)ctx->stage_rows * row_bytes) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("out of device memory for the staging blocks of the per-row outputs");
+      return B2_E_CUDA;
+    }
+  ctx->row_out_bytes = row_bytes;
+  return B2_OK;
+}
+
+// A per-row output of a row pass: the caller's destination (device memory for device rows, host memory for host rows,
+// null: not wanted) and its bytes per row.
+struct RowOut {
+  void* dst = nullptr;
+  size_t row_bytes = 0;
+};
+
+// One pass over the rows [0, n_rows) of a call, wherever they live: launch(span, out0, out1) enqueues the pass over the
+// rows of `span` and writes the per-row outputs to out0 / out1 (null when not wanted).
+// Device rows: one launch on the caller's pointers.  Host rows: one launch per block of the staging ring, its outputs
+// written to the row-output blocks and copied back behind it; with outputs, the stream is synchronised before the
+// return, so the caller may reuse every host buffer -- also when a block failed.  Zero rows: one launch on zero rows.
+template <typename Launch>
+int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+             const uint8_t* mask, Launch&& launch, RowOut out0 = {}, RowOut out1 = {}) {
+  if (mem_kind == B2_MEM_DEVICE) return launch(RowSpan{X, y, mask, ldx, 0, n_rows, true}, out0.dst, out1.dst);
+  if (n_rows == 0) return launch(RowSpan{nullptr, nullptr, nullptr, d, 0, 0, true}, nullptr, nullptr);
   if (int r = ensure_staging(ctx)) return r;
+  RowOut out[2] = {out0, out1};
+  size_t out_bytes = 0;
+  for (RowOut& o : out) {
+    if (o.dst == nullptr) o.row_bytes = 0;
+    out_bytes += o.row_bytes;
+  }
+  if (out_bytes > 0)
+    if (int r = ensure_row_out(ctx, out_bytes)) return r;
   const int es = x_dtype == B2_F32 ? 4 : 2;
   const bool x_pinned = host_pointer_is_pinned(X);
-  return stream_host_blocks(
+  const int rc = stream_host_blocks(
       ctx, n_rows, ctx->stage_rows,
       [&](int buf, int64_t r0, int64_t rows) {
         return stage_rows_h2d(ctx, buf, X, es, y, mask, r0, rows, d, ldx, x_pinned);
       },
-      [&](int buf, int64_t, int64_t rows) {
-        return gram_dispatch(ctx, ctx->stage_x[buf], x_dtype, ctx->stage_y[buf], rows, d, d,
-                             mask != nullptr ? ctx->stage_m[buf] : nullptr, keep);
+      [&](int buf, int64_t r0, int64_t rows) -> int {
+        char* const block = ctx->row_out[buf];   // [stage_rows] of output 0, then [stage_rows] of output 1
+        char* dev[2] = {out[0].dst != nullptr ? block : nullptr,
+                        out[1].dst != nullptr ? block + (size_t)ctx->stage_rows * out[0].row_bytes : nullptr};
+        const RowSpan s{ctx->stage_x[buf], y != nullptr ? ctx->stage_y[buf] : nullptr,
+                        mask != nullptr ? ctx->stage_m[buf] : nullptr, d, r0, rows, r0 == 0};
+        if (int r = launch(s, dev[0], dev[1])) return r;
+        for (int k = 0; k < 2; ++k)
+          if (out[k].dst != nullptr)
+            B2_CUDA(cudaMemcpyAsync(static_cast<char*>(out[k].dst) + (size_t)r0 * out[k].row_bytes, dev[k],
+                                    (size_t)rows * out[k].row_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        return B2_OK;
       });
+  if (out_bytes == 0) return rc;
+  const cudaError_t done = cudaStreamSynchronize(ctx->stream);   // the outputs' copies into the caller's buffers
+  if (rc != B2_OK) return rc;
+  B2_CUDA(done);
+  return B2_OK;
+}
+
+// The rows of a call into S through the Gram dispatch (b2_fit's device rows call gram_dispatch themselves, for the
+// fused exchange)
+int gram_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+              const uint8_t* mask, int keep) {
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, mask, [&](const RowSpan& s, void*, void*) {
+    return gram_dispatch(ctx, s.X, x_dtype, s.y, s.rows, d, s.ldx, s.mask, keep);
+  });
 }
 
 // honours a lazy b2_gram_reset where S is read before any kernel wrote it (exchange, export, solves after zero rows)
@@ -410,9 +474,8 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   if (ctx->xchg != nullptr) cudaFree(ctx->xchg);
   void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
-                  ctx->stage_m[0], ctx->stage_m[1], ctx->yhat_stage[0], ctx->yhat_stage[1], ctx->tc_sync, ctx->synth_count,
-                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->cv_stage[0], ctx->cv_stage[1],
-                  ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part};
+                  ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
+                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -607,8 +670,7 @@ int b2_gram_accumulate(b2_ctx* ctx, const void* X, int x_dtype, const float* y, 
   if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
   if (d != ctx->d) { set_error("d=%d differs from the statistic's d=%d", d, ctx->d); return B2_E_ARG; }
   if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
-  if (mem_kind == B2_MEM_DEVICE) return gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep);
-  return gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep);
+  return gram_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep);
 }
 
 // The peer-memory exchange reports a peer that did not deliver within the timeout through a status word in the
@@ -770,7 +832,7 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
     if (int r = gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep, &tc_last, &gather_epoch))
       return r;
     if (tc_last) ctx->fused_fits += 1;
-  } else if (int r = gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) {
+  } else if (int r = gram_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) {
     return r;
   }
   if (gather_epoch == 0) {
@@ -784,21 +846,32 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
 // g_j, g_1 and sum e^2 to ctx->refine + kRfGrad; host rows re-stream through the staging ring.
 static int grad_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                      int mem_kind, const uint8_t* row_mask, int mask_keep) {
-  if (mem_kind == B2_MEM_DEVICE) return launch_grad(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, true);
-  if (int r = ensure_staging(ctx)) return r;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = host_pointer_is_pinned(X);
-  if (int r = stream_host_blocks(
-          ctx, n_rows, ctx->stage_rows,
-          [&](int buf, int64_t r0, int64_t rows) {
-            return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-          },
-          [&](int buf, int64_t r0, int64_t rows) {
-            return launch_grad(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
-                               row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, r0 == 0);
-          }))
-    return r;
-  if (n_rows == 0) return launch_grad(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, true);
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*) {
+    return launch_grad(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, s.first);
+  });
+}
+
+// The model b0' + (x - m).beta of the residual passes into ctx->refine, with beta = coef and m the column means of the
+// resident S (0 without an intercept), also as the state before the last correction (step +inf).  intercept null: b0'
+// is S's mean label (0 without an intercept), the state of the fit of S; otherwise b0' = *intercept + m.beta, the model
+// *intercept + x.beta.  The upload is from pageable memory, so it has read the state when this returns.
+static int load_refine_state(b2_ctx* ctx, int d, const double* coef, int fit_intercept, const double* intercept) {
+  if (int r = ensure_s_cleared(ctx)) return r;
+  const int dp = d + 2;
+  std::vector<double> S((size_t)dp * dp), st(kRfDoubles, 0.0);
+  B2_CUDA(cudaMemcpyAsync(S.data(), ctx->S, sizeof(double) * dp * dp, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const double n = S[(size_t)d * dp + d];
+  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
+  double b0 = intercept != nullptr ? *intercept : (fit_intercept ? S[(size_t)d * dp + d + 1] * inv_n : 0.0);
+  for (int j = 0; j < d; ++j) {
+    st[kRfBeta + j] = st[kRfPrevBeta + j] = coef[j];
+    st[kRfMean + j] = fit_intercept ? S[(size_t)j * dp + d] * inv_n : 0.0;
+    if (intercept != nullptr) b0 += st[kRfMean + j] * coef[j];
+  }
+  st[kRfB0] = st[kRfPrevB0] = b0;
+  st[kRfStep] = INFINITY;
+  B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
   return B2_OK;
 }
 
@@ -825,20 +898,7 @@ int b2_fit_refined(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
     return r;
   if (max_passes == 0) return B2_OK;
   // the state: beta from the fit; m and b0' from S as the solve forms them
-  const int dp = d + 2;
-  std::vector<double> S((size_t)dp * dp), st(kRfDoubles, 0.0);
-  B2_CUDA(cudaMemcpyAsync(S.data(), ctx->S, sizeof(double) * dp * dp, cudaMemcpyDeviceToHost, ctx->stream));
-  B2_CUDA(cudaStreamSynchronize(ctx->stream));
-  const double n = S[(size_t)d * dp + d];
-  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
-  for (int j = 0; j < d; ++j) {
-    st[kRfBeta + j] = coef[j];
-    st[kRfPrevBeta + j] = coef[j];
-    st[kRfMean + j] = fit_intercept ? S[(size_t)j * dp + d] * inv_n : 0.0;
-  }
-  st[kRfB0] = st[kRfPrevB0] = fit_intercept ? S[(size_t)d * dp + d + 1] * inv_n : 0.0;
-  st[kRfStep] = INFINITY;
-  B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
+  if (int r = load_refine_state(ctx, d, coef, fit_intercept, nullptr)) return r;
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   const double* h = ctx->solve_host;
   int kept = 0;
@@ -1046,10 +1106,7 @@ int b2_gram_folds(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64
     const int64_t r0 = first[k] & ~(int64_t)15, rows = last[k] + 1 - r0;
     const void* Xk = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
     ctx->s_zero_pending = true;
-    const int rc = mem_kind == B2_MEM_DEVICE
-                       ? gram_dispatch(ctx, Xk, x_dtype, y + r0, rows, d, ldx, fold_of_row + r0, k)
-                       : gram_host_rows(ctx, Xk, x_dtype, y + r0, rows, d, ldx, fold_of_row + r0, k);
-    if (rc != B2_OK) return rc;
+    if (int r = gram_rows(ctx, Xk, x_dtype, y + r0, rows, d, ldx, mem_kind, fold_of_row + r0, k)) return r;
     B2_CUDA(cudaMemcpyAsync(ctx->folds + k * count, ctx->S, sizeof(double) * count, cudaMemcpyDeviceToDevice,
                             ctx->stream));
   }
@@ -1144,27 +1201,6 @@ int b2_solve_enet_cv(b2_ctx* ctx, const double* fold_S, int n_folds, int fit_int
   return B2_OK;
 }
 
-// The device output blocks of host rows (b2_ridge_loo's e^2, b2_score_std's ystd and yhat): two blocks of stage_rows x
-// per_row doubles, grown to the widest call so far and freed with the context.
-static int ensure_cv_stage(b2_ctx* ctx, int per_row) {
-  if (ctx->cv_stage_alphas >= per_row) return B2_OK;
-  B2_CUDA(cudaStreamSynchronize(ctx->stream));                 // an earlier call's copies may still read them
-  for (int b = 0; b < 2; ++b) {
-    if (ctx->cv_stage[b] != nullptr) cudaFree(ctx->cv_stage[b]);
-    ctx->cv_stage[b] = nullptr;
-  }
-  ctx->cv_stage_alphas = 0;
-  for (int b = 0; b < 2; ++b)
-    if (cudaMalloc(reinterpret_cast<void**>(&ctx->cv_stage[b]), sizeof(double) * ctx->stage_rows * per_row) !=
-        cudaSuccess) {
-      cudaGetLastError();
-      set_error("out of device memory for the staging blocks of the per-row outputs");
-      return B2_E_CUDA;
-    }
-  ctx->cv_stage_alphas = per_row;
-  return B2_OK;
-}
-
 // The Gram of b2_fit, the eigendecomposition of its centred Gram, one leave-one-out pass over the same rows (host rows
 // re-stream through the staging ring, their e^2 through a device block per row block), then the LDL^T solve of b2_fit
 // at the chosen alpha from the same S.
@@ -1192,11 +1228,7 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
     return B2_E_UNSUPPORTED;
   }
   if (int r = b2_gram_reset(ctx, d)) return r;
-  if (mem_kind == B2_MEM_DEVICE) {
-    if (int r = gram_dispatch(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) return r;
-  } else if (int r = gram_host_rows(ctx, X, x_dtype, y, n_rows, d, ldx, row_mask, mask_keep)) {
-    return r;
-  }
+  if (int r = gram_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
   if (int r = ensure_s_cleared(ctx)) return r;
   if (int r = launch_solve_eigh(ctx, fit_intercept)) return r;
   B2_CUDA(cudaMemcpyAsync(ctx->loo + kLooAlpha, alphas, sizeof(double) * n_alphas, cudaMemcpyHostToDevice, ctx->stream));
@@ -1206,30 +1238,14 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
   const double n_kept = misc[1];
   if (!(n_kept > 0.0)) { set_error("no row kept: the leave-one-out error needs at least one row"); return B2_E_ARG; }
   if (int r = eigh_converged(misc[3])) return r;
-  if (mem_kind == B2_MEM_DEVICE) {
-    if (int r = launch_loo(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, n_alphas, cv_out, true)) return r;
-  } else {
-    const int es = x_dtype == B2_F32 ? 4 : 2;
-    const bool x_pinned = host_pointer_is_pinned(X);
-    if (cv_out != nullptr)
-      if (int r = ensure_cv_stage(ctx, n_alphas)) return r;
-    const int rc = stream_host_blocks(
-        ctx, n_rows, ctx->stage_rows,
-        [&](int buf, int64_t r0, int64_t rows) {
-          return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-        },
-        [&](int buf, int64_t r0, int64_t rows) -> int {
-          double* cv_dev = cv_out != nullptr ? ctx->cv_stage[buf] : nullptr;
-          if (int r = launch_loo(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
-                                 row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, n_alphas, cv_dev, r0 == 0))
-            return r;
-          if (cv_out != nullptr)
-            B2_CUDA(cudaMemcpyAsync(cv_out + r0 * n_alphas, cv_dev, sizeof(double) * rows * n_alphas,
-                                    cudaMemcpyDeviceToHost, ctx->stream));
-          return B2_OK;
-        });
-    if (rc != B2_OK) return rc;
-  }
+  if (int r = row_pass(
+          ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask,
+          [&](const RowSpan& s, void* cv, void*) {
+            return launch_loo(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_alphas,
+                              static_cast<double*>(cv), s.first);
+          },
+          RowOut{cv_out, sizeof(double) * n_alphas}))
+    return r;
   double sums[kMaxAlphas];
   B2_CUDA(cudaMemcpyAsync(sums, ctx->loo + kLooSum, sizeof(double) * n_alphas, cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1257,21 +1273,7 @@ int b2_residual_moments(b2_ctx* ctx, const void* X, int x_dtype, const float* y,
     return B2_E_UNSUPPORTED;
   }
   if (ctx->d != d) { set_error("the resident statistic has %d features, the rows %d", ctx->d, d); return B2_E_STATE; }
-  if (int r = ensure_s_cleared(ctx)) return r;
-  const int dp = d + 2;
-  std::vector<double> S((size_t)dp * dp), st(kRfDoubles, 0.0);
-  B2_CUDA(cudaMemcpyAsync(S.data(), ctx->S, sizeof(double) * dp * dp, cudaMemcpyDeviceToHost, ctx->stream));
-  B2_CUDA(cudaStreamSynchronize(ctx->stream));
-  const double n = S[(size_t)d * dp + d];
-  const double inv_n = n > 0.0 ? 1.0 / n : 0.0;
-  double b0 = intercept;
-  for (int j = 0; j < d; ++j) {
-    st[kRfBeta + j] = coef[j];
-    st[kRfMean + j] = fit_intercept ? S[(size_t)j * dp + d] * inv_n : 0.0;
-    b0 += st[kRfMean + j] * coef[j];
-  }
-  st[kRfB0] = b0;                        // the model b0' + (x - m).w is intercept + x.w
-  B2_CUDA(cudaMemcpyAsync(ctx->refine, st.data(), sizeof(double) * kRfDoubles, cudaMemcpyHostToDevice, ctx->stream));
+  if (int r = load_refine_state(ctx, d, coef, fit_intercept, &intercept)) return r;
   if (int r = grad_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
   double g[kGradOut];
   B2_CUDA(cudaMemcpyAsync(g, ctx->refine + kRfGrad, sizeof(g), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1425,33 +1427,15 @@ int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d,
   op[kStdMisc] = b_eff;
   op[kStdMisc + 1] = noise_var;
   B2_CUDA(cudaMemcpyAsync(ctx->enet, op.data(), sizeof(double) * kStdDoubles, cudaMemcpyHostToDevice, ctx->stream));
-  if (mem_kind == B2_MEM_DEVICE) {
-    if (int r = launch_score_std(ctx, X, x_dtype, n_rows, d, ldx, yhat, ystd)) return r;
-    B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
-    return B2_OK;
-  }
-  if (int r = ensure_staging(ctx)) return r;
-  if (int r = ensure_cv_stage(ctx, 2)) return r;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = host_pointer_is_pinned(X);
-  const int64_t blk = ctx->stage_rows;
-  const int rc = stream_host_blocks(
-      ctx, n_rows, blk,
-      [&](int buf, int64_t r0, int64_t rows) {
-        return stage_rows_h2d(ctx, buf, X, es, nullptr, nullptr, r0, rows, d, ldx, x_pinned);
-      },
-      [&](int buf, int64_t r0, int64_t rows) -> int {
-        double* sd = ctx->cv_stage[buf];
-        double* yd = yhat != nullptr ? sd + blk : nullptr;
-        if (int r = launch_score_std(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, yd, sd)) return r;
-        B2_CUDA(cudaMemcpyAsync(ystd + r0, sd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-        if (yhat != nullptr)
-          B2_CUDA(cudaMemcpyAsync(yhat + r0, yd, sizeof(double) * rows, cudaMemcpyDeviceToHost, ctx->stream));
-        return B2_OK;
-      });
-  const cudaError_t done = cudaStreamSynchronize(ctx->stream);
-  if (rc != B2_OK) return rc;
-  B2_CUDA(done);
+  if (int r = row_pass(
+          ctx, X, x_dtype, nullptr, n_rows, d, ldx, mem_kind, nullptr,
+          [&](const RowSpan& s, void* sd, void* yd) {
+            return launch_score_std(ctx, s.X, x_dtype, s.rows, d, s.ldx, static_cast<double*>(yd),
+                                    static_cast<double*>(sd));
+          },
+          RowOut{ystd, sizeof(double)}, RowOut{yhat, sizeof(double)}))
+    return r;
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
   return B2_OK;
 }
 
@@ -1493,27 +1477,12 @@ static int glm_setup(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ld
   return B2_OK;
 }
 
-// One pass over the rows into ctx->glm: device rows in one call of launch_glm, host rows block by block through the
-// staging ring (the first block overwrites the sums, the others add to them).
+// One pass over the rows into ctx->glm (the first rows overwrite the sums, the others add to them)
 static int glm_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                     int mem_kind, const uint8_t* row_mask, int mask_keep, int mode, int link, double power, int n_steps) {
-  if (mem_kind == B2_MEM_DEVICE)
-    return launch_glm(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, mode, link, power, n_steps, true);
-  if (n_rows == 0)
-    return launch_glm(ctx, nullptr, x_dtype, 0, d, d, nullptr, nullptr, mask_keep, mode, link, power, n_steps, true);
-  if (int r = ensure_staging(ctx)) return r;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = host_pointer_is_pinned(X);
-  return stream_host_blocks(
-      ctx, n_rows, ctx->stage_rows,
-      [&](int buf, int64_t r0, int64_t rows) {
-        return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-      },
-      [&](int buf, int64_t r0, int64_t rows) {
-        return launch_glm(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, ctx->stage_y[buf],
-                          row_mask != nullptr ? ctx->stage_m[buf] : nullptr, mask_keep, mode, link, power, n_steps,
-                          r0 == 0);
-      });
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*) {
+    return launch_glm(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, mode, link, power, n_steps, s.first);
+  });
 }
 
 int b2_glm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
@@ -1563,30 +1532,15 @@ int b2_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int 
   if (int r = glm_setup(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, nullptr, false, link, 0.0, coef, intercept, nullptr,
                         0.0))
     return r;
-  if (mem_kind == B2_MEM_DEVICE) {
-    if (int r = launch_glm_predict(ctx, X, x_dtype, n_rows, d, ldx, link, mu_out)) return r;
-    B2_CUDA(cudaStreamSynchronize(ctx->stream));
-    return B2_OK;
-  }
   if (n_rows == 0) return B2_OK;
-  if (int r = ensure_staging(ctx)) return r;
-  if (int r = ensure_cv_stage(ctx, 1)) return r;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  const bool x_pinned = host_pointer_is_pinned(X);
-  const int rc = stream_host_blocks(
-      ctx, n_rows, ctx->stage_rows,
-      [&](int buf, int64_t r0, int64_t rows) {
-        return stage_rows_h2d(ctx, buf, X, es, nullptr, nullptr, r0, rows, d, ldx, x_pinned);
-      },
-      [&](int buf, int64_t r0, int64_t rows) -> int {
-        if (int r = launch_glm_predict(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, link, ctx->cv_stage[buf])) return r;
-        B2_CUDA(cudaMemcpyAsync(mu_out + r0, ctx->cv_stage[buf], sizeof(double) * rows, cudaMemcpyDeviceToHost,
-                                ctx->stream));
-        return B2_OK;
-      });
-  const cudaError_t done = cudaStreamSynchronize(ctx->stream);
-  if (rc != B2_OK) return rc;
-  B2_CUDA(done);
+  if (int r = row_pass(
+          ctx, X, x_dtype, nullptr, n_rows, d, ldx, mem_kind, nullptr,
+          [&](const RowSpan& s, void* mu, void*) {
+            return launch_glm_predict(ctx, s.X, x_dtype, s.rows, d, s.ldx, link, static_cast<double*>(mu));
+          },
+          RowOut{mu_out, sizeof(double)}))
+    return r;
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
 }
 
@@ -1613,42 +1567,14 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
   double* acc = score_totals(ctx);
   if (n_rows == 0) {
     B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * kNStats, ctx->stream));
-  } else if (mem_kind == B2_MEM_DEVICE) {
-    if (int r = launch_score(ctx, X, x_dtype, n_rows, d, ldx, y, row_mask, mask_keep, yhat, true)) return r;
-  } else {
-    if (int r = ensure_staging(ctx)) return r;
-    const int es = x_dtype == B2_F32 ? 4 : 2;
-    const bool x_pinned = host_pointer_is_pinned(X);
-    // predictions of a staged block land in a device block of their own (allocated once per context) and are copied
-    // back behind the kernel
-    float* yhat_dev[2] = {nullptr, nullptr};
-    if (yhat != nullptr) {
-      for (int b = 0; b < 2; ++b) {
-        if (ctx->yhat_stage[b] == nullptr &&
-            cudaMalloc(reinterpret_cast<void**>(&ctx->yhat_stage[b]), (size_t)ctx->stage_rows * 4) != cudaSuccess) {
-          cudaGetLastError();
-          set_error("out of device memory for the prediction staging blocks");
-          return B2_E_CUDA;
-        }
-        yhat_dev[b] = ctx->yhat_stage[b];
-      }
-    }
-    const int rc = stream_host_blocks(
-        ctx, n_rows, ctx->stage_rows,
-        [&](int buf, int64_t r0, int64_t rows) {
-          return stage_rows_h2d(ctx, buf, X, es, y, row_mask, r0, rows, d, ldx, x_pinned);
-        },
-        [&](int buf, int64_t r0, int64_t rows) -> int {
-          if (int r = launch_score(ctx, ctx->stage_x[buf], x_dtype, rows, d, d, y ? ctx->stage_y[buf] : nullptr,
-                                   row_mask ? ctx->stage_m[buf] : nullptr, mask_keep, yhat_dev[buf], r0 == 0))
-            return r;
-          if (yhat != nullptr)
-            B2_CUDA(cudaMemcpyAsync(yhat + r0, yhat_dev[buf], (size_t)rows * 4, cudaMemcpyDeviceToHost, ctx->stream));
-          return B2_OK;
-        });
-    const cudaError_t done = cudaStreamSynchronize(ctx->stream);   // the predictions' copies into the caller's yhat
-    if (rc != B2_OK) return rc;
-    B2_CUDA(done);
+  } else if (int r = row_pass(
+                 ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask,
+                 [&](const RowSpan& s, void* yh, void*) {
+                   return launch_score(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep,
+                                       static_cast<float*>(yh), s.first);
+                 },
+                 RowOut{yhat, sizeof(float)})) {
+    return r;
   }
   if (stats_out != nullptr && y != nullptr) {
     B2_CUDA(cudaMemcpyAsync(stats_out, acc, sizeof(double) * kNStats, cudaMemcpyDeviceToHost, ctx->stream));

@@ -204,8 +204,6 @@ struct b2_ctx {
   // ridge leave-one-out scratch
   double* loo = nullptr;               // [kLooDoubles] Q, lambda, m, c, ybar / n / h0, alphas, the B operands, the sums
   double* loo_part = nullptr;          // [sm_count][kMaxAlphas] per-CTA sums of e^2
-  double* cv_stage[2] = {nullptr, nullptr};   // e^2 staging blocks of host rows [stage_rows][cv_stage_alphas]
-  int cv_stage_alphas = 0;             // alphas per row the staging blocks hold (grown to a call's n_alphas)
   // elastic-net path: inputs and outputs of b2_solve_enet_path (b2::EnetArgs), grown to the largest call
   double* enet = nullptr;
   size_t enet_doubles = 0;
@@ -235,7 +233,10 @@ struct b2_ctx {
   cudaEvent_t ev_copied[2] = {nullptr, nullptr};
   cudaEvent_t ev_consumed[2] = {nullptr, nullptr};
   bool ev_consumed_valid[2] = {false, false};   // a kernel of an earlier call may still read stage buffer b
-  float* yhat_stage[2] = {nullptr, nullptr};    // prediction staging blocks of the host-streamed b2_score
+  // the per-row outputs of host rows (yhat, ystd, e^2, mu): two blocks of stage_rows x row_out_bytes, grown to the
+  // widest call
+  char* row_out[2] = {nullptr, nullptr};
+  size_t row_out_bytes = 0;
   void* bounce[2] = {nullptr, nullptr};         // pinned bounce blocks for pageable host rows (filled by host threads)
   cudaEvent_t ev_bounce[2] = {nullptr, nullptr};
   bool s_zero_pending = false;         // b2_gram_reset is lazy: the first kernel to write S overwrites it
@@ -306,6 +307,44 @@ struct RowPlan {
 
 RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                   const uint8_t* mask);
+
+// The rows [r0, r0 + rows) of a call: X (row pitch ldx), y and mask point at row r0 (y / mask null when the call has
+// none); `first`: no earlier rows of the call have written its sums.
+struct RowSpan {
+  const void* X;
+  const float* y;
+  const uint8_t* mask;
+  int64_t ldx, r0, rows;
+  bool first;
+};
+
+// The rows [0, n) of a pass with a ring flavour that reads whole tiles of tile_rows rows: f(true, span) for the whole
+// tiles when plan_rows streams the rows through a ring, then f(false, span) for the rest.  A part with no rows is
+// skipped, except the direct part of an empty call that writes the sums first.
+template <typename F>
+int split_ring_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                    const uint8_t* mask, int tile_rows, bool first, F&& f) {
+  const bool ring_ok = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask).kind != RowPlan::kDirect;
+  const int64_t ring_rows = ring_ok ? (n / tile_rows) * tile_rows : 0;
+  const int es = x_dtype == B2_F32 ? 4 : 2;
+  for (int part = 0; part < 2; ++part) {
+    const bool ring = part == 0;
+    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
+    if (rows == 0 && (ring || !first)) continue;
+    const RowSpan s{static_cast<const char*>(X) + (size_t)r0 * ldx * es, y != nullptr ? y + r0 : nullptr,
+                    mask != nullptr ? mask + r0 : nullptr, ldx, r0, rows, first};
+    if (int r = f(ring, s)) return r;
+    first = false;
+  }
+  return B2_OK;
+}
+
+// acc[e] = (first ? 0 : acc[e]) + part[0][e] + part[1][e] + ... over n_ctas per-CTA partials of pitch `stride`, in CTA
+// order, so repeated calls are bit-identical.  The entries [0, n_lin), combined with fmax where bit e of max_mask is set;
+// with d1 > 0 also the upper triangle i <= j < d1 at tri_off + i * tri_pitch + j.  One launch, counted with the pass
+// whose partials it reduces (ctx->launches += 2).
+int launch_ordered_reduce(b2_ctx* ctx, const double* part, int stride, int n_ctas, bool first, int n_lin,
+                          unsigned max_mask, double* acc, int d1 = 0, int tri_off = 0, int tri_pitch = 0);
 
 // ---- kernel launchers (each enqueues on ctx->stream and bumps ctx->launches) -----------------
 // The Gram launchers are called by gram_dispatch (b2_api.cu) only.  assign: the kernel that writes S overwrites

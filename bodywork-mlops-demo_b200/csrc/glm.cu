@@ -16,7 +16,7 @@
 //       tile below the diagonal of a diagonal block skipped: 153 of the 289 8 x 8 tiles at D = 128.
 // The rows take scoring's plan (plan_rows): contiguous 16-byte aligned rows stream through the bulk-copy ring in whole
 // tiles, the rest (and every other layout) is read by the same consumers from global memory.  Each CTA writes its sums
-// in a fixed order, glm_reduce_kernel adds the CTAs in order: two calls return identical sums.
+// in a fixed order, the ordered reduce adds the CTAs in order: two calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
 #include "b2_ptx.cuh"
@@ -328,24 +328,6 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   }
 }
 
-// acc (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites.  The entries [0, n_lin), then with d1 > 0
-// the Hessian entries i <= j < d1.
-__global__ void glm_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, int n_lin, int d1,
-                                  double* __restrict__ acc) {
-  const int total = n_lin + d1 * d1;
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
-    int off = e;
-    if (e >= n_lin) {
-      const int q = e - n_lin, i = q / d1, j = q - i * d1;
-      if (i > j) continue;
-      off = kGlmHess + i * kGlmHp + j;
-    }
-    double v = first ? 0.0 : acc[off];
-    for (int c = 0; c < n_ctas; ++c) v += part[(size_t)c * kGlmPart + off];
-    acc[off] = v;
-  }
-}
-
 // mu = exp(eta) (log link) or eta (identity) per row, eta = x.w + b in fp64: one warp per row
 template <typename T>
 __global__ void __launch_bounds__(256)
@@ -374,41 +356,26 @@ glm_predict_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
 // into ctx->glm (`first_block` overwrites, otherwise adds).
 int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                const uint8_t* mask, int keep, int mode, int link, double power, int n_steps, bool first_block) {
-  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
-  const int64_t ring_rows = p.kind != RowPlan::kDirect ? (n / kGlmRows) * kGlmRows : 0;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  bool first = first_block;
-  for (int part = 0; part < 2; ++part) {
-    const bool ring = part == 0;
-    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
-    if (ring ? rows == 0 : (rows == 0 && !first)) continue;            // an empty call still writes the sums once
+  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kGlmRows, first_block, [&](bool ring, const RowSpan& s) {
     // two CTAs per SM hide the latency of the per-tile steps where the shared memory allows it (all but the Hessian)
-    const int64_t n_tiles = (rows + kGlmRows - 1) / kGlmRows, cap = (int64_t)ctx->sm_count * (mode == kGlmHessian ? 1 : 2);
+    const int64_t n_tiles = (s.rows + kGlmRows - 1) / kGlmRows, cap = (int64_t)ctx->sm_count * (mode == kGlmHessian ? 1 : 2);
     int grid = (int)(n_tiles < cap ? n_tiles : cap);
     if (grid < 1) grid = 1;
-    const char* Xt = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
-    const float* yt = y != nullptr ? y + r0 : nullptr;
-    const uint8_t* mt = mask != nullptr ? mask + r0 : nullptr;
     const uint32_t smem = (uint32_t)glm_smem_bytes(glm_dp(d), ring, mode);
-    const int rc = with_rows(x_dtype, Xt, [&](auto* Xr) {
+    const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
       return with_int<kGlmGradient, kGlmHessian, kGlmLadder>(mode, [&](auto M) {
         constexpr int MODE = decltype(M)::value;
         auto kernel = ring ? glm_kernel<T, true, MODE> : glm_kernel<T, false, MODE>;
-        return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, rows, d, ldx, yt,
-                           mt, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
+        return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, s.rows, d, ldx, s.y,
+                           s.mask, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
                            ctx->glm_part);
       });
     });
     if (rc != B2_OK) return rc;
     const int n_lin = mode == kGlmLadder ? 32 : kGlmHess, d1 = mode == kGlmHessian ? d + 1 : 0;
-    glm_reduce_kernel<<<(n_lin + d1 * d1 + 255) / 256, 256, 0, ctx->stream>>>(ctx->glm_part, grid, first ? 1 : 0, n_lin,
-                                                                               d1, ctx->glm);
-    B2_CUDA(cudaGetLastError());
-    ctx->launches += 2;
-    first = false;
-  }
-  return B2_OK;
+    return launch_ordered_reduce(ctx, ctx->glm_part, kGlmPart, grid, s.first, n_lin, 0u, ctx->glm, d1, kGlmHess, kGlmHp);
+  });
 }
 
 int launch_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, int link, double* mu) {

@@ -13,7 +13,7 @@
 // runs ring_produce with 32-row tiles of X and y and the consumers convert each slot in (1); the rows after the last whole
 // tile, and every other layout, are read by the same consumers straight from global memory.
 // A row not kept has v = 0 and e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA writes its sums per
-// alpha in a fixed order; loo_reduce_kernel adds the CTAs in order, so two calls return identical sums.
+// alpha in a fixed order; the ordered reduce adds the CTAs in order, so two calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
 #include "b2_ptx.cuh"
@@ -237,15 +237,6 @@ loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   }
 }
 
-// acc[kMaxAlphas] (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites
-__global__ void loo_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
-  const int a = threadIdx.x;
-  if (a >= kMaxAlphas) return;
-  double v = first ? 0.0 : acc[a];
-  for (int c = 0; c < n_ctas; ++c) v += part[(size_t)c * kMaxAlphas + a];
-  acc[a] = v;
-}
-
 }  // namespace
 
 // The rows [0, n) in the launches of scoring's plan: whole 32-row tiles of what plan_rows streams through the ring go to the
@@ -257,35 +248,21 @@ int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
     B2_CUDA(cudaGetLastError());
     ctx->launches += 1;
   }
-  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, y, mask);
-  const int64_t ring_rows = p.kind != RowPlan::kDirect ? (n / kLooRows) * kLooRows : 0;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  bool first = first_block;
-  for (int part = 0; part < 2; ++part) {
-    const bool ring = part == 0;
-    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
-    if (ring ? rows == 0 : (rows == 0 && !first)) continue;            // an empty call still writes the sums once
-    const int64_t n_tiles = (rows + kLooRows - 1) / kLooRows;
+  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kLooRows, first_block, [&](bool ring, const RowSpan& s) {
+    const int64_t n_tiles = (s.rows + kLooRows - 1) / kLooRows;
     int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
     if (grid < 1) grid = 1;
-    const char* Xt = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
-    const float* yt = y != nullptr ? y + r0 : nullptr;
-    const uint8_t* mt = mask != nullptr ? mask + r0 : nullptr;
-    double* cvt = cv != nullptr ? cv + r0 * n_alphas : nullptr;
+    double* cvt = cv != nullptr ? cv + s.r0 * n_alphas : nullptr;
     const uint32_t smem = (uint32_t)loo_smem_bytes(loo_dp(d), ring);
-    const int rc = with_rows(x_dtype, Xt, [&](auto* Xr) {
+    const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
       auto kernel = ring ? loo_kernel<T, true> : loo_kernel<T, false>;
-      return launch_smem(kernel, grid, ring ? kLooThreads : kLooConsumers, smem, ctx->stream, Xr, rows, d, ldx, yt, mt,
-                         keep, static_cast<const double*>(ctx->loo), n_alphas, cvt, ctx->loo_part);
+      return launch_smem(kernel, grid, ring ? kLooThreads : kLooConsumers, smem, ctx->stream, Xr, s.rows, d, ldx, s.y,
+                         s.mask, keep, static_cast<const double*>(ctx->loo), n_alphas, cvt, ctx->loo_part);
     });
     if (rc != B2_OK) return rc;
-    loo_reduce_kernel<<<1, kMaxAlphas, 0, ctx->stream>>>(ctx->loo_part, grid, first ? 1 : 0, ctx->loo + kLooSum);
-    B2_CUDA(cudaGetLastError());
-    ctx->launches += 2;
-    first = false;
-  }
-  return B2_OK;
+    return launch_ordered_reduce(ctx, ctx->loo_part, kMaxAlphas, grid, s.first, kMaxAlphas, 0u, ctx->loo + kLooSum);
+  });
 }
 
 }  // namespace b2

@@ -598,17 +598,6 @@ score_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* _
   stats_fold<kSnWarps>(red, part);
 }
 
-// acc[kNStats] (the running totals, score_totals) = the partials of n_ctas CTAs combined in CTA order; `first`
-// overwrites, otherwise they are combined with acc.
-__global__ void score_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
-  const int k = threadIdx.x;
-  if (k >= kNStats) return;
-  double v = first ? 0.0 : acc[k];
-  for (int c = 0; c < n_ctas; ++c)
-    v = stat_is_max(k) ? fmax(v, part[(size_t)c * kNStats + k]) : v + part[(size_t)c * kNStats + k];
-  acc[k] = v;
-}
-
 // ---- model_metrics on two vectors (stage_1_train_model.py:79-90): no X, no dot product -- the statistics alone, on
 // fp32 or fp64 inputs (the reference computes them on float64 arrays; b2_metrics(B2_F64) matches it to rounding) -----
 template <typename V>
@@ -632,7 +621,7 @@ metrics_kernel(const V* __restrict__ ya, const V* __restrict__ yp, int64_t n, do
 // exactly converted x: e is a small difference of large terms.  The three layouts of scoring carry it: register-fed (any layout, the tails), the TMA ring (wide contiguous
 // rows), one lane per row (d <= 16).  A lane keeps the fp64 sums of the features it loads.  A dropped row gets x = 0 and
 // e = 0 by selects, so whatever it holds never reaches a sum.  Each CTA combines its sums in a fixed order into
-// part[blockIdx.x][kGradOut] (features, then g_1 at kMaxD, sum e^2 at kMaxD + 1); grad_reduce_kernel adds the CTAs in order.
+// part[blockIdx.x][kGradOut] (features, then g_1 at kMaxD, sum e^2 at kMaxD + 1); the ordered reduce adds the CTAs in order.
 template <typename T>
 __device__ __forceinline__ float ld_x_f32(const T* __restrict__ p);
 template <>
@@ -919,43 +908,47 @@ grad_narrow_kernel(const T* __restrict__ X, int n_tiles, int d, const double* __
   grad_fold<kSnWarps>(red, d, part);
 }
 
-// acc[kGradOut] (+)= the partials of n_ctas CTAs, added in CTA order; `first` overwrites
-__global__ void grad_reduce_kernel(const double* __restrict__ part, int n_ctas, int first, double* __restrict__ acc) {
-  const int t = threadIdx.x;
-  if (t >= kGradOut) return;
-  double v = first ? 0.0 : acc[t];
-  int c = 0;
-  for (; c + 8 <= n_ctas; c += 8) {          // eight loads in flight, the adds in CTA order
-    double p[8];
+// launch_ordered_reduce: one thread per entry, eight loads in flight, the combines in CTA order
+__global__ void ordered_reduce_kernel(const double* __restrict__ part, int stride, int n_ctas, int first, int n_lin,
+                                      unsigned max_mask, int d1, int tri_off, int tri_pitch, double* __restrict__ acc) {
+  const int total = n_lin + d1 * d1;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
+    int off = e;
+    if (e >= n_lin) {
+      const int q = e - n_lin, i = q / d1, j = q - i * d1;
+      if (i > j) continue;
+      off = tri_off + i * tri_pitch + j;
+    }
+    const bool is_max = e < n_lin && e < 32 && ((max_mask >> e) & 1u) != 0;
+    double v = first ? 0.0 : acc[off];
+    int c = 0;
+    for (; c + 8 <= n_ctas; c += 8) {
+      double p[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) p[u] = part[(size_t)(c + u) * kGradOut + t];
+      for (int u = 0; u < 8; ++u) p[u] = part[(size_t)(c + u) * stride + off];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) v += p[u];
+      for (int u = 0; u < 8; ++u) v = is_max ? fmax(v, p[u]) : v + p[u];
+    }
+    for (; c < n_ctas; ++c) v = is_max ? fmax(v, part[(size_t)c * stride + off]) : v + part[(size_t)c * stride + off];
+    acc[off] = v;
   }
-  for (; c < n_ctas; ++c) v += part[(size_t)c * kGradOut + t];
-  acc[t] = v;
 }
 
-// ---- host ---------------------------------------------------------------------------------------------------------
-// Every kernel writes per-CTA partials, and an ordered reduce combines them into the running totals: 2 launches per
-// segment of rows.  `first` overwrites the totals, otherwise the segment's rows are added to them.
-int score_reduce(b2_ctx* ctx, int grid, bool first) {
-  B2_CUDA(cudaGetLastError());
-  score_reduce_kernel<<<1, 32, 0, ctx->stream>>>(ctx->score_part, grid, first ? 1 : 0, score_totals(ctx));
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
-}
-// the gradient's totals are ctx->refine + kRfGrad
-int grad_reduce(b2_ctx* ctx, int grid, bool first) {
-  B2_CUDA(cudaGetLastError());
-  grad_reduce_kernel<<<1, 160, 0, ctx->stream>>>(ctx->grad_part, grid, first ? 1 : 0, ctx->refine + kRfGrad);
-  B2_CUDA(cudaGetLastError());
-  ctx->launches += 2;
-  return B2_OK;
-}
+// scoring's statistics combine their two maxima (4 and 9) with fmax
+constexpr unsigned kStatsMaxMask = (1u << 4) | (1u << 9);
 
 }  // namespace
+
+int launch_ordered_reduce(b2_ctx* ctx, const double* part, int stride, int n_ctas, bool first, int n_lin,
+                          unsigned max_mask, double* acc, int d1, int tri_off, int tri_pitch) {
+  B2_CUDA(cudaGetLastError());
+  const int total = n_lin + d1 * d1;
+  ordered_reduce_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>(part, stride, n_ctas, first ? 1 : 0, n_lin,
+                                                                      max_mask, d1, tri_off, tri_pitch, acc);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  return B2_OK;
+}
 
 RowPlan plan_rows(const b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                   const uint8_t* mask) {
@@ -1004,7 +997,7 @@ int launch_metrics(b2_ctx* ctx, const void* y, const void* yhat, int dtype, int6
   else
     metrics_kernel<double><<<grid, kScoreThreads, 0, ctx->stream>>>(static_cast<const double*>(y),
                                                                     static_cast<const double*>(yhat), n, ctx->score_part);
-  return score_reduce(ctx, grid, first);
+  return launch_ordered_reduce(ctx, ctx->score_part, kNStats, grid, first, kNStats, kStatsMaxMask, score_totals(ctx));
 }
 
 int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
@@ -1028,7 +1021,9 @@ int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int6
       });
     });
     if (rc != B2_OK) return rc;
-    if (int r = score_reduce(ctx, p.grid, first_block)) return r;
+    if (int r = launch_ordered_reduce(ctx, ctx->score_part, kNStats, p.grid, first_block, kNStats, kStatsMaxMask,
+                                     score_totals(ctx)))
+      return r;
     first_block = false;
   }
   if (!p.direct) return B2_OK;
@@ -1048,7 +1043,8 @@ int launch_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int6
                                                                          yhat_t, p.vec, ctx->score_part);
     return B2_OK;
   });
-  return score_reduce(ctx, p.direct_grid, first_block);
+  return launch_ordered_reduce(ctx, ctx->score_part, kNStats, p.direct_grid, first_block, kNStats, kStatsMaxMask,
+                               score_totals(ctx));
 }
 
 // The residual gradient over the rows [0, n): the kernels of launch_score's plan (the labels are always present).
@@ -1071,7 +1067,9 @@ int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64
       });
     });
     if (rc != B2_OK) return rc;
-    if (int r = grad_reduce(ctx, p.grid, first_block)) return r;
+    if (int r = launch_ordered_reduce(ctx, ctx->grad_part, kGradOut, p.grid, first_block, kGradOut, 0u,
+                                     ctx->refine + kRfGrad))
+      return r;
     first_block = false;
   }
   if (!p.direct) return B2_OK;
@@ -1084,7 +1082,8 @@ int launch_grad(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64
                                                                       p.vec, ctx->grad_part);
     return B2_OK;
   });
-  return grad_reduce(ctx, p.direct_grid, first_block);
+  return launch_ordered_reduce(ctx, ctx->grad_part, kGradOut, p.direct_grid, first_block, kGradOut, 0u,
+                               ctx->refine + kRfGrad);
 }
 
 }  // namespace b2

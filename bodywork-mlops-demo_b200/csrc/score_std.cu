@@ -173,28 +173,22 @@ score_std_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const d
 // The rows [0, n) in the launches of scoring's plan: the whole 32-row tiles of what plan_rows streams through the ring go
 // to the ring flavour, the rest (or every row of another layout) to the direct one.
 int launch_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* yhat, double* ystd) {
-  const RowPlan p = plan_rows(ctx, X, x_dtype, n, d, ldx, nullptr, nullptr);
-  const int64_t ring_rows = p.kind != RowPlan::kDirect ? (n / kStdRows) * kStdRows : 0;
-  const int es = x_dtype == B2_F32 ? 4 : 2;
-  for (int part = 0; part < 2; ++part) {
-    const bool ring = part == 0;
-    const int64_t r0 = ring ? 0 : ring_rows, rows = ring ? ring_rows : n - ring_rows;
-    if (rows == 0) continue;
-    const int64_t n_tiles = (rows + kStdRows - 1) / kStdRows;
+  // no sums: `first` is false, so a part without rows is never launched
+  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, nullptr, nullptr, kStdRows, false, [&](bool ring, const RowSpan& s) {
+    const int64_t n_tiles = (s.rows + kStdRows - 1) / kStdRows;
     const int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
-    const char* Xt = static_cast<const char*>(X) + (size_t)r0 * ldx * es;
-    double* yh = yhat != nullptr ? yhat + r0 : nullptr;
+    double* yh = yhat != nullptr ? yhat + s.r0 : nullptr;
     const uint32_t smem = (uint32_t)std_smem_bytes(std_dp(d), ring);
-    const int rc = with_rows(x_dtype, Xt, [&](auto* Xr) {
+    const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
       auto kernel = ring ? score_std_kernel<T, true> : score_std_kernel<T, false>;
-      return launch_smem(kernel, grid, ring ? kStdThreads : kStdConsumers, smem, ctx->stream, Xr, rows, d, ldx,
-                         static_cast<const double*>(ctx->enet), yh, ystd + r0);
+      return launch_smem(kernel, grid, ring ? kStdThreads : kStdConsumers, smem, ctx->stream, Xr, s.rows, d, ldx,
+                         static_cast<const double*>(ctx->enet), yh, ystd + s.r0);
     });
     if (rc != B2_OK) return rc;
     ctx->launches += 1;
-  }
-  return B2_OK;
+    return B2_OK;
+  });
 }
 
 }  // namespace b2
