@@ -20,9 +20,11 @@
 //            D2[i][j] += sum_r lo[r][i] * [hi | E][r][j]             m64n(128 + EW): small zero-mean terms, drained
 //                                                                     once at the end
 //        so D1[:, :128] = hi^T hi (i <= j), D2[:, :128] = lo^T hi, column 128 = sum v, columns 129/130 = sum v*y'.
-//     --every `drain_rows` rows the two consumer warpgroups fold the entries of D1 the fold reads (i <= j, and E) into
-//        this CTA's fp64 partial in global memory (L2-resident; fire-and-forget red.add.f64; layout: tc_part_index)
-//        and restart it from zero; the producer warps keep filling stages meanwhile.
+//     --every `drain_rows` rows the two consumer warpgroups add the entries of D1 the fold reads (i <= j, and E) to
+//        their running fp64 sums and restart D1 from zero; the producer warps keep filling stages meanwhile.  A sum
+//        lives in its owner thread's registers, in a shared-memory slab, or for the entries that fit in neither in
+//        this CTA's fp64 partial in global memory (L2-resident; fire-and-forget red.add.f64); the end of the range
+//        stores the on-chip sums to the partial (layout: tc_part_index).
 //       The accumulator registers (136 or 144 per thread of warpgroup 0) come from the producers (setmaxnreg).
 //
 // Why the shift and the split: the tensor core accumulates fp32 with truncation, so raw (uncentred)
@@ -90,7 +92,11 @@ struct TcGeo {
   static constexpr int kNumBars = 2 * kRawStages + 2 * kOpStages;
   static constexpr uint32_t kOffShift = kOffBar + kNumBars * 8;
   static constexpr uint32_t kOffESum = kOffShift + (kMaxD + 4) * 4;    // kEWarp's per-lane fp64 sums [3][32]
-  static constexpr uint32_t kSmemBytes = kOffESum + 3 * 32 * 8 + 1024;  // + alignment slack (~205 KB)
+  // the consumers' running fp64 sums of drained D1 entries that live in shared memory (TcSums):
+  // [consumer warp 0..3 of warpgroup 0, then of warpgroup 1][slot][lane], conflict-free, the rest of the 227 KB
+  static constexpr int kSlabSlots = RAWB ? 22 : 21;                     // per thread, both warpgroups together
+  static constexpr uint32_t kOffSlab = kOffESum + 3 * 32 * 8;
+  static constexpr uint32_t kSmemBytes = kOffSlab + kSlabSlots * 4 * 32 * 8 + 1024;  // + alignment slack (~227 KB)
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
   // setmaxnreg split of the 64 K-register file (128 x 512 threads): up to 144 fp32 accumulators per consumer thread.  A
   // transform lane holds 16 values of two features and, at runtime d, eight row addresses: 64 registers.  RAWB's
@@ -98,6 +104,24 @@ struct TcGeo {
   static constexpr uint32_t kConsumerRegs = RAWB ? 200 : 192, kProducerRegs = RAWB ? 56 : 64;
   static_assert(kConsumerRegs * 128 * kConsumerWGs + kProducerRegs * (kThreads - 128 * kConsumerWGs) <= 65536,
                 "register budget");
+};
+
+// Where a consumer thread keeps the running fp64 sum of each D1 entry it drains, between the drains of a range:
+// the top kRegs of its kR1 D1 registers in `double` registers, the kSlab below them in its slots of the shared slab,
+// the rest in the CTA's partial in L2 (red.add.f64).  The top registers hold the E columns and the highest feature
+// columns, the ones whose entries are all in the upper triangle.  The budgets are what the accumulators leave of the
+// consumers' setmaxnreg registers without spills (-Xptxas -v): warpgroup 1 keeps all its sums in registers, so warpgroup
+// 0 takes the whole slab.
+template <int DFIX, bool SPLIT, bool RAWB, int EW, int WG>
+struct TcSums {
+  static constexpr int kR1 = (kTcM - 64 * WG + EW) / 2;
+  static constexpr bool kTight = SPLIT && !RAWB && (EW == 16 || DFIX == 0);
+  static constexpr int kRegs = WG == 1 ? (kTight ? (EW == 16 ? 24 : 28) : kR1)
+                                       : (!SPLIT ? 40 : (RAWB || EW == 16 ? 0 : (DFIX ? 16 : 8)));
+  static constexpr int kSlab = WG == 1 ? 0 : TcGeo<RAWB>::kSlabSlots;
+  static constexpr int kSlabBase = WG == 1 ? TcSums<DFIX, SPLIT, RAWB, EW, 0>::kSlab : 0;   // slots of warpgroup 0 before
+  static constexpr int kFirstSlab = kR1 - kRegs - kSlab, kFirstReg = kR1 - kRegs;      // register index ranges
+  static_assert(kFirstSlab >= 0 && kSlabBase + kSlab <= TcGeo<RAWB>::kSlabSlots, "fp64 sum homes");
 };
 
 // ------------------------------------------------------------------------------------------
@@ -269,6 +293,10 @@ __device__ __forceinline__ void put_f64(double* p, double v, bool add, bool on) 
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.f64 [%0], %1;\n\t}"
                  ::"l"(p), "d"(v), "r"((uint32_t)on) : "memory");
 }
+__device__ __forceinline__ void st_shared_f64_if(uint32_t addr, double v, bool on) {   // predicated, as put_f64
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.shared.f64 [%0], %1;\n\t}"
+               ::"r"(addr), "d"(v), "r"((uint32_t)on) : "memory");
+}
 __device__ __forceinline__ void st_shared_u16(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)v) : "memory");
 }
@@ -408,7 +436,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
                int64_t n_rows, int d_arg, int pack, int d_orig, const float* __restrict__ shift,
                int chunk_tiles, double* __restrict__ part, uint32_t wait_ns, uint32_t dbg_arg) {
 #ifdef B2_DEV_KNOBS
-  const uint32_t dbg = dbg_arg;      // ablation switches (tools/build_dev.sh): results are WRONG when non-zero
+  const uint32_t dbg = dbg_arg;      // ablation switches (tools/build_dev.sh): results are WRONG when non-zero, except
+                                     // with bit 8 alone
 #else
   constexpr uint32_t dbg = 0u;       // product build: the ablation branches compile away
   (void)dbg_arg;
@@ -484,11 +513,20 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       // accumulator column 8 j + 2 (lane % 4) + e, partial column col0 + that (an E column from 128 on).
       // store(dst_acc, col0, add, val) writes (or adds) val(r, col, h) for every register r whose element the fold reads
       // from accumulator dst_acc: D1's upper triangle i <= j and E columns, every D2 column.
-      // The add is a fire-and-forget reduction in L2 (red.add.f64, one IEEE fp64 add like `*p += v`): a load-add-store
-      // would stall the consumers for an L2 round trip per few registers, and since every CTA drains after the same
-      // number of tiles, all SMs would stop reading HBM at the same time.  Each element has one writer, whose
-      // store and reductions to it take effect in program order (same-address coherence): the sums are those of `*p += v`.
+      // A D1 entry's running fp64 sum lives in its owner thread's registers or shared slab slots (TcSums), or in L2:
+      // there the add is a fire-and-forget reduction (red.add.f64, one IEEE fp64 add like `*p += v`).  Each element has
+      // one writer, whose store and reductions to it take effect in program order (same-address coherence), so every
+      // home holds the same sum: the chunks' values added in chunk order with round-to-nearest.  The on-chip homes keep
+      // the drain off L2, where the ~9 300 reductions per CTA of a drain, issued by all SMs after the same number of
+      // tiles, stalled every SM's stream of loads at once.
+      using H = TcSums<DFIX, SPLIT, RAWB, EW, WG>;
       double* my_part = part + (size_t)blockIdx.x * kTcAccElems;
+      double sums[H::kRegs > 0 ? H::kRegs : 1];
+      // off: the development knob that sends every entry through L2
+      const bool on_chip_off = (dbg & 256u) != 0u;
+      auto slab_addr = [&](int s, int ln) {
+        return sbase + G::kOffSlab + (uint32_t)(((4 * H::kSlabBase + (warp & 3) * H::kSlab + s) * 32 + ln) * 8);
+      };
       auto store = [&](auto n_regs, int dst_acc, int col0, bool add, auto val) {
         // the lane is re-read here: partial indices computed from a kept one are hoisted out of the tile loop and hold a
         // register each
@@ -497,7 +535,26 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         for (int r = 0; r < decltype(n_regs)::value; ++r) {
           const int col = col0 + 8 * (r >> 2) + 2 * (ln & 3) + (r & 1), h = (r >> 1) & 1, i = row0 + 8 * h;
           const bool lower = dst_acc == 0 && col < kTcM && i > col;   // D1's lower triangle: (col, i) holds it
-          put_f64(my_part + tc_part_index(dst_acc, i, col, EW), val(r, col, h), add, !lower);
+          const double v = val(r, col, h);
+          const bool on_chip = dst_acc == 0 && r >= H::kFirstSlab;
+          if (on_chip && r >= H::kFirstReg) {
+            double& s = sums[r - H::kFirstReg];
+            s = add ? __dadd_rn(s, v) : v;
+          } else if (on_chip) {
+            const uint32_t a = slab_addr(r - H::kFirstSlab, ln);
+            st_shared_f64_if(a, add ? __dadd_rn(ld_shared_f64(a), v) : v, !on_chip_off);
+          }
+          put_f64(my_part + tc_part_index(dst_acc, i, col, EW), v, add, !lower && (!on_chip || on_chip_off));
+        }
+      };
+      // the end of the range: the on-chip sums to their partial entries
+      auto flush = [&]() {
+        const int ln = (int)lane_id(), row0 = 64 * WG + 16 * (warp & 3) + (ln >> 2);
+#pragma unroll
+        for (int r = H::kFirstSlab; r < H::kR1; ++r) {
+          const int col = kC1 + 8 * (r >> 2) + 2 * (ln & 3) + (r & 1), i = row0 + 8 * ((r >> 1) & 1);
+          const double s = r >= H::kFirstReg ? sums[r - H::kFirstReg] : ld_shared_f64(slab_addr(r - H::kFirstSlab, ln));
+          put_f64(my_part + tc_part_index(0, i, col, EW), s, false, !(col < kTcM && i > col) && !on_chip_off);
         }
       };
       // RAWB's feature columns carry the raw x: sum_r a_i x_j - c_j sum_r a_i = sum_r a_i v_j, where sum_r a_i is E's ones
@@ -583,6 +640,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         fence_regs(acc2);
         drain(acc2, RAWB ? 0 : 1, RAWB ? kC1 : 0, RAWB);
       }
+      flush();
     };
     // branch on a shuffled warp index: ptxas serialises the wgmma of both copies when the branch depends on the thread
     // index directly (it cannot tell that the condition is uniform over each warpgroup)
@@ -977,7 +1035,7 @@ int launch_gram_tc(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int6
                                            // bit6 skip the E columns and the y' sums, bit7 skip the whole transform
     const char* e = getenv("B2_TC_DEBUG");
     return e ? (uint32_t)atoi(e) : 0u;
-  }();
+  }();                                     // bit8 every drained D1 sum in L2 (no on-chip homes; results unchanged)
 #else
   constexpr uint32_t dbg = 0u;
 #endif
