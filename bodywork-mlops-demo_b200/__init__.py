@@ -17,18 +17,20 @@ Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- th
     B200PoissonRegressor, B200GammaRegressor, B200TweedieRegressor
                            sklearn's GLM regressors (solver="newton-cholesky"): each Newton iteration is one pass for the
                            loss, gradient and fp64 tensor-core Hessian and one pass for every line-search step
+    B200LogisticRegression sklearn's binary LogisticRegression (solver="newton-cholesky"): the same Newton passes on the
+                           half-binomial loss, labels as stored, probabilities and labels in one predict pass
     stage_1_train_model    drop-in for mlops_simulation/stage_1_train_model.py
 """
 from . import _native as native
 from ._native import (BF16, F32, KERNEL_AUTO, KERNEL_NARROW, KERNEL_SIMT, KERNEL_TCGEN05, PRECISION_BF16, PRECISION_SPLIT, Context,
                       DeviceArray, PinnedArray)
 from .estimator import (B200ARDRegression, B200BayesianRidge, B200ElasticNet, B200ElasticNetCV, B200GammaRegressor,
-                        B200Lasso, B200LassoCV, B200LinearRegression, B200PoissonRegressor, B200RidgeCV,
+                        B200Lasso, B200LassoCV, B200LinearRegression, B200LogisticRegression, B200PoissonRegressor, B200RidgeCV,
                         B200TweedieRegressor, default_context, enet_path, fold_ids, lasso_path)
 from . import sharding, tranche_io  # noqa: F401
 
 __all__ = ["native", "Context", "DeviceArray", "PinnedArray", "B200LinearRegression", "B200RidgeCV", "B200ElasticNet",
            "B200Lasso", "B200ElasticNetCV", "B200LassoCV", "B200BayesianRidge", "B200ARDRegression",
-           "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "fold_ids", "enet_path", "lasso_path", "default_context",
+           "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression", "fold_ids", "enet_path", "lasso_path", "default_context",
            "F32", "BF16", "KERNEL_AUTO", "KERNEL_SIMT", "KERNEL_TCGEN05", "KERNEL_NARROW", "PRECISION_SPLIT", "PRECISION_BF16"]
 __version__ = "0.1.0"

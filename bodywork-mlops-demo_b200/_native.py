@@ -89,6 +89,13 @@ _SIGNATURES = {
     "b2_glm_line_search": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_int,
                                      C.c_double, _vp, C.c_double, _vp, C.c_double, C.c_int, _vp]),
     "b2_glm_predict": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, C.c_int, _vp, C.c_double, _vp]),
+    "b2_logistic_pass": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_double,
+                                   C.c_double, _vp, C.c_double, C.c_int, _vp, _vp]),
+    "b2_logistic_line_search": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int,
+                                          C.c_double, C.c_double, _vp, C.c_double, _vp, C.c_double, C.c_int, _vp]),
+    "b2_logistic_predict": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, C.c_double,
+                                      C.c_double, _vp, _vp, _vp]),
+    "b2_label_scan": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, _vp]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -742,6 +749,88 @@ class Context:
             raise ValueError(last_error())
         _check(rc, "b2_glm_predict")
         return mu
+
+    # -- LogisticRegression, binary (DESIGN.md section 11) ----------------------------------------------------------
+    def logistic_pass(self, X, y, coef, intercept: float, neg_label: float = 0.0, pos_label: float = 1.0, *,
+                      row_mask=None, mask_keep: int = 1, fit_intercept: bool = True, hessian: bool = True) -> dict:
+        """One pass of the Newton solver's statistics for HalfBinomialLoss at (coef, intercept) over the kept rows
+        (b2_logistic_pass); y holds the labels as stored, the target is 1 where y == pos_label and 0 where y == neg_label.
+        Returns ``glm_pass``'s dict (sum_y: the positive rows, y_out_of_range: the rows with neither label) and correct:
+        the rows classified correctly by the sign of eta.  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        w = self._glm_coef(coef, d)
+        sums = np.empty(d + 9, dtype=np.float64)
+        hess = np.empty((d + 1, d + 1), dtype=np.float64) if hessian else None
+        rc = load().b2_logistic_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(neg_label),
+                                     float(pos_label), w.ctypes.data, float(intercept), int(bool(fit_intercept)),
+                                     sums.ctypes.data, hess.ctypes.data if hess is not None else None)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_logistic_pass")
+        keys = ("loss", "const", "sum_y", "kept", "y_out_of_range", "h_nonpos", "y_nonfinite")
+        out = {k: float(sums[i]) for i, k in enumerate(keys)}
+        out["grad"] = sums[7:8 + d].copy()
+        out["correct"] = float(sums[8 + d])
+        out["hessian"] = hess
+        return out
+
+    def logistic_line_search(self, X, y, coef, intercept: float, step, step_intercept: float, neg_label: float = 0.0,
+                             pos_label: float = 1.0, *, n_steps: int = GLM_STEPS, row_mask=None,
+                             mask_keep: int = 1) -> np.ndarray:
+        """The backtracking ladder of a logistic Newton step in one pass (b2_logistic_line_search)."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        yp = _vec_ptr(y, "f32", mk, n, "y")
+        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        w, s = self._glm_coef(coef, d), self._glm_coef(step, d)
+        out = np.empty(max(int(n_steps), 1), dtype=np.float64)
+        rc = load().b2_logistic_line_search(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(neg_label),
+                                            float(pos_label), w.ctypes.data, float(intercept), s.ctypes.data,
+                                            float(step_intercept), int(n_steps), out.ctypes.data)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_logistic_line_search")
+        return out
+
+    def logistic_predict(self, X, coef, intercept: float, neg_label: float = 0.0, pos_label: float = 1.0, *,
+                         decision: bool = False, proba: bool = False, label: bool = False) -> dict:
+        """The logistic model per row in one pass (b2_logistic_predict): the wanted ones of decision (eta, fp64), proba
+        ((n, 2) [1 - p, p], fp64) and label (pos_label where eta > 0, else neg_label; fp32) -- ndarrays for host rows,
+        DeviceArrays for device rows."""
+        ptr, xdt, mk, n, d = _x_kind(X)
+        w = self._glm_coef(coef, d)
+        out, ptrs = {}, {}
+        for name, want, shape, kind, dtype in (("decision", decision, (n,), "f64", np.float64),
+                                               ("proba", proba, (n, 2), "f64", np.float64),
+                                               ("label", label, (n,), "f32", np.float32)):
+            if not want:
+                ptrs[name] = None
+                continue
+            a = self.empty(shape, kind) if mk == MEM_DEVICE else np.empty(shape, dtype=dtype)
+            out[name] = a
+            ptrs[name] = a.ptr if mk == MEM_DEVICE else a.ctypes.data
+        rc = load().b2_logistic_predict(self._h, ptr, xdt, n, d, d, mk, w.ctypes.data, float(intercept),
+                                        float(neg_label), float(pos_label), ptrs["decision"], ptrs["proba"],
+                                        ptrs["label"])
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_logistic_predict")
+        return out
+
+    def label_scan(self, y, row_mask=None, mask_keep: int = 1) -> dict:
+        """The labels of an f32 DeviceArray y over the kept rows (b2_label_scan): kept, nonfinite, nonintegral (finite y
+        != rint(y)), min and max of the finite kept y (NaN without any), n_min and n_max (kept rows equal to each)."""
+        if not isinstance(y, DeviceArray) or y.kind != "f32":
+            raise RuntimeError("label_scan: y must be an f32 DeviceArray")
+        n = int(np.prod(y.shape))
+        mp = _vec_ptr(row_mask, "u8", MEM_DEVICE, n, "row_mask")
+        st = np.empty(7, dtype=np.float64)
+        rc = load().b2_label_scan(self._h, y.ptr, n, mp, int(mask_keep), st.ctypes.data)
+        if rc == E_ARG:
+            raise ValueError(last_error())
+        _check(rc, "b2_label_scan")
+        return dict(zip(("kept", "nonfinite", "nonintegral", "min", "max", "n_min", "n_max"), st.tolist()))
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

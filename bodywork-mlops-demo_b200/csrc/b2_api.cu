@@ -308,18 +308,18 @@ struct RowOut {
   size_t row_bytes = 0;
 };
 
-// One pass over the rows [0, n_rows) of a call, wherever they live: launch(span, out0, out1) enqueues the pass over the
-// rows of `span` and writes the per-row outputs to out0 / out1 (null when not wanted).
+// One pass over the rows [0, n_rows) of a call, wherever they live: launch(span, out0, out1, out2) enqueues the pass over
+// the rows of `span` and writes the per-row outputs to out0 / out1 / out2 (null when not wanted).
 // Device rows: one launch on the caller's pointers.  Host rows: one launch per block of the staging ring, its outputs
 // written to the row-output blocks and copied back behind it; with outputs, the stream is synchronised before the
 // return, so the caller may reuse every host buffer -- also when a block failed.  Zero rows: one launch on zero rows.
 template <typename Launch>
 int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
-             const uint8_t* mask, Launch&& launch, RowOut out0 = {}, RowOut out1 = {}) {
-  if (mem_kind == B2_MEM_DEVICE) return launch(RowSpan{X, y, mask, ldx, 0, n_rows, true}, out0.dst, out1.dst);
-  if (n_rows == 0) return launch(RowSpan{nullptr, nullptr, nullptr, d, 0, 0, true}, nullptr, nullptr);
+             const uint8_t* mask, Launch&& launch, RowOut out0 = {}, RowOut out1 = {}, RowOut out2 = {}) {
+  if (mem_kind == B2_MEM_DEVICE) return launch(RowSpan{X, y, mask, ldx, 0, n_rows, true}, out0.dst, out1.dst, out2.dst);
+  if (n_rows == 0) return launch(RowSpan{nullptr, nullptr, nullptr, d, 0, 0, true}, nullptr, nullptr, nullptr);
   if (int r = ensure_staging(ctx)) return r;
-  RowOut out[2] = {out0, out1};
+  RowOut out[3] = {out0, out1, out2};
   size_t out_bytes = 0;
   for (RowOut& o : out) {
     if (o.dst == nullptr) o.row_bytes = 0;
@@ -335,13 +335,15 @@ int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_
         return stage_rows_h2d(ctx, buf, X, es, y, mask, r0, rows, d, ldx, x_pinned);
       },
       [&](int buf, int64_t r0, int64_t rows) -> int {
-        char* const block = ctx->row_out[buf];   // [stage_rows] of output 0, then [stage_rows] of output 1
-        char* dev[2] = {out[0].dst != nullptr ? block : nullptr,
-                        out[1].dst != nullptr ? block + (size_t)ctx->stage_rows * out[0].row_bytes : nullptr};
+        char* const block = ctx->row_out[buf];   // [stage_rows] of output 0, then of output 1, then of output 2
+        char* dev[3] = {out[0].dst != nullptr ? block : nullptr,
+                        out[1].dst != nullptr ? block + (size_t)ctx->stage_rows * out[0].row_bytes : nullptr,
+                        out[2].dst != nullptr
+                            ? block + (size_t)ctx->stage_rows * (out[0].row_bytes + out[1].row_bytes) : nullptr};
         const RowSpan s{ctx->stage_x[buf], y != nullptr ? ctx->stage_y[buf] : nullptr,
                         mask != nullptr ? ctx->stage_m[buf] : nullptr, d, r0, rows, r0 == 0};
-        if (int r = launch(s, dev[0], dev[1])) return r;
-        for (int k = 0; k < 2; ++k)
+        if (int r = launch(s, dev[0], dev[1], dev[2])) return r;
+        for (int k = 0; k < 3; ++k)
           if (out[k].dst != nullptr)
             B2_CUDA(cudaMemcpyAsync(static_cast<char*>(out[k].dst) + (size_t)r0 * out[k].row_bytes, dev[k],
                                     (size_t)rows * out[k].row_bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -358,7 +360,7 @@ int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_
 // fused exchange)
 int gram_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
               const uint8_t* mask, int keep) {
-  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, mask, [&](const RowSpan& s, void*, void*) {
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, mask, [&](const RowSpan& s, void*, void*, void*) {
     return gram_dispatch(ctx, s.X, x_dtype, s.y, s.rows, d, s.ldx, s.mask, keep);
   });
 }
@@ -846,7 +848,7 @@ int b2_fit(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_ro
 // g_j, g_1 and sum e^2 to ctx->refine + kRfGrad; host rows re-stream through the staging ring.
 static int grad_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                      int mem_kind, const uint8_t* row_mask, int mask_keep) {
-  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*) {
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
     return launch_grad(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, s.first);
   });
 }
@@ -1240,7 +1242,7 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
   if (int r = eigh_converged(misc[3])) return r;
   if (int r = row_pass(
           ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask,
-          [&](const RowSpan& s, void* cv, void*) {
+          [&](const RowSpan& s, void* cv, void*, void*) {
             return launch_loo(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_alphas,
                               static_cast<double*>(cv), s.first);
           },
@@ -1429,7 +1431,7 @@ int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d,
   B2_CUDA(cudaMemcpyAsync(ctx->enet, op.data(), sizeof(double) * kStdDoubles, cudaMemcpyHostToDevice, ctx->stream));
   if (int r = row_pass(
           ctx, X, x_dtype, nullptr, n_rows, d, ldx, mem_kind, nullptr,
-          [&](const RowSpan& s, void* sd, void* yd) {
+          [&](const RowSpan& s, void* sd, void* yd, void*) {
             return launch_score_std(ctx, s.X, x_dtype, s.rows, d, s.ldx, static_cast<double*>(yd),
                                     static_cast<double*>(sd));
           },
@@ -1449,17 +1451,11 @@ static int ensure_glm(b2_ctx* ctx) {
   return B2_OK;
 }
 
-// The checks the three entry points share, then the operands (w, step, b, db) into ctx->glm
-static int glm_setup(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, const void* X,
-                     const float* y, bool need_y, int link, double power, const double* coef, double intercept,
-                     const double* step, double step_intercept) {
+// The checks the GLM and logistic entry points share, then the operands (w, step, b, db, the two labels) into ctx->glm
+static int glm_operands(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, const void* X,
+                        const float* y, bool need_y, const double* coef, double intercept, const double* step,
+                        double step_intercept, double neg_label, double pos_label) {
   if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
-  if (link != B2_GLM_LOG && link != B2_GLM_IDENTITY) { set_error("link=%d must be B2_GLM_LOG or B2_GLM_IDENTITY", link); return B2_E_ARG; }
-  if (!isfinite(power)) { set_error("power=%g must be finite", power); return B2_E_ARG; }
-  if (link == B2_GLM_IDENTITY && power != 0.0) {
-    set_error("the identity link is supported at power 0 only (got power=%g)", power);
-    return B2_E_ARG;
-  }
   if (coef == nullptr) { set_error("coef is null"); return B2_E_ARG; }
   if (n_rows > 0 && (X == nullptr || (need_y && y == nullptr))) { set_error("X / y is null"); return B2_E_ARG; }
   if (ctx->n_ranks > 1) {
@@ -1472,17 +1468,52 @@ static int glm_setup(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ld
   if (step != nullptr) memcpy(op.data() + kGlmOpStep, step, sizeof(double) * d);
   op[kGlmOpMisc] = intercept;
   op[kGlmOpMisc + 1] = step_intercept;
+  op[kGlmOpMisc + 2] = neg_label;
+  op[kGlmOpMisc + 3] = pos_label;
   B2_CUDA(cudaMemcpyAsync(ctx->glm + kGlmOp, op.data(), sizeof(double) * op.size(), cudaMemcpyHostToDevice, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
   return B2_OK;
 }
 
+static int glm_setup(b2_ctx* ctx, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, const void* X,
+                     const float* y, bool need_y, int link, double power, const double* coef, double intercept,
+                     const double* step, double step_intercept) {
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (link != B2_GLM_LOG && link != B2_GLM_IDENTITY) { set_error("link=%d must be B2_GLM_LOG or B2_GLM_IDENTITY", link); return B2_E_ARG; }
+  if (!isfinite(power)) { set_error("power=%g must be finite", power); return B2_E_ARG; }
+  if (link == B2_GLM_IDENTITY && power != 0.0) {
+    set_error("the identity link is supported at power 0 only (got power=%g)", power);
+    return B2_E_ARG;
+  }
+  return glm_operands(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, need_y, coef, intercept, step, step_intercept, 0.0,
+                      0.0);
+}
+
 // One pass over the rows into ctx->glm (the first rows overwrite the sums, the others add to them)
 static int glm_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
-                    int mem_kind, const uint8_t* row_mask, int mask_keep, int mode, int link, double power, int n_steps) {
-  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*) {
-    return launch_glm(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, mode, link, power, n_steps, s.first);
+                    int mem_kind, const uint8_t* row_mask, int mask_keep, int mode, int family, int link, double power,
+                    int n_steps) {
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+    return launch_glm(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, mode, family, link, power, n_steps,
+                      s.first);
   });
+}
+
+// The sums of the last pass (and the mirrored Hessian when hess_out is not null) to the host: [0, 7) and the gradient
+// [7, 8 + d), then the extra scalars at 8 + d
+static int fetch_glm_sums(b2_ctx* ctx, int d, int n_extra, double* sums_out, double* hess_out) {
+  const int d1 = d + 1;
+  std::vector<double> h(hess_out != nullptr ? (size_t)kGlmPart : (size_t)kGlmHess);
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->glm, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, h.data(), sizeof(double) * 7);
+  memcpy(sums_out + 7, h.data() + kGlmGrad, sizeof(double) * d1);
+  if (n_extra > 0) sums_out[8 + d] = h[kGlmCorrect];
+  if (hess_out != nullptr)
+    for (int i = 0; i < d1; ++i)
+      for (int j = i; j < d1; ++j)       // the upper triangle, mirrored
+        hess_out[(size_t)i * d1 + j] = hess_out[(size_t)j * d1 + i] = h[kGlmHess + (size_t)i * kGlmHp + j];
+  return B2_OK;
 }
 
 int b2_glm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
@@ -1494,18 +1525,10 @@ int b2_glm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t
                         fit_intercept ? intercept : 0.0, nullptr, 0.0))
     return r;
   const int mode = hess_out != nullptr ? kGlmHessian : kGlmGradient;
-  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, mode, link, power, 0)) return r;
-  const int d1 = d + 1;
-  std::vector<double> h(hess_out != nullptr ? (size_t)kGlmPart : (size_t)kGlmHess);
-  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->glm, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  B2_CUDA(cudaStreamSynchronize(ctx->stream));
-  memcpy(sums_out, h.data(), sizeof(double) * 7);
-  memcpy(sums_out + 7, h.data() + kGlmGrad, sizeof(double) * d1);
-  if (hess_out != nullptr)
-    for (int i = 0; i < d1; ++i)
-      for (int j = i; j < d1; ++j)       // the upper triangle, mirrored
-        hess_out[(size_t)i * d1 + j] = hess_out[(size_t)j * d1 + i] = h[kGlmHess + (size_t)i * kGlmHp + j];
-  return B2_OK;
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, mode, kGlmTweedie, link, power,
+                       0))
+    return r;
+  return fetch_glm_sums(ctx, d, 0, sums_out, hess_out);
 }
 
 int b2_glm_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
@@ -1517,8 +1540,8 @@ int b2_glm_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, 
   if (int r = glm_setup(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, link, power, coef, intercept, step,
                         step_intercept))
     return r;
-  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, kGlmLadder, link, power,
-                       n_steps))
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, kGlmLadder, kGlmTweedie, link,
+                       power, n_steps))
     return r;
   B2_CUDA(cudaMemcpyAsync(loss_out, ctx->glm, sizeof(double) * n_steps, cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1535,12 +1558,116 @@ int b2_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int 
   if (n_rows == 0) return B2_OK;
   if (int r = row_pass(
           ctx, X, x_dtype, nullptr, n_rows, d, ldx, mem_kind, nullptr,
-          [&](const RowSpan& s, void* mu, void*) {
+          [&](const RowSpan& s, void* mu, void*, void*) {
             return launch_glm_predict(ctx, s.X, x_dtype, s.rows, d, s.ldx, link, static_cast<double*>(mu));
           },
           RowOut{mu_out, sizeof(double)}))
     return r;
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+// ---- LogisticRegression (DESIGN.md section 11) ----------------------------------------------------------------------
+// The labels are fp32 values: finite, distinct and exactly representable in fp32
+static int check_labels(double neg_label, double pos_label) {
+  if (!isfinite(neg_label) || !isfinite(pos_label) || (double)(float)neg_label != neg_label ||
+      (double)(float)pos_label != pos_label || neg_label == pos_label) {
+    set_error("neg_label=%g / pos_label=%g must be two distinct finite fp32 values", neg_label, pos_label);
+    return B2_E_ARG;
+  }
+  return B2_OK;
+}
+
+int b2_logistic_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const uint8_t* row_mask, int mask_keep, double neg_label, double pos_label,
+                     const double* coef, double intercept, int fit_intercept, double* sums_out, double* hess_out) {
+  if (int r = use_device(ctx)) return r;
+  if (sums_out == nullptr) { set_error("sums_out is null"); return B2_E_ARG; }
+  if (int r = check_labels(neg_label, pos_label)) return r;
+  if (int r = glm_operands(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, coef, fit_intercept ? intercept : 0.0,
+                           nullptr, 0.0, neg_label, pos_label))
+    return r;
+  const int mode = hess_out != nullptr ? kGlmHessian : kGlmGradient;
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, mode, kGlmBinomial, 0, 0.0, 0))
+    return r;
+  return fetch_glm_sums(ctx, d, 1, sums_out, hess_out);
+}
+
+int b2_logistic_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d,
+                            int64_t ldx, int mem_kind, const uint8_t* row_mask, int mask_keep, double neg_label,
+                            double pos_label, const double* coef, double intercept, const double* step,
+                            double step_intercept, int n_steps, double* loss_out) {
+  if (int r = use_device(ctx)) return r;
+  if (step == nullptr || loss_out == nullptr) { set_error("step / loss_out is null"); return B2_E_ARG; }
+  if (n_steps < 1 || n_steps > kGlmSteps) { set_error("n_steps=%d out of range [1,%d]", n_steps, kGlmSteps); return B2_E_ARG; }
+  if (int r = check_labels(neg_label, pos_label)) return r;
+  if (int r = glm_operands(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, coef, intercept, step, step_intercept,
+                           neg_label, pos_label))
+    return r;
+  if (int r = glm_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, kGlmLadder, kGlmBinomial, 0,
+                       0.0, n_steps))
+    return r;
+  B2_CUDA(cudaMemcpyAsync(loss_out, ctx->glm, sizeof(double) * n_steps, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+int b2_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+                        const double* coef, double intercept, double neg_label, double pos_label, double* decision_out,
+                        double* proba_out, float* label_out) {
+  if (int r = use_device(ctx)) return r;
+  if (decision_out == nullptr && proba_out == nullptr && label_out == nullptr) {
+    set_error("decision_out, proba_out and label_out are all null");
+    return B2_E_ARG;
+  }
+  if (int r = check_labels(neg_label, pos_label)) return r;
+  if (int r = glm_operands(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, nullptr, false, coef, intercept, nullptr, 0.0,
+                           neg_label, pos_label))
+    return r;
+  if (n_rows == 0) return B2_OK;
+  if (int r = row_pass(
+          ctx, X, x_dtype, nullptr, n_rows, d, ldx, mem_kind, nullptr,
+          [&](const RowSpan& s, void* dec, void* pr, void* lab) {
+            return launch_logistic_predict(ctx, s.X, x_dtype, s.rows, d, s.ldx, static_cast<double*>(dec),
+                                           static_cast<double*>(pr), static_cast<float*>(lab));
+          },
+          RowOut{decision_out, sizeof(double)}, RowOut{proba_out, 2 * sizeof(double)},
+          RowOut{label_out, sizeof(float)}))
+    return r;
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep,
+                  double* stats_out) {
+  if (int r = use_device(ctx)) return r;
+  if (stats_out == nullptr) { set_error("stats_out is null"); return B2_E_ARG; }
+  if (n_rows < 0 || (n_rows > 0 && y == nullptr)) { set_error("n_rows=%lld / y is null", (long long)n_rows); return B2_E_ARG; }
+  if (ctx->n_ranks > 1) {
+    set_error("the label scan runs on one rank only (its counts are not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (int r = ensure_glm(ctx)) return r;
+  unsigned long long* st = reinterpret_cast<unsigned long long*>(ctx->glm_part);
+  if (int r = launch_label_scan(ctx, y, n_rows, row_mask, mask_keep, st)) return r;
+  unsigned long long h[kLabelWords];
+  B2_CUDA(cudaMemcpyAsync(h, st, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const bool any = h[kLabelMin] <= h[kLabelMax];     // some kept y is finite
+  auto value = [](unsigned long long k) {            // the inverse of the kernel's order-preserving key
+    uint32_t u = (uint32_t)k;
+    u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+    float f;
+    memcpy(&f, &u, sizeof(f));
+    return (double)f;
+  };
+  stats_out[0] = (double)h[kLabelKept];
+  stats_out[1] = (double)h[kLabelNonFinite];
+  stats_out[2] = (double)h[kLabelNonIntegral];
+  stats_out[3] = any ? value(h[kLabelMin]) : NAN;
+  stats_out[4] = any ? value(h[kLabelMax]) : NAN;
+  stats_out[5] = (double)h[kLabelNMin];
+  stats_out[6] = (double)h[kLabelNMax];
   return B2_OK;
 }
 
@@ -1569,7 +1696,7 @@ int b2_score(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int
     B2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * kNStats, ctx->stream));
   } else if (int r = row_pass(
                  ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask,
-                 [&](const RowSpan& s, void* yh, void*) {
+                 [&](const RowSpan& s, void* yh, void*, void*) {
                    return launch_score(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep,
                                        static_cast<float*>(yh), s.first);
                  },

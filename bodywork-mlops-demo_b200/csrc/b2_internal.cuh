@@ -121,7 +121,8 @@ struct BayesArgs {
 
 // ---- the generalised linear regressors (glm.cu; DESIGN.md section 10) -------------------------------------------------
 // ctx->glm: the reduced sums [kGlmPart] of the last pass, then the operands at kGlmOp: w [kMaxD], the Newton step [kMaxD],
-// [b, db].  The sums: [0] loss [1] const [2] sum y [3] rows kept [4] y out of range [5] h <= 0 [6] y not finite, the
+// [b, db, negative label, positive label].  The sums: [0] loss [1] const [2] sum y [3] rows kept [4] y out of range
+// [5] h <= 0 [6] y not finite [7] (logistic passes) rows classified correctly, the
 // gradient sum g x_j at kGlmGrad + j (sum g at kGlmGrad + d), the Hessian sum |h| z_i z_j (z = [x 1]) at kGlmHess +
 // i kGlmHp + j, i <= j; a line search leaves the loss at step k in [k].  ctx->glm_part holds one kGlmPart per CTA, for
 // up to two CTAs per SM.
@@ -134,6 +135,11 @@ constexpr int kGlmOp = kGlmPart;
 constexpr int kGlmOpW = 0, kGlmOpStep = kMaxD, kGlmOpMisc = 2 * kMaxD;
 constexpr int kGlmDoubles = kGlmOp + 2 * kMaxD + 8;
 enum GlmMode { kGlmGradient = 0, kGlmHessian = 1, kGlmLadder = 2 };   // what a pass computes
+enum GlmFamily { kGlmTweedie = 0, kGlmBinomial = 1 };                 // the loss: half-Tweedie (link, power) or half-binomial
+constexpr int kGlmCorrect = 7;
+// b2_label_scan's counters (unsigned long long, in ctx->glm_part): the extremes as order-preserving keys of the fp32 value
+enum LabelWord { kLabelKept = 0, kLabelNonFinite, kLabelNonIntegral, kLabelMin, kLabelMax, kLabelNMin, kLabelNMax,
+                 kLabelWords };
 
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
@@ -395,12 +401,19 @@ int launch_ard(b2_ctx* ctx, const BayesArgs& args);
 // ystd (and yhat when not null) of the rows [0, n): sqrt(max((x - m)^T sigma (x - m), 0) + noise_var) and x.w + b, from
 // the operands at ctx->enet (kStd* in score_std.cu, written by the caller)
 int launch_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* yhat, double* ystd);
-// one pass of the GLM regressors over the rows [0, n) at the operands of ctx->glm (mode: GlmMode; kGlmLadder takes the
-// n_steps losses), then the ordered reduce of the per-CTA sums into ctx->glm (`first_block` overwrites, otherwise adds)
+// one pass of the GLM regressors or the logistic fits over the rows [0, n) at the operands of ctx->glm (mode: GlmMode;
+// kGlmLadder takes the n_steps losses; family: GlmFamily, link and power for kGlmTweedie), then the ordered reduce of the
+// per-CTA sums into ctx->glm (`first_block` overwrites, otherwise adds)
 int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
-               const uint8_t* mask, int keep, int mode, int link, double power, int n_steps, bool first_block);
+               const uint8_t* mask, int keep, int mode, int family, int link, double power, int n_steps,
+               bool first_block);
 // mu of the rows [0, n): exp(x.w + b) (B2_GLM_LOG) or x.w + b, fp64
 int launch_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, int link, double* mu);
+// the logistic model of ctx->glm on the rows [0, n): eta (fp64), [1 - p, p] (fp64) and the label (fp32), each if not null
+int launch_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* decision,
+                            double* proba, float* label);
+// the kLabelWords counters of the kept rows of device y into st (two launches after two memsets)
+int launch_label_scan(b2_ctx* ctx, const float* y, int64_t n, const uint8_t* mask, int keep, unsigned long long* st);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

@@ -1,5 +1,5 @@
 // glm.cu -- the row passes of the generalised linear regressors (b2_glm_pass, b2_glm_line_search, b2_glm_predict;
-// DESIGN.md section 10).
+// DESIGN.md section 10) and of binary logistic regression (b2_logistic_*, b2_label_scan; DESIGN.md section 11).
 //
 // scikit-learn's Newton solver (solver="newton-cholesky") needs, at the coefficients w, b of each iteration and with
 // eta = x.w + b per kept row, the half-Tweedie loss, its gradient g and Hessian h (loss(y, eta) and its derivatives in
@@ -99,6 +99,39 @@ __device__ __forceinline__ double glm_const(int link, double p, double y) {
   return pow(fmax(y, 0.0), 2.0 - p) / (1.0 - p) / (2.0 - p);
 }
 
+// The half-binomial loss of the logistic fits (sklearn's HalfBinomialLoss), t = 1 for the positive label, 0 otherwise.
+// closs_half_binomial: log1pexp(eta) - t eta, log1pexp with sklearn's branches
+__device__ __forceinline__ double binom_loss(double t, double eta) {
+  double l;
+  if (eta <= -37.0) l = exp(eta);
+  else if (eta <= -2.0) l = log1p(exp(eta));
+  else if (eta <= 18.0) l = log(1.0 + exp(eta));
+  else if (eta <= 33.3) l = eta + exp(-eta);
+  else l = eta;
+  return l - t * eta;
+}
+
+// the loss of closs_grad_half_binomial: sklearn's line search evaluates loss_gradient, whose loss is written this way
+__device__ __forceinline__ double binom_ladder_loss(double t, double eta) {
+  if (eta <= -37.0) return exp(eta) - t * eta;
+  if (eta <= -2.0) return log1p(exp(eta)) - t * eta;
+  if (eta <= 18.0) return log1p(exp(-eta)) + (1.0 - t) * eta;
+  return exp(-eta) + (1.0 - t) * eta;
+}
+
+// cgrad_hess_half_binomial: g = expit(eta) - t, h = expit(eta) (1 - expit(eta)), exp(eta) to first order below -37
+__device__ __forceinline__ void binom_grad_hess(double t, double eta, double& g, double& h) {
+  if (eta > -37.0) {
+    const double e = exp(-eta);
+    g = ((1.0 - t) - t * e) / (1.0 + e);
+    h = e / ((1.0 + e) * (1.0 + e));
+  } else {
+    const double e = exp(eta);
+    g = e - t;
+    h = e;
+  }
+}
+
 // y inside the loss's interval: (-inf, inf) for p <= 0, [0, inf) for 0 < p < 2, (0, inf) for p >= 2
 __device__ __forceinline__ bool glm_y_in_range(double p, double y) {
   const bool low = p <= 0.0 ? y > -INFINITY : (p < 2.0 ? y >= 0.0 : y > 0.0);
@@ -107,8 +140,12 @@ __device__ __forceinline__ bool glm_y_in_range(double p, double y) {
 
 // MODE kGlmGradient / kGlmHessian: per-CTA [loss, const, sum y, kept, y out of range, h <= 0, y not finite, 0 | g.x (d), sum g,
 // zeros | (kGlmHessian) the Hessian blocks at kGlmHess, pitch kGlmHp]; kGlmLadder: the loss at step k in [k], k < n_steps.
-// op: w [kMaxD], step [kMaxD], [b, db] (kGlmOp* in b2_internal.cuh).
-template <typename T, bool RING, int MODE>
+// op: w [kMaxD], step [kMaxD], [b, db, negative label, positive label] (kGlmOp* in b2_internal.cuh).
+// FAM kGlmTweedie: link and power select the loss.  kGlmBinomial: the half-binomial loss on the labels of op (link and
+// power unused); sum y counts the positive rows, y out of range the rows with neither label, and slot 7 the rows
+// classified correctly ((eta > 0) == positive label, a row with neither label never).  A compile-time family keeps the
+// Tweedie instantiations as they were.
+template <typename T, bool RING, int MODE, int FAM>
 __global__ void __launch_bounds__(kGlmThreads, 1)
 glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
            const uint8_t* __restrict__ mask, int keep, const double* __restrict__ op, int link, double power,
@@ -223,7 +260,11 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
         const double t = ldexp(1.0, -lane);           // t = 1, 1/2, ... 2^-20: lane k < n_steps takes step k
 #pragma unroll
         for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
-          const double l = glm_loss(link, power, yv[warp + kGlmWarps * u], eta[u] + t * deta[u]);
+          double l;
+          if constexpr (FAM == kGlmBinomial)
+            l = binom_ladder_loss(yv[warp + kGlmWarps * u] == op[kGlmOpMisc + 3] ? 1.0 : 0.0, eta[u] + t * deta[u]);
+          else
+            l = glm_loss(link, power, yv[warp + kGlmWarps * u], eta[u] + t * deta[u]);
           s_loss += (use[u] && lane < n_steps) ? l : 0.0;
         }
       } else {
@@ -238,16 +279,30 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
           const int r = warp + kGlmWarps * lane;
           const double yy = yv[r];
           double l, gg, hh;
-          glm_point(link, power, yy, e, l, gg, hh);
-          const double cst = glm_const(link, power, yy);
           double* ls = lsum + (warp * 4 + lane) * 8;
-          ls[0] += kept ? l : 0.0;
-          ls[1] += kept ? cst : 0.0;
-          ls[2] += kept ? yy : 0.0;
-          ls[3] += kept ? 1.0 : 0.0;
-          ls[4] += (kept && !glm_y_in_range(power, yy)) ? 1.0 : 0.0;
-          ls[5] += (kept && hh <= 0.0) ? 1.0 : 0.0;
-          ls[6] += (kept && !isfinite(yy)) ? 1.0 : 0.0;
+          if constexpr (FAM == kGlmBinomial) {
+            const bool is_pos = yy == op[kGlmOpMisc + 3], in_range = is_pos || yy == op[kGlmOpMisc + 2];
+            const double tt = is_pos ? 1.0 : 0.0;
+            l = binom_loss(tt, e);
+            binom_grad_hess(tt, e, gg, hh);
+            ls[0] += kept ? l : 0.0;
+            ls[2] += kept ? tt : 0.0;
+            ls[3] += kept ? 1.0 : 0.0;
+            ls[4] += (kept && !in_range) ? 1.0 : 0.0;
+            ls[5] += (kept && hh <= 0.0) ? 1.0 : 0.0;
+            ls[6] += (kept && !isfinite(yy)) ? 1.0 : 0.0;
+            ls[kGlmCorrect] += (kept && in_range && (e > 0.0) == is_pos) ? 1.0 : 0.0;
+          } else {
+            glm_point(link, power, yy, e, l, gg, hh);
+            const double cst = glm_const(link, power, yy);
+            ls[0] += kept ? l : 0.0;
+            ls[1] += kept ? cst : 0.0;
+            ls[2] += kept ? yy : 0.0;
+            ls[3] += kept ? 1.0 : 0.0;
+            ls[4] += (kept && !glm_y_in_range(power, yy)) ? 1.0 : 0.0;
+            ls[5] += (kept && hh <= 0.0) ? 1.0 : 0.0;
+            ls[6] += (kept && !isfinite(yy)) ? 1.0 : 0.0;
+          }
           gs[r] = kept ? gg : 0.0;
           hs[r] = kept ? fabs(hh) : 0.0;
         }
@@ -303,7 +358,7 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     __syncthreads();
     if (tid < kGlmHess) {                          // the scalars, the gradient, zeros in the unused entries
       double r = 0.0;
-      if (tid < 7)
+      if (tid < (FAM == kGlmBinomial ? kGlmCorrect + 1 : 7))
         for (int q = 0; q < kGlmWarps * 4; ++q) r += lsum[q * 8 + tid];
       else if (tid >= kGlmGrad && tid <= kGlmGrad + d)
         r = gsum[tid - kGlmGrad];
@@ -349,13 +404,119 @@ glm_predict_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
   }
 }
 
+// The logistic model's outputs per row, eta = x.w + b in fp64: one warp per row.  Each output may be null: eta; the
+// probabilities [1 - p, p] with p = 1 / (1 + exp(-eta)) (scipy's expit, as sklearn's _predict_proba_lr computes it); the
+// label, the positive one when eta > 0.
+template <typename T>
+__global__ void __launch_bounds__(256)
+logistic_predict_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const double* __restrict__ op,
+                        double* __restrict__ decision, double* __restrict__ proba, float* __restrict__ label) {
+  __shared__ double wv[kMaxD];
+  for (int t = threadIdx.x; t < kMaxD; t += blockDim.x) wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
+  __syncthreads();
+  const double b = op[kGlmOpMisc];
+  const float neg = (float)op[kGlmOpMisc + 2], pos = (float)op[kGlmOpMisc + 3];
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < n; row += warps) {
+    const T* xr = X + row * ldx;
+    double a = 0.0;
+    for (int j = lane; j < d; j += 32) a = fma((double)ld_row_val<T>(xr + j), wv[j], a);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) {
+      const double eta = a + b;
+      if (decision != nullptr) decision[row] = eta;
+      if (proba != nullptr) {
+        const double p = 1.0 / (1.0 + exp(-eta));
+        proba[2 * row] = 1.0 - p;
+        proba[2 * row + 1] = p;
+      }
+      if (label != nullptr) label[row] = eta > 0.0 ? pos : neg;
+    }
+  }
+}
+
+// The label scan of a device fp32 y over its kept rows (kLabel* in b2_internal.cuh): counts by integer atomics and the
+// extremes by atomics on order-preserving keys, so the result does not depend on the order of the rows.
+__device__ __forceinline__ unsigned long long label_key(float v) {   // monotone in v for finite v
+  const uint32_t u = __float_as_uint(v);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float label_of_key(unsigned long long k) {
+  const uint32_t u = (uint32_t)k;
+  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// pass 1: kept, not finite, finite but not integral, the smallest and largest key of the finite kept y
+__global__ void __launch_bounds__(256)
+label_scan_kernel(const float* __restrict__ y, int64_t n, const uint8_t* __restrict__ mask, int keep,
+                  unsigned long long* __restrict__ st) {
+  unsigned long long kept = 0, nonfinite = 0, nonint = 0, kmin = ~0ull, kmax = 0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (mask != nullptr && __ldg(mask + i) != (uint8_t)keep) continue;
+    const float v = __ldg(y + i);
+    ++kept;
+    if (!isfinite(v)) { ++nonfinite; continue; }
+    nonint += v != rintf(v);
+    const unsigned long long k = label_key(v);
+    kmin = k < kmin ? k : kmin;
+    kmax = k > kmax ? k : kmax;
+  }
+  kept = warp_sum_u64(kept);
+  nonfinite = warp_sum_u64(nonfinite);
+  nonint = warp_sum_u64(nonint);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long a = __shfl_xor_sync(0xffffffffu, kmin, o), c = __shfl_xor_sync(0xffffffffu, kmax, o);
+    kmin = a < kmin ? a : kmin;
+    kmax = c > kmax ? c : kmax;
+  }
+  if ((threadIdx.x & 31) == 0 && kept > 0) {
+    atomicAdd(st + kLabelKept, kept);
+    atomicAdd(st + kLabelNonFinite, nonfinite);
+    atomicAdd(st + kLabelNonIntegral, nonint);
+    atomicMin(st + kLabelMin, kmin);
+    atomicMax(st + kLabelMax, kmax);
+  }
+}
+
+// pass 2: the kept rows equal to the smallest and to the largest value
+__global__ void __launch_bounds__(256)
+label_count_kernel(const float* __restrict__ y, int64_t n, const uint8_t* __restrict__ mask, int keep,
+                   unsigned long long* __restrict__ st) {
+  if (st[kLabelMin] > st[kLabelMax]) return;            // no finite kept y
+  const float lo = label_of_key(st[kLabelMin]), hi = label_of_key(st[kLabelMax]);
+  unsigned long long n_lo = 0, n_hi = 0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (mask != nullptr && __ldg(mask + i) != (uint8_t)keep) continue;
+    const float v = __ldg(y + i);
+    n_lo += v == lo;
+    n_hi += v == hi;
+  }
+  n_lo = warp_sum_u64(n_lo);
+  n_hi = warp_sum_u64(n_hi);
+  if ((threadIdx.x & 31) == 0) {
+    if (n_lo > 0) atomicAdd(st + kLabelNMin, n_lo);
+    if (n_hi > 0) atomicAdd(st + kLabelNMax, n_hi);
+  }
+}
+
 }  // namespace
 
 // The rows [0, n) in the launches of scoring's plan: whole 32-row tiles of what plan_rows streams through the ring go to the
 // ring flavour, the rest (or every row of another layout) to the direct one; each launch is followed by its ordered reduce
 // into ctx->glm (`first_block` overwrites, otherwise adds).
 int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
-               const uint8_t* mask, int keep, int mode, int link, double power, int n_steps, bool first_block) {
+               const uint8_t* mask, int keep, int mode, int family, int link, double power, int n_steps,
+               bool first_block) {
   return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kGlmRows, first_block, [&](bool ring, const RowSpan& s) {
     // two CTAs per SM hide the latency of the per-tile steps where the shared memory allows it (all but the Hessian)
     const int64_t n_tiles = (s.rows + kGlmRows - 1) / kGlmRows, cap = (int64_t)ctx->sm_count * (mode == kGlmHessian ? 1 : 2);
@@ -365,11 +526,13 @@ int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
     const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
       return with_int<kGlmGradient, kGlmHessian, kGlmLadder>(mode, [&](auto M) {
-        constexpr int MODE = decltype(M)::value;
-        auto kernel = ring ? glm_kernel<T, true, MODE> : glm_kernel<T, false, MODE>;
-        return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, s.rows, d, ldx, s.y,
-                           s.mask, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
-                           ctx->glm_part);
+        return with_int<kGlmTweedie, kGlmBinomial>(family, [&](auto F) {
+          constexpr int MODE = decltype(M)::value, FAM = decltype(F)::value;
+          auto kernel = ring ? glm_kernel<T, true, MODE, FAM> : glm_kernel<T, false, MODE, FAM>;
+          return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, s.rows, d, ldx,
+                             s.y, s.mask, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
+                             ctx->glm_part);
+        });
       });
     });
     if (rc != B2_OK) return rc;
@@ -389,6 +552,34 @@ int launch_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d
   });
   B2_CUDA(cudaGetLastError());
   ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, double* decision,
+                            double* proba, float* label) {
+  if (n == 0) return B2_OK;
+  const int64_t want = (n + 7) / 8, cap = (int64_t)ctx->sm_count * 8;
+  const int grid = (int)(want < cap ? want : cap);
+  with_rows(x_dtype, X, [&](auto* Xr) {
+    logistic_predict_kernel<<<grid, 256, 0, ctx->stream>>>(Xr, n, d, ldx, ctx->glm + kGlmOp, decision, proba, label);
+    return B2_OK;
+  });
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_label_scan(b2_ctx* ctx, const float* y, int64_t n, const uint8_t* mask, int keep, unsigned long long* st) {
+  B2_CUDA(cudaMemsetAsync(st, 0, sizeof(unsigned long long) * kLabelWords, ctx->stream));
+  B2_CUDA(cudaMemsetAsync(st + kLabelMin, 0xff, sizeof(unsigned long long), ctx->stream));
+  if (n == 0) return B2_OK;
+  const int64_t want = (n + 2047) / 2048, cap = (int64_t)ctx->sm_count * 8;
+  const int grid = (int)(want < cap ? want : cap);
+  label_scan_kernel<<<grid, 256, 0, ctx->stream>>>(y, n, mask, keep, st);
+  B2_CUDA(cudaGetLastError());
+  label_count_kernel<<<grid, 256, 0, ctx->stream>>>(y, n, mask, keep, st);
+  B2_CUDA(cudaGetLastError());
+  ctx->launches += 2;
   return B2_OK;
 }
 

@@ -1028,8 +1028,37 @@ class _B200GLM:
         ctx = self.ctx
         X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
         d = X.shape[1]
+        fi = bool(self.fit_intercept)
+
+        def run(c, hessian):
+            return ctx.glm_pass(X, y, c[:d], float(c[d]) if fi else 0.0, link=link, power=power, row_mask=row_mask,
+                                mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
+
+        def line_search(c, step):
+            return ctx.glm_line_search(X, y, c[:d], float(c[d]) if fi else 0.0, step[:d],
+                                       float(step[d]) if fi else 0.0, link=link, power=power,
+                                       n_steps=native.GLM_STEPS, row_mask=row_mask, mask_keep=mask_keep)
+
+        def start():                              # the first pass checks y; the intercept starts at link(mean y)
+            coef, warm = self._start_coef(d)
+            first = run(coef, warm)
+            n = first["kept"]
+            if n == 0:
+                raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
+                                 f"B200{self._sk_name}.")
+            if first["y_nonfinite"] > 0 or not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
+                raise ValueError(_NAN_MESSAGE)
+            if first["y_out_of_range"] > 0:
+                raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
+            if warm:
+                return coef, first, n
+            if fi:
+                ybar = first["sum_y"] / n
+                coef[-1] = np.log(ybar) if link == native.GLM_LOG else ybar
+            return coef, run(coef, True), n
+
         try:
-            coef, n_iter = self._newton(ctx, X, y, row_mask, mask_keep, d, link, power, loss_name)
+            coef, n_iter = self._newton(d, float(self.alpha), start, run, line_search)
         finally:
             for a in owned:
                 a.free()
@@ -1041,18 +1070,29 @@ class _B200GLM:
         self.n_features_in_ = int(d)
         return self
 
-    def _newton(self, ctx, X, y, row_mask, mask_keep, d, link, power, loss_name):
-        """NewtonSolver.solve (NewtonCholeskySolver) step by step; returns (coef with the intercept last, n_iter)."""
+    def _start_coef(self, d):
+        """(the starting coefficients with the intercept last, zeros unless warm_start finds a fit; warm)"""
+        fi = bool(self.fit_intercept)
+        warm = bool(self.warm_start) and getattr(self, "coef_", None) is not None
+        if not warm:
+            return np.zeros(d + int(fi)), False
+        coef = np.asarray(self.coef_, dtype=np.float64).ravel().copy()
+        if coef.size != d:
+            raise ValueError(f"X has {d} features, but the warm start coef_ has {coef.size}")
+        if fi:
+            coef = np.concatenate([coef, [float(np.ravel(self.intercept_)[0])]])
+        return coef, True
+
+    def _newton(self, d, alpha, start, run, line_search):
+        """NewtonSolver.solve (NewtonCholeskySolver) step by step on the caller's passes: start() -> (coef, the pass
+        with the Hessian at coef, the kept rows), run(coef, hessian) -> the pass sums at coef, line_search(coef, step)
+        -> the loss sums of the 21 ladder steps.  Returns (coef with the intercept last, n_iter)."""
         import scipy.linalg
         import scipy.optimize
         from sklearn.exceptions import ConvergenceWarning
         from sklearn.utils.optimize import _check_optimize_result
-        fi, alpha, tol, max_iter = bool(self.fit_intercept), float(self.alpha), float(self.tol), int(self.max_iter)
+        fi, tol, max_iter = bool(self.fit_intercept), float(self.tol), int(self.max_iter)
         n_dof = d + int(fi)
-
-        def run(c, hessian):
-            return ctx.glm_pass(X, y, c[:d], float(c[d]) if fi else 0.0, link=link, power=power, row_mask=row_mask,
-                                mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
 
         def loss_of(c, loss_sum):                 # LinearModelLoss.loss: mean loss + alpha / 2 |w|^2
             w = c[:d]
@@ -1065,31 +1105,7 @@ class _B200GLM:
                 g[d] = s["grad"][d] / n
             return g
 
-        warm = bool(self.warm_start) and getattr(self, "coef_", None) is not None
-        if warm:
-            coef = np.asarray(self.coef_, dtype=np.float64).ravel().copy()
-            if coef.size != d:
-                raise ValueError(f"X has {d} features, but the warm start coef_ has {coef.size}")
-            if fi:
-                coef = np.concatenate([coef, [float(self.intercept_)]])
-        else:
-            coef = np.zeros(n_dof)
-        first = run(coef, warm)
-        n = first["kept"]
-        if n == 0:
-            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
-                             f"B200{self._sk_name}.")
-        if first["y_nonfinite"] > 0 or not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
-            raise ValueError(_NAN_MESSAGE)
-        if first["y_out_of_range"] > 0:
-            raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
-        if warm:
-            cur = first
-        else:
-            if fi:
-                ybar = first["sum_y"] / n
-                coef[-1] = np.log(ybar) if link == native.GLM_LOG else ybar
-            cur = run(coef, True)
+        coef, cur, n = start()
         loss_value = loss_of(coef, cur["loss"])
 
         beta, sigma = 0.5, 0.00048828125
@@ -1127,9 +1143,7 @@ class _B200GLM:
                 fallback = True
                 break
             # line search: every candidate step from one pass
-            ladder = ctx.glm_line_search(X, y, coef[:d], float(coef[d]) if fi else 0.0, coef_newton[:d],
-                                         float(coef_newton[d]) if fi else 0.0, link=link, power=power,
-                                         n_steps=native.GLM_STEPS, row_mask=row_mask, mask_keep=mask_keep)
+            ladder = line_search(coef, coef_newton)
             armijo_term = sigma * gradient_times_newton
             coef_old, loss_value_old, gradient_old = coef, loss_value, gradient
             sum_abs_grad_old = -1
@@ -1305,3 +1319,253 @@ class B200TweedieRegressor(_B200GLM):
 
     def __repr__(self) -> str:
         return f"B200TweedieRegressor(power={self.power}, alpha={self.alpha}, link={self.link!r})"
+
+
+# ---- LogisticRegression, binary: Newton fits on the GLM passes with the half-binomial loss (DESIGN.md section 11) -----
+_CONTINUOUS_MESSAGE = ("Unknown label type: continuous. Maybe you are trying to fit a classifier, which expects discrete "
+                       "classes on a regression target with continuous values.")
+
+
+def _one_class_message(c) -> str:
+    return ("This solver needs samples of at least 2 classes in the data, but the data contains only one class: "
+            f"{c!r}")
+
+
+def _fp32_exact(v) -> bool:
+    try:
+        f = float(v)
+    except (TypeError, ValueError):
+        return False
+    return bool(np.isfinite(f)) and float(np.float32(f)) == f
+
+
+class B200LogisticRegression(_B200GLM):
+    """``sklearn.linear_model.LogisticRegression(solver="newton-cholesky")`` for two classes, fitted on the H100.  The
+    Newton iteration is the GLM regressors' (``_B200GLM._newton``) on the half-binomial loss: one pass for the loss,
+    gradient and fp64 Hessian and one pass for the 21 line-search steps, from zeros (or the last fit with warm_start),
+    with the L2 strength 1 / (C n) over the n kept rows (0 at C = inf).
+
+    Labels: host y of any dtype (``classes_`` is ``np.unique`` over the kept rows; y is mapped to {0, 1} before staging),
+    or an f32 ``DeviceArray`` scanned on the device (``classes_`` are its two fp32 values, the passes read y as stored).
+    Refused: more than two classes (multinomial fits are not supported), l1_ratio != 0, class_weight, sample_weight and
+    any solver but 'newton-cholesky'.  verbose is accepted and has no effect."""
+    _sk_name = "LogisticRegression"
+
+    def __init__(self, *, C: float = 1.0, l1_ratio: float = 0.0, tol: float = 1e-4, fit_intercept: bool = True,
+                 class_weight=None, solver: str = "newton-cholesky", max_iter: int = 100, verbose: int = 0,
+                 warm_start: bool = False, ctx: Optional[native.Context] = None):
+        self.C = C
+        self.l1_ratio = l1_ratio
+        self.tol = tol
+        self.fit_intercept = fit_intercept
+        self.class_weight = class_weight
+        self.solver = solver
+        self.max_iter = max_iter
+        self.verbose = verbose
+        self.warm_start = warm_start
+        self._ctx = ctx
+
+    def _check_params(self):
+        if self.solver != "newton-cholesky":
+            raise ValueError(f"solver={self.solver!r} is not supported: B200LogisticRegression runs scikit-learn's "
+                             "'newton-cholesky' solver (L-BFGS-B runs only as its fallback)")
+        C = self.C
+        if isinstance(C, bool) or not isinstance(C, (int, float, np.integer, np.floating)) or not C > 0:
+            raise ValueError(f"The 'C' parameter of LogisticRegression must be a float in the range (0.0, inf]. "
+                             f"Got {C!r} instead.")
+        if self.l1_ratio != 0:
+            raise ValueError(f"l1_ratio={self.l1_ratio!r} is not supported: B200LogisticRegression fits the L2 penalty "
+                             "only (l1_ratio=0)")
+        if self.class_weight is not None:
+            raise ValueError("class_weight is not supported by B200LogisticRegression: every kept row has weight 1")
+        if isinstance(self.max_iter, bool) or not isinstance(self.max_iter, (int, np.integer)) or self.max_iter < 0:
+            raise ValueError(f"The 'max_iter' parameter of LogisticRegression must be an int in the range [0, inf). "
+                             f"Got {self.max_iter!r} instead.")
+        if not (np.isfinite(self.tol) and self.tol >= 0):
+            raise ValueError(f"The 'tol' parameter of LogisticRegression must be a float in the range [0.0, inf). "
+                             f"Got {self.tol!r} instead.")
+
+    @staticmethod
+    def _host_labels(y, row_mask, mask_keep):
+        """(classes_, y as float32 {0, 1}, kept rows) of host y, with scikit-learn's checks on the kept rows"""
+        from sklearn.utils.multiclass import check_classification_targets
+        y = np.asarray(y)
+        if y.ndim == 2 and y.shape[1] == 1:
+            y = y.ravel()
+        if y.ndim != 1:
+            raise ValueError(f"y should be a 1d array, got an array of shape {y.shape} instead.")
+        if isinstance(row_mask, native.DeviceArray):
+            row_mask = row_mask.to_host()
+        kept = y if row_mask is None else y[np.asarray(row_mask).ravel() == mask_keep]
+        if kept.size == 0:
+            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required by "
+                             "B200LogisticRegression.")
+        if kept.dtype.kind in "fc":
+            if np.isnan(kept).any():
+                raise ValueError("Input y contains NaN.")
+            if np.isinf(kept).any():
+                raise ValueError(f"Input y contains infinity or a value too large for {kept.dtype!r}.")
+        check_classification_targets(kept)
+        classes = np.unique(kept)
+        if classes.size < 2:
+            raise ValueError(_one_class_message(classes[0]))
+        if classes.size > 2:
+            raise ValueError(f"B200LogisticRegression fits two classes only, y has {classes.size}: multinomial fits are "
+                             "not supported")
+        return classes, (y == classes[1]).astype(np.float32), int(kept.size)
+
+    @staticmethod
+    def _device_labels(ctx, y, row_mask, mask_keep):
+        """(classes_ (fp32), kept rows) of an f32 DeviceArray y, from one label scan on the device"""
+        st = ctx.label_scan(y, row_mask, mask_keep)
+        if st["kept"] == 0:
+            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required by "
+                             "B200LogisticRegression.")
+        if st["nonfinite"] > 0:
+            raise ValueError("Input y contains NaN or infinity.")
+        if st["nonintegral"] > 0:
+            raise ValueError(_CONTINUOUS_MESSAGE)
+        if st["min"] == st["max"]:
+            raise ValueError(_one_class_message(np.float32(st["min"])))
+        if st["n_min"] + st["n_max"] != st["kept"]:
+            raise ValueError("B200LogisticRegression fits two classes only, y has more than two: multinomial fits are "
+                             "not supported")
+        return np.array([st["min"], st["max"]], dtype=np.float32), int(st["kept"])
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None):
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); y: host labels of
+        any dtype or an f32 ``DeviceArray``; ``row_mask`` (uint8 per row) restricts the fit to rows equal to
+        ``mask_keep``.  Sets coef_ (1, D), intercept_ (1,), classes_, n_iter_ (1,) and n_features_in_."""
+        if sample_weight is not None:
+            raise ValueError("sample_weight is not supported by B200LogisticRegression: every kept row has weight 1")
+        self._check_params()
+        ctx = self.ctx
+        owned = []
+        try:
+            if isinstance(y, native.DeviceArray):
+                if not isinstance(X, native.DeviceArray):
+                    raise ValueError("device y needs device rows: X must be a DeviceArray too")
+                classes, n = self._device_labels(ctx, y, row_mask, mask_keep)
+                neg, pos = float(classes[0]), float(classes[1])
+            else:
+                classes, y01, n = self._host_labels(y, row_mask, mask_keep)
+                neg, pos = 0.0, 1.0
+                if isinstance(X, native.DeviceArray):
+                    y = ctx.to_device(y01)
+                    owned.append(y)
+                else:
+                    X, y, row_mask, owned = _stage_rows(ctx, X, y01, row_mask)
+            d = X.shape[1]
+            fi = bool(self.fit_intercept)
+
+            def run(c, hessian):
+                return ctx.logistic_pass(X, y, c[:d], float(c[d]) if fi else 0.0, neg, pos, row_mask=row_mask,
+                                         mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
+
+            def line_search(c, step):
+                return ctx.logistic_line_search(X, y, c[:d], float(c[d]) if fi else 0.0, step[:d],
+                                                float(step[d]) if fi else 0.0, neg, pos, n_steps=native.GLM_STEPS,
+                                                row_mask=row_mask, mask_keep=mask_keep)
+
+            def start():                          # the first pass is the Hessian pass at the start
+                coef, _ = self._start_coef(d)
+                first = run(coef, True)
+                if first["kept"] != n or first["y_out_of_range"] > 0:
+                    raise RuntimeError("the logistic pass saw other labels than the label check")
+                if not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
+                    raise ValueError(_NAN_MESSAGE)
+                return coef, first, n
+
+            coef, n_iter = self._newton(d, 1.0 / (float(self.C) * n), start, run, line_search)
+        finally:
+            for a in owned:
+                a.free()
+        self.coef_ = coef[:d].reshape(1, d).copy()
+        self.intercept_ = np.array([coef[d]]) if self.fit_intercept else np.zeros(1)
+        self.classes_ = classes
+        self.n_iter_ = np.array([n_iter], dtype=np.int32)
+        self.n_features_in_ = int(d)
+        return self
+
+    def _fp32_classes(self):
+        """(neg, pos): classes_ as the fp32 labels device y holds and device predictions return"""
+        if self.classes_.dtype.kind not in "biuf" or not all(_fp32_exact(c) for c in self.classes_):
+            raise ValueError(f"device labels are fp32 values, but classes_ is {self.classes_!r}")
+        return float(self.classes_[0]), float(self.classes_[1])
+
+    def _predict(self, X, **want):
+        """one logistic_predict pass; host rows take the labels 0 and 1 (indices into classes_)"""
+        X = self._staged(X)
+        neg, pos = self._fp32_classes() if isinstance(X, native.DeviceArray) else (0.0, 1.0)
+        return self.ctx.logistic_predict(X, self.coef_[0], float(self.intercept_[0]), neg, pos, **want)
+
+    def decision_function(self, X):
+        """eta = X coef_ + intercept_ in fp64: float64 for host rows, an f64 ``DeviceArray`` for device rows."""
+        return self._predict(X, decision=True)["decision"]
+
+    def predict_proba(self, X):
+        """[1 - p, p] per row, p = expit(eta), in fp64: (n, 2) float64 for host rows, an (n, 2) f64 ``DeviceArray``
+        for device rows."""
+        return self._predict(X, proba=True)["proba"]
+
+    def predict_log_proba(self, X):
+        """log(predict_proba(X)) for host rows."""
+        if isinstance(X, native.DeviceArray):
+            raise ValueError("predict_log_proba takes host rows (predict_proba returns device probabilities)")
+        return np.log(self.predict_proba(X))
+
+    def predict(self, X):
+        """classes_[1] where eta > 0, else classes_[0]: an ndarray of classes_' dtype for host rows, an f32
+        ``DeviceArray`` for device rows (classes_ must then be fp32 values)."""
+        labels = self._predict(X, label=True)["label"]
+        if isinstance(labels, native.DeviceArray):
+            return labels
+        return self.classes_[labels.astype(np.intp)]
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """Accuracy over the kept rows (labels outside classes_ count as wrong): the correct count of one pass."""
+        ctx = self.ctx
+        owned = []
+        try:
+            if isinstance(y, native.DeviceArray):
+                if not isinstance(X, native.DeviceArray):
+                    raise ValueError("device y needs device rows: X must be a DeviceArray too")
+                neg, pos = self._fp32_classes()
+            else:
+                yh = np.asarray(y).ravel()
+                y01 = np.where(yh == self.classes_[1], 1.0, np.where(yh == self.classes_[0], 0.0, np.nan))
+                y01 = y01.astype(np.float32)
+                neg, pos = 0.0, 1.0
+                if isinstance(X, native.DeviceArray):
+                    y = ctx.to_device(y01)
+                    owned.append(y)
+                else:
+                    X, y, row_mask, owned = _stage_rows(ctx, X, y01, row_mask)
+            if X.shape[1] != self.n_features_in_:
+                raise ValueError(f"X has {X.shape[1]} features, but B200LogisticRegression is expecting "
+                                 f"{self.n_features_in_} features as input.")
+            s = ctx.logistic_pass(X, y, self.coef_[0], float(self.intercept_[0]), neg, pos, row_mask=row_mask,
+                                  mask_keep=mask_keep, hessian=False)
+        finally:
+            for a in owned:
+                a.free()
+        if s["kept"] == 0:
+            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required.")
+        return float(s["correct"] / s["kept"])
+
+    def to_sklearn(self):
+        """A real ``sklearn.linear_model.LogisticRegression(solver="newton-cholesky")`` with the fitted attributes
+        (joblib-dumpable)."""
+        from sklearn.linear_model import LogisticRegression
+        clf = LogisticRegression(C=self.C, l1_ratio=self.l1_ratio, tol=self.tol, fit_intercept=self.fit_intercept,
+                                 solver="newton-cholesky", max_iter=self.max_iter, verbose=self.verbose,
+                                 warm_start=self.warm_start)
+        clf.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
+        clf.intercept_ = np.asarray(self.intercept_, dtype=np.float64).copy()
+        clf.classes_ = np.asarray(self.classes_).copy()
+        clf.n_iter_ = np.asarray(self.n_iter_, dtype=np.int32).copy()
+        clf.n_features_in_ = int(self.n_features_in_)
+        return clf
+
+    def __repr__(self) -> str:
+        return f"B200LogisticRegression(C={self.C})"

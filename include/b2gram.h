@@ -322,6 +322,38 @@ int b2_glm_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, 
 int b2_glm_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind, int link,
                    const double* coef, double intercept, double* mu_out);
 
+/* ---- LogisticRegression, binary (DESIGN.md section 11) ----------------------------------------------------------
+ * The row passes of scikit-learn's Newton solver for HalfBinomialLoss, the passes of b2_glm_pass on the half-binomial
+ * loss: per kept row eta = x.coef + intercept in fp64, the target t = 1 where y == pos_label and 0 where y == neg_label,
+ * and sklearn's closs_half_binomial / cgrad_hess_half_binomial branch by branch.  y: fp32 labels as stored (no binarised
+ * copy); neg_label and pos_label are two distinct finite values exactly representable in fp32.  B2_E_ARG: bad shapes or
+ * labels, null coef or outputs; B2_E_UNSUPPORTED with more than one rank. */
+/* b2_logistic_pass: sums_out (host, d + 9 doubles): [0] sum loss [1] 0 [2] kept rows with y == pos_label [3] rows kept
+ * [4] kept rows with y equal to neither label (NaN included) [5] rows with h <= 0 [6] rows with y not finite,
+ * [7, 7 + d) sum g x_j, [7 + d] sum g, [8 + d] rows classified correctly: y == pos_label and eta > 0, or y == neg_label
+ * and eta <= 0 (scikit-learn's predict rule).  hess_out as b2_glm_pass. */
+int b2_logistic_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const uint8_t* row_mask, int mask_keep, double neg_label, double pos_label,
+                     const double* coef, double intercept, int fit_intercept, double* sums_out, double* hess_out);
+/* b2_logistic_line_search: loss_out[k] = sum over kept rows of the loss at eta + 2^-k (x.step + step_intercept), k <
+ * n_steps (1..21), with the loss as sklearn's line search evaluates it (closs_grad_half_binomial). */
+int b2_logistic_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d,
+                            int64_t ldx, int mem_kind, const uint8_t* row_mask, int mask_keep, double neg_label,
+                            double pos_label, const double* coef, double intercept, const double* step,
+                            double step_intercept, int n_steps, double* loss_out);
+/* b2_logistic_predict: per row, where X lives (mem_kind), each output optional (not all null): decision_out[i] = eta_i
+ * (fp64), proba_out[2 i + c] = [1 - p_i, p_i] with p_i = 1 / (1 + exp(-eta_i)) (fp64), label_out[i] = pos_label if
+ * eta_i > 0, else neg_label (fp32).  Host rows use device staging blocks in the context. */
+int b2_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind,
+                        const double* coef, double intercept, double neg_label, double pos_label, double* decision_out,
+                        double* proba_out, float* label_out);
+/* b2_label_scan: the labels of device fp32 y over the kept rows (row_mask / mask_keep as b2_score).  stats_out (host, 7
+ * doubles): [0] kept rows [1] y not finite [2] finite y with y != rint(y) [3] min and [4] max of the finite kept y (NaN
+ * when there is none) [5] kept rows equal to the min [6] kept rows equal to the max.  Counted with atomics: the result
+ * does not depend on the order of the rows. */
+int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep,
+                  double* stats_out);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
