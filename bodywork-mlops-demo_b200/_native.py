@@ -163,6 +163,13 @@ def _check(rc: int, what: str) -> None:
         raise RuntimeError(f"{what} failed (code {rc}): {last_error()}")
 
 
+def _check_args(rc: int, what: str) -> None:
+    """``_check``, with the library's refusal of an argument (E_ARG) raised as ``ValueError``."""
+    if rc == E_ARG:
+        raise ValueError(last_error())
+    _check(rc, what)
+
+
 def device_count() -> int:
     n = C.c_int(0)
     rc = load().b2_device_count(C.byref(n))
@@ -282,6 +289,13 @@ def _vec_ptr(v, kind: str, mem_kind: int, n: int, what: str) -> Optional[int]:
     return v.ctypes.data
 
 
+def _row_args(X, y, row_mask, mask_what: str = "row_mask"):
+    """(ptr, x_dtype, mem_kind, n, d, y_ptr, mask_ptr) of rows, their f32 targets and their u8 mask (either may be
+    None), all three where X lives."""
+    ptr, xdt, mk, n, d = _x_kind(X)
+    return ptr, xdt, mk, n, d, _vec_ptr(y, "f32", mk, n, "y"), _vec_ptr(row_mask, "u8", mk, n, mask_what)
+
+
 class Context:
     """One GPU: streams, the fp64 statistic S, scratch, (optionally) one NCCL communicator."""
 
@@ -373,6 +387,17 @@ class Context:
     def pinned(self, shape, dtype) -> PinnedArray:
         return PinnedArray(self, tuple(np.atleast_1d(shape)), dtype)
 
+    def _out(self, mem_kind: int, shape, kind: str, want: bool = True):
+        """(buffer, pointer) of an output the library fills, where the rows live: a ``DeviceArray`` of ``kind`` (f64 /
+        f32) for device rows, a numpy array otherwise; (None, None) unless ``want``."""
+        if not want:
+            return None, None
+        if mem_kind == MEM_DEVICE:
+            a = self.empty(shape, kind)
+            return a, a.ptr
+        a = np.empty(shape, dtype=DeviceArray._NP[kind])
+        return a, a.ctypes.data
+
     # -- Gram ----------------------------------------------------------------------------------------
     def gram_reset(self, d: int) -> None:
         _check(load().b2_gram_reset(self._h, int(d)), "b2_gram_reset")
@@ -380,11 +405,9 @@ class Context:
         self.serial += 1
 
     def gram_accumulate(self, X, y, row_mask=None, mask_keep: int = 1) -> None:
-        ptr, xdt, mk, n, d = _x_kind(X)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
         if self.d == 0:
             self.gram_reset(d)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
         self.serial += 1
         _check(load().b2_gram_accumulate(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep)),
                "b2_gram_accumulate")
@@ -409,9 +432,7 @@ class Context:
             fit_intercept: bool = True) -> Tuple[np.ndarray, float]:
         """The whole fit in one C call (b2_fit): reset + accumulate + all-reduce + solve.  Device-resident rows on the
         tensor-core path run as four launches (shift sample, Gram, finalize + peer scatter, gather + solve).  Raises ``np.linalg.LinAlgError`` on a rank-deficient Gram."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
         coef = np.empty(d, dtype=np.float64)
         b0 = C.c_double(0.0)
         rc = load().b2_fit(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(alpha),
@@ -429,9 +450,7 @@ class Context:
         rows once for the fp64 gradient and corrects the solution through the factor of the Gram.  Returns (coef,
         intercept, passes kept, last step); the step is max_j |dcoef_j| sigma_j / sigma_y.  Raises
         ``np.linalg.LinAlgError`` on a rank-deficient Gram."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
         coef = np.empty(d, dtype=np.float64)
         b0, step, passes = C.c_double(0.0), C.c_double(0.0), C.c_int(0)
         rc = load().b2_fit_refined(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(alpha),
@@ -508,9 +527,7 @@ class Context:
                                        out["alphas"].ctypes.data, out["coefs"].ctypes.data,
                                        out["intercepts"].ctypes.data, out["gaps"].ctypes.data,
                                        out["n_iter"].ctypes.data, C.byref(tol_out))
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_solve_enet_path")
+        _check_args(rc, "b2_solve_enet_path")
         out["tol"] = float(tol_out.value)
         return out
 
@@ -518,15 +535,11 @@ class Context:
         """The statistic of every fold in one call (b2_gram_folds): row r belongs to fold ``fold_of_row[r]`` (uint8, where
         X lives; ids >= n_folds drop the row).  Leaves S = the sum of the folds resident and the fold statistics in the
         context for ``solve_enet_cv``; returns them, (n_folds, d + 2, d + 2)."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        fp = _vec_ptr(fold_of_row, "u8", mk, n, "fold_of_row")
+        ptr, xdt, mk, n, d, yp, fp = _row_args(X, y, fold_of_row, "fold_of_row")
         out = np.empty((int(n_folds), d + 2, d + 2), dtype=np.float64)
         self.serial += 1
         rc = load().b2_gram_folds(self._h, ptr, xdt, yp, n, d, d, mk, fp, int(n_folds), out.ctypes.data)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_gram_folds")
+        _check_args(rc, "b2_gram_folds")
         self.d = d
         return out
 
@@ -562,9 +575,7 @@ class Context:
                                      int(n_alphas), float(eps), int(max_iter), float(tol), int(bool(positive)),
                                      out["alphas"].ctypes.data, out["mse"].ctypes.data, out["n_iter"].ctypes.data,
                                      out["gaps"].ctypes.data, out["coefs"].ctypes.data if want_coefs else None)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_solve_enet_cv")
+        _check_args(rc, "b2_solve_enet_cv")
         return out
 
     def ridge_loo(self, X, y, alphas, row_mask=None, mask_keep: int = 1, fit_intercept: bool = True,
@@ -573,17 +584,12 @@ class Context:
         first smallest, coef, intercept at that alpha, cv) where cv is None or the (n, n_alphas) e^2 per row and alpha
         (NaN on rows not kept) -- a float64 ndarray for host rows, an f64 DeviceArray for device rows.  Up to MAX_ALPHAS
         alphas per call."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
         al = np.ascontiguousarray(np.asarray(alphas, dtype=np.float64).ravel())
         mse = np.empty(max(al.size, 1), dtype=np.float64)
         coef = np.empty(d, dtype=np.float64)
         b0, best = C.c_double(0.0), C.c_int(0)
-        cv, cv_ptr = None, None
-        if store_cv:
-            cv = self.empty((n, al.size), "f64") if mk == MEM_DEVICE else np.empty((n, al.size), dtype=np.float64)
-            cv_ptr = cv.ptr if mk == MEM_DEVICE else cv.ctypes.data
+        cv, cv_ptr = self._out(mk, (n, al.size), "f64", store_cv)
         rc = load().b2_ridge_loo(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), al.ctypes.data, int(al.size),
                                  int(bool(fit_intercept)), mse.ctypes.data, cv_ptr, C.byref(best), coef.ctypes.data,
                                  C.byref(b0))
@@ -592,18 +598,20 @@ class Context:
         _check(rc, "b2_ridge_loo")
         return mse[: al.size], int(best.value), coef, float(b0.value), cv
 
+    def _f64_coef(self, coef, d: int) -> np.ndarray:
+        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
+        if w.size != d:
+            raise ValueError(f"coef has {w.size} entries, X has {d} columns")
+        return w
+
     # -- BayesianRidge / ARDRegression (DESIGN.md section 9) ---------------------------------------------------
     def residual_moments(self, X, y, coef, intercept: float, row_mask=None, mask_keep: int = 1,
                          fit_intercept: bool = True) -> np.ndarray:
         """One fp64 pass over the kept rows at (coef, intercept) (b2_residual_moments): returns the d + 2 values
         [sum (x - m) e, sum e, sum e^2], e = y - intercept - x.coef, m the column means of the resident statistic (0
         without an intercept).  [coef, result] is the anchor of ``solve_bayes_ridge`` / ``solve_ard``."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
-        if w.size != d:
-            raise ValueError(f"coef has {w.size} entries, X has {d} columns")
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w = self._f64_coef(coef, d)
         out = np.empty(d + 2, dtype=np.float64)
         _check(load().b2_residual_moments(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), w.ctypes.data,
                                           float(intercept), int(bool(fit_intercept)), out.ctypes.data),
@@ -628,11 +636,9 @@ class Context:
                 int(bool(compute_score)), coef.ctypes.data, C.byref(b0), C.byref(alpha), lam.ctypes.data,
                 C.byref(n_iter), scores.ctypes.data if scores is not None else None,
                 sigma.ctypes.data if sigma is not None else None)
-        if rc == E_ARG:
-            raise ValueError(last_error())
         if rc == E_SINGULAR:
             raise np.linalg.LinAlgError(last_error())
-        _check(rc, what)
+        _check_args(rc, what)
         k = int(n_iter.value)
         return {"coef": coef, "intercept": float(b0.value), "alpha": float(alpha.value),
                 "lambda": lam if ard else float(lam[0]), "n_iter": k,
@@ -674,46 +680,28 @@ class Context:
         sg = np.ascontiguousarray(sigma, dtype=np.float64)
         if w.size != d or sg.shape != (d, d) or (m is not None and m.size != d):
             raise ValueError(f"coef / mean need {d} entries and sigma shape ({d}, {d})")
-        if mk == MEM_DEVICE:
-            ystd = self.empty((n,), "f64")
-            yhat = self.empty((n,), "f64") if want_yhat else None
-            sp, hp = ystd.ptr, (yhat.ptr if yhat is not None else None)
-        else:
-            ystd = np.empty(n, dtype=np.float64)
-            yhat = np.empty(n, dtype=np.float64) if want_yhat else None
-            sp, hp = ystd.ctypes.data, (yhat.ctypes.data if yhat is not None else None)
+        ystd, sp = self._out(mk, (n,), "f64")
+        yhat, hp = self._out(mk, (n,), "f64", want_yhat)
         rc = load().b2_score_std(self._h, ptr, xdt, n, d, d, mk, m.ctypes.data if m is not None else None,
                                  sg.ctypes.data, float(noise_var), w.ctypes.data, float(intercept), hp, sp)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_score_std")
+        _check_args(rc, "b2_score_std")
         return yhat, ystd
 
     # -- PoissonRegressor / GammaRegressor / TweedieRegressor (DESIGN.md section 10) --------------------------------
-    def _glm_coef(self, coef, d: int) -> np.ndarray:
-        w = np.ascontiguousarray(coef, dtype=np.float64).ravel()
-        if w.size != d:
-            raise ValueError(f"coef has {w.size} entries, X has {d} columns")
-        return w
-
     def glm_pass(self, X, y, coef, intercept: float, *, link: int = GLM_LOG, power: float = 1.0, row_mask=None,
                  mask_keep: int = 1, fit_intercept: bool = True, hessian: bool = True) -> dict:
         """One pass of the Newton solver's statistics at (coef, intercept) over the kept rows (b2_glm_pass).  Returns
         a dict of unscaled sums: loss, const (constant_to_optimal_zero), sum_y, kept, y_out_of_range, h_nonpos,
         y_nonfinite (floats), grad ((d + 1,): sum g x_j, then sum g) and hessian ((d + 1, d + 1) sum |h| [x 1][x 1]^T,
         or None without ``hessian``).  Raises ``ValueError`` for bad arguments."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        w = self._glm_coef(coef, d)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w = self._f64_coef(coef, d)
         sums = np.empty(d + 8, dtype=np.float64)
         hess = np.empty((d + 1, d + 1), dtype=np.float64) if hessian else None
         rc = load().b2_glm_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), int(link), float(power),
                                 w.ctypes.data, float(intercept), int(bool(fit_intercept)), sums.ctypes.data,
                                 hess.ctypes.data if hess is not None else None)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_glm_pass")
+        _check_args(rc, "b2_glm_pass")
         keys = ("loss", "const", "sum_y", "kept", "y_out_of_range", "h_nonpos", "y_nonfinite")
         out = {k: float(sums[i]) for i, k in enumerate(keys)}
         out["grad"] = sums[7:].copy()
@@ -724,30 +712,23 @@ class Context:
                         power: float = 1.0, n_steps: int = GLM_STEPS, row_mask=None, mask_keep: int = 1) -> np.ndarray:
         """The backtracking ladder in one pass (b2_glm_line_search): the summed loss over the kept rows at
         (coef, intercept) + 2^-k (step, step_intercept) for k < n_steps."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        w, s = self._glm_coef(coef, d), self._glm_coef(step, d)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w, s = self._f64_coef(coef, d), self._f64_coef(step, d)
         out = np.empty(max(int(n_steps), 1), dtype=np.float64)
         rc = load().b2_glm_line_search(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), int(link), float(power),
                                        w.ctypes.data, float(intercept), s.ctypes.data, float(step_intercept),
                                        int(n_steps), out.ctypes.data)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_glm_line_search")
+        _check_args(rc, "b2_glm_line_search")
         return out
 
     def glm_predict(self, X, coef, intercept: float, *, link: int = GLM_LOG):
         """mu = exp(X coef + intercept) (GLM_LOG) or X coef + intercept per row in fp64 (b2_glm_predict): a float64
         ndarray for host rows, an f64 DeviceArray for device rows."""
         ptr, xdt, mk, n, d = _x_kind(X)
-        w = self._glm_coef(coef, d)
-        mu = self.empty((n,), "f64") if mk == MEM_DEVICE else np.empty(n, dtype=np.float64)
-        rc = load().b2_glm_predict(self._h, ptr, xdt, n, d, d, mk, int(link), w.ctypes.data, float(intercept),
-                                   mu.ptr if mk == MEM_DEVICE else mu.ctypes.data)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_glm_predict")
+        w = self._f64_coef(coef, d)
+        mu, mu_ptr = self._out(mk, (n,), "f64")
+        rc = load().b2_glm_predict(self._h, ptr, xdt, n, d, d, mk, int(link), w.ctypes.data, float(intercept), mu_ptr)
+        _check_args(rc, "b2_glm_predict")
         return mu
 
     # -- LogisticRegression, binary (DESIGN.md section 11) ----------------------------------------------------------
@@ -757,18 +738,14 @@ class Context:
         (b2_logistic_pass); y holds the labels as stored, the target is 1 where y == pos_label and 0 where y == neg_label.
         Returns ``glm_pass``'s dict (sum_y: the positive rows, y_out_of_range: the rows with neither label) and correct:
         the rows classified correctly by the sign of eta.  Raises ``ValueError`` for bad arguments."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        w = self._glm_coef(coef, d)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w = self._f64_coef(coef, d)
         sums = np.empty(d + 9, dtype=np.float64)
         hess = np.empty((d + 1, d + 1), dtype=np.float64) if hessian else None
         rc = load().b2_logistic_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(neg_label),
                                      float(pos_label), w.ctypes.data, float(intercept), int(bool(fit_intercept)),
                                      sums.ctypes.data, hess.ctypes.data if hess is not None else None)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_logistic_pass")
+        _check_args(rc, "b2_logistic_pass")
         keys = ("loss", "const", "sum_y", "kept", "y_out_of_range", "h_nonpos", "y_nonfinite")
         out = {k: float(sums[i]) for i, k in enumerate(keys)}
         out["grad"] = sums[7:8 + d].copy()
@@ -780,17 +757,13 @@ class Context:
                              pos_label: float = 1.0, *, n_steps: int = GLM_STEPS, row_mask=None,
                              mask_keep: int = 1) -> np.ndarray:
         """The backtracking ladder of a logistic Newton step in one pass (b2_logistic_line_search)."""
-        ptr, xdt, mk, n, d = _x_kind(X)
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        w, s = self._glm_coef(coef, d), self._glm_coef(step, d)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w, s = self._f64_coef(coef, d), self._f64_coef(step, d)
         out = np.empty(max(int(n_steps), 1), dtype=np.float64)
         rc = load().b2_logistic_line_search(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), float(neg_label),
                                             float(pos_label), w.ctypes.data, float(intercept), s.ctypes.data,
                                             float(step_intercept), int(n_steps), out.ctypes.data)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_logistic_line_search")
+        _check_args(rc, "b2_logistic_line_search")
         return out
 
     def logistic_predict(self, X, coef, intercept: float, neg_label: float = 0.0, pos_label: float = 1.0, *,
@@ -799,23 +772,17 @@ class Context:
         ((n, 2) [1 - p, p], fp64) and label (pos_label where eta > 0, else neg_label; fp32) -- ndarrays for host rows,
         DeviceArrays for device rows."""
         ptr, xdt, mk, n, d = _x_kind(X)
-        w = self._glm_coef(coef, d)
+        w = self._f64_coef(coef, d)
         out, ptrs = {}, {}
-        for name, want, shape, kind, dtype in (("decision", decision, (n,), "f64", np.float64),
-                                               ("proba", proba, (n, 2), "f64", np.float64),
-                                               ("label", label, (n,), "f32", np.float32)):
-            if not want:
-                ptrs[name] = None
-                continue
-            a = self.empty(shape, kind) if mk == MEM_DEVICE else np.empty(shape, dtype=dtype)
-            out[name] = a
-            ptrs[name] = a.ptr if mk == MEM_DEVICE else a.ctypes.data
+        for name, want, shape, kind in (("decision", decision, (n,), "f64"), ("proba", proba, (n, 2), "f64"),
+                                        ("label", label, (n,), "f32")):
+            a, ptrs[name] = self._out(mk, shape, kind, want)
+            if want:
+                out[name] = a
         rc = load().b2_logistic_predict(self._h, ptr, xdt, n, d, d, mk, w.ctypes.data, float(intercept),
                                         float(neg_label), float(pos_label), ptrs["decision"], ptrs["proba"],
                                         ptrs["label"])
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_logistic_predict")
+        _check_args(rc, "b2_logistic_predict")
         return out
 
     def label_scan(self, y, row_mask=None, mask_keep: int = 1) -> dict:
@@ -827,9 +794,7 @@ class Context:
         mp = _vec_ptr(row_mask, "u8", MEM_DEVICE, n, "row_mask")
         st = np.empty(7, dtype=np.float64)
         rc = load().b2_label_scan(self._h, y.ptr, n, mp, int(mask_keep), st.ctypes.data)
-        if rc == E_ARG:
-            raise ValueError(last_error())
-        _check(rc, "b2_label_scan")
+        _check_args(rc, "b2_label_scan")
         return dict(zip(("kept", "nonfinite", "nonintegral", "min", "max", "n_min", "n_max"), st.tolist()))
 
     # -- scoring ------------------------------------------------------------------------------------------
@@ -859,14 +824,10 @@ class Context:
         ([sum_ape, sse, sum_y, sum_yy, max_abs_res, rows, sum_p, sum_pp, sum_yp, max_ape]).
         ``out``: a preallocated prediction buffer (DeviceArray f32 for device rows, float32 ndarray for host rows)
         to write into instead of allocating one per call."""
-        ptr, xdt, mk, n, d = _x_kind(X)
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
         coef = np.ascontiguousarray(coef, dtype=np.float64).ravel()
         if coef.size != d:
             raise RuntimeError(f"coef has {coef.size} entries, X has {d} columns")
-        yp = _vec_ptr(y, "f32", mk, n, "y")
-        mp = _vec_ptr(row_mask, "u8", mk, n, "row_mask")
-        yhat = None
-        yhat_ptr = None
         if out is not None:
             if mk == MEM_DEVICE:
                 if not isinstance(out, DeviceArray) or out.kind != "f32" or int(np.prod(out.shape)) != n:
@@ -877,9 +838,8 @@ class Context:
                         and out.flags.c_contiguous):
                     raise RuntimeError("out must be a C-contiguous float32 ndarray with one element per row")
                 yhat, yhat_ptr = out, out.ctypes.data
-        elif want_yhat:
-            yhat = self.empty((n,), "f32") if mk == MEM_DEVICE else np.empty(n, dtype=np.float32)
-            yhat_ptr = yhat.ptr if mk == MEM_DEVICE else yhat.ctypes.data
+        else:
+            yhat, yhat_ptr = self._out(mk, (n,), "f32", want_yhat)
         stats = np.zeros(10, dtype=np.float64) if y is not None else None
         _check(load().b2_score(self._h, ptr, xdt, n, d, d, mk, coef.ctypes.data, float(intercept), yp, mp,
                                int(mask_keep), yhat_ptr, stats.ctypes.data if stats is not None else None),

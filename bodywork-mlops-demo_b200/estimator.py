@@ -12,6 +12,7 @@ joblib importable, calls ``.predict`` and ``str(model)`` -- a custom class could
 """
 from __future__ import annotations
 
+import contextlib
 import warnings
 from typing import Optional
 
@@ -44,41 +45,138 @@ def _as_f32_matrix(X) -> np.ndarray:
     return np.ascontiguousarray(X, dtype=np.float32)
 
 
+# ---- the refusals and messages every estimator shares: scikit-learn's wording, which tests and users match on ---------
+_NAN_MESSAGE = "Input X or y contains NaN, infinity or a value too large for dtype('float32')."
+
+
+def _too_few_rows(shape, need: int = 1, by: Optional[str] = None) -> ValueError:
+    """check_array's refusal of an input with fewer than ``need`` rows; ``shape``: the kept rows' (n, d) or (n,)."""
+    shape = tuple(int(s) for s in shape)
+    return ValueError(f"Found array with {shape[0]} sample(s) (shape={shape}) while a minimum of {need} is required"
+                      + (f" by {by}." if by else "."))
+
+
+def _check_finite(*values) -> None:
+    """check_array's refusal of non-finite input, which the GPU paths see in what the rows produce (the statistic, the
+    solution, the loss)."""
+    if not all(np.all(np.isfinite(v)) for v in values):
+        raise ValueError(_NAN_MESSAGE)
+
+
+def _refuse_sample_weight(sample_weight, who: str) -> None:
+    if sample_weight is not None:
+        raise ValueError(f"sample_weight is not supported by {who}: every kept row has weight 1")
+
+
+def _check_selection(selection) -> None:
+    if selection == "random":
+        raise ValueError("selection='random' is not supported: the GPU solver runs sklearn's cyclic order only")
+    if selection != "cyclic":
+        raise ValueError("selection should be either random or cyclic.")
+
+
+def _alpha_grid(alphas):
+    """(alphas sorted descending, their count), or (None, n) for sklearn's grid of n alphas when ``alphas`` is an int."""
+    if isinstance(alphas, (int, np.integer)) and not isinstance(alphas, bool):
+        if int(alphas) < 1:
+            raise ValueError(f"alphas must be >= 1 when given as an integer, got {int(alphas)}")
+        return None, int(alphas)
+    al = np.sort(np.asarray(alphas, dtype=np.float64).ravel())[::-1]
+    return al, al.size
+
+
+@contextlib.contextmanager
 def _stage_rows(ctx: native.Context, X, y, row_mask):
-    """(X, y, row_mask, owned) in a form the context's fit entry points take: a ``DeviceArray`` as it is, float64 host
-    rows (65 536 or more) converted on the way up by ``upload_columns`` and left resident (``owned``: the device buffers
-    this call created, for the caller to free), any other host rows as contiguous float32."""
+    """(X, y, row_mask) in a form the context's fit entry points take, for the body of the ``with``: a ``DeviceArray``
+    as it is, float64 host rows (65 536 or more) converted on the way up by ``upload_columns`` and resident until the
+    ``with`` ends (on success and on error), any other host rows as contiguous float32."""
     owned = []
-    if isinstance(X, native.DeviceArray):
-        return X, y, row_mask, owned
-    Xh = np.asarray(X)
-    if Xh.ndim == 2 and Xh.dtype == np.float64 and 0 < Xh.shape[1] <= native.MAX_D and Xh.shape[0] >= 65_536 \
-            and Xh.size * 4 <= _F64_UPLOAD_LIMIT:
-        # what scikit-learn users hand over: float64 rows.  numpy's astype(float32) is one thread; b2_upload_columns
-        # converts with the host threads of the bounce ring beside the H2D copies and leaves the rows resident
-        if np.asarray(y).size != Xh.shape[0]:
-            raise ValueError(f"Found input variables with inconsistent numbers of samples: "
-                             f"[{Xh.shape[0]}, {np.asarray(y).size}]")
-        X = ctx.upload_columns([Xh[:, j] for j in range(Xh.shape[1])])
-        y = ctx.to_device(np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32))
-        owned = [X, y]
-        if row_mask is not None and not isinstance(row_mask, native.DeviceArray):
-            row_mask = ctx.to_device(np.ascontiguousarray(row_mask, dtype=np.uint8))
-            owned.append(row_mask)
-        return X, y, row_mask, owned
-    X = _as_f32_matrix(X)
-    y = np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32)
-    if y.shape[0] != X.shape[0]:
-        raise ValueError(f"Found input variables with inconsistent numbers of samples: "
-                         f"[{X.shape[0]}, {y.shape[0]}]")
-    return X, y, row_mask, owned
+    try:
+        Xh = None if isinstance(X, native.DeviceArray) else np.asarray(X)
+        if Xh is not None and Xh.ndim == 2 and Xh.dtype == np.float64 and 0 < Xh.shape[1] <= native.MAX_D \
+                and Xh.shape[0] >= 65_536 and Xh.size * 4 <= _F64_UPLOAD_LIMIT:
+            # what scikit-learn users hand over: float64 rows.  numpy's astype(float32) is one thread; b2_upload_columns
+            # converts with the host threads of the bounce ring beside the H2D copies and leaves the rows resident
+            if np.asarray(y).size != Xh.shape[0]:
+                raise ValueError(f"Found input variables with inconsistent numbers of samples: "
+                                 f"[{Xh.shape[0]}, {np.asarray(y).size}]")
+            X = ctx.upload_columns([Xh[:, j] for j in range(Xh.shape[1])])
+            owned.append(X)
+            y = ctx.to_device(np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32))
+            owned.append(y)
+            if row_mask is not None and not isinstance(row_mask, native.DeviceArray):
+                row_mask = ctx.to_device(np.ascontiguousarray(row_mask, dtype=np.uint8))
+                owned.append(row_mask)
+        elif Xh is not None:
+            X = _as_f32_matrix(X)
+            y = np.ascontiguousarray(np.asarray(y).ravel(), dtype=np.float32)
+            if y.shape[0] != X.shape[0]:
+                raise ValueError(f"Found input variables with inconsistent numbers of samples: "
+                                 f"[{X.shape[0]}, {y.shape[0]}]")
+        yield X, y, row_mask
+    finally:
+        for a in owned:
+            a.free()
 
 
-class B200LinearRegression:
+@contextlib.contextmanager
+def _on_device(ctx: native.Context, host: np.ndarray):
+    """``host`` copied to the device for the body of the ``with``."""
+    a = ctx.to_device(host)
+    try:
+        yield a
+    finally:
+        a.free()
+
+
+class _B200Estimator:
+    """What every estimator shares: its context, the width check of the rows it predicts on, the linear ``predict``
+    and the export to scikit-learn.  ``_sk_name``: the scikit-learn class restated; ``_sk_attrs``: the fitted
+    attributes ``to_sklearn`` copies onto it."""
+    _sk_name = ""
+    _sk_attrs: tuple = ()
+
+    @property
+    def ctx(self) -> native.Context:
+        return self._ctx if self._ctx is not None else default_context()
+
+    def _checked_rows(self, X):
+        """host rows as contiguous float32, device rows as they are; either must have ``n_features_in_`` columns."""
+        X = X if isinstance(X, native.DeviceArray) else _as_f32_matrix(X)
+        if X.shape[1] != self.n_features_in_:
+            raise ValueError(f"X has {X.shape[1]} features, but B200{self._sk_name} is expecting "
+                             f"{self.n_features_in_} features as input.")
+        return X
+
+    def predict(self, X):
+        """X coef_ + intercept_: float64 for host rows, an f32 ``DeviceArray`` for device rows."""
+        ctx = self.ctx
+        X = self._checked_rows(X)
+        yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
+        return yhat if isinstance(X, native.DeviceArray) else yhat.astype(np.float64)
+
+    def _sk_prepare(self, reg) -> None:
+        """whatever the export needs beyond copying ``_sk_attrs``"""
+
+    def to_sklearn(self):
+        """A real scikit-learn estimator with the attributes ``fit`` would have set (joblib-dumpable; its own
+        ``predict`` works)."""
+        from sklearn import linear_model
+        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        self._sk_prepare(reg)
+        for name in self._sk_attrs:
+            v = getattr(self, name)
+            setattr(reg, name, v.copy() if isinstance(v, np.ndarray) else v)
+        return reg
+
+
+class B200LinearRegression(_B200Estimator):
     """The statistic S = [X 1 y]^T [X 1 y] of a fit lives in the (shared) context while the fit runs; whatever an
     estimator needs of it later -- the next ``partial_fit``, a deferred ``singular_`` / ``rank_`` -- is kept per
     estimator (``_S``) or guarded by the context's serial number, so two estimators on one context never see each
     other's rows."""
+    _sk_name = "LinearRegression"
+    _sk_attrs = ("coef_", "intercept_", "rank_", "singular_", "n_features_in_")
 
     def __init__(self, *, fit_intercept: bool = True, alpha: float = 0.0, tol: float = 1e-6,
                  ctx: Optional[native.Context] = None, refine: int = 0):
@@ -92,15 +190,9 @@ class B200LinearRegression:
         self._S: Optional[np.ndarray] = None     # this estimator's statistic (set by partial_fit / deferred attributes)
         self._serial = -1                        # ctx.serial right after this estimator's last fit
 
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
-
     # -- fit -------------------------------------------------------------------------------------
     def _set_solution(self, coef, b0, d: int) -> None:
-        if not (np.all(np.isfinite(coef)) and np.isfinite(b0)):
-            # sklearn's check_array refuses such input up front; here it shows up in the statistic
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(coef, b0)
         self.coef_ = coef
         self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
         self.n_features_in_ = int(d)
@@ -110,8 +202,7 @@ class B200LinearRegression:
         number of rows in the statistic."""
         sing, rank, rows = self.ctx.solve_eigvals(cond=self.tol, fit_intercept=self.fit_intercept)
         if rows == 0:
-            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
-                             "B200LinearRegression.")
+            raise _too_few_rows((0, d), by="B200LinearRegression")
         self.singular_ = sing[: min(rows, d)]
         self.rank_ = int(rank)
         return rows
@@ -150,29 +241,25 @@ class B200LinearRegression:
         computed.  Wherever the spectrum is computed, a fit that keeps no rows (e.g. through ``row_mask``) raises
         ``ValueError``, as sklearn does for 0 samples."""
         ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        d = X.shape[1]
-        self._S = None
-        self._drop_spectrum()
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = X.shape[1]
+            self._S = None
+            self._drop_spectrum()
 
-        def solve():
-            if self.refine == 0:
-                return ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
-            self.n_refine_passes_, self.refine_step_ = 0, 0.0      # the min-norm fallback stays unrefined
-            coef, b0, passes, step = ctx.fit_refined(X, y, row_mask, mask_keep, alpha=self.alpha,
-                                                     fit_intercept=self.fit_intercept, max_passes=self.refine,
-                                                     tol=_REFINE_TOL)
-            self.n_refine_passes_, self.refine_step_ = passes, step
-            if step > _REFINE_TOL:
-                warnings.warn(f"refined fit stopped at step {step:.3e} after {passes} kept correction(s) "
-                              f"(tolerance {_REFINE_TOL:.0e}): more passes may help, or the features are too "
-                              "ill-conditioned for the Gram path's precision", RuntimeWarning, stacklevel=4)
-            return coef, b0
-        try:
+            def solve():
+                if self.refine == 0:
+                    return ctx.fit(X, y, row_mask, mask_keep, alpha=self.alpha, fit_intercept=self.fit_intercept)
+                self.n_refine_passes_, self.refine_step_ = 0, 0.0      # the min-norm fallback stays unrefined
+                coef, b0, passes, step = ctx.fit_refined(X, y, row_mask, mask_keep, alpha=self.alpha,
+                                                         fit_intercept=self.fit_intercept, max_passes=self.refine,
+                                                         tol=_REFINE_TOL)
+                self.n_refine_passes_, self.refine_step_ = passes, step
+                if step > _REFINE_TOL:
+                    warnings.warn(f"refined fit stopped at step {step:.3e} after {passes} kept correction(s) "
+                                  f"(tolerance {_REFINE_TOL:.0e}): more passes may help, or the features are too "
+                                  "ill-conditioned for the Gram path's precision", RuntimeWarning, stacklevel=4)
+                return coef, b0
             self._solve_statistic(d, solve, with_spectrum)
-        finally:
-            for a in owned:
-                a.free()
         self._serial = ctx.serial
         return self
 
@@ -225,32 +312,12 @@ class B200LinearRegression:
         self._spectrum(self.n_features_in_)
         self._serial = ctx.serial
 
-    # -- predict -------------------------------------------------------------------------------------
-    def predict(self, X):
-        ctx = self.ctx
-        if isinstance(X, native.DeviceArray):
-            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
-            return yhat
-        Xh = _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200LinearRegression is expecting "
-                             f"{self.n_features_in_} features as input.")
-        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
-        return yhat.astype(np.float64)
-
     # -- artefact ----------------------------------------------------------------------------------------
-    def to_sklearn(self):
-        """A real sklearn LinearRegression with the attributes ``fit`` would have set
-        (the joblib layout stage_1_train_model.py:113-114 dumps and stage_2_serve_model.py:65 loads)."""
-        from sklearn.linear_model import LinearRegression
+    def _sk_params(self) -> dict:
+        return dict(fit_intercept=self.fit_intercept)
+
+    def _sk_prepare(self, reg) -> None:
         self._ensure_spectrum()
-        reg = LinearRegression(fit_intercept=self.fit_intercept)
-        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        reg.intercept_ = np.float64(self.intercept_)
-        reg.rank_ = int(self.rank_)
-        reg.singular_ = np.asarray(self.singular_, dtype=np.float64).copy()
-        reg.n_features_in_ = int(self.n_features_in_)
-        return reg
 
     def __repr__(self) -> str:
         args = ([f"alpha={self.alpha}"] if self.alpha != 0.0 else []) + ([f"refine={self.refine}"] if self.refine else [])
@@ -281,11 +348,12 @@ def merge_alpha_chunks(chunks):
     return best
 
 
-class B200RidgeCV:
+class B200RidgeCV(_B200Estimator):
     """``sklearn.linear_model.RidgeCV(alphas, fit_intercept=..., store_cv_results=...)`` with its default ``cv=None``:
     the alpha with the smallest exact leave-one-out squared error, found on the H100 by ``b2_ridge_loo`` (Gram,
     eigendecomposition and one fp64 pass over the rows per chunk of up to MAX_ALPHAS alphas).  Ties go to the lowest
     index, as in sklearn.  ``to_sklearn()`` returns a genuine RidgeCV carrying the fitted attributes."""
+    _sk_name = "RidgeCV"
 
     def __init__(self, alphas=(0.1, 1.0, 10.0), *, fit_intercept: bool = True, store_cv_results: bool = False,
                  ctx: Optional[native.Context] = None):
@@ -294,19 +362,14 @@ class B200RidgeCV:
         self.store_cv_results = store_cv_results
         self._ctx = ctx
 
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
-
     def fit(self, X, y, row_mask=None, mask_keep: int = 1) -> "B200RidgeCV":
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets alpha_, best_score_, coef_, intercept_,
         n_features_in_ and, with store_cv_results, cv_results_ of shape (rows kept, n_alphas)."""
         al = _check_alphas(self.alphas)
         ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        d = X.shape[1]
-        try:
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = X.shape[1]
             chunks, cvs, sols = [], [], []
             for off in range(0, al.size, native.MAX_ALPHAS):
                 part = al[off: off + native.MAX_ALPHAS]
@@ -316,8 +379,7 @@ class B200RidgeCV:
                                                             store_cv=self.store_cv_results)
                 except RuntimeError as exc:
                     if "no row kept" in str(exc):
-                        raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is "
-                                         "required by B200RidgeCV.") from None
+                        raise _too_few_rows((0, d), by="B200RidgeCV") from None
                     raise
                 chunks.append((off, mse))
                 sols.append((off + best, coef, b0))
@@ -325,14 +387,10 @@ class B200RidgeCV:
                     cvs.append(cv.to_host() if isinstance(cv, native.DeviceArray) else cv)
                     if isinstance(cv, native.DeviceArray):
                         cv.free()
-        finally:
-            for a in owned:
-                a.free()
         best = merge_alpha_chunks(chunks)
         mse_all = np.concatenate([m for _, m in chunks])
         coef, b0 = next((c, b) for i, c, b in sols if i == best)
-        if not (np.all(np.isfinite(coef)) and np.isfinite(b0) and np.isfinite(mse_all[best])):
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(coef, b0, mse_all[best])
         self.alpha_ = float(al[best])
         self.best_score_ = float(-mse_all[best])
         self.coef_ = coef
@@ -344,32 +402,14 @@ class B200RidgeCV:
             self.cv_results_ = cv[keep]
         return self
 
-    def predict(self, X):
-        ctx = self.ctx
-        if isinstance(X, native.DeviceArray):
-            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
-            return yhat
-        Xh = _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200RidgeCV is expecting "
-                             f"{self.n_features_in_} features as input.")
-        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
-        return yhat.astype(np.float64)
+    @property
+    def _sk_attrs(self) -> tuple:
+        return ("alpha_", "best_score_", "coef_", "intercept_", "n_features_in_") \
+            + (("cv_results_",) if self.store_cv_results else ())
 
-    def to_sklearn(self):
-        """A real sklearn RidgeCV with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
-        intercept_)."""
-        from sklearn.linear_model import RidgeCV
-        reg = RidgeCV(alphas=np.asarray(self.alphas, dtype=np.float64), fit_intercept=self.fit_intercept,
-                      store_cv_results=self.store_cv_results)
-        reg.alpha_ = float(self.alpha_)
-        reg.best_score_ = float(self.best_score_)
-        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        reg.intercept_ = np.float64(self.intercept_)
-        reg.n_features_in_ = int(self.n_features_in_)
-        if self.store_cv_results:
-            reg.cv_results_ = np.asarray(self.cv_results_, dtype=np.float64).copy()
-        return reg
+    def _sk_params(self) -> dict:
+        return dict(alphas=np.asarray(self.alphas, dtype=np.float64), fit_intercept=self.fit_intercept,
+                    store_cv_results=self.store_cv_results)
 
     def __repr__(self) -> str:
         return f"B200RidgeCV(alphas={self.alphas!r})"
@@ -384,15 +424,10 @@ _MESSAGE_RIDGE = ("Linear regression models with a zero l1 penalization strength
 
 def _gram_of_rows(ctx: native.Context, X, y, row_mask, mask_keep: int) -> int:
     """S of the rows (b2_gram_reset + b2_gram_accumulate: the Gram dispatch every fit uses) left resident; returns D."""
-    X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-    d = X.shape[1]
-    try:
-        ctx.gram_reset(d)
+    with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+        ctx.gram_reset(X.shape[1])
         ctx.gram_accumulate(X, y, row_mask, mask_keep)
-    finally:
-        for a in owned:
-            a.free()
-    return d
+    return X.shape[1]
 
 
 def _solve_path(ctx: native.Context, d: int, who: str, **kw) -> dict:
@@ -400,8 +435,7 @@ def _solve_path(ctx: native.Context, d: int, who: str, **kw) -> dict:
         return ctx.solve_enet_path(**kw)
     except ValueError as exc:
         if "no row kept" in str(exc):
-            raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
-                             f"{who}.") from None
+            raise _too_few_rows((0, d), by=who) from None
         raise
 
 
@@ -421,12 +455,13 @@ def _warn_unconverged(ctx: native.Context, res: dict, l1_ratio: float, max_iter:
         warnings.warn(message, ConvergenceWarning, stacklevel=3)
 
 
-class B200ElasticNet:
+class B200ElasticNet(_B200Estimator):
     """``sklearn.linear_model.ElasticNet`` (cyclic selection) fitted on the H100: the rows go through the Gram kernels
     once, then ``b2_solve_enet_path`` runs sklearn's Gram coordinate descent (``precompute=True``) for the one alpha on
     one SM.  Sets coef_, intercept_, dual_gap_, n_iter_ and n_features_in_; ``to_sklearn()`` returns a genuine
-    ElasticNet carrying them."""
+    ElasticNet carrying them (``precompute=True``: the Gram solver this fit restates)."""
     _sk_name = "ElasticNet"
+    _sk_attrs = ("coef_", "intercept_", "dual_gap_", "n_iter_", "n_features_in_")
 
     def __init__(self, alpha: float = 1.0, *, l1_ratio: float = 0.5, fit_intercept: bool = True, max_iter: int = 1000,
                  tol: float = 1e-4, positive: bool = False, warm_start: bool = False, selection: str = "cyclic",
@@ -441,17 +476,10 @@ class B200ElasticNet:
         self.selection = selection
         self._ctx = ctx
 
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
-
     def fit(self, X, y, row_mask=None, mask_keep: int = 1):
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit to rows equal to ``mask_keep``."""
-        if self.selection == "random":
-            raise ValueError("selection='random' is not supported: the GPU solver runs sklearn's cyclic order only")
-        if self.selection != "cyclic":
-            raise ValueError("selection should be either random or cyclic.")
+        _check_selection(self.selection)
         if not (np.isfinite(self.alpha) and self.alpha >= 0):
             raise ValueError(f"alpha must be a finite float >= 0, got {self.alpha!r}")
         ctx = self.ctx
@@ -463,8 +491,7 @@ class B200ElasticNet:
                           max_iter=self.max_iter, tol=self.tol, positive=self.positive, coef_init=coef_init,
                           fit_intercept=self.fit_intercept)
         coef, b0 = res["coefs"][0], float(res["intercepts"][0])
-        if not (np.all(np.isfinite(coef)) and np.isfinite(b0)):
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(coef, b0)
         _warn_unconverged(ctx, res, self.l1_ratio, self.max_iter)
         self.coef_ = coef.copy()
         self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
@@ -473,34 +500,10 @@ class B200ElasticNet:
         self.n_features_in_ = int(d)
         return self
 
-    def predict(self, X):
-        ctx = self.ctx
-        if isinstance(X, native.DeviceArray):
-            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
-            return yhat
-        Xh = _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
-                             f"{self.n_features_in_} features as input.")
-        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
-        return yhat.astype(np.float64)
-
     def _sk_params(self) -> dict:
         return dict(alpha=self.alpha, l1_ratio=self.l1_ratio, fit_intercept=self.fit_intercept, precompute=True,
                     max_iter=self.max_iter, tol=self.tol, positive=self.positive, warm_start=self.warm_start,
                     selection=self.selection)
-
-    def to_sklearn(self):
-        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
-        intercept_).  ``precompute=True``: the Gram solver this fit restates."""
-        from sklearn import linear_model
-        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
-        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        reg.intercept_ = np.float64(self.intercept_)
-        reg.dual_gap_ = np.float64(self.dual_gap_)
-        reg.n_iter_ = int(self.n_iter_)
-        reg.n_features_in_ = int(self.n_features_in_)
-        return reg
 
     def __repr__(self) -> str:
         return f"B200{self._sk_name}(alpha={self.alpha}, l1_ratio={self.l1_ratio})"
@@ -534,13 +537,7 @@ def enet_path(X, y, *, l1_ratio=0.5, eps=1e-3, alphas=100, coef_init=None, retur
     ``fit_intercept=True`` the path runs on the centred Gram and the intercepts of every alpha are appended to the
     returned tuple."""
     ctx = ctx if ctx is not None else default_context()
-    if isinstance(alphas, (int, np.integer)) and not isinstance(alphas, bool):
-        al, n_alphas = None, int(alphas)
-        if n_alphas < 1:
-            raise ValueError(f"alphas must be >= 1 when given as an integer, got {n_alphas}")
-    else:
-        al = np.sort(np.asarray(alphas, dtype=np.float64).ravel())[::-1]
-        n_alphas = al.size
+    al, n_alphas = _alpha_grid(alphas)
     d = _gram_of_rows(ctx, X, y, row_mask, mask_keep)
     res = _solve_path(ctx, d, "enet_path", l1_ratio=l1_ratio, alphas=al, n_alphas=n_alphas, eps=eps,
                       max_iter=max_iter, tol=tol, positive=positive, coef_init=coef_init, fit_intercept=fit_intercept)
@@ -637,13 +634,16 @@ def _fold_tolerances(fold_S: np.ndarray, tol: float, fit_intercept: bool):
     return rows, tols
 
 
-class B200ElasticNetCV:
+class B200ElasticNetCV(_B200Estimator):
     """``sklearn.linear_model.ElasticNetCV`` (Gram solver, cyclic selection) on the H100: one pass over the rows gives
     the statistic of every fold (``b2_gram_folds``), one launch runs the path of every (l1_ratio, fold) on the sum of
     the other folds and forms its held-out error from the fold's own statistic (``b2_solve_enet_cv``), and the refit at
     the chosen (alpha, l1_ratio) runs on the summed statistic (``b2_solve_enet_path``).  Sets sklearn's attributes;
-    ``to_sklearn()`` returns a genuine ElasticNetCV carrying them."""
+    ``to_sklearn()`` returns a genuine ElasticNetCV carrying them (``precompute=True``: the Gram solver this fit
+    restates)."""
     _sk_name = "ElasticNetCV"
+    _sk_attrs = ("alpha_", "l1_ratio_", "alphas_", "mse_path_", "coef_", "intercept_", "dual_gap_", "n_iter_",
+                 "n_features_in_")
 
     def __init__(self, *, l1_ratio=0.5, eps: float = 1e-3, alphas=100, fit_intercept: bool = True, precompute="auto",
                  max_iter: int = 1000, tol: float = 1e-4, cv=None, positive: bool = False, selection: str = "cyclic",
@@ -660,48 +660,27 @@ class B200ElasticNetCV:
         self.selection = selection
         self._ctx = ctx
 
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
-
     def _l1_ratios(self) -> np.ndarray:
         return np.atleast_1d(np.asarray(self.l1_ratio, dtype=np.float64)).ravel()
 
     def fit(self, X, y, row_mask=None, mask_keep: int = 1):
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit and the folds to rows equal to ``mask_keep``."""
-        if self.selection == "random":
-            raise ValueError("selection='random' is not supported: the GPU solver runs sklearn's cyclic order only")
-        if self.selection != "cyclic":
-            raise ValueError("selection should be either random or cyclic.")
+        _check_selection(self.selection)
         l1 = self._l1_ratios()
-        grid = isinstance(self.alphas, (int, np.integer)) and not isinstance(self.alphas, bool)
-        if grid:
-            al, n_alphas = None, int(self.alphas)
-            if n_alphas < 1:
-                raise ValueError(f"alphas must be >= 1 when given as an integer, got {n_alphas}")
-            if np.any(l1 == 0.0):
-                raise ValueError("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a "
-                                 "grid by providing your estimator with the appropriate `alphas=` argument.")
-        else:
-            al = np.sort(np.asarray(self.alphas, dtype=np.float64).ravel())[::-1]
-            n_alphas = al.size
+        al, n_alphas = _alpha_grid(self.alphas)
+        if al is None and np.any(l1 == 0.0):
+            raise ValueError("Automatic alpha grid generation is not supported for l1_ratio=0. Please supply a "
+                             "grid by providing your estimator with the appropriate `alphas=` argument.")
         ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        d = X.shape[1]
-        try:
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = X.shape[1]
             ids, K = fold_ids(X.shape[0], row_mask, mask_keep, self.cv)
-            if isinstance(X, native.DeviceArray):
-                ids = ctx.to_device(ids)
-                owned.append(ids)
-            fold_S = ctx.gram_folds(X, y, ids, K)
-        finally:
-            for a in owned:
-                a.free()
+            with _on_device(ctx, ids) if isinstance(X, native.DeviceArray) else contextlib.nullcontext(ids) as ids:
+                fold_S = ctx.gram_folds(X, y, ids, K)
         res = ctx.solve_enet_cv(K, l1, alphas=al, n_alphas=n_alphas, eps=self.eps, max_iter=self.max_iter,
                                 tol=self.tol, positive=self.positive, fit_intercept=self.fit_intercept)
-        if not np.all(np.isfinite(res["mse"])):
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(res["mse"])
         rows, tols = _fold_tolerances(fold_S, self.tol, self.fit_intercept)
         for li in range(l1.size):
             for k in range(K):
@@ -719,12 +698,11 @@ class B200ElasticNetCV:
                           max_iter=self.max_iter, tol=self.tol, positive=self.positive,
                           fit_intercept=self.fit_intercept)
         coef, b0 = ref["coefs"][0], float(ref["intercepts"][0])
-        if not (np.all(np.isfinite(coef)) and np.isfinite(b0)):
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(coef, b0)
         _warn_unconverged(ctx, ref, best_l1, self.max_iter)
         self.alpha_ = best_alpha
         self.l1_ratio_ = best_l1
-        self.alphas_ = (res["alphas"][0] if l1.size == 1 else res["alphas"]) if grid else al.copy()
+        self.alphas_ = (res["alphas"][0] if l1.size == 1 else res["alphas"]) if al is None else al.copy()
         self.mse_path_ = np.squeeze(res["mse"])
         self.coef_ = coef.copy()
         self.intercept_ = np.float64(b0 if self.fit_intercept else 0.0)
@@ -732,18 +710,6 @@ class B200ElasticNetCV:
         self.n_iter_ = int(ref["n_iter"][0])
         self.n_features_in_ = int(d)
         return self
-
-    def predict(self, X):
-        ctx = self.ctx
-        if isinstance(X, native.DeviceArray):
-            yhat, _ = ctx.score(X, self.coef_, float(self.intercept_))
-            return yhat
-        Xh = _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
-                             f"{self.n_features_in_} features as input.")
-        yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
-        return yhat.astype(np.float64)
 
     def _sk_params(self) -> dict:
         cv = self.cv
@@ -754,23 +720,6 @@ class B200ElasticNetCV:
                     precompute=True, max_iter=self.max_iter, tol=self.tol, cv=cv, positive=self.positive,
                     selection=self.selection)
 
-    def to_sklearn(self):
-        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable, predicts with coef_ and
-        intercept_).  ``precompute=True``: the Gram solver this fit restates."""
-        from sklearn import linear_model
-        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
-        reg.alpha_ = float(self.alpha_)
-        if hasattr(self, "l1_ratio_"):
-            reg.l1_ratio_ = float(self.l1_ratio_)
-        reg.alphas_ = np.asarray(self.alphas_, dtype=np.float64).copy()
-        reg.mse_path_ = np.asarray(self.mse_path_, dtype=np.float64).copy()
-        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        reg.intercept_ = np.float64(self.intercept_)
-        reg.dual_gap_ = np.float64(self.dual_gap_)
-        reg.n_iter_ = int(self.n_iter_)
-        reg.n_features_in_ = int(self.n_features_in_)
-        return reg
-
     def __repr__(self) -> str:
         return f"B200{self._sk_name}(l1_ratio={self.l1_ratio}, cv={self.cv!r})"
 
@@ -778,6 +727,7 @@ class B200ElasticNetCV:
 class B200LassoCV(B200ElasticNetCV):
     """``sklearn.linear_model.LassoCV``: B200ElasticNetCV with l1_ratio = 1 (no ``l1_ratio_``)."""
     _sk_name = "LassoCV"
+    _sk_attrs = tuple(a for a in B200ElasticNetCV._sk_attrs if a != "l1_ratio_")
 
     def __init__(self, *, eps: float = 1e-3, alphas=100, fit_intercept: bool = True, precompute="auto",
                  max_iter: int = 1000, tol: float = 1e-4, cv=None, positive: bool = False, selection: str = "cyclic",
@@ -800,16 +750,13 @@ class B200LassoCV(B200ElasticNetCV):
 
 
 # ---- BayesianRidge / ARDRegression: evidence maximisation on the fp64 Gram (DESIGN.md section 9) -------------------------
-class _B200Bayes:
+class _B200Bayes(_B200Estimator):
     """What BayesianRidge and ARDRegression share: a fit is the Gram pass with the least-squares solution w0 (``ctx.fit``;
     the minimum-norm solution when the factorisation refuses), one fp64 pass over the same rows for the anchor
     (``residual_moments`` at w0, which makes the residual sum of squares of every iteration exact), then one solve on the
     resident statistic.  ``predict(X, return_std=True)`` is one fp64 tensor-core pass (``score_std``)."""
-    _sk_name = ""
-
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
+    _sk_attrs = ("coef_", "intercept_", "alpha_", "lambda_", "sigma_", "scores_", "n_iter_", "X_offset_", "X_scale_",
+                 "n_features_in_")
 
     def _solve(self, ctx: native.Context, anchor) -> dict:
         raise NotImplementedError
@@ -817,29 +764,22 @@ class _B200Bayes:
     def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None):
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit to rows equal to ``mask_keep``."""
-        if sample_weight is not None:
-            raise ValueError(f"sample_weight is not supported by B200{self._sk_name}: every kept row has weight 1")
+        _refuse_sample_weight(sample_weight, f"B200{self._sk_name}")
         ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        d = X.shape[1]
-        try:
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = X.shape[1]
             try:
                 w0, b0 = ctx.fit(X, y, row_mask, mask_keep, 0.0, fit_intercept=self.fit_intercept)
             except np.linalg.LinAlgError:
                 w0, b0, _, _ = ctx.solve_spectral(1e-12, fit_intercept=self.fit_intercept)
             moments = ctx.residual_moments(X, y, w0, b0, row_mask, mask_keep, fit_intercept=self.fit_intercept)
-        finally:
-            for a in owned:
-                a.free()
         S = ctx.gram_export()
         n = S[d, d]
         need = 2 if self._sk_name == "ARDRegression" else 1
         if not n >= need:
-            raise ValueError(f"Found array with {int(n)} sample(s) (shape=({int(n)}, {d})) while a minimum of {need} is "
-                             f"required by B200{self._sk_name}.")
+            raise _too_few_rows((n, d), need, by=f"B200{self._sk_name}")
         res = self._solve(ctx, np.concatenate([w0, moments]))
-        if not (np.all(np.isfinite(res["coef"])) and np.isfinite(res["intercept"]) and np.isfinite(res["alpha"])):
-            raise ValueError("Input X or y contains NaN, infinity or a value too large for dtype('float32').")
+        _check_finite(res["coef"], res["intercept"], res["alpha"])
         self.coef_ = res["coef"]
         self.intercept_ = np.float64(res["intercept"] if self.fit_intercept else 0.0)
         self.alpha_ = np.float64(res["alpha"])
@@ -855,31 +795,13 @@ class _B200Bayes:
         return self.sigma_
 
     def predict(self, X, return_std: bool = False):
-        ctx = self.ctx
-        on_device = isinstance(X, native.DeviceArray)
-        Xh = X if on_device else _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
-                             f"{self.n_features_in_} features as input.")
+        """The linear prediction; with ``return_std`` (yhat, ystd) from one fp64 pass, float64 for host rows and f64
+        ``DeviceArray``s for device rows."""
         if not return_std:
-            yhat, _ = ctx.score(Xh, self.coef_, float(self.intercept_))
-            return yhat if on_device else yhat.astype(np.float64)
-        return ctx.score_std(Xh, self.X_offset_, self._full_sigma(), 1.0 / float(self.alpha_), self.coef_,
-                             float(self.intercept_))
-
-    def _sk_params(self) -> dict:
-        raise NotImplementedError
-
-    def to_sklearn(self):
-        """A real sklearn estimator with the attributes ``fit`` would have set (joblib-dumpable; its own
-        ``predict(X, return_std=True)`` works)."""
-        from sklearn import linear_model
-        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
-        for name in ("coef_", "intercept_", "alpha_", "lambda_", "sigma_", "scores_", "n_iter_", "X_offset_", "X_scale_",
-                     "n_features_in_"):
-            v = getattr(self, name)
-            setattr(reg, name, v.copy() if isinstance(v, np.ndarray) else v)
-        return reg
+            return super().predict(X)
+        ctx = self.ctx
+        return ctx.score_std(self._checked_rows(X), self.X_offset_, self._full_sigma(), 1.0 / float(self.alpha_),
+                             self.coef_, float(self.intercept_))
 
 
 class B200BayesianRidge(_B200Bayes):
@@ -975,10 +897,7 @@ class B200ARDRegression(_B200Bayes):
 
 
 # ---- PoissonRegressor / GammaRegressor / TweedieRegressor: Newton fits on GPU passes (DESIGN.md section 10) ------------
-_NAN_MESSAGE = "Input X or y contains NaN, infinity or a value too large for dtype('float32')."
-
-
-class _B200GLM:
+class _B200GLM(_B200Estimator):
     """What the three generalised linear regressors share: scikit-learn 1.9's ``_GeneralizedLinearRegressor.fit`` with
     ``solver="newton-cholesky"``, its ``NewtonSolver.solve`` restated on the host around GPU passes over the rows.  Each
     Newton iteration is one pass for the loss, gradient and fp64 Hessian (``glm_pass``) and one pass for all 21 candidate
@@ -988,12 +907,9 @@ class _B200GLM:
     loss-and-gradient passes, with scikit-learn's warnings.
 
     The fit is the float64 fit of the stored fp32 / bf16 values: it matches scikit-learn run on float64 copies of those
-    values (scikit-learn computes float32 input in float32)."""
-    _sk_name = ""
-
-    @property
-    def ctx(self) -> native.Context:
-        return self._ctx if self._ctx is not None else default_context()
+    values (scikit-learn computes float32 input in float32).  ``B200LogisticRegression`` runs the same ``fit`` with its
+    own hooks."""
+    _sk_attrs = ("coef_", "intercept_", "n_iter_", "n_features_in_")
 
     def _link_power(self):
         """(link, power, the name of scikit-learn's loss class)"""
@@ -1022,13 +938,26 @@ class _B200GLM:
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, n_iter_ and
         n_features_in_."""
-        if sample_weight is not None:
-            raise ValueError(f"sample_weight is not supported by B200{self._sk_name}: every kept row has weight 1")
-        link, power, loss_name = self._check_params()
-        ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        d = X.shape[1]
-        fi = bool(self.fit_intercept)
+        _refuse_sample_weight(sample_weight, f"B200{self._sk_name}")
+        model = self._check_params()
+        with self._stage_targets(X, y, row_mask, mask_keep) as (X, y, row_mask, labels):
+            d = X.shape[1]
+            run, line_search = self._passes(X, y, row_mask, mask_keep, model, labels)
+            coef, n_iter = self._newton(d, self._l2(labels), lambda: self._start(d, run, model, labels), run,
+                                        line_search)
+        self._store(coef, n_iter, d, labels)
+        return self
+
+    # -- the hooks of fit: (X, y, row_mask, labels) staged; the pass pair; the start; the L2 strength; the attributes --
+    @contextlib.contextmanager
+    def _stage_targets(self, X, y, row_mask, mask_keep):
+        with _stage_rows(self.ctx, X, y, row_mask) as rows:
+            yield rows + (None,)
+
+    def _passes(self, X, y, row_mask, mask_keep, model, labels):
+        """(run(coef, hessian), line_search(coef, step)) as ``_newton`` takes them"""
+        ctx, fi, d = self.ctx, bool(self.fit_intercept), X.shape[1]
+        link, power, _ = model
 
         def run(c, hessian):
             return ctx.glm_pass(X, y, c[:d], float(c[d]) if fi else 0.0, link=link, power=power, row_mask=row_mask,
@@ -1038,37 +967,38 @@ class _B200GLM:
             return ctx.glm_line_search(X, y, c[:d], float(c[d]) if fi else 0.0, step[:d],
                                        float(step[d]) if fi else 0.0, link=link, power=power,
                                        n_steps=native.GLM_STEPS, row_mask=row_mask, mask_keep=mask_keep)
+        return run, line_search
 
-        def start():                              # the first pass checks y; the intercept starts at link(mean y)
-            coef, warm = self._start_coef(d)
-            first = run(coef, warm)
-            n = first["kept"]
-            if n == 0:
-                raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required by "
-                                 f"B200{self._sk_name}.")
-            if first["y_nonfinite"] > 0 or not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
-                raise ValueError(_NAN_MESSAGE)
-            if first["y_out_of_range"] > 0:
-                raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
-            if warm:
-                return coef, first, n
-            if fi:
-                ybar = first["sum_y"] / n
-                coef[-1] = np.log(ybar) if link == native.GLM_LOG else ybar
-            return coef, run(coef, True), n
+    def _start(self, d, run, model, labels):
+        """the first pass checks y; the intercept starts at link(mean y)"""
+        link, _, loss_name = model
+        coef, warm = self._start_coef(d)
+        first = run(coef, warm)
+        n = first["kept"]
+        if n == 0:
+            raise _too_few_rows((0, d), by=f"B200{self._sk_name}")
+        if first["y_nonfinite"] > 0:
+            raise ValueError(_NAN_MESSAGE)
+        _check_finite(first["loss"], first["grad"])
+        if first["y_out_of_range"] > 0:
+            raise ValueError(f"Some value(s) of y are out of the valid range of the loss {loss_name!r}.")
+        if warm:
+            return coef, first, n
+        if self.fit_intercept:
+            ybar = first["sum_y"] / n
+            coef[-1] = np.log(ybar) if link == native.GLM_LOG else ybar
+        return coef, run(coef, True), n
 
-        try:
-            coef, n_iter = self._newton(d, float(self.alpha), start, run, line_search)
-        finally:
-            for a in owned:
-                a.free()
+    def _l2(self, labels) -> float:
+        return float(self.alpha)
+
+    def _store(self, coef, n_iter, d, labels) -> None:
         if self.fit_intercept:
             self.coef_, self.intercept_ = coef[:-1].copy(), np.float64(coef[-1])
         else:
             self.coef_, self.intercept_ = coef.copy(), 0.0
         self.n_iter_ = int(n_iter)
         self.n_features_in_ = int(d)
-        return self
 
     def _start_coef(self, d):
         """(the starting coefficients with the intercept last, zeros unless warm_start finds a fit; warm)"""
@@ -1189,36 +1119,24 @@ class _B200GLM:
                               stacklevel=3)
         return coef, iteration - 1
 
-    def _staged(self, X):
-        on_device = isinstance(X, native.DeviceArray)
-        Xh = X if on_device else _as_f32_matrix(X)
-        if Xh.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {Xh.shape[1]} features, but B200{self._sk_name} is expecting "
-                             f"{self.n_features_in_} features as input.")
-        return Xh
-
     def predict(self, X):
         """mu = exp(X coef_ + intercept_) (log link) or X coef_ + intercept_ in fp64: float64 for host rows, an f64
         ``DeviceArray`` for device rows."""
         link = self._link_power()[0]
-        return self.ctx.glm_predict(self._staged(X), self.coef_, float(self.intercept_), link=link)
+        return self.ctx.glm_predict(self._checked_rows(X), self.coef_, float(self.intercept_), link=link)
 
     def score(self, X, y, row_mask=None, mask_keep: int = 1):
         """D^2, the fraction of deviance explained (scikit-learn's ``score``): one pass at the model and one at the
         intercept-only model link(mean y), both over the kept rows."""
         link, power, loss_name = self._link_power()
         ctx = self.ctx
-        X, y, row_mask, owned = _stage_rows(ctx, X, y, row_mask)
-        if X.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {X.shape[1]} features, but B200{self._sk_name} is expecting "
-                             f"{self.n_features_in_} features as input.")
-        d = X.shape[1]
-        try:
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = self._checked_rows(X).shape[1]
             kw = dict(link=link, power=power, row_mask=row_mask, mask_keep=mask_keep, hessian=False)
             model = ctx.glm_pass(X, y, self.coef_, float(self.intercept_), **kw)
             n = model["kept"]
             if n == 0:
-                raise ValueError(f"Found array with 0 sample(s) (shape=(0, {d})) while a minimum of 1 is required.")
+                raise _too_few_rows((0, d))
             if model["y_nonfinite"] > 0:
                 raise ValueError(_NAN_MESSAGE)
             if model["y_out_of_range"] > 0:
@@ -1226,24 +1144,12 @@ class _B200GLM:
             ybar = model["sum_y"] / n
             y_mean = np.log(ybar) if link == native.GLM_LOG else ybar
             null = ctx.glm_pass(X, y, np.zeros(d), float(y_mean), **kw)
-        finally:
-            for a in owned:
-                a.free()
         constant = model["const"] / n
         deviance, deviance_null = model["loss"] / n, null["loss"] / n
         return float(1 - (deviance + constant) / (deviance_null + constant))
 
-    def to_sklearn(self):
-        """A real scikit-learn estimator with the attributes ``fit`` would have set (joblib-dumpable); ``_base_loss`` is
-        set as scikit-learn's fit sets it, because its ``predict`` and ``score`` read it."""
-        from sklearn import linear_model
-        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
-        reg.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        reg.intercept_ = self.intercept_
-        reg.n_iter_ = int(self.n_iter_)
-        reg.n_features_in_ = int(self.n_features_in_)
-        reg._base_loss = reg._get_loss()
-        return reg
+    def _sk_prepare(self, reg) -> None:
+        reg._base_loss = reg._get_loss()          # scikit-learn's fit sets it; its predict and score read it
 
     def __repr__(self) -> str:
         return f"B200{self._sk_name}(alpha={self.alpha})"
@@ -1350,6 +1256,7 @@ class B200LogisticRegression(_B200GLM):
     Refused: more than two classes (multinomial fits are not supported), l1_ratio != 0, class_weight, sample_weight and
     any solver but 'newton-cholesky'.  verbose is accepted and has no effect."""
     _sk_name = "LogisticRegression"
+    _sk_attrs = ("coef_", "intercept_", "classes_", "n_iter_", "n_features_in_")
 
     def __init__(self, *, C: float = 1.0, l1_ratio: float = 0.0, tol: float = 1e-4, fit_intercept: bool = True,
                  class_weight=None, solver: str = "newton-cholesky", max_iter: int = 100, verbose: int = 0,
@@ -1398,8 +1305,7 @@ class B200LogisticRegression(_B200GLM):
             row_mask = row_mask.to_host()
         kept = y if row_mask is None else y[np.asarray(row_mask).ravel() == mask_keep]
         if kept.size == 0:
-            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required by "
-                             "B200LogisticRegression.")
+            raise _too_few_rows((0,), by="B200LogisticRegression")
         if kept.dtype.kind in "fc":
             if np.isnan(kept).any():
                 raise ValueError("Input y contains NaN.")
@@ -1419,8 +1325,7 @@ class B200LogisticRegression(_B200GLM):
         """(classes_ (fp32), kept rows) of an f32 DeviceArray y, from one label scan on the device"""
         st = ctx.label_scan(y, row_mask, mask_keep)
         if st["kept"] == 0:
-            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required by "
-                             "B200LogisticRegression.")
+            raise _too_few_rows((0,), by="B200LogisticRegression")
         if st["nonfinite"] > 0:
             raise ValueError("Input y contains NaN or infinity.")
         if st["nonintegral"] > 0:
@@ -1432,60 +1337,69 @@ class B200LogisticRegression(_B200GLM):
                              "not supported")
         return np.array([st["min"], st["max"]], dtype=np.float32), int(st["kept"])
 
-    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None):
-        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); y: host labels of
-        any dtype or an f32 ``DeviceArray``; ``row_mask`` (uint8 per row) restricts the fit to rows equal to
-        ``mask_keep``.  Sets coef_ (1, D), intercept_ (1,), classes_, n_iter_ (1,) and n_features_in_."""
-        if sample_weight is not None:
-            raise ValueError("sample_weight is not supported by B200LogisticRegression: every kept row has weight 1")
-        self._check_params()
+    # -- the hooks of _B200GLM.fit; labels: (classes_, kept rows, the negative and the positive label y holds) ----------
+    @contextlib.contextmanager
+    def _stage_targets(self, X, y, row_mask, mask_keep, fitting: bool = True):
+        """(X, y, row_mask, labels) for the logistic passes, for the body of the ``with``; ``fit`` and ``score`` share
+        it.  Device y (device rows only) is read as stored, with the labels of a label scan (fitting) or of classes_.
+        Host y becomes float32 {0, 1}: classes_ found in y (fitting), or NaN outside classes_; it goes up to the
+        device beside device rows and is staged with host rows."""
         ctx = self.ctx
-        owned = []
-        try:
-            if isinstance(y, native.DeviceArray):
-                if not isinstance(X, native.DeviceArray):
-                    raise ValueError("device y needs device rows: X must be a DeviceArray too")
+        if isinstance(y, native.DeviceArray):
+            if not isinstance(X, native.DeviceArray):
+                raise ValueError("device y needs device rows: X must be a DeviceArray too")
+            if fitting:
                 classes, n = self._device_labels(ctx, y, row_mask, mask_keep)
-                neg, pos = float(classes[0]), float(classes[1])
+                yield X, y, row_mask, (classes, n, float(classes[0]), float(classes[1]))
             else:
-                classes, y01, n = self._host_labels(y, row_mask, mask_keep)
-                neg, pos = 0.0, 1.0
-                if isinstance(X, native.DeviceArray):
-                    y = ctx.to_device(y01)
-                    owned.append(y)
-                else:
-                    X, y, row_mask, owned = _stage_rows(ctx, X, y01, row_mask)
-            d = X.shape[1]
-            fi = bool(self.fit_intercept)
+                yield X, y, row_mask, (None, None) + self._fp32_classes()
+            return
+        if fitting:
+            classes, y01, n = self._host_labels(y, row_mask, mask_keep)
+        else:
+            yh = np.asarray(y).ravel()
+            y01 = np.where(yh == self.classes_[1], 1.0, np.where(yh == self.classes_[0], 0.0, np.nan))
+            y01, classes, n = y01.astype(np.float32), None, None
+        if isinstance(X, native.DeviceArray):
+            with _on_device(ctx, y01) as y:
+                yield X, y, row_mask, (classes, n, 0.0, 1.0)
+        else:
+            with _stage_rows(ctx, X, y01, row_mask) as (X, y, row_mask):
+                yield X, y, row_mask, (classes, n, 0.0, 1.0)
 
-            def run(c, hessian):
-                return ctx.logistic_pass(X, y, c[:d], float(c[d]) if fi else 0.0, neg, pos, row_mask=row_mask,
-                                         mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
+    def _passes(self, X, y, row_mask, mask_keep, model, labels):
+        ctx, fi, d = self.ctx, bool(self.fit_intercept), X.shape[1]
+        neg, pos = labels[2:]
 
-            def line_search(c, step):
-                return ctx.logistic_line_search(X, y, c[:d], float(c[d]) if fi else 0.0, step[:d],
-                                                float(step[d]) if fi else 0.0, neg, pos, n_steps=native.GLM_STEPS,
-                                                row_mask=row_mask, mask_keep=mask_keep)
+        def run(c, hessian):
+            return ctx.logistic_pass(X, y, c[:d], float(c[d]) if fi else 0.0, neg, pos, row_mask=row_mask,
+                                     mask_keep=mask_keep, fit_intercept=fi, hessian=hessian)
 
-            def start():                          # the first pass is the Hessian pass at the start
-                coef, _ = self._start_coef(d)
-                first = run(coef, True)
-                if first["kept"] != n or first["y_out_of_range"] > 0:
-                    raise RuntimeError("the logistic pass saw other labels than the label check")
-                if not (np.isfinite(first["loss"]) and np.all(np.isfinite(first["grad"]))):
-                    raise ValueError(_NAN_MESSAGE)
-                return coef, first, n
+        def line_search(c, step):
+            return ctx.logistic_line_search(X, y, c[:d], float(c[d]) if fi else 0.0, step[:d],
+                                            float(step[d]) if fi else 0.0, neg, pos, n_steps=native.GLM_STEPS,
+                                            row_mask=row_mask, mask_keep=mask_keep)
+        return run, line_search
 
-            coef, n_iter = self._newton(d, 1.0 / (float(self.C) * n), start, run, line_search)
-        finally:
-            for a in owned:
-                a.free()
+    def _start(self, d, run, model, labels):
+        """the first pass is the Hessian pass at the start"""
+        n = labels[1]
+        coef, _ = self._start_coef(d)
+        first = run(coef, True)
+        if first["kept"] != n or first["y_out_of_range"] > 0:
+            raise RuntimeError("the logistic pass saw other labels than the label check")
+        _check_finite(first["loss"], first["grad"])
+        return coef, first, n
+
+    def _l2(self, labels) -> float:
+        return 1.0 / (float(self.C) * labels[1])
+
+    def _store(self, coef, n_iter, d, labels) -> None:
         self.coef_ = coef[:d].reshape(1, d).copy()
         self.intercept_ = np.array([coef[d]]) if self.fit_intercept else np.zeros(1)
-        self.classes_ = classes
+        self.classes_ = labels[0]
         self.n_iter_ = np.array([n_iter], dtype=np.int32)
         self.n_features_in_ = int(d)
-        return self
 
     def _fp32_classes(self):
         """(neg, pos): classes_ as the fp32 labels device y holds and device predictions return"""
@@ -1495,7 +1409,7 @@ class B200LogisticRegression(_B200GLM):
 
     def _predict(self, X, **want):
         """one logistic_predict pass; host rows take the labels 0 and 1 (indices into classes_)"""
-        X = self._staged(X)
+        X = self._checked_rows(X)
         neg, pos = self._fp32_classes() if isinstance(X, native.DeviceArray) else (0.0, 1.0)
         return self.ctx.logistic_predict(X, self.coef_[0], float(self.intercept_[0]), neg, pos, **want)
 
@@ -1525,47 +1439,18 @@ class B200LogisticRegression(_B200GLM):
     def score(self, X, y, row_mask=None, mask_keep: int = 1):
         """Accuracy over the kept rows (labels outside classes_ count as wrong): the correct count of one pass."""
         ctx = self.ctx
-        owned = []
-        try:
-            if isinstance(y, native.DeviceArray):
-                if not isinstance(X, native.DeviceArray):
-                    raise ValueError("device y needs device rows: X must be a DeviceArray too")
-                neg, pos = self._fp32_classes()
-            else:
-                yh = np.asarray(y).ravel()
-                y01 = np.where(yh == self.classes_[1], 1.0, np.where(yh == self.classes_[0], 0.0, np.nan))
-                y01 = y01.astype(np.float32)
-                neg, pos = 0.0, 1.0
-                if isinstance(X, native.DeviceArray):
-                    y = ctx.to_device(y01)
-                    owned.append(y)
-                else:
-                    X, y, row_mask, owned = _stage_rows(ctx, X, y01, row_mask)
-            if X.shape[1] != self.n_features_in_:
-                raise ValueError(f"X has {X.shape[1]} features, but B200LogisticRegression is expecting "
-                                 f"{self.n_features_in_} features as input.")
-            s = ctx.logistic_pass(X, y, self.coef_[0], float(self.intercept_[0]), neg, pos, row_mask=row_mask,
-                                  mask_keep=mask_keep, hessian=False)
-        finally:
-            for a in owned:
-                a.free()
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=False) as (X, y, row_mask, labels):
+            s = ctx.logistic_pass(self._checked_rows(X), y, self.coef_[0], float(self.intercept_[0]), *labels[2:],
+                                  row_mask=row_mask, mask_keep=mask_keep, hessian=False)
         if s["kept"] == 0:
-            raise ValueError("Found array with 0 sample(s) (shape=(0,)) while a minimum of 1 is required.")
+            raise _too_few_rows((0,))
         return float(s["correct"] / s["kept"])
 
-    def to_sklearn(self):
-        """A real ``sklearn.linear_model.LogisticRegression(solver="newton-cholesky")`` with the fitted attributes
-        (joblib-dumpable)."""
-        from sklearn.linear_model import LogisticRegression
-        clf = LogisticRegression(C=self.C, l1_ratio=self.l1_ratio, tol=self.tol, fit_intercept=self.fit_intercept,
-                                 solver="newton-cholesky", max_iter=self.max_iter, verbose=self.verbose,
-                                 warm_start=self.warm_start)
-        clf.coef_ = np.asarray(self.coef_, dtype=np.float64).copy()
-        clf.intercept_ = np.asarray(self.intercept_, dtype=np.float64).copy()
-        clf.classes_ = np.asarray(self.classes_).copy()
-        clf.n_iter_ = np.asarray(self.n_iter_, dtype=np.int32).copy()
-        clf.n_features_in_ = int(self.n_features_in_)
-        return clf
+    def _sk_params(self) -> dict:
+        return dict(C=self.C, l1_ratio=self.l1_ratio, tol=self.tol, fit_intercept=self.fit_intercept,
+                    solver="newton-cholesky", max_iter=self.max_iter, verbose=self.verbose, warm_start=self.warm_start)
+
+    _sk_prepare = _B200Estimator._sk_prepare      # LogisticRegression has no _base_loss to set
 
     def __repr__(self) -> str:
         return f"B200LogisticRegression(C={self.C})"
