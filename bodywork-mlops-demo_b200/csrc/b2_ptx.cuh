@@ -1,6 +1,7 @@
 // b2_ptx.cuh -- PTX wrappers shared by the TMA / mbarrier pipelines (gram_tc.cu, gram_narrow.cu, score.cu), and the
 // bulk-copy ring (ring_init, ring_produce) of the streaming kernels gram_narrow_kernel, score_tma_kernel,
-// score_narrow_kernel, grad_tma_kernel and grad_narrow_kernel.
+// score_narrow_kernel, grad_tma_kernel and grad_narrow_kernel, and of the fp64 tile passes' TileRing (b2_dmma.cuh:
+// glm_kernel, loo_kernel, score_std_kernel).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>

@@ -19,34 +19,20 @@
 // in a fixed order, the ordered reduce adds the CTAs in order: two calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
-#include "b2_ptx.cuh"
 
 namespace b2 {
 namespace {
 
-constexpr int kGlmRows = 32;                       // rows per tile
-constexpr int kGlmWarps = 8;                       // consumer warps
-constexpr int kGlmConsumers = 32 * kGlmWarps;
-constexpr int kGlmThreads = kGlmConsumers + 32;    // + the producer warp of the ring
-constexpr int kGlmStages = 3;
 constexpr int kGlmBlocks = (kMaxD + 1 + 15) / 16;  // 9 blocks of 16 columns of [x 1]
-constexpr int kGlmSB = (kGlmBlocks * (kGlmBlocks + 1) / 2 + kGlmWarps - 1) / kGlmWarps;   // 16 x 16 blocks per warp: 6
-constexpr uint32_t kGlmXStage = kGlmRows * kMaxD * 4;                       // 16 KB: 32 fp32 rows of 128 features
-constexpr uint32_t kGlmYStage = kGlmRows * 4;
-constexpr uint32_t kGlmOffY = kGlmStages * kGlmXStage;
-constexpr uint32_t kGlmOffBar = kGlmOffY + kGlmStages * kGlmYStage;
-constexpr uint32_t kGlmRingBytes = kGlmOffBar + 2 * kGlmStages * 8 + 16;    // the doubles start here (16-byte aligned)
+// 16 x 16 blocks per warp: 6
+constexpr int kGlmSB = (kGlmBlocks * (kGlmBlocks + 1) / 2 + kTileWarps - 1) / kTileWarps;
 
 __host__ __device__ inline int glm_dp(int d) { return (d + 1 + 15) & ~15; }   // columns of [x 1], padded to 16
-__host__ __device__ inline int glm_zpitch(int dp) { return dp + 4; }          // 4 mod 16 doubles: no bank conflicts
 size_t glm_smem_bytes(int dp, bool ring, int mode) {
-  const size_t tile = (size_t)kGlmRows * glm_zpitch(dp);
-  return (ring ? kGlmRingBytes : 0) +
-         sizeof(double) * (tile * (mode == kGlmHessian ? 2 : 1) + 3 * kMaxD + 8 + 3 * kGlmRows + 2 * kGlmWarps * 32 + 48);
-}
-
-__device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
-  asm volatile("bar.sync 1, %0;" ::"r"(kGlmConsumers) : "memory");
+  const size_t tile = (size_t)kTileRows * tile_vpitch(dp);
+  return tile_ring_bytes(ring, true) +
+         sizeof(double) *
+             (tile * (mode == kGlmHessian ? 2 : 1) + 3 * kMaxD + 8 + 3 * kTileRows + 2 * kTileWarps * 32 + 48);
 }
 
 // The pointwise half-Tweedie loss, gradient and Hessian in eta, sklearn's Cython branches: the log link at any power
@@ -146,28 +132,27 @@ __device__ __forceinline__ bool glm_y_in_range(double p, double y) {
 // classified correctly ((eta > 0) == positive label, a row with neither label never).  A compile-time family keeps the
 // Tweedie instantiations as they were.
 template <typename T, bool RING, int MODE, int FAM>
-__global__ void __launch_bounds__(kGlmThreads, 1)
+__global__ void __launch_bounds__(kTileThreads, 1)
 glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
            const uint8_t* __restrict__ mask, int keep, const double* __restrict__ op, int link, double power,
            int n_steps, double* __restrict__ part) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const uint32_t sbase = smem_u32(smem_raw);
-  const uint32_t bar_full = sbase + kGlmOffBar, bar_empty = bar_full + 8 * kGlmStages;
-  const int dp = glm_dp(d), zp = glm_zpitch(dp), nb = dp / 16, nsb = nb * (nb + 1) / 2;
-  double* Zs = reinterpret_cast<double*>(smem_raw + (RING ? kGlmRingBytes : 0));   // [row][zp]: z = [x 1 0...]
-  double* HZs = Zs + (MODE == kGlmHessian ? kGlmRows * zp : 0);                    // |h| z
-  double* wv = HZs + kGlmRows * zp;        // [kMaxD] w
+  TileRing<T, RING, true> tiles{X, n, d, ldx, y, mask, keep, smem_u32(smem_raw)};
+  const int dp = glm_dp(d), zp = tile_vpitch(dp), nb = dp / 16, nsb = nb * (nb + 1) / 2;
+  double* Zs = reinterpret_cast<double*>(smem_raw + tile_ring_bytes(RING, true));   // [row][zp]: z = [x 1 0...]
+  double* HZs = Zs + (MODE == kGlmHessian ? kTileRows * zp : 0);                   // |h| z
+  double* wv = HZs + kTileRows * zp;       // [kMaxD] w
   double* sv = wv + kMaxD;                 // [kMaxD] the Newton step (kGlmLadder)
   double* yv = sv + kMaxD;                 // y (0 for rows not kept)
-  double* gs = yv + kGlmRows;              // g (0 for rows not kept)
-  double* hs = gs + kGlmRows;              // |h| (0 for rows not kept)
-  double* red = hs + kGlmRows;             // [warp][32] the warps' sums
-  double* lsum = red + kGlmWarps * 32;     // [warp][u][8] the scalar sums of the rows warp + 8 u (kGlmGradient / Hessian)
-  double* gsum = lsum + kGlmWarps * 32;    // [kMaxD + 8] the gradient sums, entry j of thread j
+  double* gs = yv + kTileRows;             // g (0 for rows not kept)
+  double* hs = gs + kTileRows;             // |h| (0 for rows not kept)
+  double* red = hs + kTileRows;            // [warp][32] the warps' sums
+  double* lsum = red + kTileWarps * 32;    // [warp][u][8] the scalar sums of the rows warp + 8 u (gradient / Hessian)
+  double* gsum = lsum + kTileWarps * 32;   // [kMaxD + 8] the gradient sums, entry j of thread j
   int* sbi = reinterpret_cast<int*>(gsum + kMaxD + 8);   // the 16 x 16 blocks on and above the diagonal
   int* sbj = sbi + 48;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
-  for (int t = tid; t < kGlmWarps * 32; t += blockDim.x) lsum[t] = 0.0;
+  for (int t = tid; t < kTileWarps * 32; t += blockDim.x) lsum[t] = 0.0;
   for (int t = tid; t < kMaxD + 8; t += blockDim.x) gsum[t] = 0.0;
   for (int t = tid; t < kMaxD; t += blockDim.x) {
     wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
@@ -179,9 +164,8 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
       for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
   }
   const double b = op[kGlmOpMisc], db = op[kGlmOpMisc + 1];
-  const int64_t n_tiles = (n + kGlmRows - 1) / kGlmRows;
-  if constexpr (RING) ring_init<kGlmStages>(bar_full, bar_empty, kGlmWarps);   // includes a block barrier
-  else __syncthreads();
+  const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
+  tiles.start();
   // kGlmLadder: lane k sums the loss at step k.  The other sums stay in shared memory (lsum, gsum), which leaves the
   // registers to the Hessian's accumulators.
   double s_loss = 0.0;
@@ -190,58 +174,21 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   for (int u = 0; u < kGlmSB; ++u)
 #pragma unroll
     for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
-  if (RING && warp == kGlmWarps) {
-    if (lane == 0)
-      ring_produce<kGlmStages>(bar_full, bar_empty, (int)n_tiles, kGlmRows, X, (uint32_t)(d * sizeof(T)), sbase,
-                               kGlmXStage, true, y, sbase + kGlmOffY, kGlmYStage, false, nullptr, 0u, 0u);
-  } else {
-    int s = 0;
-    uint32_t phase = 0;
+  if (!tiles.produce()) {
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int64_t row0 = tile * kGlmRows;
-      bool use[kGlmRows / kGlmWarps];
-      // (1) the tile
-      if constexpr (RING) {
-#pragma unroll
-        for (int u = 0; u < kGlmRows / kGlmWarps; ++u)   // the mask comes from global memory, before the wait
-          use[u] = mask == nullptr || __ldg(mask + row0 + warp + kGlmWarps * u) == (uint8_t)keep;
-        mbar_wait(bar_full + 8 * s, phase);
-        const uint32_t xs = sbase + s * kGlmXStage, ys = sbase + kGlmOffY + s * kGlmYStage;
-#pragma unroll
-        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
-          const int r = warp + kGlmWarps * u;
-          const uint32_t xr = xs + (uint32_t)(r * d) * (uint32_t)sizeof(T);
-          for (int j = lane; j < dp; j += 32) {
-            const bool live = use[u] && j < d;
-            const float x = live ? raw_ld_shared<T>(xr + (uint32_t)j * (uint32_t)sizeof(T)) : 0.f;
-            Zs[r * zp + j] = live ? (double)x : (use[u] && j == d ? 1.0 : 0.0);
-          }
-          if (lane == 0) yv[r] = use[u] ? (double)ld_shared_f32(ys + 4u * (uint32_t)r) : 0.0;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_empty + 8 * s);      // the slot is converted: the producer may refill it
-        if (++s == kGlmStages) { s = 0; phase ^= 1u; }
-      } else {
-#pragma unroll
-        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
-          const int r = warp + kGlmWarps * u;
-          const int64_t row = row0 + r;
-          use[u] = row < n && (mask == nullptr || __ldg(mask + row) == (uint8_t)keep);
-          const T* xr = X + row * ldx;
-          for (int j = lane; j < dp; j += 32) {
-            const bool live = use[u] && j < d;
-            const float x = live ? ld_row_val<T>(xr + j) : 0.f;
-            Zs[r * zp + j] = live ? (double)x : (use[u] && j == d ? 1.0 : 0.0);
-          }
-          if (lane == 0) yv[r] = use[u] ? (double)__ldg(y + row) : 0.0;
-        }
-      }
+      // (1) the tile: z = [x 1 0...] and y, zero for rows not kept
+      bool use[kTileRowsPerWarp];
+      tiles.load(tile * kTileRows, dp, use,
+                 [&](int r, int j, bool kept, bool live, float x) {
+                   Zs[r * zp + j] = live ? (double)x : (kept && j == d ? 1.0 : 0.0);
+                 },
+                 [&](int r, bool, double yr) { yv[r] = yr; });
       __syncwarp();
       // (2) eta (and deta) of the warp's rows: every lane ends with the same value
-      double eta[kGlmRows / kGlmWarps], deta[kGlmRows / kGlmWarps];
+      double eta[kTileRowsPerWarp], deta[kTileRowsPerWarp];
 #pragma unroll
-      for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
-        const double* zr = Zs + (warp + kGlmWarps * u) * zp;
+      for (int u = 0; u < kTileRowsPerWarp; ++u) {
+        const double* zr = Zs + (warp + kTileWarps * u) * zp;
         double a = 0.0, c = 0.0;
         for (int j = lane; j < d; j += 32) {
           a = fma(zr[j], wv[j], a);
@@ -259,24 +206,24 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
       if constexpr (MODE == kGlmLadder) {
         const double t = ldexp(1.0, -lane);           // t = 1, 1/2, ... 2^-20: lane k < n_steps takes step k
 #pragma unroll
-        for (int u = 0; u < kGlmRows / kGlmWarps; ++u) {
+        for (int u = 0; u < kTileRowsPerWarp; ++u) {
           double l;
           if constexpr (FAM == kGlmBinomial)
-            l = binom_ladder_loss(yv[warp + kGlmWarps * u] == op[kGlmOpMisc + 3] ? 1.0 : 0.0, eta[u] + t * deta[u]);
+            l = binom_ladder_loss(yv[warp + kTileWarps * u] == op[kGlmOpMisc + 3] ? 1.0 : 0.0, eta[u] + t * deta[u]);
           else
-            l = glm_loss(link, power, yv[warp + kGlmWarps * u], eta[u] + t * deta[u]);
+            l = glm_loss(link, power, yv[warp + kTileWarps * u], eta[u] + t * deta[u]);
           s_loss += (use[u] && lane < n_steps) ? l : 0.0;
         }
       } else {
-        if (lane < kGlmRows / kGlmWarps) {            // lane u takes row warp + 8 u
+        if (lane < kTileRowsPerWarp) {            // lane u takes row warp + 8 u
           double e = eta[0];
           bool kept = use[0];
 #pragma unroll
-          for (int u = 1; u < kGlmRows / kGlmWarps; ++u) {
+          for (int u = 1; u < kTileRowsPerWarp; ++u) {
             e = lane == u ? eta[u] : e;
             kept = lane == u ? use[u] : kept;
           }
-          const int r = warp + kGlmWarps * lane;
+          const int r = warp + kTileWarps * lane;
           const double yy = yv[r];
           double l, gg, hh;
           double* ls = lsum + (warp * 4 + lane) * 8;
@@ -306,29 +253,29 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
           gs[r] = kept ? gg : 0.0;
           hs[r] = kept ? fabs(hh) : 0.0;
         }
-        consumer_sync();
+        tile_consumer_sync();
         // (4) the gradient, then (kGlmHessian) the |h|-scaled rows
         if (tid <= d) {
           double a = gsum[tid];
 #pragma unroll 8
-          for (int r = 0; r < kGlmRows; ++r) a = fma(gs[r], Zs[r * zp + tid], a);
+          for (int r = 0; r < kTileRows; ++r) a = fma(gs[r], Zs[r * zp + tid], a);
           gsum[tid] = a;
         }
         if constexpr (MODE == kGlmHessian) {
-          for (int t = tid; t < kGlmRows * dp; t += kGlmConsumers) {
+          for (int t = tid; t < kTileRows * dp; t += kTileConsumers) {
             const int r = t / dp, j = t - r * dp;
             HZs[r * zp + j] = hs[r] * Zs[r * zp + j];
           }
-          consumer_sync();
+          tile_consumer_sync();
           // (5) H += (|h| z)^T z over the tile's rows, the warp's blocks
 #pragma unroll
           for (int u = 0; u < kGlmSB; ++u) {
-            const int sb = warp + kGlmWarps * u;
+            const int sb = warp + kTileWarps * u;
             if (sb < nsb) {                               // warp-uniform
               const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
               const bool diag = sbi[sb] == sbj[sb];
 #pragma unroll
-              for (int ks = 0; ks < kGlmRows / 4; ++ks) {
+              for (int ks = 0; ks < kTileRows / 4; ++ks) {
                 const int r = 4 * ks + t4;
                 const double a0 = HZs[r * zp + ci], a1 = HZs[r * zp + ci + 8];
                 const double b0 = Zs[r * zp + cj], b1 = Zs[r * zp + cj + 8];
@@ -341,17 +288,17 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
           }
         }
       }
-      consumer_sync();
+      tile_consumer_sync();
     }
   }
   // the CTA's sums in a fixed order: the lanes of a warp, then the warps in order
   double* out = part + (size_t)blockIdx.x * kGlmPart;
   if constexpr (MODE == kGlmLadder) {
-    if (warp < kGlmWarps) red[warp * 32 + lane] = s_loss;
+    if (warp < kTileWarps) red[warp * 32 + lane] = s_loss;
     __syncthreads();
     if (tid < 32) {
       double v = 0.0;
-      for (int w = 0; w < kGlmWarps; ++w) v += red[w * 32 + tid];
+      for (int w = 0; w < kTileWarps; ++w) v += red[w * 32 + tid];
       out[tid] = v;
     }
   } else {
@@ -359,7 +306,7 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     if (tid < kGlmHess) {                          // the scalars, the gradient, zeros in the unused entries
       double r = 0.0;
       if (tid < (FAM == kGlmBinomial ? kGlmCorrect + 1 : 7))
-        for (int q = 0; q < kGlmWarps * 4; ++q) r += lsum[q * 8 + tid];
+        for (int q = 0; q < kTileWarps * 4; ++q) r += lsum[q * 8 + tid];
       else if (tid >= kGlmGrad && tid <= kGlmGrad + d)
         r = gsum[tid - kGlmGrad];
       out[tid] = r;
@@ -367,8 +314,8 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     if constexpr (MODE == kGlmHessian) {
 #pragma unroll
       for (int u = 0; u < kGlmSB; ++u) {
-        const int sb = warp + kGlmWarps * u;
-        if (warp < kGlmWarps && sb < nsb) {
+        const int sb = warp + kTileWarps * u;
+        if (warp < kTileWarps && sb < nsb) {
           const bool diag = sbi[sb] == sbj[sb];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -517,11 +464,9 @@ label_count_kernel(const float* __restrict__ y, int64_t n, const uint8_t* __rest
 int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                const uint8_t* mask, int keep, int mode, int family, int link, double power, int n_steps,
                bool first_block) {
-  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kGlmRows, first_block, [&](bool ring, const RowSpan& s) {
+  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kTileRows, first_block, [&](bool ring, const RowSpan& s) {
     // two CTAs per SM hide the latency of the per-tile steps where the shared memory allows it (all but the Hessian)
-    const int64_t n_tiles = (s.rows + kGlmRows - 1) / kGlmRows, cap = (int64_t)ctx->sm_count * (mode == kGlmHessian ? 1 : 2);
-    int grid = (int)(n_tiles < cap ? n_tiles : cap);
-    if (grid < 1) grid = 1;
+    const int grid = tile_grid(s.rows, ctx->sm_count, mode == kGlmHessian ? 1 : 2);
     const uint32_t smem = (uint32_t)glm_smem_bytes(glm_dp(d), ring, mode);
     const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
@@ -529,9 +474,8 @@ int launch_glm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
         return with_int<kGlmTweedie, kGlmBinomial>(family, [&](auto F) {
           constexpr int MODE = decltype(M)::value, FAM = decltype(F)::value;
           auto kernel = ring ? glm_kernel<T, true, MODE, FAM> : glm_kernel<T, false, MODE, FAM>;
-          return launch_smem(kernel, grid, ring ? kGlmThreads : kGlmConsumers, smem, ctx->stream, Xr, s.rows, d, ldx,
-                             s.y, s.mask, keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps,
-                             ctx->glm_part);
+          return launch_smem(kernel, grid, tile_threads(ring), smem, ctx->stream, Xr, s.rows, d, ldx, s.y, s.mask,
+                             keep, static_cast<const double*>(ctx->glm + kGlmOp), link, power, n_steps, ctx->glm_part);
         });
       });
     });

@@ -16,34 +16,14 @@
 // alpha in a fixed order; the ordered reduce adds the CTAs in order, so two calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
-#include "b2_ptx.cuh"
 
 namespace b2 {
 namespace {
 
-constexpr int kLooRows = 32;                       // rows per tile
-constexpr int kLooMT = kLooRows / 8;               // m-tiles of the DMMA per tile
-constexpr int kLooWarps = 8;                       // consumer warps
-constexpr int kLooConsumers = 32 * kLooWarps;
-constexpr int kLooThreads = kLooConsumers + 32;    // + the producer warp of the ring
-constexpr int kLooStages = 3;
-constexpr uint32_t kLooXStage = kLooRows * kMaxD * 4;                       // 16 KB: 32 fp32 rows of 128 features
-constexpr uint32_t kLooYStage = kLooRows * 4;
-constexpr uint32_t kLooOffY = kLooStages * kLooXStage;
-constexpr uint32_t kLooOffBar = kLooOffY + kLooStages * kLooYStage;
-constexpr uint32_t kLooRingBytes = kLooOffBar + 2 * kLooStages * 8 + 16;    // the doubles start here (16-byte aligned)
-
-__host__ __device__ inline int loo_dp(int d) { return (d + 7) & ~7; }
-__host__ __device__ inline int loo_qpitch(int dp) { return dp + 8; }
-__host__ __device__ inline int loo_vpitch(int dp) { return dp + 4; }
 size_t loo_smem_bytes(int dp, bool ring) {
-  return (ring ? kLooRingBytes : 0) +
-         sizeof(double) * ((size_t)dp * loo_qpitch(dp) + (size_t)kLooRows * loo_vpitch(dp) + 2 * kLooRows + kMaxD +
-                           (size_t)kLooWarps * kMaxAlphas);
-}
-
-__device__ __forceinline__ void consumer_sync() {   // the consumer warps only (the producer is inside ring_produce)
-  asm volatile("bar.sync 1, %0;" ::"r"(kLooConsumers) : "memory");
+  return tile_ring_bytes(ring, true) +
+         sizeof(double) * ((size_t)dp * tile_bpitch(dp) + (size_t)kTileRows * tile_vpitch(dp) + 2 * kTileRows + kMaxD +
+                           (size_t)kTileWarps * kMaxAlphas);
 }
 
 // the B operands of (3): Cw[j][a] = c_j / (lambda_j + alpha_a), W[j][a] = 1 / (lambda_j + alpha_a); 0 outside d x n_alphas
@@ -60,26 +40,25 @@ __global__ void loo_prep_kernel(double* __restrict__ loo, int d, int n_alphas) {
   }
 }
 
-// RING: rows [0, n), n a multiple of kLooRows, contiguous (ldx == d) and 16-byte aligned with y, through the bulk-copy
+// RING: rows [0, n), n a multiple of kTileRows, contiguous (ldx == d) and 16-byte aligned with y, through the bulk-copy
 // ring; otherwise rows [0, n) of any layout (stride ldx, fp32 or bf16, any alignment) from global memory.  Tiles
 // blockIdx.x, + gridDim.x, ...
 // Work of (3): the n_alphas are ceil(n_alphas / 8) n-tiles; each gets G = 8 / n-tiles warps, each warp a group of
-// ceil(kLooMT / G) m-tiles, so every warp holds at most one (n-tile, group) for the whole launch and its sums stay in
+// ceil(kTileMT / G) m-tiles, so every warp holds at most one (n-tile, group) for the whole launch and its sums stay in
 // registers.
 template <typename T, bool RING>
-__global__ void __launch_bounds__(kLooThreads, 1)
+__global__ void __launch_bounds__(kTileThreads, 1)
 loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
            const uint8_t* __restrict__ mask, int keep, const double* __restrict__ loo, int n_alphas,
            double* __restrict__ cv, double* __restrict__ part) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const uint32_t sbase = smem_u32(smem_raw);
-  const uint32_t bar_full = sbase + kLooOffBar, bar_empty = bar_full + 8 * kLooStages;
-  const int dp = loo_dp(d), qp = loo_qpitch(dp), vp = loo_vpitch(dp);
-  double* Qs = reinterpret_cast<double*>(smem_raw + (RING ? kLooRingBytes : 0));   // Q[i][k], zero padded to dp x dp
+  TileRing<T, RING, true> tiles{X, n, d, ldx, y, mask, keep, smem_u32(smem_raw)};
+  const int dp = tile_dp(d), qp = tile_bpitch(dp), vp = tile_vpitch(dp);
+  double* Qs = reinterpret_cast<double*>(smem_raw + tile_ring_bytes(RING, true));   // Q[i][k], zero padded to dp x dp
   double* Vs = Qs + dp * qp;               // the tile: v = x - m, then Z = V Q
-  double* yc = Vs + kLooRows * vp;         // y - ybar (0 for rows not kept)
-  double* usef = yc + kLooRows;            // 1: kept
-  double* mean = usef + kLooRows;          // [kMaxD]
+  double* yc = Vs + kTileRows * vp;        // y - ybar (0 for rows not kept)
+  double* usef = yc + kTileRows;           // 1: kept
+  double* mean = usef + kTileRows;         // [kMaxD]
   double* sums = mean + kMaxD;             // [group][kMaxAlphas]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t4 = lane & 3;
   for (int t = tid; t < dp * dp; t += blockDim.x) {
@@ -87,113 +66,56 @@ loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     Qs[i * qp + k] = (i < d && k < d) ? loo[kLooQ + i * kMaxD + k] : 0.0;
   }
   for (int t = tid; t < kMaxD; t += blockDim.x) mean[t] = t < d ? loo[kLooMean + t] : 0.0;
-  for (int t = tid; t < kLooWarps * kMaxAlphas; t += blockDim.x) sums[t] = 0.0;
+  for (int t = tid; t < kTileWarps * kMaxAlphas; t += blockDim.x) sums[t] = 0.0;
   const double ybar = loo[kLooMisc], h0 = loo[kLooMisc + 2];
   const int na = (n_alphas + 7) >> 3;
-  const int G = kLooWarps / na, mpg = (kLooMT + G - 1) / G;
+  const int G = kTileWarps / na, mpg = (kTileMT + G - 1) / G;
   const bool has_item = warp < na * G;     // warp-uniform
   const int nt_a = has_item ? warp / G : 0, grp = has_item ? warp % G : 0, mt0 = grp * mpg;
   const int a0 = 8 * nt_a + 2 * t4;        // the two alphas of this lane's accumulators
   const int ab = 8 * nt_a + g;             // the alpha of this lane's B fragment
-  const int64_t n_tiles = (n + kLooRows - 1) / kLooRows;
-  if constexpr (RING) ring_init<kLooStages>(bar_full, bar_empty, kLooWarps);   // includes a block barrier
-  else __syncthreads();
-  if (RING && warp == kLooWarps) {
-    if (lane == 0)
-      ring_produce<kLooStages>(bar_full, bar_empty, (int)n_tiles, kLooRows, X, (uint32_t)(d * sizeof(T)), sbase,
-                               kLooXStage, true, y, sbase + kLooOffY, kLooYStage, false, nullptr, 0u, 0u);
-  } else {
+  const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
+  tiles.start();
+  if (!tiles.produce()) {
     double acc_e[2] = {0.0, 0.0};
-    int s = 0;
-    uint32_t phase = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int64_t row0 = tile * kLooRows;
-      // (1) the tile
-      if constexpr (RING) {
-        bool use[kLooRows / kLooWarps];
-#pragma unroll
-        for (int u = 0; u < kLooRows / kLooWarps; ++u)   // the mask comes from global memory, before the wait
-          use[u] = mask == nullptr || __ldg(mask + row0 + warp + kLooWarps * u) == (uint8_t)keep;
-        mbar_wait(bar_full + 8 * s, phase);
-        const uint32_t xs = sbase + s * kLooXStage, ys = sbase + kLooOffY + s * kLooYStage;
-#pragma unroll
-        for (int u = 0; u < kLooRows / kLooWarps; ++u) {
-          const int r = warp + kLooWarps * u;
-          const uint32_t xr = xs + (uint32_t)(r * d) * (uint32_t)sizeof(T);
-          for (int j = lane; j < dp; j += 32) {
-            const bool live = use[u] && j < d;
-            const float x = live ? raw_ld_shared<T>(xr + (uint32_t)j * (uint32_t)sizeof(T)) : 0.f;
-            Vs[r * vp + j] = live ? (double)x - mean[j] : 0.0;
-          }
-          if (lane == 0) {
-            yc[r] = use[u] ? (double)ld_shared_f32(ys + 4u * (uint32_t)r) - ybar : 0.0;
-            usef[r] = use[u] ? 1.0 : 0.0;
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_empty + 8 * s);      // the slot is converted: the producer may refill it
-        if (++s == kLooStages) { s = 0; phase ^= 1u; }
-      } else {
-        for (int r = warp; r < kLooRows; r += kLooWarps) {
-          const int64_t row = row0 + r;
-          bool use = row < n;
-          if (use && mask != nullptr) use = __ldg(mask + row) == (uint8_t)keep;
-          const T* xr = X + row * ldx;
-          for (int j = lane; j < dp; j += 32) {
-            const bool live = use && j < d;
-            const float x = live ? ld_row_val<T>(xr + j) : 0.f;
-            Vs[r * vp + j] = live ? (double)x - mean[j] : 0.0;
-          }
-          if (lane == 0) {
-            yc[r] = use ? (double)__ldg(y + row) - ybar : 0.0;
-            usef[r] = use ? 1.0 : 0.0;
-          }
-        }
-      }
-      consumer_sync();
+      const int64_t row0 = tile * kTileRows;
+      // (1) the tile: v = x - m, y - ybar and 1 for kept rows, 0 for the others
+      tiles.load(row0, dp,
+                 [&](int r, int j, bool, bool live, float x) { Vs[r * vp + j] = live ? (double)x - mean[j] : 0.0; },
+                 [&](int r, bool kept, double yr) {
+                   yc[r] = kept ? yr - ybar : 0.0;
+                   usef[r] = kept ? 1.0 : 0.0;
+                 });
+      tile_consumer_sync();
       // (2) Z = V Q: warp w takes the n-tiles w and w + 8 of the dp / 8, all m-tiles
-      double z[2][kLooMT][2];
+      double z[2][kTileMT][2];
+      tile_product(Vs, vp, Qs, qp, dp, dp / 8, z);
+      tile_consumer_sync();
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
-#pragma unroll
-        for (int mt = 0; mt < kLooMT; ++mt) { z[u][mt][0] = 0.0; z[u][mt][1] = 0.0; }
-        const int nt = warp + kLooWarps * u;
-        if (nt < dp / 8) {
-          for (int ks = 0; ks < dp / 4; ++ks) {
-            const double b = Qs[(4 * ks + t4) * qp + 8 * nt + g];
-            double a[kLooMT];
-#pragma unroll
-            for (int mt = 0; mt < kLooMT; ++mt) a[mt] = Vs[(8 * mt + g) * vp + 4 * ks + t4];
-#pragma unroll
-            for (int mt = 0; mt < kLooMT; ++mt) dmma(z[u][mt][0], z[u][mt][1], a[mt], b);
-          }
-        }
-      }
-      consumer_sync();
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int nt = warp + kLooWarps * u;
+        const int nt = warp + kTileWarps * u;
         if (nt < dp / 8) {
 #pragma unroll
-          for (int mt = 0; mt < kLooMT; ++mt) {
+          for (int mt = 0; mt < kTileMT; ++mt) {
             Vs[(8 * mt + g) * vp + 8 * nt + 2 * t4] = z[u][mt][0];
             Vs[(8 * mt + g) * vp + 8 * nt + 2 * t4 + 1] = z[u][mt][1];
           }
         }
       }
-      consumer_sync();
+      tile_consumer_sync();
       // (3) yhat and h of every kept row and alpha, then e^2
       if (has_item) {
-        double yh[kLooMT][2], hh[kLooMT][2];
+        double yh[kTileMT][2], hh[kTileMT][2];
 #pragma unroll
-        for (int mm = 0; mm < kLooMT; ++mm) { yh[mm][0] = yh[mm][1] = hh[mm][0] = hh[mm][1] = 0.0; }
+        for (int mm = 0; mm < kTileMT; ++mm) { yh[mm][0] = yh[mm][1] = hh[mm][0] = hh[mm][1] = 0.0; }
         for (int ks = 0; ks < dp / 4; ++ks) {
           const int j = 4 * ks + t4;
           const double bc = __ldg(loo + kLooCw + j * kMaxAlphas + ab);
           const double bw = __ldg(loo + kLooW + j * kMaxAlphas + ab);
 #pragma unroll
-          for (int mm = 0; mm < kLooMT; ++mm) {
-            if (mm < mpg && mt0 + mm < kLooMT) {              // warp-uniform
+          for (int mm = 0; mm < kTileMT; ++mm) {
+            if (mm < mpg && mt0 + mm < kTileMT) {              // warp-uniform
               const double zz = Vs[(8 * (mt0 + mm) + g) * vp + j];
               dmma(yh[mm][0], yh[mm][1], zz, bc);
               dmma(hh[mm][0], hh[mm][1], zz * zz, bw);
@@ -201,24 +123,24 @@ loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
           }
         }
 #pragma unroll
-        for (int mm = 0; mm < kLooMT; ++mm) {
-          if (mm < mpg && mt0 + mm < kLooMT) {
+        for (int mm = 0; mm < kTileMT; ++mm) {
+          if (mm < mpg && mt0 + mm < kTileMT) {
             const int r = 8 * (mt0 + mm) + g;
             const int64_t row = row0 + r;
-            const bool use = usef[r] != 0.0;
+            const bool kept = usef[r] != 0.0;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const double err = use ? (yc[r] - yh[mm][e]) / (1.0 - (h0 + hh[mm][e])) : 0.0;
+              const double err = kept ? (yc[r] - yh[mm][e]) / (1.0 - (h0 + hh[mm][e])) : 0.0;
               const double e2 = err * err;
               acc_e[e] += e2;
               const int a = a0 + e;
               if (cv != nullptr && row < n && a < n_alphas)
-                cv[row * n_alphas + a] = use ? e2 : __longlong_as_double(0x7ff8000000000000ll);
+                cv[row * n_alphas + a] = kept ? e2 : __longlong_as_double(0x7ff8000000000000ll);
             }
           }
         }
       }
-      consumer_sync();
+      tile_consumer_sync();
     }
     // the CTA's sums: the 8 row lanes of an alpha pair combined, then the groups of an alpha in group order
 #pragma unroll
@@ -232,7 +154,7 @@ loo_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   __syncthreads();
   for (int a = tid; a < kMaxAlphas; a += blockDim.x) {
     double v = 0.0;
-    for (int q = 0; q < kLooWarps; ++q) v += sums[q * kMaxAlphas + a];
+    for (int q = 0; q < kTileWarps; ++q) v += sums[q * kMaxAlphas + a];
     part[(size_t)blockIdx.x * kMaxAlphas + a] = v;
   }
 }
@@ -248,17 +170,15 @@ int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
     B2_CUDA(cudaGetLastError());
     ctx->launches += 1;
   }
-  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kLooRows, first_block, [&](bool ring, const RowSpan& s) {
-    const int64_t n_tiles = (s.rows + kLooRows - 1) / kLooRows;
-    int grid = (int)(n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count);
-    if (grid < 1) grid = 1;
+  return split_ring_rows(ctx, X, x_dtype, n, d, ldx, y, mask, kTileRows, first_block, [&](bool ring, const RowSpan& s) {
+    const int grid = tile_grid(s.rows, ctx->sm_count, 1);
     double* cvt = cv != nullptr ? cv + s.r0 * n_alphas : nullptr;
-    const uint32_t smem = (uint32_t)loo_smem_bytes(loo_dp(d), ring);
+    const uint32_t smem = (uint32_t)loo_smem_bytes(tile_dp(d), ring);
     const int rc = with_rows(x_dtype, s.X, [&](auto* Xr) {
       using T = row_t<decltype(Xr)>;
       auto kernel = ring ? loo_kernel<T, true> : loo_kernel<T, false>;
-      return launch_smem(kernel, grid, ring ? kLooThreads : kLooConsumers, smem, ctx->stream, Xr, s.rows, d, ldx, s.y,
-                         s.mask, keep, static_cast<const double*>(ctx->loo), n_alphas, cvt, ctx->loo_part);
+      return launch_smem(kernel, grid, tile_threads(ring), smem, ctx->stream, Xr, s.rows, d, ldx, s.y, s.mask, keep,
+                         static_cast<const double*>(ctx->loo), n_alphas, cvt, ctx->loo_part);
     });
     if (rc != B2_OK) return rc;
     return launch_ordered_reduce(ctx, ctx->loo_part, kMaxAlphas, grid, s.first, kMaxAlphas, 0u, ctx->loo + kLooSum);

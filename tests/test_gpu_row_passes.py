@@ -3,10 +3,11 @@ tests run each host-streamed entry point on masked host rows of three staging bl
 ring) and d = 64 (the wide ring), and on one strided layout.
 
   * pinned and pageable rows give bit-identical outputs in the same number of launches;
-  * every per-row output (yhat, ystd, mu) is bit-identical to the same call on each staging block's rows alone;
+  * every per-row output (yhat, ystd, mu, the logistic decision, proba and label) is bit-identical to the same call on
+    each staging block's rows alone;
   * the outputs agree with the same call on device rows.  The Gram runs on the exact fp64 kernel, so every difference
     is the order of fp64 sums: relative ROW_TOL on fp64 results (LOO_TOL behind b2_ridge_loo's eigendecomposition),
-    FP32_TOL on b2_score's fp32 predictions and test_gpu_glm.PASS_TOL on the GLM sums.
+    FP32_TOL on b2_score's fp32 predictions and test_gpu_glm.PASS_TOL on the GLM and logistic sums.
 """
 import ctypes as C
 
@@ -41,26 +42,28 @@ def _ok(rc):
 
 
 class Rows:
-    """One layout of the same rows: X (row pitch ldx), y and the mask as host (pageable or pinned) or device pointers."""
+    """One layout of the same rows: X (row pitch ldx), y, the mask and the labels y > 1 (0 / 1) as host (pageable or
+    pinned) or device pointers."""
 
     def __init__(self, ctx, Xs, y, mask, kind, d, ld_off=0):
         self.ctx, self.kind, self.n, self.d = ctx, kind, y.size, d
         self.ldx, self.host = Xs.shape[1], kind != "device"
         self._keep = []
+        self._labels = labels = (y > 1.0).astype(np.float32)    # pageable rows point into it
         if kind == "pageable":
-            arrs = [Xs, y, mask]
+            arrs = [Xs, y, mask, labels]
         elif kind == "pinned":
             arrs = []
-            for a in (Xs, y, mask):
+            for a in (Xs, y, mask, labels):
                 p = ctx.pinned(a.shape, a.dtype)
                 p.array[:] = a
                 self._keep.append(p)
                 arrs.append(p.array)
         else:
-            self._keep = [ctx.to_device(Xs), ctx.to_device(y), ctx.to_device(mask)]
+            self._keep = [ctx.to_device(Xs), ctx.to_device(y), ctx.to_device(mask), ctx.to_device(labels)]
             arrs = self._keep
         ptr = [a.ctypes.data if isinstance(a, np.ndarray) else a.ptr for a in arrs]
-        self.X, self.y, self.mask = ptr[0] + 4 * ld_off, ptr[1], ptr[2]
+        self.X, self.y, self.mask, self.labels = ptr[0] + 4 * ld_off, ptr[1], ptr[2], ptr[3]
         self.mk = native.MEM_HOST if self.host else native.MEM_DEVICE
 
     def out(self, shape, dtype):
@@ -138,8 +141,29 @@ def _calls(ctx, r, coef, b0):
         _ok(lib.b2_glm_predict(*base, n, d, r.ldx, r.mk, native.GLM_LOG, coef.ctypes.data, b0, mp))
         return {"mu": mu().copy()}
 
+    def logistic_pass(hessian):
+        sums, H = np.empty(d + 9), np.empty((d + 1, d + 1)) if hessian else None
+        _ok(lib.b2_logistic_pass(*base, r.labels, n, d, r.ldx, r.mk, r.mask, 1, 0.0, 1.0, coef.ctypes.data, b0, 1,
+                                 sums.ctypes.data, H.ctypes.data if hessian else None))
+        return {"sums": sums, "hessian": H} if hessian else {"sums": sums}
+
+    def logistic_line_search():
+        step, out = coef[::-1].copy(), np.empty(native.GLM_STEPS)
+        _ok(lib.b2_logistic_line_search(*base, r.labels, n, d, r.ldx, r.mk, r.mask, 1, 0.0, 1.0, coef.ctypes.data, b0,
+                                        step.ctypes.data, -0.1, native.GLM_STEPS, out.ctypes.data))
+        return {"ladder": out}
+
+    def logistic_predict():
+        _, dp_, dec = r.out(n, np.float64)
+        _, pp, proba = r.out((n, 2), np.float64)
+        _, lp, lab = r.out(n, np.float32)
+        _ok(lib.b2_logistic_predict(*base, n, d, r.ldx, r.mk, coef.ctypes.data, b0, 0.0, 1.0, dp_, pp, lp))
+        return {"decision": dec().copy(), "proba": proba().copy(), "label": lab().copy()}
+
     for name, fn in (("score", score), ("fit", fit), ("moments", moments), ("loo", loo), ("score_std", score_std),
-                     ("glm_pass", glm_pass), ("line_search", line_search), ("glm_predict", glm_predict)):
+                     ("glm_pass", glm_pass), ("line_search", line_search), ("glm_predict", glm_predict),
+                     ("logistic_pass", lambda: logistic_pass(True)), ("logistic_grad", lambda: logistic_pass(False)),
+                     ("logistic_line_search", logistic_line_search), ("logistic_predict", logistic_predict)):
         run(name, fn)
     return res
 
@@ -179,7 +203,7 @@ def _compare_layouts(ctx, Xs, y, mask, coef, d, ld_off=0):
     dev = {name: res for name, (res, _) in out["device"].items()}
     host = {name: res for name, (res, _) in out["pageable"].items()}
     worst = {}
-    for name in ("fit", "moments", "loo", "score_std", "glm_predict"):
+    for name in ("fit", "moments", "loo", "score_std", "glm_predict", "logistic_predict"):
         for k, v in host[name].items():
             if k == "best":
                 assert np.array_equal(v, dev[name][k])
@@ -193,9 +217,11 @@ def _compare_layouts(ctx, Xs, y, mask, coef, d, ld_off=0):
     assert rel(host["score"]["yhat"], dev["score"]["yhat"]) < FP32_TOL
     sums = host["score"]["stats"]
     assert rel(sums, dev["score"]["stats"]) < FP32_TOL and sums[5] == dev["score"]["stats"][5] == mask.sum()
-    for k in ("sums", "hessian"):
-        assert rel(host["glm_pass"][k], dev["glm_pass"][k]) < PASS_TOL, k
-    assert rel(host["line_search"]["ladder"], dev["line_search"]["ladder"]) < PASS_TOL
+    for name in ("glm_pass", "logistic_pass", "logistic_grad"):
+        for k in host[name]:
+            assert rel(host[name][k], dev[name][k]) < PASS_TOL, (name, k)
+    for name in ("line_search", "logistic_line_search"):
+        assert rel(host[name]["ladder"], dev[name]["ladder"]) < PASS_TOL, name
     return host
 
 
@@ -204,7 +230,7 @@ def test_host_rows_stream_like_device_rows(ctx, d):
     Xs, y, mask, coef = _table(d, 70 + d)
     host = _compare_layouts(ctx, Xs, y, mask, coef, d)
     # per-row outputs: the same call on each staging block's rows alone
-    parts = {"score": [], "score_std": [], "glm_predict": []}
+    parts = {"score": [], "score_std": [], "glm_predict": [], "logistic_predict": []}
     for r0 in range(0, N, BLOCK):
         sl = slice(r0, min(r0 + BLOCK, N))
         r = Rows(ctx, np.ascontiguousarray(Xs[sl]), np.ascontiguousarray(y[sl]), np.ascontiguousarray(mask[sl]),
@@ -217,6 +243,8 @@ def test_host_rows_stream_like_device_rows(ctx, d):
     for k in ("ystd", "yhat"):
         assert np.array_equal(np.concatenate([p[k] for p in parts["score_std"]]), host["score_std"][k])
     assert np.array_equal(np.concatenate([p["mu"] for p in parts["glm_predict"]]), host["glm_predict"]["mu"])
+    for k in ("decision", "proba", "label"):
+        assert np.array_equal(np.concatenate([p[k] for p in parts["logistic_predict"]]), host["logistic_predict"][k])
 
 
 def test_strided_host_rows(ctx):
