@@ -19,18 +19,22 @@ Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- th
                            loss, gradient and fp64 tensor-core Hessian and one pass for every line-search step
     B200LogisticRegression sklearn's binary LogisticRegression (solver="newton-cholesky"): the same Newton passes on the
                            half-binomial loss, labels as stored, probabilities and labels in one predict pass
+    B200RidgeClassifier    sklearn's RidgeClassifier, 2 to 32 classes: the fp64 Gram, one class-sum pass and one solve
+                           with every class as a right-hand side; decisions and labels in one fp64 tensor-core pass
     stage_1_train_model    drop-in for mlops_simulation/stage_1_train_model.py
 """
 from . import _native as native
 from ._native import (BF16, F32, KERNEL_AUTO, KERNEL_NARROW, KERNEL_SIMT, KERNEL_TCGEN05, PRECISION_BF16, PRECISION_SPLIT, Context,
                       DeviceArray, PinnedArray)
 from .estimator import (B200ARDRegression, B200BayesianRidge, B200ElasticNet, B200ElasticNetCV, B200GammaRegressor,
-                        B200Lasso, B200LassoCV, B200LinearRegression, B200LogisticRegression, B200PoissonRegressor, B200RidgeCV,
-                        B200TweedieRegressor, default_context, enet_path, fold_ids, lasso_path)
+                        B200Lasso, B200LassoCV, B200LinearRegression, B200LogisticRegression, B200PoissonRegressor,
+                        B200RidgeClassifier, B200RidgeCV, B200TweedieRegressor, default_context, enet_path, fold_ids,
+                        lasso_path)
 from . import sharding, tranche_io  # noqa: F401
 
 __all__ = ["native", "Context", "DeviceArray", "PinnedArray", "B200LinearRegression", "B200RidgeCV", "B200ElasticNet",
            "B200Lasso", "B200ElasticNetCV", "B200LassoCV", "B200BayesianRidge", "B200ARDRegression",
-           "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression", "fold_ids", "enet_path", "lasso_path", "default_context",
+           "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression",
+           "B200RidgeClassifier", "fold_ids", "enet_path", "lasso_path", "default_context",
            "F32", "BF16", "KERNEL_AUTO", "KERNEL_SIMT", "KERNEL_TCGEN05", "KERNEL_NARROW", "PRECISION_SPLIT", "PRECISION_BF16"]
 __version__ = "0.1.0"

@@ -27,6 +27,7 @@ MAX_D = 128
 MAX_ALPHAS = 64
 GLM_LOG, GLM_IDENTITY = 0, 1
 GLM_STEPS = 21
+MAX_CLASSES = 32
 
 _c_i64 = C.c_int64
 _vp = C.c_void_p
@@ -96,6 +97,13 @@ _SIGNATURES = {
     "b2_logistic_predict": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, C.c_double,
                                       C.c_double, _vp, _vp, _vp]),
     "b2_label_scan": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, _vp]),
+    "b2_class_sums": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
+                                _vp, _vp, _vp]),
+    "b2_solve_classes": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.c_int, _vp, _vp]),
+    "b2_classify": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int,
+                              _vp, _vp, _vp, _vp]),
+    "b2_label_values": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, C.c_int, _vp, C.POINTER(C.c_int),
+                                  C.POINTER(C.c_int)]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -796,6 +804,96 @@ class Context:
         rc = load().b2_label_scan(self._h, y.ptr, n, mp, int(mask_keep), st.ctypes.data)
         _check_args(rc, "b2_label_scan")
         return dict(zip(("kept", "nonfinite", "nonintegral", "min", "max", "n_min", "n_max"), st.tolist()))
+
+    # -- RidgeClassifier (DESIGN.md section 12) -----------------------------------------------------------------------
+    @staticmethod
+    def _f32_classes(classes, k: int) -> np.ndarray:
+        c = np.ascontiguousarray(classes, dtype=np.float32).ravel()
+        if c.size != k:
+            raise ValueError(f"{k} classes expected, got {c.size}")
+        return c
+
+    def class_sums(self, X, y, classes, center=None, *, row_mask=None, mask_keep: int = 1) -> dict:
+        """One pass over the kept rows for the class sums of a ridge classifier (b2_class_sums): ``classes`` are K sorted
+        fp32 values and a row's class is the index of its y among them.  Returns sums ((K, d + 1): per class the sum of
+        x - center over its rows, then their count), kept, unmatched (kept rows of no class, NaN included) and nonfinite
+        (kept rows with y not finite).  ``center``: d values, None for zeros.  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        c = None if center is None else self._f64_coef(center, d)
+        sums = np.empty((cl.size, d + 1), dtype=np.float64)
+        counts = np.empty(3, dtype=np.float64)
+        rc = load().b2_class_sums(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data, cl.size,
+                                  c.ctypes.data if c is not None else None, sums.ctypes.data, counts.ctypes.data)
+        _check_args(rc, "b2_class_sums")
+        return {"sums": sums, "kept": float(counts[0]), "unmatched": float(counts[1]), "nonfinite": float(counts[2])}
+
+    def solve_classes(self, class_sums, alpha: float = 1.0, fit_intercept: bool = True,
+                      n_classes: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """(coef (T, d), intercept (T,)) of the ridge classifier of the resident statistic and the class sums
+        (b2_solve_classes): ``class_sums`` the (K, d + 1) ``sums`` of ``class_sums``, or None for the context's last ones
+        (then ``n_classes`` = K).  T = 1 for two classes, else K.  Raises ``np.linalg.LinAlgError`` when the LDL^T meets
+        a non-positive pivot."""
+        if class_sums is not None:
+            cs = np.ascontiguousarray(class_sums, dtype=np.float64)
+            if cs.ndim != 2 or cs.shape[1] != self.d + 1:
+                raise ValueError(f"class_sums must be (K, {self.d + 1}), got {cs.shape}")
+            k, cs_ptr = cs.shape[0], cs.ctypes.data
+        else:
+            k, cs_ptr = int(n_classes or 0), None
+        t = 1 if k == 2 else max(k, 1)
+        coef = np.empty((t, max(self.d, 1)), dtype=np.float64)
+        b0 = np.empty(t, dtype=np.float64)
+        rc = load().b2_solve_classes(self._h, float(alpha), int(bool(fit_intercept)), cs_ptr, k, coef.ctypes.data,
+                                     b0.ctypes.data)
+        if rc == E_SINGULAR:
+            raise np.linalg.LinAlgError(last_error())
+        _check_args(rc, "b2_solve_classes")
+        return coef, b0
+
+    def classify(self, X, coef, intercept, classes, y=None, *, row_mask=None, mask_keep: int = 1,
+                 decision: bool = False, label: bool = False) -> dict:
+        """The ridge classifier per row in one pass (b2_classify): eta = X coef^T + intercept for the T rows of coef.
+        The wanted ones of decision ((n, T) fp64) and label (classes[argmax eta], the first largest; for T = 1
+        classes[1] where eta > 0, else classes[0]; fp32) -- ndarrays for host rows, DeviceArrays for device rows -- and,
+        with y, kept and correct (kept rows whose y equals their label)."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w = np.ascontiguousarray(coef, dtype=np.float64)
+        w = w.reshape(1, -1) if w.ndim == 1 else w
+        if w.ndim != 2 or w.shape[1] != d:
+            raise ValueError(f"coef must be (T, {d}), got {np.shape(coef)}")
+        t = w.shape[0]
+        b0 = np.ascontiguousarray(intercept, dtype=np.float64).ravel()
+        if b0.size != t:
+            raise ValueError(f"intercept has {b0.size} entries, coef {t} rows")
+        cl = self._f32_classes(classes, max(t, 2))
+        out, ptrs = {}, {}
+        for name, want, shape, kind in (("decision", decision, (n, t), "f64"), ("label", label, (n,), "f32")):
+            a, ptrs[name] = self._out(mk, shape, kind, want)
+            if want:
+                out[name] = a
+        counts = np.zeros(2, dtype=np.float64) if y is not None else None
+        rc = load().b2_classify(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), w.ctypes.data, b0.ctypes.data,
+                                t, cl.ctypes.data, ptrs["decision"], ptrs["label"],
+                                counts.ctypes.data if counts is not None else None)
+        _check_args(rc, "b2_classify")
+        if counts is not None:
+            out["kept"], out["correct"] = float(counts[0]), float(counts[1])
+        return out
+
+    def label_values(self, y, row_mask=None, mask_keep: int = 1, max_values: int = MAX_CLASSES):
+        """(values, more): the distinct finite values of an f32 DeviceArray y over the kept rows, ascending (-0.0 as
+        0.0), at most ``max_values`` of them, and whether there are more (b2_label_values)."""
+        if not isinstance(y, DeviceArray) or y.kind != "f32":
+            raise RuntimeError("label_values: y must be an f32 DeviceArray")
+        n = int(np.prod(y.shape))
+        mp = _vec_ptr(row_mask, "u8", MEM_DEVICE, n, "row_mask")
+        vals = np.empty(max(int(max_values), 1), dtype=np.float32)
+        found, more = C.c_int(0), C.c_int(0)
+        rc = load().b2_label_values(self._h, y.ptr, n, mp, int(mask_keep), int(max_values), vals.ctypes.data,
+                                    C.byref(found), C.byref(more))
+        _check_args(rc, "b2_label_values")
+        return vals[: found.value].copy(), bool(more.value)
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

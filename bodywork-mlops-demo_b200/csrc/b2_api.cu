@@ -477,7 +477,8 @@ int b2_ctx_destroy(b2_ctx* ctx) {
   void* bufs[] = {ctx->S, ctx->tc_part, ctx->tc_red, ctx->shift, ctx->simt_part, ctx->score_part,
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
-                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part};
+                  ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part,
+                  ctx->cls};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1668,6 +1669,175 @@ int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* ro
   stats_out[4] = any ? value(h[kLabelMax]) : NAN;
   stats_out[5] = (double)h[kLabelNMin];
   stats_out[6] = (double)h[kLabelNMax];
+  return B2_OK;
+}
+
+// ---- RidgeClassifier (DESIGN.md section 12) ------------------------------------------------------------------------
+// The operands and sums (ctx->cls) beside the GLM block, whose per-CTA partials the passes share; allocated by the first
+// call and freed with the context.
+static int ensure_cls(b2_ctx* ctx, const char* what) {
+  if (ctx->n_ranks > 1) {
+    set_error("%s runs on one rank only (its sums are not exchanged between ranks)", what);
+    return B2_E_UNSUPPORTED;
+  }
+  if (int r = ensure_glm(ctx)) return r;
+  if (ctx->cls == nullptr) B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->cls), sizeof(double) * kClsDoubles));
+  return B2_OK;
+}
+
+// n_classes sorted, distinct, finite fp32 values, 2 <= n_classes <= B2_MAX_CLASSES
+static int check_classes(const float* classes, int n_classes) {
+  if (classes == nullptr || n_classes < 2 || n_classes > kMaxClasses) {
+    set_error("classes: 2..%d sorted fp32 values expected (got %d%s)", kMaxClasses, n_classes,
+              classes == nullptr ? ", null" : "");
+    return B2_E_ARG;
+  }
+  for (int k = 0; k < n_classes; ++k)
+    if (!isfinite(classes[k]) || (k > 0 && !(classes[k] > classes[k - 1]))) {
+      set_error("classes must be finite and strictly ascending (class %d is %g)", k, (double)classes[k]);
+      return B2_E_ARG;
+    }
+  return B2_OK;
+}
+
+// doubles [at, at + n) of ctx->cls from the host
+static int upload_cls(b2_ctx* ctx, int at, const std::vector<double>& v) {
+  B2_CUDA(cudaMemcpyAsync(ctx->cls + at, v.data(), sizeof(double) * v.size(), cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // v belongs to the caller's frame
+  return B2_OK;
+}
+
+int b2_class_sums(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                  int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                  const double* center, double* sums_out, double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (sums_out == nullptr || counts_out == nullptr) { set_error("sums_out / counts_out is null"); return B2_E_ARG; }
+  if (int r = check_classes(classes, n_classes)) return r;
+  if (int r = ensure_cls(ctx, "b2_class_sums")) return r;
+  std::vector<double> op(kMaxD + kMaxClasses, 0.0);     // kClsCenter, then kClsClasses
+  if (center != nullptr) memcpy(op.data() + kClsCenter, center, sizeof(double) * d);
+  for (int k = 0; k < n_classes; ++k) op[kClsClasses + k] = classes[k];
+  if (int r = upload_cls(ctx, kClsCenter, op)) return r;
+  if (int r = row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+        return launch_class_sums(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_classes, s.first);
+      }))
+    return r;
+  const int n_sums = n_classes * (d + 1);
+  std::vector<double> h((size_t)n_sums + 3);
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->cls + kClsSums, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, h.data(), sizeof(double) * n_sums);
+  memcpy(counts_out, h.data() + n_sums, sizeof(double) * 3);
+  return B2_OK;
+}
+
+int b2_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, const double* class_sums, int n_classes,
+                     double* coef_out, double* intercept_out) {
+  if (int r = use_device(ctx)) return r;
+  if (ctx->d == 0) { set_error("b2_gram_reset has not been called"); return B2_E_STATE; }
+  if (!(alpha >= 0.0) || !isfinite(alpha)) { set_error("alpha must be finite and >= 0"); return B2_E_ARG; }
+  if (n_classes < 2 || n_classes > kMaxClasses) {
+    set_error("n_classes=%d out of range [2,%d]", n_classes, kMaxClasses);
+    return B2_E_ARG;
+  }
+  if (coef_out == nullptr || intercept_out == nullptr) { set_error("coef_out / intercept_out is null"); return B2_E_ARG; }
+  if (int r = ensure_cls(ctx, "b2_solve_classes")) return r;
+  const int d = ctx->d, T = n_classes == 2 ? 1 : n_classes;
+  if (class_sums != nullptr) {
+    std::vector<double> v(class_sums, class_sums + (size_t)n_classes * (d + 1));
+    if (int r = upload_cls(ctx, kClsSums, v)) return r;
+  }
+  if (int r = ensure_s_cleared(ctx)) return r;
+  if (int r = launch_solve_classes(ctx, alpha, fit_intercept, n_classes)) return r;
+  std::vector<double> h(kClsInfo + 1 - kClsCoef);       // W, b, info
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->cls + kClsCoef, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  const double info = h[kClsInfo - kClsCoef];
+  if (info != 0.0) {
+    set_error("pivot %d of the LDL^T factorisation is not positive: the centred Gram matrix is rank deficient "
+              "(use alpha > 0 or b2_solve_eigh)", (int)info);
+    return B2_E_SINGULAR;
+  }
+  for (int t = 0; t < T; ++t) {
+    memcpy(coef_out + (size_t)t * d, h.data() + (size_t)t * kMaxD, sizeof(double) * d);
+    intercept_out[t] = h[kClsIntercept - kClsCoef + t];
+  }
+  return B2_OK;
+}
+
+int b2_classify(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, const double* coef, const double* intercept,
+                int n_targets, const float* classes, double* decision_out, float* label_out, double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_targets < 1 || n_targets > kMaxClasses) {
+    set_error("n_targets=%d out of range [1,%d]", n_targets, kMaxClasses);
+    return B2_E_ARG;
+  }
+  if (coef == nullptr || intercept == nullptr) { set_error("coef / intercept is null"); return B2_E_ARG; }
+  if (decision_out == nullptr && label_out == nullptr && counts_out == nullptr) {
+    set_error("decision_out, label_out and counts_out are all null");
+    return B2_E_ARG;
+  }
+  if (n_rows > 0 && (X == nullptr || (counts_out != nullptr && y == nullptr))) {
+    set_error("X / y is null (counts_out needs y)");
+    return B2_E_ARG;
+  }
+  const int n_classes = n_targets == 1 ? 2 : n_targets;
+  if (int r = check_classes(classes, n_classes)) return r;
+  if (int r = ensure_cls(ctx, "b2_classify")) return r;
+  std::vector<double> op(kClsInfo - kClsClasses, 0.0);  // classes, W, b
+  for (int k = 0; k < n_classes; ++k) op[k] = classes[k];
+  for (int t = 0; t < n_targets; ++t) {
+    memcpy(op.data() + kClsCoef - kClsClasses + (size_t)t * kMaxD, coef + (size_t)t * d, sizeof(double) * d);
+    op[kClsIntercept - kClsClasses + t] = intercept[t];
+  }
+  if (int r = upload_cls(ctx, kClsClasses, op)) return r;
+  // y and the mask only count: every row gets its decision and label
+  const float* yc = counts_out != nullptr ? y : nullptr;
+  const uint8_t* mc = counts_out != nullptr ? row_mask : nullptr;
+  if (int r = row_pass(
+          ctx, X, x_dtype, yc, n_rows, d, ldx, mem_kind, mc,
+          [&](const RowSpan& s, void* dec, void* lab, void*) {
+            return launch_classify(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_targets,
+                                   static_cast<double*>(dec), static_cast<float*>(lab), s.first);
+          },
+          RowOut{decision_out, sizeof(double) * n_targets}, RowOut{label_out, sizeof(float)}))
+    return r;
+  if (counts_out != nullptr)
+    B2_CUDA(cudaMemcpyAsync(counts_out, ctx->cls + kClsCounts, sizeof(double) * 2, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep,
+                    int max_values, float* values_out, int* n_values_out, int* more_out) {
+  if (int r = use_device(ctx)) return r;
+  if (n_rows < 0 || (n_rows > 0 && y == nullptr)) { set_error("n_rows=%lld / y is null", (long long)n_rows); return B2_E_ARG; }
+  if (max_values < 1 || max_values > kMaxClasses) {
+    set_error("max_values=%d out of range [1,%d]", max_values, kMaxClasses);
+    return B2_E_ARG;
+  }
+  if (values_out == nullptr || n_values_out == nullptr || more_out == nullptr) {
+    set_error("values_out / n_values_out / more_out is null");
+    return B2_E_ARG;
+  }
+  if (int r = ensure_cls(ctx, "b2_label_values")) return r;
+  unsigned long long* st = reinterpret_cast<unsigned long long*>(ctx->glm_part);
+  if (int r = launch_label_values(ctx, y, n_rows, row_mask, mask_keep, max_values, st)) return r;
+  unsigned long long h[kMaxClasses + 1];
+  B2_CUDA(cudaMemcpyAsync(h, st, sizeof(unsigned long long) * (max_values + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  int found = 0;
+  for (; found < max_values && h[found] != ~0ull; ++found) {
+    uint32_t u = (uint32_t)h[found];                   // the inverse of the kernel's order-preserving key
+    u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+    memcpy(values_out + found, &u, sizeof(float));
+  }
+  *n_values_out = found;
+  *more_out = h[max_values] != ~0ull ? 1 : 0;
   return B2_OK;
 }
 

@@ -140,6 +140,29 @@ constexpr int kGlmCorrect = 7;
 // b2_label_scan's counters (unsigned long long, in ctx->glm_part): the extremes as order-preserving keys of the fp32 value
 enum LabelWord { kLabelKept = 0, kLabelNonFinite, kLabelNonIntegral, kLabelMin, kLabelMax, kLabelNMin, kLabelNMax,
                  kLabelWords };
+// the order-preserving key of an fp32 label (monotone in v for finite v) and its inverse
+__device__ __forceinline__ unsigned long long label_key(float v) {
+  const uint32_t u = __float_as_uint(v);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float label_of_key(unsigned long long k) {
+  const uint32_t u = (uint32_t)k;
+  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+
+// ---- the ridge classifier (classify.cu, solve.cu: solve_classes_kernel; DESIGN.md section 12) -------------------------
+// doubles of ctx->cls: the centre c of the class sums, the sorted classes, the model W [kMaxClasses][kMaxD] and b, the
+// solve's info (1-based failing pivot), the classify counts [kept, correct], the reduced class sums [K][d + 1] + 3 counts
+constexpr int kMaxClasses = B2_MAX_CLASSES;
+constexpr int kClsPart = kMaxClasses * (kMaxD + 1) + 8;   // one CTA's class sums (also the classify pass's two counts)
+constexpr int kClsCenter = 0;
+constexpr int kClsClasses = kMaxD;
+constexpr int kClsCoef = kClsClasses + kMaxClasses;
+constexpr int kClsIntercept = kClsCoef + kMaxClasses * kMaxD;
+constexpr int kClsInfo = kClsIntercept + kMaxClasses;
+constexpr int kClsCounts = kClsInfo + 8;
+constexpr int kClsSums = kClsCounts + 8;
+constexpr int kClsDoubles = kClsSums + kClsPart;
 
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
@@ -224,6 +247,8 @@ struct b2_ctx {
   // allocated by the first call
   double* glm = nullptr;
   double* glm_part = nullptr;
+  // the ridge classifier's operands and sums (b2::kCls*), allocated by the first call; its per-CTA partials in glm_part
+  double* cls = nullptr;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -414,6 +439,20 @@ int launch_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, 
                             double* proba, float* label);
 // the kLabelWords counters of the kept rows of device y into st (two launches after two memsets)
 int launch_label_scan(b2_ctx* ctx, const float* y, int64_t n, const uint8_t* mask, int keep, unsigned long long* st);
+// the class sums of the rows [0, n) at the centre and classes of ctx->cls, then the ordered reduce of the per-CTA sums
+// into ctx->cls + kClsSums (`first_block` overwrites, otherwise adds)
+int launch_class_sums(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                      const uint8_t* mask, int keep, int n_classes, bool first_block);
+// the model of ctx->cls on the rows [0, n): decision [n][n_targets] (fp64) and label (fp32), each if not null; with y,
+// the kept and correct rows into ctx->cls + kClsCounts (`first_block` overwrites, otherwise adds)
+int launch_classify(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                    const uint8_t* mask, int keep, int n_targets, double* decision, float* label, bool first_block);
+// st[i], i <= max_values: the keys of the distinct finite kept y in ascending order, ~0 past the last (max_values + 1
+// launches after one memset)
+int launch_label_values(b2_ctx* ctx, const float* y, int64_t n, const uint8_t* mask, int keep, int max_values,
+                        unsigned long long* st);
+// W and b of the ridge classifier from the resident S and the class sums at ctx->cls + kClsSums (one launch)
+int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes);
 int launch_p2p_allreduce(b2_ctx* ctx);
 int launch_synth(b2_ctx* ctx, uint64_t seed, int64_t row_offset, int64_t n, int d, int64_t ldx,
                  int x_dtype, double alpha, double beta, double sigma, void* X, float* y);

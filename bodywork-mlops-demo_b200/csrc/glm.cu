@@ -385,15 +385,8 @@ logistic_predict_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, 
 }
 
 // The label scan of a device fp32 y over its kept rows (kLabel* in b2_internal.cuh): counts by integer atomics and the
-// extremes by atomics on order-preserving keys, so the result does not depend on the order of the rows.
-__device__ __forceinline__ unsigned long long label_key(float v) {   // monotone in v for finite v
-  const uint32_t u = __float_as_uint(v);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float label_of_key(unsigned long long k) {
-  const uint32_t u = (uint32_t)k;
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
+// extremes by atomics on order-preserving keys (label_key, b2_internal.cuh), so the result does not depend on the order of
+// the rows.
 __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

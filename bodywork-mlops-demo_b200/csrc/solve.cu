@@ -1707,6 +1707,96 @@ ard_kernel(const double* __restrict__ S, int d, const BayesArgs a) {
   }
 }
 
+// ---- the ridge classifier's solve (b2_solve_classes; DESIGN.md section 12) ---------------------------------------------
+// (Xc^T Xc + alpha I) W^T = Xc^T Yc for the T = n_classes targets (1 with two classes: the second class is the positive
+// one) of LabelBinarizer(pos_label=1, neg_label=-1).  From the class sums s_k = sum_{y = k} (x - c) and counts n_k of
+// the kept rows (any centre c, every kept row of some class), with s = sum_k s_k and n the rows of S:
+//   Xc^T Yc[:, k] = sum (x - c)(y_k - ybar_k) = 2 (s_k - (n_k / n) s)   (2 s_k - s without an intercept, c = 0)
+//   b_k = ybar_k - mean.w_k,  ybar_k = 2 n_k / n - 1.
+// A is build_normal_equations'; the T right-hand sides ride as extra rows of [A ; Rhs^T] through an unblocked
+// right-looking LDL^T (the pivot rule of solve_cholesky_kernel: a pivot <= 1e-12 of the largest diagonal entry refuses the
+// system), which leaves D^-1 M^-1 r_t in row d + t; then M^T w_t = that row, one warp per target.
+constexpr int kClsThreads = 512;
+size_t solve_classes_smem_bytes(int d, int n_targets) {
+  return sizeof(double) * ((size_t)(d + n_targets) * (d + 1) + 3 * kMaxD + kMaxClasses + 16);
+}
+
+__global__ void __launch_bounds__(kClsThreads, 1)
+solve_classes_kernel(double* S, int d, double alpha, int fit_intercept, int n_classes, double* __restrict__ cls) {
+  extern __shared__ double sm[];
+  const int T = n_classes == 2 ? 1 : n_classes, pitch = d + 1, rows = d + T;
+  double* A = sm;                          // rows 0..d-1 = A, row d + t = the right-hand side of target t
+  double* mean = A + rows * pitch;         // [kMaxD]
+  double* tot = mean + kMaxD;              // [kMaxD] s = sum_k s_k
+  double* col = tot + kMaxD;               // [kMaxD + kMaxClasses] column k of the current step
+  double* misc = col + kMaxD + kMaxClasses;   // [0] ybar of S (unused), [1] the largest diagonal entry
+  const double* sums = cls + kClsSums;     // [K][d + 1]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  build_normal_equations(S, d, alpha, fit_intercept, A, A + d * pitch, mean, &misc[0]);
+  const double n = __ldcg(S + d * (d + 2) + d);
+  if (tid < d) {
+    double s = 0.0;
+    for (int k = 0; k < n_classes; ++k) s += sums[k * (d + 1) + tid];
+    tot[tid] = s;
+  }
+  __syncthreads();
+  for (int t = tid; t < T * d; t += blockDim.x) {
+    const int tt = t / d, j = t - tt * d, k = T == 1 ? 1 : tt;
+    const double sk = sums[k * (d + 1) + j], nk = sums[k * (d + 1) + d];
+    A[(d + tt) * pitch + j] = fit_intercept ? 2.0 * (sk - (nk / n) * tot[j]) : 2.0 * sk - tot[j];
+  }
+  if (warp == 0) {
+    double mx = 0.0;
+    for (int i = lane; i < d; i += 32) mx = fmax(mx, A[i * pitch + i]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) misc[1] = mx;
+  }
+  __syncthreads();
+  const double tiny = misc[1] * 1e-12;
+  int info = 0;
+  for (int k = 0; k < d; ++k) {
+    const double piv = A[k * pitch + k];
+    if (!(piv > tiny)) { info = k + 1; break; }   // block-uniform
+    const double rc = 1.0 / piv;
+    for (int i = k + 1 + tid; i < rows; i += blockDim.x) col[i] = A[i * pitch + k];
+    __syncthreads();
+    // a_ij -= u_ik u_jk / D_k for k < j <= i (every j > k in the right-hand sides); m_ik = u_ik / D_k; warp per row
+    for (int i = k + 1 + warp; i < rows; i += nwarps) {
+      const double f = col[i] * rc;
+      const int jend = i < d ? i : d - 1;
+      for (int j = k + 1 + lane; j <= jend; j += 32) A[i * pitch + j] = fma(-f, col[j], A[i * pitch + j]);
+      if (lane == 0) A[i * pitch + k] = f;
+    }
+    __syncthreads();
+  }
+  // M^T w = z per target, from the bottom: w_i is final once every m > i has been subtracted
+  for (int t = warp; t < T; t += nwarps) {
+    double* z = A + (d + t) * pitch;
+    if (info == 0) {
+      for (int i = d - 1; i > 0; --i) {
+        const double wi = z[i];
+        for (int m = lane; m < i; m += 32) z[m] = fma(-A[i * pitch + m], wi, z[m]);
+        __syncwarp();
+      }
+    }
+    double part = 0.0;
+    for (int j = lane; j < d; j += 32) {
+      const double w = info == 0 ? z[j] : 0.0;
+      cls[kClsCoef + t * kMaxD + j] = w;
+      part = fma(mean[j], w, part);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if (lane == 0) {
+      const int k = T == 1 ? 1 : t;
+      const double ybar = fit_intercept ? 2.0 * sums[k * (d + 1) + d] / n - 1.0 : 0.0;
+      cls[kClsIntercept + t] = info == 0 ? ybar - part : 0.0;
+    }
+  }
+  if (tid == 0) cls[kClsInfo] = (double)info;
+}
+
 size_t solve_smem_bytes(int d) {
   // Cholesky: A, mean, invd, misc, U panel; eigenvalue kernel: A, r, mean, misc, (v, w) x 2, pv, dd, ee2, lam
   const size_t chol = (size_t)(d + 1) * (d + 1) + 3 * d + 16 + (size_t)(d + 1) * kUPitch;
@@ -1748,6 +1838,15 @@ int launch_solve_cholesky(b2_ctx* ctx, double alpha, int fit_intercept, unsigned
                                                                                            fit_intercept, ctx->solve_host,
                                                                                            xc, nullptr);
   B2_CUDA(cudaGetLastError());
+  ctx->launches += 1;
+  return B2_OK;
+}
+
+int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes) {
+  const int T = n_classes == 2 ? 1 : n_classes;
+  if (int r = launch_smem(solve_classes_kernel, 1, kClsThreads, (uint32_t)solve_classes_smem_bytes(ctx->d, T),
+                          ctx->stream, ctx->S, ctx->d, alpha, fit_intercept, n_classes, ctx->cls))
+    return r;
   ctx->launches += 1;
   return B2_OK;
 }

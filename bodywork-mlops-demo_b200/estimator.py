@@ -1454,3 +1454,252 @@ class B200LogisticRegression(_B200GLM):
 
     def __repr__(self) -> str:
         return f"B200LogisticRegression(C={self.C})"
+
+
+# ---- RidgeClassifier: the Gram, one class-sum pass and one multi-target solve (DESIGN.md section 12) -----------------
+_SK_RIDGE_SOLVERS = ("saga", "sag", "svd", "lbfgs", "lsqr", "auto", "cholesky", "sparse_cg")
+
+
+def _class_index(classes: np.ndarray, y: np.ndarray) -> np.ndarray:
+    """float32 index of each y in the sorted classes, -1 where y is none of them"""
+    try:
+        idx = np.clip(np.searchsorted(classes, y), 0, classes.size - 1)
+        hit = classes[idx] == y
+    except TypeError:                           # labels that do not compare with classes_
+        return np.full(y.shape, -1.0, dtype=np.float32)
+    return np.where(hit, idx, -1).astype(np.float32)
+
+
+class B200RidgeClassifier(_B200Estimator):
+    """``sklearn.linear_model.RidgeClassifier`` fitted on the H100: the ridge regression of LabelBinarizer's +-1 targets
+    (one target for two classes, one per class for more) from the fp64 Gram of [x 1] (the Gram dispatch every fit uses),
+    one pass for the centred class sums and one single-SM LDL^T solve with every target as a right-hand side.  A system
+    the factorisation refuses (alpha = 0 on a rank-deficient Gram) is solved through the eigendecomposition of the
+    centred Gram instead, as scikit-learn falls back to its 'svd' solver (``solver_ = "svd"``).
+
+    Labels: host y of any dtype (``classes_`` is ``np.unique`` over the kept rows; y is staged as float32 class indices),
+    or an f32 ``DeviceArray`` beside device rows (``classes_`` are its distinct fp32 values, found on the device).
+    Refused: one class, continuous or non-finite y, multilabel (2-D) y, more than ``native.MAX_CLASSES`` classes,
+    class_weight, sample_weight, positive=True, solvers other than 'auto' / 'cholesky' and an array alpha.  copy_X,
+    max_iter, tol and random_state are accepted and have no effect."""
+    _sk_name = "RidgeClassifier"
+    _sk_attrs = ("coef_", "intercept_", "classes_", "n_features_in_", "solver_", "n_iter_")
+
+    def __init__(self, alpha: float = 1.0, *, fit_intercept: bool = True, copy_X: bool = True, max_iter=None,
+                 tol: float = 1e-4, class_weight=None, solver: str = "auto", positive: bool = False, random_state=None,
+                 ctx: Optional[native.Context] = None):
+        self.alpha = alpha
+        self.fit_intercept = fit_intercept
+        self.copy_X = copy_X
+        self.max_iter = max_iter
+        self.tol = tol
+        self.class_weight = class_weight
+        self.solver = solver
+        self.positive = positive
+        self.random_state = random_state
+        self._ctx = ctx
+
+    def _check_params(self) -> float:
+        a = self.alpha
+        if np.ndim(a) != 0:
+            raise ValueError("an array alpha (one per class) is not supported by B200RidgeClassifier: alpha must be one "
+                             "float shared by every class")
+        if isinstance(a, bool) or not isinstance(a, (int, float, np.integer, np.floating)) or not 0 <= a < np.inf:
+            raise ValueError(f"The 'alpha' parameter of RidgeClassifier must be a float in the range [0.0, inf) or an "
+                             f"array-like. Got {a!r} instead.")
+        if self.solver not in _SK_RIDGE_SOLVERS:
+            raise ValueError(f"The 'solver' parameter of RidgeClassifier must be a str among "
+                             f"{{{', '.join(repr(s) for s in _SK_RIDGE_SOLVERS)}}}. Got {self.solver!r} instead.")
+        if self.solver not in ("auto", "cholesky"):
+            raise ValueError(f"solver={self.solver!r} is not supported: B200RidgeClassifier solves the normal equations "
+                             "('auto' / 'cholesky')")
+        if self.positive:
+            raise ValueError("positive=True is not supported by B200RidgeClassifier: the coefficients are unconstrained")
+        if self.class_weight is not None:
+            raise ValueError("class_weight is not supported by B200RidgeClassifier: every kept row has weight 1")
+        return float(a)
+
+    @staticmethod
+    def _host_labels(y, row_mask, mask_keep):
+        """(classes_, y as float32 class indices (-1 for rows not kept whose label is no class), kept rows) of host y,
+        with scikit-learn's checks on the kept rows"""
+        from sklearn.utils.multiclass import check_classification_targets
+        y = np.asarray(y)
+        if y.ndim == 2 and y.shape[1] == 1:
+            y = y.ravel()
+        if y.ndim != 1:
+            raise ValueError(f"multilabel y (shape {y.shape}) is not supported by B200RidgeClassifier: y must hold one "
+                             "label per row")
+        if isinstance(row_mask, native.DeviceArray):
+            row_mask = row_mask.to_host()
+        kept = y if row_mask is None else y[np.asarray(row_mask).ravel() == mask_keep]
+        if kept.size == 0:
+            raise _too_few_rows((0,), by="B200RidgeClassifier")
+        if kept.dtype.kind in "fc":
+            if np.isnan(kept).any():
+                raise ValueError("Input y contains NaN.")
+            if np.isinf(kept).any():
+                raise ValueError(f"Input y contains infinity or a value too large for {kept.dtype!r}.")
+        check_classification_targets(kept)
+        classes = np.unique(kept)
+        B200RidgeClassifier._check_class_count(classes, classes.size > native.MAX_CLASSES)
+        return classes, _class_index(classes, y)
+
+    @staticmethod
+    def _check_class_count(classes, more: bool) -> None:
+        if more:
+            raise ValueError(f"B200RidgeClassifier fits at most {native.MAX_CLASSES} classes, y has more")
+        if classes.size < 2:
+            raise ValueError(f"B200RidgeClassifier needs samples of at least 2 classes, y holds only one: {classes[0]!r}")
+
+    @staticmethod
+    def _device_labels(ctx, y, row_mask, mask_keep):
+        """classes_ (fp32) of an f32 DeviceArray y: one label scan and one label discovery on the device"""
+        st = ctx.label_scan(y, row_mask, mask_keep)
+        if st["kept"] == 0:
+            raise _too_few_rows((0,), by="B200RidgeClassifier")
+        if st["nonfinite"] > 0:
+            raise ValueError("Input y contains NaN or infinity.")
+        if st["nonintegral"] > 0:
+            raise ValueError(_CONTINUOUS_MESSAGE)
+        values, more = ctx.label_values(y, row_mask, mask_keep, native.MAX_CLASSES)
+        B200RidgeClassifier._check_class_count(values, more)
+        return values
+
+    @contextlib.contextmanager
+    def _stage_targets(self, X, y, row_mask, mask_keep, fitting: bool):
+        """(X, y, row_mask, the fp32 classes the passes read y against, classes_) for the body of the ``with``; ``fit``
+        (classes_ found in y) and ``score`` (the fitted classes_) share it.  Device y (device rows only) is read as stored
+        against classes_; host y becomes float32 indices into classes_ (-1 outside them), uploaded beside device rows or
+        staged with host rows."""
+        ctx = self.ctx
+        if isinstance(y, native.DeviceArray):
+            if not isinstance(X, native.DeviceArray):
+                raise ValueError("device y needs device rows: X must be a DeviceArray too")
+            classes = self._device_labels(ctx, y, row_mask, mask_keep) if fitting else self.classes_
+            yield X, y, row_mask, self._fp32_classes(classes), classes
+            return
+        if fitting:
+            classes, yk = self._host_labels(y, row_mask, mask_keep)
+        else:
+            classes = self.classes_
+            yk = _class_index(classes, np.asarray(y).ravel())
+        labels = np.arange(classes.size, dtype=np.float32)
+        if isinstance(X, native.DeviceArray):
+            with _on_device(ctx, yk) as yd:
+                yield X, yd, row_mask, labels, classes
+        else:
+            with _stage_rows(ctx, X, yk, row_mask) as (X, yd, row_mask):
+                yield X, yd, row_mask, labels, classes
+
+    @staticmethod
+    def _fp32_classes(classes) -> np.ndarray:
+        """classes as the fp32 labels device y holds and device predictions return"""
+        if classes.dtype.kind not in "biuf" or not all(_fp32_exact(c) for c in classes):
+            raise ValueError(f"device labels are fp32 values, but classes_ is {classes!r}")
+        return classes.astype(np.float32)
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None) -> "B200RidgeClassifier":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, classes_,
+        n_features_in_, solver_ and n_iter_ (None)."""
+        _refuse_sample_weight(sample_weight, "B200RidgeClassifier")
+        alpha = self._check_params()
+        ctx, fi = self.ctx, bool(self.fit_intercept)
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=True) as (X, y, row_mask, labels, classes):
+            d = X.shape[1]
+            ctx.gram_reset(d)
+            ctx.gram_accumulate(X, y, row_mask, mask_keep)
+            S = ctx.gram_export()
+            n = S[d, d]
+            if n == 0:
+                raise _too_few_rows((0, d), by="B200RidgeClassifier")
+            _check_finite(S)
+            cs = ctx.class_sums(X, y, labels, S[:d, d] / n if fi else None, row_mask=row_mask, mask_keep=mask_keep)
+        if cs["kept"] != n or cs["unmatched"] > 0 or cs["nonfinite"] > 0:
+            raise RuntimeError("the class-sum pass saw other labels than the label check")
+        try:
+            coef, b0 = ctx.solve_classes(cs["sums"], alpha, fi)
+            solver = "cholesky"
+        except np.linalg.LinAlgError:
+            coef, b0 = self._solve_spectral(ctx, S, cs["sums"], alpha, fi)
+            solver = "svd"
+        _check_finite(coef, b0)
+        self.classes_, self.solver_ = classes, solver
+        self.coef_ = coef[0].copy() if classes.size == 2 else coef
+        self.intercept_ = b0 if fi else 0.0
+        self.n_features_in_ = int(d)
+        self.n_iter_ = None
+        return self
+
+    @staticmethod
+    def _solve_spectral(ctx, S, sums, alpha, fi):
+        """(W (T, d), b) of a system the LDL^T refuses, through the eigendecomposition of the centred Gram: the
+        minimum-norm solution over the eigenvalues above 1e-12 of the largest, the right-hand sides from the class sums
+        as solve_classes_kernel forms them"""
+        d = S.shape[0] - 2
+        n = S[d, d]
+        lam, Q = ctx.solve_eigh(fit_intercept=fi)
+        tot, nk = sums[:, :d].sum(axis=0), sums[:, d]
+        ks = [1] if sums.shape[0] == 2 else list(range(sums.shape[0]))
+        R = np.stack([2.0 * (sums[k, :d] - nk[k] / n * tot) if fi else 2.0 * sums[k, :d] - tot for k in ks], axis=1)
+        ev = lam + alpha
+        inv = np.where(ev > ev.max() * 1e-12, 1.0 / np.where(ev > 0, ev, 1.0), 0.0)
+        W = (Q * inv) @ (Q.T @ R)
+        if not fi:
+            return W.T, np.zeros(len(ks))
+        return W.T, (2.0 * nk[ks] / n - 1.0) - (S[:d, d] / n) @ W
+
+    def _model(self):
+        """(W (T, d), b (T,)) of the fit"""
+        W = np.atleast_2d(np.asarray(self.coef_, dtype=np.float64))
+        b = np.broadcast_to(np.asarray(self.intercept_, dtype=np.float64), (W.shape[0],))
+        return W, b
+
+    def _classify(self, X, **want):
+        """one classify pass; host rows take the class indices as labels"""
+        X = self._checked_rows(X)
+        labels = self._fp32_classes(self.classes_) if isinstance(X, native.DeviceArray) else \
+            np.arange(self.classes_.size, dtype=np.float32)
+        return self.ctx.classify(X, *self._model(), labels, **want)
+
+    def decision_function(self, X):
+        """X coef_^T + intercept_ in fp64: (n,) for two classes, (n, K) for more; float64 for host rows, an f64
+        ``DeviceArray`` for device rows."""
+        out = self._classify(X, decision=True)["decision"]
+        if self.classes_.size == 2:
+            if isinstance(out, native.DeviceArray):
+                out.shape = out.shape[:1]
+            else:
+                out = out.ravel()
+        return out
+
+    def predict(self, X):
+        """classes_ of the largest decision (two classes: classes_[1] where it is > 0): an ndarray of classes_' dtype for
+        host rows, an f32 ``DeviceArray`` for device rows (classes_ must then be fp32 values)."""
+        labels = self._classify(X, label=True)["label"]
+        if isinstance(labels, native.DeviceArray):
+            return labels
+        return self.classes_[labels.astype(np.intp)]
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """Accuracy over the kept rows (labels outside classes_ count as wrong): the counts of one classify pass."""
+        ctx = self.ctx
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=False) as (X, y, row_mask, labels, _):
+            s = ctx.classify(self._checked_rows(X), *self._model(), labels, y, row_mask=row_mask, mask_keep=mask_keep)
+        if s["kept"] == 0:
+            raise _too_few_rows((0,))
+        return float(s["correct"] / s["kept"])
+
+    def _sk_params(self) -> dict:
+        return dict(alpha=self.alpha, fit_intercept=self.fit_intercept, copy_X=self.copy_X, max_iter=self.max_iter,
+                    tol=self.tol, class_weight=self.class_weight, solver=self.solver, positive=self.positive,
+                    random_state=self.random_state)
+
+    def _sk_prepare(self, reg) -> None:
+        """the fitted LabelBinarizer scikit-learn's predict reads classes_ from"""
+        from sklearn.preprocessing import LabelBinarizer
+        reg._label_binarizer = LabelBinarizer(pos_label=1, neg_label=-1).fit(self.classes_)
+
+    def __repr__(self) -> str:
+        return f"B200RidgeClassifier(alpha={self.alpha})"

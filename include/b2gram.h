@@ -354,6 +354,43 @@ int b2_logistic_predict(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows,
 int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep,
                   double* stats_out);
 
+/* ---- RidgeClassifier (DESIGN.md section 12) ----------------------------------------------------------------------
+ * scikit-learn's RidgeClassifier solves (Xc^T Xc + alpha I) W = Xc^T Yc for the +-1 targets of LabelBinarizer: one target
+ * (the second class) with two classes, one per class with more.  A fit is the Gram of the kept rows (b2_gram_reset +
+ * b2_gram_accumulate), one b2_class_sums pass and one b2_solve_classes.  classes: n_classes (2..B2_MAX_CLASSES) finite
+ * fp32 values in strictly ascending order (host); a row's class is the index of its fp32 y among them.  B2_E_ARG: bad
+ * shapes, classes or null outputs; B2_E_UNSUPPORTED with more than one rank. */
+#define B2_MAX_CLASSES 32
+/* b2_class_sums: one fp64 pass over the kept rows (row_mask / mask_keep as b2_score; y fp32 where X lives).  sums_out
+ * (host, n_classes x (d + 1)): [k][j] = sum over the kept rows of class k of x_j - center_j (j < d, x converted exactly),
+ * [k][d] = their count; counts_out (host, 3): [0] kept rows [1] kept rows whose y is no class (NaN included) [2] kept rows
+ * whose y is not finite.  center: NULL (zeros) or d doubles (host), the column means of S for a fit with an intercept.
+ * Sums in a fixed order: repeated calls are bit-identical. */
+int b2_class_sums(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                  int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                  const double* center, double* sums_out, double* counts_out);
+/* b2_solve_classes: the model of the resident S (every kept row of some class) and the class sums (host, n_classes x
+ * (d + 1) as b2_class_sums returns them, at any center; NULL: the sums of the last b2_class_sums).  T = 1 for two
+ * classes, else n_classes: coef_out (host, T x d) and intercept_out (host, T; ybar_t - mean.w_t, 0 without
+ * fit_intercept).  Single-SM fp64 LDL^T with the T right-hand sides carried through the factorisation; B2_E_SINGULAR on a
+ * non-positive pivot (the rule of b2_solve). */
+int b2_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, const double* class_sums, int n_classes,
+                     double* coef_out, double* intercept_out);
+/* b2_classify: per row eta_t = x.coef_t + intercept_t in fp64, t < n_targets (1..B2_MAX_CLASSES); classes holds
+ * max(2, n_targets) values.  Each output optional (not all null): decision_out[i][t] = eta_t (fp64, where X lives),
+ * label_out[i] = classes[argmax_t eta_t] with the first largest winning, for n_targets = 1 classes[1] where eta > 0 and
+ * classes[0] otherwise (fp32, where X lives); counts_out (host, 2; needs y): [0] kept rows [1] kept rows whose y equals
+ * their label.  Host rows use device staging blocks in the context. */
+int b2_classify(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, const double* coef, const double* intercept,
+                int n_targets, const float* classes, double* decision_out, float* label_out, double* counts_out);
+/* b2_label_values: the distinct finite values of device fp32 y over the kept rows in ascending order (-0.0 is 0.0):
+ * values_out (host, max_values floats, 1 <= max_values <= B2_MAX_CLASSES) gets the first *n_values_out of them, *more_out
+ * = 1 when there are more.  max_values + 1 launches of integer atomics on order-preserving keys: the result does not
+ * depend on the order of the rows.  Run it after b2_label_scan has found y finite. */
+int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep, int max_values,
+                    float* values_out, int* n_values_out, int* more_out);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
