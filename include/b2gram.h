@@ -291,7 +291,8 @@ int b2_solve_ard(b2_ctx* ctx, int fit_intercept, const double* hyper, double thr
  *   ystd = sqrt(max(v^T sigma v, 0) + noise_var),  yhat = x.coef + intercept
  * mean (NULL: zeros; sklearn's X_offset_), sigma d x d, coef d: host; noise_var = 1 / alpha_.  yhat (may be NULL) and
  * ystd are n_rows fp64 where X lives (mem_kind); host rows hold two device staging blocks of 262 144 x 2 doubles in the
- * context.  One fp64 tensor-core pass over the rows.  B2_E_ARG: null sigma / coef / ystd, noise_var < 0 or not finite. */
+ * context.  One fp64 tensor-core pass over the rows; n_rows = 0 writes nothing.  B2_E_ARG: null sigma / coef / ystd,
+ * noise_var < 0 or not finite. */
 int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx, int mem_kind,
                  const double* mean, const double* sigma, double noise_var, const double* coef, double intercept,
                  double* yhat, double* ystd);
@@ -302,7 +303,8 @@ int b2_score_std(b2_ctx* ctx, const void* X, int x_dtype, int64_t n_rows, int d,
  * sklearn's pointwise loss(y, eta), gradient g and Hessian h in eta.  Sums over the kept rows are unscaled (no 1 / n, no
  * penalty) and bit-identical between calls.  y: fp32 where X lives; row_mask / mask_keep as b2_score.
  * fit_intercept = 0 takes the intercept as 0.  B2_E_ARG: bad shapes, link not one of the two below, power not finite,
- * B2_GLM_IDENTITY with power != 0, null coef or outputs; B2_E_UNSUPPORTED with more than one rank. */
+ * B2_GLM_IDENTITY with power != 0, null coef or outputs; B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or no
+ * kept row) is no error: every sum, the Hessian and the ladder are 0. */
 #define B2_GLM_LOG 0       /* mu = exp(eta), HalfTweedieLoss(power); power 1 is HalfPoissonLoss, 2 HalfGammaLoss */
 #define B2_GLM_IDENTITY 1  /* mu = eta, HalfTweedieLossIdentity, power 0 only (squared error) */
 /* b2_glm_pass: one pass at (coef, intercept).  sums_out (host, d + 8 doubles): [0] sum loss [1] sum
@@ -359,7 +361,8 @@ int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* ro
  * (the second class) with two classes, one per class with more.  A fit is the Gram of the kept rows (b2_gram_reset +
  * b2_gram_accumulate), one b2_class_sums pass and one b2_solve_classes.  classes: n_classes (2..B2_MAX_CLASSES) finite
  * fp32 values in strictly ascending order (host); a row's class is the index of its fp32 y among them.  B2_E_ARG: bad
- * shapes, classes or null outputs; B2_E_UNSUPPORTED with more than one rank. */
+ * shapes, classes or null outputs; B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or no kept row) is no error:
+ * the sums and counts are 0, and b2_classify writes no row. */
 #define B2_MAX_CLASSES 32
 /* b2_class_sums: one fp64 pass over the kept rows (row_mask / mask_keep as b2_score; y fp32 where X lives).  sums_out
  * (host, n_classes x (d + 1)): [k][j] = sum over the kept rows of class k of x_j - center_j (j < d, x converted exactly),

@@ -46,7 +46,9 @@ class NumpyGLMContext:
             pointwise = loss.loss(y_true=yd, raw_prediction=raw)
             g, h = loss.gradient_hessian(y_true=yd, raw_prediction=raw)
             const = loss.constant_to_optimal_zero(yd)
-        in_range = np.array([loss.in_y_true_range(np.array([v])) for v in yd], dtype=bool)
+        iv = loss.interval_y_true          # in_y_true_range's test, row by row
+        in_range = (yd >= iv.low if iv.low_inclusive else yd > iv.low) & \
+            (yd <= iv.high if iv.high_inclusive else yd < iv.high)
         Z = np.c_[Xd, np.ones(len(yd))]
         return {"loss": float(pointwise.sum()), "const": float(const.sum()), "sum_y": float(yd.sum()),
                 "kept": float(len(yd)), "y_out_of_range": float(np.sum(~in_range)), "h_nonpos": float(np.sum(h <= 0)),
