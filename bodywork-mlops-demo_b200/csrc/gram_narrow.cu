@@ -19,7 +19,12 @@
 //
 // Precision: products are fp32 FMAs (round to nearest, 2^-24) of shifted values, chains are at most kFlushRows long
 // before they are folded into fp64, and the rounding errors are zero-mean across ~10^5 lanes: the statistic is
-// accurate to ~1e-7 relative, coefficient error vs the fp64 oracle ~1e-7 (tests/test_gpu_parity.py).
+// accurate to ~1e-7 relative, coefficient error vs the fp64 oracle ~1e-7 (tests/test_gpu_parity.py).  That rests on the
+// averaging: the worst case of one 2048-row chain is 2047 x 2^-24 = 1.2e-4 relative.  bf16 rows do not average as well:
+// their values sit on a coarse grid, so x - c has the same low bits in every row and the roundings of a chain have a mean
+// that depends on the shift (a float32 model of the chains gives 5e-9 to 2e-6 relative on sum v^2 across shifts, against
+// ~4e-8 for fp32 values).  Measured at 7e7-2e8 bf16 rows on one dataset: 4e-7 relative on the raw statistic, 9e-6 on the
+// centred moments and 5e-6 on the coefficients (tests/test_gpu_stream_rings.py).
 #include <cuda_bf16.h>
 
 #include "b2_internal.cuh"

@@ -253,7 +253,8 @@ int b2_ridge_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_
  * gradient kernels: out (host, d + 2 doubles) = sum (x_j - m_j) e, then sum e, then sum e^2, e = y - intercept - x.coef,
  * everything from the exactly converted stored values; m are the column means of the resident S (0 without
  * fit_intercept), which must have d features.  At the least-squares solution w0 of S (b2_fit, or b2_solve_spectral when
- * the factorisation refuses) with intercept ybar - m.w0 this is the anchor [w0 | out] of the solves below.
+ * the factorisation refuses) with intercept ybar - m.w0 this is the anchor [w0 | out] of the solves below.  No rows (or
+ * no kept row): out is d + 2 zeros.
  * B2_E_UNSUPPORTED with more than one rank; B2_E_STATE when the resident S has another d. */
 int b2_residual_moments(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                         int mem_kind, const uint8_t* row_mask, int mask_keep, const double* coef, double intercept,
@@ -397,7 +398,8 @@ int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* 
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
- * yhat may be NULL (metrics only); y may be NULL (predict only; stats_out untouched).
+ * yhat may be NULL (metrics only); y may be NULL (predict only; stats_out untouched).  n_rows == 0: no launch, yhat
+ * untouched, stats_out (with y) ten zeros.
  * stats_out (host, 10 doubles):
  *   [0] sum |yhat-y|/max(|y|,eps_f64)  [1] sum (y-yhat)^2  [2] sum y  [3] sum y^2  [4] max |y-yhat|  [5] rows used
  *   [6] sum yhat  [7] sum yhat^2  [8] sum y*yhat  [9] max |yhat/y - 1|
