@@ -28,6 +28,7 @@ MAX_ALPHAS = 64
 GLM_LOG, GLM_IDENTITY = 0, 1
 GLM_STEPS = 21
 MAX_CLASSES = 32
+LOO_SQUARED, LOO_ACCURACY = 0, 1
 
 _c_i64 = C.c_int64
 _vp = C.c_void_p
@@ -104,6 +105,9 @@ _SIGNATURES = {
                               _vp, _vp, _vp, _vp]),
     "b2_label_values": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, C.c_int, _vp, C.POINTER(C.c_int),
                                   C.POINTER(C.c_int)]),
+    "b2_ridge_classifier_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
+                                          C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_int), _vp,
+                                          _vp, _vp]),
     "b2_score": (C.c_int, [_vp, _vp, C.c_int, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_double, _vp, _vp,
                            C.c_int, _vp, _vp]),
     "b2_score_allreduce": (C.c_int, [_vp, _vp]),
@@ -894,6 +898,46 @@ class Context:
                                     C.byref(found), C.byref(more))
         _check_args(rc, "b2_label_values")
         return vals[: found.value].copy(), bool(more.value)
+
+    # -- RidgeClassifierCV (DESIGN.md section 13) ------------------------------------------------------------------
+    def ridge_classifier_loo(self, X, y, classes, alphas, row_mask=None, mask_keep: int = 1, *,
+                             fit_intercept: bool = True, scoring: int = LOO_SQUARED, store_cv: bool = False) -> dict:
+        """RidgeClassifierCV(alphas).fit's leave-one-out search in one call (b2_ridge_classifier_loo): ``classes`` are K
+        sorted fp32 values (a row's class is the index of its y among them), up to MAX_ALPHAS alphas.  Returns a dict:
+        mse and correct per alpha, best (the first smallest mse, or the first largest correct with LOO_ACCURACY), coef
+        (T, d) and intercept (T,) at alphas[best] (T = 1 for two classes, else K), kept / unmatched / nonfinite (the
+        class-sum pass's counts) and cv: None, or (n, T, n_alphas) e^2 (p = t - e with LOO_ACCURACY), NaN on rows not
+        kept -- a float64 ndarray for host rows, an f64 DeviceArray for device rows.  Raises ``ValueError`` for bad
+        arguments and no kept row, ``np.linalg.LinAlgError`` when the solve at alphas[best] meets a non-positive pivot
+        (every other entry is then set: the dict rides on the exception as its ``result``)."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        al = np.ascontiguousarray(np.asarray(alphas, dtype=np.float64).ravel())
+        t = 1 if cl.size == 2 else max(cl.size, 1)
+        mse = np.empty(max(al.size, 1), dtype=np.float64)
+        correct = np.empty(max(al.size, 1), dtype=np.float64)
+        coef = np.empty((t, max(d, 1)), dtype=np.float64)
+        b0 = np.empty(t, dtype=np.float64)
+        counts = np.zeros(3, dtype=np.float64)
+        best = C.c_int(0)
+        cv, cv_ptr = self._out(mk, (n, t, al.size), "f64", store_cv)
+        rc = load().b2_ridge_classifier_loo(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data,
+                                            cl.size, al.ctypes.data, int(al.size), int(bool(fit_intercept)),
+                                            int(scoring), mse.ctypes.data, correct.ctypes.data, cv_ptr,
+                                            C.byref(best), coef.ctypes.data, b0.ctypes.data, counts.ctypes.data)
+        self.d = int(d)
+        self.serial += 1
+        out = {"mse": mse[: al.size], "correct": correct[: al.size], "best": int(best.value), "coef": coef,
+               "intercept": b0, "kept": float(counts[0]), "unmatched": float(counts[1]),
+               "nonfinite": float(counts[2]), "cv": cv}
+        if rc == E_SINGULAR and "LDL" in last_error():
+            exc = np.linalg.LinAlgError(last_error())
+            exc.result = out
+            raise exc
+        if rc != 0 and isinstance(cv, DeviceArray):
+            cv.free()
+        _check_args(rc, "b2_ridge_classifier_loo")
+        return out
 
     # -- scoring ------------------------------------------------------------------------------------------
     def metrics(self, y_actual, y_predicted) -> np.ndarray:

@@ -282,9 +282,9 @@ int stream_host_blocks(b2_ctx* ctx, int64_t n_rows, int64_t blk_rows, Stage stag
   return B2_OK;
 }
 
-// The row-output blocks grown to row_bytes per row (their contents are not kept)
-int ensure_row_out(b2_ctx* ctx, size_t row_bytes) {
-  if (ctx->row_out_bytes >= row_bytes) return B2_OK;
+// The row-output blocks grown to block_bytes each (their contents are not kept)
+int ensure_row_out(b2_ctx* ctx, size_t block_bytes) {
+  if (ctx->row_out_bytes >= block_bytes) return B2_OK;
   if (ctx->row_out[0] != nullptr) B2_CUDA(cudaStreamSynchronize(ctx->stream));   // an earlier call's copies may still read them
   for (int b = 0; b < 2; ++b) {
     if (ctx->row_out[b] != nullptr) cudaFree(ctx->row_out[b]);
@@ -292,12 +292,12 @@ int ensure_row_out(b2_ctx* ctx, size_t row_bytes) {
   }
   ctx->row_out_bytes = 0;
   for (int b = 0; b < 2; ++b)
-    if (cudaMalloc(reinterpret_cast<void**>(&ctx->row_out[b]), (size_t)ctx->stage_rows * row_bytes) != cudaSuccess) {
+    if (cudaMalloc(reinterpret_cast<void**>(&ctx->row_out[b]), block_bytes) != cudaSuccess) {
       cudaGetLastError();
       set_error("out of device memory for the staging blocks of the per-row outputs");
       return B2_E_CUDA;
     }
-  ctx->row_out_bytes = row_bytes;
+  ctx->row_out_bytes = block_bytes;
   return B2_OK;
 }
 
@@ -313,12 +313,15 @@ struct RowOut {
 // Device rows: one launch on the caller's pointers.  Host rows: one launch per block of the staging ring, its outputs
 // written to the row-output blocks and copied back behind it; with outputs, the stream is synchronised before the
 // return, so the caller may reuse every host buffer -- also when a block failed.  Zero rows: one launch on zero rows.
+// max_blk_rows > 0 caps the rows of a host block below the staging ring's (wide per-row outputs).
 template <typename Launch>
 int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx, int mem_kind,
-             const uint8_t* mask, Launch&& launch, RowOut out0 = {}, RowOut out1 = {}, RowOut out2 = {}) {
+             const uint8_t* mask, Launch&& launch, RowOut out0 = {}, RowOut out1 = {}, RowOut out2 = {},
+             int64_t max_blk_rows = 0) {
   if (mem_kind == B2_MEM_DEVICE) return launch(RowSpan{X, y, mask, ldx, 0, n_rows, true}, out0.dst, out1.dst, out2.dst);
   if (n_rows == 0) return launch(RowSpan{nullptr, nullptr, nullptr, d, 0, 0, true}, nullptr, nullptr, nullptr);
   if (int r = ensure_staging(ctx)) return r;
+  const int64_t blk = max_blk_rows > 0 && max_blk_rows < ctx->stage_rows ? max_blk_rows : ctx->stage_rows;
   RowOut out[3] = {out0, out1, out2};
   size_t out_bytes = 0;
   for (RowOut& o : out) {
@@ -326,20 +329,19 @@ int row_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_
     out_bytes += o.row_bytes;
   }
   if (out_bytes > 0)
-    if (int r = ensure_row_out(ctx, out_bytes)) return r;
+    if (int r = ensure_row_out(ctx, (size_t)blk * out_bytes)) return r;
   const int es = x_dtype == B2_F32 ? 4 : 2;
   const bool x_pinned = host_pointer_is_pinned(X);
   const int rc = stream_host_blocks(
-      ctx, n_rows, ctx->stage_rows,
+      ctx, n_rows, blk,
       [&](int buf, int64_t r0, int64_t rows) {
         return stage_rows_h2d(ctx, buf, X, es, y, mask, r0, rows, d, ldx, x_pinned);
       },
       [&](int buf, int64_t r0, int64_t rows) -> int {
-        char* const block = ctx->row_out[buf];   // [stage_rows] of output 0, then of output 1, then of output 2
+        char* const block = ctx->row_out[buf];   // [blk] of output 0, then of output 1, then of output 2
         char* dev[3] = {out[0].dst != nullptr ? block : nullptr,
-                        out[1].dst != nullptr ? block + (size_t)ctx->stage_rows * out[0].row_bytes : nullptr,
-                        out[2].dst != nullptr
-                            ? block + (size_t)ctx->stage_rows * (out[0].row_bytes + out[1].row_bytes) : nullptr};
+                        out[1].dst != nullptr ? block + (size_t)blk * out[0].row_bytes : nullptr,
+                        out[2].dst != nullptr ? block + (size_t)blk * (out[0].row_bytes + out[1].row_bytes) : nullptr};
         const RowSpan s{ctx->stage_x[buf], y != nullptr ? ctx->stage_y[buf] : nullptr,
                         mask != nullptr ? ctx->stage_m[buf] : nullptr, d, r0, rows, r0 == 0};
         if (int r = launch(s, dev[0], dev[1], dev[2])) return r;
@@ -478,7 +480,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part,
-                  ctx->cls};
+                  ctx->cls, ctx->loo_cls};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1839,6 +1841,87 @@ int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* 
   *n_values_out = found;
   *more_out = h[max_values] != ~0ull ? 1 : 0;
   return B2_OK;
+}
+
+// ---- RidgeClassifierCV (DESIGN.md section 13) -----------------------------------------------------------------------
+// Host rows with cv_out stream in blocks whose cv block stays within the 262 144 x 64 doubles of b2_ridge_loo's widest
+constexpr size_t kLooOutBlockBytes = ((size_t)1 << 18) * kMaxAlphas * sizeof(double);
+
+// The Gram of the kept rows, the class sums at its column means (b2_class_sums), the eigendecomposition of the centred
+// Gram, one leave-one-out pass with T targets over the same rows, the first best alpha, then b2_solve_classes there.
+int b2_ridge_classifier_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                            int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                            const double* alphas, int n_alphas, int fit_intercept, int scoring, double* mse_out,
+                            double* correct_out, double* cv_out, int* best_out, double* coef_out, double* intercept_out,
+                            double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (alphas == nullptr || n_alphas < 1 || n_alphas > kMaxAlphas) {
+    set_error("n_alphas=%d out of range [1,%d] (or alphas is null)", n_alphas, kMaxAlphas);
+    return B2_E_ARG;
+  }
+  for (int a = 0; a < n_alphas; ++a)
+    if (!(isfinite(alphas[a]) && alphas[a] > 0.0)) {
+      set_error("alphas[%d] == %g, must be > 0.0 and finite", a, alphas[a]);
+      return B2_E_ARG;
+    }
+  if (int r = check_classes(classes, n_classes)) return r;
+  if (scoring != B2_LOO_SQUARED && scoring != B2_LOO_ACCURACY) {
+    set_error("scoring=%d: B2_LOO_SQUARED or B2_LOO_ACCURACY expected", scoring);
+    return B2_E_ARG;
+  }
+  if (mse_out == nullptr || correct_out == nullptr || best_out == nullptr || coef_out == nullptr ||
+      intercept_out == nullptr || counts_out == nullptr) {
+    set_error("mse_out / correct_out / best_out / coef_out / intercept_out / counts_out is null");
+    return B2_E_ARG;
+  }
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (int r = ensure_cls(ctx, "b2_ridge_classifier_loo")) return r;
+  if (ctx->loo_cls == nullptr) B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->loo_cls), sizeof(double) * kLcDoubles));
+  // (1) the Gram, (2) the class sums at its column means
+  if (int r = b2_gram_reset(ctx, d)) return r;
+  if (int r = gram_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep)) return r;
+  std::vector<double> S((size_t)(d + 2) * (d + 2));
+  if (int r = b2_gram_export(ctx, S.data(), nullptr)) return r;
+  const double n_kept = S[(size_t)d * (d + 2) + d];
+  if (!(n_kept > 0.0)) { set_error("no row kept: the leave-one-out error needs at least one row"); return B2_E_ARG; }
+  std::vector<double> center(d), sums((size_t)n_classes * (d + 1));
+  for (int j = 0; j < d; ++j) center[j] = S[(size_t)j * (d + 2) + d] / n_kept;
+  if (int r = b2_class_sums(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, classes, n_classes,
+                            fit_intercept ? center.data() : nullptr, sums.data(), counts_out))
+    return r;
+  // (3) the eigendecomposition, (4) the pass
+  if (int r = launch_solve_eigh(ctx, fit_intercept)) return r;
+  B2_CUDA(cudaMemcpyAsync(ctx->loo + kLooAlpha, alphas, sizeof(double) * n_alphas, cudaMemcpyHostToDevice, ctx->stream));
+  double converged = 0.0;
+  B2_CUDA(cudaMemcpyAsync(&converged, ctx->loo + kLooMisc + 3, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (int r = eigh_converged(converged)) return r;
+  const int T = n_classes == 2 ? 1 : n_classes;
+  const size_t cv_row = sizeof(double) * T * n_alphas;
+  const bool accuracy = scoring == B2_LOO_ACCURACY;
+  if (int r = row_pass(
+          ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask,
+          [&](const RowSpan& s, void* cv, void*, void*) {
+            return launch_loo_classes(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_classes, n_alphas,
+                                      fit_intercept, accuracy, static_cast<double*>(cv), s.first);
+          },
+          RowOut{cv_out, cv_row}, {}, {}, cv_out != nullptr ? (int64_t)(kLooOutBlockBytes / cv_row) & ~(int64_t)31 : 0))
+    return r;
+  double h[kLcPart];
+  B2_CUDA(cudaMemcpyAsync(h, ctx->loo_cls + kLcSum, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  // (5) the first alpha with the strictly best score: the smallest mse, or the most rows right
+  int best = 0;
+  for (int a = 0; a < n_alphas; ++a) {
+    mse_out[a] = h[a] / (n_kept * T);
+    correct_out[a] = h[kMaxAlphas + a];
+    const bool better = accuracy ? correct_out[a] > correct_out[best] : mse_out[a] < mse_out[best];
+    if (better) best = a;
+  }
+  *best_out = best;
+  // (6) the model there
+  return b2_solve_classes(ctx, alphas[best], fit_intercept, nullptr, n_classes, coef_out, intercept_out);
 }
 
 // ---- scoring ---------------------------------------------------------------------------------------

@@ -163,6 +163,24 @@ constexpr int kClsInfo = kClsIntercept + kMaxClasses;
 constexpr int kClsCounts = kClsInfo + 8;
 constexpr int kClsSums = kClsCounts + 8;
 constexpr int kClsDoubles = kClsSums + kClsPart;
+// the class of a kept row: the index of y in the sorted classes, -1 when y is none of them (NaN included)
+__device__ __forceinline__ int class_of(const float* cls, int n_classes, float y) {
+  int k = -1;
+  for (int c = 0; c < n_classes; ++c) k = cls[c] == y ? c : k;
+  return k;
+}
+
+// ---- the leave-one-out pass of b2_ridge_classifier_loo (ridge_loo.cu; DESIGN.md section 13) --------------------------
+// doubles of ctx->loo_cls: the B operands of one call (built by its prep kernel from ctx->loo and the class sums at
+// ctx->cls + kClsSums), ybar per target, and the reduced sums per alpha: sum e^2 over every target, rows whose first
+// argmax of p = t - e is their class.  The per-CTA partials [grid][kLcPart] live in ctx->glm_part.
+constexpr int kLcW = 0;                                    // [kMaxD][kMaxAlphas] 1 / (lambda_j + alpha_a)
+constexpr int kLcCw = kLcW + kMaxD * kMaxAlphas;           // [kMaxD][T][8 ceil(A / 8)] C_jt / (lambda_j + alpha_a)
+constexpr int kLcC = kLcCw + kMaxD * kMaxClasses * kMaxAlphas;   // [kMaxD][kMaxClasses] C = Q^T R
+constexpr int kLcYbar = kLcC + kMaxD * kMaxClasses;        // [kMaxClasses] 2 n_k / n - 1 (0 without an intercept)
+constexpr int kLcSum = kLcYbar + kMaxClasses;              // [2][kMaxAlphas] sum e^2, correct rows
+constexpr int kLcPart = 2 * kMaxAlphas;
+constexpr int kLcDoubles = kLcSum + kLcPart;
 
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
@@ -249,6 +267,8 @@ struct b2_ctx {
   double* glm_part = nullptr;
   // the ridge classifier's operands and sums (b2::kCls*), allocated by the first call; its per-CTA partials in glm_part
   double* cls = nullptr;
+  // the classifier's leave-one-out operands and sums (b2::kLc*, 2.1 MB), allocated by the first call
+  double* loo_cls = nullptr;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -264,8 +284,8 @@ struct b2_ctx {
   cudaEvent_t ev_copied[2] = {nullptr, nullptr};
   cudaEvent_t ev_consumed[2] = {nullptr, nullptr};
   bool ev_consumed_valid[2] = {false, false};   // a kernel of an earlier call may still read stage buffer b
-  // the per-row outputs of host rows (yhat, ystd, e^2, mu): two blocks of stage_rows x row_out_bytes, grown to the
-  // widest call
+  // the per-row outputs of host rows (yhat, ystd, e^2, mu): two blocks of row_out_bytes each (at most stage_rows rows),
+  // grown to the largest call
   char* row_out[2] = {nullptr, nullptr};
   size_t row_out_bytes = 0;
   void* bounce[2] = {nullptr, nullptr};         // pinned bounce blocks for pageable host rows (filled by host threads)
@@ -417,6 +437,13 @@ int launch_solve_eigh(b2_ctx* ctx, int fit_intercept);
 // reduce of the per-CTA sums into ctx->loo + kLooSum (`first_block` overwrites, otherwise adds)
 int launch_loo(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                const uint8_t* mask, int keep, int n_alphas, double* cv, bool first_block);
+// the classifier's leave-one-out pass over the rows [0, n) for the n_alphas alphas at ctx->loo + kLooAlpha, the
+// eigendecomposition in ctx->loo and the classes and class sums in ctx->cls: the B operands (once per call,
+// `first_block`), the pass (cv [row][T][n_alphas] when not null: e^2, or p = t - e with `accuracy`; NaN for rows not
+// kept) and the ordered reduce of the per-CTA sums into ctx->loo_cls + kLcSum (`first_block` overwrites, else adds)
+int launch_loo_classes(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                       const uint8_t* mask, int keep, int n_classes, int n_alphas, int fit_intercept, bool accuracy,
+                       double* cv, bool first_block);
 // the elastic-net path of the resident S (one launch; `args` points into ctx->enet)
 int launch_solve_enet(b2_ctx* ctx, const EnetArgs& args);
 // BayesianRidge's iteration in the eigenbasis of ctx->loo (launch_solve_eigh first); one launch

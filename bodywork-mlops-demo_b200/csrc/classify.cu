@@ -17,13 +17,6 @@
 namespace b2 {
 namespace {
 
-// the class of a kept row: the index of y in the sorted classes, -1 when y is none of them (NaN included)
-__device__ __forceinline__ int class_of(const float* cls, int n_classes, float y) {
-  int k = -1;
-  for (int c = 0; c < n_classes; ++c) k = cls[c] == y ? c : k;
-  return k;
-}
-
 // shared memory of the class-sum pass: the ring, the tile [kTileRows][vp], the two halves' class rows [2][K][dp], the
 // centre, the classes, the rows' classes and the warps' counts [kTileWarps][K + 3]
 size_t class_sums_smem_bytes(int dp, int n_classes, bool ring) {

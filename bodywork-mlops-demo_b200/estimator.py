@@ -1703,3 +1703,122 @@ class B200RidgeClassifier(_B200Estimator):
 
     def __repr__(self) -> str:
         return f"B200RidgeClassifier(alpha={self.alpha})"
+
+
+# ---- RidgeClassifierCV: the leave-one-out error of every class and alpha in one pass (DESIGN.md section 13) ------------
+def _checked_statistic(ctx: native.Context, d: int, res: dict) -> np.ndarray:
+    """S of one b2_ridge_classifier_loo call, after B200RidgeClassifier.fit's checks: finite, and the class-sum pass kept
+    the Gram's rows, every one of them of some class"""
+    S = ctx.gram_export()
+    _check_finite(S)
+    if res["kept"] != S[d, d] or res["unmatched"] > 0 or res["nonfinite"] > 0:
+        raise RuntimeError("the class-sum pass saw other labels than the label check")
+    return S
+
+
+class B200RidgeClassifierCV(B200RidgeClassifier):
+    """``sklearn.linear_model.RidgeClassifierCV(alphas, scoring=..., store_cv_results=...)`` with its default ``cv=None``,
+    fitted on the H100 by ``b2_ridge_classifier_loo``: the Gram, the class sums, the eigendecomposition of the centred
+    Gram and one fp64 pass over the rows for the exact leave-one-out error of every class target and alpha, per chunk of
+    up to MAX_ALPHAS alphas; then ``B200RidgeClassifier``'s solve at the chosen alpha (and its eigendecomposition fallback
+    when the factorisation refuses the system).
+
+    ``scoring=None`` chooses the first alpha with the smallest mean of e^2 over every row and target; ``"accuracy"`` the
+    first with the most kept rows whose largest leave-one-out prediction p = t - e is at their class.  With two classes
+    there is one target, and scikit-learn's accuracy scorer then compares the argmax of one column with the argmax of one
+    column: every alpha scores 1.0 and the first alpha is chosen.  This restates scikit-learn exactly.
+
+    Labels, predict, decision_function, score and the export are ``B200RidgeClassifier``'s.  Refused: alphas <= 0 or not
+    finite, cv other than None (the k-fold grid search), scorers other than None and "accuracy", class_weight,
+    sample_weight, and what ``B200RidgeClassifier`` refuses of y."""
+    _sk_name = "RidgeClassifierCV"
+
+    def __init__(self, alphas=(0.1, 1.0, 10.0), *, fit_intercept: bool = True, scoring=None, cv=None,
+                 class_weight=None, store_cv_results: bool = False, ctx: Optional[native.Context] = None):
+        self.alphas = alphas
+        self.fit_intercept = fit_intercept
+        self.scoring = scoring
+        self.cv = cv
+        self.class_weight = class_weight
+        self.store_cv_results = store_cv_results
+        self._ctx = ctx
+
+    def _check_params(self) -> np.ndarray:
+        al = _check_alphas(self.alphas)
+        if self.cv is not None:
+            raise ValueError(f"cv={self.cv!r} is not supported by B200RidgeClassifierCV: it runs the leave-one-out "
+                             "search of cv=None, not the k-fold grid search")
+        if not (self.scoring is None or (isinstance(self.scoring, str) and self.scoring == "accuracy")):
+            raise ValueError(f"scoring={self.scoring!r} is not supported by B200RidgeClassifierCV: None (mean squared "
+                             "leave-one-out error) or 'accuracy'")
+        if self.class_weight is not None:
+            raise ValueError("class_weight is not supported by B200RidgeClassifierCV: every kept row has weight 1")
+        return al
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None) -> "B200RidgeClassifierCV":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets alpha_, best_score_, coef_, intercept_,
+        classes_, n_features_in_ and, with store_cv_results, cv_results_ of shape (rows kept, T, n_alphas)."""
+        _refuse_sample_weight(sample_weight, "B200RidgeClassifierCV")
+        al = self._check_params()
+        ctx, fi = self.ctx, bool(self.fit_intercept)
+        accuracy = self.scoring == "accuracy"
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=True) as (X, y, row_mask, labels, classes):
+            d = X.shape[1]
+            chunks, cvs, sols = [], [], []
+            for off in range(0, al.size, native.MAX_ALPHAS):
+                part = al[off: off + native.MAX_ALPHAS]
+                try:
+                    res = ctx.ridge_classifier_loo(X, y, labels, part, row_mask, mask_keep, fit_intercept=fi,
+                                                   scoring=native.LOO_ACCURACY if accuracy else native.LOO_SQUARED,
+                                                   store_cv=self.store_cv_results)
+                    coef, b0 = res["coef"], res["intercept"]
+                    _checked_statistic(ctx, d, res)
+                except np.linalg.LinAlgError as exc:
+                    # scikit-learn's fallback to its 'svd' solver, from the statistic the call left resident
+                    res = exc.result
+                    S = _checked_statistic(ctx, d, res)
+                    cs = ctx.class_sums(X, y, labels, S[:d, d] / S[d, d] if fi else None, row_mask=row_mask,
+                                        mask_keep=mask_keep)
+                    coef, b0 = self._solve_spectral(ctx, S, cs["sums"], float(part[res["best"]]), fi)
+                except ValueError as exc:
+                    if "no row kept" in str(exc):
+                        raise _too_few_rows((0, d), by="B200RidgeClassifierCV") from None
+                    raise
+                n = res["kept"]
+                chunks.append((off, res["mse"], res["correct"]))
+                sols.append((off + res["best"], coef, b0))
+                cv = res["cv"]
+                if cv is not None:
+                    cvs.append(cv.to_host() if isinstance(cv, native.DeviceArray) else cv)
+                    if isinstance(cv, native.DeviceArray):
+                        cv.free()
+        best = merge_alpha_chunks([(off, -c if accuracy else m) for off, m, c in chunks])
+        mse_all = np.concatenate([m for _, m, _ in chunks])
+        correct_all = np.concatenate([c for _, _, c in chunks])
+        coef, b0 = next((c, b) for i, c, b in sols if i == best)
+        _check_finite(coef, b0, mse_all[best])
+        self.alpha_ = float(al[best])
+        self.best_score_ = float(correct_all[best] / n) if accuracy else float(-mse_all[best])
+        self.classes_ = classes
+        self.coef_ = coef[0].copy() if classes.size == 2 else coef
+        self.intercept_ = b0 if fi else 0.0
+        self.n_features_in_ = int(d)
+        if self.store_cv_results:
+            cv = np.concatenate(cvs, axis=2)
+            keep = ~np.isnan(cv[:, 0, 0]) if cv.shape[0] else np.zeros(0, bool)
+            self.cv_results_ = cv[keep]
+        return self
+
+    @property
+    def _sk_attrs(self) -> tuple:
+        return ("alpha_", "best_score_", "coef_", "intercept_", "classes_", "n_features_in_") \
+            + (("cv_results_",) if self.store_cv_results else ())
+
+    def _sk_params(self) -> dict:
+        return dict(alphas=np.asarray(self.alphas, dtype=np.float64), fit_intercept=self.fit_intercept,
+                    scoring=self.scoring, cv=self.cv, class_weight=self.class_weight,
+                    store_cv_results=self.store_cv_results)
+
+    def __repr__(self) -> str:
+        return f"B200RidgeClassifierCV(alphas={self.alphas!r})"

@@ -395,6 +395,34 @@ int b2_classify(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t
 int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep, int max_values,
                     float* values_out, int* n_values_out, int* more_out);
 
+/* ---- RidgeClassifierCV: replaces sklearn.linear_model.RidgeClassifierCV(alphas).fit with cv=None (DESIGN.md
+ * section 13) ---------------------------------------------------------------------------------------------------------
+ * The leave-one-out error of every class target and alpha: the Gram of the kept rows, b2_class_sums at its column means,
+ * the eigendecomposition of the centred Gram (b2_solve_eigh), one fp64 pass over the same rows with the T targets
+ * (T = 1 for two classes, else n_classes) t_k = +1 where the row's class is k (class 1 when T = 1) and -1 otherwise,
+ * centred by ybar_k = 2 n_k / n - 1 with an intercept; then b2_solve_classes at alphas[best].  Per kept row, target and
+ * alpha: e_k = ((t_k - ybar_k) - yhat_k) / (1 - h), p_k = t_k - e_k.  classes and y as b2_class_sums; as for
+ * b2_solve_classes, the right-hand sides assume every kept row is of some class (counts_out[1] == 0).
+ *   scoring      B2_LOO_SQUARED: best is the first smallest mse_out; B2_LOO_ACCURACY: the first largest correct_out
+ *   mse_out      n_alphas (host): sum of e_k^2 over the kept rows and targets / (n T)
+ *   correct_out  n_alphas (host): kept rows whose first argmax of p is the first argmax of t (every kept row when T = 1,
+ *                as scikit-learn's accuracy scorer counts one column)
+ *   cv_out       NULL, or n_rows x T x n_alphas doubles where X lives (mem_kind): e^2 (B2_LOO_SQUARED) or p
+ *                (B2_LOO_ACCURACY), NaN for rows not kept.  Host rows hold two device staging blocks of at most 134 MB
+ *                (fewer rows per block as T n_alphas grows) in the context.
+ *   best_out     the chosen alpha's index; coef_out (T x d) and intercept_out (T): b2_solve_classes there
+ *   counts_out   3 (host): the class-sum pass's kept rows, kept rows of no class, kept rows with y not finite
+ * Sums in a fixed order: repeated calls are bit-identical.  B2_E_ARG: bad alphas, classes or scoring, null outputs, or
+ * no kept row; B2_E_UNSUPPORTED with more than one rank; B2_E_SINGULAR from the eigendecomposition or the solve (every
+ * output but coef_out / intercept_out is then written). */
+#define B2_LOO_SQUARED 0
+#define B2_LOO_ACCURACY 1
+int b2_ridge_classifier_loo(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                            int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                            const double* alphas, int n_alphas, int fit_intercept, int scoring, double* mse_out,
+                            double* correct_out, double* cv_out, int* best_out, double* coef_out, double* intercept_out,
+                            double* counts_out);
+
 /* ---- scoring: replaces model.predict and model_metrics ------------------------------------------
  * reference: stage_1_train_model.py:107 / stage_2_serve_model.py:78 (X @ coef_ + intercept_)
  *            stage_1_train_model.py:79-90 (MAPE, r2_score, max_error)
