@@ -23,13 +23,18 @@ Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- th
                            with every class as a right-hand side; decisions and labels in one fp64 tensor-core pass
     B200RidgeClassifierCV  sklearn's RidgeClassifierCV (cv=None): the alpha chosen by the exact leave-one-out error of
                            every class target, all alphas in one fp64 pass over the rows
+    B200MultinomialLogisticRegression
+                           sklearn's LogisticRegression (solver="newton-cholesky") for 2 to 32 classes: multinomial
+                           Newton fits with every class-pair Hessian block on the fp64 tensor core (two classes: the
+                           binary fit)
     stage_1_train_model    drop-in for mlops_simulation/stage_1_train_model.py
 """
 from . import _native as native
 from ._native import (BF16, F32, KERNEL_AUTO, KERNEL_NARROW, KERNEL_SIMT, KERNEL_TCGEN05, PRECISION_BF16, PRECISION_SPLIT, Context,
                       DeviceArray, PinnedArray)
 from .estimator import (B200ARDRegression, B200BayesianRidge, B200ElasticNet, B200ElasticNetCV, B200GammaRegressor,
-                        B200Lasso, B200LassoCV, B200LinearRegression, B200LogisticRegression, B200PoissonRegressor,
+                        B200Lasso, B200LassoCV, B200LinearRegression, B200LogisticRegression, B200MultinomialLogisticRegression,
+                        B200PoissonRegressor,
                         B200RidgeClassifier, B200RidgeClassifierCV, B200RidgeCV, B200TweedieRegressor, default_context,
                         enet_path, fold_ids, lasso_path)
 from . import sharding, tranche_io  # noqa: F401
@@ -37,6 +42,6 @@ from . import sharding, tranche_io  # noqa: F401
 __all__ = ["native", "Context", "DeviceArray", "PinnedArray", "B200LinearRegression", "B200RidgeCV", "B200ElasticNet",
            "B200Lasso", "B200ElasticNetCV", "B200LassoCV", "B200BayesianRidge", "B200ARDRegression",
            "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression",
-           "B200RidgeClassifier", "B200RidgeClassifierCV", "fold_ids", "enet_path", "lasso_path", "default_context",
+           "B200RidgeClassifier", "B200RidgeClassifierCV", "B200MultinomialLogisticRegression", "fold_ids", "enet_path", "lasso_path", "default_context",
            "F32", "BF16", "KERNEL_AUTO", "KERNEL_SIMT", "KERNEL_TCGEN05", "KERNEL_NARROW", "PRECISION_SPLIT", "PRECISION_BF16"]
 __version__ = "0.1.0"

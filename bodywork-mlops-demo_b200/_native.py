@@ -105,6 +105,11 @@ _SIGNATURES = {
                               _vp, _vp, _vp, _vp]),
     "b2_label_values": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, C.c_int, _vp, C.POINTER(C.c_int),
                                   C.POINTER(C.c_int)]),
+    "b2_multinomial_pass": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
+                                      C.c_int, _vp, C.c_int, _vp, _vp]),
+    "b2_multinomial_line_search": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int,
+                                             _vp, C.c_int, _vp, _vp, C.c_int, _vp]),
+    "b2_softmax_rows": (C.c_int, [_vp, _vp, _c_i64, C.c_int, C.c_int]),
     "b2_ridge_classifier_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
                                           C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_int), _vp,
                                           _vp, _vp]),
@@ -898,6 +903,65 @@ class Context:
                                     C.byref(found), C.byref(more))
         _check_args(rc, "b2_label_values")
         return vals[: found.value].copy(), bool(more.value)
+
+    # -- LogisticRegression, multinomial (DESIGN.md section 14) ----------------------------------------------------
+    @staticmethod
+    def _f64_classes_coef(coef, k: int, d: int, what: str = "coef") -> np.ndarray:
+        w = np.ascontiguousarray(coef, dtype=np.float64)
+        if w.shape != (k, d + 1):
+            raise ValueError(f"{what} must be ({k}, {d + 1}) (row k = [w_k, b_k]), got {w.shape}")
+        return w
+
+    def multinomial_pass(self, X, y, classes, coef, *, row_mask=None, mask_keep: int = 1, fit_intercept: bool = True,
+                         hessian: bool = True) -> dict:
+        """One pass of the Newton solver's statistics for HalfMultinomialLoss at coef ((K, d + 1), row k = [w_k, b_k])
+        over the kept rows (b2_multinomial_pass); ``classes`` are K (3..MAX_CLASSES) sorted fp32 values and a row's class
+        is the index of its y among them.  Returns a dict of unscaled sums: loss, kept, unmatched (kept rows of no class,
+        NaN included), nonfinite (kept rows with y not finite), correct (kept rows whose first largest eta is their
+        class), grad ((K, d + 1): sum g_k [x 1]) and hessian ((K, K, d + 1, d + 1) sum h_kl [x 1][x 1]^T, or None without
+        ``hessian``).  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        k = cl.size
+        w = self._f64_classes_coef(coef, k, d)
+        sums = np.empty(5 + k * (d + 1), dtype=np.float64)
+        hess = np.empty((k, k, d + 1, d + 1), dtype=np.float64) if hessian else None
+        rc = load().b2_multinomial_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data, k,
+                                        w.ctypes.data, int(bool(fit_intercept)), sums.ctypes.data,
+                                        hess.ctypes.data if hess is not None else None)
+        _check_args(rc, "b2_multinomial_pass")
+        out = {key: float(sums[i]) for i, key in enumerate(("loss", "kept", "unmatched", "nonfinite", "correct"))}
+        out["grad"] = sums[5:].reshape(k, d + 1).copy()
+        out["hessian"] = hess
+        return out
+
+    def multinomial_line_search(self, X, y, classes, coef, step, *, n_steps: int = GLM_STEPS, row_mask=None,
+                                mask_keep: int = 1) -> np.ndarray:
+        """The backtracking ladder of a multinomial Newton step in one pass (b2_multinomial_line_search): the summed
+        loss over the kept rows at coef + 2^-t step (both (K, d + 1)) for t < n_steps."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        w = self._f64_classes_coef(coef, cl.size, d)
+        s = self._f64_classes_coef(step, cl.size, d, "step")
+        out = np.empty(max(int(n_steps), 1), dtype=np.float64)
+        rc = load().b2_multinomial_line_search(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data,
+                                               cl.size, w.ctypes.data, s.ctypes.data, int(n_steps), out.ctypes.data)
+        _check_args(rc, "b2_multinomial_line_search")
+        return out
+
+    def softmax_rows(self, values) -> None:
+        """Each row of a 2-D float64 array (an f64 ``DeviceArray`` or a C-contiguous ndarray) replaced in place by its
+        softmax, as sklearn.utils.extmath.softmax computes it (b2_softmax_rows)."""
+        if isinstance(values, DeviceArray):
+            if values.kind != "f64" or len(values.shape) != 2:
+                raise RuntimeError("softmax_rows: values must be a 2-D f64 DeviceArray")
+            ptr, mk, (n, k) = values.ptr, MEM_DEVICE, values.shape
+        else:
+            if not isinstance(values, np.ndarray) or values.dtype != np.float64 or values.ndim != 2 \
+                    or not values.flags.c_contiguous:
+                raise RuntimeError("softmax_rows: host values must be a C-contiguous 2-D float64 ndarray")
+            ptr, mk, (n, k) = values.ctypes.data, MEM_HOST, values.shape
+        _check_args(load().b2_softmax_rows(self._h, ptr, int(n), int(k), mk), "b2_softmax_rows")
 
     # -- RidgeClassifierCV (DESIGN.md section 13) ------------------------------------------------------------------
     def ridge_classifier_loo(self, X, y, classes, alphas, row_mask=None, mask_keep: int = 1, *,

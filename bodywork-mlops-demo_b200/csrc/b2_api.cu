@@ -480,7 +480,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part,
-                  ctx->cls, ctx->loo_cls};
+                  ctx->cls, ctx->loo_cls, ctx->mn_op, ctx->mn_sum, ctx->mn_part};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1840,6 +1840,134 @@ int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* 
   }
   *n_values_out = found;
   *more_out = h[max_values] != ~0ull ? 1 : 0;
+  return B2_OK;
+}
+
+// ---- multinomial LogisticRegression (DESIGN.md section 14) ---------------------------------------------------------
+// The checks the multinomial entry points share, then the classes, coefficients and step (K x (d + 1) each, row k =
+// [w_k, b_k]; step may be null) into ctx->mn_op and room for the reduced sums of `mode` in ctx->mn_sum
+static int mn_setup(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                    int mem_kind, const float* classes, int n_classes, const double* coef, const double* step,
+                    int fit_intercept, int mode) {
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (coef == nullptr) { set_error("coef is null"); return B2_E_ARG; }
+  if (n_classes < 3 || n_classes > kMaxClasses) {
+    set_error("n_classes=%d out of range [3,%d] (two classes: b2_logistic_pass)", n_classes, kMaxClasses);
+    return B2_E_ARG;
+  }
+  if (int r = check_classes(classes, n_classes)) return r;
+  if (ctx->n_ranks > 1) {
+    set_error("the multinomial passes run on one rank only (their sums are not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (ctx->mn_op == nullptr) B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->mn_op), sizeof(double) * kMnOpDoubles));
+  const size_t sum = multinomial_sum_doubles(d, n_classes, mode);
+  if (sum > ctx->mn_sum_doubles) {
+    if (ctx->mn_sum != nullptr) cudaFree(ctx->mn_sum);
+    ctx->mn_sum = nullptr;
+    ctx->mn_sum_doubles = 0;
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->mn_sum), sizeof(double) * sum));
+    ctx->mn_sum_doubles = sum;
+  }
+  std::vector<double> op(kMnOpDoubles, 0.0);
+  for (int k = 0; k < n_classes; ++k) {
+    op[kMnClasses + k] = classes[k];
+    for (int j = 0; j <= d; ++j) {
+      const bool w = j < d || fit_intercept;   // the intercept column is zero without fit_intercept
+      op[kMnCoef + k * (kMaxD + 1) + j] = w ? coef[(size_t)k * (d + 1) + j] : 0.0;
+      if (step != nullptr) op[kMnStep + k * (kMaxD + 1) + j] = w ? step[(size_t)k * (d + 1) + j] : 0.0;
+    }
+  }
+  B2_CUDA(cudaMemcpyAsync(ctx->mn_op, op.data(), sizeof(double) * op.size(), cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
+  return B2_OK;
+}
+
+static int mn_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                   int mem_kind, const uint8_t* row_mask, int mask_keep, int mode, int n_classes, int n_steps) {
+  return row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+    return launch_multinomial(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, mode, n_classes, n_steps,
+                              s.first);
+  });
+}
+
+int b2_multinomial_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                        int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                        const double* coef, int fit_intercept, double* sums_out, double* hess_out) {
+  if (int r = use_device(ctx)) return r;
+  if (sums_out == nullptr) { set_error("sums_out is null"); return B2_E_ARG; }
+  const int mode = hess_out != nullptr ? kGlmHessian : kGlmGradient;
+  if (int r = mn_setup(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, classes, n_classes, coef, nullptr, fit_intercept,
+                       mode))
+    return r;
+  if (int r = mn_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, mode, n_classes, 0)) return r;
+  const int K = n_classes, d1 = d + 1, dp = (d1 + 15) & ~15;
+  std::vector<double> h(multinomial_sum_doubles(d, K, mode));
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->mn_sum, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, h.data(), sizeof(double) * 5);
+  memcpy(sums_out + 5, h.data() + kMnHead, sizeof(double) * K * d1);
+  if (hess_out != nullptr) {
+    // block (k, l) and block (l, k) are the same symmetric matrix: its upper triangle, mirrored
+    const double* blk = h.data() + kMnHead + (size_t)K * d1;
+    for (int k = 0, p = 0; k < K; ++k)
+      for (int l = k; l < K; ++l, ++p) {
+        const double* b = blk + (size_t)p * dp * dp;
+        double* hk = hess_out + ((size_t)k * K + l) * d1 * d1;
+        double* hl = hess_out + ((size_t)l * K + k) * d1 * d1;
+        for (int i = 0; i < d1; ++i)
+          for (int j = i; j < d1; ++j) {
+            const double v = b[(size_t)i * dp + j];
+            hk[(size_t)i * d1 + j] = hk[(size_t)j * d1 + i] = v;
+            hl[(size_t)i * d1 + j] = hl[(size_t)j * d1 + i] = v;
+          }
+      }
+  }
+  return B2_OK;
+}
+
+int b2_multinomial_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d,
+                               int64_t ldx, int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes,
+                               int n_classes, const double* coef, const double* step, int n_steps, double* loss_out) {
+  if (int r = use_device(ctx)) return r;
+  if (step == nullptr || loss_out == nullptr) { set_error("step / loss_out is null"); return B2_E_ARG; }
+  if (n_steps < 1 || n_steps > kGlmSteps) { set_error("n_steps=%d out of range [1,%d]", n_steps, kGlmSteps); return B2_E_ARG; }
+  if (int r = mn_setup(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, classes, n_classes, coef, step, 1, kGlmLadder))
+    return r;
+  if (int r = mn_rows(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, mask_keep, kGlmLadder, n_classes,
+                      n_steps))
+    return r;
+  B2_CUDA(cudaMemcpyAsync(loss_out, ctx->mn_sum, sizeof(double) * n_steps, cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B2_OK;
+}
+
+int b2_softmax_rows(b2_ctx* ctx, double* values, int64_t n_rows, int n_cols, int mem_kind) {
+  if (int r = use_device(ctx)) return r;
+  if (n_rows < 0 || n_cols < 1 || (n_rows > 0 && values == nullptr)) {
+    set_error("n_rows=%lld / n_cols=%d / values is null", (long long)n_rows, n_cols);
+    return B2_E_ARG;
+  }
+  if (mem_kind != B2_MEM_DEVICE && mem_kind != B2_MEM_HOST) { set_error("bad mem_kind %d", mem_kind); return B2_E_ARG; }
+  if (n_rows == 0) return B2_OK;
+  const size_t bytes = sizeof(double) * (size_t)n_rows * n_cols;
+  if (mem_kind == B2_MEM_DEVICE) {
+    if (int r = launch_softmax_rows(ctx, values, n_rows, n_cols)) return r;
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    return B2_OK;
+  }
+  double* dev = nullptr;                            // host values: one round trip through a temporary device copy
+  B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev), bytes));
+  int rc = B2_OK;
+  if (cudaMemcpyAsync(dev, values, bytes, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) rc = B2_E_CUDA;
+  if (rc == B2_OK) rc = launch_softmax_rows(ctx, dev, n_rows, n_cols);
+  if (rc == B2_OK && cudaMemcpyAsync(values, dev, bytes, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = B2_E_CUDA;
+  const cudaError_t done = cudaStreamSynchronize(ctx->stream);
+  cudaFree(dev);
+  if (rc == B2_E_CUDA) set_error("b2_softmax_rows: copying the host values failed");
+  if (rc != B2_OK) return rc;
+  B2_CUDA(done);
   return B2_OK;
 }
 

@@ -182,6 +182,18 @@ constexpr int kLcSum = kLcYbar + kMaxClasses;              // [2][kMaxAlphas] su
 constexpr int kLcPart = 2 * kMaxAlphas;
 constexpr int kLcDoubles = kLcSum + kLcPart;
 
+// ---- multinomial logistic regression (multinomial.cu; DESIGN.md section 14) ------------------------------------------
+// doubles of ctx->mn_op: the sorted classes, the coefficients [K][kMaxD + 1] (row k = [w_k, b_k]) and the step beside
+// them.  The reduced sums at ctx->mn_sum: the head [kMnHead] ([0] loss [1] kept [2] kept rows of no class [3] kept rows
+// with y not finite [4] rows whose first argmax of eta is their class; a line search leaves the loss at step t in [t]),
+// the gradient [K][d + 1], then (Hessian) the upper triangle of each class pair's block [P][dp][dp], dp = d + 1 padded
+// to 16, pairs k <= l in row-major order.  Per-CTA partials in ctx->mn_part, [slice][the same layout], grown lazily.
+constexpr int kMnHead = 32;
+constexpr int kMnClasses = 0;
+constexpr int kMnCoef = kMaxClasses;
+constexpr int kMnStep = kMnCoef + kMaxClasses * (kMaxD + 1);
+constexpr int kMnOpDoubles = kMnStep + kMaxClasses * (kMaxD + 1);
+
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
 // first and last row of every fold of fold ids in device memory: range[2 k] = n - first, range[2 k + 1] = last + 1
@@ -269,6 +281,13 @@ struct b2_ctx {
   double* cls = nullptr;
   // the classifier's leave-one-out operands and sums (b2::kLc*, 2.1 MB), allocated by the first call
   double* loo_cls = nullptr;
+  // multinomial logistic regression: the operands (b2::kMn*), the reduced sums and the per-CTA partials, each grown to the
+  // largest call
+  double* mn_op = nullptr;
+  double* mn_sum = nullptr;
+  size_t mn_sum_doubles = 0;
+  double* mn_part = nullptr;
+  size_t mn_part_doubles = 0;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -478,6 +497,14 @@ int launch_classify(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, i
 // launches after one memset)
 int launch_label_values(b2_ctx* ctx, const float* y, int64_t n, const uint8_t* mask, int keep, int max_values,
                         unsigned long long* st);
+// one pass of multinomial logistic regression over the rows [0, n) at the classes, coefficients and step of ctx->mn_op
+// (mode: GlmMode; kGlmLadder takes the n_steps losses), then one ordered reduce of every slice's partial into ctx->mn_sum
+// (`first_block` overwrites, otherwise adds); ctx->mn_sum must hold multinomial_sum_doubles(d, n_classes, mode)
+size_t multinomial_sum_doubles(int d, int n_classes, int mode);
+int launch_multinomial(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                       const uint8_t* mask, int keep, int mode, int n_classes, int n_steps, bool first_block);
+// sklearn.utils.extmath.softmax of each row of the device (n, k) fp64 array, in place (one launch)
+int launch_softmax_rows(b2_ctx* ctx, double* values, int64_t n, int k);
 // W and b of the ridge classifier from the resident S and the class sums at ctx->cls + kClsSums (one launch)
 int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes);
 int launch_p2p_allreduce(b2_ctx* ctx);

@@ -144,7 +144,7 @@ class _B200Estimator:
         """host rows as contiguous float32, device rows as they are; either must have ``n_features_in_`` columns."""
         X = X if isinstance(X, native.DeviceArray) else _as_f32_matrix(X)
         if X.shape[1] != self.n_features_in_:
-            raise ValueError(f"X has {X.shape[1]} features, but B200{self._sk_name} is expecting "
+            raise ValueError(f"X has {X.shape[1]} features, but {type(self).__name__} is expecting "
                              f"{self.n_features_in_} features as input.")
         return X
 
@@ -938,13 +938,13 @@ class _B200GLM(_B200Estimator):
         """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
         (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, n_iter_ and
         n_features_in_."""
-        _refuse_sample_weight(sample_weight, f"B200{self._sk_name}")
+        _refuse_sample_weight(sample_weight, type(self).__name__)
         model = self._check_params()
         with self._stage_targets(X, y, row_mask, mask_keep) as (X, y, row_mask, labels):
             d = X.shape[1]
             run, line_search = self._passes(X, y, row_mask, mask_keep, model, labels)
             coef, n_iter = self._newton(d, self._l2(labels), lambda: self._start(d, run, model, labels), run,
-                                        line_search)
+                                        line_search, **self._layout(d, labels))
         self._store(coef, n_iter, d, labels)
         return self
 
@@ -992,6 +992,10 @@ class _B200GLM(_B200Estimator):
     def _l2(self, labels) -> float:
         return float(self.alpha)
 
+    def _layout(self, d, labels) -> dict:
+        """the coefficient layout ``_newton`` takes beyond one row [w, b] (its defaults)"""
+        return {}
+
     def _store(self, coef, n_iter, d, labels) -> None:
         if self.fit_intercept:
             self.coef_, self.intercept_ = coef[:-1].copy(), np.float64(coef[-1])
@@ -1013,27 +1017,34 @@ class _B200GLM(_B200Estimator):
             coef = np.concatenate([coef, [float(np.ravel(self.intercept_)[0])]])
         return coef, True
 
-    def _newton(self, d, alpha, start, run, line_search):
+    def _newton(self, d, alpha, start, run, line_search, n_classes=1, free=None):
         """NewtonSolver.solve (NewtonCholeskySolver) step by step on the caller's passes: start() -> (coef, the pass
         with the Hessian at coef, the kept rows), run(coef, hessian) -> the pass sums at coef, line_search(coef, step)
-        -> the loss sums of the 21 ladder steps.  Returns (coef with the intercept last, n_iter)."""
+        -> the loss sums of the 21 ladder steps.  The coefficients are scikit-learn's: n_classes rows [w, b] raveled
+        with the classes of one feature contiguous (order "F"), so the weights come first; the pass's "grad" holds the
+        n_classes rows of sum g [x 1] and its "hessian" is in the same order.  free: None, or the coefficients the Newton
+        step solves for, the others held where they are (NewtonCholeskySolver's gauge of an overparametrised multinomial
+        fit).  Returns (coef, n_iter)."""
         import scipy.linalg
         import scipy.optimize
         from sklearn.exceptions import ConvergenceWarning
         from sklearn.utils.optimize import _check_optimize_result
         fi, tol, max_iter = bool(self.fit_intercept), float(self.tol), int(self.max_iter)
         n_dof = d + int(fi)
+        n_w = n_classes * d                       # the weights, before the intercepts
 
         def loss_of(c, loss_sum):                 # LinearModelLoss.loss: mean loss + alpha / 2 |w|^2
-            w = c[:d]
+            w = c[:n_w]
             return float(loss_sum / n) + float(0.5 * alpha * (w @ w))
 
         def grad_of(c, s):                        # LinearModelLoss.gradient
-            g = np.empty(n_dof)
-            g[:d] = s["grad"][:d] / n + alpha * c[:d]
+            G = np.reshape(s["grad"], (n_classes, -1))
+            W = np.reshape(c, (n_classes, n_dof), order="F")
+            g = np.empty((n_classes, n_dof))
+            g[:, :d] = G[:, :d] / n + alpha * W[:, :d]
             if fi:
-                g[d] = s["grad"][d] / n
-            return g
+                g[:, d] = G[:, d] / n
+            return g.ravel(order="F")
 
         coef, cur, n = start()
         loss_value = loss_of(coef, cur["loss"])
@@ -1053,12 +1064,23 @@ class _B200GLM(_B200Estimator):
                 break
             hessian = cur["hessian"] / n
             if not fi:
-                hessian = hessian[:d, :d].copy()
-            hessian[np.arange(d), np.arange(d)] += alpha
+                hessian = hessian[:n_w, :n_w].copy()
+            hessian[np.arange(n_w), np.arange(n_w)] += alpha
+            if free is None:
+                h_free, g_free = hessian, gradient
+            else:                                 # the held coefficients leave the gradient and the Hessian
+                held = np.setdiff1d(np.arange(gradient.size), free)
+                gradient[held] = 0
+                hessian[held, :] = 0
+                hessian[:, held] = 0
+                h_free, g_free = hessian[np.ix_(free, free)], gradient[free]
             try:
                 with warnings.catch_warnings():
                     warnings.simplefilter("error", scipy.linalg.LinAlgWarning)
-                    coef_newton = scipy.linalg.solve(hessian, -gradient, check_finite=False, assume_a="sym")
+                    coef_newton = scipy.linalg.solve(h_free, -g_free, check_finite=False, assume_a="sym")
+                    if free is not None:
+                        coef_newton, step_free = np.zeros(gradient.size), coef_newton
+                        coef_newton[free] = step_free
                     gradient_times_newton = gradient @ coef_newton
                     if gradient_times_newton > 0:
                         fallback = True
@@ -1274,17 +1296,17 @@ class B200LogisticRegression(_B200GLM):
 
     def _check_params(self):
         if self.solver != "newton-cholesky":
-            raise ValueError(f"solver={self.solver!r} is not supported: B200LogisticRegression runs scikit-learn's "
+            raise ValueError(f"solver={self.solver!r} is not supported: {type(self).__name__} runs scikit-learn's "
                              "'newton-cholesky' solver (L-BFGS-B runs only as its fallback)")
         C = self.C
         if isinstance(C, bool) or not isinstance(C, (int, float, np.integer, np.floating)) or not C > 0:
             raise ValueError(f"The 'C' parameter of LogisticRegression must be a float in the range (0.0, inf]. "
                              f"Got {C!r} instead.")
         if self.l1_ratio != 0:
-            raise ValueError(f"l1_ratio={self.l1_ratio!r} is not supported: B200LogisticRegression fits the L2 penalty "
+            raise ValueError(f"l1_ratio={self.l1_ratio!r} is not supported: {type(self).__name__} fits the L2 penalty "
                              "only (l1_ratio=0)")
         if self.class_weight is not None:
-            raise ValueError("class_weight is not supported by B200LogisticRegression: every kept row has weight 1")
+            raise ValueError(f"class_weight is not supported by {type(self).__name__}: every kept row has weight 1")
         if isinstance(self.max_iter, bool) or not isinstance(self.max_iter, (int, np.integer)) or self.max_iter < 0:
             raise ValueError(f"The 'max_iter' parameter of LogisticRegression must be an int in the range [0, inf). "
                              f"Got {self.max_iter!r} instead.")
@@ -1470,6 +1492,29 @@ def _class_index(classes: np.ndarray, y: np.ndarray) -> np.ndarray:
     return np.where(hit, idx, -1).astype(np.float32)
 
 
+def _kept_class_labels(y, row_mask, mask_keep, who: str, shape_message: str):
+    """(host y as 1-D, its kept rows) after scikit-learn's checks of classification targets on the kept rows;
+    ``shape_message``: the refusal of y with more than one column, formatted with its shape"""
+    from sklearn.utils.multiclass import check_classification_targets
+    y = np.asarray(y)
+    if y.ndim == 2 and y.shape[1] == 1:
+        y = y.ravel()
+    if y.ndim != 1:
+        raise ValueError(shape_message.format(y.shape))
+    if isinstance(row_mask, native.DeviceArray):
+        row_mask = row_mask.to_host()
+    kept = y if row_mask is None else y[np.asarray(row_mask).ravel() == mask_keep]
+    if kept.size == 0:
+        raise _too_few_rows((0,), by=who)
+    if kept.dtype.kind in "fc":
+        if np.isnan(kept).any():
+            raise ValueError("Input y contains NaN.")
+        if np.isinf(kept).any():
+            raise ValueError(f"Input y contains infinity or a value too large for {kept.dtype!r}.")
+    check_classification_targets(kept)
+    return y, kept
+
+
 class B200RidgeClassifier(_B200Estimator):
     """``sklearn.linear_model.RidgeClassifier`` fitted on the H100: the ridge regression of LabelBinarizer's +-1 targets
     (one target for two classes, one per class for more) from the fp64 Gram of [x 1] (the Gram dispatch every fit uses),
@@ -1523,24 +1568,9 @@ class B200RidgeClassifier(_B200Estimator):
     def _host_labels(y, row_mask, mask_keep):
         """(classes_, y as float32 class indices (-1 for rows not kept whose label is no class), kept rows) of host y,
         with scikit-learn's checks on the kept rows"""
-        from sklearn.utils.multiclass import check_classification_targets
-        y = np.asarray(y)
-        if y.ndim == 2 and y.shape[1] == 1:
-            y = y.ravel()
-        if y.ndim != 1:
-            raise ValueError(f"multilabel y (shape {y.shape}) is not supported by B200RidgeClassifier: y must hold one "
-                             "label per row")
-        if isinstance(row_mask, native.DeviceArray):
-            row_mask = row_mask.to_host()
-        kept = y if row_mask is None else y[np.asarray(row_mask).ravel() == mask_keep]
-        if kept.size == 0:
-            raise _too_few_rows((0,), by="B200RidgeClassifier")
-        if kept.dtype.kind in "fc":
-            if np.isnan(kept).any():
-                raise ValueError("Input y contains NaN.")
-            if np.isinf(kept).any():
-                raise ValueError(f"Input y contains infinity or a value too large for {kept.dtype!r}.")
-        check_classification_targets(kept)
+        y, kept = _kept_class_labels(y, row_mask, mask_keep, "B200RidgeClassifier",
+                                     "multilabel y (shape {}) is not supported by B200RidgeClassifier: y must hold one "
+                                     "label per row")
         classes = np.unique(kept)
         B200RidgeClassifier._check_class_count(classes, classes.size > native.MAX_CLASSES)
         return classes, _class_index(classes, y)
@@ -1822,3 +1852,208 @@ class B200RidgeClassifierCV(B200RidgeClassifier):
 
     def __repr__(self) -> str:
         return f"B200RidgeClassifierCV(alphas={self.alphas!r})"
+
+
+# ---- LogisticRegression, multinomial: Newton fits with the class-pair Hessian blocks on the GPU (DESIGN.md section 14) --
+class B200MultinomialLogisticRegression(B200LogisticRegression):
+    """``sklearn.linear_model.LogisticRegression(solver="newton-cholesky")`` for 2 to ``native.MAX_CLASSES`` classes,
+    fitted on the H100.  Three or more classes fit the multinomial loss (HalfMultinomialLoss) with ``_B200GLM._newton``:
+    each iteration is one pass for the loss, the K x (D + 1) gradient and the K (K + 1) / 2 class-pair blocks of the fp64
+    Hessian (``multinomial_pass``) and one pass for the 21 line-search steps (``multinomial_line_search``), from zeros (or
+    the last fit with warm_start), with the L2 strength 1 / (C n) on the weights only and NewtonCholeskySolver's gauge:
+    at C = inf the last class is held at zero, with an intercept at C < inf its intercept; the result is centred over
+    the classes.  Two classes run ``B200LogisticRegression``'s binary fit, as scikit-learn does.
+
+    Labels: host y of any dtype (``classes_`` is ``np.unique`` over the kept rows; y is staged as float32 class indices),
+    or an f32 ``DeviceArray`` beside device rows (``classes_`` are its distinct fp32 values, found on the device).
+    Refused: one class, more than ``native.MAX_CLASSES`` classes, continuous or non-finite y, l1_ratio != 0,
+    class_weight, sample_weight and any solver but 'newton-cholesky'.  verbose is accepted and has no effect."""
+
+    @staticmethod
+    def _host_labels(y, row_mask, mask_keep):
+        """(classes_, y as float32 class indices (-1 for rows not kept whose label is no class), kept rows) of host y"""
+        y, kept = _kept_class_labels(y, row_mask, mask_keep, "B200MultinomialLogisticRegression",
+                                     "y should be a 1d array, got an array of shape {} instead.")
+        classes = np.unique(kept)
+        if classes.size < 2:
+            raise ValueError(_one_class_message(classes[0]))
+        if classes.size > native.MAX_CLASSES:
+            raise ValueError(f"B200MultinomialLogisticRegression fits at most {native.MAX_CLASSES} classes, y has "
+                             f"{classes.size}")
+        return classes, _class_index(classes, y), int(kept.size)
+
+    @staticmethod
+    def _device_labels(ctx, y, row_mask, mask_keep):
+        """(classes_ (fp32), kept rows) of an f32 DeviceArray y: one label scan and one label discovery on the device"""
+        st = ctx.label_scan(y, row_mask, mask_keep)
+        if st["kept"] == 0:
+            raise _too_few_rows((0,), by="B200MultinomialLogisticRegression")
+        if st["nonfinite"] > 0:
+            raise ValueError("Input y contains NaN or infinity.")
+        if st["nonintegral"] > 0:
+            raise ValueError(_CONTINUOUS_MESSAGE)
+        if st["min"] == st["max"]:
+            raise ValueError(_one_class_message(np.float32(st["min"])))
+        values, more = ctx.label_values(y, row_mask, mask_keep, native.MAX_CLASSES)
+        if more:
+            raise ValueError(f"B200MultinomialLogisticRegression fits at most {native.MAX_CLASSES} classes, y has more")
+        return values, int(st["kept"])
+
+    # -- the hooks of _B200GLM.fit; labels: (classes_, kept rows, the K fp32 labels y holds), as the binary fit's for K = 2
+    @contextlib.contextmanager
+    def _stage_targets(self, X, y, row_mask, mask_keep, fitting: bool = True):
+        """(X, y, row_mask, labels) for the passes, for the body of the ``with``; ``fit`` and ``score`` share it.  Device
+        y (device rows only) is read as stored against the fp32 classes; host y becomes float32 indices into classes_
+        (-1 outside them), uploaded beside device rows or staged with host rows.  Scoring leaves classes_ and the kept
+        rows None."""
+        ctx = self.ctx
+        if isinstance(y, native.DeviceArray):
+            if not isinstance(X, native.DeviceArray):
+                raise ValueError("device y needs device rows: X must be a DeviceArray too")
+            classes, n = self._device_labels(ctx, y, row_mask, mask_keep) if fitting else (self.classes_, None)
+            values = tuple(float(c) for c in B200RidgeClassifier._fp32_classes(classes))
+            yield X, y, row_mask, (classes if fitting else None, n) + values
+            return
+        if fitting:
+            classes, yk, n = self._host_labels(y, row_mask, mask_keep)
+        else:                                     # class by class: labels of any type, outside classes_ too
+            classes, n = self.classes_, None
+            yh = np.asarray(y).ravel()
+            yk = np.full(yh.shape, -1.0, dtype=np.float32)
+            for k, c in enumerate(classes):
+                yk[yh == c] = k
+        labels = (classes if fitting else None, n) + tuple(float(k) for k in range(classes.size))
+        if isinstance(X, native.DeviceArray):
+            with _on_device(ctx, yk) as yd:
+                yield X, yd, row_mask, labels
+        else:
+            with _stage_rows(ctx, X, yk, row_mask) as (X, yd, row_mask):
+                yield X, yd, row_mask, labels
+
+    def _passes(self, X, y, row_mask, mask_keep, model, labels):
+        if len(labels) == 4:
+            return super()._passes(X, y, row_mask, mask_keep, model, labels)
+        ctx, fi, d = self.ctx, bool(self.fit_intercept), X.shape[1]
+        k, n_dof = len(labels) - 2, d + int(fi)
+        classes = np.array(labels[2:], dtype=np.float32)
+
+        def rows(c):                              # the raveled coefficients as the pass's rows [w_k, b_k]
+            full = np.zeros((k, d + 1))
+            full[:, :n_dof] = np.reshape(c, (k, n_dof), order="F")
+            return full
+
+        def run(c, hessian):
+            s = ctx.multinomial_pass(X, y, classes, rows(c), row_mask=row_mask, mask_keep=mask_keep,
+                                     fit_intercept=fi, hessian=hessian)
+            if hessian:                           # blocks [k][l][i][j] -> scikit-learn's order, (i, k) x (j, l)
+                s["hessian"] = s["hessian"].transpose(2, 0, 3, 1).reshape(k * (d + 1), k * (d + 1))
+            s["h_nonpos"] = 0.0                   # the multinomial pointwise Hessian is never negative
+            return s
+
+        def line_search(c, step):
+            return ctx.multinomial_line_search(X, y, classes, rows(c), rows(step), n_steps=native.GLM_STEPS,
+                                               row_mask=row_mask, mask_keep=mask_keep)
+        return run, line_search
+
+    def _start(self, d, run, model, labels):
+        """the start (zeros, or the last fit with warm_start) in NewtonCholeskySolver's gauge, then its Hessian pass"""
+        if len(labels) == 4:
+            return super()._start(d, run, model, labels)
+        fi, k, n = bool(self.fit_intercept), len(labels) - 2, labels[1]
+        coef = np.zeros((k, d + int(fi)))
+        if self.warm_start and getattr(self, "coef_", None) is not None:
+            prev = np.asarray(self.coef_, dtype=np.float64)
+            if prev.shape != (k, d):
+                raise ValueError(f"the warm start coef_ has shape {prev.shape}, ({k}, {d}) expected")
+            coef[:, :d] = prev
+            if fi:
+                coef[:, d] = np.asarray(self.intercept_, dtype=np.float64)
+        if self._l2(labels) == 0:
+            coef -= coef[-1, :]
+        elif fi:
+            coef[:, -1] -= coef[-1, -1]
+        coef = coef.ravel(order="F")
+        first = run(coef, True)
+        if first["kept"] != n or first["unmatched"] > 0 or first["nonfinite"] > 0:
+            raise RuntimeError("the multinomial pass saw other labels than the label check")
+        _check_finite(first["loss"], first["grad"])
+        return coef, first, n
+
+    def _layout(self, d, labels) -> dict:
+        k = len(labels) - 2
+        if k == 2:
+            return {}
+        size = k * (d + int(bool(self.fit_intercept)))
+        if self._l2(labels) == 0:                 # the last class held at zero
+            free = np.flatnonzero(np.arange(size) % k != k - 1)
+        elif self.fit_intercept:                  # the last intercept held at zero
+            free = np.arange(size - 1)
+        else:
+            free = None
+        return dict(n_classes=k, free=free)
+
+    def _store(self, coef, n_iter, d, labels) -> None:
+        if len(labels) == 4:
+            return super()._store(coef, n_iter, d, labels)
+        fi, k = bool(self.fit_intercept), len(labels) - 2
+        w = np.reshape(coef, (k, d + int(fi)), order="F").copy()
+        if self._l2(labels) == 0:                 # NewtonCholeskySolver.finalize: the symmetric parametrisation
+            w -= np.mean(w, axis=0)
+        elif fi:
+            w[:, -1] -= np.mean(w[:, -1])
+        self.coef_ = w[:, :d].copy()
+        self.intercept_ = w[:, d].copy() if fi else np.zeros(k)
+        self.classes_ = labels[0]
+        self.n_iter_ = np.array([n_iter], dtype=np.int32)
+        self.n_features_in_ = int(d)
+
+    # -- predictions: two classes as the binary estimator, more through one classify pass ------------------------------
+    def _classify(self, X, **want):
+        X = self._checked_rows(X)
+        labels = B200RidgeClassifier._fp32_classes(self.classes_) if isinstance(X, native.DeviceArray) else \
+            np.arange(self.classes_.size, dtype=np.float32)
+        return self.ctx.classify(X, self.coef_, self.intercept_, labels, **want)
+
+    def decision_function(self, X):
+        """X coef_^T + intercept_ in fp64: (n,) for two classes, (n, K) for more; float64 for host rows, an f64
+        ``DeviceArray`` for device rows."""
+        if self.classes_.size == 2:
+            return super().decision_function(X)
+        return self._classify(X, decision=True)["decision"]
+
+    def predict_proba(self, X):
+        """The class probabilities, (n, K) fp64: scikit-learn's softmax of the decision for host rows; for device rows
+        an f64 ``DeviceArray``, the decision turned into probabilities in place on the device."""
+        if self.classes_.size == 2:
+            return super().predict_proba(X)
+        from sklearn.utils.extmath import softmax
+        dec = self.decision_function(X)
+        if isinstance(dec, native.DeviceArray):
+            self.ctx.softmax_rows(dec)
+            return dec
+        return softmax(dec, copy=False)
+
+    def predict(self, X):
+        """classes_ of the first largest decision: an ndarray of classes_' dtype for host rows, an f32 ``DeviceArray``
+        for device rows (classes_ must then be fp32 values)."""
+        if self.classes_.size == 2:
+            return super().predict(X)
+        labels = self._classify(X, label=True)["label"]
+        if isinstance(labels, native.DeviceArray):
+            return labels
+        return self.classes_[labels.astype(np.intp)]
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """Accuracy over the kept rows (labels outside classes_ count as wrong): the counts of one pass."""
+        if self.classes_.size == 2:
+            return super().score(X, y, row_mask, mask_keep)
+        ctx = self.ctx
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=False) as (X, y, row_mask, labels):
+            s = ctx.classify(self._checked_rows(X), self.coef_, self.intercept_, np.array(labels[2:], np.float32), y,
+                             row_mask=row_mask, mask_keep=mask_keep)
+        if s["kept"] == 0:
+            raise _too_few_rows((0,))
+        return float(s["correct"] / s["kept"])
+
+    def __repr__(self) -> str:
+        return f"B200MultinomialLogisticRegression(C={self.C})"

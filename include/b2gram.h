@@ -395,6 +395,35 @@ int b2_classify(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t
 int b2_label_values(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* row_mask, int mask_keep, int max_values,
                     float* values_out, int* n_values_out, int* more_out);
 
+/* ---- LogisticRegression, multinomial (DESIGN.md section 14) -------------------------------------------------------
+ * The row passes of scikit-learn's Newton solver for HalfMultinomialLoss with 3..B2_MAX_CLASSES classes.  Per kept row,
+ * z = [x 1] and eta_k = z.coef_k in fp64 (x converted exactly), the softmax p_k = exp(eta_k - m) / s with m = max_k eta_k
+ * and s the sum of the exponentials, the loss log(s) + m - eta_y and g_k = p_k - [y = k].  classes and y as
+ * b2_class_sums (a row's class is the index of its fp32 y among the classes).  coef (host): n_classes x (d + 1) doubles,
+ * row k = [w_k, b_k].  Sums in a fixed order: repeated calls are bit-identical.  B2_E_ARG: bad shapes, n_classes outside
+ * 3..B2_MAX_CLASSES, classes that are not finite and strictly ascending, null outputs, n_steps outside 1..21;
+ * B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or no kept row) is no error: every sum is 0. */
+/* b2_multinomial_pass: sums_out (host, 5 + n_classes (d + 1) doubles): [0] sum loss [1] kept rows [2] kept rows whose y
+ * is no class (NaN included; their loss lacks the -eta_y term and their g the -1) [3] kept rows with y not finite [4] kept
+ * rows whose first largest eta_k is their class, then G[k][j] = sum g_k z_j at 5 + k (d + 1) + j.  hess_out: NULL (no
+ * Hessian), or (host) n_classes x n_classes x (d + 1) x (d + 1) doubles, block (k, l) = sum h_kl z z^T with h_kk =
+ * p_k (1 - p_k) and h_kl = -p_k p_l (symmetric, and block (l, k) equals block (k, l)).  Without fit_intercept the
+ * intercepts of coef are read as 0; the intercept column of the sums is always present.  One fp64 tensor-core CTA per
+ * class pair and row slice. */
+int b2_multinomial_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                        int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                        const double* coef, int fit_intercept, double* sums_out, double* hess_out);
+/* b2_multinomial_line_search: loss_out[t] = sum over kept rows of the loss at eta + 2^-t z.step_k, t < n_steps (1..21);
+ * step (host) as coef. */
+int b2_multinomial_line_search(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d,
+                               int64_t ldx, int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes,
+                               int n_classes, const double* coef, const double* step, int n_steps, double* loss_out);
+/* b2_softmax_rows: each row of the n_rows x n_cols fp64 array `values` (where mem_kind says) replaced by its softmax in
+ * place, by the steps of sklearn.utils.extmath.softmax: v - max, exp, then / the sum (in column order, where numpy sums
+ * 8-way unrolled and pairwise, so the two may differ by rounding).  Host values make
+ * one round trip through a temporary device copy. */
+int b2_softmax_rows(b2_ctx* ctx, double* values, int64_t n_rows, int n_cols, int mem_kind);
+
 /* ---- RidgeClassifierCV: replaces sklearn.linear_model.RidgeClassifierCV(alphas).fit with cv=None (DESIGN.md
  * section 13) ---------------------------------------------------------------------------------------------------------
  * The leave-one-out error of every class target and alpha: the Gram of the kept rows, b2_class_sums at its column means,
