@@ -27,6 +27,7 @@ MAX_D = 128
 MAX_ALPHAS = 64
 GLM_LOG, GLM_IDENTITY = 0, 1
 GLM_STEPS = 21
+SVM_SQUARED_HINGE, SVM_SQUARED_EPSILON = 0, 1
 MAX_CLASSES = 32
 LOO_SQUARED, LOO_ACCURACY = 0, 1
 
@@ -110,6 +111,8 @@ _SIGNATURES = {
     "b2_multinomial_line_search": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int,
                                              _vp, C.c_int, _vp, _vp, C.c_int, _vp]),
     "b2_softmax_rows": (C.c_int, [_vp, _vp, _c_i64, C.c_int, C.c_int]),
+    "b2_svm_pass": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, C.c_int,
+                              C.c_double, _vp, C.c_double, _vp, C.c_double, C.c_int, _vp, _vp]),
     "b2_ridge_classifier_loo": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
                                           C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_int), _vp,
                                           _vp, _vp]),
@@ -962,6 +965,33 @@ class Context:
                 raise RuntimeError("softmax_rows: host values must be a C-contiguous 2-D float64 ndarray")
             ptr, mk, (n, k) = values.ctypes.data, MEM_HOST, values.shape
         _check_args(load().b2_softmax_rows(self._h, ptr, int(n), int(k), mk), "b2_softmax_rows")
+
+    # -- LinearSVC / LinearSVR (DESIGN.md section 15) ----------------------------------------------------------------
+    def svm_pass(self, X, y, coef, intercept: float, *, loss: int = SVM_SQUARED_HINGE, param: float = 1.0,
+                 coef_from=None, intercept_from: float = 0.0, row_mask=None, mask_keep: int = 1,
+                 fit_intercept: bool = True, hessian: bool = True) -> dict:
+        """One pass of liblinear's TRON statistics at the trial point (coef, intercept) over the kept rows (b2_svm_pass),
+        ``param`` the positive label (SVM_SQUARED_HINGE) or epsilon (SVM_SQUARED_EPSILON).  Returns a dict of unscaled
+        sums over the rows active at the trial point: loss, kept, active, entering and leaving (the rows that joined or
+        left the active set since (coef_from, intercept_from); coef_from None: the empty set), positive (kept rows with
+        y == param, squared hinge), y_nonfinite (floats), grad ((d + 1,): sum g [x 1]) and dhessian ((d + 1, d + 1)
+        sum (active - active_from) [x 1][x 1]^T, or None without ``hessian``).  Raises ``ValueError`` for bad
+        arguments."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        w = self._f64_coef(coef, d)
+        wf = None if coef_from is None else self._f64_coef(coef_from, d)
+        sums = np.empty(d + 8, dtype=np.float64)
+        dh = np.empty((d + 1, d + 1), dtype=np.float64) if hessian else None
+        rc = load().b2_svm_pass(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), int(loss), float(param),
+                                wf.ctypes.data if wf is not None else None, float(intercept_from), w.ctypes.data,
+                                float(intercept), int(bool(fit_intercept)), sums.ctypes.data,
+                                dh.ctypes.data if dh is not None else None)
+        _check_args(rc, "b2_svm_pass")
+        keys = ("loss", "kept", "active", "entering", "leaving", "positive", "y_nonfinite")
+        out = {k: float(sums[i]) for i, k in enumerate(keys)}
+        out["grad"] = sums[7:].copy()
+        out["dhessian"] = dh
+        return out
 
     # -- RidgeClassifierCV (DESIGN.md section 13) ------------------------------------------------------------------
     def ridge_classifier_loo(self, X, y, classes, alphas, row_mask=None, mask_keep: int = 1, *,

@@ -1971,6 +1971,38 @@ int b2_softmax_rows(b2_ctx* ctx, double* values, int64_t n_rows, int n_cols, int
   return B2_OK;
 }
 
+// ---- LinearSVC / LinearSVR (DESIGN.md section 15) -------------------------------------------------------------------
+// The operands go where the GLM passes keep theirs: the trial point as (w, b), the accepted point as (step, db), then
+// 1 when there is an accepted point and the positive label (or eps) in the two label slots.
+int b2_svm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, int loss, double pos_label_or_epsilon,
+                const double* coef_from, double intercept_from, const double* coef, double intercept, int fit_intercept,
+                double* sums_out, double* dhess_out) {
+  if (int r = use_device(ctx)) return r;
+  if (sums_out == nullptr) { set_error("sums_out is null"); return B2_E_ARG; }
+  if (loss != B2_SVM_SQUARED_HINGE && loss != B2_SVM_SQUARED_EPSILON) {
+    set_error("loss=%d must be B2_SVM_SQUARED_HINGE or B2_SVM_SQUARED_EPSILON", loss);
+    return B2_E_ARG;
+  }
+  const double p = pos_label_or_epsilon;
+  if (!isfinite(p) || (loss == B2_SVM_SQUARED_EPSILON && p < 0.0)) {
+    set_error(loss == B2_SVM_SQUARED_HINGE ? "pos_label=%g must be finite" : "epsilon=%g must be finite and >= 0", p);
+    return B2_E_ARG;
+  }
+  const std::vector<double> zero(kMaxD, 0.0);
+  const bool has_from = coef_from != nullptr;
+  if (int r = glm_operands(ctx, x_dtype, n_rows, d, ldx, mem_kind, X, y, true, coef, fit_intercept ? intercept : 0.0,
+                           has_from ? coef_from : zero.data(), (has_from && fit_intercept) ? intercept_from : 0.0,
+                           has_from ? 1.0 : 0.0, p))
+    return r;
+  const bool hess = dhess_out != nullptr;
+  if (int r = row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+        return launch_svm(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, loss, hess, s.first);
+      }))
+    return r;
+  return fetch_glm_sums(ctx, d, 0, sums_out, dhess_out);
+}
+
 // ---- RidgeClassifierCV (DESIGN.md section 13) -----------------------------------------------------------------------
 // Host rows with cv_out stream in blocks whose cv block stays within the 262 144 x 64 doubles of b2_ridge_loo's widest
 constexpr size_t kLooOutBlockBytes = ((size_t)1 << 18) * kMaxAlphas * sizeof(double);

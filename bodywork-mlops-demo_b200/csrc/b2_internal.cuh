@@ -505,6 +505,11 @@ int launch_multinomial(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d
                        const uint8_t* mask, int keep, int mode, int n_classes, int n_steps, bool first_block);
 // sklearn.utils.extmath.softmax of each row of the device (n, k) fp64 array, in place (one launch)
 int launch_softmax_rows(b2_ctx* ctx, double* values, int64_t n, int k);
+// one pass of the linear SVMs (svm.cu) over the rows [0, n) at the operands of ctx->glm (loss: B2_SVM_*; hess: the
+// Hessian change too), then the ordered reduce into ctx->glm in the GLM passes' layout (`first_block` overwrites,
+// otherwise adds)
+int launch_svm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+               const uint8_t* mask, int keep, int loss, bool hess, bool first_block);
 // W and b of the ridge classifier from the resident S and the class sums at ctx->cls + kClsSums (one launch)
 int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes);
 int launch_p2p_allreduce(b2_ctx* ctx);

@@ -131,9 +131,9 @@ def _on_device(ctx: native.Context, host: np.ndarray):
 
 class _B200Estimator:
     """What every estimator shares: its context, the width check of the rows it predicts on, the linear ``predict``
-    and the export to scikit-learn.  ``_sk_name``: the scikit-learn class restated; ``_sk_attrs``: the fitted
-    attributes ``to_sklearn`` copies onto it."""
-    _sk_name = ""
+    and the export to scikit-learn.  ``_sk_name``: the scikit-learn class restated (in ``sklearn._sk_module``);
+    ``_sk_attrs``: the fitted attributes ``to_sklearn`` copies onto it."""
+    _sk_module, _sk_name = "linear_model", ""
     _sk_attrs: tuple = ()
 
     @property
@@ -161,8 +161,8 @@ class _B200Estimator:
     def to_sklearn(self):
         """A real scikit-learn estimator with the attributes ``fit`` would have set (joblib-dumpable; its own
         ``predict`` works)."""
-        from sklearn import linear_model
-        reg = getattr(linear_model, self._sk_name)(**self._sk_params())
+        import importlib
+        reg = getattr(importlib.import_module(f"sklearn.{self._sk_module}"), self._sk_name)(**self._sk_params())
         self._sk_prepare(reg)
         for name in self._sk_attrs:
             v = getattr(self, name)
@@ -1527,7 +1527,7 @@ class B200RidgeClassifier(_B200Estimator):
     Refused: one class, continuous or non-finite y, multilabel (2-D) y, more than ``native.MAX_CLASSES`` classes,
     class_weight, sample_weight, positive=True, solvers other than 'auto' / 'cholesky' and an array alpha.  copy_X,
     max_iter, tol and random_state are accepted and have no effect."""
-    _sk_name = "RidgeClassifier"
+    _sk_name, _label_who = "RidgeClassifier", "B200RidgeClassifier"   # _label_who: the name the label refusals give
     _sk_attrs = ("coef_", "intercept_", "classes_", "n_features_in_", "solver_", "n_iter_")
 
     def __init__(self, alpha: float = 1.0, *, fit_intercept: bool = True, copy_X: bool = True, max_iter=None,
@@ -1564,36 +1564,36 @@ class B200RidgeClassifier(_B200Estimator):
             raise ValueError("class_weight is not supported by B200RidgeClassifier: every kept row has weight 1")
         return float(a)
 
-    @staticmethod
-    def _host_labels(y, row_mask, mask_keep):
+    @classmethod
+    def _host_labels(cls, y, row_mask, mask_keep):
         """(classes_, y as float32 class indices (-1 for rows not kept whose label is no class), kept rows) of host y,
         with scikit-learn's checks on the kept rows"""
-        y, kept = _kept_class_labels(y, row_mask, mask_keep, "B200RidgeClassifier",
-                                     "multilabel y (shape {}) is not supported by B200RidgeClassifier: y must hold one "
+        y, kept = _kept_class_labels(y, row_mask, mask_keep, cls._label_who,
+                                     f"multilabel y (shape {{}}) is not supported by {cls._label_who}: y must hold one "
                                      "label per row")
         classes = np.unique(kept)
-        B200RidgeClassifier._check_class_count(classes, classes.size > native.MAX_CLASSES)
+        cls._check_class_count(classes, classes.size > native.MAX_CLASSES)
         return classes, _class_index(classes, y)
 
-    @staticmethod
-    def _check_class_count(classes, more: bool) -> None:
+    @classmethod
+    def _check_class_count(cls, classes, more: bool) -> None:
         if more:
-            raise ValueError(f"B200RidgeClassifier fits at most {native.MAX_CLASSES} classes, y has more")
+            raise ValueError(f"{cls._label_who} fits at most {native.MAX_CLASSES} classes, y has more")
         if classes.size < 2:
-            raise ValueError(f"B200RidgeClassifier needs samples of at least 2 classes, y holds only one: {classes[0]!r}")
+            raise ValueError(f"{cls._label_who} needs samples of at least 2 classes, y holds only one: {classes[0]!r}")
 
-    @staticmethod
-    def _device_labels(ctx, y, row_mask, mask_keep):
+    @classmethod
+    def _device_labels(cls, ctx, y, row_mask, mask_keep):
         """classes_ (fp32) of an f32 DeviceArray y: one label scan and one label discovery on the device"""
         st = ctx.label_scan(y, row_mask, mask_keep)
         if st["kept"] == 0:
-            raise _too_few_rows((0,), by="B200RidgeClassifier")
+            raise _too_few_rows((0,), by=cls._label_who)
         if st["nonfinite"] > 0:
             raise ValueError("Input y contains NaN or infinity.")
         if st["nonintegral"] > 0:
             raise ValueError(_CONTINUOUS_MESSAGE)
         values, more = ctx.label_values(y, row_mask, mask_keep, native.MAX_CLASSES)
-        B200RidgeClassifier._check_class_count(values, more)
+        cls._check_class_count(values, more)
         return values
 
     @contextlib.contextmanager
@@ -2057,3 +2057,376 @@ class B200MultinomialLogisticRegression(B200LogisticRegression):
 
     def __repr__(self) -> str:
         return f"B200MultinomialLogisticRegression(C={self.C})"
+
+
+# ---- LinearSVC / LinearSVR: liblinear's primal trust-region Newton fits (DESIGN.md section 15) -----------------------
+_LIBLINEAR_CONV = "Liblinear failed to converge, increase the number of iterations."
+
+
+def _tron(prob, f, g, eps: float, max_iter: int):
+    """``TRON::tron`` of liblinear (sklearn/svm/src/liblinear/tron.cpp) line by line, from w = 0 with f and g there:
+    ``prob.trial(w_new)`` is fun(w_new), ``prob.accept()`` takes the trial point and is grad(w), ``prob.hv(v)`` is Hv.
+    Returns (w, n_iter) with n_iter = --iter, as liblinear counts it."""
+    eta0, eta1, eta2 = 1e-4, 0.25, 0.75
+    sigma1, sigma2, sigma3 = 0.25, 0.5, 4.0
+    w = np.zeros(g.size)
+    delta = float(np.linalg.norm(g))
+    gnorm1 = delta
+    search = not delta <= eps * gnorm1
+    it = 1
+    while it <= max_iter and search:
+        s, r = _trcg(prob.hv, delta, g)
+        w_new = w + s
+        gs = float(g @ s)
+        prered = -0.5 * (gs - float(s @ r))
+        fnew = prob.trial(w_new)
+        actred = f - fnew
+        snorm = float(np.linalg.norm(s))
+        if it == 1:
+            delta = min(delta, snorm)
+        if fnew - f - gs <= 0:
+            alpha = sigma3
+        else:
+            alpha = max(sigma1, -0.5 * (gs / (fnew - f - gs)))
+        if actred < eta0 * prered:
+            delta = min(max(alpha, sigma1) * snorm, sigma2 * delta)
+        elif actred < eta1 * prered:
+            delta = max(sigma1 * delta, min(alpha * snorm, sigma2 * delta))
+        elif actred < eta2 * prered:
+            delta = max(sigma1 * delta, min(alpha * snorm, sigma3 * delta))
+        else:
+            delta = max(delta, min(alpha * snorm, sigma3 * delta))
+        if actred > eta0 * prered:
+            it += 1
+            w, f = w_new, fnew
+            g = prob.accept()
+            if np.linalg.norm(g) <= eps * gnorm1:
+                break
+        if f < -1.0e32:
+            break
+        if abs(actred) <= 0 and prered <= 0:
+            break
+        if abs(actred) <= 1.0e-12 * abs(f) and abs(prered) <= 1.0e-12 * abs(f):
+            break
+    return w, it - 1
+
+
+def _trcg(hv, delta: float, g):
+    """``TRON::trcg``: conjugate gradients on H s = -g inside the trust region of radius delta; returns (s, r)"""
+    s = np.zeros(g.size)
+    r = -g
+    d = r.copy()
+    cgtol = 0.1 * np.linalg.norm(g)
+    rTr = float(r @ r)
+    while np.linalg.norm(r) > cgtol:
+        Hd = hv(d)
+        alpha = rTr / float(d @ Hd)
+        s += alpha * d
+        if np.linalg.norm(s) > delta:            # back to the boundary of the trust region
+            s -= alpha * d
+            std, sts, dtd, dsq = float(s @ d), float(s @ s), float(d @ d), delta * delta
+            rad = np.sqrt(std * std + dtd * (dsq - sts))
+            alpha = (dsq - sts) / (std + rad) if std >= 0 else (rad - std) / dtd
+            s += alpha * d
+            r -= alpha * Hd
+            break
+        r -= alpha * Hd
+        rnewTrnew = float(r @ r)
+        d = d * (rnewTrnew / rTr) + r
+        rTr = rnewTrnew
+    return s, r
+
+
+class _SvmProblem:
+    """liblinear's l2r_l2_svc_fun / l2r_l2_svr_fun on GPU passes.  w = [coef, w_b] with w_b the weight of the bias
+    feature of value ``scale`` (intercept_scaling; absent without an intercept); f(w) = w.w / 2 + C sum loss, g = w +
+    2 C sum g z, H = I + 2 C sum z z^T over the active rows.  H's sum is carried from pass to pass: each pass at
+    (accepted w, trial w) returns the change over the rows that crossed, kept when the step is accepted.
+    ``run(w_from, w_to, hessian)`` is one ``svm_pass`` (w_from None: the empty active set)."""
+
+    def __init__(self, run, C: float, d: int, fit_intercept: bool, scale: float):
+        self.run, self.C, self.d, self.fi, self.scale = run, C, d, fit_intercept, scale
+        self.n = d + int(fit_intercept)
+        self.w = self.pending = self.H = None
+
+    def _fg(self, w, res):
+        G = res["grad"][: self.n].copy()
+        if self.fi:
+            G[self.d] *= self.scale
+        return 0.5 * float(w @ w) + self.C * res["loss"], w + 2.0 * self.C * G
+
+    def start(self, gram=None):
+        """(f, g, the pass) at w = 0; the Hessian sum from this pass, or ``gram`` (the sum over every kept row, which
+        is the active set at 0 of the squared hinge) with a pass that changes no row"""
+        self.w = np.zeros(self.n)
+        res = self.run(None if gram is None else self.w, self.w, gram is None)
+        self.H = (res["dhessian"] if gram is None else gram).copy()
+        _check_finite(res["loss"], res["grad"])
+        f, g = self._fg(self.w, res)
+        self.g = g
+        return f, g, res
+
+    def trial(self, w_new) -> float:
+        self.pending = (w_new, self.run(self.w, w_new, True))
+        f, self.g_pending = self._fg(w_new, self.pending[1])
+        return f
+
+    def accept(self):
+        self.w, res = self.pending
+        self.H += res["dhessian"]
+        self.g = self.g_pending
+        return self.g
+
+    def hv(self, v):
+        u = v.copy()
+        if self.fi:
+            u[self.d] *= self.scale
+        Hu = self.H[: self.n, : self.n] @ u
+        if self.fi:
+            Hu[self.d] *= self.scale
+        return v + 2.0 * self.C * Hu
+
+    def coef(self, w):
+        """(coef, intercept): intercept = intercept_scaling w_b"""
+        return w[: self.d].copy(), (self.scale * w[self.d] if self.fi else 0.0)
+
+
+def _svm_run(ctx, X, y, row_mask, mask_keep, loss: int, param: float, fit_intercept: bool, scale: float):
+    """run(w_from, w_to, hessian) of _SvmProblem: one svm_pass, the bias feature's weight as its intercept"""
+    d = X.shape[1]
+
+    def split(w):
+        return w[:d], (scale * float(w[d]) if fit_intercept else 0.0)
+
+    def run(w_from, w_to, hessian):
+        c, b = split(w_to)
+        cf, bf = split(w_from) if w_from is not None else (None, 0.0)
+        return ctx.svm_pass(X, y, c, b, loss=loss, param=param, coef_from=cf, intercept_from=bf, row_mask=row_mask,
+                            mask_keep=mask_keep, fit_intercept=fit_intercept, hessian=hessian)
+    return run
+
+
+class _B200LinearSVM:
+    """The parameter checks LinearSVC and LinearSVR share: anything that selects another liblinear solver is refused"""
+
+    def _check_svm_params(self, sk: str, loss_ok: str, penalty: str = "l2"):
+        C = self.C
+        if isinstance(C, bool) or not isinstance(C, (int, float, np.integer, np.floating)) or not 0 < C < np.inf:
+            raise ValueError(f"The 'C' parameter of {sk} must be a float in the range (0.0, inf). Got {C!r} instead.")
+        if not (isinstance(self.tol, (int, float, np.integer, np.floating)) and np.isfinite(self.tol) and self.tol > 0):
+            raise ValueError(f"The 'tol' parameter of {sk} must be a float in the range (0.0, inf). Got {self.tol!r} "
+                             "instead.")
+        if isinstance(self.max_iter, bool) or not isinstance(self.max_iter, (int, np.integer)) or self.max_iter < 0:
+            raise ValueError(f"The 'max_iter' parameter of {sk} must be an int in the range [0, inf). "
+                             f"Got {self.max_iter!r} instead.")
+        if self.loss != loss_ok:
+            raise ValueError(f"loss={self.loss!r} is not supported: B200{sk} runs liblinear's primal solver for "
+                             f"loss={loss_ok!r}")
+        if penalty != "l2":
+            raise ValueError(f"penalty={penalty!r} is not supported: B200{sk} runs liblinear's primal solver for the L2 "
+                             "penalty")
+        if self.dual not in ("auto", False):
+            raise ValueError(f"dual={self.dual!r} is not supported: B200{sk} runs liblinear's primal solver "
+                             "(dual=False, or 'auto' with at least as many rows as features)")
+        if self.fit_intercept and not self.intercept_scaling > 0:
+            raise ValueError(f"Intercept scaling is {self.intercept_scaling!r} but needs to be greater than 0. To "
+                             "disable fitting an intercept, set fit_intercept=False.")
+
+    def _check_rows(self, sk: str, n: float, d: int) -> None:
+        """the kept rows: some, and (dual='auto') at least as many as features, where scikit-learn picks the primal
+        solver"""
+        if n == 0:
+            raise _too_few_rows((0, d), by=f"B200{sk}")
+        if self.dual == "auto" and n < d:
+            raise ValueError(f"dual='auto' selects liblinear's dual solver with fewer rows ({int(n)}) than features "
+                             f"({d}): B200{sk} runs the primal solver only (set dual=False)")
+
+    def _warn_iter(self, n_iter: int) -> None:
+        if n_iter >= self.max_iter:
+            from sklearn.exceptions import ConvergenceWarning
+            warnings.warn(_LIBLINEAR_CONV, ConvergenceWarning)
+
+
+class B200LinearSVC(_B200LinearSVM, B200RidgeClassifier):
+    """``sklearn.svm.LinearSVC`` with liblinear's primal solver (penalty='l2', loss='squared_hinge', dual=False, or
+    dual='auto' with at least as many rows as features), fitted on the H100.  liblinear's trust-region Newton method
+    (``_tron``) runs on the host; each iteration is one pass (``svm_pass``) for the loss and gradient at the trial point
+    and the change of the generalized Hessian over the rows that crossed the margin, on the fp64 tensor core.  The
+    intercept is liblinear's regularised bias feature of value intercept_scaling.  Two classes: one problem with
+    classes_[1] as +1; more: one-vs-rest, one fit per class in class order.  At w = 0 every kept row is active for every
+    class, so the first class's start pass computes the Gram of [x 1] and the others start from it.
+
+    Labels, ``decision_function``, ``predict`` and ``score`` are ``B200RidgeClassifier``'s.  Refused: loss='hinge',
+    penalty='l1', dual=True, multi_class='crammer_singer', class_weight, sample_weight, one class, more than
+    ``native.MAX_CLASSES`` classes, non-finite X or y.  verbose and random_state are accepted and have no effect."""
+    _sk_module = "svm"
+    _sk_name = "LinearSVC"
+    _sk_attrs = ("coef_", "intercept_", "classes_", "n_iter_", "n_features_in_")
+    _label_who = "B200LinearSVC"
+
+    def __init__(self, penalty: str = "l2", loss: str = "squared_hinge", *, dual="auto", tol: float = 1e-4,
+                 C: float = 1.0, multi_class: str = "ovr", fit_intercept: bool = True, intercept_scaling: float = 1,
+                 class_weight=None, verbose: int = 0, random_state=None, max_iter: int = 1000,
+                 ctx: Optional[native.Context] = None):
+        self.penalty = penalty
+        self.loss = loss
+        self.dual = dual
+        self.tol = tol
+        self.C = C
+        self.multi_class = multi_class
+        self.fit_intercept = fit_intercept
+        self.intercept_scaling = intercept_scaling
+        self.class_weight = class_weight
+        self.verbose = verbose
+        self.random_state = random_state
+        self.max_iter = max_iter
+        self._ctx = ctx
+
+    @classmethod
+    def _check_class_count(cls, classes, more: bool) -> None:
+        if more:
+            raise ValueError(f"B200LinearSVC fits at most {native.MAX_CLASSES} classes, y has more")
+        if classes.size < 2:
+            raise ValueError(_one_class_message(classes[0]))
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None) -> "B200LinearSVC":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, classes_, n_iter_
+        and n_features_in_."""
+        _refuse_sample_weight(sample_weight, "B200LinearSVC")
+        if self.multi_class == "crammer_singer":
+            raise ValueError("multi_class='crammer_singer' is not supported: B200LinearSVC runs liblinear's primal "
+                             "one-vs-rest solver")
+        if self.multi_class != "ovr":
+            raise ValueError(f"`multi_class` must be one of `ovr`, `crammer_singer`, got {self.multi_class!r}")
+        if self.class_weight is not None:
+            raise ValueError("class_weight is not supported by B200LinearSVC: every kept row has weight 1")
+        self._check_svm_params("LinearSVC", "squared_hinge", self.penalty)
+        ctx, fi, scale = self.ctx, bool(self.fit_intercept), float(self.intercept_scaling)
+        C = float(self.C)
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=True) as (X, y, row_mask, labels, classes):
+            d = X.shape[1]
+            targets = labels[1:] if classes.size == 2 else labels
+            W, b, iters, gram = [], [], [], None
+            for pos in targets:
+                prob = _SvmProblem(_svm_run(ctx, X, y, row_mask, mask_keep, native.SVM_SQUARED_HINGE, float(pos), fi,
+                                            scale), C, d, fi, scale)
+                f, g, first = prob.start(gram)
+                n = first["kept"]
+                self._check_rows("LinearSVC", n, d)
+                if gram is None:
+                    gram = prob.H.copy()
+                # train_one: eps max(min(pos, neg), 1) / l
+                eps = float(self.tol) * max(min(first["positive"], n - first["positive"]), 1) / n
+                w, n_iter = _tron(prob, f, g, eps, int(self.max_iter))
+                _check_finite(w)
+                c, b0 = prob.coef(w)
+                W.append(c)
+                b.append(b0)
+                iters.append(n_iter)
+        self.classes_ = classes
+        self.coef_ = np.array(W)
+        self.intercept_ = np.array(b) if fi else 0.0
+        self.n_iter_ = int(max(iters))
+        self.n_features_in_ = int(d)
+        self._warn_iter(self.n_iter_)
+        return self
+
+    def _sk_params(self) -> dict:
+        return dict(penalty=self.penalty, loss=self.loss, dual=self.dual, tol=self.tol, C=self.C,
+                    multi_class=self.multi_class, fit_intercept=self.fit_intercept,
+                    intercept_scaling=self.intercept_scaling, class_weight=self.class_weight, verbose=self.verbose,
+                    random_state=self.random_state, max_iter=self.max_iter)
+
+    _sk_prepare = _B200Estimator._sk_prepare      # LinearSVC's predict reads classes_, coef_ and intercept_ only
+
+    def __repr__(self) -> str:
+        return f"B200LinearSVC(C={self.C})"
+
+
+class B200LinearSVR(_B200LinearSVM, _B200Estimator):
+    """``sklearn.svm.LinearSVR(loss="squared_epsilon_insensitive")`` with liblinear's primal solver (dual=False, or
+    dual='auto' with at least as many rows as features), fitted on the H100: ``B200LinearSVC``'s trust-region Newton
+    method on the squared epsilon-insensitive loss, with liblinear's tolerance tol.  ``predict`` is one fp64 pass and
+    ``score`` is R^2 from two passes over the kept rows.  Refused: loss='epsilon_insensitive' (scikit-learn's default,
+    a dual solver), dual=True, sample_weight, non-finite X or y.  verbose and random_state are accepted and have no
+    effect."""
+    _sk_module = "svm"
+    _sk_name = "LinearSVR"
+    _sk_attrs = ("coef_", "intercept_", "n_iter_", "n_features_in_")
+
+    def __init__(self, *, epsilon: float = 0.0, tol: float = 1e-4, C: float = 1.0, loss: str = "epsilon_insensitive",
+                 fit_intercept: bool = True, intercept_scaling: float = 1.0, dual="auto", verbose: int = 0,
+                 random_state=None, max_iter: int = 1000, ctx: Optional[native.Context] = None):
+        self.epsilon = epsilon
+        self.tol = tol
+        self.C = C
+        self.loss = loss
+        self.fit_intercept = fit_intercept
+        self.intercept_scaling = intercept_scaling
+        self.dual = dual
+        self.verbose = verbose
+        self.random_state = random_state
+        self.max_iter = max_iter
+        self._ctx = ctx
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1, sample_weight=None) -> "B200LinearSVR":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16), y float (an f32
+        ``DeviceArray`` beside device rows); ``row_mask`` (uint8 per row) restricts the fit to rows equal to
+        ``mask_keep``.  Sets coef_, intercept_, n_iter_ and n_features_in_."""
+        _refuse_sample_weight(sample_weight, "B200LinearSVR")
+        self._check_svm_params("LinearSVR", "squared_epsilon_insensitive")
+        eps = self.epsilon
+        if isinstance(eps, bool) or not isinstance(eps, (int, float, np.integer, np.floating)) or not 0 <= eps < np.inf:
+            raise ValueError(f"The 'epsilon' parameter of LinearSVR must be a float in the range [0.0, inf). Got "
+                             f"{eps!r} instead.")
+        ctx, fi, scale = self.ctx, bool(self.fit_intercept), float(self.intercept_scaling)
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = X.shape[1]
+            prob = _SvmProblem(_svm_run(ctx, X, y, row_mask, mask_keep, native.SVM_SQUARED_EPSILON, float(eps), fi,
+                                        scale), float(self.C), d, fi, scale)
+            f, g, first = prob.start()
+            self._check_rows("LinearSVR", first["kept"], d)
+            if first["y_nonfinite"] > 0:
+                raise ValueError(_NAN_MESSAGE)
+            w, n_iter = _tron(prob, f, g, float(self.tol), int(self.max_iter))
+            _check_finite(w)
+        c, b0 = prob.coef(w)
+        self.coef_ = c
+        self.intercept_ = np.array([b0]) if fi else 0.0
+        self.n_iter_ = int(n_iter)
+        self.n_features_in_ = int(d)
+        self._warn_iter(self.n_iter_)
+        return self
+
+    def predict(self, X):
+        """X coef_ + intercept_ in fp64: float64 for host rows, an f64 ``DeviceArray`` for device rows."""
+        return self.ctx.glm_predict(self._checked_rows(X), self.coef_, float(np.sum(self.intercept_)),
+                                    link=native.GLM_IDENTITY)
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """R^2 over the kept rows, as scikit-learn's ``RegressorMixin.score`` computes it: the squared residuals of
+        the model and of the mean of y, one pass each."""
+        ctx = self.ctx
+        with _stage_rows(ctx, X, y, row_mask) as (X, y, row_mask):
+            d = self._checked_rows(X).shape[1]
+            kw = dict(link=native.GLM_IDENTITY, power=0.0, row_mask=row_mask, mask_keep=mask_keep, hessian=False)
+            model = ctx.glm_pass(X, y, self.coef_, float(np.sum(self.intercept_)), **kw)
+            n = model["kept"]
+            if n == 0:
+                raise _too_few_rows((0, d))
+            if model["y_nonfinite"] > 0:
+                raise ValueError(_NAN_MESSAGE)
+            null = ctx.glm_pass(X, y, np.zeros(d), model["sum_y"] / n, **kw)
+        num, den = model["loss"], null["loss"]
+        if den == 0:                                # r2_score's force_finite
+            return 1.0 if num == 0 else 0.0
+        return float(1 - num / den)
+
+    def _sk_params(self) -> dict:
+        return dict(epsilon=self.epsilon, tol=self.tol, C=self.C, loss=self.loss, fit_intercept=self.fit_intercept,
+                    intercept_scaling=self.intercept_scaling, dual=self.dual, verbose=self.verbose,
+                    random_state=self.random_state, max_iter=self.max_iter)
+
+    def __repr__(self) -> str:
+        return f"B200LinearSVR(C={self.C}, epsilon={self.epsilon})"

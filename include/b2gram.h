@@ -424,6 +424,30 @@ int b2_multinomial_line_search(b2_ctx* ctx, const void* X, int x_dtype, const fl
  * one round trip through a temporary device copy. */
 int b2_softmax_rows(b2_ctx* ctx, double* values, int64_t n_rows, int n_cols, int mem_kind);
 
+/* ---- LinearSVC / LinearSVR, primal (DESIGN.md section 15) ---------------------------------------------------------
+ * The row pass of liblinear's trust-region Newton solver (TRON) for the L2-regularised squared hinge and squared
+ * epsilon-insensitive losses, the GLM passes' row handling: per kept row z = [x 1] and eta = x.coef + intercept in fp64
+ * (x converted exactly), at the trial point (coef, intercept) and, when coef_from is not NULL, at the accepted point
+ * (coef_from, intercept_from), both by the same arithmetic in the same order.  A row is active at a point when
+ *   B2_SVM_SQUARED_HINGE: m = 1 - t eta > 0, t = +1 where y == pos_label and -1 otherwise; loss m^2, g = eta - t;
+ *   B2_SVM_SQUARED_EPSILON: |r| > eps with r = eta - y (eps = pos_label_or_epsilon); e = r - eps or r + eps, loss e^2,
+ *   g = e.
+ * Sums over the kept rows active at the trial point, unscaled (no C, no factor 2; z holds 1, not liblinear's bias
+ * value), in a fixed order: repeated calls are bit-identical.  sums_out (host, d + 8 doubles): [0] sum loss [1] kept rows
+ * [2] rows active at the trial point [3] rows entering the active set [4] rows leaving it [5] (squared hinge) kept rows
+ * with y == pos_label [6] kept rows with y not finite, [7, 8 + d) sum g z.  dhess_out: NULL (no Hessian), or (host)
+ * (d + 1) x (d + 1) doubles, sum sigma z z^T with sigma = active(trial) - active(from) in {-1, 0, 1}: the change of the
+ * generalized Hessian between the two points, on the fp64 tensor core for the rows that changed side only.  coef_from =
+ * NULL is the empty active set, so dhess_out is the Gram of the active rows.  fit_intercept = 0 takes both intercepts as
+ * 0.  B2_E_ARG: bad shapes, an unknown loss, a non-finite pos_label, eps < 0 or not finite, null coef or sums_out;
+ * B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or no kept row) is no error: every sum is 0. */
+#define B2_SVM_SQUARED_HINGE 0    /* LinearSVC(loss="squared_hinge"): liblinear's l2r_l2_svc_fun */
+#define B2_SVM_SQUARED_EPSILON 1  /* LinearSVR(loss="squared_epsilon_insensitive"): liblinear's l2r_l2_svr_fun */
+int b2_svm_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                int mem_kind, const uint8_t* row_mask, int mask_keep, int loss, double pos_label_or_epsilon,
+                const double* coef_from, double intercept_from, const double* coef, double intercept, int fit_intercept,
+                double* sums_out, double* dhess_out);
+
 /* ---- RidgeClassifierCV: replaces sklearn.linear_model.RidgeClassifierCV(alphas).fit with cv=None (DESIGN.md
  * section 13) ---------------------------------------------------------------------------------------------------------
  * The leave-one-out error of every class target and alpha: the Gram of the kept rows, b2_class_sums at its column means,
