@@ -30,6 +30,10 @@ Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- th
     B200LinearSVC          sklearn's LinearSVC (liblinear's primal solver, squared hinge) for 2 to 32 classes: trust-region
                            Newton fits whose Hessian is updated on the fp64 tensor core from the rows that cross the margin
     B200LinearSVR          sklearn's LinearSVR (loss="squared_epsilon_insensitive", primal): the same solver
+    B200LinearDiscriminantAnalysis
+                           sklearn's LinearDiscriminantAnalysis (svd, lsqr, eigen) for 2 to 32 classes: the class means
+                           and one fp64 tensor-core pass for the within-class scatter, the solvers on the host;
+                           probabilities and projections in one fp64 decision pass
     stage_1_train_model    drop-in for mlops_simulation/stage_1_train_model.py
 """
 from . import _native as native
@@ -37,6 +41,7 @@ from ._native import (BF16, F32, KERNEL_AUTO, KERNEL_NARROW, KERNEL_SIMT, KERNEL
                       DeviceArray, PinnedArray)
 from .estimator import (B200ARDRegression, B200BayesianRidge, B200ElasticNet, B200ElasticNetCV, B200GammaRegressor,
                         B200Lasso, B200LassoCV, B200LinearRegression, B200LinearSVC, B200LinearSVR, B200LogisticRegression,
+                        B200LinearDiscriminantAnalysis,
                         B200MultinomialLogisticRegression,
                         B200PoissonRegressor,
                         B200RidgeClassifier, B200RidgeClassifierCV, B200RidgeCV, B200TweedieRegressor, default_context,
@@ -46,6 +51,7 @@ from . import sharding, tranche_io  # noqa: F401
 __all__ = ["native", "Context", "DeviceArray", "PinnedArray", "B200LinearRegression", "B200RidgeCV", "B200ElasticNet",
            "B200Lasso", "B200ElasticNetCV", "B200LassoCV", "B200BayesianRidge", "B200ARDRegression",
            "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression",
-           "B200RidgeClassifier", "B200RidgeClassifierCV", "B200MultinomialLogisticRegression", "B200LinearSVC", "B200LinearSVR", "fold_ids", "enet_path", "lasso_path", "default_context",
+           "B200RidgeClassifier", "B200RidgeClassifierCV", "B200MultinomialLogisticRegression", "B200LinearSVC", "B200LinearSVR",
+           "B200LinearDiscriminantAnalysis", "fold_ids", "enet_path", "lasso_path", "default_context",
            "F32", "BF16", "KERNEL_AUTO", "KERNEL_SIMT", "KERNEL_TCGEN05", "KERNEL_NARROW", "PRECISION_SPLIT", "PRECISION_BF16"]
 __version__ = "0.1.0"

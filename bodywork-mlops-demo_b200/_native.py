@@ -101,6 +101,8 @@ _SIGNATURES = {
     "b2_label_scan": (C.c_int, [_vp, _vp, _c_i64, _vp, C.c_int, _vp]),
     "b2_class_sums": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
                                 _vp, _vp, _vp]),
+    "b2_class_scatter": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
+                                   _vp, _vp, _vp, _vp]),
     "b2_solve_classes": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.c_int, _vp, _vp]),
     "b2_classify": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int,
                               _vp, _vp, _vp, _vp]),
@@ -839,6 +841,29 @@ class Context:
                                   c.ctypes.data if c is not None else None, sums.ctypes.data, counts.ctypes.data)
         _check_args(rc, "b2_class_sums")
         return {"sums": sums, "kept": float(counts[0]), "unmatched": float(counts[1]), "nonfinite": float(counts[2])}
+
+    def class_scatter(self, X, y, classes, means, weights=None, *, row_mask=None, mask_keep: int = 1) -> dict:
+        """The pooled within-class scatter of the kept rows in one fp64 pass (b2_class_scatter): ``classes`` are K
+        sorted fp32 values and a row's class is the index of its y among them, ``means`` the (K, d) class means and
+        ``weights`` K class weights (None: all 1).  Returns scatter ((d, d): sum over the rows of class k of
+        w_k (x - m_k)(x - m_k)^T, exactly symmetric), kept, unmatched (kept rows of no class, NaN included) and nonfinite
+        (kept rows with y not finite).  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        m = np.ascontiguousarray(means, dtype=np.float64)
+        if m.shape != (cl.size, d):
+            raise ValueError(f"means must be ({cl.size}, {d}), got {m.shape}")
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float64).ravel()
+        if w is not None and w.size != cl.size:
+            raise ValueError(f"weights has {w.size} entries, {cl.size} classes")
+        scatter = np.empty((d, d), dtype=np.float64)
+        counts = np.empty(3, dtype=np.float64)
+        rc = load().b2_class_scatter(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data, cl.size,
+                                     m.ctypes.data, w.ctypes.data if w is not None else None, scatter.ctypes.data,
+                                     counts.ctypes.data)
+        _check_args(rc, "b2_class_scatter")
+        return {"scatter": scatter, "kept": float(counts[0]), "unmatched": float(counts[1]),
+                "nonfinite": float(counts[2])}
 
     def solve_classes(self, class_sums, alpha: float = 1.0, fit_intercept: bool = True,
                       n_classes: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:

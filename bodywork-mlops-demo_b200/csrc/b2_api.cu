@@ -480,7 +480,7 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part,
-                  ctx->cls, ctx->loo_cls, ctx->mn_op, ctx->mn_sum, ctx->mn_part};
+                  ctx->cls, ctx->loo_cls, ctx->mn_op, ctx->mn_sum, ctx->mn_part, ctx->disc, ctx->disc_part};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1732,6 +1732,56 @@ int b2_class_sums(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(sums_out, h.data(), sizeof(double) * n_sums);
   memcpy(counts_out, h.data() + n_sums, sizeof(double) * 3);
+  return B2_OK;
+}
+
+// ---- LinearDiscriminantAnalysis (DESIGN.md section 16) ---------------------------------------------------------------
+// The operands and sums (ctx->disc) and the per-CTA partials (ctx->disc_part, one CTA per SM), allocated by the first
+// call and freed with the context: no other pass's buffers are touched.
+int b2_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                     const double* means, const double* weights, double* scatter_out, double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_rows > 0 && (X == nullptr || y == nullptr)) { set_error("X / y is null"); return B2_E_ARG; }
+  if (means == nullptr || scatter_out == nullptr || counts_out == nullptr) {
+    set_error("means / scatter_out / counts_out is null");
+    return B2_E_ARG;
+  }
+  if (int r = check_classes(classes, n_classes)) return r;
+  std::vector<double> op(kDaSums, 0.0);                 // kDaClasses, kDaWeights, kDaMeans
+  for (int k = 0; k < n_classes; ++k) {
+    const double w = weights != nullptr ? weights[k] : 1.0;
+    if (!(w >= 0.0) || !isfinite(w)) { set_error("weights[%d]=%g must be finite and >= 0", k, w); return B2_E_ARG; }
+    op[kDaClasses + k] = classes[k];
+    op[kDaWeights + k] = w;
+    for (int j = 0; j < d; ++j) {
+      const double m = means[(size_t)k * d + j];
+      if (!isfinite(m)) { set_error("means[%d][%d]=%g is not finite", k, j, m); return B2_E_ARG; }
+      op[kDaMeans + k * kMaxD + j] = m;
+    }
+  }
+  if (ctx->n_ranks > 1) {
+    set_error("b2_class_scatter runs on one rank only (its sums are not exchanged between ranks)");
+    return B2_E_UNSUPPORTED;
+  }
+  if (ctx->disc == nullptr) {
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->disc), sizeof(double) * kDaDoubles));
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->disc_part), sizeof(double) * (size_t)ctx->sm_count * kDaPart));
+  }
+  B2_CUDA(cudaMemcpyAsync(ctx->disc, op.data(), sizeof(double) * op.size(), cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on this frame's stack
+  if (int r = row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+        return launch_class_scatter(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_classes, s.first);
+      }))
+    return r;
+  std::vector<double> h(kDaPart);
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->disc + kDaSums, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(counts_out, h.data(), sizeof(double) * 3);
+  for (int i = 0; i < d; ++i)
+    for (int j = i; j < d; ++j)        // the upper triangle, mirrored
+      scatter_out[(size_t)i * d + j] = scatter_out[(size_t)j * d + i] = h[kDaHead + (size_t)i * kMaxD + j];
   return B2_OK;
 }
 

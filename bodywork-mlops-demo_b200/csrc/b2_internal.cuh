@@ -194,6 +194,18 @@ constexpr int kMnCoef = kMaxClasses;
 constexpr int kMnStep = kMnCoef + kMaxClasses * (kMaxD + 1);
 constexpr int kMnOpDoubles = kMnStep + kMaxClasses * (kMaxD + 1);
 
+// ---- LinearDiscriminantAnalysis (discriminant.cu; DESIGN.md section 16) -------------------------------------------
+// doubles of ctx->disc: the sorted classes, the class weights, the class means [kMaxClasses][kMaxD], then the reduced sums
+// at kDaSums ([0] kept rows [1] kept rows of no class [2] kept rows with y not finite, then the upper triangle of the
+// scatter at kDaHead + i kMaxD + j).  One CTA's partial in ctx->disc_part has the sums' layout, kDaPart doubles.
+constexpr int kDaHead = 8;
+constexpr int kDaPart = kDaHead + kMaxD * kMaxD;
+constexpr int kDaClasses = 0;
+constexpr int kDaWeights = kMaxClasses;
+constexpr int kDaMeans = 2 * kMaxClasses;
+constexpr int kDaSums = kDaMeans + kMaxClasses * kMaxD;
+constexpr int kDaDoubles = kDaSums + kDaPart;
+
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
 // first and last row of every fold of fold ids in device memory: range[2 k] = n - first, range[2 k + 1] = last + 1
@@ -288,6 +300,10 @@ struct b2_ctx {
   size_t mn_sum_doubles = 0;
   double* mn_part = nullptr;
   size_t mn_part_doubles = 0;
+  // LinearDiscriminantAnalysis: the operands and sums of b2_class_scatter (b2::kDa*) and the per-CTA partials
+  // [sm_count][kDaPart], allocated by the first call
+  double* disc = nullptr;
+  double* disc_part = nullptr;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -510,6 +526,10 @@ int launch_softmax_rows(b2_ctx* ctx, double* values, int64_t n, int k);
 // otherwise adds)
 int launch_svm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                const uint8_t* mask, int keep, int loss, bool hess, bool first_block);
+// the within-class scatter of the rows [0, n) at the classes, weights and means of ctx->disc, then the ordered reduce of
+// the per-CTA sums into ctx->disc + kDaSums (`first_block` overwrites, otherwise adds)
+int launch_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                         const uint8_t* mask, int keep, int n_classes, bool first_block);
 // W and b of the ridge classifier from the resident S and the class sums at ctx->cls + kClsSums (one launch)
 int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes);
 int launch_p2p_allreduce(b2_ctx* ctx);

@@ -2430,3 +2430,258 @@ class B200LinearSVR(_B200LinearSVM, _B200Estimator):
 
     def __repr__(self) -> str:
         return f"B200LinearSVR(C={self.C}, epsilon={self.epsilon})"
+
+
+# ---- LinearDiscriminantAnalysis: the class means and one fp64 within-class scatter pass (DESIGN.md section 16) --------
+_LDA_SOLVERS = ("svd", "lsqr", "eigen")
+
+
+def _shrunk(cov: np.ndarray, shrinkage) -> np.ndarray:
+    """sklearn.covariance.shrunk_covariance of a covariance (None: the covariance as it is)"""
+    if shrinkage is None:
+        return cov
+    s = float(shrinkage)
+    out = (1.0 - s) * cov
+    out += s * (np.trace(cov) / cov.shape[0]) * np.eye(cov.shape[0])
+    return out
+
+
+def _lda_svd(sw1: np.ndarray, means: np.ndarray, nk: np.ndarray, priors: np.ndarray, tol: float, max_components: int):
+    """scikit-learn's ``_solve_svd`` from the statistics: the within-class singular values and right singular vectors
+    of the scaled centred rows are the square roots and eigenvectors of their Gram, S_w(1) / (n - K) / (std std^T);
+    from the K x rank product on, scikit-learn's code as it is.  Returns (coef, intercept, xbar, scalings,
+    explained_variance_ratio) before the two-class collapse."""
+    import scipy.linalg
+    n, K = float(nk.sum()), nk.size
+    std = np.sqrt(np.diag(sw1) / n)
+    std[std == 0] = 1.0
+    lam, V = np.linalg.eigh(sw1 / (n - K) / np.outer(std, std))
+    lam, V = lam[::-1], V[:, ::-1]
+    S = np.sqrt(np.maximum(lam, 0.0))
+    rank = int(np.sum(S > tol))
+    scalings = V[:, :rank] / std[:, None] / S[:rank]
+    xbar = priors @ means
+    fac = 1.0 if K == 1 else 1.0 / (K - 1)
+    Xb = ((np.sqrt((n * priors) * fac)) * (means - xbar).T).T @ scalings
+    _, S, Vt = scipy.linalg.svd(Xb, full_matrices=False)
+    evr = np.empty((0,)) if max_components == 0 else (S ** 2 / np.sum(S ** 2))[:max_components]
+    rank = int(np.sum(S > tol * S[0]))
+    scalings = scalings @ Vt.T[:, :rank]
+    coef = (means - xbar) @ scalings
+    intercept = -0.5 * np.sum(coef ** 2, axis=1) + np.log(priors)
+    coef = coef @ scalings.T
+    intercept -= xbar @ coef.T
+    return coef, intercept, xbar, scalings, evr
+
+
+def _lda_lstsq(cov: np.ndarray, means: np.ndarray, priors: np.ndarray):
+    """scikit-learn's ``_solve_lstsq`` on the (shrunk) covariance"""
+    import scipy.linalg
+    coef = scipy.linalg.lstsq(cov, means.T)[0].T
+    return coef, -0.5 * np.diag(np.dot(means, coef.T)) + np.log(priors)
+
+
+def _lda_eigen(cov: np.ndarray, total: np.ndarray, means: np.ndarray, priors: np.ndarray, max_components: int):
+    """scikit-learn's ``_solve_eigen`` on the (shrunk) within-class covariance and total covariance"""
+    import scipy.linalg
+    evals, evecs = scipy.linalg.eigh(total - cov, cov)
+    evr = np.sort(evals / np.sum(evals))[::-1][:max_components]
+    evecs = evecs[:, np.argsort(evals)[::-1]]
+    coef = np.dot(means, evecs).dot(evecs.T)
+    return coef, -0.5 * np.diag(np.dot(means, coef.T)) + np.log(priors), evecs, evr
+
+
+class B200LinearDiscriminantAnalysis(B200RidgeClassifier):
+    """``sklearn.discriminant_analysis.LinearDiscriminantAnalysis`` for 2 to ``native.MAX_CLASSES`` classes, fitted on
+    the H100.  Every solver needs only the class counts and means (one class-sum pass) and the pooled within-class
+    scatter S_w(w) = sum w_y (x - m_y)(x - m_y)^T, which one fp64 tensor-core pass (``class_scatter``) forms from rows
+    centred on their class mean: w = 1 for 'svd', w_k = p_k / n_k (the priors' covariance) for 'lsqr' and 'eigen'.  A
+    second pass with the other weights runs only where a fit needs both matrices and the priors are given: 'svd' with
+    store_covariance, and 'eigen' (the total scatter is S_w(1) plus the between-class scatter of the means).  The
+    solvers are scikit-learn's, restated on these statistics with numpy and scipy on the host; 'svd' takes the
+    eigenvectors of the scaled scatter for the right singular vectors of the scaled rows.
+
+    Labels, ``decision_function``, ``predict`` and ``score`` are ``B200RidgeClassifier``'s.  ``predict_proba`` is the
+    logistic of the decision for two classes and scikit-learn's softmax of the decisions for more (on the device for
+    device rows); ``transform`` is one fp64 decision pass with one output per component.  The columns of ``scalings_``
+    and ``transform`` equal scikit-learn's up to the sign of each column; every other attribute and prediction does not
+    depend on those signs.  ``transform`` computes x.s - xbar.s, so its error is relative to sum |x_j s_j|.
+
+    Refused: shrinkage='auto' (Ledoit-Wolf needs each class's own covariance), a covariance_estimator, shrinkage with
+    the 'svd' solver, other solvers, one class, more than ``native.MAX_CLASSES`` classes, continuous, multilabel or
+    non-finite y, and non-finite X."""
+    _sk_module = "discriminant_analysis"
+    _sk_name = "LinearDiscriminantAnalysis"
+    _sk_attrs = ("coef_", "intercept_", "classes_", "means_", "priors_", "n_features_in_", "_max_components",
+                 "_n_features_out")
+    _label_who = "B200LinearDiscriminantAnalysis"
+
+    def __init__(self, solver: str = "svd", shrinkage=None, priors=None, n_components=None,
+                 store_covariance: bool = False, tol: float = 1e-4, covariance_estimator=None,
+                 ctx: Optional[native.Context] = None):
+        self.solver = solver
+        self.shrinkage = shrinkage
+        self.priors = priors
+        self.n_components = n_components
+        self.store_covariance = store_covariance
+        self.tol = tol
+        self.covariance_estimator = covariance_estimator
+        self._ctx = ctx
+
+    def _check_params(self):
+        who = "B200LinearDiscriminantAnalysis"
+        if self.solver not in _LDA_SOLVERS:
+            raise ValueError(f"The 'solver' parameter of {who} must be a str among {{'eigen', 'lsqr', 'svd'}}. Got "
+                             f"{self.solver!r} instead.")
+        s = self.shrinkage
+        if isinstance(s, str) and s == "auto":
+            raise ValueError(f"shrinkage='auto' is not supported by {who}: the Ledoit-Wolf estimate needs each class's "
+                             "own covariance, and its weight falls like 1/n, so at the row counts this estimator serves "
+                             "shrinkage=None or a float gives the same model")
+        if s is not None and (isinstance(s, (bool, str)) or not isinstance(s, (int, float, np.integer, np.floating))
+                              or not 0 <= s <= 1):
+            raise ValueError(f"The 'shrinkage' parameter of {who} must be a str among {{'auto'}}, a float in the range "
+                             f"[0, 1] or None. Got {s!r} instead.")
+        if self.covariance_estimator is not None:
+            raise ValueError(f"covariance_estimator is not supported by {who}: the covariance is the empirical one "
+                             "(with shrinkage=None or a float)")
+        if self.solver == "svd" and s is not None:
+            raise NotImplementedError(f"shrinkage not supported with 'svd' solver. ({who})")
+        if isinstance(self.tol, bool) or not isinstance(self.tol, (int, float, np.integer, np.floating)) \
+                or not 0 <= self.tol < np.inf:
+            raise ValueError(f"The 'tol' parameter of {who} must be a float in the range [0.0, inf). Got {self.tol!r} "
+                             "instead.")
+
+    def _priors(self, nk: np.ndarray) -> np.ndarray:
+        """priors_: the class frequencies, or the given priors (non-negative, renormalised with scikit-learn's warning)"""
+        if self.priors is None:
+            return nk / float(nk.sum())
+        p = np.asarray(self.priors, dtype=np.float64).ravel()
+        if p.size != nk.size:
+            raise ValueError(f"priors has {p.size} entries, but y holds {nk.size} classes")
+        if np.any(p < 0):
+            raise ValueError("priors must be non-negative")
+        if np.abs(np.sum(p) - 1.0) > 1e-5:
+            warnings.warn("The priors do not sum to 1. Renormalizing", UserWarning)
+            p = p / p.sum()
+        return p
+
+    @staticmethod
+    def _scatter(ctx, X, y, labels, means, weights, row_mask, mask_keep, n: float) -> np.ndarray:
+        """one scatter pass, checked against the class-sum pass's rows"""
+        res = ctx.class_scatter(X, y, labels, means, weights, row_mask=row_mask, mask_keep=mask_keep)
+        if res["kept"] != n or res["unmatched"] > 0 or res["nonfinite"] > 0:
+            raise RuntimeError("the scatter pass saw other labels than the label check")
+        _check_finite(res["scatter"])
+        return res["scatter"]
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1) -> "B200LinearDiscriminantAnalysis":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets coef_, intercept_, classes_, means_,
+        priors_, covariance_ (lsqr, eigen, or store_covariance), xbar_ (svd), scalings_ and explained_variance_ratio_
+        (svd, eigen) and n_features_in_."""
+        self._check_params()
+        ctx, solver, shrink = self.ctx, self.solver, self.shrinkage
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=True) as (X, y, row_mask, labels, classes):
+            d, K = X.shape[1], classes.size
+            cs = ctx.class_sums(X, y, labels, None, row_mask=row_mask, mask_keep=mask_keep)
+            nk, n = cs["sums"][:, d], cs["kept"]
+            if cs["unmatched"] > 0 or cs["nonfinite"] > 0 or nk.sum() != n or np.any(nk == 0):
+                raise RuntimeError("the class-sum pass saw other labels than the label check")
+            _check_finite(cs["sums"])
+            means = cs["sums"][:, :d] / nk[:, None]
+            if n <= K:
+                raise ValueError("The number of samples must be more than the number of classes.")
+            priors = self._priors(nk)
+            max_components = min(K - 1, d)
+            if self.n_components is not None and self.n_components > max_components:
+                raise ValueError("n_components cannot be larger than min(n_features, n_classes - 1).")
+            freq = self.priors is None
+
+            def scatter(weights):
+                return self._scatter(ctx, X, y, labels, means, weights, row_mask, mask_keep, n)
+            if solver == "svd":
+                sw1 = scatter(None)
+                cov = None if not self.store_covariance else (sw1 / n if freq else scatter(priors / nk))
+            else:
+                cov = scatter(priors / nk)
+                sw1 = None if solver != "eigen" else (cov * n if freq else scatter(None))
+        self._max_components = max_components if self.n_components is None else int(self.n_components)
+        for name in ("covariance_", "xbar_", "scalings_", "explained_variance_ratio_"):
+            self.__dict__.pop(name, None)
+        if solver == "svd":
+            coef, intercept, self.xbar_, self.scalings_, self.explained_variance_ratio_ = _lda_svd(
+                sw1, means, nk, priors, float(self.tol), self._max_components)
+            if cov is not None:
+                self.covariance_ = cov
+        elif solver == "lsqr":
+            self.covariance_ = _shrunk(cov, shrink)
+            coef, intercept = _lda_lstsq(self.covariance_, means, priors)
+        else:
+            self.covariance_ = _shrunk(cov, shrink)
+            xbar = nk @ means / n
+            total = (sw1 + (nk[:, None] * (means - xbar)).T @ (means - xbar)) / n
+            coef, intercept, self.scalings_, self.explained_variance_ratio_ = _lda_eigen(
+                self.covariance_, _shrunk(total, shrink), means, priors, self._max_components)
+        if K == 2:                                      # scikit-learn's binary collapse
+            coef = (coef[1, :] - coef[0, :]).reshape(1, -1)
+            intercept = np.reshape(intercept[1] - intercept[0], (1,))
+        _check_finite(coef)
+        self.coef_, self.intercept_ = coef, intercept
+        self.classes_, self.means_, self.priors_ = classes, means, priors
+        self.n_features_in_ = int(d)
+        self._n_features_out = self._max_components
+        return self
+
+    def predict_proba(self, X):
+        """The class probabilities, (n, K) fp64: [1 - p, p] with p = expit(decision) for two classes (one pass), else
+        scikit-learn's softmax of the decisions -- on the host for host rows, in place on the device for device rows
+        (an f64 ``DeviceArray``)."""
+        if self.classes_.size == 2:
+            Xc = self._checked_rows(X)
+            return self.ctx.logistic_predict(Xc, self.coef_[0], float(self.intercept_[0]), proba=True)["proba"]
+        from sklearn.utils.extmath import softmax
+        dec = self.decision_function(X)
+        if isinstance(dec, native.DeviceArray):
+            self.ctx.softmax_rows(dec)
+            return dec
+        return softmax(dec, copy=False)
+
+    def predict_log_proba(self, X):
+        """log(predict_proba(X)) for host rows, zeros raised to the smallest normal first, as scikit-learn does."""
+        if isinstance(X, native.DeviceArray):
+            raise ValueError("predict_log_proba takes host rows (predict_proba returns device probabilities)")
+        p = self.predict_proba(X)
+        p[p == 0.0] += np.finfo(p.dtype).smallest_normal
+        return np.log(p)
+
+    def transform(self, X):
+        """The projection on the discriminant directions, (n, c) fp64 in one pass: (x - xbar_) scalings_ for 'svd'
+        (c = min(rank, n_components)), x scalings_ for 'eigen' (c = n_components); float64 for host rows, an f64
+        ``DeviceArray`` for device rows."""
+        if self.solver == "lsqr":
+            raise NotImplementedError("transform not implemented for 'lsqr' solver (use 'svd' or 'eigen').")
+        S = self.scalings_[:, : self._max_components]
+        Xc = self._checked_rows(X)
+        if S.shape[1] == 0:
+            return np.empty((Xc.shape[0], 0))
+        b = -(self.xbar_ @ S) if self.solver == "svd" else np.zeros(S.shape[1])
+        return self.ctx.classify(Xc, S.T, b, np.arange(max(S.shape[1], 2), dtype=np.float32),
+                                 decision=True)["decision"]
+
+    def fit_transform(self, X, y, row_mask=None, mask_keep: int = 1):
+        """fit, then transform every row of X."""
+        return self.fit(X, y, row_mask, mask_keep).transform(X)
+
+    def _sk_params(self) -> dict:
+        return dict(solver=self.solver, shrinkage=self.shrinkage, priors=self.priors, n_components=self.n_components,
+                    store_covariance=self.store_covariance, tol=self.tol)
+
+    def _sk_prepare(self, reg) -> None:
+        """the attributes only some solvers set"""
+        for name in ("covariance_", "xbar_", "scalings_", "explained_variance_ratio_"):
+            if name in self.__dict__:
+                setattr(reg, name, getattr(self, name).copy())
+
+    def __repr__(self) -> str:
+        return f"B200LinearDiscriminantAnalysis(solver={self.solver!r})"

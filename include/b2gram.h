@@ -373,6 +373,19 @@ int b2_label_scan(b2_ctx* ctx, const float* y, int64_t n_rows, const uint8_t* ro
 int b2_class_sums(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                   int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
                   const double* center, double* sums_out, double* counts_out);
+/* b2_class_scatter (LinearDiscriminantAnalysis, DESIGN.md section 16): the pooled within-class scatter of the kept
+ * rows in one fp64 pass, scatter_out (host, d x d, both triangles, exactly symmetric) = sum over the kept rows of class
+ * k of w_k (x - m_k)(x - m_k)^T, x converted exactly and u = x - m_k formed in fp64; the rows of no class add nothing.
+ * classes and y as b2_class_sums; means (host, n_classes x d) the class means m_k; weights (host, n_classes; NULL: all 1)
+ * the class weights w_k (1 for the scatter, p_k / n_k for the priors' covariance).  counts_out (host, 3): [0] kept rows
+ * [1] kept rows whose y is no class (NaN included) [2] kept rows whose y is not finite.  On the fp64 tensor core, the
+ * upper 16 x 16 blocks of the product; sums in a fixed order: repeated calls are bit-identical.  B2_E_ARG: bad shapes,
+ * n_classes outside 2..B2_MAX_CLASSES, classes that are not finite and strictly ascending, null means or outputs,
+ * non-finite means, weights that are negative or not finite; B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or
+ * no kept row) is no error: the scatter and counts are 0. */
+int b2_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                     const double* means, const double* weights, double* scatter_out, double* counts_out);
 /* b2_solve_classes: the model of the resident S (every kept row of some class) and the class sums (host, n_classes x
  * (d + 1) as b2_class_sums returns them, at any center; NULL: the sums of the last b2_class_sums).  T = 1 for two
  * classes, else n_classes: coef_out (host, T x d) and intercept_out (host, T; ybar_t - mean.w_t, 0 without
