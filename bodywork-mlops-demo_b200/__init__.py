@@ -34,6 +34,10 @@ Import name: ``bodywork_mlops_demo_b200`` (a shim package that points here -- th
                            sklearn's LinearDiscriminantAnalysis (svd, lsqr, eigen) for 2 to 32 classes: the class means
                            and one fp64 tensor-core pass for the within-class scatter, the solvers on the host;
                            probabilities and projections in one fp64 decision pass
+    B200QuadraticDiscriminantAnalysis
+                           sklearn's QuadraticDiscriminantAnalysis (svd, eigen) for 2 to 32 classes: the class means and
+                           every class's scatter from one fp64 tensor-core pass over the rows in class order, the
+                           solvers on the host; K quadratic forms per row in one fp64 decision pass
     stage_1_train_model    drop-in for mlops_simulation/stage_1_train_model.py
 """
 from . import _native as native
@@ -42,6 +46,7 @@ from ._native import (BF16, F32, KERNEL_AUTO, KERNEL_NARROW, KERNEL_SIMT, KERNEL
 from .estimator import (B200ARDRegression, B200BayesianRidge, B200ElasticNet, B200ElasticNetCV, B200GammaRegressor,
                         B200Lasso, B200LassoCV, B200LinearRegression, B200LinearSVC, B200LinearSVR, B200LogisticRegression,
                         B200LinearDiscriminantAnalysis,
+                        B200QuadraticDiscriminantAnalysis,
                         B200MultinomialLogisticRegression,
                         B200PoissonRegressor,
                         B200RidgeClassifier, B200RidgeClassifierCV, B200RidgeCV, B200TweedieRegressor, default_context,
@@ -52,6 +57,6 @@ __all__ = ["native", "Context", "DeviceArray", "PinnedArray", "B200LinearRegress
            "B200Lasso", "B200ElasticNetCV", "B200LassoCV", "B200BayesianRidge", "B200ARDRegression",
            "B200PoissonRegressor", "B200GammaRegressor", "B200TweedieRegressor", "B200LogisticRegression",
            "B200RidgeClassifier", "B200RidgeClassifierCV", "B200MultinomialLogisticRegression", "B200LinearSVC", "B200LinearSVR",
-           "B200LinearDiscriminantAnalysis", "fold_ids", "enet_path", "lasso_path", "default_context",
+           "B200LinearDiscriminantAnalysis", "B200QuadraticDiscriminantAnalysis", "fold_ids", "enet_path", "lasso_path", "default_context",
            "F32", "BF16", "KERNEL_AUTO", "KERNEL_SIMT", "KERNEL_TCGEN05", "KERNEL_NARROW", "PRECISION_SPLIT", "PRECISION_BF16"]
 __version__ = "0.1.0"

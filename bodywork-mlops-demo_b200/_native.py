@@ -103,6 +103,10 @@ _SIGNATURES = {
                                 _vp, _vp, _vp]),
     "b2_class_scatter": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
                                    _vp, _vp, _vp, _vp]),
+    "b2_class_scatters": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp,
+                                    C.c_int, _vp, _vp, _vp, _vp]),
+    "b2_qda_decision": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, C.c_int,
+                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b2_solve_classes": (C.c_int, [_vp, C.c_double, C.c_int, _vp, C.c_int, _vp, _vp]),
     "b2_classify": (C.c_int, [_vp, _vp, C.c_int, _vp, _c_i64, C.c_int, _c_i64, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int,
                               _vp, _vp, _vp, _vp]),
@@ -864,6 +868,58 @@ class Context:
         _check_args(rc, "b2_class_scatter")
         return {"scatter": scatter, "kept": float(counts[0]), "unmatched": float(counts[1]),
                 "nonfinite": float(counts[2])}
+
+    # -- QuadraticDiscriminantAnalysis (DESIGN.md section 17) ----------------------------------------------------------
+    def class_scatters(self, X, y, classes, means, *, row_mask=None, mask_keep: int = 1) -> dict:
+        """Every class's own scatter of the kept rows in one fp64 pass over the rows in class order (b2_class_scatters):
+        ``classes`` are K sorted fp32 values and a row's class is the index of its y among them, ``means`` the (K, d)
+        class means.  Returns scatters ((K, d, d): sum over the rows of class k of (x - m_k)(x - m_k)^T, exactly
+        symmetric, zero for a class without rows), class_counts ((K,) kept rows per class), kept, unmatched (kept rows of
+        no class, NaN included) and nonfinite (kept rows with y not finite).  Raises ``ValueError`` for bad arguments."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        m = np.ascontiguousarray(means, dtype=np.float64)
+        if m.shape != (cl.size, d):
+            raise ValueError(f"means must be ({cl.size}, {d}), got {m.shape}")
+        scatters = np.empty((cl.size, d, d), dtype=np.float64)
+        nk = np.empty(cl.size, dtype=np.float64)
+        counts = np.empty(3, dtype=np.float64)
+        rc = load().b2_class_scatters(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data, cl.size,
+                                      m.ctypes.data, scatters.ctypes.data, nk.ctypes.data, counts.ctypes.data)
+        _check_args(rc, "b2_class_scatters")
+        return {"scatters": scatters, "class_counts": nk, "kept": float(counts[0]), "unmatched": float(counts[1]),
+                "nonfinite": float(counts[2])}
+
+    def qda_decision(self, X, means, transforms, offsets, classes, y=None, *, row_mask=None, mask_keep: int = 1,
+                     decision: bool = False, label: bool = False, diff: bool = False) -> dict:
+        """The quadratic discriminant per row and class in one fp64 pass (b2_qda_decision):
+        d_k = -1/2 |(x - m_k) W_k|^2 + c_k with ``means`` (K, d), ``transforms`` (K, d, d) and ``offsets`` (K,).  The
+        wanted ones of decision ((n, K) fp64), label (classes[argmax_k d_k], the first largest; fp32) and diff (d_1 - d_0,
+        two classes only; fp64) -- ndarrays for host rows, DeviceArrays for device rows -- and, with y, kept and correct
+        (kept rows whose y equals their label)."""
+        ptr, xdt, mk, n, d, yp, mp = _row_args(X, y, row_mask)
+        cl = self._f32_classes(classes, np.size(classes))
+        k = cl.size
+        m = np.ascontiguousarray(means, dtype=np.float64)
+        w = np.ascontiguousarray(transforms, dtype=np.float64)
+        c = np.ascontiguousarray(offsets, dtype=np.float64).ravel()
+        if m.shape != (k, d) or w.shape != (k, d, d) or c.size != k:
+            raise ValueError(f"means, transforms and offsets must be ({k}, {d}), ({k}, {d}, {d}) and ({k},), got "
+                             f"{m.shape}, {w.shape} and {c.shape}")
+        out, ptrs = {}, {}
+        for name, want, shape, kind in (("decision", decision, (n, k), "f64"), ("label", label, (n,), "f32"),
+                                        ("diff", diff, (n,), "f64")):
+            a, ptrs[name] = self._out(mk, shape, kind, want)
+            if want:
+                out[name] = a
+        counts = np.zeros(2, dtype=np.float64) if y is not None else None
+        rc = load().b2_qda_decision(self._h, ptr, xdt, yp, n, d, d, mk, mp, int(mask_keep), cl.ctypes.data, k,
+                                    m.ctypes.data, w.ctypes.data, c.ctypes.data, ptrs["decision"], ptrs["label"],
+                                    ptrs["diff"], counts.ctypes.data if counts is not None else None)
+        _check_args(rc, "b2_qda_decision")
+        if counts is not None:
+            out["kept"], out["correct"] = float(counts[0]), float(counts[1])
+        return out
 
     def solve_classes(self, class_sums, alpha: float = 1.0, fit_intercept: bool = True,
                       n_classes: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:

@@ -480,7 +480,8 @@ int b2_ctx_destroy(b2_ctx* ctx) {
                   ctx->coef_dev, ctx->solve_out, ctx->stage_x[0], ctx->stage_x[1], ctx->stage_y[0], ctx->stage_y[1],
                   ctx->stage_m[0], ctx->stage_m[1], ctx->row_out[0], ctx->row_out[1], ctx->tc_sync, ctx->synth_count,
                   ctx->grad_part, ctx->refine, ctx->loo, ctx->loo_part, ctx->enet, ctx->folds, ctx->fold_range, ctx->glm, ctx->glm_part,
-                  ctx->cls, ctx->loo_cls, ctx->mn_op, ctx->mn_sum, ctx->mn_part, ctx->disc, ctx->disc_part};
+                  ctx->cls, ctx->loo_cls, ctx->mn_op, ctx->mn_sum, ctx->mn_part, ctx->disc, ctx->disc_part,
+                  ctx->qda, ctx->qda_hd, ctx->qda_scratch, ctx->qda_part};
   for (void* p : bufs) if (p != nullptr) cudaFree(p);
   if (ctx->solve_host != nullptr) cudaFreeHost(ctx->solve_host);
   if (ctx->xchg_status_host != nullptr) cudaFreeHost(ctx->xchg_status_host);
@@ -1782,6 +1783,148 @@ int b2_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, const float* y, in
   for (int i = 0; i < d; ++i)
     for (int j = i; j < d; ++j)        // the upper triangle, mirrored
       scatter_out[(size_t)i * d + j] = scatter_out[(size_t)j * d + i] = h[kDaHead + (size_t)i * kMaxD + j];
+  return B2_OK;
+}
+
+// ---- QuadraticDiscriminantAnalysis (DESIGN.md section 17) -----------------------------------------------------------
+// The operands and sums (ctx->qda), the int header (ctx->qda_hd) and the scratch, allocated by the first call and freed
+// with the context: no other pass's buffers are touched.  The classes and means (both entry points) into ctx->qda.
+static int qda_setup(b2_ctx* ctx, const char* what, const void* X, int x_dtype, int64_t n_rows, int d, int64_t ldx,
+                     int mem_kind, const float* classes, int n_classes, const double* means, std::vector<double>& op) {
+  if (int r = check_shape(x_dtype, n_rows, d, ldx, mem_kind)) return r;
+  if (n_rows > 0 && X == nullptr) { set_error("X is null"); return B2_E_ARG; }
+  if (means == nullptr) { set_error("means is null"); return B2_E_ARG; }
+  if (int r = check_classes(classes, n_classes)) return r;
+  for (int k = 0; k < n_classes; ++k) {
+    op[kQdClasses + k] = classes[k];
+    for (int j = 0; j < d; ++j) {
+      const double m = means[(size_t)k * d + j];
+      if (!isfinite(m)) { set_error("means[%d][%d]=%g is not finite", k, j, m); return B2_E_ARG; }
+      op[kQdMeans + k * kMaxD + j] = m;
+    }
+  }
+  if (ctx->n_ranks > 1) {
+    set_error("%s runs on one rank only (its sums are not exchanged between ranks)", what);
+    return B2_E_UNSUPPORTED;
+  }
+  if (ctx->qda == nullptr) {
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->qda), sizeof(double) * kQdDoubles));
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->qda_hd), sizeof(int) * (kQdHdItems + 3 * (size_t)qda_max_items(ctx))));
+    B2_CUDA(cudaMalloc(&ctx->qda_scratch, kQdScratchBytes));
+  }
+  B2_CUDA(cudaMemcpyAsync(ctx->qda, op.data(), sizeof(double) * op.size(), cudaMemcpyHostToDevice, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));     // op is on the caller's stack
+  return B2_OK;
+}
+
+int b2_class_scatters(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                      int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                      const double* means, double* scatters_out, double* class_counts_out, double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (n_rows > 0 && y == nullptr) { set_error("y is null"); return B2_E_ARG; }
+  if (scatters_out == nullptr || class_counts_out == nullptr || counts_out == nullptr) {
+    set_error("scatters_out / class_counts_out / counts_out is null");
+    return B2_E_ARG;
+  }
+  std::vector<double> op(kQdConst, 0.0);                 // kQdClasses, kQdMeans
+  if (int r = qda_setup(ctx, "b2_class_scatters", X, x_dtype, n_rows, d, ldx, mem_kind, classes, n_classes, means, op))
+    return r;
+  if (ctx->qda_part == nullptr)
+    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&ctx->qda_part),
+                       sizeof(double) * (size_t)qda_max_items(ctx) * kMaxD * kMaxD));
+  // device rows in spans of at most kQdSpan rows (host blocks are shorter), the sums accumulating across them
+  if (int r = row_pass(ctx, X, x_dtype, y, n_rows, d, ldx, mem_kind, row_mask, [&](const RowSpan& s, void*, void*, void*) {
+        const int es = x_dtype == B2_F32 ? 4 : 2;
+        for (int64_t r0 = 0; r0 < s.rows || (r0 == 0 && s.first); r0 += kQdSpan) {
+          const int64_t rows = s.rows - r0 < kQdSpan ? s.rows - r0 : kQdSpan;
+          const void* Xs = static_cast<const char*>(s.X) + (size_t)r0 * s.ldx * es;
+          if (int rc = launch_class_scatters(ctx, Xs, x_dtype, rows, d, s.ldx, s.y != nullptr ? s.y + r0 : nullptr,
+                                             s.mask != nullptr ? s.mask + r0 : nullptr, mask_keep, n_classes,
+                                             s.first && r0 == 0))
+            return rc;
+          if (rows == 0) break;
+        }
+        return (int)B2_OK;
+      }))
+    return r;
+  std::vector<double> h((size_t)n_classes * kMaxD * kMaxD);
+  B2_CUDA(cudaMemcpyAsync(h.data(), ctx->qda + kQdSums, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  double c[kMaxClasses + 3];
+  B2_CUDA(cudaMemcpyAsync(c, ctx->qda + kQdCounts, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (int k = 0; k < n_classes; ++k) {
+    class_counts_out[k] = c[k];
+    const double* src = h.data() + (size_t)k * kMaxD * kMaxD;
+    double* dst = scatters_out + (size_t)k * d * d;
+    for (int i = 0; i < d; ++i)
+      for (int j = i; j < d; ++j)        // the upper triangle, mirrored
+        dst[(size_t)i * d + j] = dst[(size_t)j * d + i] = src[(size_t)i * kMaxD + j];
+  }
+  memcpy(counts_out, c + kMaxClasses, sizeof(double) * 3);
+  return B2_OK;
+}
+
+int b2_qda_decision(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                    int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                    const double* means, const double* transforms, const double* offsets, double* decision_out,
+                    float* label_out, double* diff_out, double* counts_out) {
+  if (int r = use_device(ctx)) return r;
+  if (transforms == nullptr || offsets == nullptr) { set_error("transforms / offsets is null"); return B2_E_ARG; }
+  if (decision_out == nullptr && label_out == nullptr && diff_out == nullptr && counts_out == nullptr) {
+    set_error("decision_out, label_out, diff_out and counts_out are all null");
+    return B2_E_ARG;
+  }
+  if (n_rows > 0 && counts_out != nullptr && y == nullptr) { set_error("counts_out needs y"); return B2_E_ARG; }
+  if (diff_out != nullptr && n_classes != 2) { set_error("diff_out needs two classes (got %d)", n_classes); return B2_E_ARG; }
+  if (n_classes < 2 || n_classes > kMaxClasses) return check_classes(classes, n_classes);
+  std::vector<double> op(kQdW + (size_t)n_classes * d * d, 0.0);   // kQdClasses, kQdMeans, kQdConst, kQdW (pitch d)
+  for (int k = 0; k < n_classes; ++k) {
+    if (!isfinite(offsets[k])) { set_error("offsets[%d]=%g is not finite", k, offsets[k]); return B2_E_ARG; }
+    op[kQdConst + k] = offsets[k];
+  }
+  for (size_t e = 0; e < (size_t)n_classes * d * d; ++e) {
+    if (!isfinite(transforms[e])) { set_error("transforms[%zu]=%g is not finite", e, transforms[e]); return B2_E_ARG; }
+    op[kQdW + e] = transforms[e];
+  }
+  if (int r = qda_setup(ctx, "b2_qda_decision", X, x_dtype, n_rows, d, ldx, mem_kind, classes, n_classes, means, op))
+    return r;
+  if (counts_out != nullptr)
+    B2_CUDA(cudaMemsetAsync(ctx->qda_hd + kQdHdCorrect, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  // y and the mask only count: every row gets its decision and label
+  const float* yc = counts_out != nullptr ? y : nullptr;
+  const uint8_t* mc = counts_out != nullptr ? row_mask : nullptr;
+  if (int r = row_pass(
+          ctx, X, x_dtype, yc, n_rows, d, ldx, mem_kind, mc,
+          [&](const RowSpan& s, void* dec, void* lab, void* dif) {
+            if (dec != nullptr)
+              return launch_qda_decision(ctx, s.X, x_dtype, s.rows, d, s.ldx, s.y, s.mask, mask_keep, n_classes,
+                                         static_cast<double*>(dec), static_cast<float*>(lab), static_cast<double*>(dif));
+            // no decisions wanted: they go through the scratch, in parts that fit it
+            const int64_t part = (int64_t)(kQdScratchBytes / sizeof(double)) / n_classes;
+            const int es = x_dtype == B2_F32 ? 4 : 2;
+            for (int64_t r0 = 0; r0 < s.rows; r0 += part) {
+              const int64_t rows = s.rows - r0 < part ? s.rows - r0 : part;
+              if (int rc = launch_qda_decision(ctx, static_cast<const char*>(s.X) + (size_t)r0 * s.ldx * es, x_dtype,
+                                               rows, d, s.ldx, s.y != nullptr ? s.y + r0 : nullptr,
+                                               s.mask != nullptr ? s.mask + r0 : nullptr, mask_keep, n_classes,
+                                               static_cast<double*>(ctx->qda_scratch),
+                                               lab != nullptr ? static_cast<float*>(lab) + r0 : nullptr,
+                                               dif != nullptr ? static_cast<double*>(dif) + r0 : nullptr))
+                return rc;
+            }
+            return (int)B2_OK;
+          },
+          RowOut{decision_out, sizeof(double) * n_classes}, RowOut{label_out, sizeof(float)},
+          RowOut{diff_out, sizeof(double)}))
+    return r;
+  if (counts_out != nullptr) {
+    unsigned long long c[2];
+    B2_CUDA(cudaMemcpyAsync(c, ctx->qda_hd + kQdHdCorrect, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
+    B2_CUDA(cudaStreamSynchronize(ctx->stream));
+    counts_out[0] = (double)c[0];
+    counts_out[1] = (double)c[1];
+  }
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
 }
 

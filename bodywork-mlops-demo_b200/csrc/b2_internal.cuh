@@ -206,6 +206,37 @@ constexpr int kDaMeans = 2 * kMaxClasses;
 constexpr int kDaSums = kDaMeans + kMaxClasses * kMaxD;
 constexpr int kDaDoubles = kDaSums + kDaPart;
 
+// ---- QuadraticDiscriminantAnalysis (qda.cu; DESIGN.md section 17) ---------------------------------------------------
+// doubles of ctx->qda: the sorted classes, the class means [kMaxClasses][kMaxD], the offsets c_k and the transforms W_k
+// ([K][d][d], pitch d) of the decision pass, then the reduced scatters [kMaxClasses][kMaxD][kMaxD] (upper triangle at
+// i kMaxD + j) and the counts (rows per class [kMaxClasses], then kept rows, kept rows of no class, kept rows with y not
+// finite).
+constexpr int kQdClasses = 0;
+constexpr int kQdMeans = kMaxClasses;
+constexpr int kQdConst = kQdMeans + kMaxClasses * kMaxD;
+constexpr int kQdW = kQdConst + kMaxClasses;
+constexpr int kQdSums = kQdW + kMaxClasses * kMaxD * kMaxD;
+constexpr int kQdCounts = kQdSums + kMaxClasses * kMaxD * kMaxD;
+constexpr int kQdDoubles = kQdCounts + kMaxClasses + 8;
+// rows of the class-order step: a span (its int32 indices fill ctx->qda_scratch, 64 MB), a chunk of its counts
+constexpr int64_t kQdSpan = 1 << 24;
+constexpr int kQdChunk = 8192;
+constexpr int kQdMaxChunks = (int)(kQdSpan / kQdChunk);
+constexpr size_t kQdScratchBytes = sizeof(int) * (size_t)kQdSpan;   // also the decisions of label-only calls
+constexpr int kQdItemsPerSm = 2;                                    // work items of the scatter pass per SM
+// ints of ctx->qda_hd: the decision pass's kept and correct rows (two unsigned long long), the span's work items and
+// counts (written by order_scan_kernel), the chunk counts [kQdMaxChunks][kMaxClasses + 3] and the items [n][3]
+// (class, begin, end) for qda_max_items
+constexpr int kQdHdCorrect = 0;
+constexpr int kQdHdNItems = 4;
+constexpr int kQdHdCounts = 5;
+constexpr int kQdHdStart = 8;                                        // [kMaxClasses + 1] class k's indices [start_k, start_k+1)
+constexpr int kQdHdFirstItem = kQdHdStart + kMaxClasses + 1;         // [kMaxClasses + 1] class k's items [first_k, first_k+1)
+constexpr int kQdHdCnt = 80;
+constexpr int kQdHdItems = kQdHdCnt + kQdMaxChunks * (kMaxClasses + 3);
+static_assert(kQdHdFirstItem + kMaxClasses + 1 <= kQdHdCnt, "qda header");
+int qda_max_items(const b2_ctx* ctx);
+
 // ---- cross-validation folds (folds.cu) ------------------------------------------------------------------------------
 constexpr int kMaxFolds = 254;        // fold ids are bytes; 255 marks a dropped row
 // first and last row of every fold of fold ids in device memory: range[2 k] = n - first, range[2 k + 1] = last + 1
@@ -304,6 +335,13 @@ struct b2_ctx {
   // [sm_count][kDaPart], allocated by the first call
   double* disc = nullptr;
   double* disc_part = nullptr;
+  // QuadraticDiscriminantAnalysis: operands and sums (b2::kQd*), the int header (b2::kQdHd*), the scratch of the class
+  // order and of label-only decisions, all allocated by the first call; the scatter pass's per-item partials
+  // [qda_max_items][kMaxD * kMaxD] by the first scatter call
+  double* qda = nullptr;
+  int* qda_hd = nullptr;
+  void* qda_scratch = nullptr;
+  double* qda_part = nullptr;
   double* coef_host = nullptr;         // pinned [2][kMaxD + 1]: upload slots of b2_score's coefficients
   cudaEvent_t ev_coef[2] = {nullptr, nullptr};
   int coef_slot = 0;
@@ -530,6 +568,14 @@ int launch_svm(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_
 // the per-CTA sums into ctx->disc + kDaSums (`first_block` overwrites, otherwise adds)
 int launch_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
                          const uint8_t* mask, int keep, int n_classes, bool first_block);
+// the per-class scatters of the rows [0, n) (n <= kQdSpan) at the classes and means of ctx->qda: the class order, the
+// work items and the ordered reduce into ctx->qda + kQdSums and kQdCounts (`first_block` overwrites, otherwise adds)
+int launch_class_scatters(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                          const uint8_t* mask, int keep, int n_classes, bool first_block);
+// the QDA decisions of the rows [0, n) at the operands of ctx->qda into decision [n][n_classes] (device), then, each if
+// not null, the labels, d_1 - d_0 (two classes) and, with y, the kept and correct rows added to ctx->qda_hd
+int launch_qda_decision(b2_ctx* ctx, const void* X, int x_dtype, int64_t n, int d, int64_t ldx, const float* y,
+                        const uint8_t* mask, int keep, int n_classes, double* decision, float* label, double* diff);
 // W and b of the ridge classifier from the resident S and the class sums at ctx->cls + kClsSums (one launch)
 int launch_solve_classes(b2_ctx* ctx, double alpha, int fit_intercept, int n_classes);
 int launch_p2p_allreduce(b2_ctx* ctx);

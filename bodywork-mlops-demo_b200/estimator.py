@@ -2685,3 +2685,225 @@ class B200LinearDiscriminantAnalysis(B200RidgeClassifier):
 
     def __repr__(self) -> str:
         return f"B200LinearDiscriminantAnalysis(solver={self.solver!r})"
+
+
+# ---- QuadraticDiscriminantAnalysis: every class's scatter in one fp64 pass, K quadratic forms per row (DESIGN.md
+# section 17) -------------------------------------------------------------------------------------------------------
+_QDA_SOLVERS = ("svd", "eigen")
+
+
+def _qda_class(scatter: np.ndarray, nk: int, solver: str, shrinkage, reg_param: float):
+    """(scalings, rotations, covariance) of one class from its scatter S_k, as scikit-learn's ``_solve_svd`` and
+    ``_solve_eigen`` compute them from its rows: 'svd' takes the eigenvalues and eigenvectors of S_k / (n_k - 1) for the
+    squared singular values and right singular vectors of the centred rows (descending), 'eigen' those of the (shrunk)
+    biased covariance S_k / n_k."""
+    import scipy.linalg
+    if solver == "svd":
+        lam, V = np.linalg.eigh(scatter / (nk - 1))
+        scaling = np.maximum(lam[::-1], 0.0)
+        scaling = (1 - reg_param) * scaling + reg_param
+        rotation = V[:, ::-1]
+        return scaling, rotation, scaling * rotation @ rotation.T
+    cov = _shrunk(scatter / nk, shrinkage)
+    scaling, rotation = scipy.linalg.eigh(cov)
+    order = np.argsort(scaling)[::-1]
+    return scaling[order], rotation[:, order], cov
+
+
+class B200QuadraticDiscriminantAnalysis(B200RidgeClassifier):
+    """``sklearn.discriminant_analysis.QuadraticDiscriminantAnalysis`` for 2 to ``native.MAX_CLASSES`` classes, fitted
+    on the H100.  A fit is the class counts and means (one class-sum pass) and every class's own scatter
+    S_k = sum over its rows of (x - m_k)(x - m_k)^T from one fp64 tensor-core pass that reads the rows once, in class
+    order (``class_scatters``).  The solvers are scikit-learn's, restated on these K D x D matrices on the host: 'svd'
+    takes the eigendecomposition of S_k / (n_k - 1) for the SVD of the class's centred rows, 'eigen' that of the (shrunk)
+    biased covariance S_k / n_k.  The columns of ``rotations_`` equal scikit-learn's up to their sign; nothing else
+    depends on those signs.
+
+    ``decision_function``, ``predict`` and ``score`` are one fp64 pass each (``qda_decision``: the K quadratic forms
+    -1/2 |(x - m_k) W_k|^2 + c_k per row on the tensor core, W_k = rotations_[k] scalings_[k]^-1/2).  ``predict_proba``
+    is scikit-learn's normalisation of the decisions, on the device for device rows.  Labels and their refusals are
+    ``B200RidgeClassifier``'s.
+
+    Refused: shrinkage='auto' (Ledoit-Wolf needs each class's fourth moments), a covariance_estimator, shrinkage with the
+    'svd' solver, sample_weight, priors whose length is not the class count, more than ``native.MAX_CLASSES`` classes,
+    continuous, multilabel or non-finite y, and non-finite X.  One class, a class of one row and a class covariance that
+    is not full rank raise scikit-learn's errors."""
+    _sk_module = "discriminant_analysis"
+    _sk_name = "QuadraticDiscriminantAnalysis"
+    _sk_attrs = ("classes_", "means_", "priors_", "n_features_in_")
+    _label_who = "B200QuadraticDiscriminantAnalysis"
+
+    def __init__(self, *, solver: str = "svd", shrinkage=None, priors=None, reg_param: float = 0.0,
+                 store_covariance: bool = False, tol: float = 1e-4, covariance_estimator=None,
+                 ctx: Optional[native.Context] = None):
+        self.solver = solver
+        self.shrinkage = shrinkage
+        self.priors = priors
+        self.reg_param = reg_param
+        self.store_covariance = store_covariance
+        self.tol = tol
+        self.covariance_estimator = covariance_estimator
+        self._ctx = ctx
+
+    @staticmethod
+    def _real(v) -> bool:
+        return not isinstance(v, (bool, str)) and isinstance(v, (int, float, np.integer, np.floating))
+
+    def _check_params(self):
+        who = "B200QuadraticDiscriminantAnalysis"
+        if self.solver not in _QDA_SOLVERS:
+            raise ValueError(f"The 'solver' parameter of {who} must be a str among {{'eigen', 'svd'}}. Got "
+                             f"{self.solver!r} instead.")
+        s = self.shrinkage
+        if isinstance(s, str) and s == "auto":
+            raise ValueError(f"shrinkage='auto' is not supported by {who}: the Ledoit-Wolf estimate needs each class's "
+                             "sum of |z|^4 over its standardised rows, a second gathered pass; use shrinkage=None or a "
+                             "float")
+        if s is not None and (not self._real(s) or not 0 <= s <= 1):
+            raise ValueError(f"The 'shrinkage' parameter of {who} must be a str among {{'auto'}}, a float in the range "
+                             f"[0, 1] or None. Got {s!r} instead.")
+        if not self._real(self.reg_param) or not 0 <= self.reg_param <= 1:
+            raise ValueError(f"The 'reg_param' parameter of {who} must be a float in the range [0, 1]. Got "
+                             f"{self.reg_param!r} instead.")
+        if not self._real(self.tol) or not 0 <= self.tol < np.inf:
+            raise ValueError(f"The 'tol' parameter of {who} must be a float in the range [0.0, inf). Got {self.tol!r} "
+                             "instead.")
+        if self.covariance_estimator is not None:
+            raise ValueError(f"covariance_estimator is not supported by {who}: each class's covariance is the "
+                             "empirical one (with shrinkage=None or a float)")
+        if self.solver == "svd" and s is not None:
+            raise NotImplementedError(f"shrinkage not supported with 'svd' solver. ({who})")
+
+    @classmethod
+    def _check_class_count(cls, classes, more: bool) -> None:
+        if more:
+            raise ValueError(f"{cls._label_who} fits at most {native.MAX_CLASSES} classes, y has more")
+        if classes.size < 2:
+            raise ValueError(f"The number of classes has to be greater than one. Got {classes.size} class.")
+
+    def fit(self, X, y, row_mask=None, mask_keep: int = 1,
+            sample_weight=None) -> "B200QuadraticDiscriminantAnalysis":
+        """X: (n, D) host array (any float dtype; staged as fp32) or a ``DeviceArray`` (f32 / bf16); ``row_mask``
+        (uint8 per row) restricts the fit to rows equal to ``mask_keep``.  Sets classes_, means_, priors_, scalings_ and
+        rotations_ (lists of K), covariance_ (with store_covariance) and n_features_in_."""
+        _refuse_sample_weight(sample_weight, "B200QuadraticDiscriminantAnalysis")
+        self._check_params()
+        ctx = self.ctx
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=True) as (X, y, row_mask, labels, classes):
+            d, K = X.shape[1], classes.size
+            if self.priors is not None and np.size(self.priors) != K:
+                raise ValueError(f"priors has {np.size(self.priors)} entries, but y holds {K} classes "
+                                 "(B200QuadraticDiscriminantAnalysis)")
+            cs = ctx.class_sums(X, y, labels, None, row_mask=row_mask, mask_keep=mask_keep)
+            nk, n = cs["sums"][:, d], cs["kept"]
+            if cs["unmatched"] > 0 or cs["nonfinite"] > 0 or nk.sum() != n or np.any(nk == 0):
+                raise RuntimeError("the class-sum pass saw other labels than the label check")
+            _check_finite(cs["sums"])
+            means = cs["sums"][:, :d] / nk[:, None]
+            sc = ctx.class_scatters(X, y, labels, means, row_mask=row_mask, mask_keep=mask_keep)
+            if sc["kept"] != n or sc["unmatched"] > 0 or sc["nonfinite"] > 0 or np.any(sc["class_counts"] != nk):
+                raise RuntimeError("the scatter pass saw other labels than the class-sum pass")
+            _check_finite(sc["scatters"])
+        priors = nk / float(n) if self.priors is None else np.array(self.priors)
+        cov, scalings, rotations = [], [], []
+        for k, label in enumerate(classes):
+            if nk[k] == 1:
+                raise ValueError(f"y has only 1 sample in class {label!s}, covariance is ill defined.")
+            n_k = int(nk[k])
+            # scikit-learn's svd of fewer rows than features has only n_k singular values, so its rank check fails
+            # whatever reg_param is; the eigendecomposition has d values and cannot decide that
+            small = self.solver == "svd" and n_k < d
+            scaling, rotation, cov_k = (None, None, None) if small else _qda_class(
+                sc["scatters"][k], n_k, self.solver, self.shrinkage, float(self.reg_param))
+            if small or np.sum(scaling > self.tol) < d:
+                if self.solver == "svd" and n_k <= d:
+                    raise np.linalg.LinAlgError(
+                        f"The covariance matrix of class {label} is not full rank. When using `solver='svd'` the "
+                        f"number of samples in each class should be more than the number of features, but class "
+                        f"{label} has {n_k} samples and {d} features. Try using `solver='eigen'` and setting the "
+                        f"parameter `shrinkage` for regularization.")
+                param = "shrinkage" if self.solver == "eigen" else "reg_param"
+                raise np.linalg.LinAlgError(f"The covariance matrix of class {label} is not full rank. Increase the "
+                                            f"value of `{param}` to reduce the collinearity.")
+            cov.append(cov_k)
+            scalings.append(scaling)
+            rotations.append(rotation)
+        self.__dict__.pop("covariance_", None)
+        if self.store_covariance:
+            self.covariance_ = cov
+        self.classes_, self.means_, self.priors_ = classes, means, priors
+        self.scalings_, self.rotations_ = scalings, rotations
+        self.n_features_in_ = int(d)
+        return self
+
+    def _operands(self):
+        """(means, W (K, d, d), c (K,)) of the decisions d_k = -1/2 |(x - m_k) W_k|^2 + c_k"""
+        W = np.stack([R * (S ** (-0.5)) for R, S in zip(self.rotations_, self.scalings_)])
+        c = -0.5 * np.array([np.sum(np.log(S)) for S in self.scalings_]) + np.log(self.priors_)
+        return self.means_, W, c
+
+    def _decide(self, X, y=None, **kw):
+        """one qda_decision pass; host rows take the class indices as labels"""
+        labels = self._fp32_classes(self.classes_) if isinstance(X, native.DeviceArray) else \
+            np.arange(self.classes_.size, dtype=np.float32)
+        return self.ctx.qda_decision(X, *self._operands(), labels, y, **kw)
+
+    def decision_function(self, X):
+        """d_1 - d_0 ((n,)) for two classes, the (n, K) decisions for more, in fp64: float64 for host rows, an f64
+        ``DeviceArray`` for device rows."""
+        X = self._checked_rows(X)
+        if self.classes_.size == 2:
+            return self._decide(X, diff=True)["diff"]
+        return self._decide(X, decision=True)["decision"]
+
+    def predict(self, X):
+        """classes_ of the largest decision (the first of equal ones): an ndarray of classes_' dtype for host rows, an
+        f32 ``DeviceArray`` for device rows (classes_ must then be fp32 values)."""
+        labels = self._decide(self._checked_rows(X), label=True)["label"]
+        if isinstance(labels, native.DeviceArray):
+            return labels
+        return self.classes_[labels.astype(np.intp)]
+
+    def score(self, X, y, row_mask=None, mask_keep: int = 1):
+        """Accuracy over the kept rows (labels outside classes_ count as wrong): the counts of one decision pass."""
+        with self._stage_targets(X, y, row_mask, mask_keep, fitting=False) as (X, y, row_mask, labels, _):
+            s = self.ctx.qda_decision(self._checked_rows(X), *self._operands(), labels, y, row_mask=row_mask,
+                                      mask_keep=mask_keep)
+        if s["kept"] == 0:
+            raise _too_few_rows((0,))
+        return float(s["correct"] / s["kept"])
+
+    def predict_proba(self, X):
+        """The class probabilities, (n, K) fp64: scikit-learn's exp(d - max - log sum exp(d - max)) of the decisions for
+        host rows, ``softmax_rows`` in place on the device for device rows (an f64 ``DeviceArray``)."""
+        X = self._checked_rows(X)
+        dec = self._decide(X, decision=True)["decision"]
+        if isinstance(dec, native.DeviceArray):
+            self.ctx.softmax_rows(dec)
+            return dec
+        return np.exp(self._log_proba(dec))
+
+    @staticmethod
+    def _log_proba(dec: np.ndarray) -> np.ndarray:
+        ll = dec - dec.max(axis=1)[:, np.newaxis]
+        return ll - np.log(np.exp(ll).sum(axis=1)[:, np.newaxis])
+
+    def predict_log_proba(self, X):
+        """The log class probabilities of host rows, scikit-learn's formula on the decisions."""
+        if isinstance(X, native.DeviceArray):
+            raise ValueError("predict_log_proba takes host rows (predict_proba returns device probabilities)")
+        return self._log_proba(self._decide(self._checked_rows(X), decision=True)["decision"])
+
+    def _sk_params(self) -> dict:
+        return dict(solver=self.solver, shrinkage=self.shrinkage, priors=self.priors, reg_param=self.reg_param,
+                    store_covariance=self.store_covariance, tol=self.tol)
+
+    def _sk_prepare(self, reg) -> None:
+        """the per-class lists"""
+        reg.scalings_ = [s.copy() for s in self.scalings_]
+        reg.rotations_ = [r.copy() for r in self.rotations_]
+        if "covariance_" in self.__dict__:
+            reg.covariance_ = [c.copy() for c in self.covariance_]
+
+    def __repr__(self) -> str:
+        return f"B200QuadraticDiscriminantAnalysis(solver={self.solver!r})"

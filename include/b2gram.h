@@ -386,6 +386,33 @@ int b2_class_sums(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64
 int b2_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
                      int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
                      const double* means, const double* weights, double* scatter_out, double* counts_out);
+/* b2_class_scatters (QuadraticDiscriminantAnalysis, DESIGN.md section 17): every class's own scatter of the kept rows in
+ * one fp64 pass that reads the rows once, in class order.  scatters_out (host, n_classes x d x d, both triangles, exactly
+ * symmetric): block k = sum over the kept rows of class k of (x - m_k)(x - m_k)^T, x converted exactly and u = x - m_k
+ * formed in fp64; a class without kept rows gets zeros, the rows of no class add nothing.  classes and y as
+ * b2_class_sums; means (host, n_classes x d) the class means m_k.  class_counts_out (host, n_classes): the kept rows of
+ * each class; counts_out (host, 3): [0] kept rows [1] kept rows whose y is no class (NaN included) [2] kept rows whose y
+ * is not finite.  The work is cut by class so that skewed classes keep every SM busy; on the fp64 tensor core, the upper
+ * 16 x 16 blocks of each product; sums in a fixed order: repeated calls are bit-identical.  Device scratch: 64 MB of
+ * row indices plus qda_max_items x 128 KB of partials, held by the context.  B2_E_ARG: bad shapes, n_classes outside
+ * 2..B2_MAX_CLASSES, classes that are not finite and strictly ascending, null means or outputs, non-finite means;
+ * B2_E_UNSUPPORTED with more than one rank.  n_rows = 0 (or no kept row) is no error: the scatters and counts are 0. */
+int b2_class_scatters(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                      int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                      const double* means, double* scatters_out, double* class_counts_out, double* counts_out);
+/* b2_qda_decision (QuadraticDiscriminantAnalysis, DESIGN.md section 17): per row and class in fp64,
+ * d_k = -1/2 |(x - m_k) W_k|^2 + c_k, u = x - m_k formed in fp64 and u W_k on the fp64 tensor core.  means (host,
+ * n_classes x d) m_k, transforms (host, n_classes x d x d, W_k row-major), offsets (host, n_classes) c_k.  Outputs where
+ * the rows live, each optional (not all null): decision_out (n_rows x n_classes), label_out (fp32: classes[argmax_k
+ * d_k], the first largest), diff_out (n_rows, two classes only: d_1 - d_0); counts_out (host, 2; needs y): [0] kept rows
+ * [1] kept rows whose y equals their label.  Every row gets its decision and label: y and the mask only count.  Sums in
+ * a fixed order: repeated calls are bit-identical.  B2_E_ARG: bad shapes, n_classes outside 2..B2_MAX_CLASSES, classes
+ * that are not finite and strictly ascending, null means, transforms, offsets or outputs, non-finite means, transforms or
+ * offsets, diff_out with more than two classes; B2_E_UNSUPPORTED with more than one rank. */
+int b2_qda_decision(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int64_t n_rows, int d, int64_t ldx,
+                    int mem_kind, const uint8_t* row_mask, int mask_keep, const float* classes, int n_classes,
+                    const double* means, const double* transforms, const double* offsets, double* decision_out,
+                    float* label_out, double* diff_out, double* counts_out);
 /* b2_solve_classes: the model of the resident S (every kept row of some class) and the class sums (host, n_classes x
  * (d + 1) as b2_class_sums returns them, at any center; NULL: the sums of the last b2_class_sums).  T = 1 for two
  * classes, else n_classes: coef_out (host, T x d) and intercept_out (host, T; ybar_t - mean.w_t, 0 without
