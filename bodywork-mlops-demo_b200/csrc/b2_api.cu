@@ -1503,6 +1503,13 @@ static int glm_rows(b2_ctx* ctx, const void* X, int x_dtype, const float* y, int
   });
 }
 
+// The full symmetric n x n matrix dst from the upper triangle of src (row pitch src_pitch): the upper-block sums of
+// b2_dmma.cuh
+static void unpack_upper(const double* src, size_t src_pitch, int n, double* dst) {
+  for (int i = 0; i < n; ++i)
+    for (int j = i; j < n; ++j) dst[(size_t)i * n + j] = dst[(size_t)j * n + i] = src[i * src_pitch + j];
+}
+
 // The sums of the last pass (and the mirrored Hessian when hess_out is not null) to the host: [0, 7) and the gradient
 // [7, 8 + d), then the extra scalars at 8 + d
 static int fetch_glm_sums(b2_ctx* ctx, int d, int n_extra, double* sums_out, double* hess_out) {
@@ -1513,10 +1520,7 @@ static int fetch_glm_sums(b2_ctx* ctx, int d, int n_extra, double* sums_out, dou
   memcpy(sums_out, h.data(), sizeof(double) * 7);
   memcpy(sums_out + 7, h.data() + kGlmGrad, sizeof(double) * d1);
   if (n_extra > 0) sums_out[8 + d] = h[kGlmCorrect];
-  if (hess_out != nullptr)
-    for (int i = 0; i < d1; ++i)
-      for (int j = i; j < d1; ++j)       // the upper triangle, mirrored
-        hess_out[(size_t)i * d1 + j] = hess_out[(size_t)j * d1 + i] = h[kGlmHess + (size_t)i * kGlmHp + j];
+  if (hess_out != nullptr) unpack_upper(h.data() + kGlmHess, kGlmHp, d1, hess_out);
   return B2_OK;
 }
 
@@ -1780,9 +1784,7 @@ int b2_class_scatter(b2_ctx* ctx, const void* X, int x_dtype, const float* y, in
   B2_CUDA(cudaMemcpyAsync(h.data(), ctx->disc + kDaSums, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(counts_out, h.data(), sizeof(double) * 3);
-  for (int i = 0; i < d; ++i)
-    for (int j = i; j < d; ++j)        // the upper triangle, mirrored
-      scatter_out[(size_t)i * d + j] = scatter_out[(size_t)j * d + i] = h[kDaHead + (size_t)i * kMaxD + j];
+  unpack_upper(h.data() + kDaHead, kMaxD, d, scatter_out);
   return B2_OK;
 }
 
@@ -1854,11 +1856,7 @@ int b2_class_scatters(b2_ctx* ctx, const void* X, int x_dtype, const float* y, i
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   for (int k = 0; k < n_classes; ++k) {
     class_counts_out[k] = c[k];
-    const double* src = h.data() + (size_t)k * kMaxD * kMaxD;
-    double* dst = scatters_out + (size_t)k * d * d;
-    for (int i = 0; i < d; ++i)
-      for (int j = i; j < d; ++j)        // the upper triangle, mirrored
-        dst[(size_t)i * d + j] = dst[(size_t)j * d + i] = src[(size_t)i * kMaxD + j];
+    unpack_upper(h.data() + (size_t)k * kMaxD * kMaxD, kMaxD, d, scatters_out + (size_t)k * d * d);
   }
   memcpy(counts_out, c + kMaxClasses, sizeof(double) * 3);
   return B2_OK;
@@ -2107,14 +2105,8 @@ int b2_multinomial_pass(b2_ctx* ctx, const void* X, int x_dtype, const float* y,
     for (int k = 0, p = 0; k < K; ++k)
       for (int l = k; l < K; ++l, ++p) {
         const double* b = blk + (size_t)p * dp * dp;
-        double* hk = hess_out + ((size_t)k * K + l) * d1 * d1;
-        double* hl = hess_out + ((size_t)l * K + k) * d1 * d1;
-        for (int i = 0; i < d1; ++i)
-          for (int j = i; j < d1; ++j) {
-            const double v = b[(size_t)i * dp + j];
-            hk[(size_t)i * d1 + j] = hk[(size_t)j * d1 + i] = v;
-            hl[(size_t)i * d1 + j] = hl[(size_t)j * d1 + i] = v;
-          }
+        unpack_upper(b, dp, d1, hess_out + ((size_t)k * K + l) * d1 * d1);
+        unpack_upper(b, dp, d1, hess_out + ((size_t)l * K + k) * d1 * d1);
       }
   }
   return B2_OK;

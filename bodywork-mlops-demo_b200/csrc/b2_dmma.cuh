@@ -1,6 +1,6 @@
-// b2_dmma.cuh -- the device side shared by the fp64 tile passes (glm_kernel in glm.cu, loo_kernel in ridge_loo.cu,
-// score_std_kernel in score_std.cu): the fp64 tensor-core MMA, the per-element row load, the 32-row tile ring, its
-// loader (step 1 of each pass) and the product with an operand resident in shared memory (step 2 of the last two).
+// b2_dmma.cuh -- the device side shared by the fp64 tile passes: the fp64 tensor-core MMA, the per-element row load,
+// the 32-row tile ring, its loader (step 1 of each pass), the product with an operand resident in shared memory
+// (tile_product), and the upper-block schedule of the passes that sum a symmetric matrix.
 //
 // A pass runs kTileWarps consumer warps over the tiles blockIdx.x, + gridDim.x, ... of 32 rows.  In the ring flavour
 // (rows [0, n), n a multiple of kTileRows, contiguous and 16-byte aligned, y too) one more warp's lane 0 runs
@@ -186,6 +186,68 @@ __device__ __forceinline__ void tile_product(const double* Vs, int vp, const dou
         for (int mt = 0; mt < kTileMT; ++mt) a[mt] = Vs[(8 * mt + g) * vp + 4 * ks + t4];
 #pragma unroll
         for (int mt = 0; mt < kTileMT; ++mt) dmma(z[u][mt][0], z[u][mt][1], a[mt], b);
+      }
+    }
+  }
+}
+
+// The upper-block schedule of the symmetric dp x dp fp64 sums (dp a multiple of 16): the Hessians of glm_kernel,
+// multinomial_kernel and svm_kernel, the scatters of class_scatter_kernel and class_scatters_kernel.  A CTA writes
+// every entry of the 16 x 16 blocks on and above the diagonal except the 8 x 8 tile below the diagonal of a diagonal
+// block: the upper triangle i <= j, which the host mirrors (unpack_upper in b2_api.cu).  Consumer warp w holds blocks
+// w, w + kTileWarps, ... in acc[u][q] for the whole launch, q the 8 x 8 tile at rows 8 (q >> 1), columns 8 (q & 1).
+constexpr int kUpperTable = 96;   // ints of shared memory for the block table: rows at [0, 48), columns at [48, 96)
+
+// the table of the nb (nb + 1) / 2 blocks on and above the diagonal (nb <= 9), row-major; thread 0 writes it, so the
+// caller's next block barrier publishes it
+__device__ __forceinline__ void upper_blocks(int* sb, int nb) {
+  if (threadIdx.x != 0) return;
+  int k = 0;
+  for (int i = 0; i < nb; ++i)
+    for (int j = i; j < nb; ++j, ++k) { sb[k] = i; sb[kUpperTable / 2 + k] = j; }
+}
+
+// acc += A^T B over the 32 rows of a tile for the calling warp's blocks: A[r][c] = load_a(r, c), B the tile at Bs
+// (pitch zp).  Four DMMAs per 2 + 2 fragment loads, three on a diagonal block.  warp, g8 = lane / 4 and t4 = lane % 4
+// are the calling thread's, as the kernel already holds them.
+template <int SB, typename LoadA>
+__device__ __forceinline__ void upper_accumulate(double (&acc)[SB][4][2], const int* sb, int nsb, LoadA&& load_a,
+                                                 const double* Bs, int zp, int warp, int g8, int t4) {
+#pragma unroll
+  for (int u = 0; u < SB; ++u) {
+    const int b = warp + kTileWarps * u;
+    if (b < nsb) {                               // warp-uniform
+      const int bi = sb[b], bj = sb[kUpperTable / 2 + b], ci = 16 * bi + g8, cj = 16 * bj + g8;
+      const bool diag = bi == bj;
+#pragma unroll
+      for (int ks = 0; ks < kTileRows / 4; ++ks) {
+        const int r = 4 * ks + t4;
+        const double a0 = load_a(r, ci), a1 = load_a(r, ci + 8);
+        const double b0 = Bs[r * zp + cj], b1 = Bs[r * zp + cj + 8];
+        dmma(acc[u][0][0], acc[u][0][1], a0, b0);
+        dmma(acc[u][1][0], acc[u][1][1], a0, b1);
+        if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
+        dmma(acc[u][3][0], acc[u][3][1], a1, b1);
+      }
+    }
+  }
+}
+
+// the calling warp's blocks to out[i * pitch + j]; the producer warp of the ring holds none
+template <int SB>
+__device__ __forceinline__ void upper_store(const double (&acc)[SB][4][2], const int* sb, int nsb, double* out,
+                                            int pitch, int warp, int g8, int t4) {
+#pragma unroll
+  for (int u = 0; u < SB; ++u) {
+    const int b = warp + kTileWarps * u;
+    if (warp < kTileWarps && b < nsb) {
+      const int bi = sb[b], bj = sb[kUpperTable / 2 + b];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        if (q == 2 && bi == bj) continue;
+        const int i = 16 * bi + 8 * (q >> 1) + g8, j = 16 * bj + 8 * (q & 1) + 2 * t4;
+        out[i * pitch + j] = acc[u][q][0];
+        out[i * pitch + j + 1] = acc[u][q][1];
       }
     }
   }

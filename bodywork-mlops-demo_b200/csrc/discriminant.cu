@@ -9,12 +9,11 @@
 //       sorted classes, -1 for a kept row of no class, NaN included, -2 for a row not kept); lane 0 of each warp counts
 //       its rows;
 //   (2) u = x - m_class in fp64, zero for rows of no class and rows not kept, and A = w_class u beside it;
-//   (3) S_w += A^T u on the fp64 tensor core with glm_kernel's register-resident schedule: 16 x 16 blocks on and above
+//   (3) S_w += A^T u on the fp64 tensor core with the upper-block schedule (b2_dmma.cuh): 16 x 16 blocks on and above
 //       the diagonal (36 at D = 128: there is no intercept column), each warp holding up to five of them for the whole
 //       launch, the 8 x 8 tile below the diagonal of a diagonal block skipped.
 // The class means (at most 32 x 128 doubles) sit in shared memory beside the tile for the whole launch.  Each CTA writes
-// its sums in ctx->disc_part and the ordered reduce adds the CTAs in order: two calls return identical sums.  The
-// schedule of (3) is a copy of glm_kernel's, as svm_kernel's is: no existing kernel changes.
+// its sums in ctx->disc_part and the ordered reduce adds the CTAs in order: two calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
 
@@ -31,12 +30,11 @@ size_t scatter_smem_bytes(int dp, int n_classes, bool ring) {
   return tile_ring_bytes(ring, true) +
          sizeof(double) * (2 * (size_t)kTileRows * tile_vpitch(dp) + (size_t)n_classes * dp + kMaxClasses +
                            kTileWarps * 4) +
-         sizeof(float) * kMaxClasses + sizeof(int) * (kTileRows + 2 * 48);
+         sizeof(float) * kMaxClasses + sizeof(int) * (kTileRows + kUpperTable);
 }
 
-// Per CTA: [0] kept rows [1] kept rows of no class [2] kept rows with y not finite, zeros to kDaHead, then the blocks of
-// sum w u u^T at kDaHead + i kMaxD + j (every entry of the blocks on and above the diagonal but the 8 x 8 tile below the
-// diagonal of a diagonal block).  op: ctx->disc.
+// Per CTA: [0] kept rows [1] kept rows of no class [2] kept rows with y not finite, zeros to kDaHead, then the upper
+// blocks of sum w u u^T at kDaHead + i kMaxD + j.  op: ctx->disc.
 template <typename T, bool RING>
 __global__ void __launch_bounds__(kTileThreads, 1)
 class_scatter_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* __restrict__ y,
@@ -52,8 +50,7 @@ class_scatter_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, con
   double* cnt = wv + kMaxClasses;          // [warp][4]: kept, no class, y not finite
   float* cls = reinterpret_cast<float*>(cnt + kTileWarps * 4);
   int* row_class = reinterpret_cast<int*>(cls + kMaxClasses);
-  int* sbi = row_class + kTileRows;        // the 16 x 16 blocks on and above the diagonal
-  int* sbj = sbi + 48;
+  int* sb = row_class + kTileRows;         // the upper blocks' table
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
   for (int t = tid; t < K * dp; t += blockDim.x) {
     const int k = t / dp, j = t - k * dp;
@@ -64,18 +61,10 @@ class_scatter_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, con
     cls[t] = t < K ? (float)op[kDaClasses + t] : 0.f;
   }
   for (int t = tid; t < kTileWarps * 4; t += blockDim.x) cnt[t] = 0.0;
-  if (tid == 0) {
-    int k = 0;
-    for (int i = 0; i < nb; ++i)
-      for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
-  }
+  upper_blocks(sb, nb);
   const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
   tiles.start();
-  double acc[kDaSB][4][2];                 // the warp's blocks, held for the whole launch
-#pragma unroll
-  for (int u = 0; u < kDaSB; ++u)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
+  double acc[kDaSB][4][2] = {};            // the warp's blocks, held for the whole launch
   if (!tiles.produce()) {
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // (1) the tile and the rows' classes
@@ -98,25 +87,8 @@ class_scatter_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, con
         As[r * zp + j] = k >= 0 ? wv[k] * u : 0.0;
       }
       tile_consumer_sync();
-      // (3) S_w += (w u)^T u over the tile's rows, the warp's blocks (glm_kernel's step (5))
-#pragma unroll
-      for (int u = 0; u < kDaSB; ++u) {
-        const int sb = warp + kTileWarps * u;
-        if (sb < nsb) {                               // warp-uniform
-          const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
-          const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-          for (int ks = 0; ks < kTileRows / 4; ++ks) {
-            const int r = 4 * ks + t4;
-            const double a0 = As[r * zp + ci], a1 = As[r * zp + ci + 8];
-            const double b0 = Us[r * zp + cj], b1 = Us[r * zp + cj + 8];
-            dmma(acc[u][0][0], acc[u][0][1], a0, b0);
-            dmma(acc[u][1][0], acc[u][1][1], a0, b1);
-            if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
-            dmma(acc[u][3][0], acc[u][3][1], a1, b1);
-          }
-        }
-      }
+      // (3) S_w += (w u)^T u over the tile's rows, the warp's blocks
+      upper_accumulate(acc, sb, nsb, [&](int r, int c) { return As[r * zp + c]; }, Us, zp, warp, g8, t4);
       tile_consumer_sync();
     }
   }
@@ -129,20 +101,7 @@ class_scatter_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, con
       for (int w = 0; w < kTileWarps; ++w) v += cnt[w * 4 + tid];
     out[tid] = v;
   }
-#pragma unroll
-  for (int u = 0; u < kDaSB; ++u) {
-    const int sb = warp + kTileWarps * u;
-    if (warp < kTileWarps && sb < nsb) {
-      const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (q == 2 && diag) continue;
-        const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
-        out[kDaHead + i * kMaxD + j] = acc[u][q][0];
-        out[kDaHead + i * kMaxD + j + 1] = acc[u][q][1];
-      }
-    }
-  }
+  upper_store(acc, sb, nsb, out + kDaHead, kMaxD, warp, g8, t4);
 }
 
 }  // namespace

@@ -10,10 +10,11 @@
 //   (2) eta (and, for the line search, deta = x.step + db) per row: the lanes of a warp over the features, a butterfly;
 //   (3) loss, g, h (or the loss at eta + t deta for t = 1, 1/2, ..., one step per lane) per kept row, by selects;
 //   (4) the gradient: thread j adds g_r z_rj over the tile's rows in order;
-//   (5) the Hessian on the fp64 tensor core (mma.sync m8n8k4 f64): A = the |h|-scaled rows, B = the rows, K = the 32 rows of
-//       the tile.  The (D + 1)^2 output is cut in 16 x 16 blocks; only blocks on or above the diagonal are computed, each
-//       warp holding up to six of them in registers for the whole launch (4 DMMAs per 2 + 2 fragment loads), the 8 x 8
-//       tile below the diagonal of a diagonal block skipped: 153 of the 289 8 x 8 tiles at D = 128.
+//   (5) the Hessian on the fp64 tensor core (mma.sync m8n8k4 f64) with the upper-block schedule (b2_dmma.cuh): A =
+//       the |h|-scaled rows, B = the rows, K = the 32 rows of the tile.  The (D + 1)^2 output is cut in 16 x 16 blocks;
+//       only blocks on or above the diagonal are computed, each warp holding up to six of them in registers for the
+//       whole launch (4 DMMAs per 2 + 2 fragment loads), the 8 x 8 tile below the diagonal of a diagonal block skipped:
+//       153 of the 289 8 x 8 tiles at D = 128.
 // The rows take scoring's plan (plan_rows): contiguous 16-byte aligned rows stream through the bulk-copy ring in whole
 // tiles, the rest (and every other layout) is read by the same consumers from global memory.  Each CTA writes its sums
 // in a fixed order, the ordered reduce adds the CTAs in order: two calls return identical sums.
@@ -31,8 +32,8 @@ __host__ __device__ inline int glm_dp(int d) { return (d + 1 + 15) & ~15; }   //
 size_t glm_smem_bytes(int dp, bool ring, int mode) {
   const size_t tile = (size_t)kTileRows * tile_vpitch(dp);
   return tile_ring_bytes(ring, true) +
-         sizeof(double) *
-             (tile * (mode == kGlmHessian ? 2 : 1) + 3 * kMaxD + 8 + 3 * kTileRows + 2 * kTileWarps * 32 + 48);
+         sizeof(double) * (tile * (mode == kGlmHessian ? 2 : 1) + 3 * kMaxD + 8 + 3 * kTileRows + 2 * kTileWarps * 32) +
+         sizeof(int) * kUpperTable;
 }
 
 // The pointwise half-Tweedie loss, gradient and Hessian in eta, sklearn's Cython branches: the log link at any power
@@ -149,8 +150,7 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   double* red = hs + kTileRows;            // [warp][32] the warps' sums
   double* lsum = red + kTileWarps * 32;    // [warp][u][8] the scalar sums of the rows warp + 8 u (gradient / Hessian)
   double* gsum = lsum + kTileWarps * 32;   // [kMaxD + 8] the gradient sums, entry j of thread j
-  int* sbi = reinterpret_cast<int*>(gsum + kMaxD + 8);   // the 16 x 16 blocks on and above the diagonal
-  int* sbj = sbi + 48;
+  int* sb = reinterpret_cast<int*>(gsum + kMaxD + 8);    // the upper blocks' table
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
   for (int t = tid; t < kTileWarps * 32; t += blockDim.x) lsum[t] = 0.0;
   for (int t = tid; t < kMaxD + 8; t += blockDim.x) gsum[t] = 0.0;
@@ -158,22 +158,14 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
     sv[t] = (MODE == kGlmLadder && t < d) ? op[kGlmOpStep + t] : 0.0;
   }
-  if (tid == 0) {
-    int k = 0;
-    for (int i = 0; i < nb; ++i)
-      for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
-  }
+  upper_blocks(sb, nb);
   const double b = op[kGlmOpMisc], db = op[kGlmOpMisc + 1];
   const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
   tiles.start();
   // kGlmLadder: lane k sums the loss at step k.  The other sums stay in shared memory (lsum, gsum), which leaves the
   // registers to the Hessian's accumulators.
   double s_loss = 0.0;
-  double acc[kGlmSB][4][2];
-#pragma unroll
-  for (int u = 0; u < kGlmSB; ++u)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
+  double acc[kGlmSB][4][2] = {};
   if (!tiles.produce()) {
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // (1) the tile: z = [x 1 0...] and y, zero for rows not kept
@@ -268,24 +260,7 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
           }
           tile_consumer_sync();
           // (5) H += (|h| z)^T z over the tile's rows, the warp's blocks
-#pragma unroll
-          for (int u = 0; u < kGlmSB; ++u) {
-            const int sb = warp + kTileWarps * u;
-            if (sb < nsb) {                               // warp-uniform
-              const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
-              const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-              for (int ks = 0; ks < kTileRows / 4; ++ks) {
-                const int r = 4 * ks + t4;
-                const double a0 = HZs[r * zp + ci], a1 = HZs[r * zp + ci + 8];
-                const double b0 = Zs[r * zp + cj], b1 = Zs[r * zp + cj + 8];
-                dmma(acc[u][0][0], acc[u][0][1], a0, b0);
-                dmma(acc[u][1][0], acc[u][1][1], a0, b1);
-                if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
-                dmma(acc[u][3][0], acc[u][3][1], a1, b1);
-              }
-            }
-          }
+          upper_accumulate(acc, sb, nsb, [&](int r, int c) { return HZs[r * zp + c]; }, Zs, zp, warp, g8, t4);
         }
       }
       tile_consumer_sync();
@@ -311,22 +286,7 @@ glm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
         r = gsum[tid - kGlmGrad];
       out[tid] = r;
     }
-    if constexpr (MODE == kGlmHessian) {
-#pragma unroll
-      for (int u = 0; u < kGlmSB; ++u) {
-        const int sb = warp + kTileWarps * u;
-        if (warp < kTileWarps && sb < nsb) {
-          const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (q == 2 && diag) continue;
-            const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
-            out[kGlmHess + i * kGlmHp + j] = acc[u][q][0];
-            out[kGlmHess + i * kGlmHp + j + 1] = acc[u][q][1];
-          }
-        }
-      }
-    }
+    if constexpr (MODE == kGlmHessian) upper_store(acc, sb, nsb, out + kGlmHess, kGlmHp, warp, g8, t4);
   }
 }
 

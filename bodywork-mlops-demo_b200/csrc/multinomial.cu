@@ -11,8 +11,9 @@
 //       against the resident [W b]^T (with the step beside it: at most 64 columns);
 //   (3) per kept row, one warp per row and one lane per class: the softmax, the loss, g, and the row's counts;
 //   (4) the gradient: thread j adds g_rk z_rj over the tile's rows in order;
-//   (5) (Hessian) blockIdx.y selects one class pair k <= l: the rows scaled by h_kl, then glm_kernel's schedule -- the
-//       16 x 16 blocks on and above the diagonal of the (D + 1)^2 block, held in registers for the whole launch;
+//   (5) (Hessian) blockIdx.y selects one class pair k <= l: the rows scaled by h_kl, then the upper-block schedule
+//       (b2_dmma.cuh) -- the 16 x 16 blocks on and above the diagonal of the (D + 1)^2 block, held in registers for the
+//       whole launch;
 //   (6) (ladder) the loss at eta + 2^-t deta, one step t per lane.
 // The grid is row slices x class pairs (one pair per CTA: the accumulators of one block fill the registers).  Each CTA
 // writes its sums at its pair's place in its slice's partial; one ordered reduce adds the slices in order for every pair
@@ -49,7 +50,7 @@ size_t mn_smem_bytes(int d, int n_classes, int mode, bool ring) {
   return tile_ring_bytes(ring, true) +
          sizeof(double) * (tile * (mode == kGlmHessian ? 2 : 1) + (size_t)dp * mn_bpitch(mn_cols(n_classes, mode)) +
                            kTileRows * (kMnEp + kMnPp + 1) + gacc + 2 * kTileWarps * 32) +
-         sizeof(float) * kMaxClasses + sizeof(int) * (kTileRows + 96);
+         sizeof(float) * kMaxClasses + sizeof(int) * (kTileRows + kUpperTable);
 }
 
 // the class pair (k, l), k <= l, of pair index p in row-major order
@@ -83,8 +84,7 @@ multinomial_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
   double* red = lsum + kTileWarps * 32;      // [warp][32] the ladder's per-lane sums
   float* cls = reinterpret_cast<float*>(red + kTileWarps * 32);
   int* row_cls = reinterpret_cast<int*>(cls + kMaxClasses);
-  int* sbi = row_cls + kTileRows;            // the 16 x 16 blocks on and above the diagonal
-  int* sbj = sbi + 48;
+  int* sb = row_cls + kTileRows;             // the upper blocks' table
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
   // this CTA's pair and its gradient rows [k0, k1)
   int pk = 0, pl = 0, k0 = 0, k1 = K;
@@ -104,19 +104,11 @@ multinomial_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
     else if (i <= d && c < cols) v = op[kMnStep + (c - K) * (kMaxD + 1) + i];
     Bs[t] = v;
   }
-  if (tid == 0) {
-    int k = 0;
-    for (int i = 0; i < nb; ++i)
-      for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
-  }
+  upper_blocks(sb, nb);
   const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
   tiles.start();
   double s_loss = 0.0;                       // kGlmLadder: lane t sums the loss at step t
-  double acc[MODE == kGlmHessian ? kMnSB : 1][4][2];
-#pragma unroll
-  for (int u = 0; u < (MODE == kGlmHessian ? kMnSB : 1); ++u)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
+  double acc[MODE == kGlmHessian ? kMnSB : 1][4][2] = {};
   if (!tiles.produce()) {
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       // (1) the tile: z = [x 1 0...], zero for rows not kept, and the rows' classes
@@ -207,24 +199,7 @@ multinomial_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
           }
           tile_consumer_sync();
           // (5) H_kl += (h_kl z)^T z over the tile's rows, the warp's blocks
-#pragma unroll
-          for (int u = 0; u < kMnSB; ++u) {
-            const int sb = warp + kTileWarps * u;
-            if (sb < nsb) {                               // warp-uniform
-              const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
-              const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-              for (int ks = 0; ks < kTileRows / 4; ++ks) {
-                const int r = 4 * ks + t4;
-                const double a0 = HZs[r * zp + ci], a1 = HZs[r * zp + ci + 8];
-                const double b0 = Zs[r * zp + cj], b1 = Zs[r * zp + cj + 8];
-                dmma(acc[u][0][0], acc[u][0][1], a0, b0);
-                dmma(acc[u][1][0], acc[u][1][1], a0, b1);
-                if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
-                dmma(acc[u][3][0], acc[u][3][1], a1, b1);
-              }
-            }
-          }
+          upper_accumulate(acc, sb, nsb, [&](int r, int c) { return HZs[r * zp + c]; }, Zs, zp, warp, g8, t4);
         }
       }
       tile_consumer_sync();
@@ -258,20 +233,7 @@ multinomial_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const
       const int i = t / dp, j = t - i * dp, bi = i >> 4, bj = j >> 4;
       if (bi > bj || (bi == bj && (i & 15) >= 8 && (j & 15) < 8)) blk[t] = 0.0;
     }
-#pragma unroll
-    for (int u = 0; u < kMnSB; ++u) {
-      const int sb = warp + kTileWarps * u;
-      if (warp < kTileWarps && sb < nsb) {
-        const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (q == 2 && diag) continue;
-          const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
-          blk[i * dp + j] = acc[u][q][0];
-          blk[i * dp + j + 1] = acc[u][q][1];
-        }
-      }
-    }
+    upper_store(acc, sb, nsb, blk, dp, warp, g8, t4);
   }
 }
 

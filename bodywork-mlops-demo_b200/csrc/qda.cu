@@ -9,9 +9,8 @@
 //       kept rows' indices written grouped by class, in row order within a class;
 //   (2) one CTA per work item gathers 32 of its rows at a time through the index (the next 32 are loaded into registers
 //       while the tensor core works on the current ones), forms u = x - m_k in fp64 from the exactly converted value,
-//       and accumulates u^T u with class_scatter_kernel's register-resident schedule: 16 x 16 blocks on and above the
-//       diagonal, each warp holding up to five for the whole item (a copy, as svm_kernel's and class_scatter_kernel's
-//       are of glm_kernel's: no existing kernel changes);
+//       and accumulates u^T u with the upper-block schedule (b2_dmma.cuh): 16 x 16 blocks on and above the diagonal,
+//       each warp holding up to five for the whole item;
 //   (3) one reduce adds each class's items in item order into its sum (`first` overwrites, otherwise adds), so repeated
 //       calls are bit-identical.
 // The indices are int32 over spans of at most kQdSpan rows, which bounds the scratch at 64 MB.
@@ -174,13 +173,13 @@ order_place_kernel(const float* __restrict__ y, const uint8_t* __restrict__ mask
 }
 
 // ---- (2) the scatter of each work item ---------------------------------------------------------------------------------
-// shared memory: the gathered rows u [kTileRows][zp], the class mean [dp], the blocks on and above the diagonal
+// shared memory: the gathered rows u [kTileRows][zp], the class mean [dp], the upper blocks' table
 size_t scatters_smem_bytes(int dp) {
-  return sizeof(double) * ((size_t)kTileRows * tile_vpitch(dp) + dp) + sizeof(int) * 2 * 48;
+  return sizeof(double) * ((size_t)kTileRows * tile_vpitch(dp) + dp) + sizeof(int) * kUpperTable;
 }
 
-// Item blockIdx.x of the header (none past its item count): sum u u^T over its rows into part[item] at i kMaxD + j (every
-// entry of the blocks on and above the diagonal but the 8 x 8 tile below the diagonal of a diagonal block).  X: the span.
+// Item blockIdx.x of the header (none past its item count): the upper blocks of sum u u^T over its rows into part[item]
+// at i kMaxD + j.  X: the span.
 template <typename T>
 __global__ void __launch_bounds__(kQsThreads, 1)
 class_scatters_kernel(const T* __restrict__ X, int d, int64_t ldx, const int* __restrict__ idx,
@@ -192,15 +191,10 @@ class_scatters_kernel(const T* __restrict__ X, int d, int64_t ldx, const int* __
   const int dp = qs_dp(d), zp = tile_vpitch(dp), nb = dp / 16, nsb = nb * (nb + 1) / 2;
   double* Us = reinterpret_cast<double*>(smem_raw);   // [row][zp]: u = x - m_k
   double* Ms = Us + kTileRows * zp;                   // [dp] m_k, zero padded
-  int* sbi = reinterpret_cast<int*>(Ms + dp);         // the 16 x 16 blocks on and above the diagonal
-  int* sbj = sbi + 48;
+  int* sb = reinterpret_cast<int*>(Ms + dp);          // the upper blocks' table
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
   for (int t = tid; t < dp; t += blockDim.x) Ms[t] = t < d ? op[kQdMeans + k * kMaxD + t] : 0.0;
-  if (tid == 0) {
-    int b = 0;
-    for (int i = 0; i < nb; ++i)
-      for (int j = i; j < nb; ++j, ++b) { sbi[b] = i; sbj[b] = j; }
-  }
+  upper_blocks(sb, nb);
   // thread (pr, pc) gathers row pr of each 32 and its columns pc + 8 q
   const int pr = tid >> 3, pc = tid & 7;
   float nx[kQsCols];
@@ -214,11 +208,7 @@ class_scatters_kernel(const T* __restrict__ X, int d, int64_t ldx, const int* __
       nx[q] = (live && j < d) ? ld_row_val<T>(xr + j) : 0.f;
     }
   };
-  double acc[kQsSB][4][2];                 // the warp's blocks, held for the whole item
-#pragma unroll
-  for (int u = 0; u < kQsSB; ++u)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
+  double acc[kQsSB][4][2] = {};            // the warp's blocks, held for the whole item
   __syncthreads();
   fetch(begin);
   for (int g0 = begin; g0 < end; g0 += kTileRows) {
@@ -231,42 +221,11 @@ class_scatters_kernel(const T* __restrict__ X, int d, int64_t ldx, const int* __
     }
     __syncthreads();
     if (g0 + kTileRows < end) fetch(g0 + kTileRows);   // the next rows' loads are in flight during the products
-    // S_k += u^T u over the 32 rows, the warp's blocks (class_scatter_kernel's step (3) with A = u)
-#pragma unroll
-    for (int u = 0; u < kQsSB; ++u) {
-      const int sb = warp + kTileWarps * u;
-      if (sb < nsb) {                               // warp-uniform
-        const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
-        const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-        for (int ks = 0; ks < kTileRows / 4; ++ks) {
-          const int r = 4 * ks + t4;
-          const double a0 = Us[r * zp + ci], a1 = Us[r * zp + ci + 8];
-          const double b0 = Us[r * zp + cj], b1 = Us[r * zp + cj + 8];
-          dmma(acc[u][0][0], acc[u][0][1], a0, b0);
-          dmma(acc[u][1][0], acc[u][1][1], a0, b1);
-          if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
-          dmma(acc[u][3][0], acc[u][3][1], a1, b1);
-        }
-      }
-    }
+    // S_k += u^T u over the 32 rows, the warp's blocks
+    upper_accumulate(acc, sb, nsb, [&](int r, int c) { return Us[r * zp + c]; }, Us, zp, warp, g8, t4);
     __syncthreads();
   }
-  double* out = part + (size_t)item * kMaxD * kMaxD;
-#pragma unroll
-  for (int u = 0; u < kQsSB; ++u) {
-    const int sb = warp + kTileWarps * u;
-    if (sb < nsb) {
-      const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (q == 2 && diag) continue;
-        const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
-        out[i * kMaxD + j] = acc[u][q][0];
-        out[i * kMaxD + j + 1] = acc[u][q][1];
-      }
-    }
-  }
+  upper_store(acc, sb, nsb, part + (size_t)item * kMaxD * kMaxD, kMaxD, warp, g8, t4);
 }
 
 // ---- (3) the ordered reduce -------------------------------------------------------------------------------------------

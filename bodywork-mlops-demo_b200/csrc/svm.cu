@@ -14,13 +14,12 @@
 //       |r| > eps, e = r -+ eps, loss e^2, g = e; sigma = active_to - active_from;
 //   (4) the gradient: thread j adds g_r z_rj over the tile's rows in order (g = 0 where not active);
 //   (5) (Hessian) the rows with sigma != 0 are compacted in row order (a ballot and a prefix count) into a staging tile;
-//       each time it holds 32 rows, sum sigma z z^T over them on the fp64 tensor core with glm_kernel's register-resident
-//       schedule (16 x 16 blocks on and above the diagonal), the partial tile flushed at the end with its unused rows
-//       zeroed.  The tensor-core work is proportional to the rows that changed side; sigma z is exact, so the +- sums
-//       round only in the additions.
+//       each time it holds 32 rows, sum sigma z z^T over them on the fp64 tensor core with the upper-block schedule
+//       (b2_dmma.cuh: 16 x 16 blocks on and above the diagonal), the partial tile flushed at the end with its unused
+//       rows zeroed.  The tensor-core work is proportional to the rows that changed side; sigma z is exact, so the +-
+//       sums round only in the additions.
 // Each CTA writes its sums in ctx->glm_part in glm_kernel's layout and the ordered reduce adds the CTAs in order: two
-// calls return identical sums.  The schedule of (5) is a copy of glm_kernel's: moving it into b2_dmma.cuh would put
-// every instantiation of glm_kernel and multinomial_kernel through a new inlining path, for twenty lines.
+// calls return identical sums.
 #include "b2_internal.cuh"
 #include "b2_dmma.cuh"
 
@@ -35,7 +34,7 @@ size_t svm_smem_bytes(int dp, bool ring, bool hess) {
   const size_t tile = (size_t)kTileRows * tile_vpitch(dp);
   return tile_ring_bytes(ring, true) +
          sizeof(double) * (tile * (hess ? 2 : 1) + 2 * kMaxD + 4 * kTileRows + kTileWarps * 32 + kMaxD + 12) +
-         sizeof(int) * (2 * 48 + 2 * kTileRows + 4);
+         sizeof(int) * (kUpperTable + 2 * kTileRows + 4);
 }
 
 // active at eta, and (active) the loss and g: the squared hinge at label sign t, or the squared epsilon-insensitive loss
@@ -67,9 +66,8 @@ svm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
   double* lsum = ssg + kTileRows;          // [warp][u][8] the scalar sums of the rows warp + 8 u
   double* gsum = lsum + kTileWarps * 32;   // [kMaxD + 8] the gradient sums, entry j of thread j
   double* msc = gsum + kMaxD + 8;          // [4] b at to, b at from, 1 when from is given, the label or eps
-  int* sbi = reinterpret_cast<int*>(msc + 4);   // the 16 x 16 blocks on and above the diagonal
-  int* sbj = sbi + 48;
-  int* dst = sbj + 48;                     // the staging slot of each changed row (-1: unchanged), past 31: next round
+  int* sb = reinterpret_cast<int*>(msc + 4);   // the upper blocks' table
+  int* dst = sb + kUpperTable;             // the staging slot of each changed row (-1: unchanged), past 31: next round
   int* kp = dst + kTileRows;               // 1 for the tile's kept rows
   int* cnt = kp + kTileRows;              // [0] rows in the staging tile, [1] the same plus the tile's changed rows
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane >> 2, t4 = lane & 3;
@@ -80,40 +78,14 @@ svm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
     wv[t] = t < d ? op[kGlmOpW + t] : 0.0;
     fv[t] = t < d ? op[kGlmOpStep + t] : 0.0;
   }
-  if (tid == 0) {
-    cnt[0] = 0;
-    int k = 0;
-    for (int i = 0; i < nb; ++i)
-      for (int j = i; j < nb; ++j, ++k) { sbi[k] = i; sbj[k] = j; }
-  }
+  if (tid == 0) cnt[0] = 0;
+  upper_blocks(sb, nb);
   const int64_t n_tiles = (n + kTileRows - 1) / kTileRows;
   tiles.start();
-  double acc[kSvSB][4][2];                          // (HESS) the warp's blocks, held for the whole launch
-#pragma unroll
-  for (int u = 0; u < kSvSB; ++u)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { acc[u][q][0] = 0.0; acc[u][q][1] = 0.0; }
-  // H += (sigma z)^T z over the 32 staged rows, the warp's blocks (glm_kernel's step (5))
+  double acc[kSvSB][4][2] = {};                     // (HESS) the warp's blocks, held for the whole launch
+  // H += (sigma z)^T z over the 32 staged rows, the warp's blocks
   auto flush = [&]() {
-#pragma unroll
-    for (int u = 0; u < kSvSB; ++u) {
-      const int sb = warp + kTileWarps * u;
-      if (sb < nsb) {                               // warp-uniform
-        const int ci = 16 * sbi[sb] + g8, cj = 16 * sbj[sb] + g8;
-        const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-        for (int ks = 0; ks < kTileRows / 4; ++ks) {
-          const int r = 4 * ks + t4;
-          const double s = ssg[r];
-          const double a0 = s * Ss[r * zp + ci], a1 = s * Ss[r * zp + ci + 8];
-          const double b0 = Ss[r * zp + cj], b1 = Ss[r * zp + cj + 8];
-          dmma(acc[u][0][0], acc[u][0][1], a0, b0);
-          dmma(acc[u][1][0], acc[u][1][1], a0, b1);
-          if (!diag) dmma(acc[u][2][0], acc[u][2][1], a1, b0);
-          dmma(acc[u][3][0], acc[u][3][1], a1, b1);
-        }
-      }
-    }
+    upper_accumulate(acc, sb, nsb, [&](int r, int c) { return ssg[r] * Ss[r * zp + c]; }, Ss, zp, warp, g8, t4);
   };
   if (!tiles.produce()) {
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -242,22 +214,7 @@ svm_kernel(const T* __restrict__ X, int64_t n, int d, int64_t ldx, const float* 
       r = gsum[tid - kGlmGrad];
     out[tid] = r;
   }
-  if constexpr (HESS) {
-#pragma unroll
-    for (int u = 0; u < kSvSB; ++u) {
-      const int sb = warp + kTileWarps * u;
-      if (warp < kTileWarps && sb < nsb) {
-        const bool diag = sbi[sb] == sbj[sb];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (q == 2 && diag) continue;
-          const int i = 16 * sbi[sb] + 8 * (q >> 1) + g8, j = 16 * sbj[sb] + 8 * (q & 1) + 2 * t4;
-          out[kGlmHess + i * kGlmHp + j] = acc[u][q][0];
-          out[kGlmHess + i * kGlmHp + j + 1] = acc[u][q][1];
-        }
-      }
-    }
-  }
+  if constexpr (HESS) upper_store(acc, sb, nsb, out + kGlmHess, kGlmHp, warp, g8, t4);
 }
 
 }  // namespace

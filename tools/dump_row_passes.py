@@ -10,7 +10,9 @@ and bf16 rows x device rows (4 133: ring tiles and a direct tail where the rows 
 of pitch d + 3 starting one element in, masked device rows (keep = 1 of a seeded 0/1 mask), and at d = 64 pinned and
 pageable host rows over two staging blocks and a tail, masked.  Per call: every output and the launch count; an output
 over 16 MB (the host cases' cv_out) as its SHA-256 digest, so a dump stays small.  Rows come from a fixed numpy seed.
-Prints one JSON line."""
+The symmetric sums: b2_multinomial_pass with the Hessian at K = 3 and 7; b2_svm_pass with dhess_out for both losses,
+with and without coef_from; b2_class_scatter with unit and per-class weights and b2_class_scatters at K = 7.  The
+multiclass labels are floor(3 y) mod 7 (at K = 3 some rows have no class).  Prints one JSON line."""
 import argparse
 import ctypes as C
 import hashlib
@@ -28,6 +30,8 @@ N_DEV = 4_133
 N_HOST = 2 * (1 << 18) + 4_321
 BIG = 16 << 20                                          # bytes: larger outputs are dumped as their digest
 GLM = (("identity", 0.0), ("log", 0.0), ("log", 1.0), ("log", 1.5), ("log", 2.0), ("log", 3.0))
+CLASSES = np.arange(7, dtype=np.float32)               # the multiclass passes' labels
+CLASS_WEIGHTS = np.linspace(0.5, 2.0, 7)
 
 
 def _rows(n, d, seed):
@@ -75,9 +79,12 @@ def dump(out):
             if dv is not None:
                 dv.free()
 
-    def calls(key, X, xdt, y, lab, mask, n, d, ldx, mk, coef, sigma, mean):
+    def calls(key, X, xdt, y, lab, mlab, mask, n, d, ldx, mk, coef, sigma, mean):
         base = (ctx._h, X, xdt)
         w, step = coef.ctypes.data, coef[::-1].copy()
+        rng = np.random.default_rng(3000 + d)
+        mn_coef = rng.normal(size=(7, d + 1)) * 0.5 / np.sqrt(d)
+        means = rng.normal(size=(7, d)) * 0.1
         for link, power in GLM:
             lk = native.GLM_LOG if link == "log" else native.GLM_IDENTITY
             for hess in (True, False):
@@ -123,6 +130,38 @@ def dump(out):
                                     output(n, np.float64) if want_yhat else None, output(n, np.float64)))
                 return []
             run(f"{key}/score_std-{'yhat' if want_yhat else 'ystd'}", mk, score_std)
+        for K in (3, 7):
+            def multinomial_pass(output, K=K):
+                W = np.ascontiguousarray(mn_coef[:K])
+                sums, H = np.empty(5 + K * (d + 1)), np.empty((K, K, d + 1, d + 1))
+                ok(lib.b2_multinomial_pass(*base, mlab, n, d, ldx, mk, mask, 1, CLASSES.ctypes.data, K, W.ctypes.data,
+                                           1, sums.ctypes.data, H.ctypes.data))
+                return [sums, H]
+            run(f"{key}/multinomial_pass-{K}-hess", mk, multinomial_pass)
+        for loss, yl, param in ((native.SVM_SQUARED_HINGE, lab, 1.0), (native.SVM_SQUARED_EPSILON, y, 0.1)):
+            for from_step in (False, True):
+                def svm_pass(output, loss=loss, yl=yl, param=param, from_step=from_step):
+                    sums, dH = np.empty(d + 8), np.empty((d + 1, d + 1))
+                    ok(lib.b2_svm_pass(*base, yl, n, d, ldx, mk, mask, 1, loss, param,
+                                       step.ctypes.data if from_step else None, -0.1, w, 0.2, 1, sums.ctypes.data,
+                                       dH.ctypes.data))
+                    return [sums, dH]
+                run(f"{key}/svm_pass-{loss}-{'from' if from_step else 'start'}", mk, svm_pass)
+        for weighted in (False, True):
+            def class_scatter(output, weighted=weighted):
+                S, counts = np.empty((d, d)), np.empty(3)
+                ok(lib.b2_class_scatter(*base, mlab, n, d, ldx, mk, mask, 1, CLASSES.ctypes.data, 7, means.ctypes.data,
+                                        CLASS_WEIGHTS.ctypes.data if weighted else None, S.ctypes.data,
+                                        counts.ctypes.data))
+                return [S, counts]
+            run(f"{key}/class_scatter-{'weighted' if weighted else 'unit'}", mk, class_scatter)
+
+        def class_scatters(output):
+            S, nk, counts = np.empty((7, d, d)), np.empty(7), np.empty(3)
+            ok(lib.b2_class_scatters(*base, mlab, n, d, ldx, mk, mask, 1, CLASSES.ctypes.data, 7, means.ctypes.data,
+                                     S.ctypes.data, nk.ctypes.data, counts.ctypes.data))
+            return [S, nk, counts]
+        run(f"{key}/class_scatters", mk, class_scatters)
 
     for kind in ("f32", "bf16"):
         xdt, es = (b2.F32, 4) if kind == "f32" else (b2.BF16, 2)
@@ -130,30 +169,32 @@ def dump(out):
         for d in DS:
             X, y, mask, coef, sigma, mean = _rows(N_DEV, d, 1000 + d)
             lab = (y > 1.0).astype(np.float32)
-            yd, ld, md = ctx.to_device(y), ctx.to_device(lab), ctx.to_device(mask)
+            mlab = (np.floor(3 * y) % 7).astype(np.float32)
+            yd, ld, mld, md = ctx.to_device(y), ctx.to_device(lab), ctx.to_device(mlab), ctx.to_device(mask)
             Xd = ctx.to_device(conv(X))
             Xs = np.zeros((N_DEV, d + 3), np.float32)           # pitch d + 3, the rows one element in
             Xs[:, 1:d + 1] = X
             Xsd = ctx.to_device(conv(Xs))
             for layout, Xp, ldx, mp in (("dev", Xd.ptr, d, None), ("strided", Xsd.ptr + es, d + 3, None),
                                         ("masked", Xd.ptr, d, md.ptr)):
-                calls(f"{kind}-d{d}-{layout}", Xp, xdt, yd.ptr, ld.ptr, mp, N_DEV, d, ldx, native.MEM_DEVICE, coef,
-                      sigma, mean)
-            for a in (yd, ld, md, Xd, Xsd):
+                calls(f"{kind}-d{d}-{layout}", Xp, xdt, yd.ptr, ld.ptr, mld.ptr, mp, N_DEV, d, ldx, native.MEM_DEVICE,
+                      coef, sigma, mean)
+            for a in (yd, ld, mld, md, Xd, Xsd):
                 a.free()
         d = 64
         X, y, mask, coef, sigma, mean = _rows(N_HOST, d, 2000)
         lab = (y > 1.0).astype(np.float32)
+        mlab = (np.floor(3 * y) % 7).astype(np.float32)
         for host in ("pageable", "pinned"):
-            arrs = [conv(X), y, lab, mask]
+            arrs = [conv(X), y, lab, mlab, mask]
             if host == "pinned":
                 pins = [ctx.pinned(a.shape, a.dtype) for a in arrs]
                 for p, a in zip(pins, arrs):
                     p.array[:] = a
                 arrs = [p.array for p in pins]
-            Xh, yh, lh, mh = arrs
-            calls(f"{kind}-d{d}-{host}", Xh.ctypes.data, xdt, yh.ctypes.data, lh.ctypes.data, mh.ctypes.data, N_HOST, d,
-                  d, native.MEM_HOST, coef, sigma, mean)
+            Xh, yh, lh, mlh, mh = arrs
+            calls(f"{kind}-d{d}-{host}", Xh.ctypes.data, xdt, yh.ctypes.data, lh.ctypes.data, mlh.ctypes.data,
+                  mh.ctypes.data, N_HOST, d, d, native.MEM_HOST, coef, sigma, mean)
             if host == "pinned":
                 for p in pins:
                     p.free()
